@@ -29,29 +29,20 @@ HIFIGAN_FLOP_PER_SAMPLE = 2.402e6      # SURVEY.md section 8d (Cin=192)
 FLOW_FLOP_PER_FRAME = 14.16e6          # SURVEY.md section 8d
 
 
-def load_measured(name, default=None):
-    """Numbers that only a GPU box can produce are committed under profiles/ by the run that measured them
-    (profiles/measured.json: FP32-FMA and dense-TF32 peaks from tools/microbench_*.cu, DRAM bytes of a decoder pass
-    per shape from an ncu capture); nothing here is a hand-typed constant.  Missing key -> `default` (None)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "measured.json")) as f:
-            return json.load(f).get(name, default)
-    except Exception:
-        return default
-
-
 def load_peaks():
+    """Peak rates the roofline field divides by: a measured MEASURED_PEAKS.json when present, else the data sheet."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             p = json.load(f)
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"],
                 "bf16_tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+        # NVIDIA H100 SXM data sheet (700 W): dense BF16 and HBM3 bandwidth -- a ceiling, not a measured rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks line).
+    """SM clock / throttle reasons sampled DURING the timed region (the `clocks` field of the result line).
 
     NVML through pynvml when importable (one nvmlInit before the warm-up, then cheap per-sample queries from a
     thread); otherwise one looping `nvidia-smi -lms` process.  Either way nothing is spawned inside the timed region:
@@ -286,7 +277,7 @@ def gpu_eager_baseline(dev, steps=3):
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
 
 
-def secondary_results(dev, peaks):
+def secondary_results(dev, peaks, steps):
     """Sub-results on the other BASELINE configs that fit one GPU (not the headline; same JSON line, key `secondary`):
     cfg3 per-GPU shard (flow reverse + HiFiGAN, B=32, 1024 frames), cfg4 MAS (512 x 200 x 1000), cfg5 multi-speaker
     B=128 mixed lengths.  CUDA events, 1 warm-up + 3 timed passes each, L2 flushed between passes."""
@@ -296,7 +287,7 @@ def secondary_results(dev, peaks):
     res = {}
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 
-    def timed(fn, n=3):
+    def timed(fn, n=steps):
         fn()
         ts = []
         for _ in range(n):
@@ -389,7 +380,7 @@ def run_cuda(args):
     tokens_pin, lengths_pin, noise_pin = tokens_h.pin_memory(), lengths_h.pin_memory(), sdp_noise_h.pin_memory()
     tokens_d, lengths_d, noise_d = tokens_h.to(dev), lengths_h.to(dev), sdp_noise_h.to(dev)
     gen = torch.Generator(device=dev).manual_seed(99 + rank)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2 of the H100
     gatherer = None
     if world > 1:
         from tts_b200.parallel import WaveformGather
@@ -470,6 +461,8 @@ def run_cuda(args):
         padded_samples += out["model_outputs"].numel()
         frames_padded += out["y_mask"].shape[0] * out["y_mask"].shape[-1]
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     samples_rank = int(sum(int(l.sum().item()) for l in lens_out))
     launches = _lib.launch_count() - launches0
     clocks = sampler.stop(first_sample)
@@ -483,7 +476,7 @@ def run_cuda(args):
         print("per-step ms:", [round(s.elapsed_time(e), 2) for s, e in ev], file=sys.stderr)
         print("per-stage:", [(n, round(a.elapsed_time(b), 2)) for n, a, b in stage_ev], file=sys.stderr)
     if _lib.lib().b200tts_debug_tc_error():
-        raise RuntimeError("bench: a tcgen05 conv launch hit a pipeline timeout -- results are invalid")
+        raise RuntimeError("bench: a tensor-core conv launch hit a pipeline timeout -- results are invalid")
 
     # ---------------- timed region 2: end to end from pinned host buffers
     for _ in range(2):
@@ -550,9 +543,6 @@ def run_cuda(args):
             cpu_nb, cpu_v, cpu_sec, cpu_samples, cores = 0, None, 0.0, 0, 0
         else:
             cpu_nb, cpu_v, cpu_sec, cpu_samples, cores = cpu
-        tf32_peak = load_measured("tf32_dense_tflops")          # tools/microbench_mma.cu on this pool (None: not measured)
-        fma_peak = load_measured("fp32_fma_tflops")
-        traffic = (load_measured("decoder_dram_bytes_per_pass") or {}).get(str(frames_padded // args.steps))
         eager = None
         secondary = None
         if world == 1 and not os.environ.get("BENCH_SKIP_EXTRA"):
@@ -560,7 +550,7 @@ def run_cuda(args):
                 eager = gpu_eager_baseline(dev)
             except Exception as ex:  # noqa: BLE001
                 eager = {"error": repr(ex)[:200]}
-            secondary = secondary_results(dev, peaks)
+            secondary = secondary_results(dev, peaks, args.steps)
         line = {
             "metric": "audio_samples_per_sec", "value": value, "unit": "samples/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": t_resident_max / args.steps * 1e3,
@@ -584,17 +574,13 @@ def run_cuda(args):
             "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches),
             "parity": parity,
-            "roofline": {"bound": "tensor", "kernel": "HiFiGAN decoder pass (tcgen05 3xTF32 conv kernels + conv_post)",
+            "roofline": {"bound": "tensor", "kernel": "HiFiGAN decoder pass (wgmma 3xTF32 conv kernels + conv_post)",
                          "achieved": dec_tflops, "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                          "frac": (dec_tflops / peaks["bf16_tflops_sustained"]) if dec_tflops else None,
-                         "traffic": traffic,
-                         "traffic_unit": "bytes per decoder pass, ncu dram__bytes_read+write (profiles/measured.json, keyed by padded frames); algorithmic layer-granular = 21.2 KB/sample",
+                         "traffic_note": "algorithmic layer-granular traffic = 21.2 KB/sample",
                          "peak_source": peaks["source"],
-                         "note": "algorithmic fp32 FLOPs; the convs run on tcgen05 kind::tf32 as 3xTF32 (3 MMAs per "
-                                 "algorithmic MAC) => ceiling = dense TF32 peak / 3; conv_post is a streaming FP32 kernel",
-                         "tf32_dense_peak_measured": tf32_peak,
-                         "frac_of_3xtf32_ceiling": (dec_tflops / (tf32_peak / 3.0)) if (dec_tflops and tf32_peak) else None,
-                         "frac_fp32_fma": (dec_tflops / fma_peak) if (dec_tflops and fma_peak) else None},
+                         "note": "algorithmic fp32 FLOPs; the convs run on wgmma tf32 as 3xTF32 (3 MMAs per "
+                                 "algorithmic MAC) => ceiling = dense TF32 peak / 3; conv_post is a streaming FP32 kernel"},
             "cpu_baseline": {"value": cpu_v, "unit": "samples/s", "cores": cores, "kind": "port",
                              "sample": f"{cpu_nb} of {B_PER_GPU} utterances, 1 warm-up (= the parity pass) + 2 timed steps ({cpu_samples} samples, {cpu_sec:.2f} s per step)",
                              "logical_cpus": os.cpu_count()},
@@ -607,6 +593,28 @@ def run_cuda(args):
 
 
 _RESULT_FD = None
+
+
+DUMP_MAX_ELEMS = 1 << 20    # per array (4 MB as float32): larger outputs are dumped as a fixed, seeded sample
+
+
+def dump_outputs(out, path):
+    """Writes what one inference step returned as <path>/<name>.npy (float32; integer outputs as float64): the same
+    arguments give the same inputs, so two builds can be compared output for output.  An array with more than
+    DUMP_MAX_ELEMS elements is written as the flattened elements at torch.randperm(numel, seed 0)[:DUMP_MAX_ELEMS],
+    sorted -- the same positions for every build."""
+    import numpy as np
+    import torch
+
+    os.makedirs(path, exist_ok=True)
+    for name, v in sorted(out.items()):
+        if not torch.is_tensor(v):
+            continue
+        a = v.detach().float() if v.is_floating_point() else v.detach().double()
+        if a.numel() > DUMP_MAX_ELEMS:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_MAX_ELEMS].sort().values
+            a = a.reshape(-1)[idx.to(a.device)]
+        np.save(os.path.join(path, name + ".npy"), a.cpu().numpy())
 
 
 def emit(line):
@@ -631,6 +639,9 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="cuda", choices=["cuda", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy; with --gpus N > 1 these are "
+                         "rank 0's own utterances, not the gathered batch")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* tts_b200 -- C ABI of the B200-native (sm_100a) VITS + HiFiGAN inference hot path.
+/* tts_b200 -- C ABI of the H100-native (sm_90a) VITS + HiFiGAN inference hot path.
  *
  * The reference (coqui-ai/TTS v0.22.0) has no FFI for this path: its "operator API" is Python
  * classes + state_dict (SURVEY.md section 8b).  Each entry point below replaces the body of one
@@ -30,14 +30,13 @@ const char* b200tts_last_error(void);
 /* number of kernels launched by this library in this process (bench.py "gpu_launches") */
 unsigned long long b200tts_launch_count(void);
 int b200tts_version(void);
-/* 1 if a tcgen05 conv launch (on any device of this process) ever hit a pipeline timeout.  The flag lives in mapped
+/* 1 if a tensor-core conv launch (on any device of this process) ever hit a pipeline timeout.  The flag lives in mapped
  * host memory: no synchronisation here (call after a stream sync to cover the launches before it).  Every later
  * conv launch on that device also checks it and returns status 1, so a timeout cannot pass silently. */
 int b200tts_debug_tc_error(void);
 
 /* Debug / test aids: record, on the calling thread, which kernel family every conv launch dispatched to.
- * ids: 0 FP32-FMA tile kernel, 1 tcgen05 v1, 2 tcgen05 v2 (M = time), 3 tcgen05 v3 (M = rows), 4 v3 + staged epilogue,
- *      5 v3 grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel. */
+ * ids: 0 FP32-FMA tile kernel, 3 tensor-core kernel (M = rows), 5 tensor-core kernel grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel. */
 void b200tts_debug_dispatch_begin(void);
 int b200tts_debug_dispatch_end(int32_t* ids, int cap); /* returns the number of launches recorded */
 
@@ -49,7 +48,7 @@ int b200tts_debug_dispatch_end(int32_t* ids, int cap); /* returns the number of 
  *   y = ((conv(leaky_relu(x, in_slope)) + bias) + residual) * scale [+ y_old if accumulate] / post_div
  * weight: host, PyTorch layout ([Cout,Cin,K], or [Cin,Cout,K] when transposed); bias host or NULL; x [B,Cin,T],
  * residual / y [B,Cout,Tout] device.  in_slope = 1 disables the prologue.  allow_tensor_cores != 0 opts the layer into
- * the tcgen05 3xTF32 kernels (the decoder / flow setting); 0 keeps it on the exact FP32-FMA kernel (text encoder).
+ * the wgmma 3xTF32 kernels (the decoder / flow setting); 0 keeps it on the exact FP32-FMA kernel (text encoder).
  */
 typedef struct {
     int in_channels, out_channels, kernel_size, dilation, padding;

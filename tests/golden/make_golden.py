@@ -1,6 +1,9 @@
 """Generates the committed golden fixtures from the UNMODIFIED reference modules.
 
-Run in the build container only (needs /root/reference):  python tests/golden/make_golden.py
+Run where the reference tree is importable (TTS_REFERENCE_ROOT, default /root/reference):
+    python tests/golden/make_golden.py
+It also re-records tests/golden/reference/: the reference-side results of the tests that compare the oracle with the
+reference live (oracle/ref_golden.py), by running those tests with TTS_WRITE_GOLDEN=1.
 Each fixture stores the reference module's state_dict, the inputs and the reference outputs for a
 SMALL configuration of the same classes the hot path uses (full-size weights would be >50 MB);
 the kernels are config-driven, so the small shapes exercise the same code.  Zero-initialised
@@ -255,5 +258,14 @@ def main_r02():
                              "vocab": list(g.vocab), "cases": tok_cases})
 
 
+def record_reference_results():
+    import subprocess
+    root = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    tests = ["tests/test_oracle_vs_reference.py", "tests/test_oracle_vs_reference_model.py", "tests/test_handoff_cpu.py"]
+    subprocess.check_call([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", *tests], cwd=root,
+                          env={**os.environ, "TTS_WRITE_GOLDEN": "1"})
+
+
 if __name__ == "__main__":
     main()
+    record_reference_results()

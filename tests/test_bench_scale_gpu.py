@@ -1,7 +1,7 @@
 """Parity in the regime the benchmark runs in (VERDICT r01, weak #1).
 
-The tcgen05 conv kernels are persistent: one CTA per SM loops over (batch, row tile, time tile) with cross-tile state
-(double-buffered TMEM accumulator phase, operand ring parities).  The small-shape tests never give a CTA more than one
+The tensor-core conv kernels are persistent: one CTA per SM loops over (batch, row tile, time tile) with cross-tile state
+(shared accumulator tile, operand ring parities).  The small-shape tests never give a CTA more than one
 tile; these do -- every case below launches 10..45 tiles per CTA, the bench's regime -- and they run the BASELINE
 configurations at their real sizes against the CPU oracle.  Where the oracle would need minutes for the full batch it
 runs on a subset of rows that contains the longest utterance (rows never interact on the path, and with the longest row
@@ -21,7 +21,7 @@ import vits_oracle as O
 
 pytestmark = pytest.mark.gpu
 FULL = bool(int(os.environ.get("B200TTS_FULL_TESTS", "0")))
-# one 3xTF32 layer on unit-variance data: the tensor core truncates when it accumulates into fp32 TMEM, which grows with
+# one 3xTF32 layer on unit-variance data: the tensor core truncates when it accumulates into fp32, which grows with
 # the reduction length Cin*K (measured 1.0e-5 at 128x11, 2.0e-5 at 256x11); single-pass TF32 sits at ~3e-4
 LAYER_REL_TOL = 5e-5
 
@@ -35,7 +35,7 @@ def _rel_rms(got, want):
 LAYER_CASES = [
     # (C, K, dil, B, T, expected kernel family)        tiles = B * ceil(T / 256 or 240) * row tiles  (148 CTAs)
     (128, 11, 5, 32, 9600, "tc3"),          # 1216 x 1 tiles: stage-1 MRF, the FLOP carrier
-    (128, 3, 1, 32, 9600, None),            # tc3 or tc3_staged (K <= 3 wide layer)
+    (128, 3, 1, 32, 9600, None),            # tc3 (K <= 3 wide layer)
     (128, 7, 3, 32, 9600, "tc3"),
     (256, 7, 1, 32, 2400, "tc3"),           # 2 row tiles
     (256, 11, 5, 16, 4800, "tc3"),
@@ -70,7 +70,7 @@ def test_conv_layer_many_tiles_per_cta(c, k, dil, b, t, family):
     if family is not None:
         assert log.names == [family], log.names
     else:
-        assert log.names in (["tc3"], ["tc3_staged"]), log.names
+        assert log.names == ["tc3"], log.names
     rel, mx = _rel_rms(got.cpu(), want)
     assert rel <= LAYER_REL_TOL and mx <= 2e-4 * float(want.abs().max()), (rel, mx)
     # plain form (no residual / accumulate), a different tile count through the same persistent loop
@@ -83,7 +83,7 @@ def test_conv_layer_many_tiles_per_cta(c, k, dil, b, t, family):
 @pytest.mark.parametrize("cin,cout,k,s,b,t", [(256, 128, 16, 8, 32, 1200), (512, 256, 16, 8, 32, 152),
                                               (128, 64, 4, 2, 32, 9600), (64, 32, 4, 2, 32, 19200)])
 def test_upsampler_many_tiles_per_cta(cin, cout, k, s, b, t):
-    """o = ups(leaky_relu(o, 0.1))  (hifigan_generator.py:248-249) as a polyphase conv on the tcgen05 kernel."""
+    """o = ups(leaky_relu(o, 0.1))  (hifigan_generator.py:248-249) as a polyphase conv on the tensor-core kernel."""
     from tts_b200 import _lib
     from tts_b200.conv import FusedConv1d
     torch.manual_seed(cin + k)
@@ -122,16 +122,15 @@ def test_decoder_and_flow_dispatch_is_pinned():
         for s in range(4):
             stage = body[s * 19:(s + 1) * 19]
             assert stage[0] == "tc3", (s, stage)
-            want = {"tc3", "tc3_staged"} if s < 2 else {"tc3_grouped"}
-            assert set(stage[1:]) <= want, (s, stage)
-    assert not ({"tc1", "tc2"} & set(names)), names          # the superseded generations are never on the bench path
+            want = {"tc3"} if s < 2 else {"tc3_grouped"}
+            assert set(stage[1:]) == want, (s, stage)
     with _lib.dispatch_log() as log:                         # a frame count that is not a multiple of 4 (unaligned rows)
         m.waveform_decoder(torch.randn(2, 192, 150).cuda())
     assert log.names[0] == "tc3" and log.names[1] == "tc3" and "fma" not in log.names, log.names
     mask = torch.ones(4, 1, 192).cuda()
     with _lib.dispatch_log() as log:
         m.flow(torch.randn(4, 192, 192).cuda(), mask, reverse=True)
-    assert set(log.names) <= {"tc3", "tc3_staged"} and len(log.names) == 4 * (2 + 2 * 4), log.names
+    assert set(log.names) == {"tc3"} and len(log.names) == 4 * (2 + 2 * 4), log.names
 
 
 # ----------------------------------------------------------------------------- decoder at length

@@ -1,15 +1,25 @@
 """Host-side widening of the path (SURVEY 8 f3 / f4), CPU only: tokenizer hand-off, fairseq checkpoint re-keying,
 HifiganConfig / setup_generator / GAN surface, and the oracle's restated vocoder hand-off -- each against the committed
-golden vectors (produced by the real reference, tests/golden/make_golden.py) and, where /root/reference exists,
-against the reference objects themselves."""
+golden vectors (produced by the real reference, tests/golden/make_golden.py) and against the reference objects
+themselves -- live where the reference tree exists, through their recorded results otherwise (oracle/ref_golden.py)."""
 import numpy as np
 import pytest
 import torch
 
 import ref_import
 import vits_oracle as O
+from ref_golden import Recorded
 
-HAVE_REF = ref_import.available()
+
+@pytest.fixture
+def rec(request):
+    r = Recorded(request.node.name)
+    yield r
+    r.save()
+
+
+def _ref():
+    return ref_import.load_full()
 
 
 # ----------------------------------------------------------------------------- tokenizer
@@ -37,23 +47,25 @@ def test_tokenizer_matches_reference_golden(golden, capsys):
     assert "ü" in tok.not_found_characters or tok.text_to_ids("ü") == [tok.characters.blank_id]   # unknown chars are dropped
 
 
-@pytest.mark.skipif(not HAVE_REF, reason="reference tree not present")
-def test_tokenizer_and_vocabulary_vs_reference_objects(capsys):
+def test_tokenizer_and_vocabulary_vs_reference_objects(rec, capsys):
     from tts_b200.text import BaseVocabulary, TTSTokenizer, basic_cleaners
-    R = ref_import.load_full()
     vocab = list("_ abcdefghijklmnopqrstuvwxyz'!?") + ["<x>"]
-    ref_v = R["characters"].BaseVocabulary(vocab, pad="_", blank=None, bos=None, eos=None)
+    ref_v = lambda: _ref()["characters"].BaseVocabulary(vocab, pad="_", blank=None, bos=None, eos=None)
     my_v = BaseVocabulary(vocab, pad="_")
     for name in ("pad_id", "blank_id", "bos_id", "eos_id", "num_chars"):
-        assert getattr(ref_v, name) == getattr(my_v, name)
+        assert rec.value(name, lambda: getattr(ref_v(), name)) == getattr(my_v, name)
     for add_blank in (False, True):
-        ref_t = R["tokenizer"].TTSTokenizer(False, R["cleaners"].basic_cleaners, ref_v, None, add_blank=add_blank)
+        ref_t = lambda: _ref()["tokenizer"].TTSTokenizer(False, _ref()["cleaners"].basic_cleaners, ref_v(), None,
+                                                         add_blank=add_blank)
         my_t = TTSTokenizer(False, basic_cleaners, my_v, None, add_blank=add_blank)
         for text in ("What's  up?", "", "UPPER lower", "x"):
-            assert ref_t.text_to_ids(text) == my_t.text_to_ids(text)
-            assert ref_t.intersperse_blank_char([1, 2, 3], True) == my_t.intersperse_blank_char([1, 2, 3], True)
-            assert ref_t.intersperse_blank_char([1, 2], False) == my_t.intersperse_blank_char([1, 2], False)
-            assert ref_t.pad_with_bos_eos([4, 5]) == my_t.pad_with_bos_eos([4, 5])
+            def ref_calls():
+                t = ref_t()
+                return (t.text_to_ids(text), t.intersperse_blank_char([1, 2, 3], True),
+                        t.intersperse_blank_char([1, 2], False), t.pad_with_bos_eos([4, 5]))
+            want = rec.value(f"{add_blank}:{text}", ref_calls)
+            assert want == (my_t.text_to_ids(text), my_t.intersperse_blank_char([1, 2, 3], True),
+                            my_t.intersperse_blank_char([1, 2], False), my_t.pad_with_bos_eos([4, 5]))
     capsys.readouterr()
 
 
@@ -68,7 +80,7 @@ def _fake_fairseq_state():
     return {k: torch.full((1,), float(i)) for i, k in enumerate(keys)}
 
 
-def test_fairseq_rekeying(tmp_path):
+def test_fairseq_rekeying(tmp_path, rec):
     from tts_b200.text import rehash_fairseq_vits_checkpoint
     sd = _fake_fairseq_state()
     p = tmp_path / "G_100000.pth"
@@ -87,11 +99,10 @@ def test_fairseq_rekeying(tmp_path):
     for old, new in want_names.items():
         assert new in got and torch.equal(got[new], sd[old]), (old, new)
     assert len(got) == len(sd)
-    if HAVE_REF:
-        ref = ref_import.load_full()["fairseq"].rehash_fairseq_vits_checkpoint(str(p))
-        assert set(ref.keys()) == set(got.keys())
-        for k in ref:
-            assert torch.equal(ref[k], got[k])
+    ref = rec.value("rehash", lambda: _ref()["fairseq"].rehash_fairseq_vits_checkpoint(str(p)))
+    assert set(ref.keys()) == set(got.keys())
+    for k in ref:
+        assert torch.equal(ref[k], got[k])
 
 
 def test_fairseq_vocab_and_tokenizer(tmp_path):
@@ -105,7 +116,7 @@ def test_fairseq_vocab_and_tokenizer(tmp_path):
 
 
 # ----------------------------------------------------------------------------- vocoder config surface
-def test_hifigan_config_and_setup_generator_surface():
+def test_hifigan_config_and_setup_generator_surface(rec):
     from tts_b200.vocoder import GAN, BaseAudioConfig, HifiganConfig, setup_generator, to_camel
     c = HifiganConfig()
     assert c.generator_model == "hifigan_generator" and c["generator_model_params"]["upsample_factors"] == [8, 8, 2, 2]
@@ -117,17 +128,22 @@ def test_hifigan_config_and_setup_generator_surface():
     assert set(k.split(".")[0] for k in gan.state_dict()) == {"model_g"}
     with pytest.raises(NotImplementedError):
         setup_generator(HifiganConfig(generator_model="melgan_generator"))
-    if HAVE_REF:
-        R = ref_import.load_full()
+    fields = ("fft_size", "win_length", "hop_length", "sample_rate", "num_mels", "ref_level_db", "min_level_db",
+              "signal_norm", "symmetric_norm", "max_norm", "clip_norm")
+
+    def ref_surface():
+        R = _ref()
         rc = R["hifigan_config"].HifiganConfig()
-        assert rc.generator_model_params == c.generator_model_params and rc.generator_model == c.generator_model
-        ref_g = R["vocoder_models"].setup_generator(rc)
-        assert list(ref_g.state_dict().keys()) == list(g.state_dict().keys())
-        assert [tuple(v.shape) for v in ref_g.state_dict().values()] == [tuple(v.shape) for v in g.state_dict().values()]
-        ra = rc.audio
-        for f in ("fft_size", "win_length", "hop_length", "sample_rate", "num_mels", "ref_level_db", "min_level_db",
-                  "signal_norm", "symmetric_norm", "max_norm", "clip_norm"):
-            assert getattr(BaseAudioConfig(), f) == getattr(ra, f), f
+        sd = R["vocoder_models"].setup_generator(rc).state_dict()
+        return {"generator_model": rc.generator_model, "generator_model_params": rc.generator_model_params,
+                "keys": list(sd.keys()), "shapes": [tuple(v.shape) for v in sd.values()],
+                "audio": {f: getattr(rc.audio, f) for f in fields}}
+    ref = rec.value("surface", ref_surface)
+    assert ref["generator_model_params"] == c.generator_model_params and ref["generator_model"] == c.generator_model
+    assert ref["keys"] == list(g.state_dict().keys())
+    assert ref["shapes"] == [tuple(v.shape) for v in g.state_dict().values()]
+    for f in fields:
+        assert getattr(BaseAudioConfig(), f) == ref["audio"][f], f
 
 
 # ----------------------------------------------------------------------------- oracle hand-off vs golden / reference

@@ -68,7 +68,7 @@ class AudioNormC(ctypes.Structure):
                 ("scaler_mean", ctypes.c_void_p), ("scaler_scale", ctypes.c_void_p)]
 
 
-DISPATCH_NAMES = {0: "fma", 1: "tc1", 2: "tc2", 3: "tc3", 4: "tc3_staged", 5: "tc3_grouped", 6: "row1", 7: "resblock"}
+DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 7: "resblock"}
 
 
 def _declare(lib):

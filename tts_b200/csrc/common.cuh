@@ -1,4 +1,4 @@
-// tts_b200 -- shared declarations for the sm_100a hot-path kernels.
+// tts_b200 -- shared declarations for the sm_90a hot-path kernels.
 // Host-side C++ here is the "engine" above the kernels; the only public surface is the
 // C ABI in include/tts_b200.h (implemented in capi.cu).
 #pragma once
@@ -93,9 +93,9 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     int ups = 1;              // >1: polyphase ConvTranspose1d
     int co_tile = 64;         // 32 or 64
     int tr_kernel = 0, tr_pad = 0;  // original transposed-conv kernel size / padding (for Tout)
-    float* w_tc = nullptr;    // device, tcgen05 packing [n_tile][chunk][tap]{hi,lo}[slab][N][4] (null: layer not eligible)
-    int tc_n = 0;             // columns (output rows) per tcgen05 CTA
-    float* w_tcg = nullptr;   // device, grouped tcgen05 packing [chunk][tap block]{hi,lo}[slab][128][4] (rows == 32 / 64)
+    float* w_tc = nullptr;    // device, tensor-core packing [n_tile][chunk][tap]{hi,lo}[slab][N][4] (null: layer not eligible)
+    int tc_n = 0;             // output rows per tensor-core tile
+    float* w_tcg = nullptr;   // device, grouped tensor-core packing [chunk][tap block]{hi,lo}[slab][128][4] (rows == 32 / 64)
     int tc_grp = 0;           // tap groups of the grouped packing (128 / rows), 0: none
     bool allow_tc = false;    // engines opt layers into the 3xTF32 tensor-core path (decoder / flow); the text and
                               // duration path stays on the exact FP32 FMA kernel so durations remain bit-stable
@@ -120,7 +120,7 @@ struct ConvIO {
     unsigned* peak_bits = nullptr;   // single-row tanh kernel only: atomicMax of |y| (as float bits) over everything stored
     // ragged batch (null: dense).  lens[b] = valid FRAMES of row b; this launch's output is only computed below
     // lens[b] * rate_out + need_out (time steps of y; for a transposed conv `rate_out` counts GEMM columns, i.e. input
-    // steps), its input is read as zero from lens[b] * rate_in + need_in on.  Honoured by the persistent tcgen05 kernels
+    // steps), its input is read as zero from lens[b] * rate_in + need_in on.  Honoured by the persistent tensor-core kernels
     // and the single-row kernel; the FMA tile kernel computes the full tensor (valid samples are identical either way).
     const int* lens = nullptr; int rate_out = 1, need_out = 0, rate_in = 1, need_in = 0;
 };
@@ -136,8 +136,7 @@ void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
 // which kernel family a launch_conv call dispatched to (recorded per thread between dispatch_begin/end; tests pin it)
-enum : int { DISPATCH_FMA = 0, DISPATCH_TC1 = 1, DISPATCH_TC2 = 2, DISPATCH_TC3 = 3, DISPATCH_TC3_STAGED = 4,
-             DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6, DISPATCH_RESBLOCK = 7 };
+enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6, DISPATCH_RESBLOCK = 7 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -1,4 +1,4 @@
-// Generic fused conv1d as an FP32 implicit GEMM on the sm_100a FMA pipe (packed FFMA2).
+// Generic fused conv1d as an FP32 implicit GEMM on the sm_90a FMA pipe.
 //
 // This one kernel carries >99% of the VITS+HiFiGAN inference FLOPs: the HiFiGAN MRF convs
 // (reference: TTS/vocoder/models/hifigan_generator.py:84-99,236-265), the polyphase form of its
@@ -12,7 +12,7 @@
 // -- mask, leaky-relu -- applied once on the way in) next to the chunk's weights
 // [8][K][CO_T] (cp.async).  Each lane owns TJ time steps strided by 32 (conflict-free LDS.32,
 // tap shifts are plain address offsets) and CJ=16 consecutive rows (warp-uniform weight LDS.128
-// broadcasts), accumulating row pairs with fma.rn.f32x2 (SASS FFMA2, x as broadcast scalar).
+// broadcasts), accumulating row pairs (x as broadcast scalar).
 // Bias / conditioning / gate / residual / mask / MRF-accumulate epilogues are fused.
 #include "common.cuh"
 #include "engines.cuh"
@@ -50,11 +50,6 @@ constexpr int CI_MAX = 16;  // CinPad granularity (largest input-channel chunk o
 
 typedef unsigned long long u64;
 
-__device__ __forceinline__ void ffma2(u64& d, u64 a, float x) {
-    u64 xx;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(xx) : "f"(x));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(xx));
-}
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
@@ -62,6 +57,13 @@ __device__ __forceinline__ u64 pack2(float lo, float hi) {
     u64 v;
     asm("mov.b64 %0, {%1, %2};" : "=l"(v) : "f"(lo), "f"(hi));
     return v;
+}
+// row pair += w pair * x: two rounded FMAs (sm_90 has no packed FP32 FMA; the register moves compile away)
+__device__ __forceinline__ void ffma2(u64& d, u64 a, float x) {
+    float d0, d1, a0, a1;
+    unpack2(d, d0, d1);
+    unpack2(a, a0, a1);
+    d = pack2(fmaf(a0, x, d0), fmaf(a1, x, d1));
 }
 __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gsrc) {
     unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
@@ -433,8 +435,8 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     for (int r = 0; r < rows; ++r) bp[r] = bl[r];
     if (upload(&L.w, P.data(), P.size())) return 2;
     if (upload(&L.bias, bp.data(), bp.size())) return 2;
-    // tcgen05 packing (3xTF32 hi/lo split) for layers the tensor-core kernel can take
-    // rows >= 32: tiles of 128 zero-padded rows (tcgen05 M = 128); exactly 32 / 64 rows additionally get the grouped
+    // tensor-core packing (3xTF32 hi/lo split) for layers the wgmma kernel can take
+    // rows >= 32: tiles of 128 zero-padded rows (M = 128: two m64 warpgroups); exactly 32 / 64 rows additionally get the grouped
     // packing below (no padding), which the dispatcher prefers; fewer rows run on the FP32-FMA kernel
     L.tc_n = 0;
     if (rows >= 32) L.tc_n = 128;
@@ -466,7 +468,7 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
         L.tc_n = 0;
     }
     // grouped packing for exactly 32 / 64 rows (conv_tc3.cuh, grouped mode): MMA row m = g * rows + co holds channel co
-    // and tap group g (a TMEM lane quarter = one group); tap block j carries tap G*j + g (zero beyond K)
+    // and tap group g; tap block j carries tap G*j + g (zero beyond K)
     L.tc_grp = 0;
     if (L.ups == 1 && (rows == 32 || rows == 64) && Cin >= 8) {
         using namespace tc;
@@ -690,11 +692,11 @@ int dispatch_end(int* ids, int cap) {
 }
 void dispatch_note(int id) { if (t_dispatch) t_dispatch->push_back(id); }
 
-// tcgen05 path: returns -1 when the layer / shape / epilogue is not eligible (caller falls through to the FMA kernel)
-// Per-device state of the tcgen05 path: the pipeline-timeout flag lives in mapped pinned host memory (the kernels
+// tensor-core path: returns -1 when the layer / shape / epilogue is not eligible (caller falls through to the FMA kernel)
+// Per-device state of the tensor-core path: the pipeline-timeout flag lives in mapped pinned host memory (the kernels
 // write it with a system-scope store), so every later launch on that device reads it WITHOUT a synchronisation and
 // fails loudly instead of returning garbage audio.
-struct TcDevice { int* err = nullptr; int num_sms = 0; };
+struct TcDevice { int* err = nullptr; int num_sms = 0; int max_smem = 0; };
 static TcDevice g_tc_dev[MAX_DEVICES];
 static DeviceOnce g_tc_once;
 
@@ -716,11 +718,11 @@ static cudaError_t launch_tc3(tc3::Tc3Kernel k, int grid, size_t smem, cudaStrea
     return cudaLaunchKernelEx(&cfg, k, t);
 }
 // ragged batches: the prefix table lives behind everything else in dynamic shared memory (when it still fits)
-static void set_ragged(tc3::Tc3Args& t, const ConvKArgs& a, size_t& smem) {
+static void set_ragged(tc3::Tc3Args& t, const ConvKArgs& a, size_t& smem, size_t max_smem) {
     t.lens = nullptr; t.rate_q = 1; t.need_q = 0; t.rate_in = 1; t.need_in = 0; t.pref_off = 0;
     if (!a.lens) return;
     const size_t off = (smem + 15) / 16 * 16, extra = tc3::ragged_table_bytes(t.B);
-    if (off + extra > 227 * 1024) return;           // enormous batch: fall back to the dense schedule (still correct)
+    if (off + extra > max_smem) return;             // enormous batch: fall back to the dense schedule (still correct)
     t.lens = a.lens; t.rate_q = a.rate_out; t.need_q = a.need_out; t.rate_in = a.rate_in; t.need_in = a.need_in;
     t.pref_off = (int)off;
     smem = off + extra;
@@ -740,22 +742,25 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
     int dev = 0;
     if (int rc = device_once(g_tc_once, &dev, [](int d) -> int {
-        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        int smem_optin = 0;
+        B200_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
+        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
         for (int g : {2, 4})
-            B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+            B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
         int* flag = nullptr;
         B200_CUDA_OK(cudaHostAlloc((void**)&flag, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
         *flag = 0;
         g_tc_dev[d].err = flag;    // unified addressing: the host pointer is valid on the device
+        g_tc_dev[d].max_smem = smem_optin;
         B200_CUDA_OK(cudaDeviceGetAttribute(&g_tc_dev[d].num_sms, cudaDevAttrMultiProcessorCount, d));
         return 0;
     })) return rc;
     int* const g_tc_err = g_tc_dev[dev].err;
     const int num_sms = g_tc_dev[dev].num_sms;
+    const size_t max_smem = (size_t)g_tc_dev[dev].max_smem;
     B200_REQUIRE(*reinterpret_cast<volatile int*>(g_tc_err) == 0,
-                 "tcgen05 conv: an earlier launch on device %d hit a pipeline timeout (its output is invalid)", dev);
+                 "tensor-core conv: an earlier launch on device %d hit a pipeline timeout (its output is invalid)", dev);
     const int rows_pad = (tc::TT + (L.K - 1) * L.dil + 7) / 8 * 8;
     // ---- persistent kernel (needs 16-byte aligned activation rows for its cp.async staging; no input mask)
     const bool aligned = ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.x_cs % 4 == 0) && (a.x_bs % 4 == 0);
@@ -764,10 +769,10 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
                                (L.ups == 1 || (!a.res && !(a.flags & EPI_ACCUM) && !a.ymask && !a.cond));
     if (grouped_enabled && persistent_ok && L.tc_grp && L.w_tcg && L.ups == 1 && !needs_v3 && !a.ymask &&
         (L.tc_grp - 1) * L.dil <= 15 && a.Tq >= 256) {
-        // grouped mode of the third-generation kernel: M = tap groups x channels, N = 256 time steps, 240 per tile
+        // grouped mode: M = tap groups x channels, N = 256 time steps, 240 per tile
         const int G = L.tc_grp, J = (L.K + G - 1) / G;
         const int rp = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
-        if (rp <= 320 && tc3::smem_bytes3(rp, rp + 4) + 128 + tc3::GROUP_XCHG_BYTES <= 227 * 1024) {
+        if (rp <= 320 && tc3::smem_bytes3(rp) <= max_smem) {
             tc3::Tc3Args t;
             memset(&t, 0, sizeof(t));
             t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
@@ -780,10 +785,8 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
             t.rows_pad = rp; t.raw_w = rp + 4;
             t.B = io.B; t.n_ttiles = (a.Tq + t.tstep - 1) / t.tstep; t.n_rtiles = 1;
             t.err = g_tc_err;
-            size_t smemg = (tc3::smem_bytes3(rp, rp + 4) + 127) / 128 * 128;
-            t.stage_off = (int)smemg;                          // partial-sum exchange tiles of the grouped epilogue
-            smemg += tc3::GROUP_XCHG_BYTES;
-            set_ragged(t, a, smemg);
+            size_t smemg = tc3::smem_bytes3(rp);
+            set_ragged(t, a, smemg, max_smem);
             const long long tiles = (long long)t.B * t.n_ttiles;
             const int grid = (int)(tiles < num_sms ? tiles : num_sms);
             B200_CUDA_OK(launch_tc3(tc3::grouped_kernel(G), grid, smemg, st, t));
@@ -793,8 +796,8 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
             return 0;
         }
     }
-    if (persistent_ok && L.tc_n == 128 && L.w_tc && tc3::smem_bytes3(rows_pad, rows_pad + 4) <= 227 * 1024) {
-        // third generation: M = rows (128, zero padded), N = 256 time steps
+    if (persistent_ok && L.tc_n == 128 && L.w_tc && rows_pad <= 320 && tc3::smem_bytes3(rows_pad) <= max_smem) {
+        // M = rows (128, zero padded), N = 256 time steps
         tc3::Tc3Args t;
         memset(&t, 0, sizeof(t));
         t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
@@ -813,40 +816,25 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         t.rows_pad = rows_pad; t.raw_w = rows_pad + 4;
         t.B = io.B; t.n_ttiles = (a.Tq + tc3::TT2 - 1) / tc3::TT2; t.n_rtiles = n_rtiles;
         t.err = g_tc_err;
-        static int staged = -1;
-        if (staged < 0) { const char* e = getenv("B200TTS_STAGED"); staged = (e && atoi(e)) ? 1 : 0; }
-        size_t smem3 = tc3::smem_bytes3(rows_pad, rows_pad + 4);
-        // staged (shared-memory transposed, coalesced) epilogue for K <= 3 layers.  It beat the r01 direct epilogue by 13 % on
-        // those layers; since the direct epilogue prefetches without register copies (r02) the direct one wins
-        // (decoder 17.2 -> 16.5 ms per bench step, same box A/B), so it is opt-in again: B200TTS_STAGED=1
-        if (staged && L.K <= 3 && L.ups == 1 && !t.gate && t.split == 0 && ((smem3 + 15) / 16 * 16 + tc3::STAGE_BYTES) <= 227 * 1024) {
-            t.stage = 1;
-            t.stage_off = (int)((smem3 + 15) / 16 * 16);
-            smem3 = (size_t)t.stage_off + tc3::STAGE_BYTES;
-        }
+        size_t smem3 = tc3::smem_bytes3(rows_pad);
         // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
         // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
         const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
-        if (!t.stage && plain_epi && (smem3 + 127) / 128 * 128 + tc3::LEAN_STAGE_BYTES + tc3::ragged_table_bytes(t.B) <= 227 * 1024) {
-            t.stage_off = (int)((smem3 + 127) / 128 * 128);     // per-warp transposition tiles of the lean epilogue
-            smem3 = (size_t)t.stage_off + tc3::LEAN_STAGE_BYTES;
-        }
-        set_ragged(t, a, smem3);
+        set_ragged(t, a, smem3, max_smem);
         const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
         const int grid = (int)(tiles < num_sms ? tiles : num_sms);
-        B200_CUDA_OK(launch_tc3(t.stage ? tc3::conv1d_tc3s_kernel : plain_epi ? tc3::conv1d_tc3_kernel : tc3::conv1d_tc3x_kernel, grid, smem3, st, t));
+        B200_CUDA_OK(launch_tc3(plain_epi ? tc3::conv1d_tc3_kernel : tc3::conv1d_tc3x_kernel, grid, smem3, st, t));
         count_launch();
-        dispatch_note(t.stage ? DISPATCH_TC3_STAGED : DISPATCH_TC3);
+        dispatch_note(DISPATCH_TC3);
         B200_CUDA_OK(cudaGetLastError());
         return 0;
     }
     // Everything else (fewer than 64 rows without a grouped packing, unaligned or masked inputs, shared-memory budget)
-    // runs on the exact FP32-FMA kernel: the first two tcgen05 generations are no longer part of the library
-    // (tools/legacy/, harness only), so a dispatch change cannot silently land on them.
+    // runs on the exact FP32-FMA kernel.
     return -1;
 }
 
-int conv_tc_error_flag() {   // 1 if any tcgen05 launch (on any device) hit a pipeline timeout; call after a sync
+int conv_tc_error_flag() {   // 1 if any tensor-core launch (on any device) hit a pipeline timeout; call after a sync
     for (int d = 0; d < MAX_DEVICES; ++d)
         if (g_tc_dev[d].err && *reinterpret_cast<volatile int*>(g_tc_dev[d].err)) return 1;
     return 0;

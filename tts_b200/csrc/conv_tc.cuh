@@ -1,26 +1,20 @@
-// Shared pieces of the tcgen05 (5th-gen tensor core) 3xTF32 implicit-GEMM conv kernels: barrier / descriptor / TMEM helpers and
-// the operand-layout description.  The kernel that runs is conv_tc3.cuh; the first two kernel generations (one tile per
-// CTA; persistent with M = time) only live on in tools/legacy/ for the stand-alone harness -- the library never launches them.
+// Shared pieces of the Hopper (sm_90a) 3xTF32 implicit-GEMM conv kernel in conv_tc3.cuh: mbarrier / bulk-copy /
+// wgmma helpers and the operand-layout description.
 //
-// conv1d as a tcgen05 implicit GEMM with 3xTF32 split precision.
+// conv1d as a wgmma implicit GEMM with 3xTF32 split precision.
 //
-//   D[t, co] += sum_ci A[t + k*dil - pad, ci] * W[co, ci, k]        for every tap k
+//   D[row, t] += sum_ci W[row, ci, k] * A[t + k*dil - pad, ci]        for every tap k
 //
-// M = 128 time steps (TMEM lanes), N = Cout tile (<= 256, TMEM columns), K = input channels, 8 per MMA.
-// Both operands are K-major, SWIZZLE_NONE ("interleave") canonical layouts: a 4-channel slab is a dense
-// [rows][4 floats] array (16 B per row), so row r of K-chunk c lives at slab_c + r*16 -- 8-row core matrices are
-// contiguous (SBO = 128 B) and the two 16-byte K chunks of one MMA are LBO = slab stride apart.  Because rows are
-// uniformly 16 B apart, the activation operand of tap k is THE SAME shared-memory tile with its descriptor start
-// address advanced by k*dil rows: one staged window serves all taps (no im2col, no per-tap copies).
+// Both operands are K-major, no-swizzle ("interleave") canonical layouts: a 4-channel slab is a dense [rows][4 floats]
+// array (16 B per row), so row r of K-chunk c lives at slab_c + r*16 -- 8-row core matrices are contiguous (SBO = 128 B)
+// and the two 16-byte K chunks of one k8 MMA are LBO = slab stride apart.  Because rows are uniformly 16 B apart, the
+// activation operand of tap k is THE SAME shared-memory tile with its descriptor start address advanced by k*dil rows:
+// one staged window serves all taps (no im2col, no per-tap copies).
 //
 // fp32 accuracy: x = hi + lo with hi = x & 0xFFFFE000 (exactly representable in TF32) and lo = x - hi (exact in
-// fp32; the tensor core keeps its top 11 bits).  D += A_hi*W_hi + A_lo*W_hi + A_hi*W_lo, accumulated in fp32 in
-// TMEM; the dropped lo*lo term is 2^-22 relative.  Activations are split on the way into shared memory (together
-// with the fused mask / leaky-ReLU prologue); weights are split once at pack time.
-//
-// Warp roles (192 threads): warps 0-3 stage activations then run the epilogue (TMEM lane quarter = warp id),
-// warp 4 streams per-tap weight blocks with cp.async.bulk + mbarrier transaction counts, warp 5 allocates TMEM and
-// one of its lanes issues tcgen05.mma / tcgen05.commit.
+// fp32; the tensor core keeps its top 11 bits).  D += A_hi*W_hi + A_lo*W_hi + A_hi*W_lo, accumulated in fp32; the
+// dropped lo*lo term is 2^-22 relative.  Activations are split on the way into shared memory (together with the fused
+// leaky-ReLU prologue); weights are split once at pack time.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,36 +22,10 @@
 namespace b200tts {
 namespace tc {
 
-constexpr int TT = 256;          // time steps per CTA (2 accumulators of 128 lanes)
+constexpr int TT = 256;          // time steps per tile (wgmma N)
 constexpr int NSLAB = 2;         // 4-channel slabs per activation stage
 constexpr int KC = 4 * NSLAB;    // input channels per stage (one MMA k-step per 2 slabs)
-constexpr int NB = 4;            // weight ring depth (one tap block each)
-constexpr int NA = 4;            // activation ring depth (two producer groups x 2)
-constexpr int PGROUP = 64;       // threads per producer group (group g stages chunks c with c%2 == g)
-constexpr int MAXIT = 10;        // max (slab,row) items per producer thread per chunk
-constexpr int NTHREADS = 192;
 constexpr uint32_t SPIN_LIMIT = 1u << 22;
-
-struct TcArgs {
-    const float* x; long long x_bs; int x_cs; int Tin;
-    const float* xmask; long long xmask_bs; float in_slope;
-    const float* w;            // packed [co_tile][chunk][tap]{hi[NSLAB][N][4], lo[NSLAB][N][4]}
-    const float* bias;         // [Rows]
-    const float* cond; long long cond_bs;
-    int Cin, K, dil, pad, Rows, N;   // N = columns per CTA (multiple of 16, <= 256)
-    float* y; long long y_bs; int y_cs; int Tout;
-    const float* res; long long res_bs; int res_cs;
-    const float* ymask; long long ymask_bs;
-    float scale; float post_div; int relu; int accum; int mask_post;
-    int rows_pad;              // activation slab rows (TT + halo, multiple of 8)
-    int* err;                  // device flag: set on a pipeline timeout
-    unsigned long long* trace; // optional [grid][16] globaltimer stamps (debug)
-    int sleep_ns;              // back-off inside barrier spin loops (0 = none)
-    int dbg;                   // debug: 1 = producers only (no MMA / weights / epilogue)
-};
-
-__device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#define TC_STAMP(slot) do { if (a.trace) a.trace[((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + (slot)] = gtime(); } while (0)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -70,68 +38,68 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity, int* err, int sleep_ns = 0) {
+__device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity, int* err) {
 #pragma unroll 1
     for (uint32_t i = 0; i < SPIN_LIMIT; ++i) {
         uint32_t ok;
         asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
                      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
         if (ok) return true;
-        if (sleep_ns) __nanosleep(sleep_ns);
     }
     if (err) { *reinterpret_cast<volatile int*>(err) = 1; __threadfence_system(); }   // mapped host flag (conv1d.cu)
     return false;
-}
-// non-blocking probe of a phase (mbarrier.test_wait: returns at once, unlike try_wait which may suspend the thread)
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// K-major, no swizzle: start address, LBO (between the two 16-byte K chunks), SBO = 128 B (next 8 rows)
+// wgmma shared-memory descriptor: K-major, no swizzle; start address, LBO (between the two 16-byte K chunks),
+// SBO = 128 B (next 8 rows), base offset 0
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((128u >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;     // descriptor version 1 (sm_100)
-    return d;                    // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
-}
-// kind::tf32, fp32 accumulate, both operands K-major, M = 128
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-    uint32_t d = 0;
-    d |= 1u << 4;                // c_format = F32
-    d |= 2u << 7;                // a_format = TF32
-    d |= 2u << 10;               // b_format = TF32
-    d |= (uint32_t)(n >> 3) << 17;
-    d |= (uint32_t)(128 >> 4) << 24;
     return d;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x 256] (+)= A[64 x 8] * B[256 x 8]^T, tf32 inputs, fp32 accumulators in registers (128 per thread):
+// d[4j + {0,1}] = D[16 w + lane/4][8j + 2(lane%4) + {0,1}], d[4j + {2,3}] = the same columns of row + 8 (w = warp of the
+// warpgroup).  acc == 0 overwrites D.
+__device__ __forceinline__ void wgmma_tf32_m64n256(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127},"
+        " %128, %129, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
 }
 
 }  // namespace tc

@@ -63,7 +63,7 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
         }
     }
     rc = pack_conv(conv_post, w[i], w[i + 1], c.out_channels, ch, 7, 1, 3);
-    // the MRF / pre convs carry ~97% of the FLOPs: run them on the tcgen05 3xTF32 kernel
+    // the MRF / pre convs carry ~97% of the FLOPs: run them on the wgmma 3xTF32 kernel
     conv_pre.allow_tc = true;
     for (auto& l : ups) l.allow_tc = true;
     for (auto& v : rb_c1) for (auto& l : v) l.allow_tc = true;
@@ -155,7 +155,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
     for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)L[s]);
     Arena ar(ws, ws_bytes);
     const int C0 = c.upsample_initial_channel;
-    // The tcgen05 kernels stage activation rows with 16-byte cp.async: rows must start 16-byte aligned.  T (decoder frames)
+    // The tensor-core kernels stage activation rows with 16-byte cp.async: rows must start 16-byte aligned.  T (decoder frames)
     // is arbitrary, so the stage-0 tensors use a row pitch rounded up to 4 floats and an unaligned input is re-pitched
     // once (B x Cin x T floats, tiny) -- otherwise conv_pre / ups[0] would silently take the FP32-FMA kernel for 3 of 4 T.
     const int Tp = (T + 3) / 4 * 4;

@@ -1,4 +1,4 @@
-// Monotonic alignment search on sm_100a.
+// Monotonic alignment search on sm_90a.
 //
 // Reference: TTS/tts/utils/monotonic_align/core.pyx:11-37 (maximum_path_each: in-place DP over a
 // band, then a backtrack reading the DP values) and :42-47 (batch loop); caller
@@ -552,8 +552,8 @@ int mas_forward(const float* value, const float* mask, const int* t_x, const int
     B200_REQUIRE(value && t_x && t_y && path, "mas: null pointer");
     static DeviceOnce attr2_once, attr_once, attr3_once;
     static int use3 = -1;
-    // measured at cfg4 (r02): 0.63 ms against mas_kernel2's 0.47 ms -- the per-lane row streaming (32 lines per LDG) and
-    // three CTAs per SM cost more than the barriers save.  Kept as an opt-in experiment (B200TTS_MAS3=1), see DESIGN.md.
+    // wavefront variant without the per-column CTA barrier: its per-lane row streaming (32 lines per LDG) and lower
+    // occupancy work against it; kept as an opt-in experiment (B200TTS_MAS3=1), see DESIGN.md.
     if (use3 < 0) { const char* e = getenv("B200TTS_MAS3"); use3 = (e && atoi(e)) ? 1 : 0; }
     const bool aligned16 = (Ty % 4 == 0) && ((reinterpret_cast<uintptr_t>(value) & 15) == 0) &&
                            (!mask || (reinterpret_cast<uintptr_t>(mask) & 15) == 0) && ((reinterpret_cast<uintptr_t>(path) & 15) == 0);

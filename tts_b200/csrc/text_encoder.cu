@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* 
     for (int j0 = 0; j0 < T; j0 += ATT_KT) {
         __syncthreads();
         // all global loads of a batch are issued before the first shared store (in-order issue would otherwise
-        // expose one full memory latency per element: profiles/r01_tc_notes.md, finding 1)
+        // expose one full memory latency per element)
         for (int i0b = 0; i0b < d * ATT_KT; i0b += 8 * 32 * ATT_Q) {
             float tmp[8];
 #pragma unroll

@@ -138,10 +138,18 @@ int launch_vocoder_input(const float* x, long long x_bs, int x_cs, int x_ts, int
     return 0;
 }
 
+// grid-stride kernels: eight CTAs per SM of the current device
+static int stride_grid(long long n) {
+    int dev = 0, sms = 132;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        sms = 132;
+    return (int)std::min<long long>((n + 1023) / 1024, (long long)sms * 8);
+}
+
 int launch_absmax(const float* x, long long n, unsigned* peak_bits, cudaStream_t st) {
     B200_REQUIRE(peak_bits && (x || n == 0), "absmax: null pointer");
     if (n == 0) return 0;
-    const int blocks = (int)std::min<long long>((n + 1023) / 1024, 148 * 8);
+    const int blocks = stride_grid(n);
     absmax_kernel<<<blocks, 256, 0, st>>>(x, n, peak_bits);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
@@ -151,7 +159,7 @@ int launch_absmax(const float* x, long long n, unsigned* peak_bits, cudaStream_t
 int launch_to_int16(const float* x, long long n, const unsigned* peak_bits, short* out, cudaStream_t st) {
     B200_REQUIRE(peak_bits && (n == 0 || (x && out)), "to_int16: null pointer");
     if (n == 0) return 0;
-    const int blocks = (int)std::min<long long>((n + 1023) / 1024, 148 * 8);
+    const int blocks = stride_grid(n);
     to_int16_kernel<<<blocks, 256, 0, st>>>(x, n, peak_bits, out);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());

@@ -161,7 +161,7 @@ def _get(obj, key, default=None):
 
 
 class Vits(nn.Module):
-    """VITS end-to-end synthesiser, inference path on sm_100a kernels."""
+    """VITS end-to-end synthesiser, inference path on sm_90a kernels."""
 
     def __init__(self, config, ap=None, tokenizer=None, speaker_manager=None, language_manager=None):
         super().__init__()
