@@ -136,6 +136,15 @@ int b200tts_hifigan_forward_ex(const b200tts_hifigan* h, const float* x, const f
                                const int32_t* frame_lengths, uint32_t* peak_bits, void* workspace, size_t workspace_bytes,
                                void* stream);
 int b200tts_hifigan_margin_frames(const b200tts_hifigan* h);
+/* Streaming decode: writes wav[b, :, frame_begin*hop : frame_end*hop) of a [B, Cout, out_len(T)] buffer (hop =
+ * prod(upsample_factors)), bit-identical to what b200tts_hifigan_forward_ex(same x, g, frame_lengths) writes there; every
+ * other sample is untouched.  x holds all T frames (the halo reads up to b200tts_hifigan_margin_frames() frames either side
+ * of the window).  Windows carry no state: any sequence of calls, e.g. consecutive chunks, may share one workspace of
+ * b200tts_hifigan_workspace_bytes(B, T) bytes.  peak_bits (nullable) folds max|wav| over the window's samples.
+ * Status 1 unless 0 <= frame_begin < frame_end <= T and out_len(T) == T * hop (every upsampler with k - u even). */
+int b200tts_hifigan_forward_window(const b200tts_hifigan* h, const float* x, const float* g, int B, int T,
+                                   int frame_begin, int frame_end, float* wav, const int32_t* frame_lengths,
+                                   uint32_t* peak_bits, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- hand-off around a standalone vocoder ---------------------------------------------------------
  * b200tts_vocoder_input replaces, in one pass on the device, what Synthesizer.tts does on the host between the TTS

@@ -90,6 +90,8 @@ def _declare(lib):
     lib.b200tts_conv1d_forward.argtypes = [vp, vp, ci, ci, ctypes.c_float, vp, ctypes.c_float, ci, ctypes.c_float, vp, vp]
     lib.b200tts_hifigan_forward_ex.restype = ci
     lib.b200tts_hifigan_forward_ex.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, sz, vp]
+    lib.b200tts_hifigan_forward_window.restype = ci
+    lib.b200tts_hifigan_forward_window.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, vp, sz, vp]
     lib.b200tts_hifigan_margin_frames.restype = ci
     lib.b200tts_hifigan_margin_frames.argtypes = [vp]
     lib.b200tts_flow_reverse_ragged.restype = ci

@@ -104,6 +104,23 @@ int b200tts_hifigan_forward_ex(const b200tts_hifigan* h, const float* x, const f
     if (!h) { set_error("hifigan_forward_ex: null handle"); return 1; }
     return h->impl.forward(x, g, B, T, wav, workspace, workspace_bytes, (cudaStream_t)stream, peak_bits, frame_lengths);
 }
+int b200tts_hifigan_forward_window(const b200tts_hifigan* h, const float* x, const float* g, int B, int T,
+                                   int frame_begin, int frame_end, float* wav, const int32_t* frame_lengths,
+                                   uint32_t* peak_bits, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("hifigan_forward_window: null handle"); return 1; }
+    if (!(0 <= frame_begin && frame_begin < frame_end && frame_end <= T)) {
+        set_error("hifigan_forward_window: frame window [%d, %d) is not inside [0, %d)", frame_begin, frame_end, T);
+        return 1;
+    }
+    const int hop = b200tts_hifigan_out_len(h, 1);
+    if (h->impl.out_len(T) != T * hop || h->impl.out_len(1) <= 0) {
+        set_error("hifigan_forward_window: the upsamplers do not multiply the length exactly (out_len(%d) = %d)", T,
+                  h->impl.out_len(T));
+        return 1;
+    }
+    return h->impl.forward(x, g, B, T, wav, workspace, workspace_bytes, (cudaStream_t)stream, peak_bits, frame_lengths,
+                           frame_begin, frame_end);
+}
 int b200tts_hifigan_margin_frames(const b200tts_hifigan* h) {   // frames past a row's end the ragged schedule still computes
     return h ? h->impl.need_P : 0;
 }

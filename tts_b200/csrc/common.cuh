@@ -123,6 +123,11 @@ struct ConvIO {
     // steps), its input is read as zero from lens[b] * rate_in + need_in on.  Honoured by the persistent tensor-core kernels
     // and the single-row kernel; the FMA tile kernel computes the full tensor (valid samples are identical either way).
     const int* lens = nullptr; int rate_out = 1, need_out = 0, rate_in = 1, need_in = 0;
+    // column window (streaming decode): only GEMM columns [q_lo, q_hi) of y must be produced, and the input holds data
+    // in columns [in_lo, in_hi) (outside is stale scratch, read as zero where a kernel reads past a conv's reach: the
+    // grouped tensor-core mode's zero-padded taps).  Tiles stay on the full tensor's column grid, so every column inside
+    // the window is computed exactly as by the unwindowed launch.  The defaults are the whole tensor.
+    int q_lo = 0, q_hi = 0x7fffffff, in_lo = 0, in_hi = 0x7fffffff;
 };
 
 // Host weights in PyTorch layout.  conv: w[Cout][Cin][K];  transposed: w[Cin][Cout][Kt].

@@ -84,6 +84,7 @@ struct ConvKArgs {
     float scale; float post_div; int act; float act_param; int flags;
     int XS;
     const int* lens; int rate_out, need_out, rate_in, need_in;
+    int q_lo, q_hi, in_lo, in_hi;   // column window (ConvIO), q_lo / in_lo >= 0
 };
 
 enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3 };
@@ -110,6 +111,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     };
     const int b = blockIdx.z, tile_co = blockIdx.y;
     const int q0 = blockIdx.x * T_T;
+    if (q0 >= a.q_hi || q0 + T_T <= a.q_lo) return;     // tile outside the column window: nothing to produce
     const int tin0 = q0 - a.pad;
     const float* xb = a.x + b * a.x_bs;
     const float* mb = a.xmask ? a.xmask + b * a.xmask_bs : nullptr;
@@ -126,7 +128,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         const int c0 = chunk * CIC;
         for (int i = tid; i < XS; i += NT) {
             const int t = tin0 + i;
-            const bool tok = (t >= 0) && (t < a.Tin);
+            const bool tok = (t >= a.in_lo) && (t < a.Tin);   // below in_lo: stale scratch of a windowed producer
             float m = 1.f;
             if (tok && mb) m = __ldg(mb + t);
 #pragma unroll
@@ -219,6 +221,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     // ---------------------------------------------------------------- epilogue
     const int row_base = tile_co * CO_T + wco * CJ;
     const int qb = q0 + wt * 32 * TJ + lane;
+    auto inw = [&](int q) { return q < a.Tout && q >= a.q_lo && q < a.q_hi; };   // stored columns: the window only
     if (EPI == KEPI_GATE) {
         // rows (2p, 2p+1) = (tanh half, sigmoid half) of output row row_base/2 + p   (wavenet.py:6-13)
 #pragma unroll
@@ -234,7 +237,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                     float v0, v1;
                     unpack2(acc[p][j], v0, v1);
                     v0 += b0; v1 += b1;
-                    if (q < a.Tout) yrow[q] = tanhf(v0) * (1.f / (1.f + expf(-v1)));
+                    if (inw(q)) yrow[q] = tanhf(v0) * (1.f / (1.f + expf(-v1)));
                 }
             }
         }
@@ -254,7 +257,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                         const int q = qb + 32 * j;
                         float v0, v1;
                         unpack2(acc[p][j], v0, v1);
-                        if (q < a.Tout) yrow[q] = tanhf((h ? v1 : v0) + bb);
+                        if (inw(q)) yrow[q] = tanhf((h ? v1 : v0) + bb);
                     }
                 }
             }
@@ -287,7 +290,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                 if (relu_p) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                 if (logc_p) { v0 = logf(fmaxf(v0, a.act_param)); v1 = logf(fmaxf(v1, a.act_param)); }
                 v0 *= mkp[j]; v1 *= mkp[j];
-                if (q < a.Tout) {
+                if (inw(q)) {
                     if (r0 < a.Rows) y0[q] = v0;
                     if (r0 + 1 < a.Rows) y1[q] = v1;
                 }
@@ -304,7 +307,8 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     int tq[TJ];
 #pragma unroll
     for (int j = 0; j < TJ; ++j) {
-        tq[j] = (qb + 32 * j) * ups;
+        const int q = qb + 32 * j;
+        tq[j] = (q >= a.q_lo && q < a.q_hi) ? q * ups : 0x7fffffff;   // outside the window: fails every bound below
         mk[j] = 1.f;
         if (a.ymask && ups == 1 && tq[j] < a.Tout) mk[j] = __ldg(a.ymask + b * a.ymask_bs + tq[j]);
     }
@@ -554,14 +558,16 @@ int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin
 // y[b, 0, t] = act(bias + sum_ci sum_k w[ci, k] * lrelu(x[b, ci, t + k - pad])), K taps, dilation 1.  One output row has
 // no reuse across rows, so this is a pure streaming kernel: each thread owns four consecutive samples and reads its
 // window as aligned float4 (neighbouring threads' overlaps are L1 hits), 4*K FMAs per channel.  HBM-bound by the x read
-// (Cin * 4 B per output sample).  Reference: hifigan_generator.py:262-264.
+// (Cin * 4 B per output sample).  Reference: hifigan_generator.py:262-264.  Eight CTAs per SM (32 registers): a full
+// SM of warps to keep the loads in flight.
 template <int K>
-__global__ void __launch_bounds__(256) conv1d_row1_kernel(const float* __restrict__ x, long long x_bs, int x_cs, int Cin,
+__global__ void __launch_bounds__(256, 8) conv1d_row1_kernel(const float* __restrict__ x, long long x_bs, int x_cs, int Cin,
                                                           int T, const float* __restrict__ w, int w_stride,
                                                           const float* __restrict__ bias, float slope, int act,
                                                           float* __restrict__ y, long long y_bs,
                                                           unsigned* __restrict__ peak_bits, const int* __restrict__ lens,
-                                                          int rate, int need_out, int need_in) {
+                                                          int rate, int need_out, int need_in, int q_lo, int q_hi,
+                                                          int in_lo, int blk_lo) {
     constexpr int PAD = (K - 1) / 2, NL = (4 + 4 + (K - 1 - PAD) + 3) / 4;   // float4 loads covering [t0 - 4, t0 + 4 + K-1-PAD)
     extern __shared__ float ws[];
     for (int i = threadIdx.x; i < Cin * K; i += blockDim.x) ws[i] = w[(size_t)i * w_stride];
@@ -576,14 +582,29 @@ __global__ void __launch_bounds__(256) conv1d_row1_kernel(const float* __restric
         Tb = (int)(e < (long long)T ? (e > 0 ? e : 0) : (long long)T);
         Ti = (int)(ei < (long long)T ? (ei > 0 ? ei : 0) : (long long)T);
     }
-    if ((int)(blockIdx.x * blockDim.x) * 4 >= Tb && !peak_bits) {        // whole block beyond the row: zero fill and leave
-        const int tz = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-        if (tz < T) *reinterpret_cast<float4*>(y + b * y_bs + tz) = make_float4(0.f, 0.f, 0.f, 0.f);
+    // column window [q_lo, hi): the grid starts at block blk_lo, only samples inside the window are stored (and folded
+    // into the peak), and the input holds data from in_lo on (whole float4s below it read as zero)
+    const int hi = min(q_hi, T), in_lo4 = in_lo & ~3;
+    const int blk0 = (int)((blockIdx.x + blk_lo) * blockDim.x) * 4;
+    const int t0 = blk0 + (int)threadIdx.x * 4;
+    const bool inside = t0 >= q_lo && t0 + 4 <= hi;              // all four samples in the window: one float4 store
+    const bool any = t0 < hi && t0 + 4 > q_lo;
+    float* yp = y + b * y_bs + t0;
+    auto store = [&](const float4& v) {
+        if (inside) {
+            *reinterpret_cast<float4*>(yp) = v;
+        } else if (any) {
+            const float* pv = &v.x;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) if (t0 + j >= q_lo && t0 + j < hi) yp[j] = pv[j];
+        }
+    };
+    if (blk0 >= Tb && !peak_bits) {        // whole block beyond the row: zero fill and leave
+        store(make_float4(0.f, 0.f, 0.f, 0.f));
         return;
     }
-    const int t0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const bool valid = t0 < Tb;
-    if (!valid && t0 < T) *reinterpret_cast<float4*>(y + b * y_bs + t0) = make_float4(0.f, 0.f, 0.f, 0.f);
+    const bool valid = t0 < Tb && any;
+    if (!valid) store(make_float4(0.f, 0.f, 0.f, 0.f));
     if (!valid && !peak_bits) return;
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
     if (valid) {
@@ -597,7 +618,7 @@ __global__ void __launch_bounds__(256) conv1d_row1_kernel(const float* __restric
             for (int l = 0; l < NL; ++l) {
                 const int t = t0 - 4 + 4 * l;
                 float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (t >= 0 && t < Ti) v = __ldg(reinterpret_cast<const float4*>(xr - 4 + 4 * l));   // Ti % 4 == 0: all in or all out
+                if (t >= in_lo4 && t < Ti) v = __ldg(reinterpret_cast<const float4*>(xr - 4 + 4 * l));   // Ti % 4 == 0: all in or all out
                 win[4 * l] = v.x; win[4 * l + 1] = v.y; win[4 * l + 2] = v.z; win[4 * l + 3] = v.w;
             }
 #pragma unroll
@@ -617,7 +638,11 @@ __global__ void __launch_bounds__(256) conv1d_row1_kernel(const float* __restric
             if (act == ACT_TANH) u = tanhf(u);
             po[j] = u;
         }
-        *reinterpret_cast<float4*>(y + b * y_bs + t0) = o;
+        store(o);
+        if (!inside) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) if (t0 + j < q_lo || t0 + j >= hi) po[j] = 0.f;   // not stored: not in the peak
+        }
     }
     if (peak_bits) {   // save_wav's max|wav| (numpy_transforms.py:439) folded into the store: one atomic per warp
         float m = fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w)));
@@ -727,6 +752,15 @@ static void set_ragged(tc3::Tc3Args& t, const ConvKArgs& a, size_t& smem, size_t
     t.pref_off = (int)off;
     smem = off + extra;
 }
+// column window: the window's tiles per row on the full call's tile grid (the whole tensor by default)
+static void set_window(tc3::Tc3Args& t, const ConvKArgs& a) {
+    // the grouped mode's zero-padded taps (K not a multiple of GRP) read past the conv's reach: 0 * stale scratch must
+    // not reach the window (NaN), so the input extent also stops where its producer's window ends
+    t.Tin = std::min(a.Tin, a.in_hi);
+    t.q_lo = a.q_lo; t.q_hi = a.q_hi; t.in_lo = a.in_lo; t.t_lo = a.q_lo / t.tstep;
+    const int hi = std::min(a.Tq, a.q_hi);
+    t.n_ttiles = std::max(0, (hi + t.tstep - 1) / t.tstep - t.t_lo);
+}
 
 static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& a, cudaStream_t st) {
     static int enabled = -1, grouped_enabled = 1;
@@ -783,12 +817,13 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
             t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
             t.scale = a.scale; t.post_div = a.post_div; t.relu = (a.act == ACT_RELU); t.accum = (a.flags & EPI_ACCUM) ? 1 : 0;
             t.rows_pad = rp; t.raw_w = rp + 4;
-            t.B = io.B; t.n_ttiles = (a.Tq + t.tstep - 1) / t.tstep; t.n_rtiles = 1;
+            t.B = io.B; t.n_rtiles = 1;
+            set_window(t, a);
             t.err = g_tc_err;
             size_t smemg = tc3::smem_bytes3(rp);
             set_ragged(t, a, smemg, max_smem);
             const long long tiles = (long long)t.B * t.n_ttiles;
-            const int grid = (int)(tiles < num_sms ? tiles : num_sms);
+            const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
             B200_CUDA_OK(launch_tc3(tc3::grouped_kernel(G), grid, smemg, st, t));
             count_launch();
             dispatch_note(DISPATCH_TC3_GROUPED);
@@ -814,7 +849,8 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         t.split = (a.flags & EPI_SPLIT) ? a.split : 0;
         t.y2 = a.y2; t.y2_bs = a.y2_bs; t.y2_cs = a.y2_cs; t.accum2 = (a.flags & EPI_ACCUM2) ? 1 : 0;
         t.rows_pad = rows_pad; t.raw_w = rows_pad + 4;
-        t.B = io.B; t.n_ttiles = (a.Tq + tc3::TT2 - 1) / tc3::TT2; t.n_rtiles = n_rtiles;
+        t.B = io.B; t.n_rtiles = n_rtiles;
+        set_window(t, a);
         t.err = g_tc_err;
         size_t smem3 = tc3::smem_bytes3(rows_pad);
         // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
@@ -822,7 +858,7 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
         set_ragged(t, a, smem3, max_smem);
         const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
-        const int grid = (int)(tiles < num_sms ? tiles : num_sms);
+        const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
         B200_CUDA_OK(launch_tc3(plain_epi ? tc3::conv1d_tc3_kernel : tc3::conv1d_tc3x_kernel, grid, smem3, st, t));
         count_launch();
         dispatch_note(DISPATCH_TC3);
@@ -855,6 +891,8 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     a.y2 = io.y2; a.y2_bs = io.y2_bs; a.y2_cs = io.y2_cs; a.split = io.split;
     a.scale = io.scale; a.post_div = io.post_div; a.act = io.act; a.act_param = io.act_param; a.flags = io.flags;
     a.lens = io.lens; a.rate_out = io.rate_out; a.need_out = io.need_out; a.rate_in = io.rate_in; a.need_in = io.need_in;
+    a.q_lo = std::max(0, io.q_lo); a.q_hi = io.q_hi; a.in_lo = std::max(0, io.in_lo); a.in_hi = io.in_hi;
+    const bool windowed = a.q_lo > 0 || a.q_hi < a.Tq;
     if (a.Tq <= 0 || io.B <= 0) return 0;
     B200_REQUIRE(!(a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)) || io.ymask,
                  "launch_conv: masked/split epilogue needs ymask");
@@ -872,12 +910,14 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
         if (L.Rows == 1 && L.K == 7 && L.dil == 1 && L.pad == 3 && !a.xmask && a.Tin == a.Tout && (a.Tout % 4) == 0 &&
             (a.x_cs % 4) == 0 && (a.x_bs % 4) == 0 && (a.y_bs % 4) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0 &&
             (reinterpret_cast<uintptr_t>(a.y) & 15) == 0 && (size_t)L.Cin * L.K * 4 <= 48 * 1024) {
-            dim3 grid((a.Tout / 4 + 255) / 256, io.B);
+            const int blk_lo = a.q_lo / 1024, blk_hi = (std::min(a.q_hi, a.Tout) + 1023) / 1024;   // 1024 samples per CTA
+            dim3 grid(std::max(1, blk_hi - blk_lo), io.B);
             if (grid.y <= 65535) {
                 conv1d_row1_kernel<7><<<grid, 256, (size_t)L.Cin * L.K * 4, st>>>(a.x, a.x_bs, a.x_cs, L.Cin, a.Tout, L.w,
                                                                                  L.co_tile, L.bias, a.in_slope, a.act, a.y,
                                                                                  a.y_bs, io.peak_bits, a.lens, a.rate_out,
-                                                                                 a.need_out, a.need_in);
+                                                                                 a.need_out, a.need_in, a.q_lo, a.q_hi,
+                                                                                 a.in_lo, blk_lo);
                 count_launch();
                 dispatch_note(DISPATCH_ROW1);
                 B200_CUDA_OK(cudaGetLastError());
@@ -887,6 +927,8 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
         if (int rc = launch_cic<KEPI_TANH>(a, L.co_tile, io.B, L.RowsPad, st)) return rc;
         if (io.peak_bits) {   // the streaming kernel was not eligible: fold the peak in a pass of its own
             B200_REQUIRE(a.y_cs == a.Tout && a.y_bs == (long long)L.Rows * a.Tout, "launch_conv: peak needs a dense output");
+            if (windowed)   // only the samples this launch stored
+                return launch_absmax_window(a.y, io.B * L.Rows, a.Tout, a.q_lo, std::min(a.q_hi, a.Tout), io.peak_bits, st);
             return launch_absmax(a.y, (long long)io.B * L.Rows * a.Tout, io.peak_bits, st);
         }
         return 0;

@@ -74,6 +74,13 @@ struct Tc3Args {
     // (it is the receptive field of the layers that still follow, worked out per launch by the engine).
     const int* lens; int rate_q, need_q, rate_in, need_in;
     int pref_off;               // byte offset in dynamic shared memory of the (B + 1)-entry tile prefix table
+    // ---- column window (default [0, INT_MAX), in_lo 0: the whole tensor).  A row's tiles run from floor(q_lo / tstep) to
+    // ceil(min(extent, q_hi) / tstep); tile origins stay multiples of tstep counted from column 0, so every column is
+    // computed (and takes the same epilogue) as in the unwindowed launch.  Input columns below in_lo are stale scratch
+    // and read as zero (whole 16-byte vectors: the ones below in_lo rounded down to a multiple of 4); the host stops Tin
+    // where the producer's window ends, so the grouped mode's zero-padded taps never multiply stale data.  n_ttiles counts
+    // the window's tiles per row (dense schedule), t_lo = floor(q_lo / tstep) is the first one.
+    int q_lo, q_hi, in_lo, t_lo;
 };
 
 static inline size_t smem_bytes3(int rows_pad) {
@@ -394,7 +401,8 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         for (int b = tid; b < a.B; b += NTHREADS2) {
             const long long e = (long long)a.lens[b] * a.rate_q + a.need_q;
             const int ext = (int)(e < (long long)a.Tq ? (e > 0 ? e : 0) : (long long)a.Tq);
-            pref[b + 1] = ((ext + a.tstep - 1) / a.tstep) * a.n_rtiles;
+            const int t_hi = (min(ext, a.q_hi) + a.tstep - 1) / a.tstep;
+            pref[b + 1] = max(0, t_hi - a.t_lo) * a.n_rtiles;
         }
         __syncthreads();
         if (warp == 0) {
@@ -433,13 +441,13 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             b = lo;
             const int local = tile - pref[b], nt = (pref[b + 1] - pref[b]) / a.n_rtiles;
             rt = local / nt;
-            q0 = (local - rt * nt) * a.tstep;
+            q0 = (a.t_lo + local - rt * nt) * a.tstep;
             return;
         }
         const int tt = tile % a.n_ttiles, rest = tile / a.n_ttiles;
         rt = rest % a.n_rtiles;
         b = rest / a.n_rtiles;
-        q0 = tt * a.tstep;
+        q0 = (a.t_lo + tt) * a.tstep;
     };
     auto input_extent = [&](int b) -> int {       // columns of x[b] that hold data; beyond it the operand is zero
         if (!ragged) return a.Tin;
@@ -497,7 +505,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     iss_Tin = input_extent(b_);
                     iss_tal = (q0_ - pad) & ~3;                            // 16-byte aligned window start (may be < 0)
                     iss_row = xg + (long long)b_ * x_bs;
-                    iss_int = iss_tal >= 0 && iss_tal + RAWW <= iss_Tin && (Cin & (KC2 - 1)) == 0;
+                    iss_int = iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KC2 - 1)) == 0;
                     iss_new = false;
                 }
                 const uint32_t dst0 = raw_u32 + (uint32_t)iss_ring * rawStage;
@@ -512,10 +520,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                         if (v_ch[e] < 0) continue;
                         const int t = iss_tal + v_t[e];
                         const int cg = iss_c * KC2 + v_ch[e];
-                        // t is a multiple of 4, so a vector is either wholly before the sequence start (zero fill),
+                        // t is a multiple of 4, so a vector is either wholly before the data start (zero fill),
                         // wholly inside, or cut by its end (partial source size, rest zero-filled by the hardware)
                         int nb = 0;
-                        if (cg < Cin && t >= 0) nb = 4 * max(0, min(4, iss_Tin - t));
+                        if (cg < Cin && t >= (a.in_lo & ~3)) nb = 4 * max(0, min(4, iss_Tin - t));
                         const int tsafe = (t >= 0 && t < iss_Tin) ? t : 0;
                         const float* src = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs + tsafe;
                         cp_async16_zfill(dst0 + v_dst[e], src, (uint32_t)nb);

@@ -25,8 +25,13 @@ struct Hifigan {
     // every launch stops `need` samples past a row's end, where `need` is the receptive field of the layers that still
     // follow (worked out in init()), so all samples below lens[b] * prod(upsample_factors) are bit-identical to the dense
     // call; the rest of the row is zero.
+    // [frame_begin, frame_end) (default: all T frames): a window of input frames.  Only wav[b, :, frame_begin * hop,
+    // frame_end * hop) is written, bit-identical to the full call; every launch produces its columns of the window plus
+    // the same margin `need` on both sides (the margins are symmetric bounds on each conv's reach), on the full call's
+    // tile grid.  Nothing is carried between windows: each one recomputes its halo from x.
     int forward(const float* x, const float* g, int B, int T, float* wav, void* ws, size_t ws_bytes,
-                cudaStream_t st, unsigned* peak_bits = nullptr, const int* lens = nullptr) const;
+                cudaStream_t st, unsigned* peak_bits = nullptr, const int* lens = nullptr, int frame_begin = 0,
+                int frame_end = -1) const;
     // per-launch exactness margins (samples at the tensor's own rate), see init()
     int need_P = 0;
     std::vector<int> need_OUT, need_U, need_q_ups, rate;
@@ -152,6 +157,7 @@ int launch_vocoder_input(const float* x, long long x_bs, int x_cs, int x_ts, int
                          const b200tts_audio_norm* denorm, const b200tts_audio_norm* norm, float scale_factor, int pad,
                          float* y, int y_pitch, cudaStream_t st);
 int launch_absmax(const float* x, long long n, unsigned* peak_bits, cudaStream_t st);
+int launch_absmax_window(const float* x, int rows, long long pitch, int lo, int hi, unsigned* peak_bits, cudaStream_t st);
 int launch_to_int16(const float* x, long long n, const unsigned* peak_bits, short* out, cudaStream_t st);
 
 // monotonic alignment search (mas.cu)

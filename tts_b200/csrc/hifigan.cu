@@ -142,15 +142,45 @@ int Hifigan::out_len(int T) const {
     return L.back();
 }
 
+// samples [lo, hi) of every row of wav that lie past the row's end (lens[b] * rate)
+__global__ void zero_past_end_kernel(float* __restrict__ wav, int C, int Tout, const int* __restrict__ lens, int rate,
+                                     int lo, int hi) {
+    const int b = blockIdx.y;
+    const long long e = (long long)lens[b] * rate;
+    const int from = (int)max((long long)lo, min(e, (long long)hi));
+    for (int c = 0; c < C; ++c) {
+        float* row = wav + ((long long)b * C + c) * Tout;
+        for (int t = from + (int)(blockIdx.x * blockDim.x + threadIdx.x); t < hi; t += (int)(gridDim.x * blockDim.x)) row[t] = 0.f;
+    }
+}
+
 int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, void* ws, size_t ws_bytes,
-                     cudaStream_t st, unsigned* peak_bits, const int* lens) const {
+                     cudaStream_t st, unsigned* peak_bits, const int* lens, int frame_begin, int frame_end) const {
     B200_REQUIRE(x && wav && ws, "hifigan_forward: null pointer");
     B200_REQUIRE((c.cond_channels > 0) == (g != nullptr) || c.cond_channels == 0,
                  "hifigan_forward: model has cond_channels=%d but g is null", c.cond_channels);
     B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "hifigan_forward: workspace too small");
+    if (frame_end < 0) frame_end = T;
+    const bool windowed = frame_begin != 0 || frame_end != T;
+    B200_REQUIRE(!windowed || (0 <= frame_begin && frame_begin < frame_end && frame_end <= T),
+                 "hifigan_forward: frame window [%d, %d) is not inside [0, %d)", frame_begin, frame_end, T);
     if (B == 0 || T == 0) return 0;
     std::vector<int> C, L;
     stage_dims(T, C, L);
+    // a window is sample-aligned only when every stage multiplies the length exactly (k - u even for each upsampler)
+    B200_REQUIRE(!windowed || L.back() == T * (rate.empty() ? 1 : rate.back()),
+                 "hifigan_forward: frame windows need out_len(T) == T * prod(upsample_factors) (got %d for T = %d)",
+                 L.back(), T);
+    // each launch's column window: its margin `need` either side of the frames' span at its own rate, and its input's
+    // data start (the producing launch's window start)
+    const long long fb = frame_begin, fe = frame_end;
+    auto window = [&](ConvIO& io) {
+        if (!windowed) return;             // the whole tensor (also for lengths that are not T * hop)
+        io.q_lo = (int)std::max(0LL, fb * io.rate_out - io.need_out);
+        io.q_hi = (int)std::min(0x7fffffffLL, fe * io.rate_out + io.need_out);
+        io.in_lo = (int)std::max(0LL, fb * io.rate_in - io.need_in);
+        io.in_hi = (int)std::min(0x7fffffffLL, fe * io.rate_in + io.need_in);
+    };
     size_t mx = 0;
     for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)L[s]);
     Arena ar(ws, ws_bytes);
@@ -189,6 +219,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
         io.y = P; io.y_bs = (long long)C0 * Tp; io.y_cs = Tp; io.Tout = T; io.B = B;
         if (has_cond) { io.cond = condv; io.cond_bs = cond.RowsPad; }
         io.lens = lens; io.rate_out = 1; io.need_out = need_P; io.rate_in = 1; io.need_in = T;   // z is defined everywhere
+        window(io);
         if ((rc = launch_conv(conv_pre, io, st))) return rc;
     }
     const float* cur = P;
@@ -203,6 +234,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
             io.y = U; io.y_bs = bs; io.y_cs = Ls; io.Tout = Ls; io.B = B;
             io.lens = lens; io.rate_in = (s == 0) ? 1 : rate[s - 1]; io.need_in = (s == 0) ? need_P : need_OUT[s - 1];
             io.rate_out = io.rate_in; io.need_out = need_q_ups[s];      // tiles run over GEMM columns = input steps
+            window(io);
             if ((rc = launch_conv(ups[s], io, st))) return rc;
         }
         for (int j = 0; j < c.num_kernels; ++j) {
@@ -221,6 +253,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
                     io.y = T1; io.y_bs = bs; io.y_cs = Ls; io.Tout = Ls; io.B = B;
                     io.lens = lens; io.rate_in = io.rate_out = rate[s];
                     io.need_in = need_xin; io.need_out = need_T1[s * c.num_kernels + j][n];
+                    window(io);
                     if ((rc = launch_conv(c1[n], io, st))) return rc;
                     convin = T1;
                     lastconv = &c2[n];
@@ -241,6 +274,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
                 io.lens = lens; io.rate_in = io.rate_out = rate[s];
                 io.need_in = type1 ? need_T1[s * c.num_kernels + j][n] : need_xin;
                 io.need_out = need_X[s * c.num_kernels + j][n];
+                window(io);
                 if ((rc = launch_conv(*lastconv, io, st))) return rc;
                 xin = dst;
                 need_xin = io.need_out;
@@ -261,8 +295,15 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
         io.peak_bits = peak_bits;
         io.lens = lens; io.rate_in = io.rate_out = rate.empty() ? 1 : rate.back(); io.need_in = need_OUT.empty() ? 0 : need_OUT.back();
         io.need_out = 0;
-        if (lens)   // rows may end before any tile of conv_post's fallback kernels writes them: the tail must be zero
-            B200_CUDA_OK(cudaMemsetAsync(wav, 0, (size_t)B * c.out_channels * curL * sizeof(float), st));
+        window(io);       // exactly the window's samples: [frame_begin * hop, frame_end * hop)
+        if (lens) {       // the window's samples past each row's end are zero (other windows' samples are left alone)
+            B200_REQUIRE(B <= 65535, "hifigan_forward: batch too large");
+            const int lo = io.q_lo, hi = std::min(io.q_hi, curL);
+            const dim3 grid((unsigned)std::max(1, std::min((hi - lo + 255) / 256, 64)), (unsigned)B);
+            zero_past_end_kernel<<<grid, 256, 0, st>>>(wav, c.out_channels, curL, lens, io.rate_out, lo, hi);
+            count_launch();
+            B200_CUDA_OK(cudaGetLastError());
+        }
         if ((rc = launch_conv(conv_post, io, st))) return rc;
     }
     return 0;

@@ -92,6 +92,17 @@ __global__ void absmax_kernel(const float* __restrict__ x, long long n, unsigned
     if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));   // non-negative floats order like uints
 }
 
+// columns [lo, hi) of `rows` rows of `pitch` floats (a streaming window of the waveform)
+__global__ void absmax_window_kernel(const float* __restrict__ x, long long pitch, int lo, int hi, unsigned* __restrict__ out) {
+    float m = 0.f;
+    const float* xr = x + (long long)blockIdx.y * pitch;
+    for (int i = lo + (int)(blockIdx.x * blockDim.x + threadIdx.x); i < hi; i += (int)(gridDim.x * blockDim.x))
+        m = fmaxf(m, fabsf(xr[i]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));
+}
+
 // wav * (32767 / max(0.01, peak)) truncated toward zero (numpy astype(int16) of an in-range float)
 __global__ void to_int16_kernel(const float* __restrict__ x, long long n, const unsigned* __restrict__ peak_bits,
                                 short* __restrict__ out) {
@@ -151,6 +162,17 @@ int launch_absmax(const float* x, long long n, unsigned* peak_bits, cudaStream_t
     if (n == 0) return 0;
     const int blocks = stride_grid(n);
     absmax_kernel<<<blocks, 256, 0, st>>>(x, n, peak_bits);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_absmax_window(const float* x, int rows, long long pitch, int lo, int hi, unsigned* peak_bits, cudaStream_t st) {
+    B200_REQUIRE(peak_bits && (x || rows == 0), "absmax: null pointer");
+    if (rows <= 0 || hi <= lo) return 0;
+    B200_REQUIRE(rows <= 65535, "absmax: too many rows");
+    const dim3 grid((unsigned)std::min((hi - lo + 255) / 256, 64), (unsigned)rows);
+    absmax_window_kernel<<<grid, 256, 0, st>>>(x, pitch, lo, hi, peak_bits);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     return 0;

@@ -210,6 +210,61 @@ class HifiganGenerator(nn.Module):
         _lib.check(rc, "hifigan_forward")
         return wav
 
+    @property
+    def hop(self):
+        """Output samples per input frame: prod(upsample_factors)."""
+        n = 1
+        for u in self._cfg["upsample_factors"]:
+            n *= u
+        return n
+
+    @torch.no_grad()
+    def forward_window(self, x, g=None, start=0, end=None, lengths=None, out=None, peak=None):
+        """Streaming decode: the samples of input frames ``[start, end)`` of ``forward(x, g, lengths=lengths)``.
+
+        Writes ``out[..., start*hop : end*hop]`` of ``out`` -- the full-length ``[B, out_channels, T*hop]`` waveform,
+        allocated when None -- and returns that view.  Every sample written is bit-identical to the one-shot call and no
+        other sample of ``out`` is touched, so consecutive windows fill ``out`` chunk by chunk.  ``x`` holds all T frames:
+        each window recomputes its halo (up to ``b200tts_hifigan_margin_frames`` frames either side) from it and carries
+        no state.  ``peak`` folds max|wav| over the window's samples, as in ``forward``.  Raises ValueError for a window
+        outside ``[0, T)`` and for upsamplers that do not multiply the length exactly (some ``k - u`` odd)."""
+        _lib.require_cuda(x, "x")
+        if hasattr(self, "cond_layer") and g is None:
+            raise ValueError("tts_b200.HifiganGenerator: model has a cond_layer but g is None")
+        x = x.to(torch.float32).contiguous()
+        b, cin, t = x.shape
+        if cin != self._cfg["in_channels"]:
+            raise ValueError(f"expected {self._cfg['in_channels']} input channels, got {cin}")
+        end = t if end is None else int(end)
+        start = int(start)
+        if not 0 <= start < end <= t:
+            raise ValueError(f"tts_b200.HifiganGenerator.forward_window: window [{start}, {end}) is not inside [0, {t})")
+        h = self._ensure_handle(x.device)
+        L = _lib.lib()
+        hop = self.hop
+        if L.b200tts_hifigan_out_len(h, t) != t * hop:
+            raise ValueError("tts_b200.HifiganGenerator.forward_window: frame windows need every upsampler to multiply the "
+                             f"length exactly (kernel - factor even); out_len({t}) = {L.b200tts_hifigan_out_len(h, t)}, "
+                             f"not {t} * {hop}")
+        shape = (b, self._cfg["out_channels"], t * hop)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=x.device)
+        elif tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != x.device or not out.is_contiguous():
+            raise ValueError(f"tts_b200.HifiganGenerator.forward_window: `out` must be a contiguous float32 {shape} "
+                             f"tensor on {x.device}")
+        gl = None
+        if hasattr(self, "cond_layer"):
+            gl = g.to(device=x.device, dtype=torch.float32).contiguous()
+        lens = None if lengths is None else lengths.to(device=x.device, dtype=torch.int32).contiguous()
+        with torch.cuda.device(x.device):
+            nbytes = L.b200tts_hifigan_workspace_bytes(h, b, t)
+            ws = _lib.workspace(x.device, nbytes, "hifigan")
+            rc = L.b200tts_hifigan_forward_window(h, _lib.ptr(x), _lib.ptr(gl), b, t, start, end, _lib.ptr(out),
+                                                  _lib.ptr(lens), _lib.ptr(peak), _lib.ptr(ws),
+                                                  ctypes.c_size_t(ws.numel()), _lib.stream_ptr(x.device))
+        _lib.check(rc, "hifigan_forward_window")
+        return out[..., start * hop: end * hop]
+
     @torch.no_grad()
     def inference(self, c):
         """Replicate-pad ``inference_padding`` frames each side, then forward (hifigan_generator.py:267-282)."""

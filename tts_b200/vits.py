@@ -292,6 +292,49 @@ class Vits(nn.Module):
         ``sdp_noise`` [B,2,T_seq] / ``prior_noise`` [B,C,T_dec] (or a callable shape->tensor) replace the two
         random draws of the reference (SURVEY appendix A7) so results can be compared exactly; by default they
         are drawn like the reference does (CPU generator, then device generator)."""
+        lat = self._latents(x, aux_input, sdp_noise, prior_noise, return_alignments)
+        zin, frame_lengths = lat["zin"], lat["frame_lengths"]
+        with _Stage(self, "waveform_decoder"):
+            o = self.waveform_decoder(zin, g=lat["g"], lengths=frame_lengths if lat["ragged"] else None)
+        hop = o.shape[-1] // max(zin.shape[-1], 1)      # prod(upsample_rates_decoder)
+        # the reference's eight keys (vits.py:1163-1172) plus: y_lengths (frames at the text-side rate), logw, and
+        # wav_lengths = valid output samples per utterance (after latent upsampling / max_inference_len cropping)
+        return {"model_outputs": o, "alignments": lat["attn"], "durations": lat["w_ceil"], "z": lat["z"],
+                "z_p": lat["z_p"], "m_p": lat["m_p"], "logs_p": lat["logs_p"], "y_mask": lat["y_mask"],
+                "y_lengths": lat["y_lengths"], "logw": lat["logw"], "wav_lengths": frame_lengths * hop}
+
+    @torch.no_grad()
+    def inference_stream(self, x, aux_input={"x_lengths": None, "d_vectors": None, "speaker_ids": None,
+                                             "language_ids": None, "durations": None}, chunk_frames=32, *,
+                         sdp_noise=None, prior_noise=None):  # pylint: disable=dangerous-default-value
+        """Streaming ``inference``: a generator of waveform chunks, the first one available long before the whole
+        batch is decoded.
+
+        The text encoder, duration predictor, path, flow (and latent upsampling / ``max_inference_len``) run whole, as
+        in ``inference``, with its one host read of the decoder length T_dec.  The decoder then runs over consecutive
+        windows of ``chunk_frames`` decoder-input frames; each yields ``{"model_outputs": [B, 1, n] waveform chunk,
+        "start": index of its first sample, "wav_lengths": [B] valid samples per utterance}``.  Every chunk is
+        bit-identical to the same samples of ``inference(...)["model_outputs"]`` with the same noise (no cross-fade:
+        each window recomputes its receptive-field halo from the latents), ``trim_padding`` included.  The chunks are
+        views of one ``[B, 1, T_dec * hop]`` buffer that later chunks do not overwrite, so earlier ones stay valid.
+        Nothing is read back to the host per chunk."""
+        if int(chunk_frames) < 1:
+            raise ValueError("tts_b200.Vits.inference_stream: chunk_frames must be >= 1")
+        lat = self._latents(x, aux_input, sdp_noise, prior_noise, False)
+        dec = self.waveform_decoder
+        zin = lat["zin"].to(torch.float32).contiguous()
+        b, _, t = zin.shape
+        hop = dec.hop
+        lengths = lat["frame_lengths"].to(torch.int32).contiguous() if lat["ragged"] else None
+        wav_lengths = lat["frame_lengths"] * hop
+        out = torch.empty((b, 1, t * hop), dtype=torch.float32, device=zin.device)
+        for f0 in range(0, t, int(chunk_frames)):
+            f1 = min(t, f0 + int(chunk_frames))
+            o = dec.forward_window(zin, g=lat["g"], start=f0, end=f1, lengths=lengths, out=out)
+            yield {"model_outputs": o, "start": f0 * hop, "wav_lengths": wav_lengths}
+
+    def _latents(self, x, aux_input, sdp_noise, prior_noise, return_alignments):
+        """Everything of ``inference`` before the decoder: text encoder -> durations -> path -> flow."""
         _lib.require_cuda(x, "x")
         a = self.args
         sid, g, lid, durations = self._set_cond_input(aux_input)
@@ -368,14 +411,9 @@ class Vits(nn.Module):
             if self.max_inference_len is not None:
                 zin = zin[:, :, : self.max_inference_len]
                 frame_lengths = torch.clamp_max(frame_lengths, int(self.max_inference_len))
-        with _Stage(self, "waveform_decoder"):
-            o = self.waveform_decoder(zin, g=g, lengths=frame_lengths if ragged else None)
-        hop = o.shape[-1] // max(zin.shape[-1], 1)      # prod(upsample_rates_decoder)
-        # the reference's eight keys (vits.py:1163-1172) plus: y_lengths (frames at the text-side rate), logw, and
-        # wav_lengths = valid output samples per utterance (after latent upsampling / max_inference_len cropping)
-        return {"model_outputs": o, "alignments": attn, "durations": w_ceil, "z": z, "z_p": z_p, "m_p": m_p,
-                "logs_p": logs_p, "y_mask": y_mask, "y_lengths": y_lengths, "logw": logw,
-                "wav_lengths": frame_lengths * hop}
+        return {"attn": attn, "w_ceil": w_ceil, "z": z, "z_p": z_p, "m_p": m_p, "logs_p": logs_p, "y_mask": y_mask,
+                "y_lengths": y_lengths, "logw": logw, "zin": zin, "frame_lengths": frame_lengths, "ragged": ragged,
+                "g": g}
 
     # ------------------------------------------------------------------ voice conversion (vits.py:1175-1232)
     @torch.no_grad()
