@@ -36,9 +36,18 @@ int b200tts_version(void);
 int b200tts_debug_tc_error(void);
 
 /* Debug / test aids: record, on the calling thread, which kernel family every conv launch dispatched to.
- * ids: 0 FP32-FMA tile kernel, 3 tensor-core kernel (M = rows), 5 tensor-core kernel grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel. */
+ * ids: 0 FP32-FMA tile kernel, 3 tensor-core kernel (M = rows), 5 tensor-core kernel grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel,
+ *      8 / 9 the tensor-core kernels 3 / 5 with 16-bit (bf16 / fp16) operands. */
 void b200tts_debug_dispatch_begin(void);
 int b200tts_debug_dispatch_end(int32_t* ids, int cap); /* returns the number of launches recorded */
+
+/* Operand precision of the tensor-core convs (opt-in; FP32 is the default everywhere).
+ *   FP32: 3xTF32 split operands, fp32-class accuracy.
+ *   BF16 / FP16: activations (after the leaky ReLU) and weights (after the weight-norm fold) are rounded to the 16-bit type
+ *     and multiplied with fp32 accumulation; epilogues, residuals and every tensor in memory stay fp32.  bf16 keeps fp32's
+ *     range with an 8-bit significand; fp16 has an 11-bit significand but overflows past +-65504 (such values become
+ *     +-inf).  Only layers with in_channels % 16 == 0 take the 16-bit kernels (dispatch ids 8 / 9); others stay FP32. */
+enum { B200TTS_PRECISION_FP32 = 0, B200TTS_PRECISION_BF16 = 1, B200TTS_PRECISION_FP16 = 2 };
 
 /* ---- one conv layer with the fused prologue / epilogue the engines use -------------------------
  * The building block every dense contraction of the path runs on; replaces one
@@ -58,6 +67,10 @@ typedef struct {
 typedef struct b200tts_conv1d b200tts_conv1d;
 int b200tts_conv1d_create(const b200tts_conv1d_config* cfg, const float* weight, const float* bias,
                           int allow_tensor_cores, b200tts_conv1d** out);
+/* the same layer on the tensor-core kernels with a chosen operand precision (B200TTS_PRECISION_*; FP32 is
+ * b200tts_conv1d_create with allow_tensor_cores = 1) */
+int b200tts_conv1d_create_ex(const b200tts_conv1d_config* cfg, const float* weight, const float* bias, int precision,
+                             b200tts_conv1d** out);
 void b200tts_conv1d_destroy(b200tts_conv1d* h);
 int b200tts_conv1d_out_len(const b200tts_conv1d* h, int T);
 int b200tts_conv1d_forward(const b200tts_conv1d* h, const float* x, int B, int T, float in_slope, const float* residual,
@@ -116,6 +129,11 @@ typedef struct {
 typedef struct b200tts_hifigan b200tts_hifigan;
 int b200tts_hifigan_create(const b200tts_hifigan_config* cfg, const float* const* weights, int num_weights,
                            b200tts_hifigan** out);
+/* the same with the operand precision (B200TTS_PRECISION_*) of conv_pre, the upsamplers and the resblock convs;
+ * cond_layer and conv_post stay fp32.  Every forward entry point below takes either kind of handle. */
+int b200tts_hifigan_create_ex(const b200tts_hifigan_config* cfg, const float* const* weights, int num_weights, int precision,
+                              b200tts_hifigan** out);
+int b200tts_hifigan_precision(const b200tts_hifigan* h); /* the handle's B200TTS_PRECISION_*, -1 for NULL */
 void b200tts_hifigan_destroy(b200tts_hifigan* h);
 size_t b200tts_hifigan_workspace_bytes(const b200tts_hifigan* h, int B, int T);
 int b200tts_hifigan_out_len(const b200tts_hifigan* h, int T);

@@ -68,7 +68,17 @@ class AudioNormC(ctypes.Structure):
                 ("scaler_mean", ctypes.c_void_p), ("scaler_scale", ctypes.c_void_p)]
 
 
-DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 7: "resblock"}
+DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 7: "resblock", 8: "tc16", 9: "tc16_grouped"}
+
+# tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
+PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2}
+
+
+def precision_id(name):
+    """B200TTS_PRECISION_* of ``"fp32"`` / ``"bf16"`` / ``"fp16"``; ValueError for anything else."""
+    if not isinstance(name, str) or name not in PRECISIONS:
+        raise ValueError(f"tts_b200: precision must be one of {sorted(PRECISIONS)}, got {name!r}")
+    return PRECISIONS[name]
 
 
 def _declare(lib):
@@ -82,6 +92,8 @@ def _declare(lib):
     lib.b200tts_debug_dispatch_end.argtypes = [vp, ci]
     lib.b200tts_conv1d_create.restype = ci
     lib.b200tts_conv1d_create.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ctypes.POINTER(vp)]
+    lib.b200tts_conv1d_create_ex.restype = ci
+    lib.b200tts_conv1d_create_ex.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ctypes.POINTER(vp)]
     lib.b200tts_conv1d_destroy.restype = None
     lib.b200tts_conv1d_destroy.argtypes = [vp]
     lib.b200tts_conv1d_out_len.restype = ci
@@ -116,6 +128,11 @@ def _declare(lib):
     lib.b200tts_hifigan_create.restype = ci
     lib.b200tts_hifigan_create.argtypes = [ctypes.POINTER(HifiganConfigC), ctypes.POINTER(vp), ci,
                                            ctypes.POINTER(vp)]
+    lib.b200tts_hifigan_create_ex.restype = ci
+    lib.b200tts_hifigan_create_ex.argtypes = [ctypes.POINTER(HifiganConfigC), ctypes.POINTER(vp), ci, ci,
+                                              ctypes.POINTER(vp)]
+    lib.b200tts_hifigan_precision.restype = ci
+    lib.b200tts_hifigan_precision.argtypes = [vp]
     lib.b200tts_hifigan_destroy.restype = None
     lib.b200tts_hifigan_destroy.argtypes = [vp]
     lib.b200tts_hifigan_workspace_bytes.restype = sz

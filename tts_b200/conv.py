@@ -15,13 +15,19 @@ from . import _lib
 
 class FusedConv1d:
     """weight [Cout,Cin,K] (or [Cin,Cout,K] with ``transposed=True``), bias [Cout] or None -- host or device tensors;
-    the packed device copy is created on first use per device."""
+    the packed device copy is created on first use per device.  ``precision`` "bf16" / "fp16" runs the tensor-core
+    kernels with 16-bit operands (fp32 accumulation; layers with Cin % 16 != 0 stay 3xTF32); "fp32" is the
+    ``tensor_cores`` setting as given."""
 
-    def __init__(self, weight, bias=None, dilation=1, padding=0, transposed=False, stride=1, tensor_cores=True):
+    def __init__(self, weight, bias=None, dilation=1, padding=0, transposed=False, stride=1, tensor_cores=True,
+                 precision="fp32"):
         self.weight = weight.detach().to(torch.float32).cpu().contiguous()
         self.bias = None if bias is None else bias.detach().to(torch.float32).cpu().contiguous()
         self.dilation, self.padding, self.transposed, self.stride = int(dilation), int(padding), bool(transposed), int(stride)
         self.tensor_cores = bool(tensor_cores)
+        self.precision = precision
+        if _lib.precision_id(precision) != 0 and not self.tensor_cores:
+            raise ValueError("tts_b200.FusedConv1d: a 16-bit precision needs tensor_cores=True")
         if transposed:
             self.cin, self.cout, self.k = self.weight.shape
         else:
@@ -41,8 +47,12 @@ class FusedConv1d:
             cfg = _lib.Conv1dConfigC(self.cin, self.cout, self.k, self.dilation, self.padding, int(self.transposed), self.stride)
             out = ctypes.c_void_p()
             with torch.cuda.device(device):
-                rc = _lib.lib().b200tts_conv1d_create(ctypes.byref(cfg), _lib.ptr(self.weight), _lib.ptr(self.bias),
-                                                      int(self.tensor_cores), ctypes.byref(out))
+                if self.precision == "fp32":
+                    rc = _lib.lib().b200tts_conv1d_create(ctypes.byref(cfg), _lib.ptr(self.weight), _lib.ptr(self.bias),
+                                                          int(self.tensor_cores), ctypes.byref(out))
+                else:
+                    rc = _lib.lib().b200tts_conv1d_create_ex(ctypes.byref(cfg), _lib.ptr(self.weight), _lib.ptr(self.bias),
+                                                             _lib.precision_id(self.precision), ctypes.byref(out))
             _lib.check(rc, "conv1d_create")
             self._handles[device] = h = out
         return h

@@ -99,6 +99,10 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     int tc_grp = 0;           // tap groups of the grouped packing (128 / rows), 0: none
     bool allow_tc = false;    // engines opt layers into the 3xTF32 tensor-core path (decoder / flow); the text and
                               // duration path stays on the exact FP32 FMA kernel so durations remain bit-stable
+    int prec = 0;             // tensor-core operand type, B200TTS_PRECISION_* (set BEFORE packing): 0 = 3xTF32; bf16 / fp16
+                              // pack the 16-bit weights below instead when Cin % 16 == 0 (otherwise the layer stays 3xTF32)
+    uint16_t* w_tc16 = nullptr;   // device, 16-bit packing [n_tile][chunk of 16][tap][slab][N][8] (null: none)
+    uint16_t* w_tcg16 = nullptr;  // device, 16-bit grouped packing [chunk of 16][tap block][slab][128][8] (rows == 32 / 64)
 };
 
 struct ConvIO {
@@ -141,7 +145,8 @@ void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
 // which kernel family a launch_conv call dispatched to (recorded per thread between dispatch_begin/end; tests pin it)
-enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6, DISPATCH_RESBLOCK = 7 };
+enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6, DISPATCH_RESBLOCK = 7,
+             DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9 };   // TC16*: the same kernels with bf16 / fp16 operands
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

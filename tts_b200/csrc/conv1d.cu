@@ -19,6 +19,8 @@
 #include "conv_tc.cuh"
 #include "conv_tc3.cuh"
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -415,7 +417,69 @@ void free_conv(ConvLayer& L) {
     if (L.bias) cudaFree(L.bias);
     if (L.w_tc) cudaFree(L.w_tc);
     if (L.w_tcg) cudaFree(L.w_tcg);
+    if (L.w_tc16) cudaFree(L.w_tc16);
+    if (L.w_tcg16) cudaFree(L.w_tcg16);
     L.w = L.bias = L.w_tc = L.w_tcg = nullptr;
+    L.w_tc16 = L.w_tcg16 = nullptr;
+}
+
+// fp32 -> the 16-bit operand type's bits, round to nearest even (what cvt.rn does to the activations on the device)
+static uint16_t to_16bit(float v, int prec) {
+    uint16_t u;
+    if (prec == tc::PREC_BF16) { const __nv_bfloat16 h = __float2bfloat16_rn(v); memcpy(&u, &h, 2); }
+    else { const __half h = __float2half_rn(v); memcpy(&u, &h, 2); }
+    return u;
+}
+static int upload16(uint16_t** dst, const std::vector<uint16_t>& src) {
+    *dst = nullptr;
+    B200_CUDA_OK(cudaMalloc((void**)dst, src.size() * sizeof(uint16_t)));
+    B200_CUDA_OK(cudaMemcpy(*dst, src.data(), src.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// 16-bit tensor-core packings (bf16 / fp16 per L.prec; Cin % 16 == 0): the layouts of pack_rows below with 16-channel
+// chunks and no hi/lo split, one tap block = [2 slabs][128 rows][8] (4 KB).  The weight norm is already folded (in fp32)
+// into Wl; each weight is rounded once, here.
+static int pack_rows16(ConvLayer& L, const std::vector<float>& Wl, int rows, int Cin, int K) {
+    const int nchunk = Cin / tc::KC16;
+    const size_t blk = (size_t)2 * 128 * 8;
+    if (L.tc_n) {
+        const int N = L.tc_n, nt = (rows + N - 1) / N;
+        std::vector<uint16_t> Q((size_t)nt * nchunk * K * blk, 0);
+        for (int tile = 0; tile < nt; ++tile)
+            for (int c = 0; c < nchunk; ++c)
+                for (int k = 0; k < K; ++k) {
+                    uint16_t* dst = Q.data() + (((size_t)tile * nchunk + c) * K + k) * blk;
+                    for (int s2 = 0; s2 < 2; ++s2)
+                        for (int n = 0; n < N; ++n)
+                            for (int i = 0; i < 8; ++i) {
+                                const int r = tile * N + n, ci = c * tc::KC16 + 8 * s2 + i;
+                                const float v = r < rows ? Wl[((size_t)r * Cin + ci) * K + k] : 0.f;
+                                dst[((size_t)s2 * N + n) * 8 + i] = to_16bit(v, L.prec);
+                            }
+                }
+        if (upload16(&L.w_tc16, Q)) return 2;
+    }
+    L.tc_grp = 0;
+    if (L.ups == 1 && (rows == 32 || rows == 64)) {     // grouped: MMA row m = g * rows + co, tap block j carries tap G*j + g
+        const int G = 128 / rows, J = (K + G - 1) / G;
+        std::vector<uint16_t> Q((size_t)nchunk * J * blk, 0);
+        for (int c = 0; c < nchunk; ++c)
+            for (int j = 0; j < J; ++j) {
+                uint16_t* dst = Q.data() + ((size_t)c * J + j) * blk;
+                for (int s2 = 0; s2 < 2; ++s2)
+                    for (int m = 0; m < 128; ++m)
+                        for (int i = 0; i < 8; ++i) {
+                            const int g = m / rows, co = m % rows;
+                            const int k = G * j + g, ci = c * tc::KC16 + 8 * s2 + i;
+                            const float v = k < K ? Wl[((size_t)co * Cin + ci) * K + k] : 0.f;
+                            dst[((size_t)s2 * 128 + m) * 8 + i] = to_16bit(v, L.prec);
+                        }
+            }
+        if (upload16(&L.w_tcg16, Q)) return 2;
+        L.tc_grp = G;
+    }
+    return 0;
 }
 
 // Wl(r, ci, k): logical weights already expressed as a correlation-form conv with `rows` GEMM rows
@@ -442,8 +506,11 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     // tensor-core packing (3xTF32 hi/lo split) for layers the wgmma kernel can take
     // rows >= 32: tiles of 128 zero-padded rows (M = 128: two m64 warpgroups); exactly 32 / 64 rows additionally get the grouped
     // packing below (no padding), which the dispatcher prefers; fewer rows run on the FP32-FMA kernel
+    // L.prec (set before packing) = bf16 / fp16 with Cin % 16 == 0: the 16-bit packings instead (pack_rows16); any other
+    // Cin keeps the 3xTF32 packing, so the layer's launches show up as tc3 / tc3_grouped in the dispatch log
     L.tc_n = 0;
     if (rows >= 32) L.tc_n = 128;
+    if (L.prec != tc::PREC_FP32 && Cin % tc::KC16 == 0) return pack_rows16(L, Wl, rows, Cin, K);
     if (L.tc_n && rows >= 16 && Cin >= 8) {
         using namespace tc;
         const int N = L.tc_n, nt = (rows + N - 1) / N, nchunk = (Cin + KC - 1) / KC;
@@ -770,7 +837,7 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         const char* e = getenv("B200TTS_NO_TC");
         enabled = (e && atoi(e)) ? 0 : 1;
     }
-    if (!enabled || !L.allow_tc || (!L.w_tc && !L.w_tcg) || a.Tq < 128) return -1;
+    if (!enabled || !L.allow_tc || (!L.w_tc && !L.w_tcg && !L.w_tc16 && !L.w_tcg16) || a.Tq < 128) return -1;
     if (a.act == ACT_LOGCLAMP || a.act == ACT_TANH) return -1;
     if (!(a.in_slope >= 0.f && a.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
     const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
@@ -778,10 +845,12 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     if (int rc = device_once(g_tc_once, &dev, [](int d) -> int {
         int smem_optin = 0;
         B200_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
-        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-        B200_CUDA_OK(cudaFuncSetAttribute(tc3::conv1d_tc3x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-        for (int g : {2, 4})
-            B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+        for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16}) {
+            for (bool lean : {true, false})
+                B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+            for (int g : {2, 4})
+                B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+        }
         int* flag = nullptr;
         B200_CUDA_OK(cudaHostAlloc((void**)&flag, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
         *flag = 0;
@@ -801,16 +870,18 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const int n_rtiles = (L.Rows + L.tc_n - 1) / L.tc_n;
     const bool persistent_ok = aligned && !a.xmask &&
                                (L.ups == 1 || (!a.res && !(a.flags & EPI_ACCUM) && !a.ymask && !a.cond));
-    if (grouped_enabled && persistent_ok && L.tc_grp && L.w_tcg && L.ups == 1 && !needs_v3 && !a.ymask &&
+    // 16-bit operands (L.prec, packed only when Cin % 16 == 0) wherever FP32 would take tc3 / tc3_grouped
+    const int pg = L.w_tcg16 ? L.prec : tc::PREC_FP32, pp = L.w_tc16 ? L.prec : tc::PREC_FP32;
+    if (grouped_enabled && persistent_ok && L.tc_grp && (L.w_tcg || L.w_tcg16) && L.ups == 1 && !needs_v3 && !a.ymask &&
         (L.tc_grp - 1) * L.dil <= 15 && a.Tq >= 256) {
         // grouped mode: M = tap groups x channels, N = 256 time steps, 240 per tile
         const int G = L.tc_grp, J = (L.K + G - 1) / G;
         const int rp = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
-        if (rp <= 320 && tc3::smem_bytes3(rp) <= max_smem) {
+        if (rp <= 320 && tc3::smem_bytes3(rp, pg) <= max_smem) {
             tc3::Tc3Args t;
             memset(&t, 0, sizeof(t));
             t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-            t.w = L.w_tcg; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
+            t.w = pg ? (const void*)L.w_tcg16 : (const void*)L.w_tcg; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
             t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = 128;
             t.KJ = J; t.dil_blk = G * L.dil; t.tstep = tc3::TSTEP_GROUPED;
             t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = 1; t.Tq = a.Tq;
@@ -820,23 +891,23 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
             t.B = io.B; t.n_rtiles = 1;
             set_window(t, a);
             t.err = g_tc_err;
-            size_t smemg = tc3::smem_bytes3(rp);
+            size_t smemg = tc3::smem_bytes3(rp, pg);
             set_ragged(t, a, smemg, max_smem);
             const long long tiles = (long long)t.B * t.n_ttiles;
             const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
-            B200_CUDA_OK(launch_tc3(tc3::grouped_kernel(G), grid, smemg, st, t));
+            B200_CUDA_OK(launch_tc3(tc3::grouped_kernel(G, pg), grid, smemg, st, t));
             count_launch();
-            dispatch_note(DISPATCH_TC3_GROUPED);
+            dispatch_note(pg ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED);
             B200_CUDA_OK(cudaGetLastError());
             return 0;
         }
     }
-    if (persistent_ok && L.tc_n == 128 && L.w_tc && rows_pad <= 320 && tc3::smem_bytes3(rows_pad) <= max_smem) {
+    if (persistent_ok && L.tc_n == 128 && (L.w_tc || L.w_tc16) && rows_pad <= 320 && tc3::smem_bytes3(rows_pad, pp) <= max_smem) {
         // M = rows (128, zero padded), N = 256 time steps
         tc3::Tc3Args t;
         memset(&t, 0, sizeof(t));
         t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-        t.w = L.w_tc; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
+        t.w = pp ? (const void*)L.w_tc16 : (const void*)L.w_tc; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
         t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = 128;
         t.KJ = L.K; t.dil_blk = L.dil; t.tstep = tc3::TT2;
         t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
@@ -852,16 +923,16 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         t.B = io.B; t.n_rtiles = n_rtiles;
         set_window(t, a);
         t.err = g_tc_err;
-        size_t smem3 = tc3::smem_bytes3(rows_pad);
+        size_t smem3 = tc3::smem_bytes3(rows_pad, pp);
         // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
         // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
         const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
         set_ragged(t, a, smem3, max_smem);
         const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
         const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
-        B200_CUDA_OK(launch_tc3(plain_epi ? tc3::conv1d_tc3_kernel : tc3::conv1d_tc3x_kernel, grid, smem3, st, t));
+        B200_CUDA_OK(launch_tc3(tc3::plain_kernel(pp, plain_epi), grid, smem3, st, t));
         count_launch();
-        dispatch_note(DISPATCH_TC3);
+        dispatch_note(pp ? DISPATCH_TC16 : DISPATCH_TC3);
         B200_CUDA_OK(cudaGetLastError());
         return 0;
     }

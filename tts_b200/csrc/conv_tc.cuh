@@ -1,5 +1,5 @@
-// Shared pieces of the Hopper (sm_90a) 3xTF32 implicit-GEMM conv kernel in conv_tc3.cuh: mbarrier / bulk-copy /
-// wgmma helpers and the operand-layout description.
+// Shared pieces of the Hopper (sm_90a) implicit-GEMM conv kernels in conv_tc3.cuh: mbarrier / bulk-copy /
+// wgmma helpers and the operand-layout description (3xTF32 by default; bf16 / fp16 operands, see the end).
 //
 // conv1d as a wgmma implicit GEMM with 3xTF32 split precision.
 //
@@ -15,6 +15,10 @@
 // fp32; the tensor core keeps its top 11 bits).  D += A_hi*W_hi + A_lo*W_hi + A_hi*W_lo, accumulated in fp32; the
 // dropped lo*lo term is 2^-22 relative.  Activations are split on the way into shared memory (together with the fused
 // leaky-ReLU prologue); weights are split once at pack time.
+//
+// Opt-in 16-bit operands (bf16 or fp16, fp32 accumulation): no split, one m64n256k16 MMA per 16 input channels and tap.
+// A slab row is still 16 bytes, now holding 8 channels of one time step, so a k16 step is two slabs LBO apart and the
+// tap shift above still holds; activations are rounded (cvt.rn) on the way into shared memory, weights at pack time.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,6 +29,9 @@ namespace tc {
 constexpr int TT = 256;          // time steps per tile (wgmma N)
 constexpr int NSLAB = 2;         // 4-channel slabs per activation stage
 constexpr int KC = 4 * NSLAB;    // input channels per stage (one MMA k-step per 2 slabs)
+constexpr int KC16 = 16;         // input channels per stage with 16-bit operands (one k16 step per 2 slabs)
+// tensor-core operand type (the values of B200TTS_PRECISION_* in include/tts_b200.h)
+enum : int { PREC_FP32 = 0, PREC_BF16 = 1, PREC_FP16 = 2 };
 constexpr uint32_t SPIN_LIMIT = 1u << 22;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -70,36 +77,75 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
+// The 128 accumulator operands of an m64n256 wgmma (%0 .. %127) and their constraints.
+#define B200_WGMMA_D128                                                                                                       \
+    "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"    \
+    "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63," \
+    "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95," \
+    "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127},"
+#define B200_WGMMA_D128_OPS(d)                                                                                                \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),                          \
+    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),                    \
+    "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),                  \
+    "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),                  \
+    "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),                  \
+    "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),                  \
+    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),                  \
+    "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),                  \
+    "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),                  \
+    "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),                  \
+    "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),                  \
+    "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),                  \
+    "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),              \
+    "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),          \
+    "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),          \
+    "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+
 // D[64 x 256] (+)= A[64 x 8] * B[256 x 8]^T, tf32 inputs, fp32 accumulators in registers (128 per thread):
 // d[4j + {0,1}] = D[16 w + lane/4][8j + 2(lane%4) + {0,1}], d[4j + {2,3}] = the same columns of row + 8 (w = warp of the
 // warpgroup).  acc == 0 overwrites D.
 __device__ __forceinline__ void wgmma_tf32_m64n256(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
-        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
-        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127},"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 " B200_WGMMA_D128
         " %128, %129, p, 1, 1;\n}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : B200_WGMMA_D128_OPS(d)
         : "l"(adesc), "l"(bdesc), "r"(acc)
         : "memory");
+}
+
+// The same tile with 16-bit operands: D[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, bf16 or fp16 inputs (both K-major,
+// no transpose), fp32 accumulators in the layout above.  A K-major no-swizzle slab row is still 16 bytes, now 8 channels,
+// so the k16 step reads two slabs LBO apart exactly as the tf32 k8 step does.
+__device__ __forceinline__ void wgmma_bf16_m64n256(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " B200_WGMMA_D128
+        " %128, %129, p, 1, 1, 0, 0;\n}"
+        : B200_WGMMA_D128_OPS(d)
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_m64n256(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " B200_WGMMA_D128
+        " %128, %129, p, 1, 1, 0, 0;\n}"
+        : B200_WGMMA_D128_OPS(d)
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+}
+
+// two fp32 values -> one register of two 16-bit values, round to nearest even; `lo` goes to the lower address
+__device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+__device__ __forceinline__ uint32_t cvt_f16x2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
 }
 
 }  // namespace tc

@@ -11,6 +11,12 @@
 //                           (NA2 stages)
 //   warp  11    loader    : per-tap weight blocks {hi,lo}[2 slabs][128 rows][4] by cp.async.bulk, one lane per ring slot
 //
+// PREC (compile time) = PREC_BF16 / PREC_FP16: 16-bit operands with fp32 accumulation.  A chunk is 16 input channels: the
+// producers stage them as two 8-channel cp.async slots of one raw ring stage, apply the leaky ReLU and round to the
+// 16-bit type into two slabs [rows][8] (no hi/lo split); the loader streams tap blocks [2 slabs][128 rows][8] (4 KB); the
+// consumers issue one m64n256k16 MMA per tap and chunk.  Epilogues, residuals and every tensor in global memory stay
+// fp32.  Shared memory: the raw ring doubles (+31 KB), the activation stages and weight slots halve (-20 KB, -12 KB).
+//
 // Grouped mode (GRP = 2 / 4) for narrow layers (exactly 64 / 32 output rows, the last two HiFiGAN stages): the 128
 // MMA rows are GRP tap-groups x (128/GRP) channels -- row g * (128/GRP) + c carries the weights of channel c for taps
 // g, g+GRP, g+2*GRP, ... so one instruction stream of ceil(K/GRP) "tap blocks" (B shifted by GRP*dil rows per block)
@@ -47,7 +53,7 @@ constexpr int NTHREADS2 = 32 * (W_LOAD + 1);
 struct Tc3Args {
     const float* x; long long x_bs; int x_cs; int Tin;
     float in_slope;
-    const float* w;            // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]}
+    const void* w;             // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32 (16-bit: [2][128][8])
     const float* bias;
     const float* cond; long long cond_bs;
     int Cin, K, dil, pad, Rows, N;
@@ -83,8 +89,10 @@ struct Tc3Args {
     int q_lo, q_hi, in_lo, t_lo;
 };
 
-static inline size_t smem_bytes3(int rows_pad) {
-    return (size_t)NRAW * KC2 * RAWS * 4 + (size_t)NA2 * (4 * rows_pad * 16) + (size_t)NB2 * (4 * MROWS * 16) + ACC_BYTES + 512;
+// prec: PREC_FP32 (8-channel chunks, hi/lo slab pairs) or a 16-bit type (16-channel chunks, two slabs)
+static inline size_t smem_bytes3(int rows_pad, int prec = PREC_FP32) {
+    const size_t kch = prec ? KC16 : KC2, nsl = prec ? 2 : 4;
+    return (size_t)NRAW * kch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + (size_t)NB2 * (nsl * MROWS * 16) + ACC_BYTES + 512;
 }
 static inline size_t ragged_table_bytes(int B) { return ((size_t)(B + 1) * sizeof(int) + 15) / 16 * 16; }
 
@@ -373,16 +381,19 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     }
 }
 
-template <int GRP, bool LEAN = true>   // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN: plain-layer kernel (lean
-                                       // epilogue inline, general one out of line) -- false for the WaveNet / masked / transposed
-                                       // layers (general epilogue inline)
+template <int GRP, bool LEAN = true, int PREC = PREC_FP32>   // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
+                                       // plain-layer kernel (lean epilogue inline, general one out of line) -- false for the
+                                       // WaveNet / masked / transposed layers (general epilogue inline); PREC: operand type
 __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     extern __shared__ __align__(128) unsigned char smem[];
+    constexpr int KCH = PREC ? KC16 : KC2;       // input channels per chunk
+    constexpr int NSL = PREC ? 2 : 4;            // 16-byte slabs per operand stage: two 16-bit slabs, or hi[2] + lo[2]
+    constexpr int SLC = PREC ? 8 : 4;            // channels per slab row
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ROWS = a.rows_pad, RAWW = a.raw_w, K = a.KJ;
-    const uint32_t rawStage = (uint32_t)KC2 * RAWS * 4;
-    const uint32_t slabA = (uint32_t)ROWS * 16, stageA = 4 * slabA;     // hi[2] + lo[2]
-    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = 4 * slabB;   // one tap block: {hi,lo}[2 slabs][128 rows][16 B]
+    const uint32_t rawStage = (uint32_t)KCH * RAWS * 4;
+    const uint32_t slabA = (uint32_t)ROWS * 16, stageA = NSL * slabA;
+    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NSL * slabB;   // one tap block: [NSL slabs][128 rows][16 B]
     unsigned char* smRaw = smem;
     unsigned char* smA = smRaw + NRAW * rawStage;
     unsigned char* smB = smA + NA2 * stageA;
@@ -392,7 +403,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
 
-    const int nchunks = (a.Cin + KC2 - 1) / KC2;
+    const int nchunks = (a.Cin + KCH - 1) / KCH;
     const bool ragged = a.lens != nullptr;
     int* pref = reinterpret_cast<int*>(smem + a.pref_off);    // pref[b] = first tile of row b (ragged only)
     if (ragged) {
@@ -486,7 +497,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         for (int e = 0; e < MAXI; ++e) {
             const int idx = ptid + e * NPROD;
             const int sl = idx / ROWS, r = idx - sl * ROWS;
-            i_raw[e] = (idx < 2 * ROWS) ? (4 * sl) * RAWS + r : -1;
+            i_raw[e] = (idx < 2 * ROWS) ? (SLC * sl) * RAWS + r : -1;
             i_dst[e] = (int)(sl * slabA) + r * 16;
         }
         // running positions instead of divisions / modulos per chunk
@@ -505,28 +516,32 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     iss_Tin = input_extent(b_);
                     iss_tal = (q0_ - pad) & ~3;                            // 16-byte aligned window start (may be < 0)
                     iss_row = xg + (long long)b_ * x_bs;
-                    iss_int = iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KC2 - 1)) == 0;
+                    iss_int = iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
                     iss_new = false;
                 }
-                const uint32_t dst0 = raw_u32 + (uint32_t)iss_ring * rawStage;
-                if (iss_int) {                                             // whole window inside the row: plain 16-byte copies
-                    const float* src = iss_row + (long long)(iss_c * KC2) * x_cs + iss_tal;
+                // a chunk is KCH / 8 slots of 8 channels (one for FP32): the per-thread work items cover one slot
 #pragma unroll
-                    for (int e = 0; e < MAXV; ++e)
-                        if (v_ch[e] >= 0) cp_async16(dst0 + v_dst[e], src + v_src[e]);
-                } else {
+                for (int h = 0; h < KCH / KC2; ++h) {
+                    const uint32_t dst0 = raw_u32 + (uint32_t)iss_ring * rawStage + (uint32_t)(h * KC2 * RAWS * 4);
+                    if (iss_int) {                                             // whole window inside the row: plain 16-byte copies
+                        const float* src = iss_row + (long long)(iss_c * KCH + h * KC2) * x_cs + iss_tal;
 #pragma unroll
-                    for (int e = 0; e < MAXV; ++e) {
-                        if (v_ch[e] < 0) continue;
-                        const int t = iss_tal + v_t[e];
-                        const int cg = iss_c * KC2 + v_ch[e];
-                        // t is a multiple of 4, so a vector is either wholly before the data start (zero fill),
-                        // wholly inside, or cut by its end (partial source size, rest zero-filled by the hardware)
-                        int nb = 0;
-                        if (cg < Cin && t >= (a.in_lo & ~3)) nb = 4 * max(0, min(4, iss_Tin - t));
-                        const int tsafe = (t >= 0 && t < iss_Tin) ? t : 0;
-                        const float* src = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs + tsafe;
-                        cp_async16_zfill(dst0 + v_dst[e], src, (uint32_t)nb);
+                        for (int e = 0; e < MAXV; ++e)
+                            if (v_ch[e] >= 0) cp_async16(dst0 + v_dst[e], src + v_src[e]);
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < MAXV; ++e) {
+                            if (v_ch[e] < 0) continue;
+                            const int t = iss_tal + v_t[e];
+                            const int cg = iss_c * KCH + h * KC2 + v_ch[e];
+                            // t is a multiple of 4, so a vector is either wholly before the data start (zero fill),
+                            // wholly inside, or cut by its end (partial source size, rest zero-filled by the hardware)
+                            int nb = 0;
+                            if (cg < Cin && t >= (a.in_lo & ~3)) nb = 4 * max(0, min(4, iss_Tin - t));
+                            const int tsafe = (t >= 0 && t < iss_Tin) ? t : 0;
+                            const float* src = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs + tsafe;
+                            cp_async16_zfill(dst0 + v_dst[e], src, (uint32_t)nb);
+                        }
                     }
                 }
                 if (++iss_c == nchunks) { iss_c = 0; ++iss_it; iss_new = true; }
@@ -549,27 +564,42 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             const int tin0 = tr_q0 - pad, off = tin0 - (tin0 & ~3);
             const float* raw = reinterpret_cast<const float*>(smRaw + tr_ring * rawStage) + off;
             unsigned char* base = smA + as * stageA;
-            float u[MAXI][4];
+            float u[MAXI][SLC];
 #pragma unroll
             for (int e = 0; e < MAXI; ++e) {           // all shared loads first ...
                 const float* rp = raw + (i_raw[e] < 0 ? 0 : i_raw[e]);
 #pragma unroll
-                for (int i = 0; i < 4; ++i) u[e][i] = rp[i * RAWS];
+                for (int i = 0; i < SLC; ++i) u[e][i] = rp[i * RAWS];
             }
+            if constexpr (PREC != PREC_FP32) {
 #pragma unroll
-            for (int e = 0; e < MAXI; ++e) {           // ... then prologue, hi/lo split and the two 16-byte stores
-                if (i_raw[e] < 0) continue;
-                float4 hi, lo;
-                float* ph = &hi.x; float* pl = &lo.x;
+                for (int e = 0; e < MAXI; ++e) {       // ... then prologue, rounding to 8 x 16 bits and one 16-byte store
+                    if (i_raw[e] < 0) continue;
+                    uint32_t p[4];
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float w_ = fmaxf(u[e][i], u[e][i] * slope);        // leaky ReLU for 0 <= slope <= 1 (1: identity)
-                    const float h = __uint_as_float(__float_as_uint(w_) & 0xFFFFE000u);
-                    ph[i] = h;
-                    pl[i] = w_ - h;
+                    for (int i = 0; i < 4; ++i) {
+                        const float w0 = fmaxf(u[e][2 * i], u[e][2 * i] * slope);
+                        const float w1 = fmaxf(u[e][2 * i + 1], u[e][2 * i + 1] * slope);
+                        p[i] = PREC == PREC_BF16 ? cvt_bf16x2(w0, w1) : cvt_f16x2(w0, w1);
+                    }
+                    *reinterpret_cast<uint4*>(base + i_dst[e]) = make_uint4(p[0], p[1], p[2], p[3]);
                 }
-                *reinterpret_cast<float4*>(base + i_dst[e]) = hi;
-                *reinterpret_cast<float4*>(base + 2 * slabA + i_dst[e]) = lo;
+            } else {
+#pragma unroll
+                for (int e = 0; e < MAXI; ++e) {           // ... then prologue, hi/lo split and the two 16-byte stores
+                    if (i_raw[e] < 0) continue;
+                    float4 hi, lo;
+                    float* ph = &hi.x; float* pl = &lo.x;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const float w_ = fmaxf(u[e][i], u[e][i] * slope);        // leaky ReLU for 0 <= slope <= 1 (1: identity)
+                        const float h = __uint_as_float(__float_as_uint(w_) & 0xFFFFE000u);
+                        ph[i] = h;
+                        pl[i] = w_ - h;
+                    }
+                    *reinterpret_cast<float4*>(base + i_dst[e]) = hi;
+                    *reinterpret_cast<float4*>(base + 2 * slabA + i_dst[e]) = lo;
+                }
             }
             fence_async_smem();                                  // generic-proxy stores -> visible to wgmma (async proxy)
             __syncwarp();
@@ -651,9 +681,15 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     if (ok) {
                         const uint64_t w_hi = wdesc0 + (uint64_t)sb * wslot, w_lo = w_hi + wlo_off;
                         wgmma_fence();
-                        wgmma_tf32_m64n256(d, w_hi, xl, acc);                   // small terms first
-                        wgmma_tf32_m64n256(d, w_lo, xh, 1u);
-                        wgmma_tf32_m64n256(d, w_hi, xh, 1u);
+                        if constexpr (PREC == PREC_BF16) {
+                            wgmma_bf16_m64n256(d, w_hi, xh, acc);
+                        } else if constexpr (PREC == PREC_FP16) {
+                            wgmma_f16_m64n256(d, w_hi, xh, acc);
+                        } else {
+                            wgmma_tf32_m64n256(d, w_hi, xl, acc);               // small terms first
+                            wgmma_tf32_m64n256(d, w_lo, xh, 1u);
+                            wgmma_tf32_m64n256(d, w_hi, xh, 1u);
+                        }
                         wgmma_commit();
                     }
                     wgmma_wait<1>();                                             // the previous tap's group is done
@@ -708,14 +744,26 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     }
 }
 
-__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1>(a); }
-__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3x_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, false>(a); }   // gate / split / mask / polyphase
-template <int GRP>
-__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3g_kernel(const __grid_constant__ Tc3Args a) { tc3_body<GRP>(a); }
+// PREC: PREC_FP32 (3xTF32), PREC_BF16 or PREC_FP16
+template <int PREC>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, true, PREC>(a); }
+template <int PREC>   // gate / split / mask / polyphase
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3x_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, false, PREC>(a); }
+template <int GRP, int PREC>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3g_kernel(const __grid_constant__ Tc3Args a) { tc3_body<GRP, true, PREC>(a); }
 
 typedef void (*Tc3Kernel)(const Tc3Args);
+static inline Tc3Kernel plain_kernel(int prec, bool lean) {
+    if (prec == PREC_BF16) return lean ? conv1d_tc3_kernel<PREC_BF16> : conv1d_tc3x_kernel<PREC_BF16>;
+    if (prec == PREC_FP16) return lean ? conv1d_tc3_kernel<PREC_FP16> : conv1d_tc3x_kernel<PREC_FP16>;
+    return lean ? conv1d_tc3_kernel<PREC_FP32> : conv1d_tc3x_kernel<PREC_FP32>;
+}
 // grouped kernel for 2 / 4 tap groups (any dilation with (GRP - 1) * dil <= 15)
-static inline Tc3Kernel grouped_kernel(int grp) { return grp == 2 ? conv1d_tc3g_kernel<2> : conv1d_tc3g_kernel<4>; }
+static inline Tc3Kernel grouped_kernel(int grp, int prec = PREC_FP32) {
+    if (prec == PREC_BF16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_BF16> : conv1d_tc3g_kernel<4, PREC_BF16>;
+    if (prec == PREC_FP16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP16> : conv1d_tc3g_kernel<4, PREC_FP16>;
+    return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP32> : conv1d_tc3g_kernel<4, PREC_FP32>;
+}
 
 }  // namespace tc3
 }  // namespace b200tts

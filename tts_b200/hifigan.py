@@ -5,6 +5,10 @@ Same constructor signature, same ``state_dict`` keys (the torch modules below ar
 containers -- weight-norm parametrizations included -- so reference checkpoints load unchanged),
 same ``forward(x, g=None)`` / ``inference(c)`` / ``remove_weight_norm()`` / ``load_checkpoint``.
 The arithmetic runs in libtts_b200.so (b200tts_hifigan_forward); there is no PyTorch fallback.
+
+``precision`` ("fp32" default, "bf16", "fp16") selects the operand type of the tensor-core convs (conv_pre, the
+upsamplers, every resblock conv): the 16-bit modes round activations and weights before each multiply and keep fp32
+accumulators and tensors, trading accuracy for speed (include/tts_b200.h, B200TTS_PRECISION_*).
 """
 import ctypes
 
@@ -100,6 +104,7 @@ class HifiganGenerator(nn.Module):
             remove_parametrizations(self.conv_post, "weight")
         self._handle = None
         self._handle_device = None
+        self._precision = "fp32"
         # a parent's load_state_dict never calls a child's load_state_dict() override (it recurses through
         # _load_from_state_dict), so the packed handle is dropped from a pre-hook: Vits.load_checkpoint twice in a row
         # must not keep the first checkpoint's decoder weights
@@ -120,6 +125,19 @@ class HifiganGenerator(nn.Module):
     def _apply(self, fn, *a, **kw):
         self._drop_handle()
         return super()._apply(fn, *a, **kw)
+
+    @property
+    def precision(self):
+        """Operand precision of the decoder's tensor-core convs: "fp32" (3xTF32, the default), "bf16" or "fp16".
+        Setting it drops the packed weights; the next call packs them for the new precision."""
+        return self._precision
+
+    @precision.setter
+    def precision(self, value):
+        _lib.precision_id(value)                      # ValueError for anything else
+        if value != self._precision:
+            self._drop_handle()
+        self._precision = value
 
     def repack(self):
         """Re-read the parameters (call after modifying weights in place)."""
@@ -168,7 +186,8 @@ class HifiganGenerator(nn.Module):
         arr = (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
         handle = ctypes.c_void_p()
         with torch.cuda.device(device):
-            rc = _lib.lib().b200tts_hifigan_create(ctypes.byref(cfg), arr, len(tensors), ctypes.byref(handle))
+            rc = _lib.lib().b200tts_hifigan_create_ex(ctypes.byref(cfg), arr, len(tensors),
+                                                      _lib.precision_id(self._precision), ctypes.byref(handle))
         _lib.check(rc, "hifigan_create")
         self._handle, self._handle_device = handle, device
         return handle
