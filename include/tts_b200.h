@@ -370,6 +370,7 @@ int b200tts_expand_prior(const float* cum, const float* x_mask, const int64_t* y
  *   pad2 samples (both each side; 0 = none), then framed with hop (no centering of its own):
  *     wav_to_spec  : pad1 = (n_fft-hop)/2, pad2 = 0,        mode 0: sqrt(re^2+im^2+1e-6)
  *     TorchSTFT    : pad1 = pad_wav ? (n_fft-hop)/2 : 0, pad2 = n_fft/2 (center=True), mode 1: sqrt(max(.,1e-8))
+ *     MelSpectrogram (torchaudio, power 2): pad1 = 0, pad2 = n_fft/2, mode 2: re^2+im^2 (no clamp, no root)
  *   power != 1 raises the magnitude to that power (TorchSTFT.power).
  * mel_project: mel [B,n_mels,n_frames] = basis @ spec, followed by log(max(., log_clamp)) when log_clamp > 0.
  */
@@ -381,6 +382,49 @@ int b200tts_stft_magnitude(const b200tts_stft* h, const float* wav, int B, int T
                            float power, float* spec, int n_frames, void* stream);
 int b200tts_stft_mel_project(const b200tts_stft* h, const float* spec, int B, int n_frames, float log_clamp,
                              float* mel, void* stream);
+
+/* ---- H/ASP ResNet speaker encoder (d-vectors) --------------------------------------------------
+ * Replaces ResNetSpeakerEncoder.forward, TTS/encoder/models/resnet.py:153-198, with the front end of
+ * BaseEncoder.get_torch_mel_spectrogram_class, TTS/encoder/models/base_encoder.py:12-61 (PreEmphasis, then
+ * torchaudio MelSpectrogram: centred STFT with reflect padding, power 2, mel filterbank).
+ * weights (host, PyTorch layout; every BatchNorm is 4 tensors: weight, bias, running_mean, running_var):
+ *   if use_torch_spec: torch_spec.0.filter [2], torch_spec.1.spectrogram.window [win_length],
+ *                      torch_spec.1.mel_scale.fb [fft_size/2+1, input_dim]
+ *   conv1.weight [F0,1,3,3], conv1.bias, bn1 (4)
+ *   per stage s, per block i (layerS.i): conv1.weight [F,Fin,3,3], bn1 (4), conv2.weight [F,F,3,3], bn2 (4),
+ *     se.fc.0.weight [F/8,F], se.fc.0.bias, se.fc.2.weight [F,F/8], se.fc.2.bias,
+ *     and for block 0 of stages 2..4: downsample.0.weight [F,Fin,1,1], downsample.1 (4)
+ *   attention.0.weight [128, F3*input_dim/8, 1], attention.0.bias, attention.2 (4), attention.3.weight, .bias
+ *   fc.weight [proj_dim, (ASP ? 2 : 1) * F3*input_dim/8], fc.bias
+ * forward: B windows of T samples (use_torch_spec) or T frames (spectrogram input), window b starting at element
+ *   starts[b] (device int32) of x.  Waveform: x is flat, each window is pre-emphasised and framed at its own edges.
+ *   Spectrogram: window b is the [input_dim, T] block at x + starts[b] (channel stride T).  Consecutive runs of
+ *   B / groups windows are averaged after the optional l2 norm: emb [groups, proj_dim].  B % groups must be 0.
+ * features: the same pipeline stopped after stage `stage` (0: instance-normed input [B, input_dim, T'];
+ *   s = 1..4: layerS output [B, F(s-1), H_s, T_s]), written densely to out.  For tests and inspection.
+ * workspace_bytes covers both calls for B windows of length T.
+ */
+typedef struct {
+    int input_dim;        /* mel bins (64) */
+    int proj_dim;         /* embedding size (512) */
+    int layers[4];        /* SE blocks per stage ([3, 4, 6, 3]) */
+    int num_filters[4];   /* channels per stage ([32, 64, 128, 256]) */
+    int encoder_type;     /* 0 = SAP, 1 = ASP */
+    int log_input;        /* log(x + 1e-6) before the instance norm */
+    int use_torch_spec;   /* 1: waveform input through the mel front end; 0: [input_dim, T] spectrogram input */
+    int fft_size, win_length, hop_length;   /* front end (use_torch_spec only) */
+} b200tts_speaker_encoder_config;
+typedef struct b200tts_speaker_encoder b200tts_speaker_encoder;
+int b200tts_speaker_encoder_create(const b200tts_speaker_encoder_config* cfg, const float* const* weights,
+                                   int num_weights, b200tts_speaker_encoder** out);
+void b200tts_speaker_encoder_destroy(b200tts_speaker_encoder* h);
+size_t b200tts_speaker_encoder_workspace_bytes(const b200tts_speaker_encoder* h, int B, int T);
+int b200tts_speaker_encoder_forward(const b200tts_speaker_encoder* h, const float* x, const int32_t* starts, int B,
+                                    int T, int groups, int l2_norm, float* emb, void* workspace, size_t workspace_bytes,
+                                    void* stream);
+int b200tts_speaker_encoder_features(const b200tts_speaker_encoder* h, const float* x, const int32_t* starts, int B,
+                                     int T, int stage, float* out, void* workspace, size_t workspace_bytes,
+                                     void* stream);
 
 #ifdef __cplusplus
 }

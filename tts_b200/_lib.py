@@ -62,6 +62,13 @@ class Conv1dConfigC(ctypes.Structure):
                                             "transposed", "stride")]
 
 
+class SpeakerEncoderConfigC(ctypes.Structure):
+    _fields_ = [("input_dim", ctypes.c_int), ("proj_dim", ctypes.c_int), ("layers", ctypes.c_int * 4),
+                ("num_filters", ctypes.c_int * 4)] + \
+               [(n, ctypes.c_int) for n in ("encoder_type", "log_input", "use_torch_spec", "fft_size", "win_length",
+                                            "hop_length")]
+
+
 class AudioNormC(ctypes.Structure):
     _fields_ = [("signal_norm", ctypes.c_int), ("symmetric_norm", ctypes.c_int), ("clip_norm", ctypes.c_int),
                 ("max_norm", ctypes.c_float), ("min_level_db", ctypes.c_float), ("ref_level_db", ctypes.c_float),
@@ -153,6 +160,17 @@ def _declare(lib):
         f = getattr(lib, f"b200tts_{name}_workspace_bytes")
         f.restype = sz
         f.argtypes = [vp, ci, ci]
+    lib.b200tts_speaker_encoder_create.restype = ci
+    lib.b200tts_speaker_encoder_create.argtypes = [ctypes.POINTER(SpeakerEncoderConfigC), ctypes.POINTER(vp), ci,
+                                                   ctypes.POINTER(vp)]
+    lib.b200tts_speaker_encoder_destroy.restype = None
+    lib.b200tts_speaker_encoder_destroy.argtypes = [vp]
+    lib.b200tts_speaker_encoder_workspace_bytes.restype = sz
+    lib.b200tts_speaker_encoder_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_speaker_encoder_forward.restype = ci
+    lib.b200tts_speaker_encoder_forward.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_speaker_encoder_features.restype = ci
+    lib.b200tts_speaker_encoder_features.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
     lib.b200tts_stft_create.restype = ci
     lib.b200tts_stft_create.argtypes = [ci, ci, vp, vp, ci, ctypes.POINTER(vp)]
     lib.b200tts_stft_destroy.restype = None

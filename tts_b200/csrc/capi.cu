@@ -12,6 +12,7 @@ struct b200tts_sdp { SDP impl; };
 struct b200tts_stft { Stft impl; };
 struct b200tts_posterior { PosteriorEnc impl; };
 struct b200tts_duration_predictor { DurPred impl; };
+struct b200tts_speaker_encoder { SpeakerEncoder impl; };
 
 extern "C" {
 
@@ -307,6 +308,23 @@ int b200tts_duration_predictor_forward(const b200tts_duration_predictor* h, cons
                                        void* workspace, size_t workspace_bytes, void* stream) {
     if (!h) { set_error("duration_predictor_forward: null handle"); return 1; }
     return h->impl.forward(x, mask, g, lang_emb, B, T, logw, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+B200_HANDLE_API(speaker_encoder, b200tts_speaker_encoder, b200tts_speaker_encoder_config)
+
+int b200tts_speaker_encoder_forward(const b200tts_speaker_encoder* h, const float* x, const int32_t* starts, int B,
+                                    int T, int groups, int l2_norm, float* emb, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+    if (!h) { set_error("speaker_encoder_forward: null handle"); return 1; }
+    return h->impl.run(x, starts, B, T, groups, l2_norm, emb, -1, nullptr, workspace, workspace_bytes,
+                       (cudaStream_t)stream);
+}
+int b200tts_speaker_encoder_features(const b200tts_speaker_encoder* h, const float* x, const int32_t* starts, int B,
+                                     int T, int stage, float* out, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+    if (!h) { set_error("speaker_encoder_features: null handle"); return 1; }
+    if (stage < 0 || stage > 4) { set_error("speaker_encoder_features: stage %d is not in 0..4", stage); return 1; }
+    return h->impl.run(x, starts, B, T, 1, 0, nullptr, stage, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

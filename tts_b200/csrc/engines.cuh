@@ -145,6 +145,32 @@ struct Stft {
     int mel_project(const float* spec, int B, int n_frames, float log_clamp, float* out, cudaStream_t st) const;
 };
 
+// H/ASP ResNet speaker encoder (speaker_encoder.cu).  Activations are freq-major with one zero row above and below,
+// [H + 2][C][L]: the B windows sit side by side on the time axis, window b in columns [b*P, b*P + T) of its stage, with
+// zero columns up to (b+1)*P; a 3x3 conv is then a 1D conv over the 3C channel rows of three adjacent freq rows.
+struct SpeakerEncoder {
+    struct Block {
+        ConvLayer c1, c2, ds;                  // c2 and ds carry their BatchNorm folded in; c1's bn1 follows the ReLU
+        float *s1 = nullptr, *t1 = nullptr;    // bn1 as a per-channel affine after the ReLU
+        float *fc1w = nullptr, *fc1b = nullptr, *fc2w = nullptr, *fc2b = nullptr;   // SE MLP
+        int C = 0, Cin = 0, Cr = 0;
+        bool down = false;                     // first block of stages 2..4: stride 2 + downsample
+    };
+    b200tts_speaker_encoder_config c;
+    Stft stft;
+    float pre0 = 0.f, pre1 = 1.f;              // pre-emphasis taps: y[t] = pre0 * x[t-1] + pre1 * x[t]
+    ConvLayer conv1, att1, att2, fc;
+    float *s0 = nullptr, *t0 = nullptr;        // stem bn1 (after the ReLU)
+    std::vector<Block> blocks;
+    int stage_first[5] = {0, 0, 0, 0, 0};      // index of each stage's first block (stage_first[4] = blocks.size())
+    ~SpeakerEncoder();
+    int init(const b200tts_speaker_encoder_config& cfg, const float* const* w, int nw);
+    size_t workspace_bytes(int B, int T) const;
+    // stop < 0: full forward into emb [groups, proj_dim]; stop = 0..4: dense features of that stage into feat
+    int run(const float* x, const int* starts, int B, int T, int groups, int l2_norm, float* emb, int stop, float* feat,
+            void* ws, size_t ws_bytes, cudaStream_t st) const;
+};
+
 // durations -> path -> expanded prior (path.cu)
 int launch_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st);

@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(STFT_NT) stft_mag_kernel(const float* wav, con
         }
         for (int f = tid; f < F; f += STFT_NT) {
             const float p = re[f] * re[f] + im[f] * im[f];
-            float m = (mode == 0) ? sqrtf(p + 1e-6f) : sqrtf(fmaxf(p, 1e-8f));
+            float m = (mode == 0) ? sqrtf(p + 1e-6f) : (mode == 2) ? p : sqrtf(fmaxf(p, 1e-8f));   // 2: power spectrum
             if (power != 1.f) m = powf(m, power);
             mag[fr * F + f] = m;
         }
