@@ -116,14 +116,12 @@ def test_decoder_and_flow_dispatch_is_pinned():
     # conv_pre, then per stage: ups + 18 resblock convs, then conv_post
     assert names[0] == "tc3" and names[-1] == "row1", names
     body = names[1:-1]
-    fused = "resblock" in body
-    if not fused:
-        assert len(body) == 4 * 19, len(body)
-        for s in range(4):
-            stage = body[s * 19:(s + 1) * 19]
-            assert stage[0] == "tc3", (s, stage)
-            want = {"tc3"} if s < 2 else {"tc3_grouped"}
-            assert set(stage[1:]) == want, (s, stage)
+    assert len(body) == 4 * 19, len(body)
+    for s in range(4):
+        stage = body[s * 19:(s + 1) * 19]
+        assert stage[0] == "tc3", (s, stage)
+        want = {"tc3"} if s < 2 else {"tc3_grouped"}
+        assert set(stage[1:]) == want, (s, stage)
     with _lib.dispatch_log() as log:                         # a frame count that is not a multiple of 4 (unaligned rows)
         m.waveform_decoder(torch.randn(2, 192, 150).cuda())
     assert log.names[0] == "tc3" and log.names[1] == "tc3" and "fma" not in log.names, log.names

@@ -1,7 +1,6 @@
 """CUDA HiFiGAN generator vs golden fixtures (reference outputs) and vs the oracle at full width.
 north_star tolerance: waveform within 1e-4 RMS.  The decoder convs run on the wgmma 3xTF32 kernel (fp32
-accumulate in registers, ~2^-25 truncation per accumulation step), so the asserted bound is 3e-5 RMS; with
-B200TTS_NO_TC=1 (FP32 FMA kernel only) the same tests hold at 1e-6."""
+accumulate in registers, ~2^-25 truncation per accumulation step), so the asserted bound is 3e-5 RMS."""
 import pytest
 import torch
 

@@ -75,7 +75,7 @@ class AudioNormC(ctypes.Structure):
                 ("scaler_mean", ctypes.c_void_p), ("scaler_scale", ctypes.c_void_p)]
 
 
-DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 7: "resblock", 8: "tc16", 9: "tc16_grouped"}
+DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2}

@@ -37,14 +37,13 @@ static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* wei
     b200tts_conv1d* h = new (std::nothrow) b200tts_conv1d();
     if (!h) { set_error("conv1d_create: out of host memory"); return 1; }
     h->c = *cfg;
-    h->L.prec = precision;
+    h->L.tc_prec = allow_tensor_cores ? precision : TC_NONE;
     int rc = cfg->transposed
                  ? pack_conv_transpose(h->L, weight, bias, cfg->in_channels, cfg->out_channels, cfg->kernel_size,
                                        cfg->stride, cfg->padding)
                  : pack_conv(h->L, weight, bias, cfg->out_channels, cfg->in_channels, cfg->kernel_size, cfg->dilation,
                              cfg->padding);
     if (rc) { delete h; return rc; }
-    h->L.allow_tc = allow_tensor_cores != 0;
     *out = h;
     return 0;
 }

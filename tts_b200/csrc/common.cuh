@@ -84,6 +84,8 @@ inline void count_launch(int n = 1) { g_launch_count += (unsigned long long)n; }
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3 };  // LOGCLAMP: log(max(v, act_param))
 enum : int { EPI_GATE = 1, EPI_MASK_PRE = 2, EPI_MASK_POST = 4, EPI_ACCUM = 8, EPI_SPLIT = 16, EPI_ACCUM2 = 32 };
 
+enum : int { TC_NONE = -1 };  // ConvLayer::tc_prec: no tensor-core images
+
 struct ConvLayer {            // immutable after pack(); owned by an engine handle
     float* w = nullptr;       // device, packed [row_tiles][CinPad][K][CO_T]
     float* bias = nullptr;    // device, [RowsPad] (zeros when the layer has no bias)
@@ -93,16 +95,13 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     int ups = 1;              // >1: polyphase ConvTranspose1d
     int co_tile = 64;         // 32 or 64
     int tr_kernel = 0, tr_pad = 0;  // original transposed-conv kernel size / padding (for Tout)
-    float* w_tc = nullptr;    // device, tensor-core packing [n_tile][chunk][tap]{hi,lo}[slab][N][4] (null: layer not eligible)
-    int tc_n = 0;             // output rows per tensor-core tile
-    float* w_tcg = nullptr;   // device, grouped tensor-core packing [chunk][tap block]{hi,lo}[slab][128][4] (rows == 32 / 64)
-    int tc_grp = 0;           // tap groups of the grouped packing (128 / rows), 0: none
-    bool allow_tc = false;    // engines opt layers into the 3xTF32 tensor-core path (decoder / flow); the text and
-                              // duration path stays on the exact FP32 FMA kernel so durations remain bit-stable
-    int prec = 0;             // tensor-core operand type, B200TTS_PRECISION_* (set BEFORE packing): 0 = 3xTF32; bf16 / fp16
-                              // pack the 16-bit weights below instead when Cin % 16 == 0 (otherwise the layer stays 3xTF32)
-    uint16_t* w_tc16 = nullptr;   // device, 16-bit packing [n_tile][chunk of 16][tap][slab][N][8] (null: none)
-    uint16_t* w_tcg16 = nullptr;  // device, 16-bit grouped packing [chunk of 16][tap block][slab][128][8] (rows == 32 / 64)
+    // tensor cores: set BEFORE packing to TC_NONE or the requested operand type (B200TTS_PRECISION_*); packing records the
+    // type of the images it built (a 16-bit request with Cin % 16 != 0 gets 3xTF32; no image: TC_NONE).  The text and
+    // duration path requests none, so durations stay bit-stable on the exact FP32 FMA kernel.
+    int tc_prec = TC_NONE;
+    void* w_tc = nullptr;     // device, plain image: [128-row tile][chunk][tap] weight blocks (rows >= 32), see pack_tc
+    void* w_tcg = nullptr;    // device, grouped image: [chunk][tap block] weight blocks (rows == 32 / 64), null: none
+    int tc_grp = 0;           // tap groups of the grouped image (128 / rows), 0: none
 };
 
 struct ConvIO {
@@ -145,7 +144,7 @@ void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
 // which kernel family a launch_conv call dispatched to (recorded per thread between dispatch_begin/end; tests pin it)
-enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6, DISPATCH_RESBLOCK = 7,
+enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6,
              DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9 };   // TC16*: the same kernels with bf16 / fp16 operands
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
@@ -155,7 +154,13 @@ inline int conv_transpose_out_len(const ConvLayer& L, int Tin) {
 }
 
 // small helpers shared by the engines
-int upload(float** dst, const float* src, size_t n);   // cudaMalloc + H2D copy
+template <class T> inline int upload(T** dst, const T* src, size_t n) {   // cudaMalloc + H2D copy (null for n == 0)
+    *dst = nullptr;
+    if (n == 0) return 0;
+    B200_CUDA_OK(cudaMalloc((void**)dst, n * sizeof(T)));
+    B200_CUDA_OK(cudaMemcpy(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+}
 
 // ------------------------------------------------------------------ bump allocator over a caller workspace
 struct Arena {

@@ -22,7 +22,6 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdarg.h>
-#include <stdlib.h>
 #include <string.h>
 
 namespace b200tts {
@@ -38,14 +37,6 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 const char* last_error() { return g_err; }
-
-int upload(float** dst, const float* src, size_t n) {
-    *dst = nullptr;
-    if (n == 0) return 0;
-    B200_CUDA_OK(cudaMalloc((void**)dst, n * sizeof(float)));
-    B200_CUDA_OK(cudaMemcpy(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice));
-    return 0;
-}
 
 // ------------------------------------------------------------------ device helpers
 constexpr int CI_MAX = 16;  // CinPad granularity (largest input-channel chunk of any instantiation)
@@ -417,69 +408,56 @@ void free_conv(ConvLayer& L) {
     if (L.bias) cudaFree(L.bias);
     if (L.w_tc) cudaFree(L.w_tc);
     if (L.w_tcg) cudaFree(L.w_tcg);
-    if (L.w_tc16) cudaFree(L.w_tc16);
-    if (L.w_tcg16) cudaFree(L.w_tcg16);
-    L.w = L.bias = L.w_tc = L.w_tcg = nullptr;
-    L.w_tc16 = L.w_tcg16 = nullptr;
+    L.w = L.bias = nullptr;
+    L.w_tc = L.w_tcg = nullptr;
 }
 
-// fp32 -> the 16-bit operand type's bits, round to nearest even (what cvt.rn does to the activations on the device)
-static uint16_t to_16bit(float v, int prec) {
-    uint16_t u;
-    if (prec == tc::PREC_BF16) { const __nv_bfloat16 h = __float2bfloat16_rn(v); memcpy(&u, &h, 2); }
-    else { const __half h = __float2half_rn(v); memcpy(&u, &h, 2); }
-    return u;
-}
-static int upload16(uint16_t** dst, const std::vector<uint16_t>& src) {
-    *dst = nullptr;
-    B200_CUDA_OK(cudaMalloc((void**)dst, src.size() * sizeof(uint16_t)));
-    B200_CUDA_OK(cudaMemcpy(*dst, src.data(), src.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-    return 0;
-}
-
-// 16-bit tensor-core packings (bf16 / fp16 per L.prec; Cin % 16 == 0): the layouts of pack_rows below with 16-channel
-// chunks and no hi/lo split, one tap block = [2 slabs][128 rows][8] (4 KB).  The weight norm is already folded (in fp32)
-// into Wl; each weight is rounded once, here.
-static int pack_rows16(ConvLayer& L, const std::vector<float>& Wl, int rows, int Cin, int K) {
-    const int nchunk = Cin / tc::KC16;
-    const size_t blk = (size_t)2 * 128 * 8;
-    if (L.tc_n) {
-        const int N = L.tc_n, nt = (rows + N - 1) / N;
-        std::vector<uint16_t> Q((size_t)nt * nchunk * K * blk, 0);
-        for (int tile = 0; tile < nt; ++tile)
-            for (int c = 0; c < nchunk; ++c)
-                for (int k = 0; k < K; ++k) {
-                    uint16_t* dst = Q.data() + (((size_t)tile * nchunk + c) * K + k) * blk;
-                    for (int s2 = 0; s2 < 2; ++s2)
-                        for (int n = 0; n < N; ++n)
-                            for (int i = 0; i < 8; ++i) {
-                                const int r = tile * N + n, ci = c * tc::KC16 + 8 * s2 + i;
-                                const float v = r < rows ? Wl[((size_t)r * Cin + ci) * K + k] : 0.f;
-                                dst[((size_t)s2 * N + n) * 8 + i] = to_16bit(v, L.prec);
-                            }
-                }
-        if (upload16(&L.w_tc16, Q)) return 2;
-    }
-    L.tc_grp = 0;
-    if (L.ups == 1 && (rows == 32 || rows == 64)) {     // grouped: MMA row m = g * rows + co, tap block j carries tap G*j + g
-        const int G = 128 / rows, J = (K + G - 1) / G;
-        std::vector<uint16_t> Q((size_t)nchunk * J * blk, 0);
-        for (int c = 0; c < nchunk; ++c)
-            for (int j = 0; j < J; ++j) {
-                uint16_t* dst = Q.data() + ((size_t)c * J + j) * blk;
-                for (int s2 = 0; s2 < 2; ++s2)
-                    for (int m = 0; m < 128; ++m)
-                        for (int i = 0; i < 8; ++i) {
-                            const int g = m / rows, co = m % rows;
-                            const int k = G * j + g, ci = c * tc::KC16 + 8 * s2 + i;
-                            const float v = k < K ? Wl[((size_t)co * Cin + ci) * K + k] : 0.f;
-                            dst[((size_t)s2 * 128 + m) * 8 + i] = to_16bit(v, L.prec);
+// One tensor-core weight image (conv_tc3.cuh): per (128-row tile, input-channel chunk, tap block) the block the weight
+// loader copies with one cp.async.bulk, [slabs][128 MMA rows][16 B], slab s holding the chunk's channels s*SLC .. +SLC-1:
+//   3xTF32 (PREC_FP32): 8-channel chunks, {hi, lo}[2 slabs] of 4 floats, hi = v & 0xFFFFE000 (exact in TF32), lo = v - hi
+//   bf16 / fp16:        16-channel chunks, [2 slabs] of 8 values rounded to nearest even (as cvt.rn rounds the activations)
+// With G tap groups (1: plain; 128 / rows: grouped), MMA row m = g * (128 / G) + co of tile t carries weight row
+// t * 128 + co and, in tap block j, tap G * j + g.  Rows >= `rows`, taps >= K and channels >= Cin are zero.  The weight
+// norm is already folded (in fp32) into Wl; each weight is rounded once, here.
+static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G) {
+    const bool tf32 = prec == tc::PREC_FP32;
+    const int kc = tf32 ? tc3::KC2 : tc3::KC16, slc = kc / 2, ch = tc3::MROWS / G;
+    const int ntiles = (rows + tc3::MROWS - 1) / tc3::MROWS, nchunks = (Cin + kc - 1) / kc, J = (K + G - 1) / G;
+    const size_t slab = (size_t)tc3::MROWS * 16, blk = (tf32 ? 4 : 2) * slab;
+    std::vector<unsigned char> img((size_t)ntiles * nchunks * J * blk, 0);
+    for (int t = 0; t < ntiles; ++t)
+        for (int c = 0; c < nchunks; ++c)
+            for (int j = 0; j < J; ++j)
+                for (int m = 0; m < tc3::MROWS; ++m) {
+                    const int r = t * tc3::MROWS + m % ch, k = G * j + m / ch;
+                    if (r >= rows || k >= K) continue;
+                    unsigned char* row = img.data() + (((size_t)t * nchunks + c) * J + j) * blk + (size_t)m * 16;
+                    for (int i = 0; i < kc && c * kc + i < Cin; ++i) {
+                        const float v = Wl[((size_t)r * Cin + c * kc + i) * K + k];
+                        unsigned char* p = row + (i / slc) * slab;
+                        const int e = i % slc;
+                        if (tf32) {
+                            uint32_t u;
+                            memcpy(&u, &v, 4);
+                            u &= 0xFFFFE000u;
+                            float hi;
+                            memcpy(&hi, &u, 4);
+                            const float lo = v - hi;
+                            memcpy(p + 4 * e, &hi, 4);
+                            memcpy(p + 2 * slab + 4 * e, &lo, 4);
+                        } else if (prec == tc::PREC_BF16) {
+                            const __nv_bfloat16 h = __float2bfloat16_rn(v);
+                            memcpy(p + 2 * e, &h, 2);
+                        } else {
+                            const __half h = __float2half_rn(v);
+                            memcpy(p + 2 * e, &h, 2);
                         }
-            }
-        if (upload16(&L.w_tcg16, Q)) return 2;
-        L.tc_grp = G;
-    }
-    return 0;
+                    }
+                }
+    unsigned char* d = nullptr;
+    const int rc = upload(&d, img.data(), img.size());
+    *dst = d;
+    return rc;
 }
 
 // Wl(r, ci, k): logical weights already expressed as a correlation-form conv with `rows` GEMM rows
@@ -503,69 +481,16 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     for (int r = 0; r < rows; ++r) bp[r] = bl[r];
     if (upload(&L.w, P.data(), P.size())) return 2;
     if (upload(&L.bias, bp.data(), bp.size())) return 2;
-    // tensor-core packing (3xTF32 hi/lo split) for layers the wgmma kernel can take
-    // rows >= 32: tiles of 128 zero-padded rows (M = 128: two m64 warpgroups); exactly 32 / 64 rows additionally get the grouped
-    // packing below (no padding), which the dispatcher prefers; fewer rows run on the FP32-FMA kernel
-    // L.prec (set before packing) = bf16 / fp16 with Cin % 16 == 0: the 16-bit packings instead (pack_rows16); any other
-    // Cin keeps the 3xTF32 packing, so the layer's launches show up as tc3 / tc3_grouped in the dispatch log
-    L.tc_n = 0;
-    if (rows >= 32) L.tc_n = 128;
-    if (L.prec != tc::PREC_FP32 && Cin % tc::KC16 == 0) return pack_rows16(L, Wl, rows, Cin, K);
-    if (L.tc_n && rows >= 16 && Cin >= 8) {
-        using namespace tc;
-        const int N = L.tc_n, nt = (rows + N - 1) / N, nchunk = (Cin + KC - 1) / KC;
-        const size_t blk = (size_t)2 * NSLAB * N * 4;
-        std::vector<float> Q((size_t)nt * nchunk * K * blk, 0.f);
-        for (int tile = 0; tile < nt; ++tile)
-            for (int c = 0; c < nchunk; ++c)
-                for (int k = 0; k < K; ++k) {
-                    float* dst = Q.data() + (((size_t)tile * nchunk + c) * K + k) * blk;
-                    for (int s2 = 0; s2 < NSLAB; ++s2)
-                        for (int n = 0; n < N; ++n)
-                            for (int i = 0; i < 4; ++i) {
-                                const int r = tile * N + n, ci = c * KC + 4 * s2 + i;
-                                const float v = (ci < Cin && r < rows) ? Wl[((size_t)r * Cin + ci) * K + k] : 0.f;
-                                uint32_t u;
-                                memcpy(&u, &v, 4);
-                                u &= 0xFFFFE000u;
-                                float hi;
-                                memcpy(&hi, &u, 4);
-                                dst[((size_t)s2 * N + n) * 4 + i] = hi;
-                                dst[((size_t)(NSLAB + s2) * N + n) * 4 + i] = v - hi;
-                            }
-                }
-        if (upload(&L.w_tc, Q.data(), Q.size())) return 2;
-    } else {
-        L.tc_n = 0;
-    }
-    // grouped packing for exactly 32 / 64 rows (conv_tc3.cuh, grouped mode): MMA row m = g * rows + co holds channel co
-    // and tap group g; tap block j carries tap G*j + g (zero beyond K)
-    L.tc_grp = 0;
-    if (L.ups == 1 && (rows == 32 || rows == 64) && Cin >= 8) {
-        using namespace tc;
-        const int G = 128 / rows, J = (K + G - 1) / G, nchunk = (Cin + KC - 1) / KC;
-        const size_t blk = (size_t)2 * NSLAB * 128 * 4;
-        std::vector<float> Q((size_t)nchunk * J * blk, 0.f);
-        for (int c = 0; c < nchunk; ++c)
-            for (int j = 0; j < J; ++j) {
-                float* dst = Q.data() + ((size_t)c * J + j) * blk;
-                for (int s2 = 0; s2 < NSLAB; ++s2)
-                    for (int m = 0; m < 128; ++m)
-                        for (int i = 0; i < 4; ++i) {
-                            const int g = m / rows, co = m % rows;
-                            const int k = G * j + g, ci = c * KC + 4 * s2 + i;
-                            const float v = (ci < Cin && k < K) ? Wl[((size_t)co * Cin + ci) * K + k] : 0.f;
-                            uint32_t u;
-                            memcpy(&u, &v, 4);
-                            u &= 0xFFFFE000u;
-                            float hi;
-                            memcpy(&hi, &u, 4);
-                            dst[((size_t)s2 * 128 + m) * 4 + i] = hi;
-                            dst[((size_t)(NSLAB + s2) * 128 + m) * 4 + i] = v - hi;
-                        }
-            }
-        if (upload(&L.w_tcg, Q.data(), Q.size())) return 2;
-        L.tc_grp = G;
+    // tensor-core images for a layer that requests them: rows >= 32 get the plain image (M = 128: two m64 warpgroups);
+    // exactly 32 / 64 rows also get the grouped one (no padding), which the dispatcher prefers.  3xTF32 needs Cin >= 8, and
+    // a 16-bit request packs 3xTF32 unless Cin % 16 == 0, so such a layer shows up as tc3 / tc3_grouped in the dispatch log
+    if (L.tc_prec != TC_NONE && Cin % tc3::KC16 != 0) L.tc_prec = tc::PREC_FP32;
+    if (rows < 32 || Cin < tc3::KC2) L.tc_prec = TC_NONE;
+    if (L.tc_prec == TC_NONE) return 0;
+    if (pack_tc(&L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1)) return 2;
+    if (L.ups == 1 && (rows == 32 || rows == 64)) {
+        if (pack_tc(&L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows)) return 2;
+        L.tc_grp = tc3::MROWS / rows;
     }
     return 0;
 }
@@ -749,12 +674,10 @@ static int launch_tiles(const ConvKArgs& a, int co_tile, int B, int RowsPad, cud
     if (co_tile == 64) {
         if constexpr (EPI == KEPI_PLAIN) {
             // launch-starved shape (fewer CTAs than SMs, long channel loop): split the channel chunks over 4 warp groups
-            static int splitk = -1;
-            if (splitk < 0) { const char* e = getenv("B200TTS_NO_SPLITK"); splitk = (e && atoi(e)) ? 0 : 1; }
             const long long ctas = (long long)((a.Tq + 63) / 64) * (RowsPad / 64) * B;
             const int nchunks = (a.Cin + CIC - 1) / CIC;
             const size_t smem4 = (size_t)4 * (2 * CIC * round_up(64 + (a.K - 1) * a.dil, 4) + 2 * CIC * a.K * 64) * sizeof(float);
-            if (splitk && small_t && ctas <= 160 && nchunks >= 8 && smem4 <= 200 * 1024)
+            if (small_t && ctas <= 160 && nchunks >= 8 && smem4 <= 200 * 1024)
                 return launch_variant<16, 2, 4, 1, CIC, EPI, 4>(a, B, RowsPad, st);
         }
         if (small_t) return launch_variant<16, 2, 4, 1, CIC, EPI>(a, B, RowsPad, st);
@@ -793,10 +716,8 @@ static TcDevice g_tc_dev[MAX_DEVICES];
 static DeviceOnce g_tc_once;
 
 // launch with programmatic stream serialization: the kernel may be scheduled while its predecessor drains (the kernel
-// itself waits with griddepcontrol.wait before touching activations).  B200TTS_NO_PDL=1 restores plain launches.
+// itself waits with griddepcontrol.wait before touching activations).
 static cudaError_t launch_tc3(tc3::Tc3Kernel k, int grid, size_t smem, cudaStream_t st, const tc3::Tc3Args& t) {
-    static int pdl = -1;
-    if (pdl < 0) { const char* e = getenv("B200TTS_NO_PDL"); pdl = (e && atoi(e)) ? 0 : 1; }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(tc3::NTHREADS2);
@@ -806,7 +727,7 @@ static cudaError_t launch_tc3(tc3::Tc3Kernel k, int grid, size_t smem, cudaStrea
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
-    cfg.numAttrs = pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, k, t);
 }
 // ragged batches: the prefix table lives behind everything else in dynamic shared memory (when it still fits)
@@ -830,14 +751,7 @@ static void set_window(tc3::Tc3Args& t, const ConvKArgs& a) {
 }
 
 static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& a, cudaStream_t st) {
-    static int enabled = -1, grouped_enabled = 1;
-    if (enabled < 0) {
-        const char* e3 = getenv("B200TTS_NO_TCG");
-        grouped_enabled = (e3 && atoi(e3)) ? 0 : 1;
-        const char* e = getenv("B200TTS_NO_TC");
-        enabled = (e && atoi(e)) ? 0 : 1;
-    }
-    if (!enabled || !L.allow_tc || (!L.w_tc && !L.w_tcg && !L.w_tc16 && !L.w_tcg16) || a.Tq < 128) return -1;
+    if (L.tc_prec == TC_NONE || a.Tq < 128) return -1;
     if (a.act == ACT_LOGCLAMP || a.act == ACT_TANH) return -1;
     if (!(a.in_slope >= 0.f && a.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
     const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
@@ -864,81 +778,52 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const size_t max_smem = (size_t)g_tc_dev[dev].max_smem;
     B200_REQUIRE(*reinterpret_cast<volatile int*>(g_tc_err) == 0,
                  "tensor-core conv: an earlier launch on device %d hit a pipeline timeout (its output is invalid)", dev);
-    const int rows_pad = (tc::TT + (L.K - 1) * L.dil + 7) / 8 * 8;
-    // ---- persistent kernel (needs 16-byte aligned activation rows for its cp.async staging; no input mask)
+    // persistent kernels: 16-byte aligned activation rows for the cp.async staging, no input mask
     const bool aligned = ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.x_cs % 4 == 0) && (a.x_bs % 4 == 0);
-    const int n_rtiles = (L.Rows + L.tc_n - 1) / L.tc_n;
     const bool persistent_ok = aligned && !a.xmask &&
                                (L.ups == 1 || (!a.res && !(a.flags & EPI_ACCUM) && !a.ymask && !a.cond));
-    // 16-bit operands (L.prec, packed only when Cin % 16 == 0) wherever FP32 would take tc3 / tc3_grouped
-    const int pg = L.w_tcg16 ? L.prec : tc::PREC_FP32, pp = L.w_tc16 ? L.prec : tc::PREC_FP32;
-    if (grouped_enabled && persistent_ok && L.tc_grp && (L.w_tcg || L.w_tcg16) && L.ups == 1 && !needs_v3 && !a.ymask &&
-        (L.tc_grp - 1) * L.dil <= 15 && a.Tq >= 256) {
-        // grouped mode: M = tap groups x channels, N = 256 time steps, 240 per tile
-        const int G = L.tc_grp, J = (L.K + G - 1) / G;
-        const int rp = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
-        if (rp <= 320 && tc3::smem_bytes3(rp, pg) <= max_smem) {
-            tc3::Tc3Args t;
-            memset(&t, 0, sizeof(t));
-            t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-            t.w = pg ? (const void*)L.w_tcg16 : (const void*)L.w_tcg; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
-            t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = 128;
-            t.KJ = J; t.dil_blk = G * L.dil; t.tstep = tc3::TSTEP_GROUPED;
-            t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = 1; t.Tq = a.Tq;
-            t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
-            t.scale = a.scale; t.post_div = a.post_div; t.relu = (a.act == ACT_RELU); t.accum = (a.flags & EPI_ACCUM) ? 1 : 0;
-            t.rows_pad = rp; t.raw_w = rp + 4;
-            t.B = io.B; t.n_rtiles = 1;
-            set_window(t, a);
-            t.err = g_tc_err;
-            size_t smemg = tc3::smem_bytes3(rp, pg);
-            set_ragged(t, a, smemg, max_smem);
-            const long long tiles = (long long)t.B * t.n_ttiles;
-            const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
-            B200_CUDA_OK(launch_tc3(tc3::grouped_kernel(G, pg), grid, smemg, st, t));
-            count_launch();
-            dispatch_note(pg ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED);
-            B200_CUDA_OK(cudaGetLastError());
-            return 0;
-        }
-    }
-    if (persistent_ok && L.tc_n == 128 && (L.w_tc || L.w_tc16) && rows_pad <= 320 && tc3::smem_bytes3(rows_pad, pp) <= max_smem) {
-        // M = rows (128, zero padded), N = 256 time steps
-        tc3::Tc3Args t;
-        memset(&t, 0, sizeof(t));
-        t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-        t.w = pp ? (const void*)L.w_tc16 : (const void*)L.w_tc; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
-        t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = 128;
-        t.KJ = L.K; t.dil_blk = L.dil; t.tstep = tc3::TT2;
-        t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
-        t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
-        t.ymask = a.ymask; t.ymask_bs = a.ymask_bs;
-        t.scale = a.scale; t.post_div = a.post_div; t.relu = (a.act == ACT_RELU); t.accum = (a.flags & EPI_ACCUM) ? 1 : 0;
-        t.mask_post = (a.flags & EPI_MASK_POST) ? 1 : 0;
-        t.mask_pre = (a.flags & EPI_MASK_PRE) ? 1 : 0;
-        t.gate = (a.flags & EPI_GATE) ? 1 : 0;
-        t.split = (a.flags & EPI_SPLIT) ? a.split : 0;
-        t.y2 = a.y2; t.y2_bs = a.y2_bs; t.y2_cs = a.y2_cs; t.accum2 = (a.flags & EPI_ACCUM2) ? 1 : 0;
-        t.rows_pad = rows_pad; t.raw_w = rows_pad + 4;
-        t.B = io.B; t.n_rtiles = n_rtiles;
-        set_window(t, a);
-        t.err = g_tc_err;
-        size_t smem3 = tc3::smem_bytes3(rows_pad, pp);
-        // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
-        // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
-        const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
-        set_ragged(t, a, smem3, max_smem);
-        const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
-        const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
-        B200_CUDA_OK(launch_tc3(tc3::plain_kernel(pp, plain_epi), grid, smem3, st, t));
-        count_launch();
-        dispatch_note(pp ? DISPATCH_TC16 : DISPATCH_TC3);
-        B200_CUDA_OK(cudaGetLastError());
-        return 0;
-    }
-    // Everything else (fewer than 64 rows without a grouped packing, unaligned or masked inputs, shared-memory budget)
-    // runs on the exact FP32-FMA kernel.
-    return -1;
+    auto fits = [&](int rp) { return rp <= 320 && tc3::smem_bytes3(rp, L.tc_prec) <= max_smem; };
+    // grouped mode for the layers with a grouped image: M = tap groups x channels, N = 256 time steps, 240 per tile
+    const int G = L.tc_grp, J = G ? (L.K + G - 1) / G : 0;
+    const int rp_grouped = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
+    const bool grouped = G && !needs_v3 && !a.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
+    // plain mode otherwise: M = rows (128 per tile, zero padded), N = 256 time steps.  Everything neither mode takes
+    // (unaligned or masked inputs, shared-memory budget) runs on the exact FP32-FMA kernel.
+    const int rows_pad = grouped ? rp_grouped : (tc3::TT2 + (L.K - 1) * L.dil + 7) / 8 * 8;
+    if (!persistent_ok || !fits(rows_pad)) return -1;
+    tc3::Tc3Args t;
+    memset(&t, 0, sizeof(t));
+    t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
+    t.w = grouped ? L.w_tcg : L.w_tc; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
+    t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = tc3::MROWS;
+    t.KJ = grouped ? J : L.K; t.dil_blk = grouped ? G * L.dil : L.dil; t.tstep = grouped ? tc3::TSTEP_GROUPED : tc3::TT2;
+    t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
+    t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
+    t.ymask = a.ymask; t.ymask_bs = a.ymask_bs;
+    t.scale = a.scale; t.post_div = a.post_div; t.relu = (a.act == ACT_RELU); t.accum = (a.flags & EPI_ACCUM) ? 1 : 0;
+    t.mask_post = (a.flags & EPI_MASK_POST) ? 1 : 0;
+    t.mask_pre = (a.flags & EPI_MASK_PRE) ? 1 : 0;
+    t.gate = (a.flags & EPI_GATE) ? 1 : 0;
+    t.split = (a.flags & EPI_SPLIT) ? a.split : 0;
+    t.y2 = a.y2; t.y2_bs = a.y2_bs; t.y2_cs = a.y2_cs; t.accum2 = (a.flags & EPI_ACCUM2) ? 1 : 0;
+    t.rows_pad = rows_pad; t.raw_w = rows_pad + 4;
+    t.B = io.B; t.n_rtiles = (L.Rows + tc3::MROWS - 1) / tc3::MROWS;   // 1 in grouped mode (32 / 64 rows)
+    set_window(t, a);
+    t.err = g_tc_err;
+    size_t smem = tc3::smem_bytes3(rows_pad, L.tc_prec);
+    set_ragged(t, a, smem, max_smem);
+    // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
+    // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
+    const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
+    const tc3::Tc3Kernel k = grouped ? tc3::grouped_kernel(G, L.tc_prec) : tc3::plain_kernel(L.tc_prec, plain_epi);
+    const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
+    const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
+    B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));
+    count_launch();
+    const bool b16 = L.tc_prec != tc::PREC_FP32;
+    dispatch_note(grouped ? (b16 ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED) : (b16 ? DISPATCH_TC16 : DISPATCH_TC3));
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 int conv_tc_error_flag() {   // 1 if any tensor-core launch (on any device) hit a pipeline timeout; call after a sync

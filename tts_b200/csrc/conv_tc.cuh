@@ -26,10 +26,6 @@
 namespace b200tts {
 namespace tc {
 
-constexpr int TT = 256;          // time steps per tile (wgmma N)
-constexpr int NSLAB = 2;         // 4-channel slabs per activation stage
-constexpr int KC = 4 * NSLAB;    // input channels per stage (one MMA k-step per 2 slabs)
-constexpr int KC16 = 16;         // input channels per stage with 16-bit operands (one k16 step per 2 slabs)
 // tensor-core operand type (the values of B200TTS_PRECISION_* in include/tts_b200.h)
 enum : int { PREC_FP32 = 0, PREC_BF16 = 1, PREC_FP16 = 2 };
 constexpr uint32_t SPIN_LIMIT = 1u << 22;

@@ -37,6 +37,7 @@ using namespace tc;       // smem_u32, mbar_*, make_desc, wgmma_*
 constexpr int TT2 = 256;          // time steps per tile = MMA N
 constexpr int MROWS = 128;        // output rows per tile (weight rows are zero padded up to it): two m64 warpgroups
 constexpr int KC2 = 8;            // input channels per chunk (2 slabs, one MMA k-step)
+constexpr int KC16 = 16;          // input channels per chunk with 16-bit operands (2 slabs, one k16 step)
 constexpr int RAWS = 324;         // raw (cp.async) row stride in floats: the widest window (320 slab rows + 4), a constant so
                                   // that the transform's shared loads use immediate offsets
 constexpr int NRAW = 3;           // raw (cp.async) ring depth

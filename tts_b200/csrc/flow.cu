@@ -32,6 +32,7 @@ int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers
     res_skip.resize(L);
     int d = 1;
     for (int l = 0; l < L; ++l) {
+        in_layers[l].tc_prec = res_skip[l].tc_prec = B200TTS_PRECISION_FP32;   // ~85% of the flow FLOPs (k5, 192 -> 384)
         if ((rc = pack_conv(in_layers[l], w[i], w[i + 1], 2 * H, H, K, d, (K * d - d) / 2, /*gate_half=*/H))) return rc;
         i += 2;
         const int rows = (l < L - 1) ? 2 * H : H;
@@ -39,8 +40,6 @@ int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers
         i += 2;
         d *= dilation_rate;
     }
-    for (auto& l : in_layers) l.allow_tc = true;     // ~85% of the flow FLOPs (k5, 192 -> 384)
-    for (auto& l : res_skip) l.allow_tc = true;
     *consumed = i;
     return 0;
 }
@@ -111,6 +110,7 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
         b->odd = fwd ? (n % 2) == 1 : ((c.num_flows - n) % 2) == 1;
         const float* const* wn = w + (size_t)n * per;
         int rc, used = 0;
+        b->pre.tc_prec = b->post.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(b->pre, wn[0], wn[1], c.hidden_channels, half, 1, 1, 0, 0, b->odd ? rev.data() : nullptr,
                             nullptr)))
             return rc;
@@ -120,8 +120,6 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
         if ((rc = pack_conv(b->post, wn[2 + used], wn[3 + used], half, c.hidden_channels, 1, 1, 0, 0, nullptr,
                             b->odd ? rev.data() : nullptr)))
             return rc;
-        b->pre.allow_tc = true;
-        b->post.allow_tc = true;
     }
     return 0;
 }
@@ -200,11 +198,10 @@ int PosteriorEnc::init(const b200tts_posterior_config& cfg, const float* const* 
     const int expect = 2 + (c.cond_channels > 0 ? 2 : 0) + 4 * c.num_layers + 2;
     B200_REQUIRE(nw == expect, "posterior_encoder: expected %d weight tensors, got %d", expect, nw);
     int rc, used = 0;
+    pre.tc_prec = proj.tc_prec = B200TTS_PRECISION_FP32;
     if ((rc = pack_conv(pre, w[0], w[1], c.hidden_channels, c.in_channels, 1, 1, 0))) return rc;
     if ((rc = wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, w + 2, &used))) return rc;
     if ((rc = pack_conv(proj, w[2 + used], w[3 + used], 2 * c.out_channels, c.hidden_channels, 1, 1, 0))) return rc;
-    pre.allow_tc = true;
-    proj.allow_tc = true;
     return 0;
 }
 

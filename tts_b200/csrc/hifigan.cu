@@ -15,8 +15,8 @@ Hifigan::~Hifigan() {
 }
 
 // weights: host pointers, canonical order (see include/tts_b200.h).  precision (B200TTS_PRECISION_*): the tensor-core
-// operand type of conv_pre, the upsamplers and every resblock conv -- the layers that run on the wgmma kernels; cond and
-// conv_post stay fp32, and so does every margin, workspace size and launch window.
+// operand type of conv_pre, the upsamplers and every resblock conv -- the layers that run on the wgmma kernels (~97% of
+// the FLOPs); cond and conv_post stay fp32, and so does every margin, workspace size and launch window.
 int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int nw, int precision) {
     c = cfg;
     B200_REQUIRE(precision == B200TTS_PRECISION_FP32 || precision == B200TTS_PRECISION_BF16 ||
@@ -31,7 +31,7 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
                        c.num_upsamples * c.num_kernels * c.num_dilations * (type1 ? 4 : 2) + 2;
     B200_REQUIRE(nw == expect, "hifigan: expected %d weight tensors, got %d", expect, nw);
     int i = 0;
-    conv_pre.prec = prec;
+    conv_pre.tc_prec = prec;
     int rc = pack_conv(conv_pre, w[i], w[i + 1], c.upsample_initial_channel, c.in_channels, 7, 1, 3);
     if (rc) return rc;
     i += 2;
@@ -46,7 +46,7 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
     int ch = c.upsample_initial_channel;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int u = c.upsample_factors[s], k = c.upsample_kernel_sizes[s];
-        ups[s].prec = prec;
+        ups[s].tc_prec = prec;
         rc = pack_conv_transpose(ups[s], w[i], w[i + 1], ch, ch / 2, k, u, (k - u) / 2);
         if (rc) return rc;
         i += 2;
@@ -59,12 +59,12 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
             if (type1) v2.resize(c.num_dilations);
             for (int n = 0; n < c.num_dilations; ++n) {
                 const int d = c.resblock_dilations[j][n];
-                v1[n].prec = prec;
+                v1[n].tc_prec = prec;
                 rc = pack_conv(v1[n], w[i], w[i + 1], ch, ch, rk, d, (rk * d - d) / 2);
                 if (rc) return rc;
                 i += 2;
                 if (type1) {
-                    v2[n].prec = prec;
+                    v2[n].tc_prec = prec;
                     rc = pack_conv(v2[n], w[i], w[i + 1], ch, ch, rk, 1, (rk - 1) / 2);
                     if (rc) return rc;
                     i += 2;
@@ -73,11 +73,6 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
         }
     }
     rc = pack_conv(conv_post, w[i], w[i + 1], c.out_channels, ch, 7, 1, 3);
-    // the MRF / pre convs carry ~97% of the FLOPs: run them on the wgmma kernels (3xTF32, or the 16-bit operands above)
-    conv_pre.allow_tc = true;
-    for (auto& l : ups) l.allow_tc = true;
-    for (auto& v : rb_c1) for (auto& l : v) l.allow_tc = true;
-    for (auto& v : rb_c2) for (auto& l : v) l.allow_tc = true;
     if (rc == 0) plan_margins();
     return rc;
 }

@@ -412,8 +412,8 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
         BN b;
         if ((rc = bn(F0, b))) return rc;
         std::vector<float> r = repack3x3(cw, F0, 1, nullptr);
+        conv1.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(conv1, r.data(), cb, F0, 3, 3, 1, 1))) return rc;
-        conv1.allow_tc = true;
         if ((rc = upload_d(&s0, b.s)) || (rc = upload_d(&t0, b.t))) return rc;
     }
     int Cprev = F0;
@@ -430,6 +430,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
             if ((rc = bn(b.C, b2))) return rc;
             const float *f1w = next(), *f1b = next(), *f2w = next(), *f2b = next();
             B200_REQUIRE(w1 && w2 && f1w && f1b && f2w && f2b, "speaker_encoder: missing block weights");
+            b.c1.tc_prec = b.c2.tc_prec = B200TTS_PRECISION_FP32;
             if (b.down) {
                 std::vector<float> r = repack3x3_s2(w1, b.C, b.Cin);
                 if ((rc = pack_conv(b.c1, r.data(), nullptr, b.C, 6 * b.Cin, 2, 1, 1))) return rc;
@@ -454,9 +455,9 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
                 std::vector<float> r((size_t)b.C * b.Cin), bias(bd.t.begin(), bd.t.end());
                 for (int co = 0; co < b.C; ++co)
                     for (int ci = 0; ci < b.Cin; ++ci) r[(size_t)co * b.Cin + ci] = (float)(dw[(size_t)co * b.Cin + ci] * bd.s[co]);
+                b.ds.tc_prec = B200TTS_PRECISION_FP32;
                 if ((rc = pack_conv(b.ds, r.data(), bias.data(), b.C, b.Cin, 1, 1, 0))) return rc;
             }
-            b.c1.allow_tc = b.c2.allow_tc = b.ds.allow_tc = true;
         }
         Cprev = c.num_filters[s];
     }
@@ -472,6 +473,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
         std::vector<int> perm(Ca);
         for (int cc = 0; cc < C4; ++cc)
             for (int h = 0; h < Hf; ++h) perm[cc * Hf + h] = h * C4 + cc;
+        att1.tc_prec = att2.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(att1, aw, ab, 128, Ca, 1, 1, 0, 0, perm.data()))) return rc;
         // BatchNorm1d after the ReLU folded into the following 1x1 conv: W3 (s x + t) + b3
         std::vector<float> r((size_t)Ca * 128), bias(Ca);
@@ -484,13 +486,12 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
             bias[o] = (float)acc;
         }
         if ((rc = pack_conv(att2, r.data(), bias.data(), Ca, 128, 1, 1, 0))) return rc;
-        att1.allow_tc = att2.allow_tc = true;
     }
     {
         const float *fw = next(), *fb = next();
         B200_REQUIRE(fw && fb, "speaker_encoder: missing fc");
+        fc.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(fc, fw, fb, c.proj_dim, (c.encoder_type ? 2 : 1) * Ca, 1, 1, 0))) return rc;
-        fc.allow_tc = true;
     }
     B200_REQUIRE(i == nw, "speaker_encoder: expected %d weight tensors, got %d", i, nw);
     return 0;
