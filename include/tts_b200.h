@@ -352,7 +352,8 @@ int b200tts_sdp_reverse(const b200tts_sdp* h, const float* x, const float* mask,
  *                     *err_flag (the duration predictor's spline flag, may be NULL -> 0)}: the one host read of
  *                     Vits.inference (sequence_mask(y_lengths, None), helpers.py:53-54) fetches both.
  * b200tts_expand_prior (after the caller has read max(y_lengths) = Ty): attn [B,Tx,Ty] one-hot (or NULL),
- *   m_p / logs_p / z_p [B,C,Ty] with z_p = m_p + noise * exp(logs_p) * noise_scale, y_mask [B,Ty] (or NULL);
+ *   m_p / logs_p / z_p [B,C,Ty] with z_p = m_p + noise * exp(logs_p) * noise_scale (z_p may be NULL, and then noise
+ *   too), y_mask [B,Ty] (or NULL);
  *   stats is the text encoder's [B,2C,Tx]; noise [B,C,Ty] is the randn_like(m_p) draw of vits.py:1155.
  */
 int b200tts_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
@@ -425,6 +426,66 @@ int b200tts_speaker_encoder_forward(const b200tts_speaker_encoder* h, const floa
 int b200tts_speaker_encoder_features(const b200tts_speaker_encoder* h, const float* x, const int32_t* starts, int B,
                                      int T, int stage, float* out, void* workspace, size_t workspace_bytes,
                                      void* stream);
+
+/* ---- Glow-TTS inference (text -> mel spectrogram) ----------------------------------------------
+ * Replaces GlowTTS.inference, TTS/tts/models/glow_tts.py:342-374, for encoder_type "rel_pos_transformer" (no
+ * relative-position window, layer_norm_type "1": LayerNorm over channels with eps 1e-4), in two calls around the one
+ * host read of the decoder length: encode (encoder + durations), then decode (path, prior, Glow decoder in reverse).
+ * weights (host, PyTorch layouts, weight norm folded), state-dict order:
+ *   encoder.emb.weight [n_vocab, H]
+ *   if use_prenet: 3 x (prenet.conv_layers.i.w [H,H,5], .b, prenet.norm_layers.i.gamma [H], .beta), prenet.proj.w [H,H,1], .b
+ *   per transformer layer: conv_q.w [H,H,1], .b, conv_k.w, .b, conv_v.w, .b, conv_o.w, .b, norm_layers_1.gamma [H],
+ *     .beta, ffn.conv_1.w [F,H,k], .b, ffn.conv_2.w [H,F,k], .b, norm_layers_2.gamma, .beta
+ *   proj_m.w [C,H,1], .b, (unless mean_only) proj_s.w [C,H,1], .b
+ *   duration_predictor: conv_1.w [Fdp, H+c_in, 3], .b, norm_1.gamma [Fdp], .beta, conv_2.w [Fdp,Fdp,3], .b,
+ *     norm_2.gamma, .beta, proj.w [1,Fdp,1], .b
+ *   per decoder block n (flows 3n, 3n+1, 3n+2; Cs = C * num_squeeze, ns = num_splits):
+ *     ActNorm logs [Cs], bias [Cs]; the INVERSE of InvConvNear.weight [ns, ns] (torch.inverse(weight.float()), as
+ *     store_inverse computes it); start.w [Hd, Cs/2, 1], .b; WaveNet (cond_layer.w, .b if c_in_channels, then per layer
+ *     in_layers.i.w [2Hd,Hd,k], .b, res_skip_layers.i.w, .b); end.w [Cs, Hd, 1], .b
+ * encode: tokens int64 [B,Tt], lengths int64 [B], g [B, c_in_channels] (the l2-normalised speaker vector) or NULL ->
+ *   o_stats [B, 2C, Tt] (o_mean rows [0,C), o_log_scale rows [C,2C)), logw [B,Tt] (durations_log), x_mask [B,Tt],
+ *   w_ceil [B,Tt], cum [B,Tt] (cumulative w_ceil), dur_log [B,Tt] (total_durations_log), y_lengths int64 [B],
+ *   meta int64 [2] = {max_b y_lengths, 0}: read it to size the decode call (Ty = meta[0]).
+ * decode: noise [B,C,Ty] (the randn_like(y_mean) draw of :361) or NULL (= noise_scale 0) ->
+ *   attn [B,Tt,Ty] (or NULL), y_mean / y_log_scale [B,C,Ty], mel [B, C, Ty'] with Ty' = num_squeeze * (Ty / num_squeeze)
+ *   (the reference's model_outputs before its transpose to [B, Ty', C]).
+ * workspace_bytes(B, Tt, Ty) covers both calls.  No float atomics: repeat calls are bit-identical.
+ */
+typedef struct {
+    int n_vocab;
+    int out_channels;          /* mel channels C */
+    int hidden_channels_enc;   /* H */
+    int hidden_channels_ffn;   /* F */
+    int num_heads;
+    int num_layers_enc;
+    int kernel_size_enc;       /* transformer FFN kernel */
+    int use_prenet;
+    int mean_only;
+    int hidden_channels_dp;    /* Fdp */
+    int c_in_channels;         /* speaker vector size, 0: single speaker */
+    int hidden_channels_dec;   /* Hd */
+    int kernel_size_dec;
+    int dilation_rate;
+    int num_flow_blocks;
+    int num_block_layers;
+    int num_splits;
+    int num_squeeze;
+    int sigmoid_scale;
+} b200tts_glow_tts_config;
+typedef struct b200tts_glow_tts b200tts_glow_tts;
+int b200tts_glow_tts_create(const b200tts_glow_tts_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_glow_tts** out);
+void b200tts_glow_tts_destroy(b200tts_glow_tts* h);
+size_t b200tts_glow_tts_workspace_bytes(const b200tts_glow_tts* h, int B, int Tt, int Ty);
+int b200tts_glow_tts_encode(const b200tts_glow_tts* h, const int64_t* tokens, const int64_t* lengths, const float* g,
+                            float length_scale, int B, int Tt, float* o_stats, float* logw, float* x_mask, float* w_ceil,
+                            float* cum, float* dur_log, int64_t* y_lengths, int64_t* meta, void* workspace,
+                            size_t workspace_bytes, void* stream);
+int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, const float* x_mask, const float* cum,
+                            const int64_t* y_lengths, const float* g, const float* noise, float noise_scale, int B, int Tt,
+                            int Ty, float* attn, float* y_mean, float* y_log_scale, float* mel, void* workspace,
+                            size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -69,6 +69,14 @@ class SpeakerEncoderConfigC(ctypes.Structure):
                                             "hop_length")]
 
 
+class GlowTTSConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "out_channels", "hidden_channels_enc", "hidden_channels_ffn",
+                                            "num_heads", "num_layers_enc", "kernel_size_enc", "use_prenet", "mean_only",
+                                            "hidden_channels_dp", "c_in_channels", "hidden_channels_dec",
+                                            "kernel_size_dec", "dilation_rate", "num_flow_blocks", "num_block_layers",
+                                            "num_splits", "num_squeeze", "sigmoid_scale")]
+
+
 class AudioNormC(ctypes.Structure):
     _fields_ = [("signal_norm", ctypes.c_int), ("symmetric_norm", ctypes.c_int), ("clip_norm", ctypes.c_int),
                 ("max_norm", ctypes.c_float), ("min_level_db", ctypes.c_float), ("ref_level_db", ctypes.c_float),
@@ -171,6 +179,18 @@ def _declare(lib):
     lib.b200tts_speaker_encoder_forward.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, vp, sz, vp]
     lib.b200tts_speaker_encoder_features.restype = ci
     lib.b200tts_speaker_encoder_features.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_glow_tts_create.restype = ci
+    lib.b200tts_glow_tts_create.argtypes = [ctypes.POINTER(GlowTTSConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+    lib.b200tts_glow_tts_destroy.restype = None
+    lib.b200tts_glow_tts_destroy.argtypes = [vp]
+    lib.b200tts_glow_tts_workspace_bytes.restype = sz
+    lib.b200tts_glow_tts_workspace_bytes.argtypes = [vp, ci, ci, ci]
+    lib.b200tts_glow_tts_encode.restype = ci
+    lib.b200tts_glow_tts_encode.argtypes = [vp, vp, vp, vp, ctypes.c_float, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                            sz, vp]
+    lib.b200tts_glow_tts_decode.restype = ci
+    lib.b200tts_glow_tts_decode.argtypes = [vp, vp, vp, vp, vp, vp, vp, ctypes.c_float, ci, ci, ci, vp, vp, vp, vp, vp,
+                                            sz, vp]
     lib.b200tts_stft_create.restype = ci
     lib.b200tts_stft_create.argtypes = [ci, ci, vp, vp, ci, ctypes.POINTER(vp)]
     lib.b200tts_stft_destroy.restype = None

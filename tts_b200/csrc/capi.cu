@@ -13,6 +13,7 @@ struct b200tts_stft { Stft impl; };
 struct b200tts_posterior { PosteriorEnc impl; };
 struct b200tts_duration_predictor { DurPred impl; };
 struct b200tts_speaker_encoder { SpeakerEncoder impl; };
+struct b200tts_glow_tts { GlowTTS impl; };
 
 extern "C" {
 
@@ -324,6 +325,39 @@ int b200tts_speaker_encoder_features(const b200tts_speaker_encoder* h, const flo
     if (!h) { set_error("speaker_encoder_features: null handle"); return 1; }
     if (stage < 0 || stage > 4) { set_error("speaker_encoder_features: stage %d is not in 0..4", stage); return 1; }
     return h->impl.run(x, starts, B, T, 1, 0, nullptr, stage, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200tts_glow_tts_create(const b200tts_glow_tts_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_glow_tts** out) {
+    if (!cfg || !weights || !out) { set_error("glow_tts_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_glow_tts* h = new (std::nothrow) b200tts_glow_tts();
+    if (!h) { set_error("glow_tts_create: out of host memory"); return 1; }
+    int rc = h->impl.init(*cfg, weights, num_weights);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+void b200tts_glow_tts_destroy(b200tts_glow_tts* h) { delete h; }
+size_t b200tts_glow_tts_workspace_bytes(const b200tts_glow_tts* h, int B, int Tt, int Ty) {
+    return h ? std::max(h->impl.encode_bytes(B, Tt), h->impl.decode_bytes(B, Ty)) : 0;
+}
+int b200tts_glow_tts_encode(const b200tts_glow_tts* h, const int64_t* tokens, const int64_t* lengths, const float* g,
+                            float length_scale, int B, int Tt, float* o_stats, float* logw, float* x_mask, float* w_ceil,
+                            float* cum, float* dur_log, int64_t* y_lengths, int64_t* meta, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("glow_tts_encode: null handle"); return 1; }
+    return h->impl.encode((const long long*)tokens, (const long long*)lengths, g, length_scale, B, Tt, o_stats, logw,
+                          x_mask, w_ceil, cum, dur_log, (long long*)y_lengths, (long long*)meta, workspace,
+                          workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, const float* x_mask, const float* cum,
+                            const int64_t* y_lengths, const float* g, const float* noise, float noise_scale, int B, int Tt,
+                            int Ty, float* attn, float* y_mean, float* y_log_scale, float* mel, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("glow_tts_decode: null handle"); return 1; }
+    return h->impl.decode(o_stats, x_mask, cum, (const long long*)y_lengths, g, noise, noise_scale, B, Tt, Ty, attn,
+                          y_mean, y_log_scale, mel, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

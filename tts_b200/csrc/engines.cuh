@@ -92,6 +92,12 @@ struct DurPred {
 int launch_upsample_linear(const float* x, int rows, int Tin, float scale_factor, float* y, int Tout, cudaStream_t st);
 int launch_add_layernorm(const float* x, const float* y, const float* gamma, const float* beta, const float* mask,
                          float* out, int B, int C, int T, float eps, cudaStream_t st);
+// text_encoder.cu's embedding (x = emb[tok] * sqrt(hidden) * mask, plus the x_mask) and multi-head attention over a fused
+// [B, 3C, T] q|k|v tensor; window < 0: no relative-position terms (rel_k / rel_v unused)
+int launch_embed(const long long* tokens, const long long* lengths, const float* emb, const float* lang_emb, int B,
+                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st);
+int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
+                     int C, int T, int num_heads, int window, cudaStream_t st);
 
 struct TextEncoder {
     struct Layer {
@@ -171,9 +177,46 @@ struct SpeakerEncoder {
             void* ws, size_t ws_bytes, cudaStream_t st) const;
 };
 
+// Glow-TTS inference (glow_tts.cu): encoder (optional prenet, transformer without relative terms, LayerNorm type "1"),
+// duration predictor on cat(x, g), then -- after the caller's one host read of max(y_lengths) -- the expanded prior and
+// the Glow decoder in reverse.  The decoder works on the squeezed latent [B, C*num_squeeze, Tq] (Tq = frames /
+// num_squeeze, padded to a multiple of 4 for the tensor-core convs, masked zero beyond); each block is start 1x1 ->
+// WaveNet -> end 1x1, then one elementwise pass for the inverse affine coupling, InvConvNear^-1 and ActNorm^-1.
+struct GlowTTS {
+    struct Prenet { ConvLayer conv; float *g = nullptr, *b = nullptr; };
+    struct Block {
+        ConvLayer start, end;
+        WaveNet wn;
+        float *mix = nullptr, *an_bias = nullptr, *an_logs = nullptr;   // inverse InvConvNear weight [ns][ns], ActNorm
+    };
+    b200tts_glow_tts_config c;
+    int Cs = 0;                        // squeezed channels out_channels * num_squeeze
+    float* emb = nullptr;
+    std::vector<Prenet> prenet;
+    ConvLayer prenet_proj, proj;       // proj: [proj_m | proj_s] rows (proj_s all zero when mean_only)
+    std::vector<TextEncoder::Layer*> layers;
+    DurPred dp;
+    std::vector<Block*> blocks;
+    ~GlowTTS();
+    int init(const b200tts_glow_tts_config& cfg, const float* const* w, int nw);
+    int tq(int Ty) const { return (Ty / c.num_squeeze + 3) / 4 * 4; }
+    size_t encode_bytes(int B, int Tt) const;
+    size_t decode_bytes(int B, int Ty) const;
+    int encode(const long long* tokens, const long long* lengths, const float* g, float length_scale, int B, int Tt,
+               float* o_stats, float* logw, float* x_mask, float* w_ceil, float* cum, float* dur_log,
+               long long* y_lengths, long long* meta, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    int decode(const float* o_stats, const float* x_mask, const float* cum, const long long* y_lengths, const float* g,
+               const float* noise, float noise_scale, int B, int Tt, int Ty, float* attn, float* y_mean,
+               float* y_log_scale, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
+};
+
 // durations -> path -> expanded prior (path.cu)
 int launch_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st);
+// Glow-TTS rule: w_ceil = max(1, ceil((exp(logw) - 1) * x_mask * length_scale)); dur_log = log(1 + w_ceil * x_mask) * x_mask
+int launch_durations_glow(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
+                          float* cum, long long* y_lengths, float* dur_log, long long* meta, cudaStream_t st);
+// z_p may be NULL (then noise may be too): attn / m_p / logs_p / y_mask only
 int launch_expand_prior(const float* cum, const float* x_mask, const long long* y_lengths, const float* stats,
                         const float* noise, float noise_scale, int B, int Tx, int Ty, int C, float* attn, float* m_p,
                         float* logs_p, float* z_p, float* y_mask, cudaStream_t st);

@@ -13,8 +13,13 @@ namespace {
 // one warp per utterance (one CTA, warps stride over the batch): inclusive scan of integral-valued fp32 durations
 // (exact below 2^24).  The same CTA reduces max(y_lengths) and forwards the duration predictor's error flag into
 // `meta` = {max y_length, flag}, so the caller's one host read fetches both (no second synchronisation).
+// GLOW: the Glow-TTS rule (glow_tts.py:350-352), w = (exp(logw) - 1) * x_mask * length_scale and w_ceil =
+// clamp_min(ceil(w), 1) -- the clamp gives every padded token one frame too -- plus dur_log = log(1 + sum(attn, -1)) *
+// x_mask of compute_outputs (:147): a valid token's path row holds w_ceil ones, a padded token's none.
+template <bool GLOW>
 __global__ void durations_kernel(const float* logw, const float* x_mask, float length_scale, float* w_ceil,
-                                 float* cum, long long* y_lengths, int B, int T, const int* err_flag, long long* meta) {
+                                 float* cum, long long* y_lengths, int B, int T, const int* err_flag, long long* meta,
+                                 float* dur_log) {
     __shared__ long long wmax[32];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     long long mymax = 0;
@@ -24,8 +29,15 @@ __global__ void durations_kernel(const float* logw, const float* x_mask, float l
             const int t = t0 + lane;
             float wc = 0.f;
             if (t < T) {
-                const float w = __fmul_rn(__fmul_rn(expf(logw[(size_t)b * T + t]), x_mask[(size_t)b * T + t]), length_scale);
-                wc = ceilf(w);
+                const float m = x_mask[(size_t)b * T + t];
+                if (GLOW) {
+                    const float w = __fmul_rn(__fmul_rn(__fsub_rn(expf(logw[(size_t)b * T + t]), 1.f), m), length_scale);
+                    wc = fmaxf(ceilf(w), 1.f);
+                    dur_log[(size_t)b * T + t] = __fmul_rn(logf(__fadd_rn(1.f, __fmul_rn(wc, m))), m);
+                } else {
+                    const float w = __fmul_rn(__fmul_rn(expf(logw[(size_t)b * T + t]), m), length_scale);
+                    wc = ceilf(w);
+                }
                 w_ceil[(size_t)b * T + t] = wc;
             }
             float s = wc;
@@ -84,7 +96,7 @@ __global__ void expand_prior_kernel(const float* cum, const float* x_mask, const
         m_p[ob + (size_t)c * Ty] = m;
         logs_p[ob + (size_t)c * Ty] = s;
         // m_p + noise * exp(logs_p) * scale, evaluated left to right like the reference
-        z_p[ob + (size_t)c * Ty] = __fadd_rn(m, __fmul_rn(__fmul_rn(noise[ob + (size_t)c * Ty], expf(s)), noise_scale));
+        if (z_p) z_p[ob + (size_t)c * Ty] = __fadd_rn(m, __fmul_rn(__fmul_rn(noise[ob + (size_t)c * Ty], expf(s)), noise_scale));
     }
 }
 
@@ -94,8 +106,19 @@ int launch_durations(const float* logw, const float* x_mask, float length_scale,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st) {
     B200_REQUIRE(logw && x_mask && w_ceil && cum && y_lengths, "durations: null pointer");
     if (B == 0) return 0;
-    durations_kernel<<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths, B, T,
-                                                          err_flag, meta);
+    durations_kernel<false><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
+                                                                 B, T, err_flag, meta, nullptr);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_durations_glow(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
+                          float* cum, long long* y_lengths, float* dur_log, long long* meta, cudaStream_t st) {
+    B200_REQUIRE(logw && x_mask && w_ceil && cum && y_lengths && dur_log, "durations_glow: null pointer");
+    if (B == 0) return 0;
+    durations_kernel<true><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
+                                                                B, T, nullptr, meta, dur_log);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     return 0;
@@ -104,7 +127,7 @@ int launch_durations(const float* logw, const float* x_mask, float length_scale,
 int launch_expand_prior(const float* cum, const float* x_mask, const long long* y_lengths, const float* stats,
                         const float* noise, float noise_scale, int B, int Tx, int Ty, int C, float* attn, float* m_p,
                         float* logs_p, float* z_p, float* y_mask, cudaStream_t st) {
-    B200_REQUIRE(cum && x_mask && y_lengths && stats && noise && m_p && logs_p && z_p, "expand_prior: null pointer");
+    B200_REQUIRE(cum && x_mask && y_lengths && stats && m_p && logs_p && (noise || !z_p), "expand_prior: null pointer");
     if (B == 0 || Ty == 0) return 0;
     dim3 grid((Ty + 127) / 128, B);
     expand_prior_kernel<<<grid, 128, 0, st>>>(cum, x_mask, y_lengths, stats, noise, noise_scale, attn, m_p, logs_p,

@@ -224,6 +224,39 @@ int launch_add_layernorm(const float* x, const float* y, const float* gamma, con
     return 0;
 }
 
+int launch_embed(const long long* tokens, const long long* lengths, const float* emb, const float* lang_emb, int B,
+                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st) {
+    dim3 grid((T + 127) / 128, C, B);
+    embed_kernel<<<grid, 128, 0, st>>>(tokens, lengths, emb, lang_emb, x, x_mask, T, hidden, C, sqrtf((float)hidden));
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
+                     int C, int T, int num_heads, int window, cudaStream_t st) {
+    const int d = C / num_heads;
+    B200_REQUIRE(C % num_heads == 0 && d <= ATT_MAXD, "attention: head dim %d (C=%d, %d heads) not supported", d, C,
+                 num_heads);
+    B200_REQUIRE(window < 0 || (rel_k && rel_v && 2 * window + 1 <= 32), "attention: bad relative window");
+    const int Tp = (T + 31) & ~31;
+    const int nrel = window < 0 ? 0 : 2 * window + 1;
+    const size_t att_smem = sizeof(float) * ((size_t)ATT_Q * d + (size_t)ATT_Q * Tp + (size_t)(ATT_KT + 1) * (d + 1) +
+                                             (size_t)2 * nrel * d);
+    B200_REQUIRE(att_smem <= 200 * 1024, "attention: T=%d too long for the attention kernel", T);
+    static DeviceOnce attr_once;
+    if (int rc0 = device_once(attr_once, nullptr, [](int) -> int {
+            B200_CUDA_OK(cudaFuncSetAttribute(rel_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+            return 0;
+        })) return rc0;
+    dim3 grid((T + ATT_Q - 1) / ATT_Q, num_heads, B);
+    rel_attention_kernel<<<grid, 32 * ATT_Q, att_smem, st>>>(qkv, x_mask, rel_k, rel_v, out, C, T, d, window,
+                                                            1.f / sqrtf((float)d));
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 TextEncoder::~TextEncoder() {
     if (emb) cudaFree(emb);
     for (auto* l : layers) {
@@ -295,24 +328,8 @@ int TextEncoder::forward(const long long* tokens, const long long* lengths, cons
     float* hb = ar.f32((size_t)B * c.hidden_channels_ffn * T);
     B200_REQUIRE(qkv && att && yb && hb, "text_encoder_forward: arena exhausted");
     const long long bs = (long long)C * T;
-    {
-        dim3 grid((T + 127) / 128, C, B);
-        embed_kernel<<<grid, 128, 0, st>>>(tokens, lengths, emb, lang_emb, x, x_mask, T, c.hidden_channels, C,
-                                           sqrtf((float)c.hidden_channels));
-        count_launch();
-        B200_CUDA_OK(cudaGetLastError());
-    }
-    const int Tp = (T + 31) & ~31;
-    const int nrel = 2 * c.rel_attn_window_size + 1;
-    const size_t att_smem = sizeof(float) * ((size_t)ATT_Q * d + (size_t)ATT_Q * Tp + (size_t)(ATT_KT + 1) * (d + 1) +
-                                             (size_t)2 * nrel * d);
-    B200_REQUIRE(att_smem <= 200 * 1024, "text_encoder_forward: T=%d too long for the attention kernel", T);
-    static DeviceOnce attr_once;
-    if (int rc0 = device_once(attr_once, nullptr, [](int) -> int {
-            B200_CUDA_OK(cudaFuncSetAttribute(rel_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            return 0;
-        })) return rc0;
     int rc;
+    if ((rc = launch_embed(tokens, lengths, emb, lang_emb, B, T, c.hidden_channels, C, x, x_mask, st))) return rc;
     for (int l = 0; l < c.num_layers; ++l) {
         const Layer& L = *layers[l];
         {   // q,k,v = conv_{q,k,v}(x)       (x is already masked: embed / previous norm2 epilogue)
@@ -321,13 +338,8 @@ int TextEncoder::forward(const long long* tokens, const long long* lengths, cons
             io.y = qkv; io.y_bs = 3 * bs; io.y_cs = T; io.Tout = T; io.B = B;
             if ((rc = launch_conv(L.qkv, io, st))) return rc;
         }
-        {
-            dim3 grid((T + ATT_Q - 1) / ATT_Q, c.num_heads, B);
-            rel_attention_kernel<<<grid, 32 * ATT_Q, att_smem, st>>>(qkv, x_mask, L.rel_k, L.rel_v, att, C, T, d,
-                                                                    c.rel_attn_window_size, 1.f / sqrtf((float)d));
-            count_launch();
-            B200_CUDA_OK(cudaGetLastError());
-        }
+        if ((rc = launch_attention(qkv, x_mask, L.rel_k, L.rel_v, att, B, C, T, c.num_heads, c.rel_attn_window_size,
+                                   st))) return rc;
         {   // y = conv_o(att)
             ConvIO io;
             io.x = att; io.x_bs = bs; io.x_cs = T; io.Tin = T;
