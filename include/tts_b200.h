@@ -75,6 +75,19 @@ void b200tts_conv1d_destroy(b200tts_conv1d* h);
 int b200tts_conv1d_out_len(const b200tts_conv1d* h, int T);
 int b200tts_conv1d_forward(const b200tts_conv1d* h, const float* x, int B, int T, float in_slope, const float* residual,
                            float scale, int accumulate, float post_div, float* y, void* stream);
+/* Padding modes of b200tts_conv1d_create_padded (nn.Conv1d's padding_mode).  REFLECT reads input column t < 0 as x[-t]
+ * and t >= T as x[2T - 2 - t] (nn.ReflectionPad1d(padding) followed by an unpadded conv); it needs padding <= T - 1 and
+ * is not available for transposed convs. */
+enum { B200TTS_PAD_ZEROS = 0, B200TTS_PAD_REFLECT = 1 };
+/* b200tts_conv1d_create / _create_ex with a padding mode (allow_tensor_cores = 0: the FP32-FMA kernel only) */
+int b200tts_conv1d_create_padded(const b200tts_conv1d_config* cfg, const float* weight, const float* bias,
+                                 int allow_tensor_cores, int precision, int padding_mode, b200tts_conv1d** out);
+/* b200tts_conv1d_forward on an input with arbitrary batch / channel strides (floats; time contiguous), with an optional
+ * tanh epilogue (tanh = 1: y = tanh(conv(leaky_relu(x)) + bias), no residual / accumulate) and an optional peak word
+ * (tanh only) that max|y| is folded into, as in b200tts_hifigan_forward_ex. */
+int b200tts_conv1d_forward_strided(const b200tts_conv1d* h, const float* x, long long x_batch_stride, int x_channel_stride,
+                                   int B, int T, float in_slope, const float* residual, float scale, int accumulate,
+                                   float post_div, int tanh, float* y, uint32_t* peak_bits, void* stream);
 
 /* ---- monotonic alignment search ------------------------------------------------------------
  * Replaces maximum_path_c / maximum_path_each, TTS/tts/utils/monotonic_align/core.pyx:11-47
@@ -486,6 +499,52 @@ int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, con
                             const int64_t* y_lengths, const float* g, const float* noise, float noise_scale, int B, int Tt,
                             int Ty, float* attn, float* y_mean, float* y_log_scale, float* mel, void* workspace,
                             size_t workspace_bytes, void* stream);
+
+/* ---- MelGAN generators (plain, full-band, multi-band with PQMF synthesis) ---------------------------
+ * Replaces MelganGenerator.forward (TTS/vocoder/models/melgan_generator.py:9-74, ResidualStack
+ * TTS/vocoder/layers/melgan.py:6-36) and, for the multi-band generator, PQMF.synthesis (TTS/vocoder/layers/pqmf.py:50-53;
+ * MultibandMelganGenerator.inference, multiband_melgan_generator.py:36-43).  Every conv with kernel > 1 reflect-pads
+ * (nn.ReflectionPad1d); the leaky-ReLU slope is 0.2 everywhere, also before conv_post.  Upsampler s is
+ * ConvTranspose1d(kernel 2u, stride u, padding u/2 + u%2, output_padding u%2), so every stage multiplies the length by u.
+ * weights (host pointers, PyTorch layouts, weight norm folded), in this order:
+ *   conv_pre.w [base, in, proj_kernel], conv_pre.b                                      (melgan_generator.py:32-35)
+ *   for each upsample stage s (Cs = base / 2^(s+1)):
+ *     ups[s].w [2 Cs, Cs, 2u] (ConvTranspose1d layout), ups[s].b                          (:43-57)
+ *     for each residual block m: blocks[m][2].w [Cs, Cs, res_kernel] (dilation res_kernel^m), blocks[m][2].b,
+ *                                blocks[m][4].w [Cs, Cs, 1], blocks[m][4].b, shortcuts[m].w [Cs, Cs, 1], shortcuts[m].b
+ *                                                                                         (melgan.py:17-31)
+ *   conv_post.w [out, Clast, proj_kernel], conv_post.b                                   (melgan_generator.py:66-70)
+ *   G [1, pqmf_bands, pqmf_taps + 1]: the PQMF synthesis filter (pqmf.py:31), only if pqmf_bands > 0
+ */
+typedef struct {
+    int in_channels, out_channels, base_channels, proj_kernel, res_kernel, num_res_blocks;
+    int num_upsamples;
+    int upsample_factors[8];
+    int pqmf_bands; /* 0: no PQMF (plain / full-band); else out_channels must equal it */
+    int pqmf_taps;  /* filter taps (62 in the reference; G has taps + 1) */
+} b200tts_melgan_config;
+typedef struct b200tts_melgan b200tts_melgan;
+int b200tts_melgan_create(const b200tts_melgan_config* cfg, const float* const* weights, int num_weights,
+                          b200tts_melgan** out);
+void b200tts_melgan_destroy(b200tts_melgan* h);
+size_t b200tts_melgan_workspace_bytes(const b200tts_melgan* h, int B, int T);
+/* samples per row of the generator output (conv_post): T * prod(upsample_factors); the synthesised waveform of a
+ * multi-band generator has pqmf_bands times as many */
+int b200tts_melgan_out_len(const b200tts_melgan* h, int T);
+/* x [B, in, T] -> out.  synthesize = 0: the generator output [B, out_channels, out_len(T)] (the band signals of a
+ * multi-band generator: its forward()); synthesize = 1 (multi-band only): the PQMF-synthesised waveform
+ * [B, 1, pqmf_bands * out_len(T) - pqmf_taps % 2].  peak_bits (nullable, zeroed by the caller) folds max|out| in, for
+ * b200tts_to_int16.  Every reflect pad needs padding <= length - 1 at its layer (at least 28 columns at stage 0 with
+ * 4 residual blocks); a shorter input returns status 1 before anything is launched. */
+int b200tts_melgan_forward(const b200tts_melgan* h, const float* x, int B, int T, int synthesize, float* out,
+                           uint32_t* peak_bits, void* workspace, size_t workspace_bytes, void* stream);
+
+/* PQMF synthesis alone (TTS/vocoder/layers/pqmf.py:50-53): x [B, N, Tb] -> y [B, 1, N * Tb - taps % 2] (an odd tap
+ * count loses one sample, as conv1d with padding taps / 2 does),
+ *   y[n] = sum_k sum_j N G[0,k,j] x[k, (n + j - taps/2) / N]   (only integer indices inside [0, Tb): zero padding).
+ * G: device [1, N, taps + 1].  peak_bits as above (nullable). */
+int b200tts_pqmf_synthesis(const float* x, int B, int N, int Tb, const float* G, int taps, float* y, uint32_t* peak_bits,
+                           void* stream);
 
 #ifdef __cplusplus
 }

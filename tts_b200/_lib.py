@@ -77,6 +77,16 @@ class GlowTTSConfigC(ctypes.Structure):
                                             "num_splits", "num_squeeze", "sigmoid_scale")]
 
 
+class MelganConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("in_channels", "out_channels", "base_channels", "proj_kernel", "res_kernel",
+                                            "num_res_blocks", "num_upsamples")] + \
+               [("upsample_factors", ctypes.c_int * 8), ("pqmf_bands", ctypes.c_int), ("pqmf_taps", ctypes.c_int)]
+
+
+# padding modes of b200tts_conv1d_create_padded (B200TTS_PAD_* in include/tts_b200.h)
+PADDING_MODES = {"zeros": 0, "reflect": 1}
+
+
 class AudioNormC(ctypes.Structure):
     _fields_ = [("signal_norm", ctypes.c_int), ("symmetric_norm", ctypes.c_int), ("clip_norm", ctypes.c_int),
                 ("max_norm", ctypes.c_float), ("min_level_db", ctypes.c_float), ("ref_level_db", ctypes.c_float),
@@ -109,6 +119,23 @@ def _declare(lib):
     lib.b200tts_conv1d_create.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ctypes.POINTER(vp)]
     lib.b200tts_conv1d_create_ex.restype = ci
     lib.b200tts_conv1d_create_ex.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ctypes.POINTER(vp)]
+    lib.b200tts_conv1d_create_padded.restype = ci
+    lib.b200tts_conv1d_create_padded.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ci, ci, ctypes.POINTER(vp)]
+    lib.b200tts_conv1d_forward_strided.restype = ci
+    lib.b200tts_conv1d_forward_strided.argtypes = [vp, vp, ctypes.c_longlong, ci, ci, ci, ctypes.c_float, vp,
+                                                   ctypes.c_float, ci, ctypes.c_float, ci, vp, vp, vp]
+    lib.b200tts_melgan_create.restype = ci
+    lib.b200tts_melgan_create.argtypes = [ctypes.POINTER(MelganConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+    lib.b200tts_melgan_destroy.restype = None
+    lib.b200tts_melgan_destroy.argtypes = [vp]
+    lib.b200tts_melgan_workspace_bytes.restype = sz
+    lib.b200tts_melgan_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_melgan_out_len.restype = ci
+    lib.b200tts_melgan_out_len.argtypes = [vp, ci]
+    lib.b200tts_melgan_forward.restype = ci
+    lib.b200tts_melgan_forward.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, sz, vp]
+    lib.b200tts_pqmf_synthesis.restype = ci
+    lib.b200tts_pqmf_synthesis.argtypes = [vp, ci, ci, ci, vp, ci, vp, vp, vp]
     lib.b200tts_conv1d_destroy.restype = None
     lib.b200tts_conv1d_destroy.argtypes = [vp]
     lib.b200tts_conv1d_out_len.restype = ci

@@ -17,15 +17,21 @@ class FusedConv1d:
     """weight [Cout,Cin,K] (or [Cin,Cout,K] with ``transposed=True``), bias [Cout] or None -- host or device tensors;
     the packed device copy is created on first use per device.  ``precision`` "bf16" / "fp16" runs the tensor-core
     kernels with 16-bit operands (fp32 accumulation; layers with Cin % 16 != 0 stay 3xTF32); "fp32" is the
-    ``tensor_cores`` setting as given."""
+    ``tensor_cores`` setting as given.  ``padding_mode`` mirrors ``nn.Conv1d``'s: "zeros" (default) or "reflect"
+    (``nn.ReflectionPad1d(padding)`` then an unpadded conv, read straight from x by the kernels: no padded copy; needs
+    ``padding = dilation * (K - 1) / 2``, ``padding <= T - 1`` and a non-transposed conv)."""
 
     def __init__(self, weight, bias=None, dilation=1, padding=0, transposed=False, stride=1, tensor_cores=True,
-                 precision="fp32"):
+                 precision="fp32", padding_mode="zeros"):
         self.weight = weight.detach().to(torch.float32).cpu().contiguous()
         self.bias = None if bias is None else bias.detach().to(torch.float32).cpu().contiguous()
         self.dilation, self.padding, self.transposed, self.stride = int(dilation), int(padding), bool(transposed), int(stride)
         self.tensor_cores = bool(tensor_cores)
         self.precision = precision
+        if padding_mode not in _lib.PADDING_MODES:
+            raise ValueError(f"tts_b200.FusedConv1d: padding_mode must be one of {sorted(_lib.PADDING_MODES)}, "
+                             f"got {padding_mode!r}")
+        self.padding_mode = padding_mode
         if _lib.precision_id(precision) != 0 and not self.tensor_cores:
             raise ValueError("tts_b200.FusedConv1d: a 16-bit precision needs tensor_cores=True")
         if transposed:
@@ -47,7 +53,11 @@ class FusedConv1d:
             cfg = _lib.Conv1dConfigC(self.cin, self.cout, self.k, self.dilation, self.padding, int(self.transposed), self.stride)
             out = ctypes.c_void_p()
             with torch.cuda.device(device):
-                if self.precision == "fp32":
+                if self.padding_mode != "zeros":
+                    rc = _lib.lib().b200tts_conv1d_create_padded(
+                        ctypes.byref(cfg), _lib.ptr(self.weight), _lib.ptr(self.bias), int(self.tensor_cores),
+                        _lib.precision_id(self.precision), _lib.PADDING_MODES[self.padding_mode], ctypes.byref(out))
+                elif self.precision == "fp32":
                     rc = _lib.lib().b200tts_conv1d_create(ctypes.byref(cfg), _lib.ptr(self.weight), _lib.ptr(self.bias),
                                                           int(self.tensor_cores), ctypes.byref(out))
                 else:
@@ -58,9 +68,20 @@ class FusedConv1d:
         return h
 
     @torch.no_grad()
-    def __call__(self, x, in_slope=1.0, residual=None, scale=1.0, accumulate_into=None, post_div=1.0):
+    def __call__(self, x, in_slope=1.0, residual=None, scale=1.0, accumulate_into=None, post_div=1.0, tanh=False,
+                 peak=None):
+        """``tanh=True``: y = tanh(conv(leaky_relu(x)) + bias) (no residual / accumulate), and ``peak`` (optional zeroed
+        int32[1] device word) folds max|y| in.  With reflection padding, ``tanh`` or ``peak``, a float32 x whose time
+        axis is contiguous is read in place through its batch / channel strides."""
         _lib.require_cuda(x, "x")
-        x = x.to(torch.float32).contiguous()
+        strided = self.padding_mode != "zeros" or tanh or peak is not None
+        if tanh and (residual is not None or accumulate_into is not None):
+            raise ValueError("tts_b200.FusedConv1d: the tanh epilogue takes no residual / accumulate")
+        if peak is not None and not tanh:
+            raise ValueError("tts_b200.FusedConv1d: peak needs tanh=True")
+        x = x.to(torch.float32)
+        if not strided or x.dim() != 3 or x.stride(-1) != 1:
+            x = x.contiguous()
         b, cin, t = x.shape
         if cin != self.cin:
             raise ValueError(f"tts_b200.FusedConv1d: expected {self.cin} input channels, got {cin}")
@@ -78,8 +99,15 @@ class FusedConv1d:
             if tuple(residual.shape) != (b, self.cout, tout):
                 raise ValueError("tts_b200.FusedConv1d: residual has the wrong shape")
         with torch.cuda.device(x.device):
-            rc = L.b200tts_conv1d_forward(h, _lib.ptr(x), b, t, ctypes.c_float(in_slope), _lib.ptr(residual),
-                                          ctypes.c_float(scale), 0 if accumulate_into is None else 1,
-                                          ctypes.c_float(post_div), _lib.ptr(y), _lib.stream_ptr(x.device))
+            if strided:
+                rc = L.b200tts_conv1d_forward_strided(h, _lib.ptr(x), ctypes.c_longlong(x.stride(0)), x.stride(1), b, t,
+                                                      ctypes.c_float(in_slope), _lib.ptr(residual), ctypes.c_float(scale),
+                                                      0 if accumulate_into is None else 1, ctypes.c_float(post_div),
+                                                      int(bool(tanh)), _lib.ptr(y), _lib.ptr(peak),
+                                                      _lib.stream_ptr(x.device))
+            else:
+                rc = L.b200tts_conv1d_forward(h, _lib.ptr(x), b, t, ctypes.c_float(in_slope), _lib.ptr(residual),
+                                              ctypes.c_float(scale), 0 if accumulate_into is None else 1,
+                                              ctypes.c_float(post_div), _lib.ptr(y), _lib.stream_ptr(x.device))
         _lib.check(rc, "conv1d_forward")
         return y

@@ -14,6 +14,7 @@ struct b200tts_posterior { PosteriorEnc impl; };
 struct b200tts_duration_predictor { DurPred impl; };
 struct b200tts_speaker_encoder { SpeakerEncoder impl; };
 struct b200tts_glow_tts { GlowTTS impl; };
+struct b200tts_melgan { Melgan impl; };
 
 extern "C" {
 
@@ -24,20 +25,32 @@ int b200tts_debug_tc_error(void) { return conv_tc_error_flag(); }
 void b200tts_debug_dispatch_begin(void) { dispatch_begin(); }
 int b200tts_debug_dispatch_end(int32_t* ids, int cap) { return dispatch_end(ids, cap); }
 
-struct b200tts_conv1d { ConvLayer L; b200tts_conv1d_config c; ~b200tts_conv1d() { free_conv(L); } };
+struct b200tts_conv1d {
+    ConvLayer L; b200tts_conv1d_config c; int reflect = 0;   // reflect: B200TTS_PAD_REFLECT
+    ~b200tts_conv1d() { free_conv(L); }
+};
 
 static bool valid_precision(int p) {
     return p == B200TTS_PRECISION_FP32 || p == B200TTS_PRECISION_BF16 || p == B200TTS_PRECISION_FP16;
 }
 
 static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* weight, const float* bias, int allow_tensor_cores,
-                              int precision, b200tts_conv1d** out) {
+                              int precision, b200tts_conv1d** out, int padding_mode = B200TTS_PAD_ZEROS) {
     if (!cfg || !weight || !out) { set_error("conv1d_create: null argument"); return 1; }
     *out = nullptr;
     if (!valid_precision(precision)) { set_error("conv1d_create: unknown precision %d", precision); return 1; }
+    if (padding_mode != B200TTS_PAD_ZEROS && padding_mode != B200TTS_PAD_REFLECT) {
+        set_error("conv1d_create: unknown padding mode %d", padding_mode);
+        return 1;
+    }
+    if (padding_mode == B200TTS_PAD_REFLECT && (cfg->transposed || 2 * cfg->padding != cfg->dilation * (cfg->kernel_size - 1))) {
+        set_error("conv1d_create: reflection padding needs a non-transposed conv with padding = dilation * (kernel_size - 1) / 2");
+        return 1;
+    }
     b200tts_conv1d* h = new (std::nothrow) b200tts_conv1d();
     if (!h) { set_error("conv1d_create: out of host memory"); return 1; }
     h->c = *cfg;
+    h->reflect = padding_mode == B200TTS_PAD_REFLECT;
     h->L.tc_prec = allow_tensor_cores ? precision : TC_NONE;
     int rc = cfg->transposed
                  ? pack_conv_transpose(h->L, weight, bias, cfg->in_channels, cfg->out_channels, cfg->kernel_size,
@@ -56,6 +69,10 @@ int b200tts_conv1d_create_ex(const b200tts_conv1d_config* cfg, const float* weig
                              b200tts_conv1d** out) {
     return conv1d_create_impl(cfg, weight, bias, 1, precision, out);
 }
+int b200tts_conv1d_create_padded(const b200tts_conv1d_config* cfg, const float* weight, const float* bias,
+                                 int allow_tensor_cores, int precision, int padding_mode, b200tts_conv1d** out) {
+    return conv1d_create_impl(cfg, weight, bias, allow_tensor_cores, precision, out, padding_mode);
+}
 void b200tts_conv1d_destroy(b200tts_conv1d* h) { delete h; }
 int b200tts_conv1d_out_len(const b200tts_conv1d* h, int T) {
     if (!h) return 0;
@@ -72,6 +89,23 @@ int b200tts_conv1d_forward(const b200tts_conv1d* h, const float* x, int B, int T
     if (residual) { io.res = residual; io.res_bs = io.y_bs; io.res_cs = Tout; }
     io.scale = scale; io.post_div = post_div;
     if (accumulate) io.flags |= EPI_ACCUM;
+    io.reflect = h->reflect;
+    return launch_conv(h->L, io, (cudaStream_t)stream);
+}
+int b200tts_conv1d_forward_strided(const b200tts_conv1d* h, const float* x, long long x_batch_stride, int x_channel_stride,
+                                   int B, int T, float in_slope, const float* residual, float scale, int accumulate,
+                                   float post_div, int tanh, float* y, uint32_t* peak_bits, void* stream) {
+    if (!h) { set_error("conv1d_forward_strided: null handle"); return 1; }
+    if (peak_bits && !tanh) { set_error("conv1d_forward_strided: peak_bits needs the tanh epilogue"); return 1; }
+    const int Tout = b200tts_conv1d_out_len(h, T);
+    ConvIO io;
+    io.x = x; io.x_bs = x_batch_stride; io.x_cs = x_channel_stride; io.Tin = T; io.in_slope = in_slope;
+    io.y = y; io.y_bs = (long long)h->c.out_channels * Tout; io.y_cs = Tout; io.Tout = Tout; io.B = B;
+    if (residual) { io.res = residual; io.res_bs = io.y_bs; io.res_cs = Tout; }
+    io.scale = scale; io.post_div = post_div;
+    if (accumulate) io.flags |= EPI_ACCUM;
+    if (tanh) { io.act = ACT_TANH; io.peak_bits = peak_bits; }
+    io.reflect = h->reflect;
     return launch_conv(h->L, io, (cudaStream_t)stream);
 }
 
@@ -358,6 +392,19 @@ int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, con
     if (!h) { set_error("glow_tts_decode: null handle"); return 1; }
     return h->impl.decode(o_stats, x_mask, cum, (const long long*)y_lengths, g, noise, noise_scale, B, Tt, Ty, attn,
                           y_mean, y_log_scale, mel, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+B200_HANDLE_API(melgan, b200tts_melgan, b200tts_melgan_config)
+
+int b200tts_melgan_out_len(const b200tts_melgan* h, int T) { return h ? h->impl.out_len(T) : 0; }
+int b200tts_melgan_forward(const b200tts_melgan* h, const float* x, int B, int T, int synthesize, float* out,
+                           uint32_t* peak_bits, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("melgan_forward: null handle"); return 1; }
+    return h->impl.forward(x, B, T, synthesize, out, peak_bits, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_pqmf_synthesis(const float* x, int B, int N, int Tb, const float* G, int taps, float* y, uint32_t* peak_bits,
+                           void* stream) {
+    return launch_pqmf_synthesis(x, (long long)N * Tb, Tb, B, N, Tb, G, taps, y, peak_bits, (cudaStream_t)stream);
 }
 
 }  // extern "C"

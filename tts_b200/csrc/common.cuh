@@ -94,7 +94,7 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     int K = 1, dil = 1, pad = 0;
     int ups = 1;              // >1: polyphase ConvTranspose1d
     int co_tile = 64;         // 32 or 64
-    int tr_kernel = 0, tr_pad = 0;  // original transposed-conv kernel size / padding (for Tout)
+    int tr_kernel = 0, tr_pad = 0, tr_outpad = 0;  // original transposed-conv kernel size / padding / output_padding (Tout)
     // tensor cores: set BEFORE packing to TC_NONE or the requested operand type (B200TTS_PRECISION_*); packing records the
     // type of the images it built (a 16-bit request with Cin % 16 != 0 gets 3xTF32; no image: TC_NONE).  The text and
     // duration path requests none, so durations stay bit-stable on the exact FP32 FMA kernel.
@@ -131,6 +131,10 @@ struct ConvIO {
     // grouped tensor-core mode's zero-padded taps).  Tiles stay on the full tensor's column grid, so every column inside
     // the window is computed exactly as by the unwindowed launch.  The defaults are the whole tensor.
     int q_lo = 0, q_hi = 0x7fffffff, in_lo = 0, in_hi = 0x7fffffff;
+    // reflection padding (nn.ReflectionPad1d before the conv): an input column t outside [0, Tin) reads x[-t] (t < 0) or
+    // x[2 Tin - 2 - t] (t >= Tin) instead of zero; no column outside [0, Tin) is ever read.  Needs pad <= Tin - 1; not
+    // combined with lens, a column window or a transposed conv.
+    int reflect = 0;
 };
 
 // Host weights in PyTorch layout.  conv: w[Cout][Cin][K];  transposed: w[Cin][Cout][Kt].
@@ -139,7 +143,7 @@ struct ConvIO {
 int pack_conv(ConvLayer& L, const float* w, const float* bias, int Cout, int Cin, int K, int dil, int pad,
               int gate_half = 0, const int* in_perm = nullptr, const int* out_perm = nullptr);
 int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin, int Cout, int Kt, int stride,
-                        int padding);
+                        int padding, int output_padding = 0);
 void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
@@ -150,7 +154,7 @@ void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);
 inline int conv_transpose_out_len(const ConvLayer& L, int Tin) {
-    return (Tin - 1) * L.ups - 2 * L.tr_pad + L.tr_kernel;
+    return (Tin - 1) * L.ups - 2 * L.tr_pad + L.tr_kernel + L.tr_outpad;
 }
 
 // small helpers shared by the engines

@@ -78,6 +78,7 @@ struct ConvKArgs {
     int XS;
     const int* lens; int rate_out, need_out, rate_in, need_in;
     int q_lo, q_hi, in_lo, in_hi;   // column window (ConvIO), q_lo / in_lo >= 0
+    int reflect;                    // reflection padding (ConvIO::reflect)
 };
 
 enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3 };
@@ -120,7 +121,8 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         float* xd = xs0 + buf * CIC * XS;
         const int c0 = chunk * CIC;
         for (int i = tid; i < XS; i += NT) {
-            const int t = tin0 + i;
+            int t = tin0 + i;
+            if (a.reflect) t = t < 0 ? -t : (t >= a.Tin ? 2 * a.Tin - 2 - t : t);   // mirrored; columns past the reach stay out
             const bool tok = (t >= a.in_lo) && (t < a.Tin);   // below in_lo: stale scratch of a windowed producer
             float m = 1.f;
             if (tok && mb) m = __ldg(mb + t);
@@ -516,9 +518,11 @@ int pack_conv(ConvLayer& L, const float* w, const float* bias, int Cout, int Cin
     return pack_rows(L, Wl, bl, Cout, Cin, K);
 }
 
-int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin, int Cout, int Kt, int s, int p) {
-    // y[co, q*s+ph] = sum_ci sum_m x[ci, q-m] * w[ci, co, ph + p + m*s]   (0 <= ph+p+m*s < Kt)
+int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin, int Cout, int Kt, int s, int p, int op) {
+    // y[co, q*s+ph] = sum_ci sum_m x[ci, q-m] * w[ci, co, ph + p + m*s]   (0 <= ph+p+m*s < Kt); output_padding `op` only
+    // lengthens the output (the extra samples follow the same formula, as in torch)
     B200_REQUIRE(w != nullptr && s >= 1 && Kt >= 1, "pack_conv_transpose: bad arguments");
+    B200_REQUIRE(op >= 0 && op < s, "pack_conv_transpose: output_padding %d must be in [0, stride %d)", op, s);
     auto floordiv = [](int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); };
     const int m_lo = -floordiv(s - 1 + p, s);  // ceil(-(s-1+p)/s)
     const int m_hi = floordiv(Kt - 1 - p, s);
@@ -543,6 +547,7 @@ int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin
     L.ups = s;
     L.tr_kernel = Kt;
     L.tr_pad = p;
+    L.tr_outpad = op;
     return pack_rows(L, Wl, bl, rows, Cin, K);
 }
 
@@ -552,8 +557,10 @@ int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin
 // window as aligned float4 (neighbouring threads' overlaps are L1 hits), 4*K FMAs per channel.  HBM-bound by the x read
 // (Cin * 4 B per output sample).  Reference: hifigan_generator.py:262-264.  Eight CTAs per SM (32 registers): a full
 // SM of warps to keep the loads in flight.
-template <int K>
-__global__ void __launch_bounds__(256, 8) conv1d_row1_kernel(const float* __restrict__ x, long long x_bs, int x_cs, int Cin,
+// REFLECT: reflection padding (ConvIO::reflect, K = 7 only), a compile-time switch: the edge threads mirror their own
+// register window, no extra loads; 40 registers (six CTAs per SM), which the two edge fix-ups need to stay unspilled
+template <int K, bool REFLECT>
+__global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const float* __restrict__ x, long long x_bs, int x_cs, int Cin,
                                                           int T, const float* __restrict__ w, int w_stride,
                                                           const float* __restrict__ bias, float slope, int act,
                                                           float* __restrict__ y, long long y_bs,
@@ -561,6 +568,7 @@ __global__ void __launch_bounds__(256, 8) conv1d_row1_kernel(const float* __rest
                                                           int rate, int need_out, int need_in, int q_lo, int q_hi,
                                                           int in_lo, int blk_lo) {
     constexpr int PAD = (K - 1) / 2, NL = (4 + 4 + (K - 1 - PAD) + 3) / 4;   // float4 loads covering [t0 - 4, t0 + 4 + K-1-PAD)
+    static_assert(!REFLECT || K == 7, "the in-window mirror below is laid out for K = 7");
     extern __shared__ float ws[];
     for (int i = threadIdx.x; i < Cin * K; i += blockDim.x) ws[i] = w[(size_t)i * w_stride];
     __syncthreads();
@@ -612,6 +620,13 @@ __global__ void __launch_bounds__(256, 8) conv1d_row1_kernel(const float* __rest
                 float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (t >= in_lo4 && t < Ti) v = __ldg(reinterpret_cast<const float4*>(xr - 4 + 4 * l));   // Ti % 4 == 0: all in or all out
                 win[4 * l] = v.x; win[4 * l + 1] = v.y; win[4 * l + 2] = v.z; win[4 * l + 3] = v.w;
+            }
+            if constexpr (REFLECT) {
+                // the mirrored columns of the two edge threads lie in their own window (T % 4 == 0, K = 7): win[i] holds
+                // column t0 - 4 + i, so at the row end (t0 = T - 4) column T + j reads T - 2 - j = win[14 - i], and at the
+                // start (t0 = 0) column -j reads j = win[8 - i] (end first: for T = 4 the start's source win[8] is past the end)
+                if (t0 + 4 == T) { win[8] = win[6]; win[9] = win[5]; win[10] = win[4]; win[11] = win[3]; }
+                if (t0 == 0) { win[0] = win[8]; win[1] = win[7]; win[2] = win[6]; win[3] = win[5]; }
             }
 #pragma unroll
             for (int i = 0; i < 4 * NL; ++i) win[i] = win[i] > 0.f ? win[i] : win[i] * slope;
@@ -762,8 +777,11 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16}) {
             for (bool lean : {true, false})
                 B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+            B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
             for (int g : {2, 4})
-                B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+                for (bool refl : {false, true})
+                    B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      smem_optin));
         }
         int* flag = nullptr;
         B200_CUDA_OK(cudaHostAlloc((void**)&flag, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
@@ -815,7 +833,9 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
     // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
     const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
-    const tc3::Tc3Kernel k = grouped ? tc3::grouped_kernel(G, L.tc_prec) : tc3::plain_kernel(L.tc_prec, plain_epi);
+    const bool reflect = a.reflect != 0;   // reflection padding: the lean kernels' reflect variants only
+    if (reflect && !grouped && !plain_epi) return -1;
+    const tc3::Tc3Kernel k = grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect) : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
     const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
     const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
     B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));
@@ -849,6 +869,13 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     a.lens = io.lens; a.rate_out = io.rate_out; a.need_out = io.need_out; a.rate_in = io.rate_in; a.need_in = io.need_in;
     a.q_lo = std::max(0, io.q_lo); a.q_hi = io.q_hi; a.in_lo = std::max(0, io.in_lo); a.in_hi = io.in_hi;
     const bool windowed = a.q_lo > 0 || a.q_hi < a.Tq;
+    a.reflect = io.reflect ? 1 : 0;
+    if (a.reflect) {   // torch's ReflectionPad1d limit; nothing needs reflection together with the options below
+        B200_REQUIRE(L.pad <= io.Tin - 1, "launch_conv: reflection padding %d needs at least %d input columns, got %d", L.pad,
+                     L.pad + 1, io.Tin);
+        B200_REQUIRE(!io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && L.ups == 1 && !io.xmask,
+                     "launch_conv: reflection padding takes no lens, column window, input mask or upsampling");
+    }
     if (a.Tq <= 0 || io.B <= 0) return 0;
     B200_REQUIRE(!(a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)) || io.ymask,
                  "launch_conv: masked/split epilogue needs ymask");
@@ -869,11 +896,11 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
             const int blk_lo = a.q_lo / 1024, blk_hi = (std::min(a.q_hi, a.Tout) + 1023) / 1024;   // 1024 samples per CTA
             dim3 grid(std::max(1, blk_hi - blk_lo), io.B);
             if (grid.y <= 65535) {
-                conv1d_row1_kernel<7><<<grid, 256, (size_t)L.Cin * L.K * 4, st>>>(a.x, a.x_bs, a.x_cs, L.Cin, a.Tout, L.w,
-                                                                                 L.co_tile, L.bias, a.in_slope, a.act, a.y,
-                                                                                 a.y_bs, io.peak_bits, a.lens, a.rate_out,
-                                                                                 a.need_out, a.need_in, a.q_lo, a.q_hi,
-                                                                                 a.in_lo, blk_lo);
+                auto kern = a.reflect ? conv1d_row1_kernel<7, true> : conv1d_row1_kernel<7, false>;
+                kern<<<grid, 256, (size_t)L.Cin * L.K * 4, st>>>(a.x, a.x_bs, a.x_cs, L.Cin, a.Tout, L.w, L.co_tile, L.bias,
+                                                                 a.in_slope, a.act, a.y, a.y_bs, io.peak_bits, a.lens,
+                                                                 a.rate_out, a.need_out, a.need_in, a.q_lo, a.q_hi, a.in_lo,
+                                                                 blk_lo);
                 count_launch();
                 dispatch_note(DISPATCH_ROW1);
                 B200_CUDA_OK(cudaGetLastError());

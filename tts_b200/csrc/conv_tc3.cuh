@@ -103,6 +103,9 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
+__device__ __forceinline__ void cp_async4_zfill(uint32_t dst, const void* src, uint32_t src_bytes) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
 __device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 // 16 consecutive accumulator columns of one row of the shared accumulator tile
 __device__ __forceinline__ void acc_ld16(const float* p, float* v) {
@@ -382,9 +385,13 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     }
 }
 
-template <int GRP, bool LEAN = true, int PREC = PREC_FP32>   // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
+template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false>
+                                       // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
                                        // plain-layer kernel (lean epilogue inline, general one out of line) -- false for the
-                                       // WaveNet / masked / transposed layers (general epilogue inline); PREC: operand type
+                                       // WaveNet / masked / transposed layers (general epilogue inline); PREC: operand type;
+                                       // REFL: reflection padding (ConvIO::reflect; dense, unwindowed launches only): input
+                                       // column t < 0 reads x[-t], t >= Tin reads x[2 Tin - 2 - t].  A compile-time switch so
+                                       // that the zero-padding kernels keep their register allocation.
 __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr int KCH = PREC ? KC16 : KC2;       // input channels per chunk
@@ -535,6 +542,20 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                             if (v_ch[e] < 0) continue;
                             const int t = iss_tal + v_t[e];
                             const int cg = iss_c * KCH + h * KC2 + v_ch[e];
+                            if (REFL && (t < 0 || t + 4 > iss_Tin)) {
+                                // edge vector of a reflect-padded conv (vectors inside the row keep the 16-byte copy): four
+                                // mirrored 4-byte copies, each from inside the row or zero-filled where the mirror leaves
+                                // it (past the conv's reach) -- never a read outside [0, Tin)
+                                const float* rowp = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs;
+#pragma unroll
+                                for (int q = 0; q < 4; ++q) {
+                                    int tt = t + q;
+                                    tt = tt < 0 ? -tt : (tt >= iss_Tin ? 2 * iss_Tin - 2 - tt : tt);
+                                    const bool in = cg < Cin && tt >= 0 && tt < iss_Tin;
+                                    cp_async4_zfill(dst0 + v_dst[e] + 4u * q, rowp + (in ? tt : 0), in ? 4u : 0u);
+                                }
+                                continue;
+                            }
                             // t is a multiple of 4, so a vector is either wholly before the data start (zero fill),
                             // wholly inside, or cut by its end (partial source size, rest zero-filled by the hardware)
                             int nb = 0;
@@ -746,24 +767,35 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
 }
 
 // PREC: PREC_FP32 (3xTF32), PREC_BF16 or PREC_FP16
-template <int PREC>
-__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, true, PREC>(a); }
+template <int PREC, bool REFL = false>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, true, PREC, REFL>(a); }
 template <int PREC>   // gate / split / mask / polyphase
 __global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3x_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, false, PREC>(a); }
-template <int GRP, int PREC>
-__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3g_kernel(const __grid_constant__ Tc3Args a) { tc3_body<GRP, true, PREC>(a); }
+template <int GRP, int PREC, bool REFL = false>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3g_kernel(const __grid_constant__ Tc3Args a) { tc3_body<GRP, true, PREC, REFL>(a); }
 
 typedef void (*Tc3Kernel)(const Tc3Args);
-static inline Tc3Kernel plain_kernel(int prec, bool lean) {
+// reflect: the reflection-padding variant (lean epilogue only; the host sends reflect-padded layers that need the general
+// epilogue to the FMA kernel)
+static inline Tc3Kernel plain_kernel(int prec, bool lean, bool reflect = false) {
+    if (reflect) {
+        if (prec == PREC_BF16) return conv1d_tc3_kernel<PREC_BF16, true>;
+        if (prec == PREC_FP16) return conv1d_tc3_kernel<PREC_FP16, true>;
+        return conv1d_tc3_kernel<PREC_FP32, true>;
+    }
     if (prec == PREC_BF16) return lean ? conv1d_tc3_kernel<PREC_BF16> : conv1d_tc3x_kernel<PREC_BF16>;
     if (prec == PREC_FP16) return lean ? conv1d_tc3_kernel<PREC_FP16> : conv1d_tc3x_kernel<PREC_FP16>;
     return lean ? conv1d_tc3_kernel<PREC_FP32> : conv1d_tc3x_kernel<PREC_FP32>;
 }
 // grouped kernel for 2 / 4 tap groups (any dilation with (GRP - 1) * dil <= 15)
-static inline Tc3Kernel grouped_kernel(int grp, int prec = PREC_FP32) {
-    if (prec == PREC_BF16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_BF16> : conv1d_tc3g_kernel<4, PREC_BF16>;
-    if (prec == PREC_FP16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP16> : conv1d_tc3g_kernel<4, PREC_FP16>;
-    return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP32> : conv1d_tc3g_kernel<4, PREC_FP32>;
+template <bool REFL>
+static inline Tc3Kernel grouped_kernel_t(int grp, int prec) {
+    if (prec == PREC_BF16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_BF16, REFL> : conv1d_tc3g_kernel<4, PREC_BF16, REFL>;
+    if (prec == PREC_FP16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP16, REFL> : conv1d_tc3g_kernel<4, PREC_FP16, REFL>;
+    return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP32, REFL> : conv1d_tc3g_kernel<4, PREC_FP32, REFL>;
+}
+static inline Tc3Kernel grouped_kernel(int grp, int prec = PREC_FP32, bool reflect = false) {
+    return reflect ? grouped_kernel_t<true>(grp, prec) : grouped_kernel_t<false>(grp, prec);
 }
 
 }  // namespace tc3

@@ -210,6 +210,29 @@ struct GlowTTS {
                float* y_log_scale, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
 };
 
+// MelGAN generators (melgan.cu): conv_pre -> per stage [lrelu 0.2 -> ConvTranspose1d -> residual stack] -> lrelu 0.2 ->
+// conv_post -> tanh, every k > 1 conv reflect-padded; optional PQMF synthesis of the band signals.  Stage tensors use a row
+// pitch rounded up to 4 floats (16-byte aligned rows for the tensor-core producers).
+struct Melgan {
+    struct Block { ConvLayer dil, c1x1, shortcut; };
+    b200tts_melgan_config c;
+    ConvLayer conv_pre, conv_post;
+    std::vector<ConvLayer> ups;
+    std::vector<std::vector<Block>> blocks;   // [stage][block]
+    float* G = nullptr;                       // device [bands][taps + 1] PQMF synthesis filter (pqmf_bands > 0)
+    ~Melgan();
+    int init(const b200tts_melgan_config& cfg, const float* const* w, int nw);
+    void stage_dims(int T, std::vector<int>& C, std::vector<int>& L) const;
+    size_t workspace_bytes(int B, int T) const;
+    int out_len(int T) const;
+    int check_len(int T) const;               // 0, or 1 with the error set when a reflect pad would exceed its input
+    int forward(const float* x, int B, int T, int synthesize, float* out, unsigned* peak_bits, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+};
+// PQMF synthesis (melgan.cu): x [B, N, Tb] (row pitch x_cs, batch stride x_bs) -> y [B, 1, N * Tb]; G [N][taps + 1]
+int launch_pqmf_synthesis(const float* x, long long x_bs, int x_cs, int B, int N, int Tb, const float* G, int taps, float* y,
+                          unsigned* peak_bits, cudaStream_t st);
+
 // durations -> path -> expanded prior (path.cu)
 int launch_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st);

@@ -3,7 +3,9 @@
 Mirrors, with the reference's names and argument meaning:
   HifiganConfig        <- /root/reference/TTS/vocoder/configs/hifigan_config.py:7-136 (+ BaseAudioConfig,
                           TTS/config/shared_configs.py:9-176: the audio fields the hand-off reads)
-  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-48   (generator_model == "hifigan_generator")
+  MelganConfig / MultibandMelganConfig / FullbandMelganConfig
+                       <- TTS/vocoder/configs/{melgan,multiband_melgan,fullband_melgan}_config.py (generator side)
+  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-94   (the HiFiGAN and MelGAN generator families)
   GAN                  <- TTS/vocoder/models/gan.py:21-66,338-352 (model_g, forward, inference, load_checkpoint)
   AudioProcessor.normalize / denormalize   <- TTS/utils/audio/processor.py:259-337   (as ``AudioNorm``)
   interpolate_vocoder_input                <- TTS/vocoder/utils/generic_utils.py:11-29
@@ -23,6 +25,7 @@ from torch import nn
 
 from . import _lib
 from .hifigan import HifiganGenerator
+from .melgan import FullbandMelganGenerator, MelganGenerator, MultibandMelganGenerator
 
 
 # ----------------------------------------------------------------------------- configs
@@ -77,6 +80,53 @@ class HifiganConfig(_ItemAccess):
     audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
 
 
+_MELGAN_DISCRIMINATOR = "melgan_multiscale_discriminator"
+
+
+@dataclass
+class MelganConfig(_ItemAccess):
+    """Generator-side fields of TTS/vocoder/configs/melgan_config.py:65-75 (+ ``use_pqmf`` of the shared GAN config)."""
+    model: str = "melgan"
+    discriminator_model: str = _MELGAN_DISCRIMINATOR
+    generator_model: str = "melgan_generator"
+    generator_model_params: dict = field(default_factory=lambda: {"upsample_factors": [8, 8, 2, 2], "num_res_blocks": 3})
+    use_pqmf: bool = False
+    audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
+
+
+@dataclass
+class MultibandMelganConfig(_ItemAccess):
+    """Generator-side fields of TTS/vocoder/configs/multiband_melgan_config.py:93-102."""
+    model: str = "multiband_melgan"
+    discriminator_model: str = _MELGAN_DISCRIMINATOR
+    generator_model: str = "multiband_melgan_generator"
+    generator_model_params: dict = field(default_factory=lambda: {"upsample_factors": [8, 4, 2], "num_res_blocks": 4})
+    use_pqmf: bool = True
+    audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
+
+
+@dataclass
+class FullbandMelganConfig(_ItemAccess):
+    """Generator-side fields of TTS/vocoder/configs/fullband_melgan_config.py:65-75.  As in the reference, the generator
+    it names is ``melgan_generator`` (a plain MelGAN with 4 residual blocks), not ``fullband_melgan_generator``."""
+    model: str = "fullband_melgan"
+    discriminator_model: str = _MELGAN_DISCRIMINATOR
+    generator_model: str = "melgan_generator"
+    generator_model_params: dict = field(default_factory=lambda: {"upsample_factors": [8, 8, 2, 2], "num_res_blocks": 4})
+    use_pqmf: bool = False
+    audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
+
+
+# the generator modules under TTS/vocoder/models/ that setup_generator can import
+_GENERATOR_MODULES = ("hifigan_generator", "melgan_generator", "multiband_melgan_generator", "fullband_melgan_generator",
+                      "parallel_wavegan_generator", "univnet_generator")
+
+
+class GeneratorParamsError(KeyError, NotImplementedError):
+    """``generator_model_params`` lacks a field the named generator needs (the reference raises KeyError there); also a
+    NotImplementedError, so that callers that treat an unbuildable generator as such keep working."""
+
+
 def to_camel(text):
     """TTS/vocoder/models/__init__.py:7-9 (generator_model name -> class name)."""
     text = text.capitalize()
@@ -84,13 +134,43 @@ def to_camel(text):
 
 
 def setup_generator(c):
-    """TTS/vocoder/models/__init__.py:34-48: builds the generator a vocoder config names.  Only
-    ``hifigan_generator`` is on the path (the other generator families are out of scope and raise)."""
+    """TTS/vocoder/models/__init__.py:34-94: builds the generator a vocoder config names, resolving the name the way the
+    reference does.  The reference first imports the module ``TTS.vocoder.models.<name.lower()>``, so only the names of
+    its generator modules (in any letter case) get as far as its ``name in "..."`` substring tests; any other name
+    raises NotImplementedError here (the reference fails it at that import).  ``melgan_fb_generator`` raises the
+    reference's ValueError ("now fullband_melgan_generator").  The HiFiGAN and MelGAN families are on the path;
+    ParallelWaveGAN and UniVNet are out of scope and raise NotImplementedError."""
     name = _get(c, "generator_model")
-    if name.lower() != "hifigan_generator":
-        raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (only hifigan_generator is on the path)")
-    audio = _get(c, "audio")
-    return HifiganGenerator(in_channels=_get(audio, "num_mels"), out_channels=1, **dict(_get(c, "generator_model_params")))
+    low = name.lower()
+    if name == "melgan_fb_generator":
+        raise ValueError("melgan_fb_generator is now fullband_melgan_generator")
+    if low not in _GENERATOR_MODULES:
+        raise NotImplementedError(f"tts_b200.setup_generator: `{name}` names no generator module "
+                                  f"(one of {sorted(_GENERATOR_MODULES)})")
+    num_mels = _get(_get(c, "audio"), "num_mels")
+    params = _get(c, "generator_model_params")
+
+    def param(key):
+        try:
+            return params[key]
+        except KeyError:
+            raise GeneratorParamsError(f"tts_b200.setup_generator: `{name}` needs generator_model_params[{key!r}]") from None
+
+    if low in "hifigan_generator":
+        return HifiganGenerator(in_channels=num_mels, out_channels=1, **dict(params))
+    melgan = dict(proj_kernel=7, res_kernel=3)
+    if low in "melgan_generator":
+        return MelganGenerator(in_channels=num_mels, out_channels=1, base_channels=512,
+                               upsample_factors=param("upsample_factors"), num_res_blocks=param("num_res_blocks"), **melgan)
+    if low in "multiband_melgan_generator":
+        return MultibandMelganGenerator(in_channels=num_mels, out_channels=4, base_channels=384,
+                                        upsample_factors=param("upsample_factors"), num_res_blocks=param("num_res_blocks"),
+                                        **melgan)
+    if low in "fullband_melgan_generator":
+        return FullbandMelganGenerator(in_channels=num_mels, out_channels=1, base_channels=512,
+                                       upsample_factors=param("upsample_factors"), num_res_blocks=param("num_res_blocks"),
+                                       **melgan)
+    raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN and MelGAN generators are)")
 
 
 def _get(obj, key, default=None):
