@@ -500,6 +500,67 @@ int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, con
                             int Ty, float* attn, float* y_mean, float* y_log_scale, float* mel, void* workspace,
                             size_t workspace_bytes, void* stream);
 
+/* ---- ForwardTTS inference (FastPitch / FastSpeech / FastSpeech2: text -> mel spectrogram) ----------------------------
+ * Replaces ForwardTTS.inference, TTS/tts/models/forward_tts.py:672-714, for encoder_type and decoder_type "fftransformer"
+ * (FFTransformerBlock, TTS/tts/layers/generic/transformer.py:6-69), in two calls around the one host read of the
+ * decoder length: encode (:685-704: encoder, speaker add, duration / pitch / energy predictors, format_durations
+ * :353-372), then decode (:417-451: generate_path, expansion, positional encoding :generic/pos_encoding.py:38-69,
+ * FFTransformerDecoder :feed_forward/decoder.py:117-122).
+ * Batched, unlike the reference (whose inference takes x_lengths = [T], :686): row b computes the reference's
+ * inference(x[b:b+1, :lengths[b]]).  Padded tokens get 0 frames; keys, conv inputs and outputs stop at each row's length.
+ * weights (host, PyTorch layouts), in this order:
+ *   emb.weight [n_vocab, C]
+ *   per encoder layer: self_attn.in_proj_weight [3C, C] (rows q|k|v), in_proj_bias [3C], out_proj.weight [C, C], .bias,
+ *     conv1.w [Fe, C, 3], .b, conv2.w [C, Fe, 3], .b, norm1.weight [C], .bias, norm2.weight, .bias
+ *   if proj_g_in > 0: proj_g.weight [C, proj_g_in], .bias [C]            (nn.Linear, :303)
+ *   duration_predictor: conv_1.w [Fd, C, k], .b, norm_1.gamma, .beta, conv_2.w, .b, norm_2.gamma, .beta, proj.w, .b
+ *   if use_pitch: pitch_predictor (same 10 tensors), pitch_emb.w [C, 1, kp], .b
+ *   if use_energy: energy_predictor (same 10 tensors), energy_emb.w [C, 1, ke], .b
+ *   if pe_len > 0: pos_encoder.pe [C, pe_len]
+ *   per decoder layer: the 12 tensors of an encoder layer (Fdec channels in the FFN)
+ *   decoder.postnet.w [out_channels, C, 1], .b
+ * encode: tokens int64 [B,Tt], lengths int64 [B], g [B, C] (emb_g row or d-vector) or [B, proj_g_in] (d-vector to
+ *   project) or NULL -> o_en [B, C, Tt] (encoder output + g, + pitch / energy embeddings), logw [B,Tt] (durations_log),
+ *   pitch / energy [B,Tt] (NULL without the predictor), x_mask [B,Tt], dur [B,Tt] (frames per token), cum [B,Tt],
+ *   y_lengths int64 [B], meta int64 [2] = {max_b y_lengths, 0}: read it to size the decode call (Ty = meta[0]).
+ * decode: attn [B, Ty, Tt] (the returned alignments; or NULL), mel [B, Ty, out_channels] (model_outputs, zero past each
+ *   row's y_length).  Ty > pe_len is an error, as in PositionalEncoding.forward.
+ * No float atomics: repeat calls are bit-identical.
+ */
+typedef struct {
+    int n_vocab;
+    int hidden_channels;       /* C */
+    int out_channels;
+    int enc_heads, enc_layers, enc_ffn;
+    int dec_heads, dec_layers, dec_ffn;
+    int proj_g_in;             /* d-vector width projected by proj_g, 0: g (if any) is added as given */
+    int dp_hidden, dp_kernel;
+    int use_pitch, pitch_hidden, pitch_kernel, pitch_emb_kernel;
+    int use_energy, energy_hidden, energy_kernel, energy_emb_kernel;
+    int pe_len;                /* columns of pos_encoder.pe, 0: no positional encoding (and no sqrt(C) scale) */
+} b200tts_forward_tts_config;
+typedef struct b200tts_forward_tts b200tts_forward_tts;
+int b200tts_forward_tts_create(const b200tts_forward_tts_config* cfg, const float* const* weights, int num_weights,
+                               b200tts_forward_tts** out);
+void b200tts_forward_tts_destroy(b200tts_forward_tts* h);
+size_t b200tts_forward_tts_encode_workspace_bytes(const b200tts_forward_tts* h, int B, int Tt);
+size_t b200tts_forward_tts_decode_workspace_bytes(const b200tts_forward_tts* h, int B, int Ty);
+int b200tts_forward_tts_encode(const b200tts_forward_tts* h, const int64_t* tokens, const int64_t* lengths,
+                               const float* g, float length_scale, int B, int Tt, float* o_en, float* logw, float* pitch,
+                               float* energy, float* x_mask, float* dur, float* cum, int64_t* y_lengths, int64_t* meta,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int b200tts_forward_tts_decode(const b200tts_forward_tts* h, const float* o_en, const float* x_mask, const float* cum,
+                               const int64_t* y_lengths, int B, int Tt, int Ty, float* attn, float* mel, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
+/* ---- self-attention on the tensor cores (ForwardTTS decoder) --------------------------------------------------------
+ * Replaces nn.MultiheadAttention's attention core (softmax((q d^-1/2) k^T) v, torch/nn/functional.py
+ * multi_head_attention_forward) over a fused [B, 3C, pitch] q|k|v tensor, per row over its first lens[b] (int32) frames.
+ * out [B, C, pitch]; columns lens[b] .. pitch-1 are zeroed.  Heads need (C / num_heads) % 8 == 0 and <= 384.
+ */
+int b200tts_attention_tc3(const float* qkv, const int* lens, int B, int C, int num_heads, int T, int pitch, float* out,
+                          void* stream);
+
 /* ---- MelGAN generators (plain, full-band, multi-band with PQMF synthesis) ---------------------------
  * Replaces MelganGenerator.forward (TTS/vocoder/models/melgan_generator.py:9-74, ResidualStack
  * TTS/vocoder/layers/melgan.py:6-36) and, for the multi-band generator, PQMF.synthesis (TTS/vocoder/layers/pqmf.py:50-53;

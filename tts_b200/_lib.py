@@ -77,6 +77,14 @@ class GlowTTSConfigC(ctypes.Structure):
                                             "num_splits", "num_squeeze", "sigmoid_scale")]
 
 
+class ForwardTTSConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "hidden_channels", "out_channels", "enc_heads", "enc_layers",
+                                            "enc_ffn", "dec_heads", "dec_layers", "dec_ffn", "proj_g_in", "dp_hidden",
+                                            "dp_kernel", "use_pitch", "pitch_hidden", "pitch_kernel",
+                                            "pitch_emb_kernel", "use_energy", "energy_hidden", "energy_kernel",
+                                            "energy_emb_kernel", "pe_len")]
+
+
 class MelganConfigC(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int) for n in ("in_channels", "out_channels", "base_channels", "proj_kernel", "res_kernel",
                                             "num_res_blocks", "num_upsamples")] + \
@@ -93,7 +101,8 @@ class AudioNormC(ctypes.Structure):
                 ("scaler_mean", ctypes.c_void_p), ("scaler_scale", ctypes.c_void_p)]
 
 
-DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped"}
+DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped", 10: "attn_tc3",
+                  11: "attn_fma"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2}
@@ -218,6 +227,22 @@ def _declare(lib):
     lib.b200tts_glow_tts_decode.restype = ci
     lib.b200tts_glow_tts_decode.argtypes = [vp, vp, vp, vp, vp, vp, vp, ctypes.c_float, ci, ci, ci, vp, vp, vp, vp, vp,
                                             sz, vp]
+    lib.b200tts_forward_tts_create.restype = ci
+    lib.b200tts_forward_tts_create.argtypes = [ctypes.POINTER(ForwardTTSConfigC), ctypes.POINTER(vp), ci,
+                                               ctypes.POINTER(vp)]
+    lib.b200tts_forward_tts_destroy.restype = None
+    lib.b200tts_forward_tts_destroy.argtypes = [vp]
+    lib.b200tts_forward_tts_encode_workspace_bytes.restype = sz
+    lib.b200tts_forward_tts_encode_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_forward_tts_decode_workspace_bytes.restype = sz
+    lib.b200tts_forward_tts_decode_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_forward_tts_encode.restype = ci
+    lib.b200tts_forward_tts_encode.argtypes = [vp, vp, vp, vp, ctypes.c_float, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp,
+                                               vp, vp, sz, vp]
+    lib.b200tts_forward_tts_decode.restype = ci
+    lib.b200tts_forward_tts_decode.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, vp, vp, vp, sz, vp]
+    lib.b200tts_attention_tc3.restype = ci
+    lib.b200tts_attention_tc3.argtypes = [vp, vp, ci, ci, ci, ci, ci, vp, vp]
     lib.b200tts_stft_create.restype = ci
     lib.b200tts_stft_create.argtypes = [ci, ci, vp, vp, ci, ctypes.POINTER(vp)]
     lib.b200tts_stft_destroy.restype = None

@@ -15,6 +15,7 @@ struct b200tts_duration_predictor { DurPred impl; };
 struct b200tts_speaker_encoder { SpeakerEncoder impl; };
 struct b200tts_glow_tts { GlowTTS impl; };
 struct b200tts_melgan { Melgan impl; };
+struct b200tts_forward_tts { ForwardTTS impl; };
 
 extern "C" {
 
@@ -392,6 +393,46 @@ int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, con
     if (!h) { set_error("glow_tts_decode: null handle"); return 1; }
     return h->impl.decode(o_stats, x_mask, cum, (const long long*)y_lengths, g, noise, noise_scale, B, Tt, Ty, attn,
                           y_mean, y_log_scale, mel, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200tts_forward_tts_create(const b200tts_forward_tts_config* cfg, const float* const* weights, int num_weights,
+                               b200tts_forward_tts** out) {
+    if (!cfg || !weights || !out) { set_error("forward_tts_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_forward_tts* h = new (std::nothrow) b200tts_forward_tts();
+    if (!h) { set_error("forward_tts_create: out of host memory"); return 1; }
+    int rc = h->impl.init(*cfg, weights, num_weights);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+void b200tts_forward_tts_destroy(b200tts_forward_tts* h) { delete h; }
+size_t b200tts_forward_tts_encode_workspace_bytes(const b200tts_forward_tts* h, int B, int Tt) {
+    return h ? h->impl.encode_bytes(B, Tt) : 0;
+}
+size_t b200tts_forward_tts_decode_workspace_bytes(const b200tts_forward_tts* h, int B, int Ty) {
+    return h ? h->impl.decode_bytes(B, Ty) : 0;
+}
+int b200tts_forward_tts_encode(const b200tts_forward_tts* h, const int64_t* tokens, const int64_t* lengths,
+                               const float* g, float length_scale, int B, int Tt, float* o_en, float* logw, float* pitch,
+                               float* energy, float* x_mask, float* dur, float* cum, int64_t* y_lengths, int64_t* meta,
+                               void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("forward_tts_encode: null handle"); return 1; }
+    return h->impl.encode((const long long*)tokens, (const long long*)lengths, g, length_scale, B, Tt, o_en, logw, pitch,
+                          energy, x_mask, dur, cum, (long long*)y_lengths, (long long*)meta, workspace, workspace_bytes,
+                          (cudaStream_t)stream);
+}
+int b200tts_forward_tts_decode(const b200tts_forward_tts* h, const float* o_en, const float* x_mask, const float* cum,
+                               const int64_t* y_lengths, int B, int Tt, int Ty, float* attn, float* mel, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("forward_tts_decode: null handle"); return 1; }
+    return h->impl.decode(o_en, x_mask, cum, (const long long*)y_lengths, B, Tt, Ty, attn, mel, workspace,
+                          workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_attention_tc3(const float* qkv, const int* lens, int B, int C, int num_heads, int T, int pitch, float* out,
+                          void* stream) {
+    return launch_attention_tc3(qkv, (long long)3 * C * pitch, pitch, lens, out, (long long)C * pitch, B, C, num_heads, T,
+                                (cudaStream_t)stream);
 }
 
 B200_HANDLE_API(melgan, b200tts_melgan, b200tts_melgan_config)

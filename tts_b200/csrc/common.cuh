@@ -149,7 +149,9 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
 // which kernel family a launch_conv call dispatched to (recorded per thread between dispatch_begin/end; tests pin it)
 enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6,
-             DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9 };   // TC16*: the same kernels with bf16 / fp16 operands
+             DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9,    // TC16*: the same kernels with bf16 / fp16 operands
+             // ForwardTTS decoder attention: the tensor-core kernel, or the FP32-FMA kernel for heads it does not take
+             DISPATCH_ATTN_TC3 = 10, DISPATCH_ATTN_FMA = 11 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -92,10 +92,11 @@ struct DurPred {
 int launch_upsample_linear(const float* x, int rows, int Tin, float scale_factor, float* y, int Tout, cudaStream_t st);
 int launch_add_layernorm(const float* x, const float* y, const float* gamma, const float* beta, const float* mask,
                          float* out, int B, int C, int T, float eps, cudaStream_t st);
-// text_encoder.cu's embedding (x = emb[tok] * sqrt(hidden) * mask, plus the x_mask) and multi-head attention over a fused
-// [B, 3C, T] q|k|v tensor; window < 0: no relative-position terms (rel_k / rel_v unused)
+// text_encoder.cu's embedding (x = emb[tok] * sqrt(hidden) * mask, plus the x_mask; without the sqrt(hidden) scale when
+// scale_sqrt_hidden is false) and multi-head attention over a fused [B, 3C, T] q|k|v tensor; window < 0: no
+// relative-position terms (rel_k / rel_v unused).  Heads up to 384 channels.
 int launch_embed(const long long* tokens, const long long* lengths, const float* emb, const float* lang_emb, int B,
-                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st);
+                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st, bool scale_sqrt_hidden = true);
 int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
                      int C, int T, int num_heads, int window, cudaStream_t st);
 
@@ -210,6 +211,39 @@ struct GlowTTS {
                float* y_log_scale, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
 };
 
+// ForwardTTS inference (forward_tts.cu): FastPitch / FastSpeech / FastSpeech2 with FFTransformer encoder and decoder.
+// encode runs the text side on the exact FP32 FMA conv (embedding, encoder, speaker add, duration / pitch / energy
+// predictors and embeddings, durations); after the caller's one host read of max(y_lengths), decode expands the encoder
+// output with the positional encoding and runs the decoder on the 3xTF32 tensor-core convs and attention_tc3.cu.
+// Decoder tensors are [B, C, Tp] with Tp = frames rounded up to 4 (16-byte rows); every row stops at its y_length.
+struct ForwardTTS {
+    struct Layer {   // FFTransformer (TTS/tts/layers/generic/transformer.py:6-35)
+        ConvLayer qkv, o, ffn1, ffn2;
+        float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
+    };
+    b200tts_forward_tts_config c;
+    float* emb = nullptr;
+    float* pe = nullptr;               // pos_encoder.pe [C][pe_len] (null without positional encoding)
+    std::vector<Layer*> enc, dec;
+    ConvLayer proj_g, pitch_emb, energy_emb, postnet;
+    DurPred dp, pitch_dp, energy_dp;
+    ~ForwardTTS();
+    int init(const b200tts_forward_tts_config& cfg, const float* const* w, int nw);
+    static int tp(int Ty) { return (Ty + 3) / 4 * 4; }
+    size_t encode_bytes(int B, int Tt) const;
+    size_t decode_bytes(int B, int Ty) const;
+    int encode(const long long* tokens, const long long* lengths, const float* g, float length_scale, int B, int Tt,
+               float* o_en, float* logw, float* pitch, float* energy, float* x_mask, float* dur, float* cum,
+               long long* y_lengths, long long* meta, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    int decode(const float* o_en, const float* x_mask, const float* cum, const long long* y_lengths, int B, int Tt,
+               int Ty, float* attn, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
+};
+// attention_tc3.cu: self-attention over a [B, 3C, pitch] q|k|v tensor (batch stride qkv_bs) into out [B, C, pitch] (batch
+// stride out_bs), per row over the first lens[b] frames only (queries and keys; the other columns of out are zeroed)
+bool attention_tc3_takes(int head_dim);
+int launch_attention_tc3(const float* qkv, long long qkv_bs, int pitch, const int* lens, float* out, long long out_bs,
+                         int B, int C, int num_heads, int T, cudaStream_t st);
+
 // MelGAN generators (melgan.cu): conv_pre -> per stage [lrelu 0.2 -> ConvTranspose1d -> residual stack] -> lrelu 0.2 ->
 // conv_post -> tanh, every k > 1 conv reflect-padded; optional PQMF synthesis of the band signals.  Stage tensors use a row
 // pitch rounded up to 4 floats (16-byte aligned rows for the tensor-core producers).
@@ -236,6 +270,10 @@ int launch_pqmf_synthesis(const float* x, long long x_bs, int x_cs, int B, int N
 // durations -> path -> expanded prior (path.cu)
 int launch_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st);
+// ForwardTTS rule (forward_tts.py:369-371): dur = round_half_even(max(1, (exp(logw) - 1) * x_mask * length_scale)) for a
+// valid token, 0 for a padded one; y_lengths = sum(dur)
+int launch_durations_forward(const float* logw, const float* x_mask, float length_scale, int B, int T, float* dur,
+                             float* cum, long long* y_lengths, long long* meta, cudaStream_t st);
 // Glow-TTS rule: w_ceil = max(1, ceil((exp(logw) - 1) * x_mask * length_scale)); dur_log = log(1 + w_ceil * x_mask) * x_mask
 int launch_durations_glow(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                           float* cum, long long* y_lengths, float* dur_log, long long* meta, cudaStream_t st);

@@ -16,7 +16,11 @@ namespace {
 // GLOW: the Glow-TTS rule (glow_tts.py:350-352), w = (exp(logw) - 1) * x_mask * length_scale and w_ceil =
 // clamp_min(ceil(w), 1) -- the clamp gives every padded token one frame too -- plus dur_log = log(1 + sum(attn, -1)) *
 // x_mask of compute_outputs (:147): a valid token's path row holds w_ceil ones, a padded token's none.
-template <bool GLOW>
+// FORWARD: the ForwardTTS rule (forward_tts.py:369-371), w = (exp(logw) - 1) * x_mask * length_scale, values below 1
+// become 1, then round half to even (torch.round); a padded token gets 0 frames.  exp is evaluated in double and
+// rounded once, so the exactly representable ties (2.5, 3.5, ...) come out as the reference's.
+enum : int { RULE_VITS = 0, RULE_GLOW = 1, RULE_FORWARD = 2 };
+template <int RULE>
 __global__ void durations_kernel(const float* logw, const float* x_mask, float length_scale, float* w_ceil,
                                  float* cum, long long* y_lengths, int B, int T, const int* err_flag, long long* meta,
                                  float* dur_log) {
@@ -30,10 +34,14 @@ __global__ void durations_kernel(const float* logw, const float* x_mask, float l
             float wc = 0.f;
             if (t < T) {
                 const float m = x_mask[(size_t)b * T + t];
-                if (GLOW) {
+                if (RULE == RULE_GLOW) {
                     const float w = __fmul_rn(__fmul_rn(__fsub_rn(expf(logw[(size_t)b * T + t]), 1.f), m), length_scale);
                     wc = fmaxf(ceilf(w), 1.f);
                     dur_log[(size_t)b * T + t] = __fmul_rn(logf(__fadd_rn(1.f, __fmul_rn(wc, m))), m);
+                } else if (RULE == RULE_FORWARD) {
+                    const float e = (float)exp((double)logw[(size_t)b * T + t]);
+                    const float w = __fmul_rn(__fmul_rn(__fsub_rn(e, 1.f), m), length_scale);
+                    wc = m != 0.f ? rintf(w < 1.f ? 1.f : w) : 0.f;
                 } else {
                     const float w = __fmul_rn(__fmul_rn(expf(logw[(size_t)b * T + t]), m), length_scale);
                     wc = ceilf(w);
@@ -50,7 +58,7 @@ __global__ void durations_kernel(const float* logw, const float* x_mask, float l
             if (t < T) cum[(size_t)b * T + t] = s;
             carry = __shfl_sync(0xffffffffu, s, 31);
         }
-        const long long yl = (long long)fmaxf(carry, 1.f);
+        const long long yl = RULE == RULE_FORWARD ? (long long)carry : (long long)fmaxf(carry, 1.f);
         if (lane == 0) y_lengths[b] = yl;
         mymax = yl > mymax ? yl : mymax;
     }
@@ -106,7 +114,7 @@ int launch_durations(const float* logw, const float* x_mask, float length_scale,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st) {
     B200_REQUIRE(logw && x_mask && w_ceil && cum && y_lengths, "durations: null pointer");
     if (B == 0) return 0;
-    durations_kernel<false><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
+    durations_kernel<RULE_VITS><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
                                                                  B, T, err_flag, meta, nullptr);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
@@ -117,8 +125,19 @@ int launch_durations_glow(const float* logw, const float* x_mask, float length_s
                           float* cum, long long* y_lengths, float* dur_log, long long* meta, cudaStream_t st) {
     B200_REQUIRE(logw && x_mask && w_ceil && cum && y_lengths && dur_log, "durations_glow: null pointer");
     if (B == 0) return 0;
-    durations_kernel<true><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
+    durations_kernel<RULE_GLOW><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, w_ceil, cum, y_lengths,
                                                                 B, T, nullptr, meta, dur_log);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_durations_forward(const float* logw, const float* x_mask, float length_scale, int B, int T, float* dur,
+                             float* cum, long long* y_lengths, long long* meta, cudaStream_t st) {
+    B200_REQUIRE(logw && x_mask && dur && cum && y_lengths, "durations_forward: null pointer");
+    if (B == 0) return 0;
+    durations_kernel<RULE_FORWARD><<<1, 32 * (B < 32 ? B : 32), 0, st>>>(logw, x_mask, length_scale, dur, cum,
+                                                                        y_lengths, B, T, nullptr, meta, nullptr);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     return 0;

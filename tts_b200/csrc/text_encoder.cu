@@ -28,9 +28,11 @@ __global__ void embed_kernel(const long long* tok, const long long* len, const f
 
 constexpr int ATT_Q = 8;        // queries per CTA (one warp each)
 constexpr int ATT_KT = 32;      // keys per tile
-constexpr int ATT_MAXD = 256;   // max head dim (8 values per lane)
+constexpr int ATT_MAXD = 256;   // max head dim of the VITS / Glow-TTS instantiation (8 values per lane)
+constexpr int ATT_MAXD_WIDE = 384;   // ForwardTTS's text encoder: one head of 384 channels (12 values per lane)
 
-// qkv [B, 3C, T] (q rows 0..C, k rows C..2C, v rows 2C..3C), head h owns channels [h*d, (h+1)*d)
+// qkv [B, 3C, T] (q rows 0..C, k rows C..2C, v rows 2C..3C), head h owns channels [h*d, (h+1)*d); MAXD bounds d
+template <int MAXD>
 __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* __restrict__ qkv, const float* __restrict__ mask,
                                                                   const float* __restrict__ emb_rel_k, const float* __restrict__ emb_rel_v,
                                                                   float* __restrict__ out, int C, int T, int d, int window,
@@ -87,9 +89,9 @@ __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* 
     }
     __syncwarp();
     const float mi = active ? mb[i] : 0.f;
-    float outv[ATT_MAXD / 32];
+    float outv[MAXD / 32];
 #pragma unroll
-    for (int u = 0; u < ATT_MAXD / 32; ++u) outv[u] = 0.f;
+    for (int u = 0; u < MAXD / 32; ++u) outv[u] = 0.f;
     if (active) {
         // ---- relative-key logits on the +-window band (transformer.py:132-138)
         if (window >= 0 && lane < nrel) {
@@ -148,7 +150,7 @@ __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* 
         if (active) {
             const float* p = sc + warp * Tp + j0;
 #pragma unroll
-            for (int u = 0; u < ATT_MAXD / 32; ++u) {
+            for (int u = 0; u < MAXD / 32; ++u) {
                 const int c = lane + 32 * u;
                 if (c < d) {
                     float a = outv[u];
@@ -160,7 +162,7 @@ __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* 
     }
     if (active) {
 #pragma unroll
-        for (int u = 0; u < ATT_MAXD / 32; ++u) {
+        for (int u = 0; u < MAXD / 32; ++u) {
             const int c = lane + 32 * u;
             if (c < d) {
                 float a = outv[u];
@@ -225,9 +227,10 @@ int launch_add_layernorm(const float* x, const float* y, const float* gamma, con
 }
 
 int launch_embed(const long long* tokens, const long long* lengths, const float* emb, const float* lang_emb, int B,
-                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st) {
+                 int T, int hidden, int C, float* x, float* x_mask, cudaStream_t st, bool scale_sqrt_hidden) {
     dim3 grid((T + 127) / 128, C, B);
-    embed_kernel<<<grid, 128, 0, st>>>(tokens, lengths, emb, lang_emb, x, x_mask, T, hidden, C, sqrtf((float)hidden));
+    embed_kernel<<<grid, 128, 0, st>>>(tokens, lengths, emb, lang_emb, x, x_mask, T, hidden, C,
+                                       scale_sqrt_hidden ? sqrtf((float)hidden) : 1.f);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     return 0;
@@ -236,7 +239,7 @@ int launch_embed(const long long* tokens, const long long* lengths, const float*
 int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
                      int C, int T, int num_heads, int window, cudaStream_t st) {
     const int d = C / num_heads;
-    B200_REQUIRE(C % num_heads == 0 && d <= ATT_MAXD, "attention: head dim %d (C=%d, %d heads) not supported", d, C,
+    B200_REQUIRE(C % num_heads == 0 && d <= ATT_MAXD_WIDE, "attention: head dim %d (C=%d, %d heads) not supported", d, C,
                  num_heads);
     B200_REQUIRE(window < 0 || (rel_k && rel_v && 2 * window + 1 <= 32), "attention: bad relative window");
     const int Tp = (T + 31) & ~31;
@@ -246,12 +249,16 @@ int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, 
     B200_REQUIRE(att_smem <= 200 * 1024, "attention: T=%d too long for the attention kernel", T);
     static DeviceOnce attr_once;
     if (int rc0 = device_once(attr_once, nullptr, [](int) -> int {
-            B200_CUDA_OK(cudaFuncSetAttribute(rel_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+            B200_CUDA_OK(cudaFuncSetAttribute(rel_attention_kernel<ATT_MAXD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              200 * 1024));
+            B200_CUDA_OK(cudaFuncSetAttribute(rel_attention_kernel<ATT_MAXD_WIDE>,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
             return 0;
         })) return rc0;
     dim3 grid((T + ATT_Q - 1) / ATT_Q, num_heads, B);
-    rel_attention_kernel<<<grid, 32 * ATT_Q, att_smem, st>>>(qkv, x_mask, rel_k, rel_v, out, C, T, d, window,
-                                                            1.f / sqrtf((float)d));
+    // heads up to 256 channels keep the narrow instantiation (fewer registers per lane)
+    auto kern = d <= ATT_MAXD ? rel_attention_kernel<ATT_MAXD> : rel_attention_kernel<ATT_MAXD_WIDE>;
+    kern<<<grid, 32 * ATT_Q, att_smem, st>>>(qkv, x_mask, rel_k, rel_v, out, C, T, d, window, 1.f / sqrtf((float)d));
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     return 0;
