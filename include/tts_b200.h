@@ -30,9 +30,12 @@ const char* b200tts_last_error(void);
 /* number of kernels launched by this library in this process (bench.py "gpu_launches") */
 unsigned long long b200tts_launch_count(void);
 int b200tts_version(void);
-/* 1 if a tensor-core conv launch (on any device of this process) ever hit a pipeline timeout.  The flag lives in mapped
- * host memory: no synchronisation here (call after a stream sync to cover the launches before it).  Every later
- * conv launch on that device also checks it and returns status 1, so a timeout cannot pass silently. */
+/* Bit 0 (value 1): a tensor-core conv launch (on any device of this process) ever hit a pipeline timeout.  Bit 1
+ * (value 2): a split-fp16 launch (B200TTS_PRECISION_F16X3, the HiFiGAN default) read an activation with |x| >= 65504,
+ * which fp16 cannot hold, so its output is invalid.  The flags live in mapped host memory: no synchronisation here
+ * (call after a stream sync to cover the launches before it).  Every later conv launch on that device also checks them
+ * and returns status 1, so neither can pass silently: a timeout for good, a range error once (that launch then clears
+ * it -- the data was out of range, the device is fine). */
 int b200tts_debug_tc_error(void);
 
 /* Debug / test aids: record, on the calling thread, which kernel family every conv launch dispatched to.
@@ -41,13 +44,20 @@ int b200tts_debug_tc_error(void);
 void b200tts_debug_dispatch_begin(void);
 int b200tts_debug_dispatch_end(int32_t* ids, int cap); /* returns the number of launches recorded */
 
-/* Operand precision of the tensor-core convs (opt-in; FP32 is the default everywhere).
- *   FP32: 3xTF32 split operands, fp32-class accuracy.
+/* Operand precision of the tensor-core convs (FP32 is the default everywhere).
+ *   FP32: fp32-class accuracy, the arithmetic chosen per engine: F16X3 for the HiFiGAN decoder's conv_pre, upsamplers
+ *     and resblock convs, TF32X3 for every other layer and for b200tts_conv1d.
+ *   TF32X3: 3xTF32 split operands (hi + lo, 3 tf32 MMAs per product), fp32-class accuracy over fp32's whole range.
+ *   F16X3: the same split in fp16 (same 11-bit significand, twice the MMA rate): weights rows scaled by a power of two
+ *     into fp16's range at pack time, activations split as hi = fp16(x), lo = fp16((x - hi) * 2^11); fp32-class accuracy
+ *     (operands to 2^-22 relative) for |x| < 65504.  A larger activation sets bit 1 of b200tts_debug_tc_error and
+ *     fails the next conv launch; TF32X3 takes such models.  Dispatch ids stay 3 / 5.
  *   BF16 / FP16: activations (after the leaky ReLU) and weights (after the weight-norm fold) are rounded to the 16-bit type
  *     and multiplied with fp32 accumulation; epilogues, residuals and every tensor in memory stay fp32.  bf16 keeps fp32's
  *     range with an 8-bit significand; fp16 has an 11-bit significand but overflows past +-65504 (such values become
  *     +-inf).  Only layers with in_channels % 16 == 0 take the 16-bit kernels (dispatch ids 8 / 9); others stay FP32. */
-enum { B200TTS_PRECISION_FP32 = 0, B200TTS_PRECISION_BF16 = 1, B200TTS_PRECISION_FP16 = 2 };
+enum { B200TTS_PRECISION_FP32 = 0, B200TTS_PRECISION_BF16 = 1, B200TTS_PRECISION_FP16 = 2, B200TTS_PRECISION_TF32X3 = 3,
+       B200TTS_PRECISION_F16X3 = 4 };
 
 /* ---- one conv layer with the fused prologue / epilogue the engines use -------------------------
  * The building block every dense contraction of the path runs on; replaces one

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Decoder precision benchmark: the cfg2 batch of bench.py (32 utterances x 64 tokens, same model, tokens and noise)
-through Vits.inference with the decoder's tensor-core convs in fp32 (3xTF32, the default), bf16 and fp16.  Prints one
-JSON line.
+through Vits.inference with the decoder's tensor-core convs in fp32 (the split-fp16 default), bf16 and fp16 (add
+tf32x3 to --precisions for 3xTF32).  Prints one JSON line.
 
   python scripts/bench_precision.py [--steps K] [--precisions fp32,bf16,fp16]
 

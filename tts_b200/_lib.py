@@ -105,11 +105,12 @@ DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9:
                   11: "attn_fma"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
-PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2}
+PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}
 
 
 def precision_id(name):
-    """B200TTS_PRECISION_* of ``"fp32"`` / ``"bf16"`` / ``"fp16"``; ValueError for anything else."""
+    """B200TTS_PRECISION_* of ``"fp32"`` / ``"bf16"`` / ``"fp16"`` / ``"tf32x3"`` / ``"f16x3"``; ValueError for anything
+    else."""
     if not isinstance(name, str) or name not in PRECISIONS:
         raise ValueError(f"tts_b200: precision must be one of {sorted(PRECISIONS)}, got {name!r}")
     return PRECISIONS[name]

@@ -16,8 +16,9 @@ from . import _lib
 class FusedConv1d:
     """weight [Cout,Cin,K] (or [Cin,Cout,K] with ``transposed=True``), bias [Cout] or None -- host or device tensors;
     the packed device copy is created on first use per device.  ``precision`` "bf16" / "fp16" runs the tensor-core
-    kernels with 16-bit operands (fp32 accumulation; layers with Cin % 16 != 0 stay 3xTF32); "fp32" is the
-    ``tensor_cores`` setting as given.  ``padding_mode`` mirrors ``nn.Conv1d``'s: "zeros" (default) or "reflect"
+    kernels with 16-bit operands (fp32 accumulation; layers with Cin % 16 != 0 stay 3xTF32); "f16x3" with the split-fp16
+    product the HiFiGAN decoder uses by default (fp32-class accuracy for activations below 65504 in magnitude, same
+    Cin rule); "fp32" (3xTF32 on the tensor cores) and "tf32x3" are the ``tensor_cores`` setting as given.  ``padding_mode`` mirrors ``nn.Conv1d``'s: "zeros" (default) or "reflect"
     (``nn.ReflectionPad1d(padding)`` then an unpadded conv, read straight from x by the kernels: no padded copy; needs
     ``padding = dilation * (K - 1) / 2``, ``padding <= T - 1`` and a non-transposed conv)."""
 
@@ -33,7 +34,7 @@ class FusedConv1d:
                              f"got {padding_mode!r}")
         self.padding_mode = padding_mode
         if _lib.precision_id(precision) != 0 and not self.tensor_cores:
-            raise ValueError("tts_b200.FusedConv1d: a 16-bit precision needs tensor_cores=True")
+            raise ValueError("tts_b200.FusedConv1d: a precision other than fp32 needs tensor_cores=True")
         if transposed:
             self.cin, self.cout, self.k = self.weight.shape
         else:

@@ -32,7 +32,8 @@ struct b200tts_conv1d {
 };
 
 static bool valid_precision(int p) {
-    return p == B200TTS_PRECISION_FP32 || p == B200TTS_PRECISION_BF16 || p == B200TTS_PRECISION_FP16;
+    return p == B200TTS_PRECISION_FP32 || p == B200TTS_PRECISION_BF16 || p == B200TTS_PRECISION_FP16 ||
+           p == B200TTS_PRECISION_TF32X3 || p == B200TTS_PRECISION_F16X3;
 }
 
 static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* weight, const float* bias, int allow_tensor_cores,
@@ -52,7 +53,9 @@ static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* wei
     if (!h) { set_error("conv1d_create: out of host memory"); return 1; }
     h->c = *cfg;
     h->reflect = padding_mode == B200TTS_PAD_REFLECT;
-    h->L.tc_prec = allow_tensor_cores ? precision : TC_NONE;
+    // FP32 and TF32X3 are both the 3xTF32 images (ConvLayer::tc_prec never holds TF32X3)
+    const int lp = precision == B200TTS_PRECISION_TF32X3 ? B200TTS_PRECISION_FP32 : precision;
+    h->L.tc_prec = allow_tensor_cores ? lp : TC_NONE;
     int rc = cfg->transposed
                  ? pack_conv_transpose(h->L, weight, bias, cfg->in_channels, cfg->out_channels, cfg->kernel_size,
                                        cfg->stride, cfg->padding)

@@ -95,13 +95,15 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     int ups = 1;              // >1: polyphase ConvTranspose1d
     int co_tile = 64;         // 32 or 64
     int tr_kernel = 0, tr_pad = 0, tr_outpad = 0;  // original transposed-conv kernel size / padding / output_padding (Tout)
-    // tensor cores: set BEFORE packing to TC_NONE or the requested operand type (B200TTS_PRECISION_*); packing records the
-    // type of the images it built (a 16-bit request with Cin % 16 != 0 gets 3xTF32; no image: TC_NONE).  The text and
+    // tensor cores: set BEFORE packing to TC_NONE or the requested operand type (B200TTS_PRECISION_* other than TF32X3,
+    // which is FP32 here); packing records the
+    // type of the images it built (a 16-bit or split-fp16 request with Cin % 16 != 0 gets 3xTF32; no image: TC_NONE).  The text and
     // duration path requests none, so durations stay bit-stable on the exact FP32 FMA kernel.
     int tc_prec = TC_NONE;
     void* w_tc = nullptr;     // device, plain image: [128-row tile][chunk][tap] weight blocks (rows >= 32), see pack_tc
     void* w_tcg = nullptr;    // device, grouped image: [chunk][tap block] weight blocks (rows == 32 / 64), null: none
     int tc_grp = 0;           // tap groups of the grouped image (128 / rows), 0: none
+    float* tc_rscale = nullptr;   // device, [Rows] 2^-e_r of the split-fp16 images (tc_prec == PREC_F16X3), else null
 };
 
 struct ConvIO {

@@ -24,6 +24,9 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <algorithm>
+#include <cmath>
+
 namespace b200tts {
 
 // ------------------------------------------------------------------ error plumbing / counters
@@ -410,7 +413,8 @@ void free_conv(ConvLayer& L) {
     if (L.bias) cudaFree(L.bias);
     if (L.w_tc) cudaFree(L.w_tc);
     if (L.w_tcg) cudaFree(L.w_tcg);
-    L.w = L.bias = nullptr;
+    if (L.tc_rscale) cudaFree(L.tc_rscale);
+    L.w = L.bias = L.tc_rscale = nullptr;
     L.w_tc = L.w_tcg = nullptr;
 }
 
@@ -418,15 +422,31 @@ void free_conv(ConvLayer& L) {
 // loader copies with one cp.async.bulk, [slabs][128 MMA rows][16 B], slab s holding the chunk's channels s*SLC .. +SLC-1:
 //   3xTF32 (PREC_FP32): 8-channel chunks, {hi, lo}[2 slabs] of 4 floats, hi = v & 0xFFFFE000 (exact in TF32), lo = v - hi
 //   bf16 / fp16:        16-channel chunks, [2 slabs] of 8 values rounded to nearest even (as cvt.rn rounds the activations)
+//   PREC_F16X3:         16-channel chunks, {hi, lo, hs}[2 slabs] of 8 fp16 values of the scaled row w' = w * 2^e_r (e_r puts
+//                       the row's max |w'| in [2^14, 2^15); all-zero rows: e_r = 0): hi = fp16(w'), lo = fp16(w' - hi),
+//                       hs = hi * 2^-11 (exact unless it falls below fp16's normal range, 2^17 under the row's max); the
+//                       kernel's epilogue multiplies by rscale[r] = 2^-e_r, which the first call returns in *rscale
 // With G tap groups (1: plain; 128 / rows: grouped), MMA row m = g * (128 / G) + co of tile t carries weight row
 // t * 128 + co and, in tap block j, tap G * j + g.  Rows >= `rows`, taps >= K and channels >= Cin are zero.  The weight
 // norm is already folded (in fp32) into Wl; each weight is rounded once, here.
-static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G) {
-    const bool tf32 = prec == tc::PREC_FP32;
+static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G,
+                   float** rscale = nullptr) {
+    const bool tf32 = prec == tc::PREC_FP32, x3 = prec == tc::PREC_F16X3;
     const int kc = tf32 ? tc3::KC2 : tc3::KC16, slc = kc / 2, ch = tc3::MROWS / G;
     const int ntiles = (rows + tc3::MROWS - 1) / tc3::MROWS, nchunks = (Cin + kc - 1) / kc, J = (K + G - 1) / G;
-    const size_t slab = (size_t)tc3::MROWS * 16, blk = (tf32 ? 4 : 2) * slab;
+    const size_t slab = (size_t)tc3::MROWS * 16, blk = (tf32 ? 4 : x3 ? 6 : 2) * slab;
     std::vector<unsigned char> img((size_t)ntiles * nchunks * J * blk, 0);
+    std::vector<float> up(x3 ? rows : 0, 1.f), down(x3 ? rows : 0, 1.f);   // 2^e_r, 2^-e_r
+    for (int r = 0; r < (x3 ? rows : 0); ++r) {
+        float m = 0.f;
+        for (size_t i = (size_t)r * Cin * K; i < (size_t)(r + 1) * Cin * K; ++i) m = std::max(m, std::fabs(Wl[i]));
+        if (m == 0.f) continue;
+        int E;
+        std::frexp(m, &E);                                 // m in [2^(E-1), 2^E)
+        const int e = std::min(126, std::max(-126, 15 - E));
+        up[r] = std::ldexp(1.f, e);
+        down[r] = std::ldexp(1.f, -e);
+    }
     for (int t = 0; t < ntiles; ++t)
         for (int c = 0; c < nchunks; ++c)
             for (int j = 0; j < J; ++j)
@@ -447,6 +467,14 @@ static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, 
                             const float lo = v - hi;
                             memcpy(p + 4 * e, &hi, 4);
                             memcpy(p + 2 * slab + 4 * e, &lo, 4);
+                        } else if (x3) {
+                            const float ws = v * up[r];
+                            const __half hi = __float2half_rn(ws);
+                            const __half lo = __float2half_rn(ws - __half2float(hi));
+                            const __half hs = __float2half_rn(__half2float(hi) * (1.f / 2048.f));
+                            memcpy(p + 2 * e, &hi, 2);
+                            memcpy(p + 2 * slab + 2 * e, &lo, 2);
+                            memcpy(p + 4 * slab + 2 * e, &hs, 2);
                         } else if (prec == tc::PREC_BF16) {
                             const __nv_bfloat16 h = __float2bfloat16_rn(v);
                             memcpy(p + 2 * e, &h, 2);
@@ -459,6 +487,7 @@ static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, 
     unsigned char* d = nullptr;
     const int rc = upload(&d, img.data(), img.size());
     *dst = d;
+    if (rc == 0 && x3 && rscale && !*rscale) return upload(rscale, down.data(), down.size());
     return rc;
 }
 
@@ -489,9 +518,9 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     if (L.tc_prec != TC_NONE && Cin % tc3::KC16 != 0) L.tc_prec = tc::PREC_FP32;
     if (rows < 32 || Cin < tc3::KC2) L.tc_prec = TC_NONE;
     if (L.tc_prec == TC_NONE) return 0;
-    if (pack_tc(&L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1)) return 2;
+    if (pack_tc(&L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1, &L.tc_rscale)) return 2;
     if (L.ups == 1 && (rows == 32 || rows == 64)) {
-        if (pack_tc(&L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows)) return 2;
+        if (pack_tc(&L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows, &L.tc_rscale)) return 2;
         L.tc_grp = tc3::MROWS / rows;
     }
     return 0;
@@ -774,7 +803,7 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     if (int rc = device_once(g_tc_once, &dev, [](int d) -> int {
         int smem_optin = 0;
         B200_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
-        for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16}) {
+        for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16, tc::PREC_F16X3}) {
             for (bool lean : {true, false})
                 B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
             B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
@@ -783,9 +812,9 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
                     B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                       smem_optin));
         }
-        int* flag = nullptr;
-        B200_CUDA_OK(cudaHostAlloc((void**)&flag, sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
-        *flag = 0;
+        int* flag = nullptr;   // [0] pipeline timeout, [tc::ERR_RANGE] fp16 range (PREC_F16X3)
+        B200_CUDA_OK(cudaHostAlloc((void**)&flag, 2 * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
+        flag[0] = flag[tc::ERR_RANGE] = 0;
         g_tc_dev[d].err = flag;    // unified addressing: the host pointer is valid on the device
         g_tc_dev[d].max_smem = smem_optin;
         B200_CUDA_OK(cudaDeviceGetAttribute(&g_tc_dev[d].num_sms, cudaDevAttrMultiProcessorCount, d));
@@ -796,6 +825,13 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const size_t max_smem = (size_t)g_tc_dev[dev].max_smem;
     B200_REQUIRE(*reinterpret_cast<volatile int*>(g_tc_err) == 0,
                  "tensor-core conv: an earlier launch on device %d hit a pipeline timeout (its output is invalid)", dev);
+    // a range error is reported once, by the next launch: the data was out of range, the device state is fine
+    volatile int* const range_err = reinterpret_cast<volatile int*>(g_tc_err + tc::ERR_RANGE);
+    if (*range_err) {
+        *range_err = 0;
+        B200_REQUIRE(false, "tensor-core conv: an earlier split-fp16 launch on device %d read an activation with |x| >= 65504, "
+                            "outside fp16's range (its output is invalid; B200TTS_PRECISION_TF32X3 takes such models)", dev);
+    }
     // persistent kernels: 16-byte aligned activation rows for the cp.async staging, no input mask
     const bool aligned = ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.x_cs % 4 == 0) && (a.x_bs % 4 == 0);
     const bool persistent_ok = aligned && !a.xmask &&
@@ -812,7 +848,7 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     tc3::Tc3Args t;
     memset(&t, 0, sizeof(t));
     t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-    t.w = grouped ? L.w_tcg : L.w_tc; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
+    t.w = grouped ? L.w_tcg : L.w_tc; t.rscale = L.tc_rscale; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
     t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = tc3::MROWS;
     t.KJ = grouped ? J : L.K; t.dil_blk = grouped ? G * L.dil : L.dil; t.tstep = grouped ? tc3::TSTEP_GROUPED : tc3::TT2;
     t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
@@ -840,16 +876,23 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
     B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));
     count_launch();
-    const bool b16 = L.tc_prec != tc::PREC_FP32;
+    const bool b16 = L.tc_prec == tc::PREC_BF16 || L.tc_prec == tc::PREC_FP16;   // PREC_F16X3 logs as tc3
     dispatch_note(grouped ? (b16 ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED) : (b16 ? DISPATCH_TC16 : DISPATCH_TC3));
     B200_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
-int conv_tc_error_flag() {   // 1 if any tensor-core launch (on any device) hit a pipeline timeout; call after a sync
-    for (int d = 0; d < MAX_DEVICES; ++d)
-        if (g_tc_dev[d].err && *reinterpret_cast<volatile int*>(g_tc_dev[d].err)) return 1;
-    return 0;
+// 1 if any tensor-core launch (on any device) hit a pipeline timeout, 2 if one read an activation outside fp16's range
+// (PREC_F16X3), 3 for both; call after a sync
+int conv_tc_error_flag() {
+    int f = 0;
+    for (int d = 0; d < MAX_DEVICES; ++d) {
+        if (!g_tc_dev[d].err) continue;
+        const volatile int* e = g_tc_dev[d].err;
+        if (e[0]) f |= 1;
+        if (e[tc::ERR_RANGE]) f |= 2;
+    }
+    return f;
 }
 
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {

@@ -19,6 +19,14 @@
 // Opt-in 16-bit operands (bf16 or fp16, fp32 accumulation): no split, one m64n256k16 MMA per 16 input channels and tap.
 // A slab row is still 16 bytes, now holding 8 channels of one time step, so a k16 step is two slabs LBO apart and the
 // tap shift above still holds; activations are rounded (cvt.rn) on the way into shared memory, weights at pack time.
+//
+// 3-product fp16 split (PREC_F16X3, the HiFiGAN decoder's default): fp16 has TF32's 11-bit significand and twice its MMA
+// rate, so the same hi/lo split costs 3 m64n256k16 MMAs per 16 channels instead of 6 m64n256k8.  fp16's small range is
+// handled by scaling: weight row r is multiplied by 2^e_r (max |w'| in [2^14, 2^15)) at pack time and stored as W_hi =
+// fp16(w'), W_lo = fp16(w' - W_hi), W_hs = W_hi * 2^-11; activations are split as X_hi = fp16(x), X_lo = fp16((x - X_hi)
+// * 2^11) (subtraction and scaling exact).  D' = W_hs*X_lo + W_lo*X_hi + W_hi*X_hi = 2^e_r * D to 2^-22 relative, and the
+// epilogue multiplies row r by 2^-e_r (exact) before the bias.  |x| >= 65504 cannot be represented: the producers report
+// it (ERR_RANGE) instead of multiplying an inf.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,8 +34,13 @@
 namespace b200tts {
 namespace tc {
 
-// tensor-core operand type (the values of B200TTS_PRECISION_* in include/tts_b200.h)
-enum : int { PREC_FP32 = 0, PREC_BF16 = 1, PREC_FP16 = 2 };
+// tensor-core operand type (the values of B200TTS_PRECISION_* in include/tts_b200.h; 3 is the header's TF32X3, which
+// packs as PREC_FP32)
+enum : int { PREC_FP32 = 0, PREC_BF16 = 1, PREC_FP16 = 2, PREC_F16X3 = 4 };
+// the mapped error flags (conv1d.cu) are two words: err[0] a pipeline timeout, err[ERR_RANGE] an activation outside
+// fp16's range (|x| >= F16X3_MAX) in PREC_F16X3
+enum : int { ERR_RANGE = 1 };
+constexpr float F16X3_MAX = 65504.f;
 constexpr uint32_t SPIN_LIMIT = 1u << 22;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -142,6 +155,14 @@ __device__ __forceinline__ uint32_t cvt_f16x2(float lo, float hi) {
     uint32_t r;
     asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
+}
+// PREC_F16X3 activation split of two values (`a` at the lower address): hi = fp16(v), lo = fp16((v - hi) * 2^11).  v - hi is
+// exact in fp32 (it is below half an fp16 ulp of v) and so is the scaling, so lo carries the next 11 bits of v.
+__device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    hi = cvt_f16x2(a, b);
+    float ha, hb;
+    asm("{\n.reg .b16 l, h;\nmov.b32 {l, h}, %2;\ncvt.f32.f16 %0, l;\ncvt.f32.f16 %1, h;\n}" : "=f"(ha), "=f"(hb) : "r"(hi));
+    lo = cvt_f16x2((a - ha) * 2048.f, (b - hb) * 2048.f);
 }
 
 }  // namespace tc

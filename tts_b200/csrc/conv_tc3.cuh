@@ -17,6 +17,13 @@
 // consumers issue one m64n256k16 MMA per tap and chunk.  Epilogues, residuals and every tensor in global memory stay
 // fp32.  Shared memory: the raw ring doubles (+31 KB), the activation stages and weight slots halve (-20 KB, -12 KB).
 //
+// PREC = PREC_F16X3: the 3-product fp16 split (conv_tc.cuh).  A chunk is 16 input channels, but the raw ring keeps the
+// FP32 kernel's 8-channel stages: the producers fill one activation stage {X_hi[2 slabs], X_lo[2 slabs]} from two raw
+// stages, one slab of each per raw stage, and arrive on it after the second; they also report any |x| >= 65504
+// (err[ERR_RANGE]).  A weight tap block is three planes {W_hi, W_lo, W_hs}[2 slabs][128 rows][8] (12 KB) and the ring
+// holds NB3 of them, so shared memory is exactly the FP32 kernel's.  The consumers issue W_hs*X_lo, W_lo*X_hi, W_hi*X_hi
+// (m64n256k16 each) per tap and chunk; every epilogue multiplies its rows by `rscale` (2^-e_r) before the bias.
+//
 // Grouped mode (GRP = 2 / 4) for narrow layers (exactly 64 / 32 output rows, the last two HiFiGAN stages): the 128
 // MMA rows are GRP tap-groups x (128/GRP) channels -- row g * (128/GRP) + c carries the weights of channel c for taps
 // g, g+GRP, g+2*GRP, ... so one instruction stream of ceil(K/GRP) "tap blocks" (B shifted by GRP*dil rows per block)
@@ -43,6 +50,7 @@ constexpr int RAWS = 324;         // raw (cp.async) row stride in floats: the wi
 constexpr int NRAW = 3;           // raw (cp.async) ring depth
 constexpr int NA2 = 2;            // transformed activation stages
 constexpr int NB2 = 3;            // weight ring depth (one 8 KB tap block per slot)
+constexpr int NB3 = 2;            // PREC_F16X3 weight ring depth (one 12 KB tap block per slot)
 constexpr int ACC_LD = 260;       // row stride (floats) of the shared accumulator tile: float4 reads of 8 rows are conflict free
 constexpr int ACC_BYTES = MROWS * ACC_LD * 4;
 constexpr int NPW = 3;            // producer warps
@@ -54,7 +62,9 @@ constexpr int NTHREADS2 = 32 * (W_LOAD + 1);
 struct Tc3Args {
     const float* x; long long x_bs; int x_cs; int Tin;
     float in_slope;
-    const void* w;             // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32 (16-bit: [2][128][8])
+    const void* w;             // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32 (16-bit: [2][128][8];
+                               // PREC_F16X3: {hi, lo, hs}[2][128][8] fp16)
+    const float* rscale;       // PREC_F16X3: [Rows] 2^-e_r, the inverse of the pack-time row scaling (see pack_tc)
     const float* bias;
     const float* cond; long long cond_bs;
     int Cin, K, dil, pad, Rows, N;
@@ -90,10 +100,12 @@ struct Tc3Args {
     int q_lo, q_hi, in_lo, t_lo;
 };
 
-// prec: PREC_FP32 (8-channel chunks, hi/lo slab pairs) or a 16-bit type (16-channel chunks, two slabs)
+// prec: PREC_FP32 (8-channel chunks, hi/lo slab pairs), a 16-bit type (16-channel chunks, two slabs) or PREC_F16X3
+// (16-channel chunks over 8-channel raw stages, hi/lo slab pairs, three-plane weight blocks: the FP32 kernel's total)
 static inline size_t smem_bytes3(int rows_pad, int prec = PREC_FP32) {
-    const size_t kch = prec ? KC16 : KC2, nsl = prec ? 2 : 4;
-    return (size_t)NRAW * kch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + (size_t)NB2 * (nsl * MROWS * 16) + ACC_BYTES + 512;
+    const bool b16 = prec == PREC_BF16 || prec == PREC_FP16, x3 = prec == PREC_F16X3;
+    const size_t raw_ch = b16 ? KC16 : KC2, nsl = b16 ? 2 : 4, wsl = x3 ? 6 : nsl, nb = x3 ? NB3 : NB2;
+    return (size_t)NRAW * raw_ch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + nb * (wsl * MROWS * 16) + ACC_BYTES + 512;
 }
 static inline size_t ragged_table_bytes(int B) { return ((size_t)(B + 1) * sizeof(int) + 15) / 16 * 16; }
 
@@ -123,14 +135,16 @@ constexpr int TSTEP_GROUPED = 240;   // 15 chunks of 16 columns: leaves room for
 // contiguous bytes; padding rows (>= Rows) have their loads clamped to the last real row and their stores switched off.
 // HR / HA are compile-time so that every load is an unconditional definition; the residual of the next 16-column group
 // is in flight while the current one is finished.  ((acc + bias) + res) + old, as in the general code.
-template <bool HR, bool HA>
-__device__ __forceinline__ void lean_tile(const float* at, const float* bias, const float* cond, int lane, const float* rq,
-                                          float* yq, long long rcs, long long ycs, int row0, int Rows, bool do_st) {
+// SC (PREC_F16X3): acc is first multiplied by the row's rscale (a power of two: exact).
+template <bool HR, bool HA, bool SC>
+__device__ __forceinline__ void lean_tile(const float* at, const float* bias, const float* rscale, const float* cond, int lane,
+                                          const float* rq, float* yq, long long rcs, long long ycs, int row0, int Rows,
+                                          bool do_st) {
     const int r8 = lane & 7, p4 = lane >> 3;
     const float* rrow[4];
     float* yrow[4];
     bool st_ok[4];
-    float bv[4];
+    float bv[4], sv[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int ri = row0 + 8 * i + r8, rci = ri < Rows ? ri : Rows - 1;
@@ -139,6 +153,7 @@ __device__ __forceinline__ void lean_tile(const float* at, const float* bias, co
         st_ok[i] = do_st && ri < Rows;
         bv[i] = bias[rci];
         if (cond) bv[i] += __ldg(cond + rci);
+        sv[i] = SC ? rscale[rci] : 1.f;
     }
     const float* ap = at + r8 * ACC_LD + 4 * p4;
     float r0[16], r1[16];
@@ -160,6 +175,7 @@ __device__ __forceinline__ void lean_tile(const float* at, const float* bias, co
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             float4 t = *reinterpret_cast<const float4*>(ap + 8 * i * ACC_LD + cg);
+            if constexpr (SC) { t.x *= sv[i]; t.y *= sv[i]; t.z *= sv[i]; t.w *= sv[i]; }
             t.x += bv[i]; t.y += bv[i]; t.z += bv[i]; t.w += bv[i];
             if constexpr (HR) { t.x += rv[4 * i]; t.y += rv[4 * i + 1]; t.z += rv[4 * i + 2]; t.w += rv[4 * i + 3]; }
             if constexpr (HA) { t.x += o[4 * i]; t.y += o[4 * i + 1]; t.z += o[4 * i + 2]; t.w += o[4 * i + 3]; }
@@ -176,6 +192,8 @@ __device__ __forceinline__ void lean_tile(const float* at, const float* bias, co
 
 // Everything the lean epilogue does not cover (WaveNet gate / res-skip split, masks, ReLU, scale, final divide, polyphase
 // stores of the transposed convs, edge tiles): one tile half per call, lane = one output row, `arow` = its accumulators.
+// SC: the accumulators are scaled by the row's rscale first (PREC_F16X3).
+template <bool SC>
 __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float* arow, int b, int rt, int q0, int lq, int half,
                                                   int lane) {
     const int ups = a.ups;
@@ -185,6 +203,14 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
     const int qb = q0 + half * 128;
     float bias = a.bias[rc];
     if (a.cond) bias += __ldg(a.cond + (long long)b * a.cond_bs + rc);
+    const float rs = SC ? a.rscale[rc] : 1.f;
+    auto acc_ld = [&](const float* p, float* v) {
+        acc_ld16(p, v);
+        if constexpr (SC) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) v[i] *= rs;
+        }
+    };
     if (a.gate) {
         // WaveNet gate (wavenet.py:6-13): even lane = tanh argument, odd lane = sigmoid argument of row r/2
         float* yrow = a.y + (long long)b * a.y_bs + (long long)(rc >> 1) * a.y_cs;
@@ -192,7 +218,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
         const bool even = (lane & 1) == 0;
         for (int cg = 0; cg < 128; cg += 16) {
             float v[16];
-            acc_ld16(arow + cg, v);
+            acc_ld(arow + cg, v);
             const int q = qb + cg;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -250,7 +276,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
         auto group = [&](int cg, const float* rv, const float* ov, float* rn, float* on) {
             float v[16];
             if (rok && cg + 16 < 128) prefetch(cg + 16, rn, on);
-            acc_ld16(arow + cg, v);
+            acc_ld(arow + cg, v);
             const int q = qb + cg;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -292,7 +318,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
         float* yrow = a.y + (long long)b * a.y_bs + (long long)co * a.y_cs + ph;
         for (int cg = 0; cg < 128; cg += 16) {
             float v[16];
-            acc_ld16(arow + cg, v);
+            acc_ld(arow + cg, v);
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
                 const int q = qb + cg + i;
@@ -308,16 +334,18 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 // Out-of-line call of the general epilogue for the kernel whose hot path is the lean one (edge tiles only): inlined into
 // its tile loop the general code's loop invariants were hoisted across the lean path.  One copy of the arguments per
 // call: through the reference every field use would be a generic load.
+template <bool SC>
 __device__ __noinline__ void general_tile_call(const Tc3Args& a_ref, const float* arow, int b, int rt, int q0, int lq, int half,
                                                int lane) {
     const Tc3Args a = a_ref;
-    general_tile_body(a, arow, b, rt, q0, lq, half, lane);
+    general_tile_body<SC>(a, arow, b, rt, q0, lq, half, lane);
 }
 
 // Grouped epilogue, one tile half: out[c, t] = sum_g D_g[c, t + g*dil] with MMA row m = g * CH + c (CH = 128 / GRP
 // channels).  Thread tq of the half's 128 finishes channel co = tq * NQ / 4, float4s j0 .. j0 + NQ - 1 of every
-// 16-column group (4 / NQ lanes = 64 contiguous bytes of a channel).
-template <int GRP>
+// 16-column group (4 / NQ lanes = 64 contiguous bytes of a channel).  SC: the GRP partials of a channel share its rscale,
+// applied to their sum (PREC_F16X3).
+template <int GRP, bool SC>
 __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs, int b, int q0, int lq, int half, int lane) {
     constexpr int CH = 128 / GRP;              // output channels
     constexpr int NQ = CH / 32;                // float4 per thread and 16-column group (1 or 2)
@@ -335,6 +363,7 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     float* yrow = a.y + (long long)b * a.y_bs + (long long)co * a.y_cs;
     float bias = a.bias[co];
     if (a.cond) bias += __ldg(a.cond + (long long)b * a.cond_bs + co);
+    const float rs = SC ? a.rscale[co] : 1.f;
     auto load = [&](const float* rr, int q, float* dst) {     // one thread's values of a column group of a row
 #pragma unroll
         for (int j = 0; j < NQ; ++j) {
@@ -359,6 +388,7 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
             const float p0 = p[i], p1 = p[CH * ACC_LD + a.dil + i];
             float s = p0 + p1;
             if constexpr (GRP == 4) s += p[2 * CH * ACC_LD + 2 * a.dil + i] + p[3 * CH * ACC_LD + 3 * a.dil + i];
+            if constexpr (SC) s *= rs;
             R[i] = s;
         }
 #pragma unroll
@@ -394,20 +424,27 @@ template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false>
                                        // that the zero-padding kernels keep their register allocation.
 __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     extern __shared__ __align__(128) unsigned char smem[];
-    constexpr int KCH = PREC ? KC16 : KC2;       // input channels per chunk
-    constexpr int NSL = PREC ? 2 : 4;            // 16-byte slabs per operand stage: two 16-bit slabs, or hi[2] + lo[2]
-    constexpr int SLC = PREC ? 8 : 4;            // channels per slab row
+    constexpr bool X3 = PREC == PREC_F16X3;      // 3-product fp16 split
+    constexpr bool B16 = PREC == PREC_BF16 || PREC == PREC_FP16;
+    constexpr int KCH = PREC != PREC_FP32 ? KC16 : KC2;   // input channels per chunk
+    constexpr int RCH = B16 ? KC16 : KC2;        // input channels per raw ring stage
+    constexpr int SPC = KCH / RCH;               // raw stages per chunk (2 for X3)
+    constexpr int NSL = B16 ? 2 : 4;             // 16-byte slabs per activation stage: two 16-bit slabs, or hi[2] + lo[2]
+    constexpr int SLC = PREC != PREC_FP32 ? 8 : 4;   // channels per slab row
+    constexpr int NWS = X3 ? 6 : NSL;            // slabs per weight tap block (X3: hi[2], lo[2], hs[2])
+    constexpr int NB = X3 ? NB3 : NB2;           // weight ring depth
+    constexpr bool SC = X3;                      // epilogues scale rows by rscale
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ROWS = a.rows_pad, RAWW = a.raw_w, K = a.KJ;
-    const uint32_t rawStage = (uint32_t)KCH * RAWS * 4;
+    const uint32_t rawStage = (uint32_t)RCH * RAWS * 4;
     const uint32_t slabA = (uint32_t)ROWS * 16, stageA = NSL * slabA;
-    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NSL * slabB;   // one tap block: [NSL slabs][128 rows][16 B]
+    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NWS * slabB;   // one tap block: [NWS slabs][128 rows][16 B]
     unsigned char* smRaw = smem;
     unsigned char* smA = smRaw + NRAW * rawStage;
     unsigned char* smB = smA + NA2 * stageA;
-    float* accs = reinterpret_cast<float*>(smB + NB2 * stageB);
+    float* accs = reinterpret_cast<float*>(smB + NB * stageB);
     uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(accs) + ACC_BYTES);
-    const int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB2;
+    const int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB;
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
 
@@ -442,7 +479,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
 
     if (tid == 0) {
         for (int i = 0; i < NA2; ++i) { mbar_init(BAR(A_FULL + i), NPW); mbar_init(BAR(A_EMPTY + i), NCONS / 32); }
-        for (int i = 0; i < NB2; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), NCONS / 32); }
+        for (int i = 0; i < NB; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), NCONS / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -477,7 +514,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     if (warp >= W_PROD && warp < W_PROD + NPW) {
         // ============================================================ producers
         const int ptid = tid - 32 * W_PROD;
-        const int total = my_tiles * nchunks;
+        const int total = my_tiles * nchunks * SPC;                      // raw stages to fill and transform
         const int vec_per_row = RAWW / 4;
         const int nvec = KC2 * vec_per_row;
         const float slope = a.in_slope;
@@ -488,7 +525,8 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         // Per-thread work items are decoded ONCE (no divisions in the loop), the raw row stride is a compile-time constant
         // (shared loads take immediate offsets), interior windows take a copy path without any bounds logic, and leaky
         // ReLU is max(x, slope * x).
-        constexpr int MAXV = (8 * 81 + NPROD - 1) / NPROD, MAXI = (2 * 320 + NPROD - 1) / NPROD;   // raw vectors / slab rows per thread
+        constexpr int NIT = X3 ? 1 : 2;                 // slabs written per raw stage (X3: X_hi and X_lo of one slab)
+        constexpr int MAXV = (8 * 81 + NPROD - 1) / NPROD, MAXI = (NIT * 320 + NPROD - 1) / NPROD;   // raw vectors / slab rows per thread
         int v_ch[MAXV], v_t[MAXV], v_src[MAXV];    // channel in chunk (-1: none), time offset from `tal`, global float offset
         uint32_t v_dst[MAXV];                      // byte offset in a raw stage
 #pragma unroll
@@ -505,17 +543,19 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         for (int e = 0; e < MAXI; ++e) {
             const int idx = ptid + e * NPROD;
             const int sl = idx / ROWS, r = idx - sl * ROWS;
-            i_raw[e] = (idx < 2 * ROWS) ? (SLC * sl) * RAWS + r : -1;
+            i_raw[e] = (idx < NIT * ROWS) ? (SLC * sl) * RAWS + r : -1;
             i_dst[e] = (int)(sl * slabA) + r * 16;
         }
         // running positions instead of divisions / modulos per chunk
-        int iss_it = 0, iss_c = 0, iss_ring = 0, iss_tal = 0, iss_Tin = 0;             // cp.async front: tile, chunk, raw slot
+        int iss_it = 0, iss_c = 0, iss_h = 0, iss_ring = 0, iss_tal = 0, iss_Tin = 0;  // cp.async front: tile, chunk, raw stage of
+                                                                                        // the chunk, raw slot
         const float* iss_row = xg;
         bool iss_new = true, iss_int = false;
-        int tr_it = 0, tr_c = 0, tr_ring = 0, tr_q0 = 0, as = 0;                       // transform: tile, chunk, raw slot, A stage
+        int tr_it = 0, tr_c = 0, tr_h = 0, tr_ring = 0, tr_q0 = 0, as = 0;             // transform: the same, A stage
         uint32_t pa_empty = 1;                                    // parity to wait for on A_EMPTY[as]: round 1 -> 0, round 2 -> 1, ...
         bool tr_new = true;
         const uint32_t raw_u32 = smem_u32(smRaw);
+        float amax = 0.f;                                         // X3: largest |activation| this thread split
         auto issue = [&](int g) {
             if (g < total) {
                 if (iss_new) {
@@ -527,12 +567,13 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     iss_int = iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
                     iss_new = false;
                 }
-                // a chunk is KCH / 8 slots of 8 channels (one for FP32): the per-thread work items cover one slot
+                // a raw stage is RCH / 8 slots of 8 channels (two for BF16 / FP16): the per-thread work items cover one slot
+                const int ch0 = iss_c * KCH + iss_h * RCH;
 #pragma unroll
-                for (int h = 0; h < KCH / KC2; ++h) {
+                for (int h = 0; h < RCH / KC2; ++h) {
                     const uint32_t dst0 = raw_u32 + (uint32_t)iss_ring * rawStage + (uint32_t)(h * KC2 * RAWS * 4);
                     if (iss_int) {                                             // whole window inside the row: plain 16-byte copies
-                        const float* src = iss_row + (long long)(iss_c * KCH + h * KC2) * x_cs + iss_tal;
+                        const float* src = iss_row + (long long)(ch0 + h * KC2) * x_cs + iss_tal;
 #pragma unroll
                         for (int e = 0; e < MAXV; ++e)
                             if (v_ch[e] >= 0) cp_async16(dst0 + v_dst[e], src + v_src[e]);
@@ -541,7 +582,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                         for (int e = 0; e < MAXV; ++e) {
                             if (v_ch[e] < 0) continue;
                             const int t = iss_tal + v_t[e];
-                            const int cg = iss_c * KCH + h * KC2 + v_ch[e];
+                            const int cg = ch0 + h * KC2 + v_ch[e];
                             if (REFL && (t < 0 || t + 4 > iss_Tin)) {
                                 // edge vector of a reflect-padded conv (vectors inside the row keep the 16-byte copy): four
                                 // mirrored 4-byte copies, each from inside the row or zero-filled where the mirror leaves
@@ -566,7 +607,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                         }
                     }
                 }
-                if (++iss_c == nchunks) { iss_c = 0; ++iss_it; iss_new = true; }
+                if (++iss_h == SPC) { iss_h = 0; if (++iss_c == nchunks) { iss_c = 0; ++iss_it; iss_new = true; } }
             }
             if (++iss_ring == NRAW) iss_ring = 0;
             asm volatile("cp.async.commit_group;" ::: "memory");
@@ -576,7 +617,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             asm volatile("cp.async.wait_group %0;" ::"n"(NRAW - 2) : "memory");
             named_bar_sync(1, NPROD);                                     // everyone's copies of chunk g have landed
             issue(g + NRAW - 1);                                          // refills the stage transformed last iteration
-            if (g >= NA2) ok = mbar_wait(BAR(A_EMPTY + as), pa_empty, a.err);
+            if (tr_h == 0 && g >= NA2 * SPC) ok = mbar_wait(BAR(A_EMPTY + as), pa_empty, a.err);
             if (!ok) break;
             if (tr_new) {
                 int b_, rt_;
@@ -593,7 +634,22 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
 #pragma unroll
                 for (int i = 0; i < SLC; ++i) u[e][i] = rp[i * RAWS];
             }
-            if constexpr (PREC != PREC_FP32) {
+            if constexpr (X3) {
+#pragma unroll
+                for (int e = 0; e < MAXI; ++e) {       // ... then prologue, fp16 hi/lo split of 8 channels, two 16-byte stores
+                    if (i_raw[e] < 0) continue;
+                    uint32_t ph[4], pl[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const float w0 = fmaxf(u[e][2 * i], u[e][2 * i] * slope);
+                        const float w1 = fmaxf(u[e][2 * i + 1], u[e][2 * i + 1] * slope);
+                        amax = fmaxf(amax, fmaxf(fabsf(w0), fabsf(w1)));
+                        split_f16x2(w0, w1, ph[i], pl[i]);
+                    }
+                    *reinterpret_cast<uint4*>(base + tr_h * slabA + i_dst[e]) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
+                    *reinterpret_cast<uint4*>(base + (2 + tr_h) * slabA + i_dst[e]) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+                }
+            } else if constexpr (B16) {
 #pragma unroll
                 for (int e = 0; e < MAXI; ++e) {       // ... then prologue, rounding to 8 x 16 bits and one 16-byte store
                     if (i_raw[e] < 0) continue;
@@ -623,19 +679,23 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     *reinterpret_cast<float4*>(base + 2 * slabA + i_dst[e]) = lo;
                 }
             }
+            if (++tr_ring == NRAW) tr_ring = 0;
+            if (++tr_h < SPC) continue;                          // X3: the stage's second half comes from the next raw stage
+            tr_h = 0;
             fence_async_smem();                                  // generic-proxy stores -> visible to wgmma (async proxy)
             __syncwarp();
             if (lane == 0) mbar_arrive(BAR(A_FULL + as));       // one arrival per producer warp
             if (++tr_c == nchunks) { tr_c = 0; ++tr_it; tr_new = true; }
-            if (++tr_ring == NRAW) tr_ring = 0;
             if (++as == NA2) { as = 0; pa_empty ^= 1u; }
         }
         asm volatile("cp.async.wait_group 0;" ::: "memory");
+        // X3: an activation fp16 cannot hold (|x| >= 65504) was split into an inf -- the launch's output is invalid
+        if (X3 && amax >= F16X3_MAX && a.err) { *reinterpret_cast<volatile int*>(a.err + ERR_RANGE) = 1; __threadfence_system(); }
     } else if (warp == W_LOAD) {
         // ============================================================ weight loader
-        // One lane per ring slot: lane s owns slot s and feeds it with tap blocks s, s + NB2, s + 2*NB2, ... of this CTA's
-        // block sequence, so NB2 independent wait -> expect_tx -> bulk-copy chains are in flight.
-        if (lane < NB2) {
+        // One lane per ring slot: lane s owns slot s and feeds it with tap blocks s, s + NB, s + 2*NB, ... of this CTA's
+        // block sequence, so NB independent wait -> expect_tx -> bulk-copy chains are in flight.
+        if (lane < NB) {
             const int total = nchunks * K;                                 // tap blocks per tile (contiguous in memory)
             const long long all = (long long)my_tiles * total;
             const uint32_t full = BAR(B_FULL + lane), empty = BAR(B_EMPTY + lane);
@@ -646,7 +706,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             const unsigned char* wsrc = nullptr;
             uint32_t par = 1;                                              // parity of B_EMPTY to wait for: round 1 -> 0, 2 -> 1
             bool ok = true, first = true;
-            for (long long gi = lane; gi < all && ok; gi += NB2) {
+            for (long long gi = lane; gi < all && ok; gi += NB) {
                 if (it != cur_it) {
                     int b_, rt, q0_;
                     decode(it, b_, rt, q0_);
@@ -658,7 +718,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 bulk_g2s(dst, wsrc + (size_t)j * stageB, stageB, full);
                 first = false;
                 par ^= 1u;
-                j += NB2;
+                j += NB;
                 while (j >= total) { j -= total; ++it; }
             }
         }
@@ -670,6 +730,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         const int wg = warp >> 2, lq = warp & 3, half = warp >> 2;
         const uint64_t wdesc0 = make_desc(smem_u32(smB) + (uint32_t)wg * 64 * 16, slabB);   // this warpgroup's 64 weight rows
         const uint64_t wlo_off = (uint64_t)((2 * slabB) >> 4), wslot = (uint64_t)(stageB >> 4);
+        const uint64_t whs_off = (uint64_t)((4 * slabB) >> 4);                             // X3: the W_hs plane
         const uint64_t xstep = (uint64_t)a.dil_blk;                                          // B rows per tap block (16 B each)
         bool ok = true;
         int sa = 0; uint32_t pa = 0;                                                         // activation stage / its parity
@@ -707,6 +768,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                             wgmma_bf16_m64n256(d, w_hi, xh, acc);
                         } else if constexpr (PREC == PREC_FP16) {
                             wgmma_f16_m64n256(d, w_hi, xh, acc);
+                        } else if constexpr (X3) {
+                            wgmma_f16_m64n256(d, w_hi + whs_off, xl, acc);      // small terms first
+                            wgmma_f16_m64n256(d, w_lo, xh, 1u);
+                            wgmma_f16_m64n256(d, w_hi, xh, 1u);
                         } else {
                             wgmma_tf32_m64n256(d, w_hi, xl, acc);               // small terms first
                             wgmma_tf32_m64n256(d, w_lo, xh, 1u);
@@ -720,7 +785,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     rel_a = (k == K - 1) ? sa : -1;
                     acc = 1u;
                     xh += xstep; xl += xstep;
-                    if (++sb == NB2) { sb = 0; pb ^= 1u; }
+                    if (++sb == NB) { sb = 0; pb ^= 1u; }
                 }
                 if (++sa == NA2) { sa = 0; pa ^= 1u; }
             }
@@ -737,7 +802,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             int b, rt, q0;
             decode(it, b, rt, q0);
             if constexpr (GRP > 1) {
-                grouped_tile<GRP>(a, accs, b, q0, lq, half, lane);
+                grouped_tile<GRP, SC>(a, accs, b, q0, lq, half, lane);
             } else {
                 const int qb = q0 + half * 128;
                 const float* at = accs + lq * 32 * ACC_LD + half * 128;            // this warp's 32 rows x 128 columns
@@ -752,21 +817,21 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     float* yq = a.y + (long long)b * a.y_bs + qb;
                     const bool hres = a.res != nullptr, hacc = a.accum != 0;
                     const float* rq = hres ? a.res + (long long)b * a.res_bs + qb : yq;
-                    if (hres) { if (hacc) lean_tile<true, true>(at, a.bias, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true);
-                                else lean_tile<true, false>(at, a.bias, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true); }
-                    else { if (hacc) lean_tile<false, true>(at, a.bias, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true);
-                           else lean_tile<false, false>(at, a.bias, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true); }
+                    if (hres) { if (hacc) lean_tile<true, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true);
+                                else lean_tile<true, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true); }
+                    else { if (hacc) lean_tile<false, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true);
+                           else lean_tile<false, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true); }
                 } else if constexpr (LEAN) {
-                    general_tile_call(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
+                    general_tile_call<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 } else {
-                    general_tile_body(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
+                    general_tile_body<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 }
             }
         }
     }
 }
 
-// PREC: PREC_FP32 (3xTF32), PREC_BF16 or PREC_FP16
+// PREC: PREC_FP32 (3xTF32), PREC_BF16, PREC_FP16 or PREC_F16X3
 template <int PREC, bool REFL = false>
 __global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3_kernel(const __grid_constant__ Tc3Args a) { tc3_body<1, true, PREC, REFL>(a); }
 template <int PREC>   // gate / split / mask / polyphase
@@ -781,10 +846,12 @@ static inline Tc3Kernel plain_kernel(int prec, bool lean, bool reflect = false) 
     if (reflect) {
         if (prec == PREC_BF16) return conv1d_tc3_kernel<PREC_BF16, true>;
         if (prec == PREC_FP16) return conv1d_tc3_kernel<PREC_FP16, true>;
+        if (prec == PREC_F16X3) return conv1d_tc3_kernel<PREC_F16X3, true>;
         return conv1d_tc3_kernel<PREC_FP32, true>;
     }
     if (prec == PREC_BF16) return lean ? conv1d_tc3_kernel<PREC_BF16> : conv1d_tc3x_kernel<PREC_BF16>;
     if (prec == PREC_FP16) return lean ? conv1d_tc3_kernel<PREC_FP16> : conv1d_tc3x_kernel<PREC_FP16>;
+    if (prec == PREC_F16X3) return lean ? conv1d_tc3_kernel<PREC_F16X3> : conv1d_tc3x_kernel<PREC_F16X3>;
     return lean ? conv1d_tc3_kernel<PREC_FP32> : conv1d_tc3x_kernel<PREC_FP32>;
 }
 // grouped kernel for 2 / 4 tap groups (any dilation with (GRP - 1) * dil <= 15)
@@ -792,6 +859,7 @@ template <bool REFL>
 static inline Tc3Kernel grouped_kernel_t(int grp, int prec) {
     if (prec == PREC_BF16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_BF16, REFL> : conv1d_tc3g_kernel<4, PREC_BF16, REFL>;
     if (prec == PREC_FP16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP16, REFL> : conv1d_tc3g_kernel<4, PREC_FP16, REFL>;
+    if (prec == PREC_F16X3) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_F16X3, REFL> : conv1d_tc3g_kernel<4, PREC_F16X3, REFL>;
     return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP32, REFL> : conv1d_tc3g_kernel<4, PREC_FP32, REFL>;
 }
 static inline Tc3Kernel grouped_kernel(int grp, int prec = PREC_FP32, bool reflect = false) {

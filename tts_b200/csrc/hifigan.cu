@@ -16,13 +16,19 @@ Hifigan::~Hifigan() {
 
 // weights: host pointers, canonical order (see include/tts_b200.h).  precision (B200TTS_PRECISION_*): the tensor-core
 // operand type of conv_pre, the upsamplers and every resblock conv -- the layers that run on the wgmma kernels (~97% of
-// the FLOPs); cond and conv_post stay fp32, and so does every margin, workspace size and launch window.
+// the FLOPs); cond and conv_post stay fp32, and so does every margin, workspace size and launch window.  FP32 runs
+// them as the split-fp16 product (F16X3: 3 fp16 MMAs where 3xTF32 needs 6 tf32 ones, same operand accuracy);
+// TF32X3 keeps 3xTF32 for models whose activations leave fp16's range.
 int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int nw, int precision) {
     c = cfg;
     B200_REQUIRE(precision == B200TTS_PRECISION_FP32 || precision == B200TTS_PRECISION_BF16 ||
-                     precision == B200TTS_PRECISION_FP16,
+                     precision == B200TTS_PRECISION_FP16 || precision == B200TTS_PRECISION_TF32X3 ||
+                     precision == B200TTS_PRECISION_F16X3,
                  "hifigan: unknown precision %d", precision);
     prec = precision;
+    const int lp = precision == B200TTS_PRECISION_FP32     ? B200TTS_PRECISION_F16X3
+                   : precision == B200TTS_PRECISION_TF32X3 ? B200TTS_PRECISION_FP32
+                                                           : precision;   // ConvLayer::tc_prec of the layers above
     B200_REQUIRE(c.num_upsamples >= 1 && c.num_upsamples <= 8 && c.num_kernels >= 1 && c.num_kernels <= 8 &&
                      c.num_dilations >= 1 && c.num_dilations <= 8,
                  "hifigan: unsupported config");
@@ -31,7 +37,7 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
                        c.num_upsamples * c.num_kernels * c.num_dilations * (type1 ? 4 : 2) + 2;
     B200_REQUIRE(nw == expect, "hifigan: expected %d weight tensors, got %d", expect, nw);
     int i = 0;
-    conv_pre.tc_prec = prec;
+    conv_pre.tc_prec = lp;
     int rc = pack_conv(conv_pre, w[i], w[i + 1], c.upsample_initial_channel, c.in_channels, 7, 1, 3);
     if (rc) return rc;
     i += 2;
@@ -46,7 +52,7 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
     int ch = c.upsample_initial_channel;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int u = c.upsample_factors[s], k = c.upsample_kernel_sizes[s];
-        ups[s].tc_prec = prec;
+        ups[s].tc_prec = lp;
         rc = pack_conv_transpose(ups[s], w[i], w[i + 1], ch, ch / 2, k, u, (k - u) / 2);
         if (rc) return rc;
         i += 2;
@@ -59,12 +65,12 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
             if (type1) v2.resize(c.num_dilations);
             for (int n = 0; n < c.num_dilations; ++n) {
                 const int d = c.resblock_dilations[j][n];
-                v1[n].tc_prec = prec;
+                v1[n].tc_prec = lp;
                 rc = pack_conv(v1[n], w[i], w[i + 1], ch, ch, rk, d, (rk * d - d) / 2);
                 if (rc) return rc;
                 i += 2;
                 if (type1) {
-                    v2[n].tc_prec = prec;
+                    v2[n].tc_prec = lp;
                     rc = pack_conv(v2[n], w[i], w[i + 1], ch, ch, rk, 1, (rk - 1) / 2);
                     if (rc) return rc;
                     i += 2;

@@ -6,9 +6,11 @@ containers -- weight-norm parametrizations included -- so reference checkpoints 
 same ``forward(x, g=None)`` / ``inference(c)`` / ``remove_weight_norm()`` / ``load_checkpoint``.
 The arithmetic runs in libtts_b200.so (b200tts_hifigan_forward); there is no PyTorch fallback.
 
-``precision`` ("fp32" default, "bf16", "fp16") selects the operand type of the tensor-core convs (conv_pre, the
-upsamplers, every resblock conv): the 16-bit modes round activations and weights before each multiply and keep fp32
-accumulators and tensors, trading accuracy for speed (include/tts_b200.h, B200TTS_PRECISION_*).
+``precision`` ("fp32" default, "tf32x3", "bf16", "fp16") selects the operand type of the tensor-core convs (conv_pre,
+the upsamplers, every resblock conv).  "fp32" runs them as a split-fp16 product (hi/lo fp16 operands, 3 MMAs, fp32-class
+accuracy while activations stay below 65504 in magnitude -- a larger one is reported as an error); "tf32x3" keeps the
+3xTF32 split over fp32's whole range.  The 16-bit modes round activations and weights before each multiply and keep
+fp32 accumulators and tensors, trading accuracy for speed (include/tts_b200.h, B200TTS_PRECISION_*).
 """
 import ctypes
 
@@ -128,7 +130,8 @@ class HifiganGenerator(nn.Module):
 
     @property
     def precision(self):
-        """Operand precision of the decoder's tensor-core convs: "fp32" (3xTF32, the default), "bf16" or "fp16".
+        """Operand precision of the decoder's tensor-core convs: "fp32" (split fp16, the default), "tf32x3", "bf16" or
+        "fp16" ("f16x3" is the same arithmetic as "fp32").
         Setting it drops the packed weights; the next call packs them for the new precision."""
         return self._precision
 
