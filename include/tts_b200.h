@@ -40,7 +40,9 @@ int b200tts_debug_tc_error(void);
 
 /* Debug / test aids: record, on the calling thread, which kernel family every conv launch dispatched to.
  * ids: 0 FP32-FMA tile kernel, 3 tensor-core kernel (M = rows), 5 tensor-core kernel grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel,
- *      8 / 9 the tensor-core kernels 3 / 5 with 16-bit (bf16 / fp16) operands. */
+ *      8 / 9 the tensor-core kernels 3 / 5 with 16-bit (bf16 / fp16) operands; the WaveGrad variants (the WaveGrad
+ *      epilogue or a nearest-resampled input): 12 / 14 tensor cores with 3xTF32 / split-fp16 operands, 16 the FMA tile
+ *      kernel, each + 1 with a resampled input. */
 void b200tts_debug_dispatch_begin(void);
 int b200tts_debug_dispatch_end(int32_t* ids, int cap); /* returns the number of launches recorded */
 
@@ -98,6 +100,18 @@ int b200tts_conv1d_create_padded(const b200tts_conv1d_config* cfg, const float* 
 int b200tts_conv1d_forward_strided(const b200tts_conv1d* h, const float* x, long long x_batch_stride, int x_channel_stride,
                                    int B, int T, float in_slope, const float* residual, float scale, int accumulate,
                                    float post_div, int tanh, float* y, uint32_t* peak_bits, void* stream);
+
+/* one conv with the WaveGrad variants (the layers of b200tts_wavegrad_*, one at a time): the input is read through
+ * nearest resampling when near_src > 0 (x holds near_src columns, the conv sees T; 0: x holds T columns), then
+ *   v = acc + bias; [lrelu(v, 0.2)] (lrelu != 0); [+ act_add[b]] (device [B], nullable); [+ residual[b, c, t]] (nullable,
+ *   any strides, batch stride 0 broadcasts); [y2 <- v] (nullable, y's strides); [v = film[b, c, t] + film[b, film_half + c,
+ *   t] * v] (film nullable); y <- v.
+ * y [B, out, out_len(T)] with the given strides.  A zero-padded, non-transposed conv only. */
+int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, long long x_batch_stride, int x_channel_stride,
+                                    int B, int T, int near_src, float in_slope, int lrelu, const float* act_add,
+                                    const float* residual, long long res_batch_stride, int res_channel_stride,
+                                    const float* film, long long film_batch_stride, int film_channel_stride, int film_half,
+                                    float* y, long long y_batch_stride, int y_channel_stride, float* y2, void* stream);
 
 /* ---- monotonic alignment search ------------------------------------------------------------
  * Replaces maximum_path_c / maximum_path_each, TTS/tts/utils/monotonic_align/core.pyx:11-47
@@ -616,6 +630,55 @@ int b200tts_melgan_forward(const b200tts_melgan* h, const float* x, int B, int T
  * G: device [1, N, taps + 1].  peak_bits as above (nullable). */
 int b200tts_pqmf_synthesis(const float* x, int B, int N, int Tb, const float* G, int taps, float* y, uint32_t* peak_bits,
                            void* stream);
+
+/* ---- WaveGrad vocoder --------------------------------------------------------------------------------------------
+ * Replaces Wavegrad.forward (TTS/vocoder/models/wavegrad.py:106-120; DBlock, FiLM, UBlock, PositionalEncoding:
+ * TTS/vocoder/layers/wavegrad.py:19-154) and the body of the refinement loop of Wavegrad.inference (wavegrad.py:138-145).
+ * Every conv zero-pads; F.interpolate is nearest (torch's index rule), the leaky-ReLU slope 0.2.  With n upsample
+ * factors f_0 .. f_{n-1}: n - 1 DBlocks (DBlock i: factor f_{n-1-i}), n FiLMs, n UBlocks (UBlock j: factor f_j, dilations
+ * upsample_dilations[j]).  hop = prod(f).  FiLM i runs at L[i], with L[0] = hop * T and L[i + 1] = L[i] / f_{n-1-i}.
+ * weights (host pointers, PyTorch layouts, weight norm folded), in state-dict order:
+ *   y_conv.w [yc, 1, 5], y_conv.b
+ *   per DBlock i: res_block.w [oc, ic, 1], .b, main_block.{0,1,2}.w [oc, ic | oc, 3], .b
+ *   per FiLM i:   input_conv.w [ic, ic, 3], .b, output_conv.w [2 oc, ic, 3], .b     (ic: yc, then dblock_out[i - 1];
+ *                                                                                  oc: ublock_out[n - 1 - i])
+ *   per UBlock j: res_block.w [hc, ic, 1], .b, main_block.{0,1}.w, .b, out_block.{0,1}.w, .b
+ *   x_conv.w [xc, in, 3], x_conv.b, out_conv.w [1, ublock_out[n-1], 3], out_conv.b
+ * pe, pe_frames (all calls): a host array of n device pointers; pe[i] = the [C_i, Lp[i]] table PositionalEncoding.pe / 5000
+ * of FiLM i (built the way the reference builds it, C_i its input channels) for pe_frames >= T mel frames, Lp[i] being
+ * L[i] at pe_frames: its row pitch.  So one set of tables, grown to the longest input, serves every shorter one, as the
+ * reference's cache does.
+ */
+typedef struct {
+    int in_channels, out_channels, y_conv_channels, x_conv_channels;
+    int num_upsamples;                 /* n, 1 .. 8; out_channels must be 1 */
+    int upsample_factors[8];
+    int dblock_out_channels[8];        /* n - 1 used; dblock_out_channels[i] == ublock_out_channels[n - 1 - i] */
+    int ublock_out_channels[8];        /* n used */
+    int upsample_dilations[8][4];
+} b200tts_wavegrad_config;
+typedef struct b200tts_wavegrad b200tts_wavegrad;
+int b200tts_wavegrad_create(const b200tts_wavegrad_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_wavegrad** out);
+void b200tts_wavegrad_destroy(b200tts_wavegrad* h);
+/* the true scratch size for [B, in, T] mel input: the conditioning x_conv(x), the n FiLM (shift, scale) tensors and five
+ * stage tensors (each as large as the largest activation of the network) */
+size_t b200tts_wavegrad_workspace_bytes(const b200tts_wavegrad* h, int B, int T);
+/* Wavegrad.forward(y, x, noise_scale) (wavegrad.py:106-120): y [B, 1, hop T], x [B, in, T], noise_scale device [B]
+ * -> eps [B, 1, hop T] */
+int b200tts_wavegrad_forward(const b200tts_wavegrad* h, const float* y, const float* x, const float* noise_scale,
+                             const float* const* pe, int pe_frames, int B, int T, float* eps, void* workspace,
+                             size_t workspace_bytes, void* stream);
+/* x_conv(x) (wavegrad.py:115) into the workspace, once per inference: the input is the same at every step */
+int b200tts_wavegrad_condition(const b200tts_wavegrad* h, const float* x, int B, int T, void* workspace,
+                               size_t workspace_bytes, void* stream);
+/* one refinement step (wavegrad.py:139-145) on the conditioning condition() left in the same workspace, in place on y:
+ *   y = clamp(c1 * (y - c2 * forward(y, x, noise_level)) + sigma * z, -1, 1)
+ * noise_level: device [B]; z (nullable: the last step, no noise term) [B, 1, hop T].  The network output never reaches
+ * memory (out_conv's epilogue applies the update); no host synchronisation. */
+int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* noise_level, const float* const* pe,
+                          int pe_frames, float c1, float c2, float sigma, const float* z, int B, int T, void* workspace,
+                          size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

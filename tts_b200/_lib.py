@@ -91,6 +91,13 @@ class MelganConfigC(ctypes.Structure):
                [("upsample_factors", ctypes.c_int * 8), ("pqmf_bands", ctypes.c_int), ("pqmf_taps", ctypes.c_int)]
 
 
+class WavegradConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("in_channels", "out_channels", "y_conv_channels", "x_conv_channels",
+                                            "num_upsamples")] + \
+               [("upsample_factors", ctypes.c_int * 8), ("dblock_out_channels", ctypes.c_int * 8),
+                ("ublock_out_channels", ctypes.c_int * 8), ("upsample_dilations", (ctypes.c_int * 4) * 8)]
+
+
 # padding modes of b200tts_conv1d_create_padded (B200TTS_PAD_* in include/tts_b200.h)
 PADDING_MODES = {"zeros": 0, "reflect": 1}
 
@@ -102,7 +109,8 @@ class AudioNormC(ctypes.Structure):
 
 
 DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped", 10: "attn_tc3",
-                  11: "attn_fma"}
+                  11: "attn_fma", 12: "tc3w_tf32", 13: "tc3w_tf32_near", 14: "tc3w_f16x3", 15: "tc3w_f16x3_near",
+                  16: "fma_wg", 17: "fma_wg_near"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}
@@ -144,6 +152,23 @@ def _declare(lib):
     lib.b200tts_melgan_out_len.argtypes = [vp, ci]
     lib.b200tts_melgan_forward.restype = ci
     lib.b200tts_melgan_forward.argtypes = [vp, vp, ci, ci, ci, vp, vp, vp, sz, vp]
+    lib.b200tts_wavegrad_create.restype = ci
+    lib.b200tts_wavegrad_create.argtypes = [ctypes.POINTER(WavegradConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+    lib.b200tts_wavegrad_destroy.restype = None
+    lib.b200tts_wavegrad_destroy.argtypes = [vp]
+    lib.b200tts_wavegrad_workspace_bytes.restype = sz
+    lib.b200tts_wavegrad_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_wavegrad_forward.restype = ci
+    lib.b200tts_wavegrad_forward.argtypes = [vp, vp, vp, vp, ctypes.POINTER(vp), ci, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_wavegrad_condition.restype = ci
+    lib.b200tts_wavegrad_condition.argtypes = [vp, vp, ci, ci, vp, sz, vp]
+    lib.b200tts_wavegrad_step.restype = ci
+    lib.b200tts_wavegrad_step.argtypes = [vp, vp, vp, ctypes.POINTER(vp), ci, ctypes.c_float, ctypes.c_float,
+                                          ctypes.c_float, vp, ci, ci, vp, sz, vp]
+    ll = ctypes.c_longlong
+    lib.b200tts_conv1d_forward_wavegrad.restype = ci
+    lib.b200tts_conv1d_forward_wavegrad.argtypes = [vp, vp, ll, ci, ci, ci, ci, ctypes.c_float, ci, vp, vp, ll, ci, vp, ll,
+                                                    ci, ci, vp, ll, ci, vp, vp]
     lib.b200tts_pqmf_synthesis.restype = ci
     lib.b200tts_pqmf_synthesis.argtypes = [vp, ci, ci, ci, vp, ci, vp, vp, vp]
     lib.b200tts_conv1d_destroy.restype = None

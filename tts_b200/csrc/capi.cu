@@ -16,6 +16,7 @@ struct b200tts_speaker_encoder { SpeakerEncoder impl; };
 struct b200tts_glow_tts { GlowTTS impl; };
 struct b200tts_melgan { Melgan impl; };
 struct b200tts_forward_tts { ForwardTTS impl; };
+struct b200tts_wavegrad { Wavegrad impl; };
 
 extern "C" {
 
@@ -110,6 +111,27 @@ int b200tts_conv1d_forward_strided(const b200tts_conv1d* h, const float* x, long
     if (accumulate) io.flags |= EPI_ACCUM;
     if (tanh) { io.act = ACT_TANH; io.peak_bits = peak_bits; }
     io.reflect = h->reflect;
+    return launch_conv(h->L, io, (cudaStream_t)stream);
+}
+
+int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, long long x_batch_stride, int x_channel_stride,
+                                    int B, int T, int near_src, float in_slope, int lrelu, const float* act_add,
+                                    const float* residual, long long res_batch_stride, int res_channel_stride,
+                                    const float* film, long long film_batch_stride, int film_channel_stride, int film_half,
+                                    float* y, long long y_batch_stride, int y_channel_stride, float* y2, void* stream) {
+    if (!h) { set_error("conv1d_forward_wavegrad: null handle"); return 1; }
+    if (h->c.transposed || h->reflect) { set_error("conv1d_forward_wavegrad: a zero-padded, non-transposed conv only"); return 1; }
+    const int Tout = b200tts_conv1d_out_len(h, T);
+    ConvIO io;
+    io.x = x; io.x_bs = x_batch_stride; io.x_cs = x_channel_stride; io.Tin = T; io.in_slope = in_slope;
+    io.y = y; io.y_bs = y_batch_stride; io.y_cs = y_channel_stride; io.Tout = Tout; io.B = B;
+    if (y2) { io.y2 = y2; io.y2_bs = y_batch_stride; io.y2_cs = y_channel_stride; }
+    if (residual) { io.res = residual; io.res_bs = res_batch_stride; io.res_cs = res_channel_stride; }
+    io.flags = EPI_WAVEGRAD;
+    io.near_src = near_src;
+    if (lrelu) { io.act = ACT_LRELU; io.act_param = 0.2f; }
+    io.act_add = act_add;
+    io.film = film; io.film_bs = film_batch_stride; io.film_cs = film_channel_stride; io.film_half = film_half;
     return launch_conv(h->L, io, (cudaStream_t)stream);
 }
 
@@ -449,6 +471,27 @@ int b200tts_melgan_forward(const b200tts_melgan* h, const float* x, int B, int T
 int b200tts_pqmf_synthesis(const float* x, int B, int N, int Tb, const float* G, int taps, float* y, uint32_t* peak_bits,
                            void* stream) {
     return launch_pqmf_synthesis(x, (long long)N * Tb, Tb, B, N, Tb, G, taps, y, peak_bits, (cudaStream_t)stream);
+}
+
+B200_HANDLE_API(wavegrad, b200tts_wavegrad, b200tts_wavegrad_config)
+
+int b200tts_wavegrad_forward(const b200tts_wavegrad* h, const float* y, const float* x, const float* noise_scale,
+                             const float* const* pe, int pe_frames, int B, int T, float* eps, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("wavegrad_forward: null handle"); return 1; }
+    return h->impl.forward(y, x, noise_scale, pe, pe_frames, B, T, eps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavegrad_condition(const b200tts_wavegrad* h, const float* x, int B, int T, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("wavegrad_condition: null handle"); return 1; }
+    return h->impl.condition(x, B, T, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* noise_level, const float* const* pe,
+                          int pe_frames, float c1, float c2, float sigma, const float* z, int B, int T, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("wavegrad_step: null handle"); return 1; }
+    return h->impl.step(y, noise_level, pe, pe_frames, c1, c2, sigma, z, B, T, workspace, workspace_bytes,
+                        (cudaStream_t)stream);
 }
 
 }  // extern "C"

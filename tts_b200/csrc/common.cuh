@@ -81,8 +81,12 @@ inline void count_launch(int n = 1) { g_launch_count += (unsigned long long)n; }
 //            SPLIT (WN res/skip): rows <  split -> (y , accum=1, mask_post=1)
 //                                 rows >= split -> (y2, accum=accum2, no mask), row index -= split
 //            ups > 1 (polyphase transposed conv): row r -> channel r/ups, time q*ups + r%ups
-enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3 };  // LOGCLAMP: log(max(v, act_param))
-enum : int { EPI_GATE = 1, EPI_MASK_PRE = 2, EPI_MASK_POST = 4, EPI_ACCUM = 8, EPI_SPLIT = 16, EPI_ACCUM2 = 32 };
+//            WAVEGRAD (EPI_WAVEGRAD / ConvIO::near_src): v = acc + bias; [lrelu(v, act_param)]; [+ act_add[b]]; [+ res];
+//                       [y2 <- v]; [v = shift + scale * v]; y <- v   (own kernel variants, see ConvIO)
+enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3,   // LOGCLAMP: log(max(v, act_param))
+             ACT_LRELU = 4 };                                             // LRELU: leaky ReLU, slope act_param (WaveGrad)
+enum : int { EPI_GATE = 1, EPI_MASK_PRE = 2, EPI_MASK_POST = 4, EPI_ACCUM = 8, EPI_SPLIT = 16, EPI_ACCUM2 = 32,
+             EPI_WAVEGRAD = 64 };
 
 enum : int { TC_NONE = -1 };  // ConvLayer::tc_prec: no tensor-core images
 
@@ -137,6 +141,18 @@ struct ConvIO {
     // x[2 Tin - 2 - t] (t >= Tin) instead of zero; no column outside [0, Tin) is ever read.  Needs pad <= Tin - 1; not
     // combined with lens, a column window or a transposed conv.
     int reflect = 0;
+    // ---- WaveGrad variants (flags EPI_WAVEGRAD or near_src > 0; dense, unwindowed, ups 1, no masks).  They run on kernel
+    // instantiations of their own, so every other launch compiles to the code it always did.
+    // nearest resampling (F.interpolate(mode="nearest") of the input): the conv reads a virtual input of Tin columns whose
+    // column t is x[nearest(t)], x holding near_src columns -- torch's rule: t when Tin == near_src, t >> 1 when
+    // Tin == 2 near_src, else min(floor(t * (float)(near_src / Tin)), near_src - 1).  Covers the UBlock upsampling and the
+    // DBlock decimation (t * f) without materialising the resampled tensor.  0: off.
+    int near_src = 0;
+    // FiLM (wavegrad.py shif_and_scale): v = shift + scale * v with shift = film[b, c, t] and scale = film[b, film_half + c,
+    // t] (the two chunks of a FiLM output_conv tensor); y2 (nullable) receives v before it.  act_add (device [B], nullable):
+    // added after the activation (the FiLM noise level).  With EPI_WAVEGRAD, act may be ACT_LRELU.
+    const float* film = nullptr; long long film_bs = 0; int film_cs = 0; int film_half = 0;
+    const float* act_add = nullptr;
 };
 
 // Host weights in PyTorch layout.  conv: w[Cout][Cin][K];  transposed: w[Cin][Cout][Kt].
@@ -153,7 +169,9 @@ int conv_tc_error_flag();
 enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6,
              DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9,    // TC16*: the same kernels with bf16 / fp16 operands
              // ForwardTTS decoder attention: the tensor-core kernel, or the FP32-FMA kernel for heads it does not take
-             DISPATCH_ATTN_TC3 = 10, DISPATCH_ATTN_FMA = 11 };
+             DISPATCH_ATTN_TC3 = 10, DISPATCH_ATTN_FMA = 11,
+             // WaveGrad variants (EPI_WAVEGRAD / ConvIO::near_src): tensor cores by operand type, FMA tile; +1: resampled input
+             DISPATCH_TC3W_TF32 = 12, DISPATCH_TC3W_F16X3 = 14, DISPATCH_FMA_WG = 16 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -82,9 +82,13 @@ struct ConvKArgs {
     const int* lens; int rate_out, need_out, rate_in, need_in;
     int q_lo, q_hi, in_lo, in_hi;   // column window (ConvIO), q_lo / in_lo >= 0
     int reflect;                    // reflection padding (ConvIO::reflect)
+    // WaveGrad (KEPI_WAVEGRAD only, see ConvIO): nearest-resampled input, FiLM, pre-FiLM store, per-batch add
+    int near_src; float near_scale;
+    const float* film; long long film_bs; int film_cs, film_half;
+    const float* act_add;
 };
 
-enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3 };
+enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3, KEPI_WAVEGRAD = 4 };
 
 // CJ rows x TJ time steps per lane, WCO x WT warps, CIC input channels per stage, EPI epilogue family.
 // KG > 1: intra-CTA split-K for launch-starved shapes (text encoder / duration predictor: 64 frames x 32 utterances
@@ -129,13 +133,17 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
             const bool tok = (t >= a.in_lo) && (t < a.Tin);   // below in_lo: stale scratch of a windowed producer
             float m = 1.f;
             if (tok && mb) m = __ldg(mb + t);
+            int ts = t;                                        // source column
+            if constexpr (EPI == KEPI_WAVEGRAD) {
+                if (a.near_src && tok) ts = tc3::near_col(t, a.near_src, a.Tin, a.near_scale);
+            }
 #pragma unroll
             for (int h = 0; h < CIC; h += 8) {
                 float v[8];
 #pragma unroll
                 for (int ci = 0; ci < 8; ++ci) {
                     v[ci] = 0.f;
-                    if (tok && (c0 + h + ci) < a.Cin) v[ci] = __ldg(xb + (long long)(c0 + h + ci) * a.x_cs + t);
+                    if (tok && (c0 + h + ci) < a.Cin) v[ci] = __ldg(xb + (long long)(c0 + h + ci) * a.x_cs + ts);
                 }
 #pragma unroll
                 for (int ci = 0; ci < 8; ++ci) {
@@ -257,6 +265,41 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                         unpack2(acc[p][j], v0, v1);
                         if (inw(q)) yrow[q] = tanhf((h ? v1 : v0) + bb);
                     }
+                }
+            }
+        }
+        return;
+    }
+    if (EPI == KEPI_WAVEGRAD) {
+        // v = acc + bias; [lrelu]; [+ act_add[b]]; [+ res]; [y2 <- v]; [v = shift + scale * v]; y <- v, each operation
+        // rounded on its own (the reference's order); res / y2 may alias element for element (load before store)
+        const bool lrelu = a.act == ACT_LRELU;
+        const float add = a.act_add ? __ldg(a.act_add + b) : 0.f;
+#pragma unroll
+        for (int p = 0; p < CJ / 2; ++p) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = row_base + 2 * p + h;
+                if (r >= a.Rows) continue;
+                const float bb = a.bias[r];
+                const long long rr = r;
+                float* yrow = a.y + b * a.y_bs + rr * a.y_cs;
+                float* y2row = a.y2 ? a.y2 + b * a.y2_bs + rr * a.y2_cs : nullptr;
+                const float* rrow = a.res ? a.res + b * a.res_bs + rr * a.res_cs : nullptr;
+                const float* srow = a.film ? a.film + b * a.film_bs + rr * a.film_cs : nullptr;
+#pragma unroll
+                for (int j = 0; j < TJ; ++j) {
+                    const int q = qb + 32 * j;
+                    if (!inw(q)) continue;
+                    float v0, v1;
+                    unpack2(acc[p][j], v0, v1);
+                    float u = __fadd_rn(h ? v1 : v0, bb);
+                    if (lrelu) u = u > 0.f ? u : __fmul_rn(u, a.act_param);
+                    if (a.act_add) u = __fadd_rn(u, add);
+                    if (rrow) u = __fadd_rn(u, rrow[q]);
+                    if (y2row) y2row[q] = u;
+                    if (srow) u = __fadd_rn(srow[q], __fmul_rn(srow[(long long)a.film_half * a.film_cs + q], u));
+                    yrow[q] = u;
                 }
             }
         }
@@ -707,7 +750,7 @@ static int launch_variant(const ConvKArgs& ka, int B, int RowsPad, cudaStream_t 
     B200_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "conv1d: grid too large");
     conv1d_kernel<CJ, TJ, WCO, WT, CIC, EPI, KG><<<grid, NT, smem, st>>>(a);
     count_launch();
-    dispatch_note(DISPATCH_FMA);
+    dispatch_note(EPI == KEPI_WAVEGRAD ? DISPATCH_FMA_WG + (a.near_src > 0 ? 1 : 0) : DISPATCH_FMA);
     B200_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -811,6 +854,10 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
                 for (bool refl : {false, true})
                     B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                       smem_optin));
+            for (bool near : {false, true})
+                if (tc3::wavegrad_kernel(p, near))
+                    B200_CUDA_OK(cudaFuncSetAttribute(tc3::wavegrad_kernel(p, near), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      smem_optin));
         }
         int* flag = nullptr;   // [0] pipeline timeout, [tc::ERR_RANGE] fp16 range (PREC_F16X3)
         B200_CUDA_OK(cudaHostAlloc((void**)&flag, 2 * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
@@ -840,7 +887,9 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     // grouped mode for the layers with a grouped image: M = tap groups x channels, N = 256 time steps, 240 per tile
     const int G = L.tc_grp, J = G ? (L.K + G - 1) / G : 0;
     const int rp_grouped = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
-    const bool grouped = G && !needs_v3 && !a.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
+    const bool wg = (a.flags & EPI_WAVEGRAD) != 0;   // WaveGrad epilogue / resampled input: conv1d_tc3w_kernel
+    if (wg && !tc3::wavegrad_kernel(L.tc_prec, false)) return -1;
+    const bool grouped = G && !wg && !needs_v3 && !a.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
     // plain mode otherwise: M = rows (128 per tile, zero padded), N = 256 time steps.  Everything neither mode takes
     // (unaligned or masked inputs, shared-memory budget) runs on the exact FP32-FMA kernel.
     const int rows_pad = grouped ? rp_grouped : (tc3::TT2 + (L.K - 1) * L.dil + 7) / 8 * 8;
@@ -871,13 +920,22 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
     const bool reflect = a.reflect != 0;   // reflection padding: the lean kernels' reflect variants only
     if (reflect && !grouped && !plain_epi) return -1;
-    const tc3::Tc3Kernel k = grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect) : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
+    if (wg) {
+        t.near_src = a.near_src; t.near_scale = a.near_scale;
+        t.film = a.film; t.film_bs = a.film_bs; t.film_cs = a.film_cs; t.film_half = a.film_half;
+        t.act_add = a.act_add; t.lrelu = a.act == ACT_LRELU; t.act_param = a.act_param;
+    }
+    const tc3::Tc3Kernel k = wg ? tc3::wavegrad_kernel(L.tc_prec, a.near_src > 0)
+                                : grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect) : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
     const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
     const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
     B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));
     count_launch();
     const bool b16 = L.tc_prec == tc::PREC_BF16 || L.tc_prec == tc::PREC_FP16;   // PREC_F16X3 logs as tc3
-    dispatch_note(grouped ? (b16 ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED) : (b16 ? DISPATCH_TC16 : DISPATCH_TC3));
+    if (wg)
+        dispatch_note((L.tc_prec == tc::PREC_F16X3 ? DISPATCH_TC3W_F16X3 : DISPATCH_TC3W_TF32) + (a.near_src > 0 ? 1 : 0));
+    else
+        dispatch_note(grouped ? (b16 ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED) : (b16 ? DISPATCH_TC16 : DISPATCH_TC3));
     B200_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -919,6 +977,22 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
         B200_REQUIRE(!io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && L.ups == 1 && !io.xmask,
                      "launch_conv: reflection padding takes no lens, column window, input mask or upsampling");
     }
+    if (io.near_src > 0) a.flags |= EPI_WAVEGRAD;
+    if (a.flags & EPI_WAVEGRAD) {   // WaveGrad layers: their own kernel variants (tensor cores, else the FMA tile kernel)
+        B200_REQUIRE(L.ups == 1 && !io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && !io.xmask && !io.ymask &&
+                         !io.cond && !a.reflect && a.flags == EPI_WAVEGRAD && a.scale == 1.f && a.post_div == 1.f &&
+                         (a.act == ACT_NONE || a.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film_cs > 0)) &&
+                         io.near_src >= 0,
+                     "launch_conv: the WaveGrad epilogue takes only lrelu / act_add / res / y2 / film, on a dense launch");
+        a.near_src = io.near_src;
+        a.near_scale = io.near_src > 0 ? (float)io.near_src / (float)io.Tin : 1.f;
+        a.film = io.film; a.film_bs = io.film_bs; a.film_cs = io.film_cs; a.film_half = io.film_half;
+        a.act_add = io.act_add;
+        if (a.Tq <= 0 || io.B <= 0) return 0;
+        if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;
+        return launch_cic<KEPI_WAVEGRAD>(a, L.co_tile, io.B, L.RowsPad, st);
+    }
+    B200_REQUIRE(a.act != ACT_LRELU, "launch_conv: the leaky-ReLU epilogue needs EPI_WAVEGRAD");
     if (a.Tq <= 0 || io.B <= 0) return 0;
     B200_REQUIRE(!(a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)) || io.ymask,
                  "launch_conv: masked/split epilogue needs ymask");

@@ -98,7 +98,21 @@ struct Tc3Args {
     // where the producer's window ends, so the grouped mode's zero-padded taps never multiply stale data.  n_ttiles counts
     // the window's tiles per row (dense schedule), t_lo = floor(q_lo / tstep) is the first one.
     int q_lo, q_hi, in_lo, t_lo;
+    // ---- WaveGrad kernels only (conv1d_tc3w_kernel, see ConvIO): nearest-resampled input (near_src source columns, 0: off;
+    // near_scale = (float)near_src / Tin), FiLM (shift / scale rows of `film`), y2 store of the pre-FiLM value, leaky ReLU
+    // (lrelu, slope act_param) and the per-batch act_add after it
+    int near_src; float near_scale;
+    const float* film; long long film_bs; int film_cs, film_half;
+    const float* act_add; int lrelu; float act_param;
 };
+
+// torch's nearest source index (upsample_nearest1d's nearest_idx): identity, the exact-2x shortcut, else
+// min(floor(dst * scale), src - 1) with the float scale src / dst
+__device__ __forceinline__ int near_col(int t, int src, int dst, float scale) {
+    if (dst == src) return t;
+    if (dst == 2 * src) return t >> 1;
+    return min((int)floorf(__fmul_rn((float)t, scale)), src - 1);
+}
 
 // prec: PREC_FP32 (8-channel chunks, hi/lo slab pairs), a 16-bit type (16-channel chunks, two slabs) or PREC_F16X3
 // (16-channel chunks over 8-channel raw stages, hi/lo slab pairs, three-plane weight blocks: the FP32 kernel's total)
@@ -193,7 +207,10 @@ __device__ __forceinline__ void lean_tile(const float* at, const float* bias, co
 // Everything the lean epilogue does not cover (WaveNet gate / res-skip split, masks, ReLU, scale, final divide, polyphase
 // stores of the transposed convs, edge tiles): one tile half per call, lane = one output row, `arow` = its accumulators.
 // SC: the accumulators are scaled by the row's rscale first (PREC_F16X3).
-template <bool SC>
+// WG: the WaveGrad epilogue instead (conv1d_tc3w_kernel):
+//   v = acc + bias; [lrelu]; [+ act_add[b]]; [+ res]; [y2 <- v]; [v = shift + scale * v]; y <- v
+// with every product and sum rounded on its own (no FMA contraction), in the reference's order.
+template <bool SC, bool WG = false>
 __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float* arow, int b, int rt, int q0, int lq, int half,
                                                   int lane) {
     const int ups = a.ups;
@@ -211,6 +228,69 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
             for (int i = 0; i < 16; ++i) v[i] *= rs;
         }
     };
+    if constexpr (WG) {
+        if (!rok) return;
+        const long long rcs = (long long)rc;
+        float* yrow = a.y + (long long)b * a.y_bs + rcs * a.y_cs;
+        float* y2row = a.y2 ? a.y2 + (long long)b * a.y2_bs + rcs * a.y2_cs : nullptr;
+        const float* rrow = a.res ? a.res + (long long)b * a.res_bs + rcs * a.res_cs : nullptr;
+        const float* srow = a.film ? a.film + (long long)b * a.film_bs + rcs * a.film_cs : nullptr;
+        const float* crow = srow ? srow + (long long)a.film_half * a.film_cs : nullptr;
+        const float add = a.act_add ? __ldg(a.act_add + b) : 0.f;
+        const bool has_add = a.act_add != nullptr, lrelu = a.lrelu != 0;
+        const float slope = a.act_param;
+        // float4 accesses when every row pointer is 16-byte aligned (all pitches multiples of 4 floats)
+        const bool vec_ok = ((reinterpret_cast<uintptr_t>(yrow) | reinterpret_cast<uintptr_t>(y2row) |
+                              reinterpret_cast<uintptr_t>(rrow) | reinterpret_cast<uintptr_t>(srow) |
+                              reinterpret_cast<uintptr_t>(crow)) & 15) == 0;
+        for (int cg = 0; cg < 128; cg += 16) {
+            float v[16];
+            acc_ld(arow + cg, v);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int qq = qb + cg + 4 * j;
+                if (qq >= a.Tout) break;
+                const bool vec = vec_ok && qq + 3 < a.Tout;
+                float r4[4] = {0.f, 0.f, 0.f, 0.f}, s4[4] = {0.f, 0.f, 0.f, 0.f}, c4[4] = {1.f, 1.f, 1.f, 1.f};
+                if (vec) {
+                    if (rrow) { const float4 t = *reinterpret_cast<const float4*>(rrow + qq); r4[0] = t.x; r4[1] = t.y; r4[2] = t.z; r4[3] = t.w; }
+                    if (srow) {
+                        const float4 t = *reinterpret_cast<const float4*>(srow + qq); s4[0] = t.x; s4[1] = t.y; s4[2] = t.z; s4[3] = t.w;
+                        const float4 u = *reinterpret_cast<const float4*>(crow + qq); c4[0] = u.x; c4[1] = u.y; c4[2] = u.z; c4[3] = u.w;
+                    }
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int qe = min(qq + e, a.Tout - 1);
+                        if (rrow) r4[e] = rrow[qe];
+                        if (srow) { s4[e] = srow[qe]; c4[e] = crow[qe]; }
+                    }
+                }
+                float o[4], p[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    float u = __fadd_rn(v[4 * j + e], bias);
+                    if (lrelu) u = u > 0.f ? u : __fmul_rn(u, slope);
+                    if (has_add) u = __fadd_rn(u, add);
+                    if (rrow) u = __fadd_rn(u, r4[e]);
+                    p[e] = u;
+                    o[e] = srow ? __fadd_rn(s4[e], __fmul_rn(c4[e], u)) : u;
+                }
+                if (vec) {
+                    if (y2row) *reinterpret_cast<float4*>(y2row + qq) = make_float4(p[0], p[1], p[2], p[3]);
+                    *reinterpret_cast<float4*>(yrow + qq) = make_float4(o[0], o[1], o[2], o[3]);
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (qq + e < a.Tout) {
+                            if (y2row) y2row[qq + e] = p[e];
+                            yrow[qq + e] = o[e];
+                        }
+                }
+            }
+        }
+        return;
+    }
     if (a.gate) {
         // WaveNet gate (wavenet.py:6-13): even lane = tanh argument, odd lane = sigmoid argument of row r/2
         float* yrow = a.y + (long long)b * a.y_bs + (long long)(rc >> 1) * a.y_cs;
@@ -415,13 +495,15 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     }
 }
 
-template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false>
+template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false, bool NEAR = false, bool WG = false>
                                        // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
                                        // plain-layer kernel (lean epilogue inline, general one out of line) -- false for the
                                        // WaveNet / masked / transposed layers (general epilogue inline); PREC: operand type;
                                        // REFL: reflection padding (ConvIO::reflect; dense, unwindowed launches only): input
                                        // column t < 0 reads x[-t], t >= Tin reads x[2 Tin - 2 - t].  A compile-time switch so
                                        // that the zero-padding kernels keep their register allocation.
+                                       // NEAR: nearest-resampled input (ConvIO::near_src): column t in [0, Tin) reads
+                                       // x[near_col(t)], staged by 4-byte copies; WG: the WaveGrad epilogue (general_tile_body).
 __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr bool X3 = PREC == PREC_F16X3;      // 3-product fp16 split
@@ -564,7 +646,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     iss_Tin = input_extent(b_);
                     iss_tal = (q0_ - pad) & ~3;                            // 16-byte aligned window start (may be < 0)
                     iss_row = xg + (long long)b_ * x_bs;
-                    iss_int = iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
+                    iss_int = !NEAR && iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
                     iss_new = false;
                 }
                 // a raw stage is RCH / 8 slots of 8 channels (two for BF16 / FP16): the per-thread work items cover one slot
@@ -583,6 +665,19 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                             if (v_ch[e] < 0) continue;
                             const int t = iss_tal + v_t[e];
                             const int cg = ch0 + h * KC2 + v_ch[e];
+                            if constexpr (NEAR) {
+                                // nearest-resampled input: four 4-byte copies from the source columns of t .. t + 3 (a
+                                // gather, so no vector copy); columns outside the virtual row [0, Tin) are the zero padding
+                                const float* rowp = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs;
+#pragma unroll
+                                for (int q = 0; q < 4; ++q) {
+                                    const int tt = t + q;
+                                    const bool in = cg < Cin && tt >= 0 && tt < iss_Tin;
+                                    const int src = in ? near_col(tt, a.near_src, iss_Tin, a.near_scale) : 0;
+                                    cp_async4_zfill(dst0 + v_dst[e] + 4u * q, rowp + src, in ? 4u : 0u);
+                                }
+                                continue;
+                            }
                             if (REFL && (t < 0 || t + 4 > iss_Tin)) {
                                 // edge vector of a reflect-padded conv (vectors inside the row keep the 16-byte copy): four
                                 // mirrored 4-byte copies, each from inside the row or zero-filled where the mirror leaves
@@ -824,7 +919,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 } else if constexpr (LEAN) {
                     general_tile_call<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 } else {
-                    general_tile_body<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
+                    general_tile_body<SC, WG>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 }
             }
         }
@@ -839,7 +934,19 @@ __global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3x_kernel(const __grid_
 template <int GRP, int PREC, bool REFL = false>
 __global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3g_kernel(const __grid_constant__ Tc3Args a) { tc3_body<GRP, true, PREC, REFL>(a); }
 
+// WaveGrad layers (EPI_WAVEGRAD / nearest-resampled input): the WaveGrad epilogue inline, NEAR for a resampled input
+template <int PREC, bool NEAR>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3w_kernel(const __grid_constant__ Tc3Args a) {
+    tc3_body<1, false, PREC, false, NEAR, true>(a);
+}
+
 typedef void (*Tc3Kernel)(const Tc3Args);
+// the WaveGrad kernels exist for 3xTF32 and the split-fp16 operands (the precisions WaveGrad packs)
+static inline Tc3Kernel wavegrad_kernel(int prec, bool near) {
+    if (prec == PREC_F16X3) return near ? conv1d_tc3w_kernel<PREC_F16X3, true> : conv1d_tc3w_kernel<PREC_F16X3, false>;
+    if (prec == PREC_FP32) return near ? conv1d_tc3w_kernel<PREC_FP32, true> : conv1d_tc3w_kernel<PREC_FP32, false>;
+    return nullptr;
+}
 // reflect: the reflection-padding variant (lean epilogue only; the host sends reflect-padded layers that need the general
 // epilogue to the FMA kernel)
 static inline Tc3Kernel plain_kernel(int prec, bool lean, bool reflect = false) {

@@ -267,6 +267,46 @@ struct Melgan {
 int launch_pqmf_synthesis(const float* x, long long x_bs, int x_cs, int B, int N, int Tb, const float* G, int taps, float* y,
                           unsigned* peak_bits, cudaStream_t st);
 
+// WaveGrad (wavegrad.cu): the refinement network on the shared conv engine.  Down path y_conv -> FiLM[0] -> per DBlock
+// [res (1x1), three lrelu -> k3 convs, dilations 1 / 2 / 4, on the decimated input] -> FiLM[i+1]; up path x_conv ->
+// per UBlock [res (1x1) and main0 on the nearest-upsampled input, main1, out0, out1 with the FiLM pair of its rate] ->
+// out_conv.  The resampling is an input addressing mode (ConvIO::near_src) and FiLM / the FiLM input epilogue are the
+// conv engine's WaveGrad epilogue, so no resampled or FiLM-ed tensor is written on its own.  x_conv(spectrogram) runs
+// once per inference (condition); each refinement step runs the network with out_conv fused into the update
+//   y = clamp(c1 * (y - c2 * eps) + sigma * z, -1, 1)
+// so eps never reaches memory.  Tensors use row pitches rounded up to 4 floats (16-byte rows).
+struct Wavegrad {
+    struct DBlock { ConvLayer res, m0, m1, m2; int f = 1; };
+    struct Film { ConvLayer in, out; };
+    struct UBlock { ConvLayer res, m0, m1, o0, o1; int f = 1; };
+    b200tts_wavegrad_config c;
+    ConvLayer y_conv, x_conv;
+    float *out_w = nullptr, *out_b = nullptr;   // out_conv [Clast][3] and its bias (own single-row kernel)
+    std::vector<DBlock> db;
+    std::vector<Film> film;
+    std::vector<UBlock> ub;
+    ~Wavegrad();
+    int init(const b200tts_wavegrad_config& cfg, const float* const* w, int nw);
+    int hop() const;
+    // down-path lengths: L[0] = hop * T, L[i + 1] = L[i] / f_i; FiLM i runs at L[i]
+    void lengths(int T, std::vector<int>& L) const;
+    size_t workspace_bytes(int B, int T) const;
+    // x_conv(x) into the workspace; step() reads it from there (same B, T and workspace)
+    int condition(const float* x, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    // Wavegrad.forward: eps [B, 1, hop T] from y [B, 1, hop T], x [B, in, T] and noise_scale (device [B]); pe[i]: device
+    // [film_in_i][Lp[i]] tables pe / 5000 of FiLM i built for pe_frames >= T frames (Lp = lengths(pe_frames): the row
+    // pitch; only the first L[i] columns are read)
+    int forward(const float* y, const float* x, const float* noise_scale, const float* const* pe, int pe_frames, int B, int T,
+                float* eps, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    // one refinement step in place on y (z nullable: no noise term); noise_level device [B]
+    int step(float* y, const float* noise_level, const float* const* pe, int pe_frames, float c1, float c2, float sigma,
+             const float* z, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const;
+  private:
+    int network(const float* y, const float* noise_level, const float* const* pe, int pe_frames, int B, int T, float* out,
+                float c1, float c2, float sigma, const float* z, int update, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+};
+
 // durations -> path -> expanded prior (path.cu)
 int launch_durations(const float* logw, const float* x_mask, float length_scale, int B, int T, float* w_ceil,
                      float* cum, long long* y_lengths, const int* err_flag, long long* meta, cudaStream_t st);

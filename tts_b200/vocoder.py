@@ -173,6 +173,27 @@ def setup_generator(c):
     raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN and MelGAN generators are)")
 
 
+def setup_model(config):
+    """TTS/vocoder/models/__init__.py:12-31: ``GAN`` for a config naming both a generator and a discriminator or for
+    ``model == "gan"`` (then built by ``setup_generator`` from ``generator_model``, as the reference's GAN does),
+    ``Wavegrad`` for ``model == "wavegrad"``.  The other vocoder models that function can name (WaveRNN, ...) are not
+    built here and raise NotImplementedError, as does a config without a ``model`` name."""
+    if "discriminator_model" in config and "generator_model" in config:
+        return GAN.init_from_config(config)
+    model = _get(config, "model")
+    if not isinstance(model, str):
+        raise NotImplementedError("tts_b200.setup_model: the config names no vocoder `model` (and no generator + "
+                                  "discriminator pair)")
+    name = model.lower()
+    if name == "gan":
+        return GAN.init_from_config(config)
+    if name == "wavegrad":
+        from .wavegrad import Wavegrad   # wavegrad.py imports this module's config classes
+        return Wavegrad.init_from_config(config)
+    raise NotImplementedError(f"tts_b200.setup_model: vocoder model `{_get(config, 'model')}` is not built "
+                              "(GAN generators and WaveGrad are)")
+
+
 def _get(obj, key, default=None):
     if isinstance(obj, dict):
         return obj.get(key, default)
