@@ -680,6 +680,81 @@ int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* nois
                           int pe_frames, float c1, float c2, float sigma, const float* z, int B, int T, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---- Overflow / Neural-HMM inference (text -> mel spectrogram, autoregressive) ----------------------------------
+ * Replaces Overflow.inference (TTS/tts/models/overflow.py:207-246) and NeuralhmmTTS.inference
+ * (TTS/tts/models/neuralhmm_tts.py) in three calls:
+ *   encode  - Encoder.inference (TTS/tts/layers/overflow/common_layers.py:70-92): embedding, 3 x ConvBNBlock
+ *             (TTS/tts/layers/tacotron/tacotron2.py:11-44, eval BatchNorm folded into the conv), bidirectional nn.LSTM,
+ *             the reshape to [B, Tt*spp, E]; plus the encoder-state part of the output net's first layer for every
+ *             state (hoisted out of the loop: the loop only gathers the current state's column).
+ *   sample  - NeuralHMM.inference / sample (TTS/tts/layers/overflow/neural_hmm.py:338-464): Prenet
+ *             (tacotron/common_layers.py:63-120, prenet_type "original"), LSTMCell, Outputnet / ParameterModel
+ *             (overflow/common_layers.py:95-219), EmissionModel.sample and the deterministic transition rule.  The loop
+ *             runs chunk_frames frames per CUDA graph replay and reads 1 + B words after each chunk; no kernel waits on
+ *             another block.
+ *   decode  - Overflow only: Decoder (overflow/decoder.py:56-78, the Glow decoder in reverse) and inverse_normalize;
+ *             for Neural-HMM (has_decoder 0) only inverse_normalize (neuralhmm_tts.py inference).
+ * Batched, unlike the reference (whose Encoder.inference ignores x_lengths): row b computes the reference's
+ * inference(text[b:b+1, :lengths[b]]).  Everything up to the decoder runs in FP32 on the FMA pipe, so the duration
+ * decisions (thresholds on a running product) do not depend on tensor-core rounding.
+ * weights (host, PyTorch layouts), in this order:
+ *   encoder.emb.weight [n_vocab, E]
+ *   per conv i < n_convs: convolution1d.weight [E, E, 5], .bias [E], batch_normalization.weight, .bias, .running_mean,
+ *     .running_var [E] (eps 1e-5)
+ *   encoder.lstm.weight_ih_l0 [4H, E], weight_hh_l0 [4H, H], bias_ih_l0, bias_hh_l0, then the same four _reverse
+ *     (H = E / 2 * state_per_phone)
+ *   neural_hmm.go_tokens [ar_order, 1]
+ *   per prenet layer: linear_layer.weight [P, in] (in = C * ar_order for the first, P after; no bias)
+ *   memory_rnn.weight_ih [4M, P], weight_hh [4M, M], bias_ih, bias_hh
+ *   per output-net layer l: linear_layer.weight [O_l, in_l] (in_0 = M + E: columns [0, M) take h, [M, M + E) the state),
+ *     .bias [O_l]; last_layer.weight [2C + 1, O_last], .bias
+ *   mean [C], std [C] (a scalar buffer expanded to C)
+ *   has_decoder: the Glow decoder blocks as for b200tts_glow_tts_config (no cond layer)
+ */
+typedef struct {
+    int n_vocab;
+    int encoder_dim;           /* E, even */
+    int n_convs;               /* encoder conv blocks, <= 8 */
+    int state_per_phone;       /* spp */
+    int out_channels;          /* C (mel channels) */
+    int ar_order;
+    int prenet_dim;            /* P */
+    int prenet_n_layers;       /* 1 .. 8 */
+    int prenet_dropout;        /* 0: no dropout layer; else p = 0.5 where drop masks are given */
+    int memory_rnn_dim;        /* M */
+    int outputnet_n_layers;    /* 1 .. 8 */
+    int outputnet_size[8];
+    float std_floor;
+    int has_decoder;           /* 1: Overflow (Glow decoder), 0: Neural-HMM */
+    int hidden_channels_dec, kernel_size_dec, dilation_rate, num_flow_blocks, num_block_layers, num_splits, num_squeeze,
+        sigmoid_scale;
+} b200tts_overflow_config;
+typedef struct b200tts_overflow b200tts_overflow;
+int b200tts_overflow_create(const b200tts_overflow_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_overflow** out);
+void b200tts_overflow_destroy(b200tts_overflow* h);
+/* one workspace serves all three calls of an utterance batch: B rows of up to Tt tokens and up to F frames */
+size_t b200tts_overflow_workspace_bytes(const b200tts_overflow* h, int B, int Tt, int F);
+/* tokens int64 [B, Tt], lengths int64 [B] (1 .. Tt) -> states [B, Tt * spp, E] (zero past lengths[b] * spp); the
+ * hoisted first-layer term stays in the workspace for sample() */
+int b200tts_overflow_encode(const b200tts_overflow* h, const int64_t* tokens, const int64_t* lengths, int B, int Tt,
+                            float* states, void* workspace, size_t workspace_bytes, void* stream);
+/* the sampling loop on the state encode() left in the same workspace.  temp: sampling_temp (> 0: x = mean +
+ * (std * temp) * noise); max_frames: max_sampling_time (>= 1); threshold: duration_threshold.  noise (nullable when
+ * temp <= 0): device [B, max_frames, C] standard-normal draws; drop (nullable: no dropout): device uint8
+ * [B, max_frames, prenet_n_layers, P], 1 keeps (x 2) and 0 drops a prenet unit.  Outputs: hmm_out [B, max_frames, C]
+ * (zero past a row's frames), states_travelled int32 [B, max_frames + 1] (-1 past a row's frames + 1 entries),
+ * frames (host int32 [B]): frames per row. */
+int b200tts_overflow_sample(const b200tts_overflow* h, const int64_t* lengths, int B, int Tt, float temp, int max_frames,
+                            float threshold, const float* noise, const uint8_t* drop, int chunk_frames, float* hmm_out,
+                            int32_t* states_travelled, int32_t* frames, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* hmm_out [B, Fpitch, C] (as sample wrote it), frames device int32 [B], F = max frames -> mel [B, F', C]:
+ * Overflow: F' = F floored to num_squeeze, each row's frames floored likewise, the decoder in reverse, x * std + mean
+ * (padded frames come out as mean); Neural-HMM: F' = F, hmm_out * std + mean. */
+int b200tts_overflow_decode(const b200tts_overflow* h, const float* hmm_out, const int32_t* frames, int B, int F,
+                            int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,6 +17,7 @@ struct b200tts_glow_tts { GlowTTS impl; };
 struct b200tts_melgan { Melgan impl; };
 struct b200tts_forward_tts { ForwardTTS impl; };
 struct b200tts_wavegrad { Wavegrad impl; };
+struct b200tts_overflow { Overflow impl; };
 
 extern "C" {
 
@@ -494,4 +495,40 @@ int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* nois
                         (cudaStream_t)stream);
 }
 
+int b200tts_overflow_create(const b200tts_overflow_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_overflow** out) {
+    if (!cfg || !weights || !out) { set_error("overflow_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_overflow* h = new (std::nothrow) b200tts_overflow();
+    if (!h) { set_error("overflow_create: out of host memory"); return 1; }
+    int rc = h->impl.init(*cfg, weights, num_weights);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+void b200tts_overflow_destroy(b200tts_overflow* h) { delete h; }
+size_t b200tts_overflow_workspace_bytes(const b200tts_overflow* h, int B, int Tt, int F) {
+    return h ? h->impl.workspace_bytes(B, Tt, F) : 0;
+}
+int b200tts_overflow_encode(const b200tts_overflow* h, const int64_t* tokens, const int64_t* lengths, int B, int Tt,
+                            float* states, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("overflow_encode: null handle"); return 1; }
+    return h->impl.encode((const long long*)tokens, (const long long*)lengths, B, Tt, states, workspace, workspace_bytes,
+                          (cudaStream_t)stream);
+}
+int b200tts_overflow_sample(const b200tts_overflow* h, const int64_t* lengths, int B, int Tt, float temp, int max_frames,
+                            float threshold, const float* noise, const uint8_t* drop, int chunk_frames, float* hmm_out,
+                            int32_t* states_travelled, int32_t* frames, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+    if (!h) { set_error("overflow_sample: null handle"); return 1; }
+    return h->impl.sample((const long long*)lengths, B, Tt, temp, max_frames, threshold, noise, drop, chunk_frames,
+                          hmm_out, states_travelled, frames, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_overflow_decode(const b200tts_overflow* h, const float* hmm_out, const int32_t* frames, int B, int F,
+                            int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("overflow_decode: null handle"); return 1; }
+    return h->impl.decode(hmm_out, frames, B, F, Fpitch, mel, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"
+

@@ -171,7 +171,9 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // ForwardTTS decoder attention: the tensor-core kernel, or the FP32-FMA kernel for heads it does not take
              DISPATCH_ATTN_TC3 = 10, DISPATCH_ATTN_FMA = 11,
              // WaveGrad variants (EPI_WAVEGRAD / ConvIO::near_src): tensor cores by operand type, FMA tile; +1: resampled input
-             DISPATCH_TC3W_TF32 = 12, DISPATCH_TC3W_F16X3 = 14, DISPATCH_FMA_WG = 16 };
+             DISPATCH_TC3W_TF32 = 12, DISPATCH_TC3W_F16X3 = 14, DISPATCH_FMA_WG = 16,
+             // Overflow / Neural-HMM (overflow.cu): the BiLSTM time step, the LSTMCell, a GEMV layer, the frame epilogue
+             DISPATCH_LSTM_BI = 18, DISPATCH_LSTM_CELL = 19, DISPATCH_HMM_LINEAR = 20, DISPATCH_HMM_STEP = 21 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -178,18 +178,35 @@ struct SpeakerEncoder {
             void* ws, size_t ws_bytes, cudaStream_t st) const;
 };
 
-// Glow-TTS inference (glow_tts.cu): encoder (optional prenet, transformer without relative terms, LayerNorm type "1"),
-// duration predictor on cat(x, g), then -- after the caller's one host read of max(y_lengths) -- the expanded prior and
-// the Glow decoder in reverse.  The decoder works on the squeezed latent [B, C*num_squeeze, Tq] (Tq = frames /
-// num_squeeze, padded to a multiple of 4 for the tensor-core convs, masked zero beyond); each block is start 1x1 ->
-// WaveNet -> end 1x1, then one elementwise pass for the inverse affine coupling, InvConvNear^-1 and ActNorm^-1.
-struct GlowTTS {
-    struct Prenet { ConvLayer conv; float *g = nullptr, *b = nullptr; };
+// The Glow decoder in reverse (glow_tts.cu; TTS/tts/layers/glow_tts/decoder.py:113-137), shared by Glow-TTS and
+// Overflow.  It works on the squeezed latent [B, C*num_squeeze, Tq] (Tq: squeezed frames padded to a multiple of 4 for
+// the tensor-core convs, masked zero beyond); each block is start 1x1 -> WaveNet -> end 1x1, then one elementwise pass
+// for the inverse affine coupling, InvConvNear^-1 and ActNorm^-1.  The last block writes the unsqueezed mel
+// [B, C, Tv * num_squeeze].
+struct GlowDecoder {
     struct Block {
         ConvLayer start, end;
         WaveNet wn;
         float *mix = nullptr, *an_bias = nullptr, *an_logs = nullptr;   // inverse InvConvNear weight [ns][ns], ActNorm
     };
+    int Cs = 0, Hd = 0, ns = 0, nsq = 0, sigmoid_scale = 0;   // Cs: squeezed channels out_channels * num_squeeze
+    std::vector<Block*> blocks;
+    ~GlowDecoder();
+    // w: per block ActNorm logs, bias, InvConvNear^-1, start.w, .b, WaveNet, end.w, .b (see b200tts_glow_tts_config)
+    int init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
+             int cond_channels, int num_splits, int num_squeeze, int sigmoid_scale, const float* const* w, int* consumed);
+    size_t workspace_bytes(int B, int Tq) const;
+    // z [B, Cs, Tq] (overwritten), msk [B, Tq] -> mel [B, C, Tv * num_squeeze]
+    int reverse(float* z, const float* msk, const float* g, int B, int Tq, int Tv, float* mel, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+};
+
+// Glow-TTS inference (glow_tts.cu): encoder (optional prenet, transformer without relative terms, LayerNorm type "1"),
+// duration predictor on cat(x, g), then -- after the caller's one host read of max(y_lengths) -- the expanded prior and
+// the Glow decoder in reverse.  Squeeze is folded into the kernel that builds the latent, unsqueeze into the last
+// block's elementwise pass.
+struct GlowTTS {
+    struct Prenet { ConvLayer conv; float *g = nullptr, *b = nullptr; };
     b200tts_glow_tts_config c;
     int Cs = 0;                        // squeezed channels out_channels * num_squeeze
     float* emb = nullptr;
@@ -197,7 +214,7 @@ struct GlowTTS {
     ConvLayer prenet_proj, proj;       // proj: [proj_m | proj_s] rows (proj_s all zero when mean_only)
     std::vector<TextEncoder::Layer*> layers;
     DurPred dp;
-    std::vector<Block*> blocks;
+    GlowDecoder dec;
     ~GlowTTS();
     int init(const b200tts_glow_tts_config& cfg, const float* const* w, int nw);
     int tq(int Ty) const { return (Ty / c.num_squeeze + 3) / 4 * 4; }
@@ -209,6 +226,37 @@ struct GlowTTS {
     int decode(const float* o_stats, const float* x_mask, const float* cum, const long long* y_lengths, const float* g,
                const float* noise, float noise_scale, int B, int Tt, int Ty, float* attn, float* y_mean,
                float* y_log_scale, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
+};
+
+// Overflow / Neural-HMM inference (overflow.cu).  encode: embedding, 3 x (conv k5 with BatchNorm folded -> ReLU), the
+// LSTM input projection of both directions as one 1x1 conv, then one BiLSTM launch per time step (lstm_bi); the encoder
+// states [B, Tt*spp, E] and the hoisted encoder-state part of the output net's first layer (W_z z + b for every state).
+// sample: the autoregressive loop, chunk_frames frames per CUDA graph replay, one host read per chunk.  decode
+// (Overflow only): the Glow decoder in reverse and x * std + mean.
+struct Overflow {
+    b200tts_overflow_config c;
+    int H = 0;                         // LSTM hidden size per direction: E / 2 * state_per_phone
+    int O1 = 0;                        // output-net first-layer width
+    float* emb = nullptr;
+    ConvLayer convs[8], lstm_in, zproj;
+    float *whh = nullptr;              // [2][4H][H]
+    std::vector<float*> prenet_w;      // [P][in] (no bias)
+    float *mem_wih = nullptr, *mem_whh = nullptr, *mem_b = nullptr;   // [4M][P], [4M][M], b_ih + b_hh
+    std::vector<float*> out_w, out_b;  // layer 0: the h part [O1][M]; layers 1..: [O_l][O_{l-1}]; last [2C+1][O_last]
+    float *go = nullptr, *mean = nullptr, *std_ = nullptr;   // go_tokens [ar_order], mean / std [C]
+    GlowDecoder dec;
+    ~Overflow();
+    int init(const b200tts_overflow_config& cfg, const float* const* w, int nw);
+    int tq(int F) const { return (F / c.num_squeeze + 3) / 4 * 4; }
+    size_t persist_bytes(int B, int Tt) const;     // zc and the loop state, kept from encode to sample
+    size_t workspace_bytes(int B, int Tt, int F) const;
+    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* states, void* ws,
+               size_t ws_bytes, cudaStream_t st) const;
+    int sample(const long long* lengths, int B, int Tt, float temp, int max_frames, float threshold, const float* noise,
+               const unsigned char* drop, int chunk_frames, float* hmm_out, int* states_travelled, int* frames,
+               void* ws, size_t ws_bytes, cudaStream_t st) const;
+    int decode(const float* hmm_out, const int* frames, int B, int F, int Fpitch, float* mel, void* ws, size_t ws_bytes,
+               cudaStream_t st) const;
 };
 
 // ForwardTTS inference (forward_tts.cu): FastPitch / FastSpeech / FastSpeech2 with FFTransformer encoder and decoder.

@@ -116,11 +116,86 @@ GlowTTS::~GlowTTS() {
         for (float* p : {l->ln1_g, l->ln1_b, l->ln2_g, l->ln2_b}) if (p) cudaFree(p);
         delete l;
     }
+}
+
+GlowDecoder::~GlowDecoder() {
     for (auto* b : blocks) {
         free_conv(b->start); free_conv(b->end);
         for (float* p : {b->mix, b->an_bias, b->an_logs}) if (p) cudaFree(p);
         delete b;
     }
+}
+
+int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
+                      int cond_channels, int num_splits, int num_squeeze, int sigmoid, const float* const* w,
+                      int* consumed) {
+    Cs = out_channels * num_squeeze;
+    Hd = hidden; ns = num_splits; nsq = num_squeeze; sigmoid_scale = sigmoid;
+    B200_REQUIRE(ns >= 2 && ns % 2 == 0 && ns <= MAX_SPLITS && Cs % ns == 0,
+                 "glow decoder: num_splits %d must be even, <= %d and divide out_channels * num_squeeze = %d", ns,
+                 MAX_SPLITS, Cs);
+    const int per_block = 3 + 2 + (cond_channels > 0 ? 2 : 0) + 4 * num_layers + 2;
+    int rc;
+    for (int n = 0; n < num_blocks; ++n) {
+        const float* const* p = w + n * per_block;
+        Block* b = new Block();
+        blocks.push_back(b);
+        if ((rc = upload(&b->an_logs, p[0], Cs))) return rc;
+        if ((rc = upload(&b->an_bias, p[1], Cs))) return rc;
+        if ((rc = upload(&b->mix, p[2], (size_t)ns * ns))) return rc;
+        b->start.tc_prec = b->end.tc_prec = B200TTS_PRECISION_FP32;
+        if ((rc = pack_conv(b->start, p[3], p[4], Hd, Cs / 2, 1, 1, 0))) return rc;
+        int used = 0;
+        if ((rc = b->wn.init(Hd, kernel_size, dilation_rate, num_layers, cond_channels, p + 5, &used))) return rc;
+        if ((rc = pack_conv(b->end, p[5 + used], p[6 + used], Cs, Hd, 1, 1, 0))) return rc;
+    }
+    *consumed = per_block * num_blocks;
+    return 0;
+}
+
+size_t GlowDecoder::workspace_bytes(int B, int Tq) const {
+    return 2 * arena_bytes((size_t)B * Cs * Tq) + 3 * arena_bytes((size_t)B * Hd * Tq) +
+           arena_bytes((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
+}
+
+int GlowDecoder::reverse(float* z, const float* msk, const float* g, int B, int Tq, int Tv, float* mel, void* ws,
+                         size_t ws_bytes, cudaStream_t st) const {
+    Arena ar(ws, ws_bytes);
+    float* zb = ar.f32((size_t)B * Cs * Tq);
+    float* eo = ar.f32((size_t)B * Cs * Tq);
+    float* h = ar.f32((size_t)B * Hd * Tq);
+    float* acts = ar.f32((size_t)B * Hd * Tq);
+    float* out = ar.f32((size_t)B * Hd * Tq);
+    float* condv = ar.f32((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
+    B200_REQUIRE(zb && eo && h && acts && out && condv, "glow decoder: arena exhausted");
+    int rc;
+    const long long zbs = (long long)Cs * Tq, hbs = (long long)Hd * Tq;
+    float* cur = z;
+    float* nxt = zb;
+    for (int n = (int)blocks.size() - 1; n >= 0; --n) {   // reversed(flows): coupling, InvConvNear, ActNorm per block
+        const Block& bl = *blocks[n];
+        {   // h = start(x0) * mask
+            ConvIO io;
+            io.x = cur; io.x_bs = zbs; io.x_cs = Tq; io.Tin = Tq;
+            io.y = h; io.y_bs = hbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
+            io.ymask = msk; io.ymask_bs = Tq; io.flags = EPI_MASK_POST;
+            if ((rc = launch_conv(bl.start, io, st))) return rc;
+        }
+        if ((rc = bl.wn.forward(h, out, msk, g, B, Tq, acts, condv, st))) return rc;
+        {   // [t | s] = end(WN(h))
+            ConvIO io;
+            io.x = out; io.x_bs = hbs; io.x_cs = Tq; io.Tin = Tq;
+            io.y = eo; io.y_bs = zbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
+            if ((rc = launch_conv(bl.end, io, st))) return rc;
+        }
+        dim3 grid((Tq + 127) / 128, Cs / ns, B);
+        flow_step_kernel<<<grid, 128, 0, st>>>(cur, eo, msk, bl.mix, bl.an_bias, bl.an_logs, n > 0 ? nxt : mel, Cs, Tq,
+                                               ns, sigmoid_scale, n > 0 ? 0 : nsq, Tv);
+        count_launch();
+        B200_CUDA_OK(cudaGetLastError());
+        std::swap(cur, nxt);
+    }
+    return 0;
 }
 
 int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int nw) {
@@ -191,19 +266,10 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
         if ((rc = dp.init(dc, w + i, 10))) return rc;
         i += 10;
     }
-    for (int n = 0; n < c.num_flow_blocks; ++n, i += per_block) {
-        const float* const* p = w + i;
-        Block* b = new Block();
-        blocks.push_back(b);
-        if ((rc = upload(&b->an_logs, p[0], Cs))) return rc;
-        if ((rc = upload(&b->an_bias, p[1], Cs))) return rc;
-        if ((rc = upload(&b->mix, p[2], (size_t)ns * ns))) return rc;
-        b->start.tc_prec = b->end.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(b->start, p[3], p[4], Hd, Cs / 2, 1, 1, 0))) return rc;
-        int used = 0;
-        if ((rc = b->wn.init(Hd, c.kernel_size_dec, c.dilation_rate, c.num_block_layers, cin, p + 5, &used))) return rc;
-        if ((rc = pack_conv(b->end, p[5 + used], p[6 + used], Cs, Hd, 1, 1, 0))) return rc;
-    }
+    int used = 0;
+    if ((rc = dec.init(C, Hd, c.kernel_size_dec, c.dilation_rate, c.num_flow_blocks, c.num_block_layers, cin, ns, nsq,
+                       c.sigmoid_scale, w + i, &used)))
+        return rc;
     return 0;
 }
 
@@ -215,9 +281,8 @@ size_t GlowTTS::encode_bytes(int B, int Tt) const {
 }
 
 size_t GlowTTS::decode_bytes(int B, int Ty) const {
-    const int Tq = tq(Ty), Hd = c.hidden_channels_dec;
-    return 3 * arena_bytes((size_t)B * Cs * Tq) + 3 * arena_bytes((size_t)B * Hd * Tq) +
-           arena_bytes((size_t)B * blocks[0]->wn.cond.RowsPad + 64) + arena_bytes((size_t)B * Tq) + 1024;
+    const int Tq = tq(Ty);
+    return arena_bytes((size_t)B * Cs * Tq) + arena_bytes((size_t)B * Tq) + dec.workspace_bytes(B, Tq) + 1024;
 }
 
 int GlowTTS::encode(const long long* tokens, const long long* lengths, const float* g, float length_scale, int B,
@@ -325,7 +390,7 @@ int GlowTTS::decode(const float* o_stats, const float* x_mask, const float* cum,
     B200_REQUIRE((c.c_in_channels > 0) == (g != nullptr), "glow_tts_decode: g must be given iff c_in_channels > 0");
     B200_REQUIRE(ws_bytes >= decode_bytes(B, Ty), "glow_tts_decode: workspace too small");
     if (B == 0 || Ty == 0) return 0;
-    const int C = c.out_channels, nsq = c.num_squeeze, ns = c.num_splits, Hd = c.hidden_channels_dec;
+    const int C = c.out_channels, nsq = c.num_squeeze;
     int rc;
     // path and expanded prior (:355-359): attn, y_mean = attn^T o_mean, y_log_scale = attn^T o_log_scale
     if ((rc = launch_expand_prior(cum, x_mask, y_lengths, o_stats, nullptr, 0.f, B, Tt, Ty, C, attn, y_mean, y_log_scale,
@@ -335,14 +400,8 @@ int GlowTTS::decode(const float* o_stats, const float* x_mask, const float* cum,
     if (Tv == 0) return 0;
     Arena ar(ws, ws_bytes);
     float* za = ar.f32((size_t)B * Cs * Tq);
-    float* zb = ar.f32((size_t)B * Cs * Tq);
-    float* eo = ar.f32((size_t)B * Cs * Tq);
-    float* h = ar.f32((size_t)B * Hd * Tq);
-    float* acts = ar.f32((size_t)B * Hd * Tq);
-    float* out = ar.f32((size_t)B * Hd * Tq);
-    float* condv = ar.f32((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
     float* msk = ar.f32((size_t)B * Tq);
-    B200_REQUIRE(za && zb && eo && h && acts && out && condv && msk, "glow_tts_decode: arena exhausted");
+    B200_REQUIRE(za && msk, "glow_tts_decode: arena exhausted");
     {
         dim3 grid((Tq + 127) / 128, Cs, B);
         squeeze_prior_kernel<<<grid, 128, 0, st>>>(y_mean, y_log_scale, noise_scale != 0.f ? noise : nullptr,
@@ -350,33 +409,7 @@ int GlowTTS::decode(const float* o_stats, const float* x_mask, const float* cum,
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
     }
-    const long long zbs = (long long)Cs * Tq, hbs = (long long)Hd * Tq;
-    float* cur = za;
-    float* nxt = zb;
-    for (int n = c.num_flow_blocks - 1; n >= 0; --n) {   // reversed(flows): coupling, InvConvNear, ActNorm per block
-        const Block& bl = *blocks[n];
-        {   // h = start(x0) * mask
-            ConvIO io;
-            io.x = cur; io.x_bs = zbs; io.x_cs = Tq; io.Tin = Tq;
-            io.y = h; io.y_bs = hbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
-            io.ymask = msk; io.ymask_bs = Tq; io.flags = EPI_MASK_POST;
-            if ((rc = launch_conv(bl.start, io, st))) return rc;
-        }
-        if ((rc = bl.wn.forward(h, out, msk, g, B, Tq, acts, condv, st))) return rc;
-        {   // [t | s] = end(WN(h))
-            ConvIO io;
-            io.x = out; io.x_bs = hbs; io.x_cs = Tq; io.Tin = Tq;
-            io.y = eo; io.y_bs = zbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
-            if ((rc = launch_conv(bl.end, io, st))) return rc;
-        }
-        dim3 grid((Tq + 127) / 128, Cs / ns, B);
-        flow_step_kernel<<<grid, 128, 0, st>>>(cur, eo, msk, bl.mix, bl.an_bias, bl.an_logs, n > 0 ? nxt : mel, Cs, Tq,
-                                               ns, c.sigmoid_scale, n > 0 ? 0 : nsq, Tv);
-        count_launch();
-        B200_CUDA_OK(cudaGetLastError());
-        std::swap(cur, nxt);
-    }
-    return 0;
+    return dec.reverse(za, msk, g, B, Tq, Tv, mel, ar.base + ar.off, ar.cap - ar.off, st);
 }
 
 }  // namespace b200tts
