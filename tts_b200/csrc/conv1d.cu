@@ -465,10 +465,10 @@ void free_conv(ConvLayer& L) {
 // loader copies with one cp.async.bulk, [slabs][128 MMA rows][16 B], slab s holding the chunk's channels s*SLC .. +SLC-1:
 //   3xTF32 (PREC_FP32): 8-channel chunks, {hi, lo}[2 slabs] of 4 floats, hi = v & 0xFFFFE000 (exact in TF32), lo = v - hi
 //   bf16 / fp16:        16-channel chunks, [2 slabs] of 8 values rounded to nearest even (as cvt.rn rounds the activations)
-//   PREC_F16X3:         16-channel chunks, {hi, lo, hs}[2 slabs] of 8 fp16 values of the scaled row w' = w * 2^e_r (e_r puts
-//                       the row's max |w'| in [2^14, 2^15); all-zero rows: e_r = 0): hi = fp16(w'), lo = fp16(w' - hi),
-//                       hs = hi * 2^-11 (exact unless it falls below fp16's normal range, 2^17 under the row's max); the
-//                       kernel's epilogue multiplies by rscale[r] = 2^-e_r, which the first call returns in *rscale
+//   PREC_F16X3:         16-channel chunks, {hi, lo}[2 slabs] of 8 fp16 values of the scaled row w' = w * 2^e_r (e_r puts
+//                       the row's max |w'| in [2^14, 2^15); all-zero rows: e_r = 0): hi = fp16(w'), lo = fp16(w' - hi);
+//                       the kernel makes the third operand, fp16(hi * 2^-11), from hi in registers, and its epilogue
+//                       multiplies by rscale[r] = 2^-e_r, which the first call returns in *rscale
 // With G tap groups (1: plain; 128 / rows: grouped), MMA row m = g * (128 / G) + co of tile t carries weight row
 // t * 128 + co and, in tap block j, tap G * j + g.  Rows >= `rows`, taps >= K and channels >= Cin are zero.  The weight
 // norm is already folded (in fp32) into Wl; each weight is rounded once, here.
@@ -477,7 +477,7 @@ static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, 
     const bool tf32 = prec == tc::PREC_FP32, x3 = prec == tc::PREC_F16X3;
     const int kc = tf32 ? tc3::KC2 : tc3::KC16, slc = kc / 2, ch = tc3::MROWS / G;
     const int ntiles = (rows + tc3::MROWS - 1) / tc3::MROWS, nchunks = (Cin + kc - 1) / kc, J = (K + G - 1) / G;
-    const size_t slab = (size_t)tc3::MROWS * 16, blk = (tf32 ? 4 : x3 ? 6 : 2) * slab;
+    const size_t slab = (size_t)tc3::MROWS * 16, blk = (tf32 || x3 ? 4 : 2) * slab;
     std::vector<unsigned char> img((size_t)ntiles * nchunks * J * blk, 0);
     std::vector<float> up(x3 ? rows : 0, 1.f), down(x3 ? rows : 0, 1.f);   // 2^e_r, 2^-e_r
     for (int r = 0; r < (x3 ? rows : 0); ++r) {
@@ -514,10 +514,8 @@ static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, 
                             const float ws = v * up[r];
                             const __half hi = __float2half_rn(ws);
                             const __half lo = __float2half_rn(ws - __half2float(hi));
-                            const __half hs = __float2half_rn(__half2float(hi) * (1.f / 2048.f));
                             memcpy(p + 2 * e, &hi, 2);
                             memcpy(p + 2 * slab + 2 * e, &lo, 2);
-                            memcpy(p + 4 * slab + 2 * e, &hs, 2);
                         } else if (prec == tc::PREC_BF16) {
                             const __nv_bfloat16 h = __float2bfloat16_rn(v);
                             memcpy(p + 2 * e, &h, 2);

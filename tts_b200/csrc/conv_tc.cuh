@@ -23,7 +23,8 @@
 // 3-product fp16 split (PREC_F16X3, the HiFiGAN decoder's default): fp16 has TF32's 11-bit significand and twice its MMA
 // rate, so the same hi/lo split costs 3 m64n256k16 MMAs per 16 channels instead of 6 m64n256k8.  fp16's small range is
 // handled by scaling: weight row r is multiplied by 2^e_r (max |w'| in [2^14, 2^15)) at pack time and stored as W_hi =
-// fp16(w'), W_lo = fp16(w' - W_hi), W_hs = W_hi * 2^-11; activations are split as X_hi = fp16(x), X_lo = fp16((x - X_hi)
+// fp16(w'), W_lo = fp16(w' - W_hi); the kernel makes W_hs = fp16(W_hi * 2^-11) from W_hi in registers (register-A MMA,
+// wgmma_f16_m64n256_rs); activations are split as X_hi = fp16(x), X_lo = fp16((x - X_hi)
 // * 2^11) (subtraction and scaling exact).  D' = W_hs*X_lo + W_lo*X_hi + W_hi*X_hi = 2^e_r * D to 2^-22 relative, and the
 // epilogue multiplies row r by 2^-e_r (exact) before the bias.  |x| >= 65504 cannot be represented: the producers report
 // it (ERR_RANGE) instead of multiplying an inf.
@@ -143,6 +144,33 @@ __device__ __forceinline__ void wgmma_f16_m64n256(float* d, uint64_t adesc, uint
         : B200_WGMMA_D128_OPS(d)
         : "l"(adesc), "l"(bdesc), "r"(acc)
         : "memory");
+}
+// The fp16 tile with A from registers: a[0..3] is the warp's m16k16 fragment of its 16 rows (warp w of the warpgroup:
+// rows 16 w ..), in mma.m16n8k16's A layout -- ldsm_x4's result.  The registers are read while the MMA is in flight:
+// they must not be rewritten before the wgmma_wait that retires its group.
+__device__ __forceinline__ void wgmma_f16_m64n256_rs(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " B200_WGMMA_D128
+        " {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n}"
+        : B200_WGMMA_D128_OPS(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc)
+        : "memory");
+}
+
+// Four 8x8 b16 matrices from shared memory; lane l gives the address of row l % 8 of matrix l / 8, and r[i] is matrix
+// i's element pair (row lane / 4, columns 2 (lane % 4) ..).  Matrices {rows 0-7, rows 8-15} x {k 0-7, k 8-15} in that
+// order form an m16k16 A fragment.
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+// two fp16 values times 2^-11, one round to nearest even (subnormal results kept): fp16(W_hi * 2^-11), as pack_tc's
+// __float2half_rn(__half2float(hi) / 2048) rounds the exact product
+__device__ __forceinline__ uint32_t f16x2_times_2m11(uint32_t v) {
+    uint32_t r;
+    asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(r) : "r"(v), "r"(0x10001000u));
+    return r;
 }
 
 // two fp32 values -> one register of two 16-bit values, round to nearest even; `lo` goes to the lower address

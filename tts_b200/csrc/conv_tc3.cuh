@@ -20,9 +20,12 @@
 // PREC = PREC_F16X3: the 3-product fp16 split (conv_tc.cuh).  A chunk is 16 input channels, but the raw ring keeps the
 // FP32 kernel's 8-channel stages: the producers fill one activation stage {X_hi[2 slabs], X_lo[2 slabs]} from two raw
 // stages, one slab of each per raw stage, and arrive on it after the second; they also report any |x| >= 65504
-// (err[ERR_RANGE]).  A weight tap block is three planes {W_hi, W_lo, W_hs}[2 slabs][128 rows][8] (12 KB) and the ring
-// holds NB3 of them, so shared memory is exactly the FP32 kernel's.  The consumers issue W_hs*X_lo, W_lo*X_hi, W_hi*X_hi
-// (m64n256k16 each) per tap and chunk; every epilogue multiplies its rows by `rscale` (2^-e_r) before the bias.
+// (err[ERR_RANGE]).  A weight tap block is two planes {W_hi, W_lo}[2 slabs][128 rows][8] (8 KB, as in 3xTF32) in the
+// same NB2-deep ring, so shared memory is exactly the FP32 kernel's.  The consumers issue W_hs*X_lo, W_lo*X_hi, W_hi*X_hi
+// (m64n256k16 each) per tap and chunk, W_hs = W_hi * 2^-11 built in registers: each warp loads its 16 rows of W_hi with
+// one ldmatrix.x4, scales them and issues that MMA with A from registers as a commit group of its own, so the wait that
+// retires the previous tap also frees the fragment registers for the next one (a second fragment set does not fit the
+// 168 registers).  Every epilogue multiplies its rows by `rscale` (2^-e_r) before the bias.
 //
 // Grouped mode (GRP = 2 / 4) for narrow layers (exactly 64 / 32 output rows, the last two HiFiGAN stages): the 128
 // MMA rows are GRP tap-groups x (128/GRP) channels -- row g * (128/GRP) + c carries the weights of channel c for taps
@@ -49,8 +52,7 @@ constexpr int RAWS = 324;         // raw (cp.async) row stride in floats: the wi
                                   // that the transform's shared loads use immediate offsets
 constexpr int NRAW = 3;           // raw (cp.async) ring depth
 constexpr int NA2 = 2;            // transformed activation stages
-constexpr int NB2 = 3;            // weight ring depth (one 8 KB tap block per slot)
-constexpr int NB3 = 2;            // PREC_F16X3 weight ring depth (one 12 KB tap block per slot)
+constexpr int NB2 = 3;            // weight ring depth (one tap block per slot: 8 KB, 16-bit operands 4 KB)
 constexpr int ACC_LD = 260;       // row stride (floats) of the shared accumulator tile: float4 reads of 8 rows are conflict free
 constexpr int ACC_BYTES = MROWS * ACC_LD * 4;
 constexpr int NPW = 3;            // producer warps
@@ -63,7 +65,7 @@ struct Tc3Args {
     const float* x; long long x_bs; int x_cs; int Tin;
     float in_slope;
     const void* w;             // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32 (16-bit: [2][128][8];
-                               // PREC_F16X3: {hi, lo, hs}[2][128][8] fp16)
+                               // PREC_F16X3: {hi, lo}[2][128][8] fp16)
     const float* rscale;       // PREC_F16X3: [Rows] 2^-e_r, the inverse of the pack-time row scaling (see pack_tc)
     const float* bias;
     const float* cond; long long cond_bs;
@@ -115,11 +117,11 @@ __device__ __forceinline__ int near_col(int t, int src, int dst, float scale) {
 }
 
 // prec: PREC_FP32 (8-channel chunks, hi/lo slab pairs), a 16-bit type (16-channel chunks, two slabs) or PREC_F16X3
-// (16-channel chunks over 8-channel raw stages, hi/lo slab pairs, three-plane weight blocks: the FP32 kernel's total)
+// (16-channel chunks over 8-channel raw stages, hi/lo slab pairs: the FP32 kernel's total)
 static inline size_t smem_bytes3(int rows_pad, int prec = PREC_FP32) {
-    const bool b16 = prec == PREC_BF16 || prec == PREC_FP16, x3 = prec == PREC_F16X3;
-    const size_t raw_ch = b16 ? KC16 : KC2, nsl = b16 ? 2 : 4, wsl = x3 ? 6 : nsl, nb = x3 ? NB3 : NB2;
-    return (size_t)NRAW * raw_ch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + nb * (wsl * MROWS * 16) + ACC_BYTES + 512;
+    const bool b16 = prec == PREC_BF16 || prec == PREC_FP16;
+    const size_t raw_ch = b16 ? KC16 : KC2, nsl = b16 ? 2 : 4;
+    return (size_t)NRAW * raw_ch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + NB2 * (nsl * MROWS * 16) + ACC_BYTES + 512;
 }
 static inline size_t ragged_table_bytes(int B) { return ((size_t)(B + 1) * sizeof(int) + 15) / 16 * 16; }
 
@@ -513,14 +515,13 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     constexpr int SPC = KCH / RCH;               // raw stages per chunk (2 for X3)
     constexpr int NSL = B16 ? 2 : 4;             // 16-byte slabs per activation stage: two 16-bit slabs, or hi[2] + lo[2]
     constexpr int SLC = PREC != PREC_FP32 ? 8 : 4;   // channels per slab row
-    constexpr int NWS = X3 ? 6 : NSL;            // slabs per weight tap block (X3: hi[2], lo[2], hs[2])
-    constexpr int NB = X3 ? NB3 : NB2;           // weight ring depth
+    constexpr int NB = NB2;                      // weight ring depth
     constexpr bool SC = X3;                      // epilogues scale rows by rscale
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ROWS = a.rows_pad, RAWW = a.raw_w, K = a.KJ;
     const uint32_t rawStage = (uint32_t)RCH * RAWS * 4;
     const uint32_t slabA = (uint32_t)ROWS * 16, stageA = NSL * slabA;
-    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NWS * slabB;   // one tap block: [NWS slabs][128 rows][16 B]
+    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NSL * slabB;   // one tap block: [NSL slabs][128 rows][16 B]
     unsigned char* smRaw = smem;
     unsigned char* smA = smRaw + NRAW * rawStage;
     unsigned char* smB = smA + NA2 * stageA;
@@ -825,7 +826,9 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         const int wg = warp >> 2, lq = warp & 3, half = warp >> 2;
         const uint64_t wdesc0 = make_desc(smem_u32(smB) + (uint32_t)wg * 64 * 16, slabB);   // this warpgroup's 64 weight rows
         const uint64_t wlo_off = (uint64_t)((2 * slabB) >> 4), wslot = (uint64_t)(stageB >> 4);
-        const uint64_t whs_off = (uint64_t)((4 * slabB) >> 4);                             // X3: the W_hs plane
+        // X3: this lane's ldmatrix row of W_hi in slot 0: matrix lane / 8 is rows {0-7, 8-15} x slab {0, 1} of the warp's
+        // 16 MMA rows (16 warp ..), so the x4 load is the m16k16 A fragment; each 8-lane phase reads 128 contiguous bytes
+        const uint32_t whi_lds = smem_u32(smB) + (uint32_t)(lane >> 4) * slabB + (uint32_t)(warp * 16 + (lane & 15)) * 16;
         const uint64_t xstep = (uint64_t)a.dil_blk;                                          // B rows per tap block (16 B each)
         bool ok = true;
         int sa = 0; uint32_t pa = 0;                                                         // activation stage / its parity
@@ -858,13 +861,22 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     if (ok) ok = mbar_wait(BAR(B_FULL + sb), pb, a.err);
                     if (ok) {
                         const uint64_t w_hi = wdesc0 + (uint64_t)sb * wslot, w_lo = w_hi + wlo_off;
+                        uint32_t whs[4];                                         // X3: W_hs = W_hi * 2^-11
+                        if constexpr (X3) {
+                            ldsm_x4(whs, whi_lds + (uint32_t)sb * stageB);
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) whs[i] = f16x2_times_2m11(whs[i]);
+                        }
                         wgmma_fence();
                         if constexpr (PREC == PREC_BF16) {
                             wgmma_bf16_m64n256(d, w_hi, xh, acc);
                         } else if constexpr (PREC == PREC_FP16) {
                             wgmma_f16_m64n256(d, w_hi, xh, acc);
                         } else if constexpr (X3) {
-                            wgmma_f16_m64n256(d, w_hi + whs_off, xl, acc);      // small terms first
+                            wgmma_f16_m64n256_rs(d, whs, xl, acc);              // small terms first
+                            // a group of its own, retired by the wait below: the next tap rewrites whs while only
+                            // this tap's two descriptor MMAs are in flight
+                            wgmma_commit();
                             wgmma_f16_m64n256(d, w_lo, xh, 1u);
                             wgmma_f16_m64n256(d, w_hi, xh, 1u);
                         } else {
