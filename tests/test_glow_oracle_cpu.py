@@ -206,3 +206,11 @@ def test_error_behaviour():
     if not torch.cuda.is_available():
         with pytest.raises(RuntimeError, match="no CPU path"):
             m.inference(x, {"x_lengths": torch.tensor([5])})
+
+
+@pytest.mark.parametrize("extra", [{"rel_attn_window_size": 4}, {"layer_norm_type": "2"}, {"input_length": 10}])
+def test_encoder_params_outside_the_engine_config(extra):
+    """The shared RelativePositionTransformer builds a window and type "2"; Glow-TTS's engine has neither."""
+    cfg = GlowTTSConfig(num_chars=40, **dict(SMALL, encoder_params=dict(SMALL["encoder_params"], **extra)))
+    with pytest.raises(NotImplementedError, match="relative window"):
+        GlowTTS(cfg)

@@ -100,15 +100,34 @@ int launch_embed(const long long* tokens, const long long* lengths, const float*
 int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
                      int C, int T, int num_heads, int window, cudaStream_t st);
 
-struct TextEncoder {
+// RelativePositionTransformer (text_encoder.cu; TTS/tts/layers/glow_tts/transformer.py:322-432) on the exact FP32 FMA
+// conv, shared by the VITS text encoder (window 4, LayerNorm type "2": eps 1e-5) and Glow-TTS (no window, type "1":
+// eps 1e-4).  Per layer: fused q|k|v 1x1, attention, conv_o, add+LayerNorm, k-tap FFN with same padding, add+LayerNorm
+// with the mask folded in.  Layer is also ForwardTTS's FFTransformer layer (without rel_k / rel_v).
+struct RelPosTransformer {
     struct Layer {
         ConvLayer qkv, o, ffn1, ffn2;
         float *rel_k = nullptr, *rel_v = nullptr, *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
+        ~Layer();
     };
-    b200tts_text_encoder_config c;
-    int C = 0, d = 0;
-    float* emb = nullptr;
+    int C = 0, F = 0, heads = 0, window = -1;   // window < 0: no relative-position terms
+    float eps = 0.f;
     std::vector<Layer*> layers;
+    ~RelPosTransformer();
+    // w per layer: emb_rel_k [1,2w+1,d], emb_rel_v (window >= 0 only), conv_q.w/.b, conv_k.w/.b, conv_v.w/.b,
+    // conv_o.w/.b, norm_1.gamma/.beta, ffn.conv_1.w/.b, ffn.conv_2.w/.b, norm_2.gamma/.beta
+    int init(int channels, int ffn_channels, int kernel_size, int num_heads, int window, float eps, int num_layers,
+             const float* const* w, int* consumed);
+    size_t workspace_bytes(int B, int T) const;   // q|k|v, attention output, y, FFN hidden
+    // x [B, C, T], already masked: every layer in place; x is left masked
+    int forward(float* x, const float* x_mask, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const;
+};
+
+struct TextEncoder {
+    b200tts_text_encoder_config c;
+    int C = 0;
+    float* emb = nullptr;
+    RelPosTransformer tf;
     ConvLayer proj;
     ~TextEncoder();
     int init(const b200tts_text_encoder_config& cfg, const float* const* w, int nw);
@@ -201,7 +220,7 @@ struct GlowDecoder {
                 cudaStream_t st) const;
 };
 
-// Glow-TTS inference (glow_tts.cu): encoder (optional prenet, transformer without relative terms, LayerNorm type "1"),
+// Glow-TTS inference (glow_tts.cu): encoder (optional prenet, RelPosTransformer without a window, LayerNorm type "1"),
 // duration predictor on cat(x, g), then -- after the caller's one host read of max(y_lengths) -- the expanded prior and
 // the Glow decoder in reverse.  Squeeze is folded into the kernel that builds the latent, unsqueeze into the last
 // block's elementwise pass.
@@ -212,7 +231,7 @@ struct GlowTTS {
     float* emb = nullptr;
     std::vector<Prenet> prenet;
     ConvLayer prenet_proj, proj;       // proj: [proj_m | proj_s] rows (proj_s all zero when mean_only)
-    std::vector<TextEncoder::Layer*> layers;
+    RelPosTransformer tf;
     DurPred dp;
     GlowDecoder dec;
     ~GlowTTS();
@@ -265,10 +284,7 @@ struct Overflow {
 // output with the positional encoding and runs the decoder on the 3xTF32 tensor-core convs and attention_tc3.cu.
 // Decoder tensors are [B, C, Tp] with Tp = frames rounded up to 4 (16-byte rows); every row stops at its y_length.
 struct ForwardTTS {
-    struct Layer {   // FFTransformer (TTS/tts/layers/generic/transformer.py:6-35)
-        ConvLayer qkv, o, ffn1, ffn2;
-        float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
-    };
+    using Layer = RelPosTransformer::Layer;   // FFTransformer (TTS/tts/layers/generic/transformer.py:6-35)
     b200tts_forward_tts_config c;
     float* emb = nullptr;
     float* pe = nullptr;               // pos_encoder.pe [C][pe_len] (null without positional encoding)

@@ -136,12 +136,6 @@ int pack_layer(ForwardTTS::Layer& L, const float* const* p, int C, int F, int pr
     return upload(&L.ln2_b, p[11], C);
 }
 
-void free_layer(ForwardTTS::Layer* L) {
-    free_conv(L->qkv); free_conv(L->o); free_conv(L->ffn1); free_conv(L->ffn2);
-    for (float* p : {L->ln1_g, L->ln1_b, L->ln2_g, L->ln2_b}) if (p) cudaFree(p);
-    delete L;
-}
-
 constexpr int PER_LAYER = 12;
 
 }  // namespace
@@ -149,8 +143,8 @@ constexpr int PER_LAYER = 12;
 ForwardTTS::~ForwardTTS() {
     if (emb) cudaFree(emb);
     if (pe) cudaFree(pe);
-    for (auto* l : enc) free_layer(l);
-    for (auto* l : dec) free_layer(l);
+    for (auto* l : enc) delete l;
+    for (auto* l : dec) delete l;
     free_conv(proj_g); free_conv(pitch_emb); free_conv(energy_emb); free_conv(postnet);
 }
 

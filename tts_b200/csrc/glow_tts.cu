@@ -111,11 +111,6 @@ GlowTTS::~GlowTTS() {
     for (auto& p : prenet) { free_conv(p.conv); if (p.g) cudaFree(p.g); if (p.b) cudaFree(p.b); }
     free_conv(prenet_proj);
     free_conv(proj);
-    for (auto* l : layers) {
-        free_conv(l->qkv); free_conv(l->o); free_conv(l->ffn1); free_conv(l->ffn2);
-        for (float* p : {l->ln1_g, l->ln1_b, l->ln2_g, l->ln2_b}) if (p) cudaFree(p);
-        delete l;
-    }
 }
 
 GlowDecoder::~GlowDecoder() {
@@ -231,24 +226,9 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
         if ((rc = pack_conv(prenet_proj, w[i], w[i + 1], H, H, 1, 1, 0))) return rc;
         i += 2;
     }
-    for (int l = 0; l < c.num_layers_enc; ++l, i += per_layer) {
-        const float* const* p = w + i;
-        TextEncoder::Layer* L = new TextEncoder::Layer();
-        layers.push_back(L);
-        std::vector<float> wq((size_t)3 * H * H), bq((size_t)3 * H);   // fused QKV: rows [q | k | v]
-        for (int s = 0; s < 3; ++s) {
-            memcpy(wq.data() + (size_t)s * H * H, p[2 * s], sizeof(float) * H * H);
-            memcpy(bq.data() + (size_t)s * H, p[2 * s + 1], sizeof(float) * H);
-        }
-        if ((rc = pack_conv(L->qkv, wq.data(), bq.data(), 3 * H, H, 1, 1, 0))) return rc;
-        if ((rc = pack_conv(L->o, p[6], p[7], H, H, 1, 1, 0))) return rc;
-        if ((rc = upload(&L->ln1_g, p[8], H))) return rc;
-        if ((rc = upload(&L->ln1_b, p[9], H))) return rc;
-        if ((rc = pack_conv(L->ffn1, p[10], p[11], F, H, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = pack_conv(L->ffn2, p[12], p[13], H, F, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = upload(&L->ln2_g, p[14], H))) return rc;
-        if ((rc = upload(&L->ln2_b, p[15], H))) return rc;
-    }
+    int used = 0;
+    if ((rc = tf.init(H, F, K, c.num_heads, -1, 1e-4f, c.num_layers_enc, w + i, &used))) return rc;
+    i += used;
     {   // [proj_m | proj_s]: with mean_only the log-scale rows are zero weights and bias, i.e. zeros_like(x_m) (:176)
         std::vector<float> wp((size_t)2 * C * H, 0.f), bp((size_t)2 * C, 0.f);
         memcpy(wp.data(), w[i], sizeof(float) * C * H);
@@ -266,7 +246,6 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
         if ((rc = dp.init(dc, w + i, 10))) return rc;
         i += 10;
     }
-    int used = 0;
     if ((rc = dec.init(C, Hd, c.kernel_size_dec, c.dilation_rate, c.num_flow_blocks, c.num_block_layers, cin, ns, nsq,
                        c.sigmoid_scale, w + i, &used)))
         return rc;
@@ -275,9 +254,8 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
 
 size_t GlowTTS::encode_bytes(int B, int Tt) const {
     const int H = c.hidden_channels_enc, Cg = H + c.c_in_channels;
-    return 4 * arena_bytes((size_t)B * H * Tt) + arena_bytes((size_t)B * 3 * H * Tt) +
-           arena_bytes((size_t)B * c.hidden_channels_ffn * Tt) + arena_bytes((size_t)B * Cg * Tt) +
-           arena_bytes(dp.workspace_bytes(B, Tt) / sizeof(float) + 1) + 1024;
+    return arena_bytes((size_t)B * H * Tt) + arena_bytes((size_t)B * Cg * Tt) +
+           arena_bytes(dp.workspace_bytes(B, Tt) / sizeof(float) + 1) + tf.workspace_bytes(B, Tt) + 1024;
 }
 
 size_t GlowTTS::decode_bytes(int B, int Ty) const {
@@ -293,25 +271,23 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
     B200_REQUIRE((c.c_in_channels > 0) == (g != nullptr), "glow_tts_encode: g must be given iff c_in_channels > 0");
     B200_REQUIRE(ws_bytes >= encode_bytes(B, Tt), "glow_tts_encode: workspace too small");
     if (B == 0 || Tt == 0) return 0;
-    const int H = c.hidden_channels_enc, F = c.hidden_channels_ffn, Cg = H + c.c_in_channels;
+    const int H = c.hidden_channels_enc, Cg = H + c.c_in_channels;
     Arena ar(ws, ws_bytes);
     float* x = ar.f32((size_t)B * H * Tt);
-    float* qkv = ar.f32((size_t)B * 3 * H * Tt);
-    float* att = ar.f32((size_t)B * H * Tt);
-    float* yb = ar.f32((size_t)B * H * Tt);
-    float* hb = ar.f32((size_t)B * F * Tt);
-    float* pb = ar.f32((size_t)B * H * Tt);
     float* xdp = ar.f32((size_t)B * Cg * Tt);
     const size_t dp_bytes = dp.workspace_bytes(B, Tt);
     float* dpws = ar.f32(dp_bytes / sizeof(float) + 1);
-    B200_REQUIRE(x && qkv && att && yb && hb && pb && xdp && dpws, "glow_tts_encode: arena exhausted");
+    const size_t tf_bytes = tf.workspace_bytes(B, Tt);
+    float* tfws = ar.f32(tf_bytes / sizeof(float));
+    B200_REQUIRE(x && xdp && dpws && tfws, "glow_tts_encode: arena exhausted");
     const long long bs = (long long)H * Tt;
     int rc;
     // x = emb(tokens) * sqrt(H), masked: the prenet and the transformer both start with x * x_mask
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, H, H, x, x_mask, st))) return rc;
     if (c.use_prenet) {   // glow.py:55-67: 3 x (conv(x * mask) -> LayerNorm(. * mask) -> ReLU), x = (x + proj(.)) * mask
+        Arena pa(tfws, tf_bytes);   // the prenet runs before the transformer: its buffers are the transformer's scratch
         const float* in = x;
-        float* bufs[2] = {yb, pb};
+        float* bufs[2] = {pa.f32((size_t)B * H * Tt), pa.f32((size_t)B * H * Tt)};
         for (int l = 0; l < 3; ++l) {
             float* out = bufs[l & 1];
             ConvIO io;
@@ -330,39 +306,7 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
         io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_ACCUM | EPI_MASK_POST;
         if ((rc = launch_conv(prenet_proj, io, st))) return rc;
     }
-    for (int l = 0; l < c.num_layers_enc; ++l) {   // transformer.py:418-431, the layer structure of the VITS text path
-        const TextEncoder::Layer& L = *layers[l];
-        {
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-            io.y = qkv; io.y_bs = 3 * bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L.qkv, io, st))) return rc;
-        }
-        if ((rc = launch_attention(qkv, x_mask, nullptr, nullptr, att, B, H, Tt, c.num_heads, -1, st))) return rc;
-        {
-            ConvIO io;
-            io.x = att; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-            io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L.o, io, st))) return rc;
-        }
-        if ((rc = launch_add_layernorm(x, yb, L.ln1_g, L.ln1_b, nullptr, x, B, H, Tt, 1e-4f, st))) return rc;
-        {
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
-            io.y = hb; io.y_bs = (long long)F * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            io.act = ACT_RELU;
-            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
-        }
-        {
-            ConvIO io;
-            io.x = hb; io.x_bs = (long long)F * Tt; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
-            io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
-            if ((rc = launch_conv(L.ffn2, io, st))) return rc;
-        }
-        // norm2(x + y), masked: the next layer's x * x_mask and the final x * x_mask (:419, :431)
-        if ((rc = launch_add_layernorm(x, yb, L.ln2_g, L.ln2_b, x_mask, x, B, H, Tt, 1e-4f, st))) return rc;
-    }
+    if ((rc = tf.forward(x, x_mask, B, Tt, tfws, tf_bytes, st))) return rc;
     {   // o_mean = proj_m(x) * mask, o_log_scale = proj_s(x) * mask (encoder.py:172-176)
         ConvIO io;
         io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;

@@ -1,4 +1,5 @@
-// VITS TextEncoder: embedding -> 6x [relative-position MHA, add+LayerNorm, conv-FFN, add+LayerNorm] -> 1x1 proj.
+// VITS TextEncoder: embedding -> 6x [relative-position MHA, add+LayerNorm, conv-FFN, add+LayerNorm] -> 1x1 proj; the
+// layer stack is RelPosTransformer, which Glow-TTS shares.
 // Reference: TTS/tts/layers/vits/networks.py:80-100 (TextEncoder.forward),
 //            TTS/tts/layers/glow_tts/transformer.py:109-163,196-241 (attention with the pad/reshape
 //            "skew" tricks, here in closed form -- SURVEY appendix A1), :290-295 (FFN), :411-432 (stack),
@@ -264,24 +265,113 @@ int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, 
     return 0;
 }
 
+RelPosTransformer::Layer::~Layer() {
+    free_conv(qkv); free_conv(o); free_conv(ffn1); free_conv(ffn2);
+    for (float* p : {rel_k, rel_v, ln1_g, ln1_b, ln2_g, ln2_b}) if (p) cudaFree(p);
+}
+
+RelPosTransformer::~RelPosTransformer() {
+    for (auto* l : layers) delete l;
+}
+
+int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int num_heads, int window_size,
+                            float ln_eps, int num_layers, const float* const* w, int* consumed) {
+    C = channels; F = ffn_channels; heads = num_heads; window = window_size; eps = ln_eps;
+    const int K = kernel_size, d = C / heads;
+    const int nrel = 2 * window + 1;
+    const int per = window >= 0 ? 18 : 16;
+    int rc;
+    for (int l = 0; l < num_layers; ++l) {
+        const float* const* p = w + (size_t)l * per;
+        Layer* L = new Layer();
+        layers.push_back(L);
+        if (window >= 0) {
+            if ((rc = upload(&L->rel_k, p[0], (size_t)nrel * d))) return rc;
+            if ((rc = upload(&L->rel_v, p[1], (size_t)nrel * d))) return rc;
+            p += 2;
+        }
+        // fused QKV: rows [q | k | v]
+        std::vector<float> wq((size_t)3 * C * C), bq((size_t)3 * C);
+        for (int s = 0; s < 3; ++s) {
+            memcpy(wq.data() + (size_t)s * C * C, p[2 * s], sizeof(float) * C * C);
+            memcpy(bq.data() + (size_t)s * C, p[2 * s + 1], sizeof(float) * C);
+        }
+        if ((rc = pack_conv(L->qkv, wq.data(), bq.data(), 3 * C, C, 1, 1, 0))) return rc;
+        if ((rc = pack_conv(L->o, p[6], p[7], C, C, 1, 1, 0))) return rc;
+        if ((rc = upload(&L->ln1_g, p[8], C))) return rc;
+        if ((rc = upload(&L->ln1_b, p[9], C))) return rc;
+        // FeedForwardNetwork._same_padding: pad_l = (k-1)//2 (transformer.py:307-313)
+        if ((rc = pack_conv(L->ffn1, p[10], p[11], F, C, K, 1, (K - 1) / 2))) return rc;
+        if ((rc = pack_conv(L->ffn2, p[12], p[13], C, F, K, 1, (K - 1) / 2))) return rc;
+        if ((rc = upload(&L->ln2_g, p[14], C))) return rc;
+        if ((rc = upload(&L->ln2_b, p[15], C))) return rc;
+    }
+    *consumed = per * num_layers;
+    return 0;
+}
+
+size_t RelPosTransformer::workspace_bytes(int B, int T) const {
+    return arena_bytes((size_t)B * 3 * C * T) + 2 * arena_bytes((size_t)B * C * T) + arena_bytes((size_t)B * F * T);
+}
+
+int RelPosTransformer::forward(float* x, const float* x_mask, int B, int T, void* ws, size_t ws_bytes,
+                               cudaStream_t st) const {
+    Arena ar(ws, ws_bytes);
+    float* qkv = ar.f32((size_t)B * 3 * C * T);
+    float* att = ar.f32((size_t)B * C * T);
+    float* yb = ar.f32((size_t)B * C * T);
+    float* hb = ar.f32((size_t)B * F * T);
+    B200_REQUIRE(qkv && att && yb && hb, "rel_pos_transformer: arena exhausted");
+    const long long bs = (long long)C * T;
+    int rc;
+    for (const Layer* L : layers) {
+        {   // q,k,v = conv_{q,k,v}(x)       (x is already masked: the caller / previous norm2 epilogue)
+            ConvIO io;
+            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;
+            io.y = qkv; io.y_bs = 3 * bs; io.y_cs = T; io.Tout = T; io.B = B;
+            if ((rc = launch_conv(L->qkv, io, st))) return rc;
+        }
+        if ((rc = launch_attention(qkv, x_mask, L->rel_k, L->rel_v, att, B, C, T, heads, window, st))) return rc;
+        {   // y = conv_o(att)
+            ConvIO io;
+            io.x = att; io.x_bs = bs; io.x_cs = T; io.Tin = T;
+            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
+            if ((rc = launch_conv(L->o, io, st))) return rc;
+        }
+        if ((rc = launch_add_layernorm(x, yb, L->ln1_g, L->ln1_b, nullptr, x, B, C, T, eps, st))) return rc;
+        {   // h = relu(conv_1(pad(x * mask)))
+            ConvIO io;
+            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
+            io.y = hb; io.y_bs = (long long)F * T; io.y_cs = T; io.Tout = T; io.B = B;
+            io.act = ACT_RELU;
+            if ((rc = launch_conv(L->ffn1, io, st))) return rc;
+        }
+        {   // y = conv_2(pad(h * mask)) * mask
+            ConvIO io;
+            io.x = hb; io.x_bs = (long long)F * T; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
+            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
+            io.ymask = x_mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+            if ((rc = launch_conv(L->ffn2, io, st))) return rc;
+        }
+        // x = norm2(x + y); the next layer and the stack's output (transformer.py:419, :431) use x * mask -> fold the
+        // mask here
+        if ((rc = launch_add_layernorm(x, yb, L->ln2_g, L->ln2_b, x_mask, x, B, C, T, eps, st))) return rc;
+    }
+    return 0;
+}
+
 TextEncoder::~TextEncoder() {
     if (emb) cudaFree(emb);
-    for (auto* l : layers) {
-        free_conv(l->qkv); free_conv(l->o); free_conv(l->ffn1); free_conv(l->ffn2);
-        for (float* p : {l->rel_k, l->rel_v, l->ln1_g, l->ln1_b, l->ln2_g, l->ln2_b}) if (p) cudaFree(p);
-        delete l;
-    }
     free_conv(proj);
 }
 
-// weights: emb [V,hidden]; per layer: emb_rel_k [1,2w+1,d], emb_rel_v, conv_q.w/.b, conv_k.w/.b, conv_v.w/.b,
-// conv_o.w/.b, norm1.gamma/.beta, ffn.conv_1.w/.b, ffn.conv_2.w/.b, norm2.gamma/.beta; proj.w [2*out,C,1], proj.b
+// weights: emb [V,hidden]; per layer: see RelPosTransformer::init (window w); proj.w [2*out,C,1], proj.b
 int TextEncoder::init(const b200tts_text_encoder_config& cfg, const float* const* w, int nw) {
     c = cfg;
     C = c.hidden_channels + c.language_emb_dim;
     B200_REQUIRE(c.num_heads >= 1 && C % c.num_heads == 0, "text_encoder: channels %d not divisible by heads %d", C,
                  c.num_heads);
-    d = C / c.num_heads;
+    const int d = C / c.num_heads;
     B200_REQUIRE(d <= ATT_MAXD, "text_encoder: head dim %d > %d", d, ATT_MAXD);
     B200_REQUIRE(c.rel_attn_window_size >= 0 && 2 * c.rel_attn_window_size + 1 <= 32, "text_encoder: bad window");
     const int per = 18;
@@ -289,38 +379,15 @@ int TextEncoder::init(const b200tts_text_encoder_config& cfg, const float* const
                  1 + per * c.num_layers + 2, nw);
     int rc;
     if ((rc = upload(&emb, w[0], (size_t)c.n_vocab * c.hidden_channels))) return rc;
-    const int nrel = 2 * c.rel_attn_window_size + 1;
-    const int K = c.kernel_size;
-    for (int l = 0; l < c.num_layers; ++l) {
-        const float* const* p = w + 1 + (size_t)l * per;
-        Layer* L = new Layer();
-        layers.push_back(L);
-        if ((rc = upload(&L->rel_k, p[0], (size_t)nrel * d))) return rc;
-        if ((rc = upload(&L->rel_v, p[1], (size_t)nrel * d))) return rc;
-        // fused QKV: rows [q | k | v]
-        std::vector<float> wq((size_t)3 * C * C), bq((size_t)3 * C);
-        for (int s = 0; s < 3; ++s) {
-            memcpy(wq.data() + (size_t)s * C * C, p[2 + 2 * s], sizeof(float) * C * C);
-            memcpy(bq.data() + (size_t)s * C, p[3 + 2 * s], sizeof(float) * C);
-        }
-        if ((rc = pack_conv(L->qkv, wq.data(), bq.data(), 3 * C, C, 1, 1, 0))) return rc;
-        if ((rc = pack_conv(L->o, p[8], p[9], C, C, 1, 1, 0))) return rc;
-        if ((rc = upload(&L->ln1_g, p[10], C))) return rc;
-        if ((rc = upload(&L->ln1_b, p[11], C))) return rc;
-        // FeedForwardNetwork._same_padding: pad_l = (k-1)//2 (transformer.py:307-313)
-        if ((rc = pack_conv(L->ffn1, p[12], p[13], c.hidden_channels_ffn, C, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = pack_conv(L->ffn2, p[14], p[15], C, c.hidden_channels_ffn, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = upload(&L->ln2_g, p[16], C))) return rc;
-        if ((rc = upload(&L->ln2_b, p[17], C))) return rc;
-    }
-    const float* const* p = w + 1 + (size_t)per * c.num_layers;
+    int used = 0;
+    if ((rc = tf.init(C, c.hidden_channels_ffn, c.kernel_size, c.num_heads, c.rel_attn_window_size, 1e-5f,
+                      c.num_layers, w + 1, &used)))
+        return rc;
+    const float* const* p = w + 1 + used;
     return pack_conv(proj, p[0], p[1], 2 * c.out_channels, C, 1, 1, 0);
 }
 
-size_t TextEncoder::workspace_bytes(int B, int T) const {
-    return arena_bytes((size_t)B * 3 * C * T) + 2 * arena_bytes((size_t)B * C * T) +
-           arena_bytes((size_t)B * c.hidden_channels_ffn * T) + 1024;
-}
+size_t TextEncoder::workspace_bytes(int B, int T) const { return tf.workspace_bytes(B, T) + 1024; }
 
 int TextEncoder::forward(const long long* tokens, const long long* lengths, const float* lang_emb, int B, int T,
                          float* x, float* stats, float* x_mask, void* ws, size_t ws_bytes, cudaStream_t st) const {
@@ -328,50 +395,10 @@ int TextEncoder::forward(const long long* tokens, const long long* lengths, cons
     B200_REQUIRE((c.language_emb_dim > 0) == (lang_emb != nullptr), "text_encoder_forward: lang_emb mismatch");
     B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "text_encoder_forward: workspace too small");
     if (B == 0 || T == 0) return 0;
-    Arena ar(ws, ws_bytes);
-    float* qkv = ar.f32((size_t)B * 3 * C * T);
-    float* att = ar.f32((size_t)B * C * T);
-    float* yb = ar.f32((size_t)B * C * T);
-    float* hb = ar.f32((size_t)B * c.hidden_channels_ffn * T);
-    B200_REQUIRE(qkv && att && yb && hb, "text_encoder_forward: arena exhausted");
     const long long bs = (long long)C * T;
     int rc;
     if ((rc = launch_embed(tokens, lengths, emb, lang_emb, B, T, c.hidden_channels, C, x, x_mask, st))) return rc;
-    for (int l = 0; l < c.num_layers; ++l) {
-        const Layer& L = *layers[l];
-        {   // q,k,v = conv_{q,k,v}(x)       (x is already masked: embed / previous norm2 epilogue)
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = qkv; io.y_bs = 3 * bs; io.y_cs = T; io.Tout = T; io.B = B;
-            if ((rc = launch_conv(L.qkv, io, st))) return rc;
-        }
-        if ((rc = launch_attention(qkv, x_mask, L.rel_k, L.rel_v, att, B, C, T, c.num_heads, c.rel_attn_window_size,
-                                   st))) return rc;
-        {   // y = conv_o(att)
-            ConvIO io;
-            io.x = att; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-            if ((rc = launch_conv(L.o, io, st))) return rc;
-        }
-        if ((rc = launch_add_layernorm(x, yb, L.ln1_g, L.ln1_b, nullptr, x, B, C, T, 1e-5f, st))) return rc;
-        {   // h = relu(conv_1(pad(x * mask)))
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
-            io.y = hb; io.y_bs = (long long)c.hidden_channels_ffn * T; io.y_cs = T; io.Tout = T; io.B = B;
-            io.act = ACT_RELU;
-            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
-        }
-        {   // y = conv_2(pad(h * mask)) * mask
-            ConvIO io;
-            io.x = hb; io.x_bs = (long long)c.hidden_channels_ffn * T; io.x_cs = T; io.Tin = T;
-            io.xmask = x_mask; io.xmask_bs = T;
-            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-            io.ymask = x_mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
-            if ((rc = launch_conv(L.ffn2, io, st))) return rc;
-        }
-        // x = norm2(x + y); the next layer (and the encoder output) use x * mask -> fold the mask here
-        if ((rc = launch_add_layernorm(x, yb, L.ln2_g, L.ln2_b, x_mask, x, B, C, T, 1e-5f, st))) return rc;
-    }
+    if ((rc = tf.forward(x, x_mask, B, T, ws, ws_bytes, st))) return rc;
     {   // stats = proj(x) * mask  -> [m_p | logs_p]
         ConvIO io;
         io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;

@@ -322,18 +322,16 @@ class ForwardTTS(EngineModule):
             a.duration_predictor_kernel_size, int(a.use_pitch), a.pitch_predictor_hidden_channels,
             a.pitch_predictor_kernel_size, a.pitch_embedding_kernel_size, int(a.use_energy),
             a.energy_predictor_hidden_channels, a.energy_predictor_kernel_size, a.energy_embedding_kernel_size, pe_len)
-        ln = lambda n: [_host(n.gamma.reshape(-1)), _host(n.beta.reshape(-1))]   # noqa: E731
-        pred = lambda p: _wb(p.conv_1) + ln(p.norm_1) + _wb(p.conv_2) + ln(p.norm_2) + _wb(p.proj)   # noqa: E731
         t = [_host(self.emb.weight)]
         for layer in enc:
             t += layer.weights()
         if proj_in:
             t += _wb(self.proj_g)
-        t += pred(self.duration_predictor)
+        t += self.duration_predictor.ordered_weights()
         if a.use_pitch:
-            t += pred(self.pitch_predictor) + _wb(self.pitch_emb)
+            t += self.pitch_predictor.ordered_weights() + _wb(self.pitch_emb)
         if a.use_energy:
-            t += pred(self.energy_predictor) + _wb(self.energy_emb)
+            t += self.energy_predictor.ordered_weights() + _wb(self.energy_emb)
         if pe_len:
             t += [_host(self.pos_encoder.pe[0])]
         for layer in dec:

@@ -20,7 +20,7 @@ from torch import nn
 from torch.nn.utils import parametrize
 
 from . import _lib
-from .layers import WN, DurationPredictor, EngineModule, _Attention, _FFN, _host, _LayerNorm1, _wb
+from .layers import WN, DurationPredictor, EngineModule, RelativePositionTransformer, _host, _LayerNorm1, _ln, _wb
 
 
 def _cfg(config, key, default=None):
@@ -100,27 +100,6 @@ class _ResidualConv1dLayerNormBlock(nn.Module):
         self.proj.bias.data.zero_()
 
 
-class _Transformer(nn.Module):
-    """Parameters of RelativePositionTransformer (glow_tts/transformer.py:343-409) as Glow-TTS builds it: no relative
-    window, layer_norm_type "1", in = hidden = out channels."""
-
-    def __init__(self, hidden_channels, hidden_channels_ffn, num_heads, num_layers, kernel_size=1, dropout_p=0.0,
-                 input_length=None, rel_attn_window_size=None, layer_norm_type="1"):
-        super().__init__()
-        if rel_attn_window_size is not None or layer_norm_type != "1" or input_length is not None:
-            raise NotImplementedError("tts_b200.GlowTTS: the encoder is built without a relative window, with "
-                                      "layer_norm_type '1' and input_length None (GlowTTSConfig's encoder)")
-        self.attn_layers = nn.ModuleList()
-        self.norm_layers_1 = nn.ModuleList()
-        self.ffn_layers = nn.ModuleList()
-        self.norm_layers_2 = nn.ModuleList()
-        for _ in range(num_layers):
-            self.attn_layers.append(_Attention(hidden_channels, hidden_channels, num_heads))
-            self.norm_layers_1.append(_LayerNorm1(hidden_channels))
-            self.ffn_layers.append(_FFN(hidden_channels, hidden_channels, hidden_channels_ffn, kernel_size))
-            self.norm_layers_2.append(_LayerNorm1(hidden_channels))
-
-
 class _Encoder(nn.Module):
     """Parameters of TTS/tts/layers/glow_tts/encoder.py:78-141 for encoder_type "rel_pos_transformer"."""
 
@@ -136,10 +115,12 @@ class _Encoder(nn.Module):
         nn.init.normal_(self.emb.weight, 0.0, hidden_channels ** -0.5)
         if use_prenet:
             self.prenet = _ResidualConv1dLayerNormBlock(hidden_channels, hidden_channels, hidden_channels, 5, 3)
-        p = dict(encoder_params)
-        p.pop("dropout_p", None)
-        self.encoder = _Transformer(hidden_channels, p.pop("hidden_channels_ffn"), p.pop("num_heads"),
-                                    p.pop("num_layers"), **p)
+        p = encoder_params
+        if p.get("rel_attn_window_size") is not None or p.get("layer_norm_type", "1") != "1" or \
+                p.get("input_length") is not None:
+            raise NotImplementedError("tts_b200.GlowTTS: the encoder is built without a relative window, with "
+                                      "layer_norm_type '1' and input_length None (GlowTTSConfig's encoder)")
+        self.encoder = RelativePositionTransformer(hidden_channels, hidden_channels, hidden_channels, **p)
         self.proj_m = nn.Conv1d(hidden_channels, out_channels, 1)
         if not mean_only:
             self.proj_s = nn.Conv1d(hidden_channels, out_channels, 1)
@@ -269,19 +250,14 @@ class GlowTTS(EngineModule):
                                   int(self.mean_only), self.hidden_channels_dp, self.c_in_channels,
                                   self.hidden_channels_dec, self.kernel_size_dec, self.dilation_rate, n_dec,
                                   self.num_block_layers, self.num_splits, self.num_squeeze, int(self.sigmoid_scale))
-        ln = lambda n: [_host(n.gamma.reshape(-1)), _host(n.beta.reshape(-1))]   # noqa: E731
         t = [_host(e.emb.weight)]
         if self.use_encoder_prenet:
             for conv, norm in zip(e.prenet.conv_layers, e.prenet.norm_layers):
-                t += _wb(conv) + ln(norm)
+                t += _wb(conv) + _ln(norm)
             t += _wb(e.prenet.proj)
-        enc = e.encoder
-        for a, n1, f, n2 in zip(enc.attn_layers, enc.norm_layers_1, enc.ffn_layers, enc.norm_layers_2):
-            t += _wb(a.conv_q) + _wb(a.conv_k) + _wb(a.conv_v) + _wb(a.conv_o) + ln(n1) + _wb(f.conv_1) + _wb(f.conv_2)
-            t += ln(n2)
+        t += e.encoder.ordered_weights()
         t += _wb(e.proj_m) + ([] if self.mean_only else _wb(e.proj_s))
-        dp = e.duration_predictor
-        t += _wb(dp.conv_1) + ln(dp.norm_1) + _wb(dp.conv_2) + ln(dp.norm_2) + _wb(dp.proj)
+        t += e.duration_predictor.ordered_weights()
         fl = self.decoder.flows
         for n in range(n_dec):
             an, ic, cb = fl[3 * n], fl[3 * n + 1], fl[3 * n + 2]

@@ -31,6 +31,11 @@ def _wb(m):
     return [_host(m.weight), _host(m.bias)]
 
 
+def _ln(n):
+    """[gamma, beta] of a LayerNorm container as flat host fp32 vectors."""
+    return [_host(n.gamma.reshape(-1)), _host(n.beta.reshape(-1))]
+
+
 class EngineModule(nn.Module):
     """Owns one C-ABI handle built lazily from the module's parameters (and rebuilt after
     ``.to()`` / ``load_state_dict``).  Call ``repack()`` after editing weights in place."""
@@ -325,16 +330,17 @@ class DurationPredictor(EngineModule):
         if self._lang:
             self.cond_lang = nn.Conv1d(self._lang, cin, 1)
 
+    def ordered_weights(self):
+        out = _wb(self.conv_1) + _ln(self.norm_1) + _wb(self.conv_2) + _ln(self.norm_2) + _wb(self.proj)
+        if self._cond:
+            out += _wb(self.cond)
+        if self._lang:
+            out += _wb(self.cond_lang)
+        return out
+
     def _create(self, device):
         cfg = _lib.DurationPredictorConfigC(self._in, self.filter_channels, self.kernel_size, self._cond, self._lang)
-        tensors = _wb(self.conv_1) + [_host(self.norm_1.gamma.reshape(-1)), _host(self.norm_1.beta.reshape(-1))]
-        tensors += _wb(self.conv_2) + [_host(self.norm_2.gamma.reshape(-1)), _host(self.norm_2.beta.reshape(-1))]
-        tensors += _wb(self.proj)
-        if self._cond:
-            tensors += _wb(self.cond)
-        if self._lang:
-            tensors += _wb(self.cond_lang)
-        return self._make("b200tts_duration_predictor_create", cfg, tensors)
+        return self._make("b200tts_duration_predictor_create", cfg, self.ordered_weights())
 
     @torch.no_grad()
     def forward(self, x, x_mask, g=None, lang_emb=None):
@@ -391,22 +397,37 @@ class _FFN(nn.Module):
 
 
 class RelativePositionTransformer(nn.Module):
-    """Parameters of glow_tts/transformer.py:343-409 (layer_norm_type "2", hidden == out channels)."""
+    """Parameters of glow_tts/transformer.py:343-409 with in == hidden == out channels: layer_norm_type "2" and a
+    relative window (the VITS text encoder) or "1" without one (Glow-TTS)."""
 
     def __init__(self, in_channels, out_channels, hidden_channels, hidden_channels_ffn, num_heads, num_layers,
-                 kernel_size=1, dropout_p=0.0, rel_attn_window_size=None, input_length=None, layer_norm_type="2"):
+                 kernel_size=1, dropout_p=0.0, rel_attn_window_size=None, input_length=None, layer_norm_type="1"):
         super().__init__()
-        if layer_norm_type != "2" or in_channels != hidden_channels or out_channels != hidden_channels:
-            raise NotImplementedError("tts_b200: only the VITS text-encoder transformer configuration is built")
+        if layer_norm_type not in ("1", "2") or in_channels != hidden_channels or out_channels != hidden_channels:
+            raise NotImplementedError("tts_b200: the transformer is built with in = hidden = out channels and "
+                                      "layer_norm_type '1' or '2'")
+        norm = _LayerNorm1 if layer_norm_type == "1" else LayerNorm2
+        self.rel_attn_window_size = rel_attn_window_size
         self.attn_layers = nn.ModuleList()
         self.norm_layers_1 = nn.ModuleList()
         self.ffn_layers = nn.ModuleList()
         self.norm_layers_2 = nn.ModuleList()
         for _ in range(num_layers):
             self.attn_layers.append(_Attention(hidden_channels, hidden_channels, num_heads, rel_attn_window_size))
-            self.norm_layers_1.append(LayerNorm2(hidden_channels))
+            self.norm_layers_1.append(norm(hidden_channels))
             self.ffn_layers.append(_FFN(hidden_channels, hidden_channels, hidden_channels_ffn, kernel_size))
-            self.norm_layers_2.append(LayerNorm2(hidden_channels))
+            self.norm_layers_2.append(norm(hidden_channels))
+
+    def ordered_weights(self):
+        out = []
+        for a, n1, f, n2 in zip(self.attn_layers, self.norm_layers_1, self.ffn_layers, self.norm_layers_2):
+            if self.rel_attn_window_size is not None:
+                if a.emb_rel_k.shape[0] != 1:
+                    raise NotImplementedError("tts_b200: heads_share=False is not built")
+                out += [_host(a.emb_rel_k), _host(a.emb_rel_v)]
+            out += _wb(a.conv_q) + _wb(a.conv_k) + _wb(a.conv_v) + _wb(a.conv_o) + _ln(n1)
+            out += _wb(f.conv_1) + _wb(f.conv_2) + _ln(n2)
+        return out
 
 
 class TextEncoder(EngineModule):
@@ -430,17 +451,8 @@ class TextEncoder(EngineModule):
         c = self._cfg
         cfg = _lib.TextEncoderConfigC(c["n_vocab"], c["out_channels"], c["hidden_channels"],
                                       c["hidden_channels_ffn"], c["num_heads"], c["num_layers"], c["kernel_size"],
-                                      4, c["language_emb_dim"])
-        e = self.encoder
-        tensors = [_host(self.emb.weight)]
-        for a, n1, f, n2 in zip(e.attn_layers, e.norm_layers_1, e.ffn_layers, e.norm_layers_2):
-            if a.emb_rel_k.shape[0] != 1:
-                raise NotImplementedError("tts_b200: heads_share=False is not built")
-            tensors += [_host(a.emb_rel_k), _host(a.emb_rel_v)]
-            tensors += _wb(a.conv_q) + _wb(a.conv_k) + _wb(a.conv_v) + _wb(a.conv_o)
-            tensors += [_host(n1.gamma), _host(n1.beta)] + _wb(f.conv_1) + _wb(f.conv_2)
-            tensors += [_host(n2.gamma), _host(n2.beta)]
-        tensors += _wb(self.proj)
+                                      self.encoder.rel_attn_window_size, c["language_emb_dim"])
+        tensors = [_host(self.emb.weight)] + self.encoder.ordered_weights() + _wb(self.proj)
         return self._make("b200tts_text_encoder_create", cfg, tensors)
 
     @torch.no_grad()
