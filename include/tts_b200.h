@@ -680,6 +680,51 @@ int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* nois
                           int pe_frames, float c1, float c2, float sigma, const float* z, int B, int T, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---- Parallel WaveGAN generator ----------------------------------------------------------------------------------
+ * Replaces ParallelWaveganGenerator.forward / .inference (TTS/vocoder/models/parallel_wavegan_generator.py:12-118;
+ * ResidualBlock TTS/vocoder/layers/parallel_wavegan.py, ConvUpsample TTS/vocoder/layers/upsample.py) for the shapes
+ * setup_generator builds: 1 noise channel in, 1 out, 64 residual / 128 gate / 64 skip channels, kernel 3, 80 mel
+ * channels, no upsampler nonlinearity.  Layer l has dilation 2^(l % (num_res_blocks / stacks)).
+ * The conditioning is folded: W_aux,l W_in (float64 at create) on the frame-rate mel, then the upsampler's linear map,
+ * tabulated at create from unit impulses (float64), added inside each layer; the residual layers run on split-fp16
+ * tensor cores (3 products, fp32 accumulation).
+ * weights (host pointers, PyTorch layouts, weight norm folded), in state-dict order:
+ *   first_conv.w [64, 1, 1], first_conv.b [64]
+ *   upsample_net.conv_in.w [80, 80, 1]
+ *   per upsample stage s: upsample_net.upsample.up_layers.(2s+1).w [1, 1, 1, 2 u_s + 1]
+ *   per layer l: conv.w [128, 64, 3], conv.b [128], conv1x1_aux.w [128, 80, 1], conv1x1_out.w [64, 64, 1], .b,
+ *                conv1x1_skip.w [64, 64, 1], .b
+ *   last_conv_layers.1.w [64, 64, 1], .b, last_conv_layers.3.w [1, 64, 1], .b
+ */
+typedef struct {
+    int num_res_blocks, stacks;        /* num_res_blocks % stacks == 0, at most 16 layers per stack */
+    int num_upsamples;                 /* 1 .. 8 */
+    int upsample_factors[8];           /* product at most 4096 */
+} b200tts_pwgan_config;
+typedef struct b200tts_pwgan b200tts_pwgan;
+int b200tts_pwgan_create(const b200tts_pwgan_config* cfg, const float* const* weights, int num_weights,
+                         b200tts_pwgan** out);
+void b200tts_pwgan_destroy(b200tts_pwgan* h);
+/* scratch for B rows of Tf frames (the length after the replicate pad) */
+size_t b200tts_pwgan_workspace_bytes(const b200tts_pwgan* h, int B, int Tf);
+/* the shortest padded input (frames) the upsampler tables are exact for; 5 or less for every factor list >= 2 */
+int b200tts_pwgan_min_frames(const b200tts_pwgan* h);
+/* mel [B, 80, T] (device, dense), replicate-padded by `pad` frames each side as read (0: forward(c), 2: inference(c));
+ * noise [B, 1, Tf * P] (device; Tf = T + 2 pad, P = prod(upsample_factors)) -> out [B, 1, Tf * P].  Split-fp16 range:
+ * a residual-layer activation with |x| >= 65504 makes the next launch on the device fail (once), as for the conv
+ * engine's split-fp16 layers. */
+int b200tts_pwgan_forward(const b200tts_pwgan* h, const float* mel, const float* noise, int B, int T, int pad, float* out,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* residual layer l alone, as b200tts_pwgan_forward runs it (0 <= l < num_res_blocks): the layer's conditioning from mel
+ * [B, 80, T] (replicate-padded by `pad`), then x [B, 64, pitch] -> x_new [B, 64, pitch] (never the buffer x is) and
+ * skip [B, 64, pitch] updated (layer 0 stores it; the last layer multiplies the sum by sqrt(1 / num_res_blocks)).  Only
+ * columns [0, Tf * P) are read or written (Tf = T + 2 pad, pitch >= Tf * P); workspace: at least
+ * b200tts_pwgan_workspace_bytes(h, B, Tf). */
+int b200tts_pwgan_layer(const b200tts_pwgan* h, int layer, const float* mel, int B, int T, int pad, const float* x,
+                        float* skip, float* x_new, int pitch, void* workspace, size_t workspace_bytes, void* stream);
+/* the upsampler's linear map alone, as the layers apply it: a [rows, Tf] (device) -> out [rows, Tf * P] */
+int b200tts_pwgan_upsample(const b200tts_pwgan* h, const float* a, int rows, int Tf, float* out, void* stream);
+
 /* ---- Overflow / Neural-HMM inference (text -> mel spectrogram, autoregressive) ----------------------------------
  * Replaces Overflow.inference (TTS/tts/models/overflow.py:207-246) and NeuralhmmTTS.inference
  * (TTS/tts/models/neuralhmm_tts.py) in three calls:

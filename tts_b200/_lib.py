@@ -98,6 +98,11 @@ class WavegradConfigC(ctypes.Structure):
                 ("ublock_out_channels", ctypes.c_int * 8), ("upsample_dilations", (ctypes.c_int * 4) * 8)]
 
 
+class PwganConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("num_res_blocks", "stacks", "num_upsamples")] + \
+               [("upsample_factors", ctypes.c_int * 8)]
+
+
 # padding modes of b200tts_conv1d_create_padded (B200TTS_PAD_* in include/tts_b200.h)
 PADDING_MODES = {"zeros": 0, "reflect": 1}
 
@@ -110,7 +115,8 @@ class AudioNormC(ctypes.Structure):
 
 DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped", 10: "attn_tc3",
                   11: "attn_fma", 12: "tc3w_tf32", 13: "tc3w_tf32_near", 14: "tc3w_f16x3", 15: "tc3w_f16x3_near",
-                  16: "fma_wg", 17: "fma_wg_near", 18: "lstm_bi", 19: "lstm_cell", 20: "hmm_linear", 21: "hmm_step"}
+                  16: "fma_wg", 17: "fma_wg_near", 18: "lstm_bi", 19: "lstm_cell", 20: "hmm_linear", 21: "hmm_step",
+                  22: "pwgan_tc", 23: "pwgan_aux"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}
@@ -169,6 +175,20 @@ def _declare(lib):
     lib.b200tts_conv1d_forward_wavegrad.restype = ci
     lib.b200tts_conv1d_forward_wavegrad.argtypes = [vp, vp, ll, ci, ci, ci, ci, ctypes.c_float, ci, vp, vp, ll, ci, vp, ll,
                                                     ci, ci, vp, ll, ci, vp, vp]
+    lib.b200tts_pwgan_create.restype = ci
+    lib.b200tts_pwgan_create.argtypes = [ctypes.POINTER(PwganConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+    lib.b200tts_pwgan_destroy.restype = None
+    lib.b200tts_pwgan_destroy.argtypes = [vp]
+    lib.b200tts_pwgan_workspace_bytes.restype = sz
+    lib.b200tts_pwgan_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_pwgan_min_frames.restype = ci
+    lib.b200tts_pwgan_min_frames.argtypes = [vp]
+    lib.b200tts_pwgan_forward.restype = ci
+    lib.b200tts_pwgan_forward.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_pwgan_layer.restype = ci
+    lib.b200tts_pwgan_layer.argtypes = [vp, ci, vp, ci, ci, ci, vp, vp, vp, ci, vp, sz, vp]
+    lib.b200tts_pwgan_upsample.restype = ci
+    lib.b200tts_pwgan_upsample.argtypes = [vp, vp, ci, ci, vp, vp]
     lib.b200tts_pqmf_synthesis.restype = ci
     lib.b200tts_pqmf_synthesis.argtypes = [vp, ci, ci, ci, vp, ci, vp, vp, vp]
     lib.b200tts_conv1d_destroy.restype = None

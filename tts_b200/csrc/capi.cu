@@ -18,6 +18,7 @@ struct b200tts_melgan { Melgan impl; };
 struct b200tts_forward_tts { ForwardTTS impl; };
 struct b200tts_wavegrad { Wavegrad impl; };
 struct b200tts_overflow { Overflow impl; };
+struct b200tts_pwgan { Pwgan impl; };
 
 extern "C" {
 
@@ -493,6 +494,24 @@ int b200tts_wavegrad_step(const b200tts_wavegrad* h, float* y, const float* nois
     if (!h) { set_error("wavegrad_step: null handle"); return 1; }
     return h->impl.step(y, noise_level, pe, pe_frames, c1, c2, sigma, z, B, T, workspace, workspace_bytes,
                         (cudaStream_t)stream);
+}
+
+B200_HANDLE_API(pwgan, b200tts_pwgan, b200tts_pwgan_config)
+
+int b200tts_pwgan_min_frames(const b200tts_pwgan* h) { return h ? h->impl.min_frames : 0; }
+int b200tts_pwgan_forward(const b200tts_pwgan* h, const float* mel, const float* noise, int B, int T, int pad, float* out,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("pwgan_forward: null handle"); return 1; }
+    return h->impl.forward(mel, noise, B, T, pad, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_pwgan_layer(const b200tts_pwgan* h, int layer, const float* mel, int B, int T, int pad, const float* x,
+                        float* skip, float* x_new, int pitch, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("pwgan_layer: null handle"); return 1; }
+    return h->impl.layer(layer, mel, B, T, pad, x, skip, x_new, pitch, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_pwgan_upsample(const b200tts_pwgan* h, const float* a, int rows, int Tf, float* out, void* stream) {
+    if (!h) { set_error("pwgan_upsample: null handle"); return 1; }
+    return h->impl.upsample(a, rows, Tf, out, (cudaStream_t)stream);
 }
 
 int b200tts_overflow_create(const b200tts_overflow_config* cfg, const float* const* weights, int num_weights,

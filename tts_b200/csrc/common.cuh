@@ -165,6 +165,13 @@ int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin
 void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
+// one tensor-core weight image of logical weights Wl(r, ci, k) in the block layout of conv_tc3.cuh (see conv1d.cu);
+// prec PREC_F16X3 also uploads the row scales 2^-e_r into *rscale (when it is still null)
+int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G, float** rscale = nullptr);
+// the tensor-core state of the current device, set up on first use: the mapped error words ([0] pipeline timeout,
+// [ERR_RANGE] split-fp16 range), the SM count and the opt-in shared memory per block.  Fails (once) when an earlier
+// launch set one of the error words.
+int tc_device(int** err, int* num_sms, size_t* max_smem);
 // which kernel family a launch_conv call dispatched to (recorded per thread between dispatch_begin/end; tests pin it)
 enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPATCH_ROW1 = 6,
              DISPATCH_TC16 = 8, DISPATCH_TC16_GROUPED = 9,    // TC16*: the same kernels with bf16 / fp16 operands
@@ -173,7 +180,9 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // WaveGrad variants (EPI_WAVEGRAD / ConvIO::near_src): tensor cores by operand type, FMA tile; +1: resampled input
              DISPATCH_TC3W_TF32 = 12, DISPATCH_TC3W_F16X3 = 14, DISPATCH_FMA_WG = 16,
              // Overflow / Neural-HMM (overflow.cu): the BiLSTM time step, the LSTMCell, a GEMV layer, the frame epilogue
-             DISPATCH_LSTM_BI = 18, DISPATCH_LSTM_CELL = 19, DISPATCH_HMM_LINEAR = 20, DISPATCH_HMM_STEP = 21 };
+             DISPATCH_LSTM_BI = 18, DISPATCH_LSTM_CELL = 19, DISPATCH_HMM_LINEAR = 20, DISPATCH_HMM_STEP = 21,
+             // Parallel WaveGAN (pwgan.cu): the fused residual layer, the folded conditioning conv
+             DISPATCH_PWGAN_TC = 22, DISPATCH_PWGAN_AUX = 23 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -472,8 +472,7 @@ void free_conv(ConvLayer& L) {
 // With G tap groups (1: plain; 128 / rows: grouped), MMA row m = g * (128 / G) + co of tile t carries weight row
 // t * 128 + co and, in tap block j, tap G * j + g.  Rows >= `rows`, taps >= K and channels >= Cin are zero.  The weight
 // norm is already folded (in fp32) into Wl; each weight is rounded once, here.
-static int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G,
-                   float** rscale = nullptr) {
+int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G, float** rscale) {
     const bool tf32 = prec == tc::PREC_FP32, x3 = prec == tc::PREC_F16X3;
     const int kc = tf32 ? tc3::KC2 : tc3::KC16, slc = kc / 2, ch = tc3::MROWS / G;
     const int ntiles = (rows + tc3::MROWS - 1) / tc3::MROWS, nchunks = (Cin + kc - 1) / kc, J = (K + G - 1) / G;
@@ -835,39 +834,35 @@ static void set_window(tc3::Tc3Args& t, const ConvKArgs& a) {
     t.n_ttiles = std::max(0, (hi + t.tstep - 1) / t.tstep - t.t_lo);
 }
 
-static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& a, cudaStream_t st) {
-    if (L.tc_prec == TC_NONE || a.Tq < 128) return -1;
-    if (a.act == ACT_LOGCLAMP || a.act == ACT_TANH) return -1;
-    if (!(a.in_slope >= 0.f && a.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
-    const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
+static int tc_device_init(int d) {
+    int smem_optin = 0;
+    B200_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
+    for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16, tc::PREC_F16X3}) {
+        for (bool lean : {true, false})
+            B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+        B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+        for (int g : {2, 4})
+            for (bool refl : {false, true})
+                B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  smem_optin));
+        for (bool near : {false, true})
+            if (tc3::wavegrad_kernel(p, near))
+                B200_CUDA_OK(cudaFuncSetAttribute(tc3::wavegrad_kernel(p, near), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  smem_optin));
+    }
+    int* flag = nullptr;   // [0] pipeline timeout, [tc::ERR_RANGE] fp16 range (PREC_F16X3)
+    B200_CUDA_OK(cudaHostAlloc((void**)&flag, 2 * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
+    flag[0] = flag[tc::ERR_RANGE] = 0;
+    g_tc_dev[d].err = flag;    // unified addressing: the host pointer is valid on the device
+    g_tc_dev[d].max_smem = smem_optin;
+    B200_CUDA_OK(cudaDeviceGetAttribute(&g_tc_dev[d].num_sms, cudaDevAttrMultiProcessorCount, d));
+    return 0;
+}
+
+int tc_device(int** err, int* num_sms, size_t* max_smem) {
     int dev = 0;
-    if (int rc = device_once(g_tc_once, &dev, [](int d) -> int {
-        int smem_optin = 0;
-        B200_CUDA_OK(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
-        for (int p : {tc::PREC_FP32, tc::PREC_BF16, tc::PREC_FP16, tc::PREC_F16X3}) {
-            for (bool lean : {true, false})
-                B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-            B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-            for (int g : {2, 4})
-                for (bool refl : {false, true})
-                    B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                      smem_optin));
-            for (bool near : {false, true})
-                if (tc3::wavegrad_kernel(p, near))
-                    B200_CUDA_OK(cudaFuncSetAttribute(tc3::wavegrad_kernel(p, near), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                      smem_optin));
-        }
-        int* flag = nullptr;   // [0] pipeline timeout, [tc::ERR_RANGE] fp16 range (PREC_F16X3)
-        B200_CUDA_OK(cudaHostAlloc((void**)&flag, 2 * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
-        flag[0] = flag[tc::ERR_RANGE] = 0;
-        g_tc_dev[d].err = flag;    // unified addressing: the host pointer is valid on the device
-        g_tc_dev[d].max_smem = smem_optin;
-        B200_CUDA_OK(cudaDeviceGetAttribute(&g_tc_dev[d].num_sms, cudaDevAttrMultiProcessorCount, d));
-        return 0;
-    })) return rc;
+    if (int rc = device_once(g_tc_once, &dev, tc_device_init)) return rc;
     int* const g_tc_err = g_tc_dev[dev].err;
-    const int num_sms = g_tc_dev[dev].num_sms;
-    const size_t max_smem = (size_t)g_tc_dev[dev].max_smem;
     B200_REQUIRE(*reinterpret_cast<volatile int*>(g_tc_err) == 0,
                  "tensor-core conv: an earlier launch on device %d hit a pipeline timeout (its output is invalid)", dev);
     // a range error is reported once, by the next launch: the data was out of range, the device state is fine
@@ -877,6 +872,21 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         B200_REQUIRE(false, "tensor-core conv: an earlier split-fp16 launch on device %d read an activation with |x| >= 65504, "
                             "outside fp16's range (its output is invalid; B200TTS_PRECISION_TF32X3 takes such models)", dev);
     }
+    *err = g_tc_err;
+    if (num_sms) *num_sms = g_tc_dev[dev].num_sms;
+    if (max_smem) *max_smem = (size_t)g_tc_dev[dev].max_smem;
+    return 0;
+}
+
+static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& a, cudaStream_t st) {
+    if (L.tc_prec == TC_NONE || a.Tq < 128) return -1;
+    if (a.act == ACT_LOGCLAMP || a.act == ACT_TANH) return -1;
+    if (!(a.in_slope >= 0.f && a.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
+    const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
+    int* g_tc_err = nullptr;
+    int num_sms = 0;
+    size_t max_smem = 0;
+    if (int rc = tc_device(&g_tc_err, &num_sms, &max_smem)) return rc;
     // persistent kernels: 16-byte aligned activation rows for the cp.async staging, no input mask
     const bool aligned = ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.x_cs % 4 == 0) && (a.x_bs % 4 == 0);
     const bool persistent_ok = aligned && !a.xmask &&

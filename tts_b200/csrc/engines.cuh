@@ -331,6 +331,46 @@ struct Melgan {
 int launch_pqmf_synthesis(const float* x, long long x_bs, int x_cs, int B, int N, int Tb, const float* G, int taps, float* y,
                           unsigned* peak_bits, cudaStream_t st);
 
+// Parallel WaveGAN generator (pwgan.cu): the folded conditioning conv A = [W_aux,l W_in]_l c (replicate pad as clamped
+// reads), first_conv, one fused split-fp16 tensor-core launch per residual layer (gate conv + U(A_l) + gate + out|skip
+// 1x1), then ReLU -> 1x1 -> ReLU -> 1x1 on the conv engine.  64 residual / 128 gate / 64 skip channels, kernel 3.
+struct UTab;
+struct Pwgan {
+    b200tts_pwgan_config c;
+    int P = 1;                                    // samples per frame, prod(upsample_factors)
+    float *first_w = nullptr, *first_b = nullptr; // [64]
+    float* aux_w = nullptr;                       // [L * 128][80]: W_aux,l W_in, gate row order
+    float *b1 = nullptr, *b2 = nullptr;           // [L][128]: gate bias (gate row order), out | skip bias
+    std::vector<void*> w1, w2;                    // per layer: gate conv / out|skip images (pack_tc, PREC_F16X3)
+    std::vector<float*> rs1, rs2;                 // their row scales
+    ConvLayer tail1, tail2;                       // last_conv_layers.1 (64 -> 64) and .3 (64 -> 1)
+    // U: coefficient rows [uE0 left edge | P interior phases | uE1 right edge][uTW frames]; interior sample n reads
+    // frames n / P - uoff ..; exact for inputs of at least min_frames frames
+    float* ucoef = nullptr;
+    int uE0 = 0, uE1 = 0, uTW = 0, uoff = 0, min_frames = 0;
+    ~Pwgan();
+    int init(const b200tts_pwgan_config& cfg, const float* const* w, int nw);
+    int dilation(int l) const;
+    size_t workspace_bytes(int B, int Tf) const;  // Tf: frames after the pad
+    // mel [B, 80, T], replicate-padded by `pad` frames each side; noise [B, 1, (T + 2 pad) P] -> out [B, 1, (T + 2 pad) P]
+    int forward(const float* mel, const float* noise, int B, int T, int pad, float* out, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+    // residual layer l of forward() on its own: the conditioning of layer l from mel (as forward), then x [B, 64, pitch]
+    // -> x_new [B, 64, pitch] and skip [B, 64, pitch] updated as that layer of forward() updates it (stored by layer 0,
+    // scaled by sqrt(1 / L) after the sum by the last layer); only columns [0, (T + 2 pad) P) are read or written
+    int layer(int l, const float* mel, int B, int T, int pad, const float* x, float* skip, float* x_new, int pitch, void* ws,
+              size_t ws_bytes, cudaStream_t st) const;
+    // U alone: a [rows, Tf] -> out [rows, Tf * P]
+    int upsample(const float* a, int rows, int Tf, float* out, cudaStream_t st) const;
+  private:
+    int build_u(const std::vector<std::vector<double>>& fir);
+    UTab utab() const;
+    int check_call(const char* who, int B, int T, int pad, int* Tf) const;
+    int launch_aux(const float* mel, int B, int T, int pad, int l0, int nl, float* A, cudaStream_t st) const;
+    int launch_layer(int l, const float* x, float* xn, float* skip, int B, int pitch, int Tf, const float* A, long long A_bs,
+                     int* err, int num_sms, cudaStream_t st) const;
+};
+
 // WaveGrad (wavegrad.cu): the refinement network on the shared conv engine.  Down path y_conv -> FiLM[0] -> per DBlock
 // [res (1x1), three lrelu -> k3 convs, dilations 1 / 2 / 4, on the decimated input] -> FiLM[i+1]; up path x_conv ->
 // per UBlock [res (1x1) and main0 on the nearest-upsampled input, main1, out0, out1 with the FiLM pair of its rate] ->

@@ -5,7 +5,9 @@ Mirrors, with the reference's names and argument meaning:
                           TTS/config/shared_configs.py:9-176: the audio fields the hand-off reads)
   MelganConfig / MultibandMelganConfig / FullbandMelganConfig
                        <- TTS/vocoder/configs/{melgan,multiband_melgan,fullband_melgan}_config.py (generator side)
-  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-94   (the HiFiGAN and MelGAN generator families)
+  ParallelWaveganConfig
+                       <- TTS/vocoder/configs/parallel_wavegan_config.py (generator side)
+  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-94   (HiFiGAN, the MelGAN family, Parallel WaveGAN)
   GAN                  <- TTS/vocoder/models/gan.py:21-66,338-352 (model_g, forward, inference, load_checkpoint)
   AudioProcessor.normalize / denormalize   <- TTS/utils/audio/processor.py:259-337   (as ``AudioNorm``)
   interpolate_vocoder_input                <- TTS/vocoder/utils/generic_utils.py:11-29
@@ -26,6 +28,7 @@ from torch import nn
 from . import _lib
 from .hifigan import HifiganGenerator
 from .melgan import FullbandMelganGenerator, MelganGenerator, MultibandMelganGenerator
+from .pwgan import ParallelWaveganGenerator
 
 
 # ----------------------------------------------------------------------------- configs
@@ -117,6 +120,20 @@ class FullbandMelganConfig(_ItemAccess):
     audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
 
 
+@dataclass
+class ParallelWaveganConfig(_ItemAccess):
+    """Generator-side fields of TTS/vocoder/configs/parallel_wavegan_config.py:79-88 (+ ``use_pqmf`` of the shared GAN
+    config)."""
+    model: str = "parallel_wavegan"
+    discriminator_model: str = "parallel_wavegan_discriminator"
+    discriminator_model_params: dict = field(default_factory=lambda: {"num_layers": 10})
+    generator_model: str = "parallel_wavegan_generator"
+    generator_model_params: dict = field(
+        default_factory=lambda: {"upsample_factors": [4, 4, 4, 4], "stacks": 3, "num_res_blocks": 30})
+    use_pqmf: bool = False
+    audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
+
+
 # the generator modules under TTS/vocoder/models/ that setup_generator can import
 _GENERATOR_MODULES = ("hifigan_generator", "melgan_generator", "multiband_melgan_generator", "fullband_melgan_generator",
                       "parallel_wavegan_generator", "univnet_generator")
@@ -138,8 +155,9 @@ def setup_generator(c):
     reference does.  The reference first imports the module ``TTS.vocoder.models.<name.lower()>``, so only the names of
     its generator modules (in any letter case) get as far as its ``name in "..."`` substring tests; any other name
     raises NotImplementedError here (the reference fails it at that import).  ``melgan_fb_generator`` raises the
-    reference's ValueError ("now fullband_melgan_generator").  The HiFiGAN and MelGAN families are on the path;
-    ParallelWaveGAN and UniVNet are out of scope and raise NotImplementedError."""
+    reference's ValueError ("now fullband_melgan_generator").  HiFiGAN, the MelGAN family and Parallel WaveGAN are on
+    the path (Parallel WaveGAN reads num_res_blocks, stacks and upsample_factors, in the reference's order, so a config
+    without ``stacks`` -- a MelGAN one -- raises GeneratorParamsError); UniVNet raises NotImplementedError."""
     name = _get(c, "generator_model")
     low = name.lower()
     if name == "melgan_fb_generator":
@@ -170,7 +188,13 @@ def setup_generator(c):
         return FullbandMelganGenerator(in_channels=num_mels, out_channels=1, base_channels=512,
                                        upsample_factors=param("upsample_factors"), num_res_blocks=param("num_res_blocks"),
                                        **melgan)
-    raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN and MelGAN generators are)")
+    if low in "parallel_wavegan_generator":
+        return ParallelWaveganGenerator(in_channels=1, out_channels=1, kernel_size=3,
+                                        num_res_blocks=param("num_res_blocks"), stacks=param("stacks"), res_channels=64,
+                                        gate_channels=128, skip_channels=64, aux_channels=num_mels, dropout=0.0,
+                                        bias=True, use_weight_norm=True, upsample_factors=param("upsample_factors"))
+    raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN, MelGAN and Parallel "
+                              "WaveGAN generators are)")
 
 
 def setup_model(config):
