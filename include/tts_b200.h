@@ -800,6 +800,76 @@ int b200tts_overflow_sample(const b200tts_overflow* h, const int64_t* lengths, i
 int b200tts_overflow_decode(const b200tts_overflow* h, const float* hmm_out, const int32_t* frames, int B, int F,
                             int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Tacotron2 inference (text -> mel spectrogram, autoregressive attention decoder) -----------------------------
+ * Replaces Tacotron2.inference (TTS/tts/models/tacotron2.py:238-300) in three calls:
+ *   encode      - embedding + Encoder.inference (TTS/tts/layers/tacotron/tacotron2.py:105-112): 3 x ConvBNBlock (eval
+ *                 BatchNorm folded), bidirectional nn.LSTM (256 per direction); for the original attention also
+ *                 inputs_layer of every encoder output (step-invariant, hoisted out of the loop).
+ *   decode_loop - Decoder.inference (tacotron2.py:329-367): Prenet (common_layers.py:63-119, no bias, "bn" folded),
+ *                 attention LSTMCell (1024), OriginalAttention (location-sensitive or not, sigmoid or softmax norm) or
+ *                 MonotonicDynamicConvolutionAttention (attentions.py), decoder LSTMCell (1024), linear_projection and
+ *                 stopnet.  The loop runs chunk_steps steps per CUDA graph replay and reads 2 + B words after each chunk.
+ *   postnet     - decoder_outputs + Postnet(decoder_outputs) (tacotron2.py:47-70), BatchNorm folded.
+ * Batched, unlike the reference (which cannot batch): row b computes the reference's inference(text[b:b+1,
+ * :lengths[b]]): attention, convolutions and the BiLSTM read only a row's tokens, the postnet only its frames, and the
+ * stop rule is the one-row rule (a row stops after step t >= 1 once sigmoid(stop logit) > 0.5, or after max_steps
+ * steps).  The loop runs in FP32 on the FMA pipe, so the stop decisions do not depend on tensor-core rounding.
+ * Fixed widths (as the reference hard-codes them): embedding / encoder 512, attention RNN and decoder RNN 1024,
+ * attention 128, prenet 256.
+ * weights (host, PyTorch layouts), in this order:
+ *   embedding.weight [n_vocab, 512]
+ *   per encoder conv i < 3: convolution1d.weight [512, 512, 5], .bias, batch_normalization.weight, .bias,
+ *     .running_mean, .running_var (eps 1e-5)
+ *   encoder.lstm.weight_ih_l0 [1024, 512], weight_hh_l0 [1024, 256], bias_ih_l0, bias_hh_l0, then the four _reverse
+ *   per prenet layer l < 2: linear_layer.weight [256, in] (in = C, then 256); prenet_bn: then batch_normalization.weight,
+ *     .bias, .running_mean, .running_var
+ *   attention_rnn.weight_ih [4096, 768], weight_hh [4096, 1024], bias_ih, bias_hh
+ *   original attention: query_layer.linear_layer.weight [128, 1024], inputs_layer.linear_layer.weight [128, 512],
+ *     v.linear_layer.weight [1, 128], .bias [1]; location_attn: location_conv1d.weight [32, 2, 31],
+ *     location_dense.linear_layer.weight [128, 32]
+ *   dynamic convolution: prior [11], query_layer.weight [128, 1024], .bias, key_layer.weight [168, 128],
+ *     static_filter_conv.weight [8, 1, 21], static_filter_layer.weight [128, 8], dynamic_filter_layer.weight [128, 8],
+ *     .bias, v.weight [1, 128]
+ *   decoder_rnn.weight_ih [4096, 1536], weight_hh [4096, 1024], bias_ih, bias_hh
+ *   linear_projection.linear_layer.weight [C * r_init, 1536], .bias; stopnet.1.linear_layer.weight
+ *     [1, 1024 + C * r_init], .bias [1]
+ *   per postnet conv i < 5: convolution1d.weight, .bias, batch_normalization.weight, .bias, .running_mean, .running_var
+ */
+typedef struct {
+    int n_vocab;
+    int out_channels;          /* C (mel channels) */
+    int r_init;                /* linear_projection has C * r_init rows */
+    int attention_type;        /* 0: "original", 1: "dynamic_convolution" */
+    int location_attn;         /* original: location-sensitive */
+    int attention_norm;        /* original: 0 sigmoid, 1 softmax */
+    int prenet_bn;             /* prenet_type "bn" */
+    int prenet_dropout;        /* 0: no dropout layer; else p = 0.5 where decode_loop is given masks */
+} b200tts_tacotron2_config;
+typedef struct b200tts_tacotron2 b200tts_tacotron2;
+int b200tts_tacotron2_create(const b200tts_tacotron2_config* cfg, const float* const* weights, int num_weights,
+                             b200tts_tacotron2** out);
+void b200tts_tacotron2_destroy(b200tts_tacotron2* h);
+/* one workspace serves all three calls of an utterance batch: B rows of up to Tt tokens and up to F mel frames */
+size_t b200tts_tacotron2_workspace_bytes(const b200tts_tacotron2* h, int B, int Tt, int F);
+/* tokens int64 [B, Tt], lengths int64 [B] (1 .. Tt) -> enc_out [B, Tt, 512] (zero past lengths[b]); the hoisted
+ * inputs_layer term stays in the workspace for decode_loop() */
+int b200tts_tacotron2_encode(const b200tts_tacotron2* h, const int64_t* tokens, const int64_t* lengths, int B, int Tt,
+                             float* enc_out, void* workspace, size_t workspace_bytes, void* stream);
+/* the decoder loop on encode()'s state in the same workspace.  r: reduction rate (1 .. r_init); max_steps: decoder
+ * steps at most (>= 1); drop (nullable; used with prenet_dropout only): uint8 [B, max_steps, 2, 256], nonzero keeps a
+ * unit (doubled), null runs the prenet without dropout;
+ * chunk_steps: steps per graph replay (even).  Out (device, zero past each row): dec_out [B, max_steps * r, C],
+ * stop_tokens [B, max_steps] (sigmoid values), alignments [B, max_steps, Tt]; steps (host int32 [B]): decoder steps per
+ * row (frames = steps * r).  Synchronises the stream. */
+int b200tts_tacotron2_decode_loop(const b200tts_tacotron2* h, const int64_t* lengths, const float* enc_out, int B,
+                                  int Tt, int r, int max_steps, const uint8_t* drop, int chunk_steps, float* dec_out,
+                                  float* stop_tokens, float* alignments, int32_t* steps, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+/* dec_out [B, Fpitch, C], frames (device int32 [B]) -> mel [B, F, C] = dec_out + Postnet(dec_out) below frames[b],
+ * zero past it */
+int b200tts_tacotron2_postnet(const b200tts_tacotron2* h, const float* dec_out, const int32_t* frames, int B, int F,
+                              int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -182,7 +182,9 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // Overflow / Neural-HMM (overflow.cu): the BiLSTM time step, the LSTMCell, a GEMV layer, the frame epilogue
              DISPATCH_LSTM_BI = 18, DISPATCH_LSTM_CELL = 19, DISPATCH_HMM_LINEAR = 20, DISPATCH_HMM_STEP = 21,
              // Parallel WaveGAN (pwgan.cu): the fused residual layer, the folded conditioning conv
-             DISPATCH_PWGAN_TC = 22, DISPATCH_PWGAN_AUX = 23 };
+             DISPATCH_PWGAN_TC = 22, DISPATCH_PWGAN_AUX = 23,
+             // Tacotron2 (tacotron2.cu): the attention step, the step epilogue; the LSTMCell with 32 rows per weight read
+             DISPATCH_TACO_ATTN = 24, DISPATCH_TACO_STEP = 25, DISPATCH_LSTM_CELL32 = 26 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -2,6 +2,7 @@
 // across streams/threads; all scratch comes from the caller's workspace.
 #pragma once
 #include <algorithm>
+#include <functional>
 #include <string.h>
 
 #include "../../include/tts_b200.h"
@@ -247,18 +248,83 @@ struct GlowTTS {
                float* y_log_scale, float* mel, void* ws, size_t ws_bytes, cudaStream_t st) const;
 };
 
-// Overflow / Neural-HMM inference (overflow.cu).  encode: embedding, 3 x (conv k5 with BatchNorm folded -> ReLU), the
-// LSTM input projection of both directions as one 1x1 conv, then one BiLSTM launch per time step (lstm_bi); the encoder
-// states [B, Tt*spp, E] and the hoisted encoder-state part of the output net's first layer (W_z z + b for every state).
-// sample: the autoregressive loop, chunk_frames frames per CUDA graph replay, one host read per chunk.  decode
+// ---- recurrent building blocks of the autoregressive text-to-mel models (recurrent.cu), exact FP32 on the FMA pipe
+// One LSTM input segment: columns [0, K) of W (row stride ldw) times x[b, 0:K] (batch stride x_bs); w_ds / x_ds: the
+// offsets of direction blockIdx.y (BiLSTM).
+struct LstmSeg {
+    const float* W = nullptr; int ldw = 0; long long w_ds = 0;
+    const float* x = nullptr; int x_bs = 0; long long x_ds = 0;
+    int K = 0;
+};
+// One LSTM time step (launch_lstm): gates = sum over the segments W_s x_s, plus
+//   pre[b, d*4H + row, t]   (BiLSTM: pre = W_ih x + b_ih + b_hh for every token; direction d; forward t = step, backward
+//                            t = len_b - 1 - step; rows with step >= len_b skip), or
+//   bias                    (LSTMCell: bias = b_ih + b_hh; rows with done[b] set skip)
+// c = f c + i g, h = o tanh(c) -> c (in place, [dirs][B][H]), h_out[d * st_ds + b * h_bs + j], out[b, t, d*H + j]
+struct LstmArgs {
+    LstmSeg seg[3]; int nseg = 0;
+    int H = 0;
+    float* h_out = nullptr; int h_bs = 0; float* c = nullptr; long long st_ds = 0;
+    const float* bias = nullptr;
+    const float* pre = nullptr; long long pre_bs = 0; int pre_cs = 0;
+    float* out = nullptr; long long out_bs = 0; int out_ts = 0;
+    const long long* lens = nullptr; int step = 0;
+    const int* done = nullptr;
+    int B = 0;
+};
+// rows_per_block (8 or 32): batch rows served by one weight read; a row's result does not depend on it.
+int launch_lstm(const LstmArgs& a, int dirs, int rows_per_block, int dispatch_id, cudaStream_t st, bool note);
+// y[b, r] = act(W[r] . [x[b, 0:K] | x2[b, 0:K2]] + bias[r] + add[b, r, state[b]]), then the prenet dropout
+// (drop[b, ctl[1], drop_layer, r] ? 2v : 0, drop [B, drop_F, drop_L, R]); rows with done[b] set skip.
+struct LinArgs {
+    const float* W = nullptr; const float* bias = nullptr; int K = 0, R = 0;
+    const float* x = nullptr; int x_bs = 0;
+    const float* x2 = nullptr; int x2_bs = 0, K2 = 0;
+    float* y = nullptr; int y_bs = 0;
+    const float* add = nullptr; long long add_bs = 0; int add_rs = 0; const int* state = nullptr;
+    int relu = 0;
+    const unsigned char* drop = nullptr; int drop_layer = 0, drop_L = 0, drop_F = 0; const int* ctl = nullptr;
+    const int* done = nullptr;
+    int B = 0;
+};
+int launch_linear(const LinArgs& a, cudaStream_t st, bool note);
+// y[b, c, n] = x[b, n, c] for x [B, N, E]
+int launch_transpose(const float* x, float* y, int B, int N, int E, cudaStream_t st);
+// An autoregressive loop as CUDA-graph chunks: step(stream, parity, note) enqueues one step (parity = step index within
+// the chunk, even chunk); `chunk` steps are captured once and replayed until ctl[0] (rows still running) reads 0 or
+// max_steps steps have run, with one read of ctl [2 + B] words into host after each chunk.
+int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_step,
+                   const std::function<int(cudaStream_t, int, bool)>& step, const int* ctl, int B, std::vector<int>& host,
+                   cudaStream_t st);
+
+// The Tacotron2 text encoder (TTS/tts/layers/tacotron/tacotron2.py:73-112, also Overflow's encoder): embedding,
+// n_convs x (conv k5 with BatchNorm folded -> ReLU), the LSTM input projection of both directions as one 1x1 conv, then
+// one BiLSTM launch per time step (lstm_bi), each row at its own length.
+struct SeqEncoder {
+    int n_vocab = 0, E = 0, H = 0, n_convs = 0;   // H: LSTM hidden size per direction
+    float* emb = nullptr;
+    ConvLayer convs[8], lstm_in;
+    float* whh = nullptr;                         // [2][4H][H]
+    ~SeqEncoder();
+    // w: emb [n_vocab, E]; per conv: weight [E, E, 5], bias, BN weight, bias, running_mean, running_var;
+    // lstm weight_ih, weight_hh, bias_ih, bias_hh, then the same four _reverse
+    int init(int n_vocab, int E, int H, int n_convs, const float* const* w, int* consumed);
+    size_t workspace_bytes(int B, int Tt) const;
+    // out [B, Tt, 2H], zero past each row's length; scratch from ar
+    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* out, Arena& ar,
+               cudaStream_t st) const;
+};
+
+// Overflow / Neural-HMM inference (overflow.cu).  encode: the SeqEncoder (hidden E / 2 * spp per direction) into the
+// encoder states [B, Tt*spp, E] and the hoisted encoder-state part of the output net's first layer (W_z z + b for every
+// state).  sample: the autoregressive loop, chunk_frames frames per CUDA graph replay, one host read per chunk.  decode
 // (Overflow only): the Glow decoder in reverse and x * std + mean.
 struct Overflow {
     b200tts_overflow_config c;
     int H = 0;                         // LSTM hidden size per direction: E / 2 * state_per_phone
     int O1 = 0;                        // output-net first-layer width
-    float* emb = nullptr;
-    ConvLayer convs[8], lstm_in, zproj;
-    float *whh = nullptr;              // [2][4H][H]
+    SeqEncoder enc;
+    ConvLayer zproj;
     std::vector<float*> prenet_w;      // [P][in] (no bias)
     float *mem_wih = nullptr, *mem_whh = nullptr, *mem_b = nullptr;   // [4M][P], [4M][M], b_ih + b_hh
     std::vector<float*> out_w, out_b;  // layer 0: the h part [O1][M]; layers 1..: [O_l][O_{l-1}]; last [2C+1][O_last]
@@ -276,6 +342,39 @@ struct Overflow {
                void* ws, size_t ws_bytes, cudaStream_t st) const;
     int decode(const float* hmm_out, const int* frames, int B, int F, int Fpitch, float* mel, void* ws, size_t ws_bytes,
                cudaStream_t st) const;
+};
+
+// Tacotron2 inference (tacotron2.cu).  encode: the SeqEncoder (hidden 256 per direction) into the encoder outputs
+// [B, Tt, 512] and, for the original attention, inputs_layer of them for every token as one 1x1 conv.  decode_loop: the
+// attention decoder, chunk_steps steps per CUDA graph replay, one host read per chunk.  postnet: the 5 ConvBNBlocks
+// (BatchNorm folded) on the conv engine, masked past each row's frames, plus the decoder output.
+struct Tacotron2 {
+    b200tts_tacotron2_config c;
+    SeqEncoder enc;
+    ConvLayer inproj;                  // attention.inputs_layer as a 1x1 conv (original attention)
+    ConvLayer post[5];
+    float *prenet_w[2] = {nullptr, nullptr}, *prenet_b[2] = {nullptr, nullptr};   // bias: the folded "bn" prenet only
+    float *arnn_wih = nullptr, *arnn_whh = nullptr, *arnn_b = nullptr;   // [4096][768], [4096][1024], b_ih + b_hh
+    float *drnn_wih = nullptr, *drnn_whh = nullptr, *drnn_b = nullptr;   // [4096][1536], [4096][1024], b_ih + b_hh
+    float *att_wq = nullptr, *att_bq = nullptr, *att_v = nullptr, *att_wc = nullptr, *att_wd = nullptr;
+    float *att_prior = nullptr, *att_wk = nullptr, *att_ws = nullptr, *att_wsl = nullptr, *att_wdl = nullptr,
+          *att_bdl = nullptr;
+    float att_vb = 0.f;
+    float *proj_w = nullptr, *proj_b = nullptr, *stop_w = nullptr, *stop_b = nullptr;
+    std::vector<float*> dev;           // every buffer above, freed together
+    ~Tacotron2();
+    int init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw);
+    size_t persist_bytes(int B, int Tt) const;
+    size_t workspace_bytes(int B, int Tt, int F) const;
+    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
+               size_t ws_bytes, cudaStream_t st) const;
+    int decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
+                    const unsigned char* drop, int chunk_steps, float* dec_out, float* stop_tokens, float* alignments,
+                    int* steps, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    int postnet(const float* dec_out, const int* frames, int B, int F, int Fpitch, float* mel, void* ws,
+                size_t ws_bytes, cudaStream_t st) const;
+  private:
+    int up(float** dst, const float* src, size_t n);
 };
 
 // ForwardTTS inference (forward_tts.cu): FastPitch / FastSpeech / FastSpeech2 with FFTransformer encoder and decoder.
