@@ -725,6 +725,52 @@ int b200tts_pwgan_layer(const b200tts_pwgan* h, int layer, const float* mel, int
 /* the upsampler's linear map alone, as the layers apply it: a [rows, Tf] (device) -> out [rows, Tf * P] */
 int b200tts_pwgan_upsample(const b200tts_pwgan* h, const float* a, int rows, int Tf, float* out, void* stream);
 
+/* ---- UnivNet generator (vocoder) ----------------------------------------------------------------------------------
+ * Replaces UnivnetGenerator.forward (TTS/vocoder/models/univnet_generator.py, LVCBlock / KernelPredictor in
+ * TTS/vocoder/layers/lvc_block.py) on supplied noise.  Per block: the kernel predictor runs at frame rate on the conv
+ * engine, kernel_conv | bias_conv as one split-fp16 tensor-core GEMM writing the kernels frame-major, the transposed
+ * upsampler on the conv engine, and one fused split-fp16 tensor-core launch per LVC layer.  hidden_channels must be 32
+ * and lvc_kernel_size 3; kpnet_hidden_channels a multiple of 16; kpnet_conv_size odd.
+ * weights (host pointers, PyTorch layouts, weight norm folded):
+ *   first_conv.w [32, in, 7], .b [32]
+ *   per block n: upsample.w [32, 32, 2 u_n], .b [32]
+ *                kernel_predictor.input_conv.0.w [Ch, cond, 5], .b
+ *                kernel_predictor.residual_conv.{1,3,6,8,11,13}.w [Ch, Ch, Kp], .b   (six convs, in that order)
+ *                kernel_predictor.kernel_conv.w [L * 32 * 64 * 3, Ch, Kp], .b
+ *                kernel_predictor.bias_conv.w [L * 64, Ch, Kp], .b
+ *                per layer i < L: convs.i.w [32, 32, 3], .b
+ *   last_conv_layers.0.w [out, 32, 7], .b
+ * (Ch = kpnet_hidden_channels, Kp = kpnet_conv_size, L = lvc_layers) */
+typedef struct {
+    int in_channels, out_channels, hidden_channels, cond_channels;
+    int num_upsamples;                 /* 1 .. 8 */
+    int upsample_factors[8];           /* product at most 4096 */
+    int lvc_layers;                    /* lvc_layers_each_block, 1 .. 8 */
+    int lvc_kernel_size;
+    int kpnet_hidden_channels, kpnet_conv_size;
+} b200tts_univnet_config;
+typedef struct b200tts_univnet b200tts_univnet;
+int b200tts_univnet_create(const b200tts_univnet_config* cfg, const float* const* weights, int num_weights,
+                           b200tts_univnet** out);
+void b200tts_univnet_destroy(b200tts_univnet* h);
+/* scratch for B rows of T frames: one block's predicted kernels (B * T * L * 6208 floats) dominate */
+size_t b200tts_univnet_workspace_bytes(const b200tts_univnet* h, int B, int T);
+/* mel [B, cond, T], noise [B, in, T] (device, dense) -> out [B, out, T * prod(upsample_factors)].  Split-fp16 range: an
+ * activation or predicted kernel with |v| >= 65504 makes the next launch on the device fail (once), as for the conv
+ * engine's split-fp16 layers. */
+int b200tts_univnet_forward(const b200tts_univnet* h, const float* mel, const float* noise, int B, int T, float* out,
+                            void* workspace, size_t workspace_bytes, void* stream);
+/* block `block`'s kernel predictor alone: mel [B, cond, T] -> pred [B * T][L * 6208] frame-major; per frame the kernels
+ * [layer][co 64][tap * 32 + ci] (channel ((l * 32 + ci) * 64 + co) * 3 + tap of kernel_conv), then the biases
+ * [layer][co 64].  Workspace: at least b200tts_univnet_workspace_bytes(h, B, T). */
+int b200tts_univnet_predict(const b200tts_univnet* h, int block, const float* mel, int B, int T, float* pred,
+                            void* workspace, size_t workspace_bytes, void* stream);
+/* LVC layer `layer` of block `block` alone, as forward runs it: x [B, 32, pitch] (columns [0, T * hop_block) used) and
+ * pred as b200tts_univnet_predict writes it -> x_new [B, 32, pitch] (never the buffer x is; only those columns are
+ * written). */
+int b200tts_univnet_lvc_layer(const b200tts_univnet* h, int block, int layer, const float* x, const float* pred, int B,
+                              int T, float* x_new, int pitch, void* stream);
+
 /* ---- Overflow / Neural-HMM inference (text -> mel spectrogram, autoregressive) ----------------------------------
  * Replaces Overflow.inference (TTS/tts/models/overflow.py:207-246) and NeuralhmmTTS.inference
  * (TTS/tts/models/neuralhmm_tts.py) in three calls:

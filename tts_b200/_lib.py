@@ -103,6 +103,13 @@ class PwganConfigC(ctypes.Structure):
                [("upsample_factors", ctypes.c_int * 8)]
 
 
+class UnivnetConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("in_channels", "out_channels", "hidden_channels", "cond_channels",
+                                            "num_upsamples")] + \
+               [("upsample_factors", ctypes.c_int * 8)] + \
+               [(n, ctypes.c_int) for n in ("lvc_layers", "lvc_kernel_size", "kpnet_hidden_channels", "kpnet_conv_size")]
+
+
 # padding modes of b200tts_conv1d_create_padded (B200TTS_PAD_* in include/tts_b200.h)
 PADDING_MODES = {"zeros": 0, "reflect": 1}
 
@@ -116,7 +123,8 @@ class AudioNormC(ctypes.Structure):
 DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9: "tc16_grouped", 10: "attn_tc3",
                   11: "attn_fma", 12: "tc3w_tf32", 13: "tc3w_tf32_near", 14: "tc3w_f16x3", 15: "tc3w_f16x3_near",
                   16: "fma_wg", 17: "fma_wg_near", 18: "lstm_bi", 19: "lstm_cell", 20: "hmm_linear", 21: "hmm_step",
-                  22: "pwgan_tc", 23: "pwgan_aux", 24: "taco_attn", 25: "taco_step", 26: "lstm_cell32"}
+                  22: "pwgan_tc", 23: "pwgan_aux", 24: "taco_attn", 25: "taco_step", 26: "lstm_cell32",
+                  27: "univnet_predict", 28: "univnet_lvc"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}
@@ -189,6 +197,18 @@ def _declare(lib):
     lib.b200tts_pwgan_layer.argtypes = [vp, ci, vp, ci, ci, ci, vp, vp, vp, ci, vp, sz, vp]
     lib.b200tts_pwgan_upsample.restype = ci
     lib.b200tts_pwgan_upsample.argtypes = [vp, vp, ci, ci, vp, vp]
+    lib.b200tts_univnet_create.restype = ci
+    lib.b200tts_univnet_create.argtypes = [ctypes.POINTER(UnivnetConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+    lib.b200tts_univnet_destroy.restype = None
+    lib.b200tts_univnet_destroy.argtypes = [vp]
+    lib.b200tts_univnet_workspace_bytes.restype = sz
+    lib.b200tts_univnet_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_univnet_forward.restype = ci
+    lib.b200tts_univnet_forward.argtypes = [vp, vp, vp, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_univnet_predict.restype = ci
+    lib.b200tts_univnet_predict.argtypes = [vp, ci, vp, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_univnet_lvc_layer.restype = ci
+    lib.b200tts_univnet_lvc_layer.argtypes = [vp, ci, ci, vp, vp, ci, ci, vp, ci, vp]
     lib.b200tts_pqmf_synthesis.restype = ci
     lib.b200tts_pqmf_synthesis.argtypes = [vp, ci, ci, ci, vp, ci, vp, vp, vp]
     lib.b200tts_conv1d_destroy.restype = None

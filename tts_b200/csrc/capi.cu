@@ -20,6 +20,7 @@ struct b200tts_wavegrad { Wavegrad impl; };
 struct b200tts_overflow { Overflow impl; };
 struct b200tts_tacotron2 { Tacotron2 impl; };
 struct b200tts_pwgan { Pwgan impl; };
+struct b200tts_univnet { Univnet impl; };
 
 extern "C" {
 
@@ -513,6 +514,24 @@ int b200tts_pwgan_layer(const b200tts_pwgan* h, int layer, const float* mel, int
 int b200tts_pwgan_upsample(const b200tts_pwgan* h, const float* a, int rows, int Tf, float* out, void* stream) {
     if (!h) { set_error("pwgan_upsample: null handle"); return 1; }
     return h->impl.upsample(a, rows, Tf, out, (cudaStream_t)stream);
+}
+
+B200_HANDLE_API(univnet, b200tts_univnet, b200tts_univnet_config)
+
+int b200tts_univnet_forward(const b200tts_univnet* h, const float* mel, const float* noise, int B, int T, float* out,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("univnet_forward: null handle"); return 1; }
+    return h->impl.forward(mel, noise, B, T, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_univnet_predict(const b200tts_univnet* h, int block, const float* mel, int B, int T, float* pred,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("univnet_predict: null handle"); return 1; }
+    return h->impl.predict(block, mel, B, T, pred, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_univnet_lvc_layer(const b200tts_univnet* h, int block, int layer, const float* x, const float* pred, int B,
+                              int T, float* x_new, int pitch, void* stream) {
+    if (!h) { set_error("univnet_lvc_layer: null handle"); return 1; }
+    return h->impl.lvc_layer(block, layer, x, pred, B, T, x_new, pitch, (cudaStream_t)stream);
 }
 
 int b200tts_overflow_create(const b200tts_overflow_config* cfg, const float* const* weights, int num_weights,

@@ -184,7 +184,9 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // Parallel WaveGAN (pwgan.cu): the fused residual layer, the folded conditioning conv
              DISPATCH_PWGAN_TC = 22, DISPATCH_PWGAN_AUX = 23,
              // Tacotron2 (tacotron2.cu): the attention step, the step epilogue; the LSTMCell with 32 rows per weight read
-             DISPATCH_TACO_ATTN = 24, DISPATCH_TACO_STEP = 25, DISPATCH_LSTM_CELL32 = 26 };
+             DISPATCH_TACO_ATTN = 24, DISPATCH_TACO_STEP = 25, DISPATCH_LSTM_CELL32 = 26,
+             // UnivNet (univnet.cu): the kernel-prediction GEMM, the fused LVC layer
+             DISPATCH_UNIVNET_PREDICT = 27, DISPATCH_UNIVNET_LVC = 28 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

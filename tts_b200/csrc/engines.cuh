@@ -470,6 +470,42 @@ struct Pwgan {
                      int* err, int num_sms, cudaStream_t st) const;
 };
 
+// UnivNet generator (univnet.cu): first_conv, per block the kernel predictor on the conv engine (frame rate) feeding one
+// split-fp16 tensor-core GEMM that writes the predicted kernels frame-major, the transposed upsampler on the conv engine
+// and one fused launch per LVC layer (conv_i + location-variable conv + gate + residual), then last_conv + tanh.
+// hidden_channels 32, lvc_kernel_size 3.
+struct Univnet {
+    struct Block {
+        ConvLayer up, kin;                        // upsample (ConvTranspose1d), kernel_predictor.input_conv
+        std::vector<ConvLayer> kres;              // the six residual_conv convs
+        float *pw = nullptr, *pb = nullptr;       // kernel_conv | bias_conv, rows permuted: [MP][Kp * Ch] (tap-major), [MP]
+        float *cw = nullptr, *cb = nullptr;       // conv_i: [L][32][3 * 32] (tap-major), [L][32]
+        int hop = 1;                              // cumulative hop of this block
+    };
+    b200tts_univnet_config c;
+    ConvLayer first, last;
+    std::vector<Block> blocks;
+    int hop_total = 1;                            // prod(upsample_factors)
+    int MP = 0;                                   // floats of one frame's predicted kernels and biases: L * (6144 + 64)
+    ~Univnet();
+    int init(const b200tts_univnet_config& cfg, const float* const* w, int nw);
+    size_t workspace_bytes(int B, int T) const;
+    // mel [B, cond, T], noise [B, in, T] -> out [B, out, T * hop_total]
+    int forward(const float* mel, const float* noise, int B, int T, float* out, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+    // block blk's predicted kernels and biases alone: P [B * T][MP] (frame-major, layout in univnet.cu)
+    int predict(int blk, const float* mel, int B, int T, float* P, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    // LVC layer l of block blk alone: x [B, 32, pitch] -> x_new, P as predict() writes it
+    int lvc_layer(int blk, int l, const float* x, const float* P, int B, int T, float* x_new, int pitch,
+                  cudaStream_t st) const;
+  private:
+    int check_call(const char* who, int B, int T) const;
+    int launch_predict(int blk, const float* mel, int B, int T, float* P, float* H0, float* H1, float* H2, int* err,
+                       cudaStream_t st) const;
+    int launch_lvc(int blk, int l, const float* x, float* xn, int B, int T, int pitch, const float* P, int* err,
+                   cudaStream_t st) const;
+};
+
 // WaveGrad (wavegrad.cu): the refinement network on the shared conv engine.  Down path y_conv -> FiLM[0] -> per DBlock
 // [res (1x1), three lrelu -> k3 convs, dilations 1 / 2 / 4, on the decimated input] -> FiLM[i+1]; up path x_conv ->
 // per UBlock [res (1x1) and main0 on the nearest-upsampled input, main1, out0, out1 with the FiLM pair of its rate] ->

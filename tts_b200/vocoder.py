@@ -7,7 +7,8 @@ Mirrors, with the reference's names and argument meaning:
                        <- TTS/vocoder/configs/{melgan,multiband_melgan,fullband_melgan}_config.py (generator side)
   ParallelWaveganConfig
                        <- TTS/vocoder/configs/parallel_wavegan_config.py (generator side)
-  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-94   (HiFiGAN, the MelGAN family, Parallel WaveGAN)
+  UnivnetConfig        <- TTS/vocoder/configs/univnet_config.py (generator side)
+  setup_generator(c)   <- TTS/vocoder/models/__init__.py:34-94   (HiFiGAN, the MelGAN family, Parallel WaveGAN, UnivNet)
   GAN                  <- TTS/vocoder/models/gan.py:21-66,338-352 (model_g, forward, inference, load_checkpoint)
   AudioProcessor.normalize / denormalize   <- TTS/utils/audio/processor.py:259-337   (as ``AudioNorm``)
   interpolate_vocoder_input                <- TTS/vocoder/utils/generic_utils.py:11-29
@@ -18,6 +19,7 @@ Mirrors, with the reference's names and argument meaning:
 Everything numeric runs in libtts_b200.so (``b200tts_vocoder_input`` / ``b200tts_absmax`` / ``b200tts_to_int16``).
 """
 import ctypes
+import inspect
 import math
 from dataclasses import dataclass, field
 from typing import Optional
@@ -29,6 +31,7 @@ from . import _lib
 from .hifigan import HifiganGenerator
 from .melgan import FullbandMelganGenerator, MelganGenerator, MultibandMelganGenerator
 from .pwgan import ParallelWaveganGenerator
+from .univnet import UnivnetGenerator
 
 
 # ----------------------------------------------------------------------------- configs
@@ -134,6 +137,25 @@ class ParallelWaveganConfig(_ItemAccess):
     audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
 
 
+@dataclass
+class UnivnetConfig(_ItemAccess):
+    """Generator-side fields of TTS/vocoder/configs/univnet_config.py; ``__post_init__`` sets
+    ``generator_model_params["cond_channels"]`` to ``audio.num_mels``, as the reference does."""
+    model: str = "univnet"
+    batch_size: int = 32
+    discriminator_model: str = "univnet_discriminator"
+    generator_model: str = "univnet_generator"
+    generator_model_params: dict = field(
+        default_factory=lambda: {"in_channels": 64, "out_channels": 1, "hidden_channels": 32, "cond_channels": 80,
+                                 "upsample_factors": [8, 8, 4], "lvc_layers_each_block": 4, "lvc_kernel_size": 3,
+                                 "kpnet_hidden_channels": 64, "kpnet_conv_size": 3, "dropout": 0.0})
+    use_pqmf: bool = False
+    audio: BaseAudioConfig = field(default_factory=BaseAudioConfig)
+
+    def __post_init__(self):
+        self.generator_model_params["cond_channels"] = self.audio.num_mels
+
+
 # the generator modules under TTS/vocoder/models/ that setup_generator can import
 _GENERATOR_MODULES = ("hifigan_generator", "melgan_generator", "multiband_melgan_generator", "fullband_melgan_generator",
                       "parallel_wavegan_generator", "univnet_generator")
@@ -142,6 +164,11 @@ _GENERATOR_MODULES = ("hifigan_generator", "melgan_generator", "multiband_melgan
 class GeneratorParamsError(KeyError, NotImplementedError):
     """``generator_model_params`` lacks a field the named generator needs (the reference raises KeyError there); also a
     NotImplementedError, so that callers that treat an unbuildable generator as such keep working."""
+
+
+class GeneratorParamsTypeError(TypeError, NotImplementedError):
+    """``generator_model_params`` does not fit the named generator's constructor (the reference raises the TypeError of
+    ``MyModel(**params)``); also a NotImplementedError, as GeneratorParamsError is."""
 
 
 def to_camel(text):
@@ -157,7 +184,8 @@ def setup_generator(c):
     raises NotImplementedError here (the reference fails it at that import).  ``melgan_fb_generator`` raises the
     reference's ValueError ("now fullband_melgan_generator").  HiFiGAN, the MelGAN family and Parallel WaveGAN are on
     the path (Parallel WaveGAN reads num_res_blocks, stacks and upsample_factors, in the reference's order, so a config
-    without ``stacks`` -- a MelGAN one -- raises GeneratorParamsError); UniVNet raises NotImplementedError."""
+    without ``stacks`` -- a MelGAN one -- raises GeneratorParamsError).  UnivNet is built from ``generator_model_params``
+    alone, as the reference does; params that do not fit its constructor raise GeneratorParamsTypeError."""
     name = _get(c, "generator_model")
     low = name.lower()
     if name == "melgan_fb_generator":
@@ -193,8 +221,14 @@ def setup_generator(c):
                                         num_res_blocks=param("num_res_blocks"), stacks=param("stacks"), res_channels=64,
                                         gate_channels=128, skip_channels=64, aux_channels=num_mels, dropout=0.0,
                                         bias=True, use_weight_norm=True, upsample_factors=param("upsample_factors"))
-    raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN, MelGAN and Parallel "
-                              "WaveGAN generators are)")
+    if low in "univnet_generator":
+        try:
+            inspect.signature(UnivnetGenerator).bind(**dict(params))
+        except TypeError as e:
+            raise GeneratorParamsTypeError(f"tts_b200.setup_generator: `{name}`: {e}") from None
+        return UnivnetGenerator(**dict(params))
+    raise NotImplementedError(f"tts_b200.setup_generator: `{name}` is not built (the HiFiGAN, MelGAN, Parallel "
+                              "WaveGAN and UnivNet generators are)")
 
 
 def setup_model(config):
