@@ -70,6 +70,15 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// shared -> global bulk copy in the issuing thread's bulk async-group; `commit` closes the group.  `wait_read` returns
+// once the thread's groups have finished reading shared memory (the source may be rewritten), `wait_all` once their writes
+// are complete (visible to a grid that depends on this one).
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // wgmma shared-memory descriptor: K-major, no swizzle; start address, LBO (between the two 16-byte K chunks),

@@ -7,6 +7,9 @@
 //                           accumulators to a shared [128][ACC_LD] tile and all eight warps run the epilogue from it
 //                           (warp w: rows 32 (w & 3) .. + 31, columns 128 (w >> 2) .. + 127).  A warpgroup starts the next
 //                           tile's MMAs as soon as its own epilogue is done; the tile is only rewritten after both are.
+//                           Whole interior tiles of plain layers without an accumulate operand skip that shared step:
+//                           each warp finishes its own 16 rows in place, with the residual prefetched into them by
+//                           cp.async.bulk during the MMAs, and writes them out with bulk stores (the bulk epilogue).
 //   warps 8-10  producers : cp.async raw [8 ch][time] windows (NRAW-deep ring) -> leaky-ReLU + hi/lo split -> K-major slabs
 //                           (NA2 stages)
 //   warp  11    loader    : per-tap weight blocks {hi,lo}[2 slabs][128 rows][4] by cp.async.bulk, one lane per ring slot
@@ -203,6 +206,26 @@ __device__ __forceinline__ void lean_tile(const float* at, const float* bias, co
     for (int cg = 0; cg < 128; cg += 32) {
         group(cg, r0, r1);
         group(cg + 16, r1, r0);
+    }
+}
+
+// Bulk epilogue of one consumer warp (whole interior tiles of the plain layers without an accumulate operand): the
+// warp's 16 MMA rows are finished in place in the shared accumulator tile, where its accumulator fragment would be stored
+// (st_row, see the consumers), each element as lean_tile computes it: ((acc * rscale) + (bias + cond)) + res.  HR: the
+// rows already hold the tile's residual (prefetched by cp.async.bulk during the MMAs).  bv / sv: rows lane / 4 and + 8.
+template <bool HR, bool SC>
+__device__ __forceinline__ void bulk_combine(const float* d, float* st_row, const float (&bv)[2], const float (&sv)[2]) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float2* p = reinterpret_cast<float2*>(st_row + h * 8 * ACC_LD + 8 * j);
+            float2 t = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+            if constexpr (SC) { t.x *= sv[h]; t.y *= sv[h]; }
+            t.x += bv[h]; t.y += bv[h];
+            if constexpr (HR) { const float2 r = *p; t.x += r.x; t.y += r.y; }
+            *p = t;
+        }
     }
 }
 
@@ -517,6 +540,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     constexpr int SLC = PREC != PREC_FP32 ? 8 : 4;   // channels per slab row
     constexpr int NB = NB2;                      // weight ring depth
     constexpr bool SC = X3;                      // epilogues scale rows by rscale
+    constexpr bool BULK = GRP == 1 && LEAN;      // plain-layer kernel: whole interior tiles may take the bulk epilogue
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ROWS = a.rows_pad, RAWW = a.raw_w, K = a.KJ;
     const uint32_t rawStage = (uint32_t)RCH * RAWS * 4;
@@ -527,7 +551,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     unsigned char* smB = smA + NA2 * stageA;
     float* accs = reinterpret_cast<float*>(smB + NB * stageB);
     uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(accs) + ACC_BYTES);
-    const int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB;
+    const int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB, RES_FULL = 2 * NA2 + 2 * NB;
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
 
@@ -563,6 +587,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     if (tid == 0) {
         for (int i = 0; i < NA2; ++i) { mbar_init(BAR(A_FULL + i), NPW); mbar_init(BAR(A_EMPTY + i), NCONS / 32); }
         for (int i = 0; i < NB; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), NCONS / 32); }
+        for (int i = 0; i < NCONS / 32; ++i) mbar_init(BAR(RES_FULL + i), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -834,8 +859,43 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         int sa = 0; uint32_t pa = 0;                                                         // activation stage / its parity
         int sb = 0; uint32_t pb = 0;                                                         // weight slot / its parity
         float* const st_row = accs + (wg * 64 + lq * 16 + (lane >> 2)) * ACC_LD + 2 * (lane & 3);
+        // Bulk epilogue: in a plain layer without an accumulate operand, a whole interior tile (q0 + 256 <= Tout) is
+        // finished by each warp on its own 16 rows, which hold all 256 columns of the warp's accumulator fragment.  Before
+        // the tile's MMAs lane 0 prefetches those rows of the residual into the warp's rows of `accs` (cp.async.bulk, 1 KB
+        // per row, completing on RES_FULL[warp]); after them the warp adds bias and residual in place and lane 0 writes
+        // the rows out with bulk stores.  No consumer-wide barrier is needed: no other warp touches these rows, except
+        // in the shared-tile epilogue of the other tiles (edge tiles, accumulate and general-epilogue layers), which
+        // is fenced off by a barrier when a bulk tile follows it and by the warp's bulk_wait_read when it follows one.
+        // The residual may alias y: a tile reads and writes only its own columns, and only the next tile is prefetched.
+        const int row_w = wg * 64 + lq * 16;            // this warp's first tile row
+        const bool bulk_layer = BULK && a.ups == 1 && !a.gate && a.split == 0 && !a.relu && !a.ymask &&
+                                a.scale == 1.f && a.post_div == 1.f && a.accum == 0 &&
+                                ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
+                                (!a.res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
+        uint32_t pr = 0;                                // parity of RES_FULL[warp]
+        bool shared_epi = false;                        // the previous tile's epilogue read other warps' rows of `accs`
 #pragma unroll 1
         for (int it = 0; it < my_tiles; ++it) {
+            bool bulk, pre;                             // bulk epilogue; residual prefetched (rows of this warp < Rows)
+            {
+                int b, rt, q0;
+                decode(it, b, rt, q0);
+                const int nrows = min(16, a.Rows - (rt * MROWS + row_w));
+                bulk = bulk_layer && q0 + TT2 <= a.Tout;
+                pre = bulk && a.res != nullptr && nrows > 0;
+                if (bulk) {
+                    if (shared_epi) { fence_async_smem(); named_bar_sync(4, NCONS); }
+                    if (lane == 0) bulk_wait_read();    // this warp's previous bulk stores are done reading its rows
+                    __syncwarp();
+                }
+                if (pre && lane == 0) {
+                    const uint32_t rf = BAR(RES_FULL + warp);
+                    const float* src = a.res + (long long)b * a.res_bs + (long long)(rt * MROWS + row_w) * a.res_cs + q0;
+                    mbar_expect_tx(rf, (uint32_t)nrows * TT2 * 4);
+                    for (int r = 0; r < nrows; ++r)
+                        bulk_g2s(smem_u32(accs + (row_w + r) * ACC_LD), src + (long long)r * a.res_cs, TT2 * 4, rf);
+                }
+            }
             float d[128];                              // per tile: not live across the epilogue
 #pragma unroll
             for (int i = 0; i < 128; ++i) d[i] = 0.f;
@@ -898,6 +958,42 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             }
             wgmma_wait<0>();
             release();
+            int b, rt, q0;
+            decode(it, b, rt, q0);
+            if (bulk) {
+                if (pre) {                             // waited for even after a failed wait: the copies always land
+                    const bool landed = mbar_wait(BAR(RES_FULL + warp), pr, a.err);
+                    ok = ok && landed;
+                    pr ^= 1u;
+                }
+                shared_epi = false;
+                if (!ok) continue;
+                const int r0 = rt * MROWS + row_w, rl = r0 + (lane >> 2);
+                float bv[2], sv[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int rc = min(rl + 8 * h, a.Rows - 1);
+                    bv[h] = a.bias[rc];
+                    if (a.cond) bv[h] += __ldg(a.cond + (long long)b * a.cond_bs + rc);
+                    sv[h] = SC ? a.rscale[rc] : 1.f;
+                }
+                if (pre) bulk_combine<true, SC>(d, st_row, bv, sv);
+                else bulk_combine<false, SC>(d, st_row, bv, sv);
+                fence_async_smem();                    // the combined rows -> visible to the bulk copies (async proxy)
+                __syncwarp();
+                if (lane == 0) {
+                    const int nrows = min(16, a.Rows - r0);
+                    float* dst = a.y + (long long)b * a.y_bs + (long long)r0 * a.y_cs + q0;
+                    for (int r = 0; r < nrows; ++r)
+                        bulk_s2g(dst + (long long)r * a.y_cs, smem_u32(accs + (row_w + r) * ACC_LD), TT2 * 4);
+                    bulk_commit();
+                }
+                continue;
+            }
+            if constexpr (BULK) {
+                if (lane == 0) bulk_wait_read();       // this warp's last bulk stores are done reading its rows
+                __syncwarp();
+            }
             named_bar_sync(4, NCONS);                  // every warp is done reading the previous tile's accumulators
 #pragma unroll
             for (int j = 0; j < 32; ++j) {
@@ -905,9 +1001,8 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 *reinterpret_cast<float2*>(st_row + 8 * ACC_LD + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
             }
             named_bar_sync(4, NCONS);
+            shared_epi = true;
             if (!ok) continue;
-            int b, rt, q0;
-            decode(it, b, rt, q0);
             if constexpr (GRP > 1) {
                 grouped_tile<GRP, SC>(a, accs, b, q0, lq, half, lane);
             } else {
@@ -934,6 +1029,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     general_tile_body<SC, WG>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 }
             }
+        }
+        if constexpr (BULK) {
+            if (lane == 0) bulk_wait_all();            // the bulk stores are complete before the dependent grid may read
+            __syncwarp();
         }
     }
 }
