@@ -37,6 +37,9 @@ int b200tts_version(void);
  * and returns status 1, so neither can pass silently: a timeout for good, a range error once (that launch then clears
  * it -- the data was out of range, the device is fine). */
 int b200tts_debug_tc_error(void);
+/* Debug / test aid: the number of device buffers the library's handles hold right now, over all handles and devices of
+ * this process.  Creating a handle raises it; destroying the handle returns it to where it was. */
+long long b200tts_debug_device_buffers(void);
 
 /* Debug / test aids: record, on the calling thread, which kernel family every conv launch dispatched to.
  * ids: 0 FP32-FMA tile kernel, 3 tensor-core kernel (M = rows), 5 tensor-core kernel grouped (narrow layers), 6 single-row streaming kernel (conv_post), 7 fused ResBlock kernel,

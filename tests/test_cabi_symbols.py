@@ -27,6 +27,15 @@ def test_library_exports_every_declared_symbol():
     assert lib.b200tts_version() >= 100
 
 
+def test_library_exports_the_device_buffer_counter():
+    from tts_b200 import _lib
+
+    lib = _lib.lib()
+    assert hasattr(lib, "b200tts_debug_device_buffers")
+    assert lib.b200tts_debug_device_buffers.restype is ctypes.c_longlong
+    assert lib.b200tts_debug_device_buffers() >= 0
+
+
 def test_product_fails_loudly_without_cuda():
     import pytest
     import torch

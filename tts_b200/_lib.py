@@ -144,6 +144,7 @@ def _declare(lib):
     lib.b200tts_launch_count.restype = ctypes.c_ulonglong
     lib.b200tts_version.restype = ci
     lib.b200tts_debug_tc_error.restype = ci
+    lib.b200tts_debug_device_buffers.restype = ctypes.c_longlong
     lib.b200tts_debug_dispatch_begin.restype = None
     lib.b200tts_debug_dispatch_end.restype = ci
     lib.b200tts_debug_dispatch_end.argtypes = [vp, ci]

@@ -1,5 +1,6 @@
 // extern "C" surface of libtts_b200.so -- see include/tts_b200.h for the contract.
 #include <new>
+#include <type_traits>
 
 #include "engines.cuh"
 
@@ -22,18 +23,37 @@ struct b200tts_tacotron2 { Tacotron2 impl; };
 struct b200tts_pwgan { Pwgan impl; };
 struct b200tts_univnet { Univnet impl; };
 
+// A handle owns its device buffers through DevBuf members: copying one would free them twice, so it must not compile.
+static_assert(!std::is_copy_constructible_v<ConvLayer>);
+static_assert(!std::is_copy_constructible_v<Hifigan>);
+static_assert(!std::is_copy_constructible_v<Flow>);
+static_assert(!std::is_copy_constructible_v<TextEncoder>);
+static_assert(!std::is_copy_constructible_v<SDP>);
+static_assert(!std::is_copy_constructible_v<Stft>);
+static_assert(!std::is_copy_constructible_v<PosteriorEnc>);
+static_assert(!std::is_copy_constructible_v<DurPred>);
+static_assert(!std::is_copy_constructible_v<SpeakerEncoder>);
+static_assert(!std::is_copy_constructible_v<GlowTTS>);
+static_assert(!std::is_copy_constructible_v<Melgan>);
+static_assert(!std::is_copy_constructible_v<ForwardTTS>);
+static_assert(!std::is_copy_constructible_v<Wavegrad>);
+static_assert(!std::is_copy_constructible_v<Overflow>);
+static_assert(!std::is_copy_constructible_v<Tacotron2>);
+static_assert(!std::is_copy_constructible_v<Pwgan>);
+static_assert(!std::is_copy_constructible_v<Univnet>);
+
 extern "C" {
 
 const char* b200tts_last_error(void) { return last_error(); }
 unsigned long long b200tts_launch_count(void) { return g_launch_count; }
 int b200tts_version(void) { return 100; }
 int b200tts_debug_tc_error(void) { return conv_tc_error_flag(); }
+long long b200tts_debug_device_buffers(void) { return g_device_buffers.load(); }
 void b200tts_debug_dispatch_begin(void) { dispatch_begin(); }
 int b200tts_debug_dispatch_end(int32_t* ids, int cap) { return dispatch_end(ids, cap); }
 
 struct b200tts_conv1d {
     ConvLayer L; b200tts_conv1d_config c; int reflect = 0;   // reflect: B200TTS_PAD_REFLECT
-    ~b200tts_conv1d() { free_conv(L); }
 };
 
 static bool valid_precision(int p) {

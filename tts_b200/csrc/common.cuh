@@ -88,11 +88,57 @@ enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3,   // LO
 enum : int { EPI_GATE = 1, EPI_MASK_PRE = 2, EPI_MASK_POST = 4, EPI_ACCUM = 8, EPI_SPLIT = 16, EPI_ACCUM2 = 32,
              EPI_WAVEGRAD = 64 };
 
+// ------------------------------------------------------------------ device memory
+// Device buffers held by the engines, all made by upload() below.
+inline std::atomic<long long> g_device_buffers{0};   // live DevBuf allocations (b200tts_debug_device_buffers)
+
+// The owner of one device allocation: freed when the owner is destroyed or assigned over.  Move-only, so a struct
+// holding DevBufs (a ConvLayer, an engine) cannot be copied and no buffer is freed twice.  Converts to T*, so kernel
+// arguments take it as they would the raw pointer.
+template <class T> class DevBuf {
+  public:
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) { release(); p_ = o.p_; o.p_ = nullptr; }
+        return *this;
+    }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+    operator T*() const { return p_; }
+    // replaces the buffer with n elements (n > 0); on failure the owner is left empty
+    cudaError_t alloc(size_t n) {
+        release();
+        const cudaError_t e = cudaMalloc((void**)&p_, n * sizeof(T));
+        if (e == cudaSuccess) g_device_buffers.fetch_add(1);
+        else p_ = nullptr;
+        return e;
+    }
+  private:
+    void release() {
+        if (!p_) return;
+        cudaFree(p_);
+        p_ = nullptr;
+        g_device_buffers.fetch_sub(1);
+    }
+    T* p_ = nullptr;
+};
+
+// allocation + H2D copy (empty for n == 0)
+template <class T> inline int upload(DevBuf<T>& dst, const T* src, size_t n) {
+    dst = DevBuf<T>();
+    if (n == 0) return 0;
+    B200_CUDA_OK(dst.alloc(n));
+    B200_CUDA_OK(cudaMemcpy(dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+}
+
 enum : int { TC_NONE = -1 };  // ConvLayer::tc_prec: no tensor-core images
 
 struct ConvLayer {            // immutable after pack(); owned by an engine handle
-    float* w = nullptr;       // device, packed [row_tiles][CinPad][K][CO_T]
-    float* bias = nullptr;    // device, [RowsPad] (zeros when the layer has no bias)
+    DevBuf<float> w;          // device, packed [row_tiles][CinPad][K][CO_T]
+    DevBuf<float> bias;       // device, [RowsPad] (zeros when the layer has no bias)
     int Cin = 0, CinPad = 0;  // input channels (padded to the ci chunk)
     int Rows = 0, RowsPad = 0;  // GEMM rows (Cout, or Cout*ups for transposed conv; 2*H interleaved for gate)
     int K = 1, dil = 1, pad = 0;
@@ -104,10 +150,10 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     // type of the images it built (a 16-bit or split-fp16 request with Cin % 16 != 0 gets 3xTF32; no image: TC_NONE).  The text and
     // duration path requests none, so durations stay bit-stable on the exact FP32 FMA kernel.
     int tc_prec = TC_NONE;
-    void* w_tc = nullptr;     // device, plain image: [128-row tile][chunk][tap] weight blocks (rows >= 32), see pack_tc
-    void* w_tcg = nullptr;    // device, grouped image: [chunk][tap block] weight blocks (rows == 32 / 64), null: none
+    DevBuf<unsigned char> w_tc;   // device, plain image: [128-row tile][chunk][tap] blocks (rows >= 32), see pack_tc
+    DevBuf<unsigned char> w_tcg;  // device, grouped image: [chunk][tap block] blocks (rows == 32 / 64), empty: none
     int tc_grp = 0;           // tap groups of the grouped image (128 / rows), 0: none
-    float* tc_rscale = nullptr;   // device, [Rows] 2^-e_r of the split-fp16 images (tc_prec == PREC_F16X3), else null
+    DevBuf<float> tc_rscale;  // device, [Rows] 2^-e_r of the split-fp16 images (tc_prec == PREC_F16X3), else empty
 };
 
 struct ConvIO {
@@ -162,12 +208,12 @@ int pack_conv(ConvLayer& L, const float* w, const float* bias, int Cout, int Cin
               int gate_half = 0, const int* in_perm = nullptr, const int* out_perm = nullptr);
 int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin, int Cout, int Kt, int stride,
                         int padding, int output_padding = 0);
-void free_conv(ConvLayer& L);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
 int conv_tc_error_flag();
 // one tensor-core weight image of logical weights Wl(r, ci, k) in the block layout of conv_tc3.cuh (see conv1d.cu);
-// prec PREC_F16X3 also uploads the row scales 2^-e_r into *rscale (when it is still null)
-int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G, float** rscale = nullptr);
+// prec PREC_F16X3 also uploads the row scales 2^-e_r into *rscale (when it is still empty)
+int pack_tc(DevBuf<unsigned char>& dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G,
+            DevBuf<float>* rscale = nullptr);
 // the tensor-core state of the current device, set up on first use: the mapped error words ([0] pipeline timeout,
 // [ERR_RANGE] split-fp16 range), the SM count and the opt-in shared memory per block.  Fails (once) when an earlier
 // launch set one of the error words.
@@ -192,15 +238,6 @@ int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);
 inline int conv_transpose_out_len(const ConvLayer& L, int Tin) {
     return (Tin - 1) * L.ups - 2 * L.tr_pad + L.tr_kernel + L.tr_outpad;
-}
-
-// small helpers shared by the engines
-template <class T> inline int upload(T** dst, const T* src, size_t n) {   // cudaMalloc + H2D copy (null for n == 0)
-    *dst = nullptr;
-    if (n == 0) return 0;
-    B200_CUDA_OK(cudaMalloc((void**)dst, n * sizeof(T)));
-    B200_CUDA_OK(cudaMemcpy(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
-    return 0;
 }
 
 // ------------------------------------------------------------------ bump allocator over a caller workspace

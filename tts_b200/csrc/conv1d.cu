@@ -451,16 +451,6 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
 // ------------------------------------------------------------------ host: packing
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
-void free_conv(ConvLayer& L) {
-    if (L.w) cudaFree(L.w);
-    if (L.bias) cudaFree(L.bias);
-    if (L.w_tc) cudaFree(L.w_tc);
-    if (L.w_tcg) cudaFree(L.w_tcg);
-    if (L.tc_rscale) cudaFree(L.tc_rscale);
-    L.w = L.bias = L.tc_rscale = nullptr;
-    L.w_tc = L.w_tcg = nullptr;
-}
-
 // One tensor-core weight image (conv_tc3.cuh): per (128-row tile, input-channel chunk, tap block) the block the weight
 // loader copies with one cp.async.bulk, [slabs][128 MMA rows][16 B], slab s holding the chunk's channels s*SLC .. +SLC-1:
 //   3xTF32 (PREC_FP32): 8-channel chunks, {hi, lo}[2 slabs] of 4 floats, hi = v & 0xFFFFE000 (exact in TF32), lo = v - hi
@@ -472,7 +462,8 @@ void free_conv(ConvLayer& L) {
 // With G tap groups (1: plain; 128 / rows: grouped), MMA row m = g * (128 / G) + co of tile t carries weight row
 // t * 128 + co and, in tap block j, tap G * j + g.  Rows >= `rows`, taps >= K and channels >= Cin are zero.  The weight
 // norm is already folded (in fp32) into Wl; each weight is rounded once, here.
-int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G, float** rscale) {
+int pack_tc(DevBuf<unsigned char>& dst, const std::vector<float>& Wl, int rows, int Cin, int K, int prec, int G,
+            DevBuf<float>* rscale) {
     const bool tf32 = prec == tc::PREC_FP32, x3 = prec == tc::PREC_F16X3;
     const int kc = tf32 ? tc3::KC2 : tc3::KC16, slc = kc / 2, ch = tc3::MROWS / G;
     const int ntiles = (rows + tc3::MROWS - 1) / tc3::MROWS, nchunks = (Cin + kc - 1) / kc, J = (K + G - 1) / G;
@@ -524,10 +515,8 @@ int pack_tc(void** dst, const std::vector<float>& Wl, int rows, int Cin, int K, 
                         }
                     }
                 }
-    unsigned char* d = nullptr;
-    const int rc = upload(&d, img.data(), img.size());
-    *dst = d;
-    if (rc == 0 && x3 && rscale && !*rscale) return upload(rscale, down.data(), down.size());
+    const int rc = upload(dst, img.data(), img.size());
+    if (rc == 0 && x3 && rscale && !*rscale) return upload(*rscale, down.data(), down.size());
     return rc;
 }
 
@@ -550,17 +539,17 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     }
     std::vector<float> bp(L.RowsPad, 0.f);
     for (int r = 0; r < rows; ++r) bp[r] = bl[r];
-    if (upload(&L.w, P.data(), P.size())) return 2;
-    if (upload(&L.bias, bp.data(), bp.size())) return 2;
+    if (upload(L.w, P.data(), P.size())) return 2;
+    if (upload(L.bias, bp.data(), bp.size())) return 2;
     // tensor-core images for a layer that requests them: rows >= 32 get the plain image (M = 128: two m64 warpgroups);
     // exactly 32 / 64 rows also get the grouped one (no padding), which the dispatcher prefers.  3xTF32 needs Cin >= 8, and
     // a 16-bit request packs 3xTF32 unless Cin % 16 == 0, so such a layer shows up as tc3 / tc3_grouped in the dispatch log
     if (L.tc_prec != TC_NONE && Cin % tc3::KC16 != 0) L.tc_prec = tc::PREC_FP32;
     if (rows < 32 || Cin < tc3::KC2) L.tc_prec = TC_NONE;
     if (L.tc_prec == TC_NONE) return 0;
-    if (pack_tc(&L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1, &L.tc_rscale)) return 2;
+    if (pack_tc(L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1, &L.tc_rscale)) return 2;
     if (L.ups == 1 && (rows == 32 || rows == 64)) {
-        if (pack_tc(&L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows, &L.tc_rscale)) return 2;
+        if (pack_tc(L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows, &L.tc_rscale)) return 2;
         L.tc_grp = tc3::MROWS / rows;
     }
     return 0;
@@ -779,17 +768,18 @@ static int launch_cic(const ConvKArgs& a, int co_tile, int B, int RowsPad, cudaS
 }
 
 // ------------------------------------------------------------------ dispatch log (debug / tests)
-static thread_local std::vector<int>* t_dispatch = nullptr;
-void dispatch_begin() { delete t_dispatch; t_dispatch = new std::vector<int>(); }
+static thread_local std::vector<int> t_dispatch;
+static thread_local bool t_dispatch_on = false;
+void dispatch_begin() { t_dispatch.clear(); t_dispatch_on = true; }
 int dispatch_end(int* ids, int cap) {
-    if (!t_dispatch) return 0;
-    const int n = (int)t_dispatch->size();
-    for (int i = 0; i < n && i < cap; ++i) ids[i] = (*t_dispatch)[i];
-    delete t_dispatch;
-    t_dispatch = nullptr;
+    if (!t_dispatch_on) return 0;
+    const int n = (int)t_dispatch.size();
+    for (int i = 0; i < n && i < cap; ++i) ids[i] = t_dispatch[i];
+    t_dispatch.clear();
+    t_dispatch_on = false;
     return n;
 }
-void dispatch_note(int id) { if (t_dispatch) t_dispatch->push_back(id); }
+void dispatch_note(int id) { if (t_dispatch_on) t_dispatch.push_back(id); }
 
 // tensor-core path: returns -1 when the layer / shape / epilogue is not eligible (caller falls through to the FMA kernel)
 // Per-device state of the tensor-core path: the pipeline-timeout flag lives in mapped pinned host memory (the kernels

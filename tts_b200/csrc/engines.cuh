@@ -16,7 +16,6 @@ struct Hifigan {
     std::vector<ConvLayer> ups;
     std::vector<std::vector<ConvLayer>> rb_c1, rb_c2;
     int prec = B200TTS_PRECISION_FP32;   // tensor-core operand type of the conv_pre / ups / resblock convs
-    ~Hifigan();
     int init(const b200tts_hifigan_config& cfg, const float* const* w, int nw, int precision = B200TTS_PRECISION_FP32);
     void stage_dims(int T, std::vector<int>& C, std::vector<int>& L) const;
     size_t workspace_bytes(int B, int T) const;
@@ -45,7 +44,6 @@ struct WaveNet {
     int H = 0, K = 0, L = 0, cond_ch = 0;
     ConvLayer cond;
     std::vector<ConvLayer> in_layers, res_skip;
-    ~WaveNet();
     int init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels,
              const float* const* w, int* consumed);
     size_t scratch_floats(int B, int T) const;
@@ -57,8 +55,11 @@ struct Flow {
     struct Block { ConvLayer pre, post; WaveNet wn; bool odd = false; };
     b200tts_flow_config c;
     bool fwd = false;
-    std::vector<Block*> blocks;
-    ~Flow();
+    std::vector<Block> blocks;
+    // no other member makes Flow move-only, and std::vector's copy constructor is declared whatever the element type
+    Flow() = default;
+    Flow(const Flow&) = delete;
+    Flow& operator=(const Flow&) = delete;
     int init(const b200tts_flow_config& cfg, const float* const* w, int nw, int forward_direction = 0);
     size_t workspace_bytes(int B, int T) const;
     // lens (nullable, device int32 [B]): frames per row; rows are neither computed nor read past their length (every
@@ -72,7 +73,6 @@ struct PosteriorEnc {
     b200tts_posterior_config c;
     ConvLayer pre, proj;
     WaveNet wn;
-    ~PosteriorEnc();
     int init(const b200tts_posterior_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     int forward(const float* x, const float* mask, const float* g, const float* noise, int B, int T, float* z,
@@ -82,8 +82,7 @@ struct PosteriorEnc {
 struct DurPred {
     b200tts_duration_predictor_config c;
     ConvLayer conv1, conv2, proj, cond, cond_lang;
-    float *g1 = nullptr, *b1 = nullptr, *g2 = nullptr, *b2 = nullptr;
-    ~DurPred();
+    DevBuf<float> g1, b1, g2, b2;
     int init(const b200tts_duration_predictor_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     int forward(const float* x, const float* mask, const float* g, const float* lang_emb, int B, int T, float* logw,
@@ -108,13 +107,11 @@ int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, 
 struct RelPosTransformer {
     struct Layer {
         ConvLayer qkv, o, ffn1, ffn2;
-        float *rel_k = nullptr, *rel_v = nullptr, *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
-        ~Layer();
+        DevBuf<float> rel_k, rel_v, ln1_g, ln1_b, ln2_g, ln2_b;
     };
     int C = 0, F = 0, heads = 0, window = -1;   // window < 0: no relative-position terms
     float eps = 0.f;
-    std::vector<Layer*> layers;
-    ~RelPosTransformer();
+    std::vector<Layer> layers;
     // w per layer: emb_rel_k [1,2w+1,d], emb_rel_v (window >= 0 only), conv_q.w/.b, conv_k.w/.b, conv_v.w/.b,
     // conv_o.w/.b, norm_1.gamma/.beta, ffn.conv_1.w/.b, ffn.conv_2.w/.b, norm_2.gamma/.beta
     int init(int channels, int ffn_channels, int kernel_size, int num_heads, int window, float eps, int num_layers,
@@ -127,10 +124,9 @@ struct RelPosTransformer {
 struct TextEncoder {
     b200tts_text_encoder_config c;
     int C = 0;
-    float* emb = nullptr;
+    DevBuf<float> emb;
     RelPosTransformer tf;
     ConvLayer proj;
-    ~TextEncoder();
     int init(const b200tts_text_encoder_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     int forward(const long long* tokens, const long long* lengths, const float* lang_emb, int B, int T, float* x,
@@ -140,20 +136,18 @@ struct TextEncoder {
 struct DDSConv {
     int C = 0, K = 0, L = 0;
     std::vector<ConvLayer> conv1x1;
-    std::vector<float*> sep_w, sep_b, g1, b1, g2, b2, dev;
-    ~DDSConv();
+    std::vector<DevBuf<float>> sep_w, sep_b, g1, b1, g2, b2;
     int init(int channels, int kernel_size, int num_layers, const float* const* w, int* consumed);
     int forward(float* x, const float* mask, int B, int T, float* y1, float* y2, cudaStream_t st) const;
 };
 
 struct SDP {
-    struct CFlow { float *pre_w = nullptr, *pre_b = nullptr; DDSConv convs; ConvLayer proj; };
+    struct CFlow { DevBuf<float> pre_w, pre_b; DDSConv convs; ConvLayer proj; };
     b200tts_sdp_config c;
     ConvLayer pre, cond, cond_lang, proj;
     DDSConv convs;
-    float *ea_t = nullptr, *ea_ls = nullptr;
-    std::vector<CFlow*> flows;
-    ~SDP();
+    DevBuf<float> ea_t, ea_ls;
+    std::vector<CFlow> flows;
     int init(const b200tts_sdp_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     int reverse(const float* x, const float* mask, const float* noise, const float* g, const float* lang_emb,
@@ -163,9 +157,9 @@ struct SDP {
 
 struct Stft {
     int n_fft = 0, hop = 0, log2n = 0, n_mels = 0;
-    float *window = nullptr, *twiddle = nullptr;
+    DevBuf<float> window;
+    DevBuf<float2> twiddle;            // n_fft / 2 (cos, sin) pairs
     ConvLayer mel;
-    ~Stft();
     int init(int n_fft, int hop, const float* window_host, const float* mel_basis_host, int n_mels);
     int magnitude(const float* wav, int B, int T, int pad1, int pad2, int mode, float power, float* spec, int n_frames,
                   cudaStream_t st) const;
@@ -178,8 +172,8 @@ struct Stft {
 struct SpeakerEncoder {
     struct Block {
         ConvLayer c1, c2, ds;                  // c2 and ds carry their BatchNorm folded in; c1's bn1 follows the ReLU
-        float *s1 = nullptr, *t1 = nullptr;    // bn1 as a per-channel affine after the ReLU
-        float *fc1w = nullptr, *fc1b = nullptr, *fc2w = nullptr, *fc2b = nullptr;   // SE MLP
+        DevBuf<float> s1, t1;                  // bn1 as a per-channel affine after the ReLU
+        DevBuf<float> fc1w, fc1b, fc2w, fc2b;  // SE MLP
         int C = 0, Cin = 0, Cr = 0;
         bool down = false;                     // first block of stages 2..4: stride 2 + downsample
     };
@@ -187,10 +181,9 @@ struct SpeakerEncoder {
     Stft stft;
     float pre0 = 0.f, pre1 = 1.f;              // pre-emphasis taps: y[t] = pre0 * x[t-1] + pre1 * x[t]
     ConvLayer conv1, att1, att2, fc;
-    float *s0 = nullptr, *t0 = nullptr;        // stem bn1 (after the ReLU)
+    DevBuf<float> s0, t0;                      // stem bn1 (after the ReLU)
     std::vector<Block> blocks;
     int stage_first[5] = {0, 0, 0, 0, 0};      // index of each stage's first block (stage_first[4] = blocks.size())
-    ~SpeakerEncoder();
     int init(const b200tts_speaker_encoder_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     // stop < 0: full forward into emb [groups, proj_dim]; stop = 0..4: dense features of that stage into feat
@@ -207,11 +200,10 @@ struct GlowDecoder {
     struct Block {
         ConvLayer start, end;
         WaveNet wn;
-        float *mix = nullptr, *an_bias = nullptr, *an_logs = nullptr;   // inverse InvConvNear weight [ns][ns], ActNorm
+        DevBuf<float> mix, an_bias, an_logs;   // inverse InvConvNear weight [ns][ns], ActNorm
     };
     int Cs = 0, Hd = 0, ns = 0, nsq = 0, sigmoid_scale = 0;   // Cs: squeezed channels out_channels * num_squeeze
-    std::vector<Block*> blocks;
-    ~GlowDecoder();
+    std::vector<Block> blocks;
     // w: per block ActNorm logs, bias, InvConvNear^-1, start.w, .b, WaveNet, end.w, .b (see b200tts_glow_tts_config)
     int init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
              int cond_channels, int num_splits, int num_squeeze, int sigmoid_scale, const float* const* w, int* consumed);
@@ -226,16 +218,15 @@ struct GlowDecoder {
 // the Glow decoder in reverse.  Squeeze is folded into the kernel that builds the latent, unsqueeze into the last
 // block's elementwise pass.
 struct GlowTTS {
-    struct Prenet { ConvLayer conv; float *g = nullptr, *b = nullptr; };
+    struct Prenet { ConvLayer conv; DevBuf<float> g, b; };
     b200tts_glow_tts_config c;
     int Cs = 0;                        // squeezed channels out_channels * num_squeeze
-    float* emb = nullptr;
+    DevBuf<float> emb;
     std::vector<Prenet> prenet;
     ConvLayer prenet_proj, proj;       // proj: [proj_m | proj_s] rows (proj_s all zero when mean_only)
     RelPosTransformer tf;
     DurPred dp;
     GlowDecoder dec;
-    ~GlowTTS();
     int init(const b200tts_glow_tts_config& cfg, const float* const* w, int nw);
     int tq(int Ty) const { return (Ty / c.num_squeeze + 3) / 4 * 4; }
     size_t encode_bytes(int B, int Tt) const;
@@ -302,10 +293,9 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
 // one BiLSTM launch per time step (lstm_bi), each row at its own length.
 struct SeqEncoder {
     int n_vocab = 0, E = 0, H = 0, n_convs = 0;   // H: LSTM hidden size per direction
-    float* emb = nullptr;
+    DevBuf<float> emb;
     ConvLayer convs[8], lstm_in;
-    float* whh = nullptr;                         // [2][4H][H]
-    ~SeqEncoder();
+    DevBuf<float> whh;                            // [2][4H][H]
     // w: emb [n_vocab, E]; per conv: weight [E, E, 5], bias, BN weight, bias, running_mean, running_var;
     // lstm weight_ih, weight_hh, bias_ih, bias_hh, then the same four _reverse
     int init(int n_vocab, int E, int H, int n_convs, const float* const* w, int* consumed);
@@ -325,12 +315,12 @@ struct Overflow {
     int O1 = 0;                        // output-net first-layer width
     SeqEncoder enc;
     ConvLayer zproj;
-    std::vector<float*> prenet_w;      // [P][in] (no bias)
-    float *mem_wih = nullptr, *mem_whh = nullptr, *mem_b = nullptr;   // [4M][P], [4M][M], b_ih + b_hh
-    std::vector<float*> out_w, out_b;  // layer 0: the h part [O1][M]; layers 1..: [O_l][O_{l-1}]; last [2C+1][O_last]
-    float *go = nullptr, *mean = nullptr, *std_ = nullptr;   // go_tokens [ar_order], mean / std [C]
+    std::vector<DevBuf<float>> prenet_w;        // [P][in] (no bias)
+    DevBuf<float> mem_wih, mem_whh, mem_b;      // [4M][P], [4M][M], b_ih + b_hh
+    // out_w / out_b layer 0: the h part [O1][M]; layers 1..: [O_l][O_{l-1}]; last [2C+1][O_last]
+    std::vector<DevBuf<float>> out_w, out_b;
+    DevBuf<float> go, mean, std_;               // go_tokens [ar_order], mean / std [C]
     GlowDecoder dec;
-    ~Overflow();
     int init(const b200tts_overflow_config& cfg, const float* const* w, int nw);
     int tq(int F) const { return (F / c.num_squeeze + 3) / 4 * 4; }
     size_t persist_bytes(int B, int Tt) const;     // zc and the loop state, kept from encode to sample
@@ -353,16 +343,13 @@ struct Tacotron2 {
     SeqEncoder enc;
     ConvLayer inproj;                  // attention.inputs_layer as a 1x1 conv (original attention)
     ConvLayer post[5];
-    float *prenet_w[2] = {nullptr, nullptr}, *prenet_b[2] = {nullptr, nullptr};   // bias: the folded "bn" prenet only
-    float *arnn_wih = nullptr, *arnn_whh = nullptr, *arnn_b = nullptr;   // [4096][768], [4096][1024], b_ih + b_hh
-    float *drnn_wih = nullptr, *drnn_whh = nullptr, *drnn_b = nullptr;   // [4096][1536], [4096][1024], b_ih + b_hh
-    float *att_wq = nullptr, *att_bq = nullptr, *att_v = nullptr, *att_wc = nullptr, *att_wd = nullptr;
-    float *att_prior = nullptr, *att_wk = nullptr, *att_ws = nullptr, *att_wsl = nullptr, *att_wdl = nullptr,
-          *att_bdl = nullptr;
+    DevBuf<float> prenet_w[2], prenet_b[2];     // bias: the folded "bn" prenet only
+    DevBuf<float> arnn_wih, arnn_whh, arnn_b;   // [4096][768], [4096][1024], b_ih + b_hh
+    DevBuf<float> drnn_wih, drnn_whh, drnn_b;   // [4096][1536], [4096][1024], b_ih + b_hh
+    DevBuf<float> att_wq, att_bq, att_v, att_wc, att_wd;
+    DevBuf<float> att_prior, att_wk, att_ws, att_wsl, att_wdl, att_bdl;
     float att_vb = 0.f;
-    float *proj_w = nullptr, *proj_b = nullptr, *stop_w = nullptr, *stop_b = nullptr;
-    std::vector<float*> dev;           // every buffer above, freed together
-    ~Tacotron2();
+    DevBuf<float> proj_w, proj_b, stop_w, stop_b;
     int init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw);
     size_t persist_bytes(int B, int Tt) const;
     size_t workspace_bytes(int B, int Tt, int F) const;
@@ -373,8 +360,6 @@ struct Tacotron2 {
                     int* steps, void* ws, size_t ws_bytes, cudaStream_t st) const;
     int postnet(const float* dec_out, const int* frames, int B, int F, int Fpitch, float* mel, void* ws,
                 size_t ws_bytes, cudaStream_t st) const;
-  private:
-    int up(float** dst, const float* src, size_t n);
 };
 
 // ForwardTTS inference (forward_tts.cu): FastPitch / FastSpeech / FastSpeech2 with FFTransformer encoder and decoder.
@@ -385,12 +370,11 @@ struct Tacotron2 {
 struct ForwardTTS {
     using Layer = RelPosTransformer::Layer;   // FFTransformer (TTS/tts/layers/generic/transformer.py:6-35)
     b200tts_forward_tts_config c;
-    float* emb = nullptr;
-    float* pe = nullptr;               // pos_encoder.pe [C][pe_len] (null without positional encoding)
-    std::vector<Layer*> enc, dec;
+    DevBuf<float> emb;
+    DevBuf<float> pe;                  // pos_encoder.pe [C][pe_len] (empty without positional encoding)
+    std::vector<Layer> enc, dec;
     ConvLayer proj_g, pitch_emb, energy_emb, postnet;
     DurPred dp, pitch_dp, energy_dp;
-    ~ForwardTTS();
     int init(const b200tts_forward_tts_config& cfg, const float* const* w, int nw);
     static int tp(int Ty) { return (Ty + 3) / 4 * 4; }
     size_t encode_bytes(int B, int Tt) const;
@@ -416,8 +400,7 @@ struct Melgan {
     ConvLayer conv_pre, conv_post;
     std::vector<ConvLayer> ups;
     std::vector<std::vector<Block>> blocks;   // [stage][block]
-    float* G = nullptr;                       // device [bands][taps + 1] PQMF synthesis filter (pqmf_bands > 0)
-    ~Melgan();
+    DevBuf<float> G;                          // device [bands][taps + 1] PQMF synthesis filter (pqmf_bands > 0)
     int init(const b200tts_melgan_config& cfg, const float* const* w, int nw);
     void stage_dims(int T, std::vector<int>& C, std::vector<int>& L) const;
     size_t workspace_bytes(int B, int T) const;
@@ -437,17 +420,16 @@ struct UTab;
 struct Pwgan {
     b200tts_pwgan_config c;
     int P = 1;                                    // samples per frame, prod(upsample_factors)
-    float *first_w = nullptr, *first_b = nullptr; // [64]
-    float* aux_w = nullptr;                       // [L * 128][80]: W_aux,l W_in, gate row order
-    float *b1 = nullptr, *b2 = nullptr;           // [L][128]: gate bias (gate row order), out | skip bias
-    std::vector<void*> w1, w2;                    // per layer: gate conv / out|skip images (pack_tc, PREC_F16X3)
-    std::vector<float*> rs1, rs2;                 // their row scales
+    DevBuf<float> first_w, first_b;               // [64]
+    DevBuf<float> aux_w;                          // [L * 128][80]: W_aux,l W_in, gate row order
+    DevBuf<float> b1, b2;                         // [L][128]: gate bias (gate row order), out | skip bias
+    std::vector<DevBuf<unsigned char>> w1, w2;    // per layer: gate conv / out|skip images (pack_tc, PREC_F16X3)
+    std::vector<DevBuf<float>> rs1, rs2;          // their row scales
     ConvLayer tail1, tail2;                       // last_conv_layers.1 (64 -> 64) and .3 (64 -> 1)
     // U: coefficient rows [uE0 left edge | P interior phases | uE1 right edge][uTW frames]; interior sample n reads
     // frames n / P - uoff ..; exact for inputs of at least min_frames frames
-    float* ucoef = nullptr;
+    DevBuf<float> ucoef;
     int uE0 = 0, uE1 = 0, uTW = 0, uoff = 0, min_frames = 0;
-    ~Pwgan();
     int init(const b200tts_pwgan_config& cfg, const float* const* w, int nw);
     int dilation(int l) const;
     size_t workspace_bytes(int B, int Tf) const;  // Tf: frames after the pad
@@ -478,8 +460,8 @@ struct Univnet {
     struct Block {
         ConvLayer up, kin;                        // upsample (ConvTranspose1d), kernel_predictor.input_conv
         std::vector<ConvLayer> kres;              // the six residual_conv convs
-        float *pw = nullptr, *pb = nullptr;       // kernel_conv | bias_conv, rows permuted: [MP][Kp * Ch] (tap-major), [MP]
-        float *cw = nullptr, *cb = nullptr;       // conv_i: [L][32][3 * 32] (tap-major), [L][32]
+        DevBuf<float> pw, pb;                     // kernel_conv | bias_conv, rows permuted: [MP][Kp * Ch] (tap-major), [MP]
+        DevBuf<float> cw, cb;                     // conv_i: [L][32][3 * 32] (tap-major), [L][32]
         int hop = 1;                              // cumulative hop of this block
     };
     b200tts_univnet_config c;
@@ -487,7 +469,6 @@ struct Univnet {
     std::vector<Block> blocks;
     int hop_total = 1;                            // prod(upsample_factors)
     int MP = 0;                                   // floats of one frame's predicted kernels and biases: L * (6144 + 64)
-    ~Univnet();
     int init(const b200tts_univnet_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int T) const;
     // mel [B, cond, T], noise [B, in, T] -> out [B, out, T * hop_total]
@@ -520,11 +501,10 @@ struct Wavegrad {
     struct UBlock { ConvLayer res, m0, m1, o0, o1; int f = 1; };
     b200tts_wavegrad_config c;
     ConvLayer y_conv, x_conv;
-    float *out_w = nullptr, *out_b = nullptr;   // out_conv [Clast][3] and its bias (own single-row kernel)
+    DevBuf<float> out_w, out_b;                 // out_conv [Clast][3] and its bias (own single-row kernel)
     std::vector<DBlock> db;
     std::vector<Film> film;
     std::vector<UBlock> ub;
-    ~Wavegrad();
     int init(const b200tts_wavegrad_config& cfg, const float* const* w, int nw);
     int hop() const;
     // down-path lengths: L[0] = hop * T, L[i + 1] = L[i] / f_i; FiLM i runs at L[i]

@@ -8,12 +8,6 @@
 
 namespace b200tts {
 
-WaveNet::~WaveNet() {
-    free_conv(cond);
-    for (auto& l : in_layers) free_conv(l);
-    for (auto& l : res_skip) free_conv(l);
-}
-
 // w: [cond.w, cond.b] (if cond_channels) then per layer: in.w, in.b, rs.w, rs.b.  Returns tensors consumed.
 int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels,
                   const float* const* w, int* consumed) {
@@ -88,10 +82,6 @@ int WaveNet::forward(float* h, float* out, const float* mask, const float* g, in
 }
 
 // ------------------------------------------------------------------ residual coupling blocks (reverse)
-Flow::~Flow() {
-    for (auto& b : blocks) { free_conv(b->pre); free_conv(b->post); delete b; }
-}
-
 int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, int forward_direction) {
     c = cfg;
     fwd = forward_direction != 0;
@@ -103,22 +93,21 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
     for (int i = 0; i < half; ++i) rev[i] = half - 1 - i;
     blocks.resize(c.num_flows);
     for (int n = 0; n < c.num_flows; ++n) {
-        Block* b = new Block();
-        blocks[n] = b;
+        Block& b = blocks[n];
         // reverse pass applies flows F-1 .. 0, each after one more flip: block n sees (F - n) flips;
         // the forward pass (networks.py:223-227) flips after each block: block n sees n flips
-        b->odd = fwd ? (n % 2) == 1 : ((c.num_flows - n) % 2) == 1;
+        b.odd = fwd ? (n % 2) == 1 : ((c.num_flows - n) % 2) == 1;
         const float* const* wn = w + (size_t)n * per;
         int rc, used = 0;
-        b->pre.tc_prec = b->post.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(b->pre, wn[0], wn[1], c.hidden_channels, half, 1, 1, 0, 0, b->odd ? rev.data() : nullptr,
+        b.pre.tc_prec = b.post.tc_prec = B200TTS_PRECISION_FP32;
+        if ((rc = pack_conv(b.pre, wn[0], wn[1], c.hidden_channels, half, 1, 1, 0, 0, b.odd ? rev.data() : nullptr,
                             nullptr)))
             return rc;
-        if ((rc = b->wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, wn + 2,
+        if ((rc = b.wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, wn + 2,
                              &used)))
             return rc;
-        if ((rc = pack_conv(b->post, wn[2 + used], wn[3 + used], half, c.hidden_channels, 1, 1, 0, 0, nullptr,
-                            b->odd ? rev.data() : nullptr)))
+        if ((rc = pack_conv(b.post, wn[2 + used], wn[3 + used], half, c.hidden_channels, 1, 1, 0, 0, nullptr,
+                            b.odd ? rev.data() : nullptr)))
             return rc;
     }
     return 0;
@@ -126,7 +115,7 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
 
 size_t Flow::workspace_bytes(int B, int T) const {
     const size_t hb = arena_bytes((size_t)B * c.hidden_channels * T);
-    return 3 * hb + arena_bytes((size_t)B * blocks[0]->wn.cond.RowsPad + 64) + 1024;
+    return 3 * hb + arena_bytes((size_t)B * blocks[0].wn.cond.RowsPad + 64) + 1024;
 }
 
 int Flow::reverse(float* z, const float* mask, const float* g, int B, int T, void* ws, size_t ws_bytes,
@@ -143,13 +132,13 @@ int Flow::reverse(float* z, const float* mask, const float* g, int B, int T, voi
     float* h = ar.f32((size_t)B * H * T);
     float* acts = ar.f32((size_t)B * H * T);
     float* out = ar.f32((size_t)B * H * T);
-    float* condv = ar.f32((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
+    float* condv = ar.f32((size_t)B * blocks[0].wn.cond.RowsPad + 64);
     B200_REQUIRE(h && acts && out && condv, "flow_reverse: arena exhausted");
     const long long zbs = (long long)c.channels * T;
     int rc;
     for (int step = 0; step < c.num_flows; ++step) {
         const int n = fwd ? step : c.num_flows - 1 - step;
-        const Block& b = *blocks[n];
+        const Block& b = blocks[n];
         // logical x0 / x1 live in the upper / lower physical half when an odd number of flips is pending
         float* x0 = z + (b.odd ? (size_t)half * T : 0);
         float* x1 = z + (b.odd ? 0 : (size_t)half * T);
@@ -189,8 +178,6 @@ __global__ void sample_posterior_kernel(const float* stats, const float* noise, 
     z[o] = __fmul_rn(__fadd_rn(m, __fmul_rn(noise[o], expf(ls))), mask[(size_t)b * T + t]);
 }
 }  // namespace
-
-PosteriorEnc::~PosteriorEnc() { free_conv(pre); free_conv(proj); }
 
 // weights: pre.w [H,Cin,1], pre.b, enc.* (WaveNet order), proj.w [2*out,H,1], proj.b
 int PosteriorEnc::init(const b200tts_posterior_config& cfg, const float* const* w, int nw) {

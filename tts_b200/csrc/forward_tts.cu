@@ -130,23 +130,15 @@ int pack_layer(ForwardTTS::Layer& L, const float* const* p, int C, int F, int pr
     if ((rc = pack_conv(L.o, p[2], p[3], C, C, 1, 1, 0))) return rc;
     if ((rc = pack_conv(L.ffn1, p[4], p[5], F, C, 3, 1, 1))) return rc;
     if ((rc = pack_conv(L.ffn2, p[6], p[7], C, F, 3, 1, 1))) return rc;
-    if ((rc = upload(&L.ln1_g, p[8], C))) return rc;
-    if ((rc = upload(&L.ln1_b, p[9], C))) return rc;
-    if ((rc = upload(&L.ln2_g, p[10], C))) return rc;
-    return upload(&L.ln2_b, p[11], C);
+    if ((rc = upload(L.ln1_g, p[8], C))) return rc;
+    if ((rc = upload(L.ln1_b, p[9], C))) return rc;
+    if ((rc = upload(L.ln2_g, p[10], C))) return rc;
+    return upload(L.ln2_b, p[11], C);
 }
 
 constexpr int PER_LAYER = 12;
 
 }  // namespace
-
-ForwardTTS::~ForwardTTS() {
-    if (emb) cudaFree(emb);
-    if (pe) cudaFree(pe);
-    for (auto* l : enc) delete l;
-    for (auto* l : dec) delete l;
-    free_conv(proj_g); free_conv(pitch_emb); free_conv(energy_emb); free_conv(postnet);
-}
 
 int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* w, int nw) {
     c = cfg;
@@ -166,13 +158,11 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
                        (c.use_energy ? 12 : 0) + (c.pe_len > 0 ? 1 : 0) + PER_LAYER * c.dec_layers + 2;
     B200_REQUIRE(nw == expect, "forward_tts: expected %d weight tensors, got %d", expect, nw);
     int rc;
-    if ((rc = upload(&emb, w[0], (size_t)c.n_vocab * C))) return rc;
+    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * C))) return rc;
     int i = 1;
-    for (int l = 0; l < c.enc_layers; ++l, i += PER_LAYER) {
-        Layer* L = new Layer();
-        enc.push_back(L);
-        if ((rc = pack_layer(*L, w + i, C, c.enc_ffn, TC_NONE))) return rc;
-    }
+    enc.resize(c.enc_layers);
+    for (int l = 0; l < c.enc_layers; ++l, i += PER_LAYER)
+        if ((rc = pack_layer(enc[l], w + i, C, c.enc_ffn, TC_NONE))) return rc;
     if (c.proj_g_in > 0) {   // nn.Linear(d_vector_dim, C) as a 1x1 conv over a one-column input
         if ((rc = pack_conv(proj_g, w[i], w[i + 1], C, c.proj_g_in, 1, 1, 0))) return rc;
         i += 2;
@@ -197,14 +187,12 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
         i += 12;
     }
     if (c.pe_len > 0) {
-        if ((rc = upload(&pe, w[i], (size_t)C * c.pe_len))) return rc;
+        if ((rc = upload(pe, w[i], (size_t)C * c.pe_len))) return rc;
         i += 1;
     }
-    for (int l = 0; l < c.dec_layers; ++l, i += PER_LAYER) {
-        Layer* L = new Layer();
-        dec.push_back(L);
-        if ((rc = pack_layer(*L, w + i, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
-    }
+    dec.resize(c.dec_layers);
+    for (int l = 0; l < c.dec_layers; ++l, i += PER_LAYER)
+        if ((rc = pack_layer(dec[l], w + i, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
     postnet.tc_prec = B200TTS_PRECISION_FP32;
     return pack_conv(postnet, w[i], w[i + 1], c.out_channels, C, 1, 1, 0);
 }
@@ -254,12 +242,12 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
     int rc;
     // x = emb(tokens), no scale (forward_tts.py:405), masked at the row's length
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, C, C, x, x_mask, st, false))) return rc;
-    for (const Layer* L : enc) {
+    for (const Layer& L : enc) {
         {
             ConvIO io;
             io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
             io.y = qkv; io.y_bs = 3 * bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L->qkv, io, st))) return rc;
+            if ((rc = launch_conv(L.qkv, io, st))) return rc;
         }
         // key_padding_mask = ~x_mask (transformer.py:60-63): masked keys get no weight
         if ((rc = launch_attention(qkv, x_mask, nullptr, nullptr, att, B, C, Tt, c.enc_heads, -1, st))) return rc;
@@ -267,24 +255,24 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
             ConvIO io;
             io.x = att; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
             io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L->o, io, st))) return rc;
+            if ((rc = launch_conv(L.o, io, st))) return rc;
         }
-        if ((rc = launch_add_norm(x, yb, true, L->ln1_g, L->ln1_b, x_mask, x, B, C, Tt, st))) return rc;
+        if ((rc = launch_add_norm(x, yb, true, L.ln1_g, L.ln1_b, x_mask, x, B, C, Tt, st))) return rc;
         {
             ConvIO io;
             io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
             io.y = hb; io.y_bs = (long long)F * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
             io.act = ACT_RELU;
-            if ((rc = launch_conv(L->ffn1, io, st))) return rc;
+            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
         }
         {
             ConvIO io;
             io.x = hb; io.x_bs = (long long)F * Tt; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
             io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L->ffn2, io, st))) return rc;
+            if ((rc = launch_conv(L.ffn2, io, st))) return rc;
         }
         // norm2(x + ffn), masked: Encoder.forward's final o * x_mask (feed_forward/encoder.py:161-162)
-        if ((rc = launch_add_norm(x, yb, false, L->ln2_g, L->ln2_b, x_mask, x, B, C, Tt, st))) return rc;
+        if ((rc = launch_add_norm(x, yb, false, L.ln2_g, L.ln2_b, x_mask, x, B, C, Tt, st))) return rc;
     }
     if (g) {   // o_en + g, g = emb_g(ids) / proj_g(d_vector) / d_vector (forward_tts.py:399-414)
         const float* gv = g;
@@ -357,9 +345,9 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
         else if (ragged) io.lens = lens;
         return io;
     };
-    for (const Layer* L : dec) {
+    for (const Layer& L : dec) {
         // the FMA attention fallback reads every column of q|k|v, so it gets them computed in full (from zero inputs)
-        if ((rc = launch_conv(L->qkv, io_for(x, C, qkv, 3 * C, attn_tc), st))) return rc;
+        if ((rc = launch_conv(L.qkv, io_for(x, C, qkv, 3 * C, attn_tc), st))) return rc;
         if (attn_tc) {
             if ((rc = launch_attention_tc3(qkv, (long long)3 * C * Tp, Tp, lens, att, (long long)C * Tp, B, C,
                                            c.dec_heads, Ty, st)))
@@ -368,15 +356,15 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
             if ((rc = launch_attention(qkv, ymask, nullptr, nullptr, att, B, C, Tp, c.dec_heads, -1, st))) return rc;
             dispatch_note(DISPATCH_ATTN_FMA);
         }
-        if ((rc = launch_conv(L->o, io_for(att, C, yb, C, true), st))) return rc;
-        if ((rc = launch_add_norm(x, yb, true, L->ln1_g, L->ln1_b, ymask, x, B, C, Tp, st))) return rc;
+        if ((rc = launch_conv(L.o, io_for(att, C, yb, C, true), st))) return rc;
+        if ((rc = launch_add_norm(x, yb, true, L.ln1_g, L.ln1_b, ymask, x, B, C, Tp, st))) return rc;
         {
             ConvIO io = io_for(x, C, hb, F, true);
             io.act = ACT_RELU;
-            if ((rc = launch_conv(L->ffn1, io, st))) return rc;
+            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
         }
-        if ((rc = launch_conv(L->ffn2, io_for(hb, F, yb, C, true), st))) return rc;
-        if ((rc = launch_add_norm(x, yb, false, L->ln2_g, L->ln2_b, ymask, x, B, C, Tp, st))) return rc;
+        if ((rc = launch_conv(L.ffn2, io_for(hb, F, yb, C, true), st))) return rc;
+        if ((rc = launch_add_norm(x, yb, false, L.ln2_g, L.ln2_b, ymask, x, B, C, Tp, st))) return rc;
     }
     if ((rc = launch_conv(postnet, io_for(x, C, pm, Co, true), st))) return rc;
     dim3 grid((unsigned)(((long long)Ty * Co + 255) / 256), B);

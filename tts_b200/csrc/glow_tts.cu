@@ -106,21 +106,6 @@ __global__ void flow_step_kernel(const float* __restrict__ x, const float* __res
 
 }  // namespace
 
-GlowTTS::~GlowTTS() {
-    if (emb) cudaFree(emb);
-    for (auto& p : prenet) { free_conv(p.conv); if (p.g) cudaFree(p.g); if (p.b) cudaFree(p.b); }
-    free_conv(prenet_proj);
-    free_conv(proj);
-}
-
-GlowDecoder::~GlowDecoder() {
-    for (auto* b : blocks) {
-        free_conv(b->start); free_conv(b->end);
-        for (float* p : {b->mix, b->an_bias, b->an_logs}) if (p) cudaFree(p);
-        delete b;
-    }
-}
-
 int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
                       int cond_channels, int num_splits, int num_squeeze, int sigmoid, const float* const* w,
                       int* consumed) {
@@ -131,18 +116,18 @@ int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilatio
                  MAX_SPLITS, Cs);
     const int per_block = 3 + 2 + (cond_channels > 0 ? 2 : 0) + 4 * num_layers + 2;
     int rc;
+    blocks.resize(num_blocks);
     for (int n = 0; n < num_blocks; ++n) {
         const float* const* p = w + n * per_block;
-        Block* b = new Block();
-        blocks.push_back(b);
-        if ((rc = upload(&b->an_logs, p[0], Cs))) return rc;
-        if ((rc = upload(&b->an_bias, p[1], Cs))) return rc;
-        if ((rc = upload(&b->mix, p[2], (size_t)ns * ns))) return rc;
-        b->start.tc_prec = b->end.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(b->start, p[3], p[4], Hd, Cs / 2, 1, 1, 0))) return rc;
+        Block& b = blocks[n];
+        if ((rc = upload(b.an_logs, p[0], Cs))) return rc;
+        if ((rc = upload(b.an_bias, p[1], Cs))) return rc;
+        if ((rc = upload(b.mix, p[2], (size_t)ns * ns))) return rc;
+        b.start.tc_prec = b.end.tc_prec = B200TTS_PRECISION_FP32;
+        if ((rc = pack_conv(b.start, p[3], p[4], Hd, Cs / 2, 1, 1, 0))) return rc;
         int used = 0;
-        if ((rc = b->wn.init(Hd, kernel_size, dilation_rate, num_layers, cond_channels, p + 5, &used))) return rc;
-        if ((rc = pack_conv(b->end, p[5 + used], p[6 + used], Cs, Hd, 1, 1, 0))) return rc;
+        if ((rc = b.wn.init(Hd, kernel_size, dilation_rate, num_layers, cond_channels, p + 5, &used))) return rc;
+        if ((rc = pack_conv(b.end, p[5 + used], p[6 + used], Cs, Hd, 1, 1, 0))) return rc;
     }
     *consumed = per_block * num_blocks;
     return 0;
@@ -150,7 +135,7 @@ int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilatio
 
 size_t GlowDecoder::workspace_bytes(int B, int Tq) const {
     return 2 * arena_bytes((size_t)B * Cs * Tq) + 3 * arena_bytes((size_t)B * Hd * Tq) +
-           arena_bytes((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
+           arena_bytes((size_t)B * blocks[0].wn.cond.RowsPad + 64);
 }
 
 int GlowDecoder::reverse(float* z, const float* msk, const float* g, int B, int Tq, int Tv, float* mel, void* ws,
@@ -161,14 +146,14 @@ int GlowDecoder::reverse(float* z, const float* msk, const float* g, int B, int 
     float* h = ar.f32((size_t)B * Hd * Tq);
     float* acts = ar.f32((size_t)B * Hd * Tq);
     float* out = ar.f32((size_t)B * Hd * Tq);
-    float* condv = ar.f32((size_t)B * blocks[0]->wn.cond.RowsPad + 64);
+    float* condv = ar.f32((size_t)B * blocks[0].wn.cond.RowsPad + 64);
     B200_REQUIRE(zb && eo && h && acts && out && condv, "glow decoder: arena exhausted");
     int rc;
     const long long zbs = (long long)Cs * Tq, hbs = (long long)Hd * Tq;
     float* cur = z;
     float* nxt = zb;
     for (int n = (int)blocks.size() - 1; n >= 0; --n) {   // reversed(flows): coupling, InvConvNear, ActNorm per block
-        const Block& bl = *blocks[n];
+        const Block& bl = blocks[n];
         {   // h = start(x0) * mask
             ConvIO io;
             io.x = cur; io.x_bs = zbs; io.x_cs = Tq; io.Tin = Tq;
@@ -213,14 +198,14 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
                        per_block * c.num_flow_blocks;
     B200_REQUIRE(nw == expect, "glow_tts: expected %d weight tensors, got %d", expect, nw);
     int rc;
-    if ((rc = upload(&emb, w[0], (size_t)c.n_vocab * H))) return rc;
+    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * H))) return rc;
     int i = 1;
     if (c.use_prenet) {   // ResidualConv1dLayerNormBlock(H, H, H, kernel_size=5, num_layers=3), encoder.py:107-110
         prenet.resize(3);
         for (auto& p : prenet) {
             if ((rc = pack_conv(p.conv, w[i], w[i + 1], H, H, 5, 1, 2))) return rc;
-            if ((rc = upload(&p.g, w[i + 2], H))) return rc;
-            if ((rc = upload(&p.b, w[i + 3], H))) return rc;
+            if ((rc = upload(p.g, w[i + 2], H))) return rc;
+            if ((rc = upload(p.b, w[i + 3], H))) return rc;
             i += 4;
         }
         if ((rc = pack_conv(prenet_proj, w[i], w[i + 1], H, H, 1, 1, 0))) return rc;

@@ -5,15 +5,6 @@
 
 namespace b200tts {
 
-Hifigan::~Hifigan() {
-    free_conv(conv_pre);
-    free_conv(cond);
-    free_conv(conv_post);
-    for (auto& l : ups) free_conv(l);
-    for (auto& v : rb_c1) for (auto& l : v) free_conv(l);
-    for (auto& v : rb_c2) for (auto& l : v) free_conv(l);
-}
-
 // weights: host pointers, canonical order (see include/tts_b200.h).  precision (B200TTS_PRECISION_*): the tensor-core
 // operand type of conv_pre, the upsamplers and every resblock conv -- the layers that run on the wgmma kernels (~97% of
 // the FLOPs); cond and conv_post stay fp32, and so does every margin, workspace size and launch window.  FP32 runs
@@ -47,8 +38,8 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
         i += 2;
     }
     ups.resize(c.num_upsamples);
-    rb_c1.assign(c.num_upsamples * c.num_kernels, std::vector<ConvLayer>());
-    rb_c2.assign(c.num_upsamples * c.num_kernels, std::vector<ConvLayer>());
+    rb_c1.resize(c.num_upsamples * c.num_kernels);
+    rb_c2.resize(c.num_upsamples * c.num_kernels);
     int ch = c.upsample_initial_channel;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int u = c.upsample_factors[s], k = c.upsample_kernel_sizes[s];

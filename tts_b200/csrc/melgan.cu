@@ -81,15 +81,6 @@ int launch_pqmf_synthesis(const float* x, long long x_bs, int x_cs, int B, int N
 // ------------------------------------------------------------------ engine
 static inline int round4(int v) { return (v + 3) / 4 * 4; }
 
-Melgan::~Melgan() {
-    free_conv(conv_pre);
-    free_conv(conv_post);
-    for (auto& l : ups) free_conv(l);
-    for (auto& st : blocks)
-        for (auto& b : st) { free_conv(b.dil); free_conv(b.c1x1); free_conv(b.shortcut); }
-    if (G) cudaFree(G);
-}
-
 int Melgan::init(const b200tts_melgan_config& cfg, const float* const* w, int nw) {
     c = cfg;
     const int S = c.num_upsamples, nb = c.num_res_blocks;
@@ -108,7 +99,7 @@ int Melgan::init(const b200tts_melgan_config& cfg, const float* const* w, int nw
     if ((rc = pack_conv(conv_pre, w[i], w[i + 1], c.base_channels, c.in_channels, c.proj_kernel, 1, ppad))) return rc;
     i += 2;
     ups.resize(S);
-    blocks.assign(S, std::vector<Block>(nb));
+    blocks.resize(S);
     int ch = c.base_channels;
     for (int s = 0; s < S; ++s) {
         const int u = c.upsample_factors[s], Cs = ch / 2;
@@ -116,6 +107,7 @@ int Melgan::init(const b200tts_melgan_config& cfg, const float* const* w, int nw
         if ((rc = pack_conv_transpose(ups[s], w[i], w[i + 1], ch, Cs, 2 * u, u, u / 2 + u % 2, u % 2))) return rc;
         i += 2;
         int d = 1;
+        blocks[s].resize(nb);
         for (int m = 0; m < nb; ++m, d *= c.res_kernel) {
             Block& bl = blocks[s][m];
             bl.dil.tc_prec = bl.c1x1.tc_prec = bl.shortcut.tc_prec = B200TTS_PRECISION_FP32;
@@ -130,7 +122,7 @@ int Melgan::init(const b200tts_melgan_config& cfg, const float* const* w, int nw
     i += 2;
     if (c.pqmf_bands > 0) {
         B200_REQUIRE(w[i] != nullptr, "melgan: null PQMF filter");
-        if (upload(&G, w[i], (size_t)c.pqmf_bands * (c.pqmf_taps + 1))) return 2;
+        if (upload(G, w[i], (size_t)c.pqmf_bands * (c.pqmf_taps + 1))) return 2;
     }
     return 0;
 }

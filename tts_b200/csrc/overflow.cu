@@ -129,14 +129,6 @@ static bool persist_layout(const Overflow& e, Arena& ar, int B, int Tt, Persist&
     return p.zc && p.ctl && p.state && p.done && p.quant && p.hm && p.cm && p.pin && p.pb && p.hid && p.outp;
 }
 
-Overflow::~Overflow() {
-    free_conv(zproj);
-    for (float* p : prenet_w) cudaFree(p);
-    for (float* p : out_w) if (p) cudaFree(p);
-    for (float* p : out_b) if (p) cudaFree(p);
-    for (float* p : {mem_wih, mem_whh, mem_b, go, mean, std_}) if (p) cudaFree(p);
-}
-
 int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, int nw) {
     c = cfg;
     const int E = c.encoder_dim, C = c.out_channels, P = c.prenet_dim, M = c.memory_rnn_dim, nL = c.outputnet_n_layers;
@@ -154,41 +146,38 @@ int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, in
     B200_REQUIRE(nw == expect, "overflow: expected %d weight tensors, got %d", expect, nw);
     int rc, i = 0;
     if ((rc = enc.init(c.n_vocab, E, H, c.n_convs, w, &i))) return rc;
-    if ((rc = upload(&go, w[i++], (size_t)c.ar_order))) return rc;
-    for (int l = 0; l < c.prenet_n_layers; ++l) {
-        float* p = nullptr;
-        if ((rc = upload(&p, w[i++], (size_t)P * (l ? P : c.ar_order * C)))) return rc;
-        prenet_w.push_back(p);
-    }
-    if ((rc = upload(&mem_wih, w[i], (size_t)4 * M * P))) return rc;
-    if ((rc = upload(&mem_whh, w[i + 1], (size_t)4 * M * M))) return rc;
+    if ((rc = upload(go, w[i++], (size_t)c.ar_order))) return rc;
+    prenet_w.resize(c.prenet_n_layers);
+    for (int l = 0; l < c.prenet_n_layers; ++l)
+        if ((rc = upload(prenet_w[l], w[i++], (size_t)P * (l ? P : c.ar_order * C)))) return rc;
+    if ((rc = upload(mem_wih, w[i], (size_t)4 * M * P))) return rc;
+    if ((rc = upload(mem_whh, w[i + 1], (size_t)4 * M * M))) return rc;
     {
         std::vector<float> b((size_t)4 * M);
         for (int r = 0; r < 4 * M; ++r) b[r] = w[i + 2][r] + w[i + 3][r];
-        if ((rc = upload(&mem_b, b.data(), b.size()))) return rc;
+        if ((rc = upload(mem_b, b.data(), b.size()))) return rc;
     }
     i += 4;
+    out_w.resize(nL + 1);
+    out_b.resize(nL + 1);
     for (int l = 0; l <= nL; ++l, i += 2) {
         const int rows = l < nL ? c.outputnet_size[l] : 2 * C + 1;
         const int in = l == 0 ? M + E : c.outputnet_size[l - 1];
-        float *pw = nullptr, *pbias = nullptr;
         if (l == 0) {   // cat(h, z): the h columns per frame, the z columns hoisted into zproj (with the bias)
             std::vector<float> wh((size_t)rows * M), wz((size_t)rows * E);
             for (int r = 0; r < rows; ++r) {
                 memcpy(wh.data() + (size_t)r * M, w[i] + (size_t)r * in, sizeof(float) * M);
                 memcpy(wz.data() + (size_t)r * E, w[i] + (size_t)r * in + M, sizeof(float) * E);
             }
-            if ((rc = upload(&pw, wh.data(), wh.size()))) return rc;
+            if ((rc = upload(out_w[l], wh.data(), wh.size()))) return rc;
             if ((rc = pack_conv(zproj, wz.data(), w[i + 1], rows, E, 1, 1, 0))) return rc;
         } else {
-            if ((rc = upload(&pw, w[i], (size_t)rows * in))) return rc;
-            if ((rc = upload(&pbias, w[i + 1], (size_t)rows))) return rc;
+            if ((rc = upload(out_w[l], w[i], (size_t)rows * in))) return rc;
+            if ((rc = upload(out_b[l], w[i + 1], (size_t)rows))) return rc;
         }
-        out_w.push_back(pw);
-        out_b.push_back(pbias);
     }
-    if ((rc = upload(&mean, w[i], (size_t)C))) return rc;
-    if ((rc = upload(&std_, w[i + 1], (size_t)C))) return rc;
+    if ((rc = upload(mean, w[i], (size_t)C))) return rc;
+    if ((rc = upload(std_, w[i + 1], (size_t)C))) return rc;
     i += 2;
     if (c.has_decoder) {
         B200_REQUIRE(c.num_squeeze >= 1 && c.hidden_channels_dec > 0 && c.kernel_size_dec % 2 == 1 &&

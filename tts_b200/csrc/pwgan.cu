@@ -368,17 +368,6 @@ static DeviceOnce g_pw_once;
 // ------------------------------------------------------------------ engine
 static inline int round4(int v) { return (v + 3) / 4 * 4; }
 
-Pwgan::~Pwgan() {
-    for (void* p : w1) cudaFree(p);
-    for (void* p : w2) cudaFree(p);
-    for (float* p : rs1) cudaFree(p);
-    for (float* p : rs2) cudaFree(p);
-    for (float* p : {first_w, first_b, aux_w, b1, b2, ucoef})
-        if (p) cudaFree(p);
-    free_conv(tail1);
-    free_conv(tail2);
-}
-
 int Pwgan::dilation(int l) const { return 1 << (l % (c.num_res_blocks / c.stacks)); }
 
 // The stage chain of UpsampleNetwork in float64 on one channel: per stage, Stretch2d (F.interpolate nearest, torch's index
@@ -492,7 +481,7 @@ int Pwgan::build_u(const std::vector<std::vector<double>>& fir) {
         if (exact_at(t) && exact_at(t + 1) && exact_at(t + 2) && exact_at(t + uTW + 1)) min_frames = t;
     B200_REQUIRE(min_frames > 0, "pwgan: no input length up to %d frames for which the upsampler tables are exact", TB / 2);
     std::vector<float> cf32(cf.begin(), cf.end());
-    return upload(&ucoef, cf32.data(), cf32.size());
+    return upload(ucoef, cf32.data(), cf32.size());
 }
 
 int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) {
@@ -510,7 +499,7 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
     const int expect = 2 + 1 + S + 7 * L + 4;
     B200_REQUIRE(nw == expect, "pwgan: expected %d weight tensors, got %d", expect, nw);
     for (int i = 0; i < nw; ++i) B200_REQUIRE(w[i] != nullptr, "pwgan: weight tensor %d is null", i);
-    if (upload(&first_w, w[0], RES) || upload(&first_b, w[1], RES)) return 2;
+    if (upload(first_w, w[0], RES) || upload(first_b, w[1], RES)) return 2;
     const float* W_in = w[2];                                          // conv_in [80][80]
     std::vector<std::vector<double>> fir(S);
     for (int s = 0; s < S; ++s) fir[s].assign(w[3 + s], w[3 + s] + 2 * c.upsample_factors[s] + 1);
@@ -518,7 +507,7 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
     // MMA row m of the gate: tanh row 8g + (m % 16) for m % 16 < 8, else sigmoid row 64 + 8g + (m % 16 - 8), g = m / 16
     auto gate_row = [](int m) { const int g = m / 16, q = m % 16; return q < 8 ? 8 * g + q : 64 + 8 * g + q - 8; };
     std::vector<float> aux((size_t)L * GATE * AUX), bias1((size_t)L * GATE), bias2((size_t)L * GATE);
-    w1.assign(L, nullptr); w2.assign(L, nullptr); rs1.assign(L, nullptr); rs2.assign(L, nullptr);
+    w1.resize(L); w2.resize(L); rs1.resize(L); rs2.resize(L);
     for (int l = 0; l < L; ++l, i += 7) {
         const float *cw = w[i], *cb = w[i + 1], *aw = w[i + 2], *ow = w[i + 3], *ob = w[i + 4], *sw = w[i + 5], *sb = w[i + 6];
         std::vector<float> W1((size_t)GATE * RES * 3), W2((size_t)GATE * RES);
@@ -538,11 +527,11 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
             bias2[(size_t)l * GATE + r] = ob[r];
             bias2[(size_t)l * GATE + RES + r] = sb[r];
         }
-        if (pack_tc(&w1[l], W1, GATE, RES, 3, tc::PREC_F16X3, 1, &rs1[l])) return 2;
-        if (pack_tc(&w2[l], W2, GATE, RES, 1, tc::PREC_F16X3, 1, &rs2[l])) return 2;
+        if (pack_tc(w1[l], W1, GATE, RES, 3, tc::PREC_F16X3, 1, &rs1[l])) return 2;
+        if (pack_tc(w2[l], W2, GATE, RES, 1, tc::PREC_F16X3, 1, &rs2[l])) return 2;
     }
-    if (upload(&aux_w, aux.data(), aux.size()) || upload(&b1, bias1.data(), bias1.size()) ||
-        upload(&b2, bias2.data(), bias2.size()))
+    if (upload(aux_w, aux.data(), aux.size()) || upload(b1, bias1.data(), bias1.size()) ||
+        upload(b2, bias2.data(), bias2.size()))
         return 2;
     tail1.tc_prec = B200TTS_PRECISION_FP32;
     int rc;
@@ -613,7 +602,7 @@ int Pwgan::launch_layer(int l, const float* x, float* xn, float* skip, int B, in
     memset(&a, 0, sizeof(a));
     a.x = x; a.xn = xn; a.skip = skip;
     a.bs = (long long)RES * pitch; a.pitch = pitch; a.Ts = Tf * P; a.dil = dilation(l);
-    a.w1 = static_cast<const unsigned char*>(w1[l]); a.w2 = static_cast<const unsigned char*>(w2[l]);
+    a.w1 = w1[l]; a.w2 = w2[l];
     a.rs1 = rs1[l]; a.rs2 = rs2[l]; a.b1 = b1 + (size_t)l * GATE; a.b2 = b2 + (size_t)l * GATE;
     a.A = A; a.A_bs = A_bs; a.Tf = Tf; a.u = utab();
     a.first = l == 0;

@@ -5,6 +5,9 @@
 // on tensor-core rounding.
 #include <math.h>
 
+#include <memory>
+#include <type_traits>
+
 #include "engines.cuh"
 
 namespace b200tts {
@@ -218,6 +221,13 @@ int launch_transpose(const float* x, float* y, int B, int N, int E, cudaStream_t
     return 0;
 }
 
+// scoped owners of run_step_graph's capture stream, graph and executable graph
+template <class H, cudaError_t (*destroy)(H)> struct CudaDestroy {
+    void operator()(H h) const { destroy(h); }
+};
+template <class H, cudaError_t (*destroy)(H)>
+using CudaOwned = std::unique_ptr<std::remove_pointer_t<H>, CudaDestroy<H, destroy>>;
+
 int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_step,
                    const std::function<int(cudaStream_t, int, bool)>& step, const int* ctl, int B, std::vector<int>& host,
                    cudaStream_t st) {
@@ -225,9 +235,9 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     B200_CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+    const CudaOwned<cudaStream_t, cudaStreamDestroy> cs_owner(cs);
     int rc = 0;
     if (cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-        cudaStreamDestroy(cs);
         set_error("%s: cannot capture the step graph", who);
         return 2;
     }
@@ -235,14 +245,13 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
     for (int f = 0; f < chunk && rc == 0; ++f) rc = step(cs, f & 1, f == 0);
     const cudaError_t ce = cudaStreamEndCapture(cs, &graph);
     g_launch_count = launches;
-    cudaStreamDestroy(cs);
+    const CudaOwned<cudaGraph_t, cudaGraphDestroy> graph_owner(graph);
     if (rc || ce != cudaSuccess) {
-        if (graph) cudaGraphDestroy(graph);
         if (!rc) set_error("%s: step graph capture failed: %s", who, cudaGetErrorString(ce));
         return rc ? rc : 2;
     }
     const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
+    const CudaOwned<cudaGraphExec_t, cudaGraphExecDestroy> exec_owner(exec);
     if (ie != cudaSuccess) {
         set_error("%s: cannot instantiate the step graph: %s", who, cudaGetErrorString(ie));
         return 2;
@@ -255,29 +264,20 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
         if (e == cudaSuccess) e = cudaMemcpyAsync(host.data(), ctl, sizeof(int) * (2 + B), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) {
-            cudaGraphExecDestroy(exec);
             set_error("%s: %s", who, cudaGetErrorString(e));
             return 2;
         }
         if (host[0] == 0) break;
     }
-    cudaGraphExecDestroy(exec);
     return 0;
 }
 
 // ------------------------------------------------------------------ the text encoder
-SeqEncoder::~SeqEncoder() {
-    if (emb) cudaFree(emb);
-    for (auto& L : convs) free_conv(L);
-    free_conv(lstm_in);
-    if (whh) cudaFree(whh);
-}
-
 int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, const float* const* w, int* consumed) {
     n_vocab = vocab; E = dim; H = hidden; n_convs = convs_n;
     B200_REQUIRE(n_vocab > 0 && E > 0 && H > 0 && n_convs >= 1 && n_convs <= 8, "encoder: unsupported config");
     int rc, i = 0;
-    if ((rc = upload(&emb, w[i++], (size_t)n_vocab * E))) return rc;
+    if ((rc = upload(emb, w[i++], (size_t)n_vocab * E))) return rc;
     for (int l = 0; l < n_convs; ++l, i += 6) {   // ConvBNBlock: BatchNorm1d (eps 1e-5) folded into the conv
         std::vector<float> wf((size_t)E * E * 5), bf(E);
         for (int o = 0; o < E; ++o) {
@@ -296,7 +296,7 @@ int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, const float* c
             for (int r = 0; r < 4 * H; ++r) bi[(size_t)d * 4 * H + r] = p[2][r] + p[3][r];
         }
         if ((rc = pack_conv(lstm_in, wi.data(), bi.data(), 8 * H, E, 1, 1, 0))) return rc;
-        if ((rc = upload(&whh, wh.data(), wh.size()))) return rc;
+        if ((rc = upload(whh, wh.data(), wh.size()))) return rc;
         i += 8;
     }
     *consumed = i;

@@ -228,11 +228,6 @@ __global__ void add_chan_bias_kernel(const float* x, const float* cb, long long 
 }
 }  // namespace
 
-DurPred::~DurPred() {
-    free_conv(conv1); free_conv(conv2); free_conv(proj); free_conv(cond); free_conv(cond_lang);
-    for (float* p : {g1, b1, g2, b2}) if (p) cudaFree(p);
-}
-
 // weights: conv_1.w [F,Cin,k], .b, norm_1.gamma [1,F,1], .beta, conv_2.w [F,F,k], .b, norm_2.gamma, .beta,
 //          proj.w [1,F,1], .b, [cond.w [Cin,cond,1], .b], [cond_lang.w, .b]
 int DurPred::init(const b200tts_duration_predictor_config& cfg, const float* const* w, int nw) {
@@ -242,11 +237,11 @@ int DurPred::init(const b200tts_duration_predictor_config& cfg, const float* con
     B200_REQUIRE(nw == expect, "duration_predictor: expected %d weight tensors, got %d", expect, nw);
     int rc;
     if ((rc = pack_conv(conv1, w[0], w[1], F, Cin, K, 1, K / 2))) return rc;
-    if ((rc = upload(&g1, w[2], F))) return rc;
-    if ((rc = upload(&b1, w[3], F))) return rc;
+    if ((rc = upload(g1, w[2], F))) return rc;
+    if ((rc = upload(b1, w[3], F))) return rc;
     if ((rc = pack_conv(conv2, w[4], w[5], F, F, K, 1, K / 2))) return rc;
-    if ((rc = upload(&g2, w[6], F))) return rc;
-    if ((rc = upload(&b2, w[7], F))) return rc;
+    if ((rc = upload(g2, w[6], F))) return rc;
+    if ((rc = upload(b2, w[7], F))) return rc;
     if ((rc = pack_conv(proj, w[8], w[9], 1, F, 1, 1, 0))) return rc;
     int i = 10;
     if (c.cond_channels > 0) { if ((rc = pack_conv(cond, w[i], w[i + 1], Cin, c.cond_channels, 1, 1, 0))) return rc; i += 2; }
@@ -315,11 +310,6 @@ int DurPred::forward(const float* x, const float* mask, const float* g, const fl
     return launch_conv(proj, io, st);
 }
 
-DDSConv::~DDSConv() {
-    for (auto& l : conv1x1) free_conv(l);
-    for (float* p : dev) if (p) cudaFree(p);
-}
-
 // per layer: sep.w [C,1,K], sep.b, 1x1.w [C,C,1], 1x1.b, norm1.gamma, norm1.beta, norm2.gamma, norm2.beta
 int DDSConv::init(int channels, int kernel_size, int num_layers, const float* const* w, int* consumed) {
     C = channels; K = kernel_size; L = num_layers;
@@ -328,14 +318,13 @@ int DDSConv::init(int channels, int kernel_size, int num_layers, const float* co
     int rc;
     for (int l = 0; l < L; ++l) {
         const float* const* p = w + 8 * l;
-        auto up = [&](float*& dst, const float* src, size_t n) { int r = upload(&dst, src, n); dev.push_back(dst); return r; };
-        if ((rc = up(sep_w[l], p[0], (size_t)C * K))) return rc;
-        if ((rc = up(sep_b[l], p[1], C))) return rc;
+        if ((rc = upload(sep_w[l], p[0], (size_t)C * K))) return rc;
+        if ((rc = upload(sep_b[l], p[1], C))) return rc;
         if ((rc = pack_conv(conv1x1[l], p[2], p[3], C, C, 1, 1, 0))) return rc;
-        if ((rc = up(g1[l], p[4], C))) return rc;
-        if ((rc = up(b1[l], p[5], C))) return rc;
-        if ((rc = up(g2[l], p[6], C))) return rc;
-        if ((rc = up(b2[l], p[7], C))) return rc;
+        if ((rc = upload(g1[l], p[4], C))) return rc;
+        if ((rc = upload(b1[l], p[5], C))) return rc;
+        if ((rc = upload(g2[l], p[6], C))) return rc;
+        if ((rc = upload(b2[l], p[7], C))) return rc;
     }
     *consumed = 8 * L;
     return 0;
@@ -362,13 +351,6 @@ int DDSConv::forward(float* x, const float* mask, int B, int T, float* y1, float
     return 0;
 }
 
-SDP::~SDP() {
-    free_conv(pre); free_conv(cond); free_conv(cond_lang); free_conv(proj);
-    for (auto* f : flows) { free_conv(f->proj); if (f->pre_w) cudaFree(f->pre_w); if (f->pre_b) cudaFree(f->pre_b); delete f; }
-    if (ea_t) cudaFree(ea_t);
-    if (ea_ls) cudaFree(ea_ls);
-}
-
 // weights: pre.w [H,in,1], pre.b, [cond.w,cond.b], [cond_lang.w,cond_lang.b], convs(3 layers x 8), proj.w, proj.b,
 //          flows.0.translation [2], flows.0.log_scale [2],
 //          for f = 1..num_flows: pre.w [H,1,1], pre.b, convs(3 x 8), proj.w [3*nb-1, H, 1], proj.b
@@ -388,18 +370,18 @@ int SDP::init(const b200tts_sdp_config& cfg, const float* const* w, int nw) {
     i += used;
     if ((rc = pack_conv(proj, w[i], w[i + 1], H, H, 1, 1, 0))) return rc;
     i += 2;
-    if ((rc = upload(&ea_t, w[i], 2))) return rc;
-    if ((rc = upload(&ea_ls, w[i + 1], 2))) return rc;
+    if ((rc = upload(ea_t, w[i], 2))) return rc;
+    if ((rc = upload(ea_ls, w[i + 1], 2))) return rc;
     i += 2;
+    flows.resize(c.num_flows);
     for (int f = 0; f < c.num_flows; ++f) {
-        CFlow* F = new CFlow();
-        flows.push_back(F);
-        if ((rc = upload(&F->pre_w, w[i], H))) return rc;
-        if ((rc = upload(&F->pre_b, w[i + 1], H))) return rc;
+        CFlow& F = flows[f];
+        if ((rc = upload(F.pre_w, w[i], H))) return rc;
+        if ((rc = upload(F.pre_b, w[i + 1], H))) return rc;
         i += 2;
-        if ((rc = F->convs.init(H, c.kernel_size, 3, w + i, &used))) return rc;
+        if ((rc = F.convs.init(H, c.kernel_size, 3, w + i, &used))) return rc;
         i += used;
-        if ((rc = pack_conv(F->proj, w[i], w[i + 1], 3 * c.num_bins - 1, H, 1, 1, 0))) return rc;
+        if ((rc = pack_conv(F.proj, w[i], w[i + 1], 3 * c.num_bins - 1, H, 1, 1, 0))) return rc;
         i += 2;
     }
     return 0;
@@ -488,7 +470,7 @@ int SDP::reverse(const float* x, const float* mask, const float* noise, const fl
             B200_CUDA_OK(cudaGetLastError());
             continue;
         }
-        const CFlow& F = *flows[f - 1];
+        const CFlow& F = flows[f - 1];
         {
             dim3 grid((T + 127) / 128, H, B);
             convflow_pre_kernel<<<grid, 128, 0, st>>>(z, ch0, F.pre_w, F.pre_b, xc, h, H, T);

@@ -264,7 +264,7 @@ BN bn_affine(const float* w, const float* b, const float* mean, const float* var
     }
     return r;
 }
-int upload_d(float** dst, const std::vector<double>& v) {
+int upload_d(DevBuf<float>& dst, const std::vector<double>& v) {
     std::vector<float> f(v.begin(), v.end());
     return upload(dst, f.data(), f.size());
 }
@@ -365,15 +365,6 @@ int zero_rows(float* buf, int H, size_t row, cudaStream_t st) {   // rows 0 and 
 
 }  // namespace
 
-SpeakerEncoder::~SpeakerEncoder() {
-    free_conv(conv1); free_conv(att1); free_conv(att2); free_conv(fc);
-    for (float* p : {s0, t0}) if (p) cudaFree(p);
-    for (auto& b : blocks) {
-        free_conv(b.c1); free_conv(b.c2); free_conv(b.ds);
-        for (float* p : {b.s1, b.t1, b.fc1w, b.fc1b, b.fc2w, b.fc2b}) if (p) cudaFree(p);
-    }
-}
-
 int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float* const* w, int nw) {
     c = cfg;
     B200_REQUIRE(c.input_dim >= 8 && c.input_dim % 8 == 0, "speaker_encoder: input_dim=%d must be a multiple of 8", c.input_dim);
@@ -414,9 +405,10 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
         std::vector<float> r = repack3x3(cw, F0, 1, nullptr);
         conv1.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(conv1, r.data(), cb, F0, 3, 3, 1, 1))) return rc;
-        if ((rc = upload_d(&s0, b.s)) || (rc = upload_d(&t0, b.t))) return rc;
+        if ((rc = upload_d(s0, b.s)) || (rc = upload_d(t0, b.t))) return rc;
     }
     int Cprev = F0;
+    blocks.reserve(c.layers[0] + c.layers[1] + c.layers[2] + c.layers[3]);
     for (int s = 0; s < 4; ++s) {
         stage_first[s] = (int)blocks.size();
         for (int k = 0; k < c.layers[s]; ++k) {
@@ -443,9 +435,9 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
                 std::vector<float> r = repack3x3(w2, b.C, b.C, &b2.s), bias(b2.t.begin(), b2.t.end());
                 if ((rc = pack_conv(b.c2, r.data(), bias.data(), b.C, 3 * b.C, 3, 1, 1))) return rc;
             }
-            if ((rc = upload_d(&b.s1, b1.s)) || (rc = upload_d(&b.t1, b1.t))) return rc;
-            if ((rc = upload(&b.fc1w, f1w, (size_t)b.Cr * b.C)) || (rc = upload(&b.fc1b, f1b, b.Cr)) ||
-                (rc = upload(&b.fc2w, f2w, (size_t)b.C * b.Cr)) || (rc = upload(&b.fc2b, f2b, b.C)))
+            if ((rc = upload_d(b.s1, b1.s)) || (rc = upload_d(b.t1, b1.t))) return rc;
+            if ((rc = upload(b.fc1w, f1w, (size_t)b.Cr * b.C)) || (rc = upload(b.fc1b, f1b, b.Cr)) ||
+                (rc = upload(b.fc2w, f2w, (size_t)b.C * b.Cr)) || (rc = upload(b.fc2b, f2b, b.C)))
                 return rc;
             if (b.down) {
                 const float* dw = next();

@@ -81,12 +81,6 @@ __global__ void __launch_bounds__(STFT_NT) stft_mag_kernel(const float* wav, con
 
 }  // namespace
 
-Stft::~Stft() {
-    if (window) cudaFree(window);
-    if (twiddle) cudaFree(twiddle);
-    free_conv(mel);
-}
-
 int Stft::init(int n_fft_, int hop_, const float* window_host, const float* mel_basis_host, int n_mels_) {
     n_fft = n_fft_; hop = hop_; n_mels = n_mels_;
     log2n = 0;
@@ -94,14 +88,13 @@ int Stft::init(int n_fft_, int hop_, const float* window_host, const float* mel_
     B200_REQUIRE((1 << log2n) == n_fft && n_fft >= 32 && n_fft <= 8192, "stft: n_fft=%d must be a power of two in [32, 8192]", n_fft);
     B200_REQUIRE(hop >= 1 && window_host, "stft: bad arguments");
     int rc;
-    if ((rc = upload(&window, window_host, n_fft))) return rc;
-    std::vector<float> tw(n_fft);  // n_fft/2 float2 entries
+    if ((rc = upload(window, window_host, n_fft))) return rc;
+    std::vector<float2> tw(n_fft / 2);
     for (int k = 0; k < n_fft / 2; ++k) {
         const double a = -2.0 * M_PI * (double)k / (double)n_fft;
-        tw[2 * k] = (float)cos(a);
-        tw[2 * k + 1] = (float)sin(a);
+        tw[k] = make_float2((float)cos(a), (float)sin(a));
     }
-    if ((rc = upload(&twiddle, tw.data(), n_fft))) return rc;
+    if ((rc = upload(twiddle, tw.data(), tw.size()))) return rc;
     if (mel_basis_host && n_mels > 0) {
         // mel = basis [n_mels, F] @ spec [F, frames]  ==  1x1 conv with Cin = F
         if ((rc = pack_conv(mel, mel_basis_host, nullptr, n_mels, n_fft / 2 + 1, 1, 1, 0))) return rc;
@@ -124,7 +117,7 @@ int Stft::magnitude(const float* wav, int B, int T, int pad1, int pad2, int mode
             return 0;
         })) return rc;
     dim3 grid((n_frames + STFT_FR - 1) / STFT_FR, B);
-    stft_mag_kernel<<<grid, STFT_NT, smem, st>>>(wav, window, reinterpret_cast<const float2*>(twiddle), spec, T, n_fft,
+    stft_mag_kernel<<<grid, STFT_NT, smem, st>>>(wav, window, twiddle, spec, T, n_fft,
                                                  log2n, hop, pad1, pad2, n_frames, mode, power);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());

@@ -313,18 +313,6 @@ size_t Tacotron2::workspace_bytes(int B, int Tt, int F) const {
     return std::max(encb, postb) + 1024;
 }
 
-Tacotron2::~Tacotron2() {
-    free_conv(inproj);
-    for (auto& L : post) free_conv(L);
-    for (float* p : dev) if (p) cudaFree(p);
-}
-
-int Tacotron2::up(float** dst, const float* src, size_t n) {
-    int rc = upload(dst, src, n);
-    if (!rc) dev.push_back(*dst);
-    return rc;
-}
-
 int Tacotron2::init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw) {
     c = cfg;
     const int C = c.out_channels;
@@ -339,7 +327,7 @@ int Tacotron2::init(const b200tts_tacotron2_config& cfg, const float* const* w, 
     for (int l = 0; l < 2; ++l) {   // prenet (no bias); "bn": eval BatchNorm folded into the layer
         const int in = l ? PN : C;
         if (!c.prenet_bn) {
-            if ((rc = up(&prenet_w[l], w[i++], (size_t)PN * in))) return rc;
+            if ((rc = upload(prenet_w[l], w[i++], (size_t)PN * in))) return rc;
             continue;
         }
         std::vector<float> wf((size_t)PN * in), bf(PN);
@@ -348,45 +336,45 @@ int Tacotron2::init(const b200tts_tacotron2_config& cfg, const float* const* w, 
             for (int k = 0; k < in; ++k) wf[(size_t)o * in + k] = (float)(w[i][(size_t)o * in + k] * s);
             bf[o] = (float)(w[i + 2][o] - w[i + 3][o] * s);
         }
-        if ((rc = up(&prenet_w[l], wf.data(), wf.size()))) return rc;
-        if ((rc = up(&prenet_b[l], bf.data(), bf.size()))) return rc;
+        if ((rc = upload(prenet_w[l], wf.data(), wf.size()))) return rc;
+        if ((rc = upload(prenet_b[l], bf.data(), bf.size()))) return rc;
         i += 5;
     }
-    auto lstm = [&](float** wih, float** whh, float** bias, int in, int H) -> int {
+    auto lstm = [&](DevBuf<float>& wih, DevBuf<float>& whh, DevBuf<float>& bias, int in, int H) -> int {
         int r;
-        if ((r = up(wih, w[i], (size_t)4 * H * in))) return r;
-        if ((r = up(whh, w[i + 1], (size_t)4 * H * H))) return r;
+        if ((r = upload(wih, w[i], (size_t)4 * H * in))) return r;
+        if ((r = upload(whh, w[i + 1], (size_t)4 * H * H))) return r;
         std::vector<float> b((size_t)4 * H);
         for (int k = 0; k < 4 * H; ++k) b[k] = w[i + 2][k] + w[i + 3][k];
         i += 4;
-        return up(bias, b.data(), b.size());
+        return upload(bias, b.data(), b.size());
     };
-    if ((rc = lstm(&arnn_wih, &arnn_whh, &arnn_b, PN + E, Q))) return rc;
+    if ((rc = lstm(arnn_wih, arnn_whh, arnn_b, PN + E, Q))) return rc;
     if (c.attention_type == 0) {
-        if ((rc = up(&att_wq, w[i++], (size_t)A * Q))) return rc;
+        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
         if ((rc = pack_conv(inproj, w[i++], nullptr, A, E, 1, 1, 0))) return rc;
-        if ((rc = up(&att_v, w[i++], A))) return rc;
+        if ((rc = upload(att_v, w[i++], A))) return rc;
         att_vb = w[i++][0];
         if (c.location_attn) {
-            if ((rc = up(&att_wc, w[i++], (size_t)LOC_F * 2 * LOC_K))) return rc;
-            if ((rc = up(&att_wd, w[i++], (size_t)A * LOC_F))) return rc;
+            if ((rc = upload(att_wc, w[i++], (size_t)LOC_F * 2 * LOC_K))) return rc;
+            if ((rc = upload(att_wd, w[i++], (size_t)A * LOC_F))) return rc;
         }
     } else {
-        if ((rc = up(&att_prior, w[i++], PRIOR_K))) return rc;
-        if ((rc = up(&att_wq, w[i++], (size_t)A * Q))) return rc;
-        if ((rc = up(&att_bq, w[i++], A))) return rc;
-        if ((rc = up(&att_wk, w[i++], (size_t)DCA_F * DCA_K * A))) return rc;
-        if ((rc = up(&att_ws, w[i++], (size_t)DCA_F * DCA_K))) return rc;
-        if ((rc = up(&att_wsl, w[i++], (size_t)A * DCA_F))) return rc;
-        if ((rc = up(&att_wdl, w[i++], (size_t)A * DCA_F))) return rc;
-        if ((rc = up(&att_bdl, w[i++], A))) return rc;
-        if ((rc = up(&att_v, w[i++], A))) return rc;
+        if ((rc = upload(att_prior, w[i++], PRIOR_K))) return rc;
+        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
+        if ((rc = upload(att_bq, w[i++], A))) return rc;
+        if ((rc = upload(att_wk, w[i++], (size_t)DCA_F * DCA_K * A))) return rc;
+        if ((rc = upload(att_ws, w[i++], (size_t)DCA_F * DCA_K))) return rc;
+        if ((rc = upload(att_wsl, w[i++], (size_t)A * DCA_F))) return rc;
+        if ((rc = upload(att_wdl, w[i++], (size_t)A * DCA_F))) return rc;
+        if ((rc = upload(att_bdl, w[i++], A))) return rc;
+        if ((rc = upload(att_v, w[i++], A))) return rc;
     }
-    if ((rc = lstm(&drnn_wih, &drnn_whh, &drnn_b, Q + E, D))) return rc;
-    if ((rc = up(&proj_w, w[i], (size_t)C * c.r_init * (D + E)))) return rc;
-    if ((rc = up(&proj_b, w[i + 1], (size_t)C * c.r_init))) return rc;
-    if ((rc = up(&stop_w, w[i + 2], (size_t)D + C * c.r_init))) return rc;
-    if ((rc = up(&stop_b, w[i + 3], 1))) return rc;
+    if ((rc = lstm(drnn_wih, drnn_whh, drnn_b, Q + E, D))) return rc;
+    if ((rc = upload(proj_w, w[i], (size_t)C * c.r_init * (D + E)))) return rc;
+    if ((rc = upload(proj_b, w[i + 1], (size_t)C * c.r_init))) return rc;
+    if ((rc = upload(stop_w, w[i + 2], (size_t)D + C * c.r_init))) return rc;
+    if ((rc = upload(stop_b, w[i + 3], 1))) return rc;
     i += 4;
     for (int l = 0; l < 5; ++l, i += 6) {   // Postnet ConvBNBlocks, BatchNorm folded
         const int ci = l ? 512 : C, co = l == 4 ? C : 512;

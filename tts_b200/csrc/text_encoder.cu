@@ -265,15 +265,6 @@ int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, 
     return 0;
 }
 
-RelPosTransformer::Layer::~Layer() {
-    free_conv(qkv); free_conv(o); free_conv(ffn1); free_conv(ffn2);
-    for (float* p : {rel_k, rel_v, ln1_g, ln1_b, ln2_g, ln2_b}) if (p) cudaFree(p);
-}
-
-RelPosTransformer::~RelPosTransformer() {
-    for (auto* l : layers) delete l;
-}
-
 int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int num_heads, int window_size,
                             float ln_eps, int num_layers, const float* const* w, int* consumed) {
     C = channels; F = ffn_channels; heads = num_heads; window = window_size; eps = ln_eps;
@@ -281,13 +272,13 @@ int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int
     const int nrel = 2 * window + 1;
     const int per = window >= 0 ? 18 : 16;
     int rc;
+    layers.resize(num_layers);
     for (int l = 0; l < num_layers; ++l) {
         const float* const* p = w + (size_t)l * per;
-        Layer* L = new Layer();
-        layers.push_back(L);
+        Layer& L = layers[l];
         if (window >= 0) {
-            if ((rc = upload(&L->rel_k, p[0], (size_t)nrel * d))) return rc;
-            if ((rc = upload(&L->rel_v, p[1], (size_t)nrel * d))) return rc;
+            if ((rc = upload(L.rel_k, p[0], (size_t)nrel * d))) return rc;
+            if ((rc = upload(L.rel_v, p[1], (size_t)nrel * d))) return rc;
             p += 2;
         }
         // fused QKV: rows [q | k | v]
@@ -296,15 +287,15 @@ int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int
             memcpy(wq.data() + (size_t)s * C * C, p[2 * s], sizeof(float) * C * C);
             memcpy(bq.data() + (size_t)s * C, p[2 * s + 1], sizeof(float) * C);
         }
-        if ((rc = pack_conv(L->qkv, wq.data(), bq.data(), 3 * C, C, 1, 1, 0))) return rc;
-        if ((rc = pack_conv(L->o, p[6], p[7], C, C, 1, 1, 0))) return rc;
-        if ((rc = upload(&L->ln1_g, p[8], C))) return rc;
-        if ((rc = upload(&L->ln1_b, p[9], C))) return rc;
+        if ((rc = pack_conv(L.qkv, wq.data(), bq.data(), 3 * C, C, 1, 1, 0))) return rc;
+        if ((rc = pack_conv(L.o, p[6], p[7], C, C, 1, 1, 0))) return rc;
+        if ((rc = upload(L.ln1_g, p[8], C))) return rc;
+        if ((rc = upload(L.ln1_b, p[9], C))) return rc;
         // FeedForwardNetwork._same_padding: pad_l = (k-1)//2 (transformer.py:307-313)
-        if ((rc = pack_conv(L->ffn1, p[10], p[11], F, C, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = pack_conv(L->ffn2, p[12], p[13], C, F, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = upload(&L->ln2_g, p[14], C))) return rc;
-        if ((rc = upload(&L->ln2_b, p[15], C))) return rc;
+        if ((rc = pack_conv(L.ffn1, p[10], p[11], F, C, K, 1, (K - 1) / 2))) return rc;
+        if ((rc = pack_conv(L.ffn2, p[12], p[13], C, F, K, 1, (K - 1) / 2))) return rc;
+        if ((rc = upload(L.ln2_g, p[14], C))) return rc;
+        if ((rc = upload(L.ln2_b, p[15], C))) return rc;
     }
     *consumed = per * num_layers;
     return 0;
@@ -324,45 +315,40 @@ int RelPosTransformer::forward(float* x, const float* x_mask, int B, int T, void
     B200_REQUIRE(qkv && att && yb && hb, "rel_pos_transformer: arena exhausted");
     const long long bs = (long long)C * T;
     int rc;
-    for (const Layer* L : layers) {
+    for (const Layer& L : layers) {
         {   // q,k,v = conv_{q,k,v}(x)       (x is already masked: the caller / previous norm2 epilogue)
             ConvIO io;
             io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;
             io.y = qkv; io.y_bs = 3 * bs; io.y_cs = T; io.Tout = T; io.B = B;
-            if ((rc = launch_conv(L->qkv, io, st))) return rc;
+            if ((rc = launch_conv(L.qkv, io, st))) return rc;
         }
-        if ((rc = launch_attention(qkv, x_mask, L->rel_k, L->rel_v, att, B, C, T, heads, window, st))) return rc;
+        if ((rc = launch_attention(qkv, x_mask, L.rel_k, L.rel_v, att, B, C, T, heads, window, st))) return rc;
         {   // y = conv_o(att)
             ConvIO io;
             io.x = att; io.x_bs = bs; io.x_cs = T; io.Tin = T;
             io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-            if ((rc = launch_conv(L->o, io, st))) return rc;
+            if ((rc = launch_conv(L.o, io, st))) return rc;
         }
-        if ((rc = launch_add_layernorm(x, yb, L->ln1_g, L->ln1_b, nullptr, x, B, C, T, eps, st))) return rc;
+        if ((rc = launch_add_layernorm(x, yb, L.ln1_g, L.ln1_b, nullptr, x, B, C, T, eps, st))) return rc;
         {   // h = relu(conv_1(pad(x * mask)))
             ConvIO io;
             io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
             io.y = hb; io.y_bs = (long long)F * T; io.y_cs = T; io.Tout = T; io.B = B;
             io.act = ACT_RELU;
-            if ((rc = launch_conv(L->ffn1, io, st))) return rc;
+            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
         }
         {   // y = conv_2(pad(h * mask)) * mask
             ConvIO io;
             io.x = hb; io.x_bs = (long long)F * T; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
             io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
             io.ymask = x_mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
-            if ((rc = launch_conv(L->ffn2, io, st))) return rc;
+            if ((rc = launch_conv(L.ffn2, io, st))) return rc;
         }
         // x = norm2(x + y); the next layer and the stack's output (transformer.py:419, :431) use x * mask -> fold the
         // mask here
-        if ((rc = launch_add_layernorm(x, yb, L->ln2_g, L->ln2_b, x_mask, x, B, C, T, eps, st))) return rc;
+        if ((rc = launch_add_layernorm(x, yb, L.ln2_g, L.ln2_b, x_mask, x, B, C, T, eps, st))) return rc;
     }
     return 0;
-}
-
-TextEncoder::~TextEncoder() {
-    if (emb) cudaFree(emb);
-    free_conv(proj);
 }
 
 // weights: emb [V,hidden]; per layer: see RelPosTransformer::init (window w); proj.w [2*out,C,1], proj.b
@@ -378,7 +364,7 @@ int TextEncoder::init(const b200tts_text_encoder_config& cfg, const float* const
     B200_REQUIRE(nw == 1 + per * c.num_layers + 2, "text_encoder: expected %d weight tensors, got %d",
                  1 + per * c.num_layers + 2, nw);
     int rc;
-    if ((rc = upload(&emb, w[0], (size_t)c.n_vocab * c.hidden_channels))) return rc;
+    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * c.hidden_channels))) return rc;
     int used = 0;
     if ((rc = tf.init(C, c.hidden_channels_ffn, c.kernel_size, c.num_heads, c.rel_attn_window_size, 1e-5f,
                       c.num_layers, w + 1, &used)))

@@ -296,18 +296,6 @@ static DeviceOnce g_uv_once;
 // ------------------------------------------------------------------ engine
 static inline int round4(int v) { return (v + 3) / 4 * 4; }
 
-Univnet::~Univnet() {
-    free_conv(first);
-    free_conv(last);
-    for (Block& bl : blocks) {
-        free_conv(bl.up);
-        free_conv(bl.kin);
-        for (auto& l : bl.kres) free_conv(l);
-        for (float* p : {bl.pw, bl.pb, bl.cw, bl.cb})
-            if (p) cudaFree(p);
-    }
-}
-
 int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int nw) {
     using namespace uv;
     c = cfg;
@@ -372,7 +360,7 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
                     }
         for (int l = 0; l < L; ++l)
             for (int co = 0; co < CO; ++co) put(L * KSZ + l * CO + co, bw + (size_t)(l * CO + co) * Ch * Kp, bb[l * CO + co]);
-        if (upload(&bl.pw, W.data(), W.size()) || upload(&bl.pb, bias.data(), bias.size())) return 2;
+        if (upload(bl.pw, W.data(), W.size()) || upload(bl.pb, bias.data(), bias.size())) return 2;
         // conv_i: [layer][co][tap * 32 + ci]
         std::vector<float> cw((size_t)L * C * KK), cb((size_t)L * C);
         for (int l = 0; l < L; ++l, i += 2) {
@@ -383,7 +371,7 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
                 cb[(size_t)l * C + co] = w[i + 1][co];
             }
         }
-        if (upload(&bl.cw, cw.data(), cw.size()) || upload(&bl.cb, cb.data(), cb.size())) return 2;
+        if (upload(bl.cw, cw.data(), cw.size()) || upload(bl.cb, cb.data(), cb.size())) return 2;
     }
     last.tc_prec = B200TTS_PRECISION_FP32;
     return pack_conv(last, w[i], w[i + 1], c.out_channels, C, 7, 1, 3);

@@ -68,16 +68,6 @@ __global__ void __launch_bounds__(256) wavegrad_out_kernel(const float* __restri
 }
 
 // ------------------------------------------------------------------ engine
-Wavegrad::~Wavegrad() {
-    free_conv(y_conv);
-    free_conv(x_conv);
-    for (auto& d : db) { free_conv(d.res); free_conv(d.m0); free_conv(d.m1); free_conv(d.m2); }
-    for (auto& f : film) { free_conv(f.in); free_conv(f.out); }
-    for (auto& u : ub) { free_conv(u.res); free_conv(u.m0); free_conv(u.m1); free_conv(u.o0); free_conv(u.o1); }
-    if (out_w) cudaFree(out_w);
-    if (out_b) cudaFree(out_b);
-}
-
 int Wavegrad::hop() const {
     int h = 1;
     for (int i = 0; i < c.num_upsamples; ++i) h *= c.upsample_factors[i];
@@ -147,7 +137,7 @@ int Wavegrad::init(const b200tts_wavegrad_config& cfg, const float* const* w, in
         ic = hc;
     }
     if ((rc = conv(x_conv, c.x_conv_channels, c.in_channels, 3, 1))) return rc;
-    if (upload(&out_w, w[i], (size_t)ic * 3) || upload(&out_b, w[i + 1], 1)) return 2;
+    if (upload(out_w, w[i], (size_t)ic * 3) || upload(out_b, w[i + 1], 1)) return 2;
     return 0;
 }
 
