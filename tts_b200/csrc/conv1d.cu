@@ -451,6 +451,16 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
 // ------------------------------------------------------------------ host: packing
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
+// PREC_F16X3 row scaling 2^e_r of row r (n weights): e_r puts the row's max |w| * 2^e_r in [2^14, 2^15); all-zero rows: 1
+static float f16x3_row_up(const std::vector<float>& Wl, int r, size_t n) {
+    float m = 0.f;
+    for (size_t i = (size_t)r * n; i < (size_t)(r + 1) * n; ++i) m = std::max(m, std::fabs(Wl[i]));
+    if (m == 0.f) return 1.f;
+    int E;
+    std::frexp(m, &E);                                     // m in [2^(E-1), 2^E)
+    return std::ldexp(1.f, std::min(126, std::max(-126, 15 - E)));
+}
+
 // One tensor-core weight image (conv_tc3.cuh): per (128-row tile, input-channel chunk, tap block) the block the weight
 // loader copies with one cp.async.bulk, [slabs][128 MMA rows][16 B], slab s holding the chunk's channels s*SLC .. +SLC-1:
 //   3xTF32 (PREC_FP32): 8-channel chunks, {hi, lo}[2 slabs] of 4 floats, hi = v & 0xFFFFE000 (exact in TF32), lo = v - hi
@@ -471,14 +481,8 @@ int pack_tc(DevBuf<unsigned char>& dst, const std::vector<float>& Wl, int rows, 
     std::vector<unsigned char> img((size_t)ntiles * nchunks * J * blk, 0);
     std::vector<float> up(x3 ? rows : 0, 1.f), down(x3 ? rows : 0, 1.f);   // 2^e_r, 2^-e_r
     for (int r = 0; r < (x3 ? rows : 0); ++r) {
-        float m = 0.f;
-        for (size_t i = (size_t)r * Cin * K; i < (size_t)(r + 1) * Cin * K; ++i) m = std::max(m, std::fabs(Wl[i]));
-        if (m == 0.f) continue;
-        int E;
-        std::frexp(m, &E);                                 // m in [2^(E-1), 2^E)
-        const int e = std::min(126, std::max(-126, 15 - E));
-        up[r] = std::ldexp(1.f, e);
-        down[r] = std::ldexp(1.f, -e);
+        up[r] = f16x3_row_up(Wl, r, (size_t)Cin * K);
+        down[r] = 1.f / up[r];
     }
     for (int t = 0; t < ntiles; ++t)
         for (int c = 0; c < nchunks; ++c)
@@ -520,6 +524,31 @@ int pack_tc(DevBuf<unsigned char>& dst, const std::vector<float>& Wl, int rows, 
     return rc;
 }
 
+// The time-major kernel's PREC_F16X3 image for exactly 32 / 64 rows (the B operand, conv_tc3.cuh tm_consumers): per
+// (16-channel chunk, tap) one block {W_hs, W_lo, W_hi}[2 slabs][rows][16 B], slab s holding channels 8 s .. 8 s + 7.  The
+// row scaling and W_hi / W_lo are pack_tc's; W_hs = fp16(W_hi * 2^-11) is stored (a B operand cannot come from registers).
+static int pack_tc_tm(DevBuf<unsigned char>& dst, const std::vector<float>& Wl, int rows, int Cin, int K) {
+    const int nchunks = (Cin + tc3::KC16 - 1) / tc3::KC16;
+    const size_t slab = (size_t)rows * 16, plane = 2 * slab, blk = tc3::tm_block_bytes(rows);
+    std::vector<unsigned char> img((size_t)nchunks * K * blk, 0);
+    for (int r = 0; r < rows; ++r) {
+        const float up = f16x3_row_up(Wl, r, (size_t)Cin * K);
+        for (int c = 0; c < nchunks; ++c)
+            for (int k = 0; k < K; ++k)
+                for (int i = 0; i < tc3::KC16 && c * tc3::KC16 + i < Cin; ++i) {
+                    const float ws = Wl[((size_t)r * Cin + c * tc3::KC16 + i) * K + k] * up;
+                    const __half hi = __float2half_rn(ws);
+                    const __half lo = __float2half_rn(ws - __half2float(hi));
+                    const __half hs = __float2half_rn(__half2float(hi) / 2048.f);
+                    unsigned char* p = img.data() + ((size_t)c * K + k) * blk + (i / 8) * slab + (size_t)r * 16 + 2 * (i % 8);
+                    memcpy(p, &hs, 2);
+                    memcpy(p + plane, &lo, 2);
+                    memcpy(p + 2 * plane, &hi, 2);
+                }
+    }
+    return upload(dst, img.data(), img.size());
+}
+
 // Wl(r, ci, k): logical weights already expressed as a correlation-form conv with `rows` GEMM rows
 static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vector<float>& bl, int rows, int Cin,
                      int K) {
@@ -549,7 +578,9 @@ static int pack_rows(ConvLayer& L, const std::vector<float>& Wl, const std::vect
     if (L.tc_prec == TC_NONE) return 0;
     if (pack_tc(L.w_tc, Wl, rows, Cin, K, L.tc_prec, 1, &L.tc_rscale)) return 2;
     if (L.ups == 1 && (rows == 32 || rows == 64)) {
-        if (pack_tc(L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows, &L.tc_rscale)) return 2;
+        const int rc = L.tc_prec == tc::PREC_F16X3 ? pack_tc_tm(L.w_tcg, Wl, rows, Cin, K)
+                                                    : pack_tc(L.w_tcg, Wl, rows, Cin, K, L.tc_prec, tc3::MROWS / rows, &L.tc_rscale);
+        if (rc) return 2;
         L.tc_grp = tc3::MROWS / rows;
     }
     return 0;
@@ -832,9 +863,15 @@ static int tc_device_init(int d) {
             B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
         B200_CUDA_OK(cudaFuncSetAttribute(tc3::plain_kernel(p, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
         for (int g : {2, 4})
-            for (bool refl : {false, true})
-                B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  smem_optin));
+            for (bool refl : {false, true}) {
+                if (p != tc::PREC_F16X3)
+                    B200_CUDA_OK(cudaFuncSetAttribute(tc3::grouped_kernel(g, p, refl), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      smem_optin));
+                else
+                    for (int tms : {1, 2})
+                        B200_CUDA_OK(cudaFuncSetAttribute(tc3::timemajor_kernel(tc3::MROWS / g, tms, refl),
+                                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+            }
         for (bool near : {false, true})
             if (tc3::wavegrad_kernel(p, near))
                 B200_CUDA_OK(cudaFuncSetAttribute(tc3::wavegrad_kernel(p, near), cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -890,14 +927,23 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const bool grouped = G && !wg && !needs_v3 && !a.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
     // plain mode otherwise: M = rows (128 per tile, zero padded), N = 256 time steps.  Everything neither mode takes
     // (unaligned or masked inputs, shared-memory budget) runs on the exact FP32-FMA kernel.
-    const int rows_pad = grouped ? rp_grouped : (tc3::TT2 + (L.K - 1) * L.dil + 7) / 8 * 8;
+    // At PREC_F16X3 the grouped layers run on the time-major kernel (M = time, N = the 32 / 64 channels): 256-column tiles,
+    // or 128 where a 256-column window (tile + reach) would not fit the 320 staging rows or, with room for a ragged
+    // prefix table of 255 rows, shared memory.  The width is fixed per layer, so every column takes the same sum whatever
+    // its tile origin (ragged / windowed calls match the dense one bit for bit).
+    const bool tm = grouped && L.tc_prec == tc::PREC_F16X3;
+    const int reach = (L.K - 1) * L.dil, rp256 = (tc3::TT2 + reach + 7) / 8 * 8;
+    const int tm_slices = rp256 <= 320 && tc3::smem_bytes_tm(rp256, L.Rows, 2) + 1024 <= max_smem ? 2 : 1;   // per warpgroup
+    const int rows_pad = tm ? (128 * tm_slices + reach + 7) / 8 * 8
+                            : grouped ? rp_grouped : rp256;
     if (!persistent_ok || !fits(rows_pad)) return -1;
     tc3::Tc3Args t;
     memset(&t, 0, sizeof(t));
     t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
     t.w = grouped ? L.w_tcg : L.w_tc; t.rscale = L.tc_rscale; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
     t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = tc3::MROWS;
-    t.KJ = grouped ? J : L.K; t.dil_blk = grouped ? G * L.dil : L.dil; t.tstep = grouped ? tc3::TSTEP_GROUPED : tc3::TT2;
+    t.KJ = grouped && !tm ? J : L.K; t.dil_blk = grouped && !tm ? G * L.dil : L.dil;
+    t.tstep = tm ? 128 * tm_slices : grouped ? tc3::TSTEP_GROUPED : tc3::TT2;
     t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
     t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
     t.ymask = a.ymask; t.ymask_bs = a.ymask_bs;
@@ -911,7 +957,7 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     t.B = io.B; t.n_rtiles = (L.Rows + tc3::MROWS - 1) / tc3::MROWS;   // 1 in grouped mode (32 / 64 rows)
     set_window(t, a);
     t.err = g_tc_err;
-    size_t smem = tc3::smem_bytes3(rows_pad, L.tc_prec);
+    size_t smem = tm ? tc3::smem_bytes_tm(rows_pad, L.Rows, tm_slices) : tc3::smem_bytes3(rows_pad, L.tc_prec);
     set_ragged(t, a, smem, max_smem);
     // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
     // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
@@ -924,7 +970,9 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
         t.act_add = a.act_add; t.lrelu = a.act == ACT_LRELU; t.act_param = a.act_param;
     }
     const tc3::Tc3Kernel k = wg ? tc3::wavegrad_kernel(L.tc_prec, a.near_src > 0)
-                                : grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect) : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
+                                : tm      ? tc3::timemajor_kernel(L.Rows, tm_slices, reflect)
+                                : grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect)
+                                          : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
     const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
     const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
     B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));

@@ -167,6 +167,33 @@ __device__ __forceinline__ void wgmma_f16_m64n256_rs(float* d, const uint32_t (&
         : "memory");
 }
 
+// Time-major tiles of the 32 / 64-channel layers (conv_tc3.cuh): D[64 time steps x N channels] (+)= A[64 x 16] *
+// B[N x 16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators in the m64nN layout:
+// d[4j + {0,1}] = D[16 w + lane/4][8j + 2(lane%4) + {0,1}], d[4j + {2,3}] = the same columns of row + 8.
+__device__ __forceinline__ void wgmma_f16_m64n64(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+        " %32, %33, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_m64n32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
+        : "memory");
+}
+
 // Four 8x8 b16 matrices from shared memory; lane l gives the address of row l % 8 of matrix l / 8, and r[i] is matrix
 // i's element pair (row lane / 4, columns 2 (lane % 4) ..).  Matrices {rows 0-7, rows 8-15} x {k 0-7, k 8-15} in that
 // order form an m16k16 A fragment.

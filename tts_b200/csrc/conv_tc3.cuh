@@ -35,7 +35,9 @@
 // g, g+GRP, g+2*GRP, ... so one instruction stream of ceil(K/GRP) "tap blocks" (B shifted by GRP*dil rows per block)
 // replaces K of them and no MMA row is zero padding.  D_g[c, col] then still misses its own g*dil shift: the epilogue
 // reads row g * (128/GRP) + c at column col + g*dil and sums the GRP partials.  Tiles advance by 240 columns so every
-// shifted read stays inside the 256-column accumulator.
+// shifted read stays inside the 256-column accumulator.  3xTF32 and 16-bit operands only: at PREC_F16X3 the same layers
+// take the time-major kernel (conv1d_tc3t_kernel, tm_consumers), which swaps the GEMM's roles -- M = time, N = the 32 / 64
+// channels -- so every tap is summed in the accumulator and no MMA multiplies a padded tap.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -125,6 +127,18 @@ static inline size_t smem_bytes3(int rows_pad, int prec = PREC_FP32) {
     const bool b16 = prec == PREC_BF16 || prec == PREC_FP16;
     const size_t raw_ch = b16 ? KC16 : KC2, nsl = b16 ? 2 : 4;
     return (size_t)NRAW * raw_ch * RAWS * 4 + (size_t)NA2 * (nsl * rows_pad * 16) + NB2 * (nsl * MROWS * 16) + ACC_BYTES + 512;
+}
+// Time-major kernel (tm_consumers): a weight tap block is {W_hs, W_lo, W_hi}[2 slabs][C rows][16 B]; each warpgroup's
+// epilogue has two [C][64 * tms + 4] fp32 tiles (residual / output, accumulate operand), rows padded by 4 floats so that
+// the fragment stores of 8 time steps x 4 channels hit 32 banks
+__host__ __device__ constexpr uint32_t tm_block_bytes(int C) { return 3u * 2u * (uint32_t)C * 16u; }
+// Its weight ring is deeper than NB2: a tap block feeds only 3 * TMS m64nC MMAs per warpgroup, and a slot is refilled
+// one tap after its MMAs retire, so NB - 2 blocks must cover the L2 -> shared copy latency.  64 channels: what shared
+// memory leaves beside the 64-channel epilogue tiles.
+__host__ __device__ constexpr int tm_ring(int C) { return C == 64 ? 4 : 12; }
+__host__ __device__ constexpr uint32_t tm_epi_bytes(int C, int tms) { return 2u * 2u * (uint32_t)C * (64u * tms + 4u) * 4u; }
+static inline size_t smem_bytes_tm(int rows_pad, int C, int tms) {
+    return (size_t)NRAW * KC2 * RAWS * 4 + (size_t)NA2 * (4 * rows_pad * 16) + tm_ring(C) * tm_block_bytes(C) + tm_epi_bytes(C, tms) + 512;
 }
 static inline size_t ragged_table_bytes(int B) { return ((size_t)(B + 1) * sizeof(int) + 15) / 16 * 16; }
 
@@ -520,7 +534,194 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     }
 }
 
-template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false, bool NEAR = false, bool WG = false>
+// Consumers of the time-major kernel (PREC_F16X3, exactly C = 32 / 64 output channels).  The GEMM is transposed: M = time,
+// N = the C channels, K = input channels x taps, all summed in the accumulator.  The staged activation window is the A
+// operand (its K-major slabs are a valid m64k16 A image; tap k and slice s start k * dil + 64 s rows further) and the
+// weight block the B operand.  Warpgroup wg owns time steps wg * HW .. + HW - 1 of the tile (HW = 64 * TMS) for all C
+// channels: TMS m64nC accumulators, W_hs*X_lo + W_lo*X_hi + W_hi*X_hi per tap and chunk (small terms first), one tap's
+// group in flight while the next is issued.  Every output column takes the same sum in the same order wherever its
+// tile starts.
+// Epilogue, per warpgroup and without cross-warpgroup hand-off: on whole interior tiles of aligned layers, warp lq's
+// lane 0 prefetches channel rows lq * C/4 .. + C/4 - 1 of the residual (and the accumulate operand) into the warpgroup's
+// [C][HW] tiles by cp.async.bulk before the MMAs (RES_FULL[warp]); after them every thread finishes its fragment in
+// the grouped epilogue's order, ((acc * rscale) + (bias + cond)), ReLU, + res, * scale, + old, / post_div, writes it
+// transposed into the residual tile, and after a warpgroup barrier the same lanes store their rows with bulk copies.
+// Edge tiles and unaligned layers finish the fragment straight to global memory with bounds checks.
+template <int C, int TMS, typename Decode>
+__device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned char* smA, const unsigned char* smB, float* epi,
+                                             uint32_t bar0, const Decode& decode, int my_tiles, int nchunks, uint32_t slabA,
+                                             int warp, int lane) {
+    constexpr int HW = 64 * TMS, P = HW + 4, NA = C / 2;      // time steps per warpgroup, tile row pitch, accumulators per slice
+    constexpr int CW = C / 4;                                   // channel rows each warp prefetches and stores
+    constexpr uint32_t PLANE = 2u * C * 16u;                    // one of W_hs / W_lo / W_hi: [2 slabs][C rows][16 B]
+    constexpr int NB = tm_ring(C);
+    constexpr int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB, RES_FULL = 2 * NA2 + 2 * NB;
+    auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
+    const uint32_t stageA = 4u * slabA;
+    const int wg = warp >> 2, lq = warp & 3, K = a.KJ;
+    float* const rbuf = epi + (size_t)wg * 2 * C * P;           // residual in, output out
+    float* const obuf = rbuf + C * P;                           // accumulate operand
+    const uint64_t wdesc0 = make_desc(smem_u32(smB), C * 16);
+    const bool has_res = a.res != nullptr, acc_r = a.accum != 0, relu = a.relu != 0;
+    const bool bulk_layer = ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
+                            (!has_res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
+    const int c0 = 2 * (lane & 3), t0 = 16 * lq + (lane >> 2);  // fragment: channels 8j + c0 + {0,1}, time steps t0 (+8) + 64 s
+    bool ok = true;
+    int sa = 0; uint32_t pa = 0;                                // activation stage / its parity
+    int sb = 0; uint32_t pb = 0;                                // weight slot / its parity
+    uint32_t pr = 0;                                            // parity of RES_FULL
+#pragma unroll 1
+    for (int it = 0; it < my_tiles; ++it) {
+        int b, rt, q0;
+        decode(it, b, rt, q0);
+        const int qw = q0 + wg * HW;                            // this warpgroup's first column
+        const bool bulk = bulk_layer && q0 + 2 * HW <= a.Tout;
+        const bool pre = bulk && (has_res || acc_r);
+        if (bulk && lane == 0) {
+            bulk_wait_read();                                   // this warp's previous bulk stores are done reading its rows
+            if (pre) {
+                const uint32_t rf = BAR(RES_FULL + warp);
+                mbar_expect_tx(rf, (uint32_t)((has_res ? 1 : 0) + (acc_r ? 1 : 0)) * CW * HW * 4);
+                for (int c = lq * CW; c < (lq + 1) * CW; ++c) {
+                    if (has_res)
+                        bulk_g2s(smem_u32(rbuf + c * P), a.res + (long long)b * a.res_bs + (long long)c * a.res_cs + qw, HW * 4, rf);
+                    if (acc_r)
+                        bulk_g2s(smem_u32(obuf + c * P), a.y + (long long)b * a.y_bs + (long long)c * a.y_cs + qw, HW * 4, rf);
+                }
+            }
+        }
+        float d[TMS][NA];
+#pragma unroll
+        for (int s = 0; s < TMS; ++s)
+#pragma unroll
+            for (int i = 0; i < NA; ++i) d[s][i] = 0.f;
+        uint32_t acc = 0u;
+        int rel_b = -1, rel_a = -1;                             // operands of the group in flight
+        auto release = [&]() {
+            __syncwarp();
+            if (lane == 0) {                                    // one arrival per consumer warp
+                if (rel_b >= 0) mbar_arrive(BAR(B_EMPTY + rel_b));
+                if (rel_a >= 0) mbar_arrive(BAR(A_EMPTY + rel_a));
+            }
+        };
+#pragma unroll 1
+        for (int c = 0; c < nchunks; ++c) {
+            if (ok) ok = mbar_wait(BAR(A_FULL + sa), pa, a.err);
+            const uint32_t abase = smem_u32(smA + sa * stageA) + (uint32_t)(wg * HW) * 16u;
+            uint64_t xh = make_desc(abase, slabA), xl = make_desc(abase + 2 * slabA, slabA);
+#pragma unroll 1
+            for (int k = 0; k < K; ++k) {
+                if (ok) ok = mbar_wait(BAR(B_FULL + sb), pb, a.err);
+                if (ok) {
+                    const uint64_t whs = wdesc0 + (uint64_t)sb * (tm_block_bytes(C) >> 4);
+                    const uint64_t wlo = whs + (PLANE >> 4), whi = whs + 2 * (PLANE >> 4);
+                    wgmma_fence();
+#pragma unroll
+                    for (int s = 0; s < TMS; ++s) {                 // slice s: 64 rows = 64 descriptor units further
+                        if constexpr (C == 64) {
+                            wgmma_f16_m64n64(d[s], xl + 64 * s, whs, acc);
+                            wgmma_f16_m64n64(d[s], xh + 64 * s, wlo, 1u);
+                            wgmma_f16_m64n64(d[s], xh + 64 * s, whi, 1u);
+                        } else {
+                            wgmma_f16_m64n32(d[s], xl + 64 * s, whs, acc);
+                            wgmma_f16_m64n32(d[s], xh + 64 * s, wlo, 1u);
+                            wgmma_f16_m64n32(d[s], xh + 64 * s, whi, 1u);
+                        }
+                    }
+                    wgmma_commit();
+                }
+                wgmma_wait<1>();                                // the previous tap's group is done
+                release();
+                rel_b = sb;
+                rel_a = (k == K - 1) ? sa : -1;
+                acc = 1u;
+                xh += (uint64_t)a.dil; xl += (uint64_t)a.dil;
+                if (++sb == NB) { sb = 0; pb ^= 1u; }
+            }
+            if (++sa == NA2) { sa = 0; pa ^= 1u; }
+        }
+        wgmma_wait<0>();
+        release();
+
+        // per-channel constants of this thread's fragment columns
+        float bv[C / 8][2], sv[C / 8][2];
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int ch = 8 * j + c0 + e;
+                bv[j][e] = a.bias[ch];
+                if (a.cond) bv[j][e] += __ldg(a.cond + (long long)b * a.cond_bs + ch);
+                sv[j][e] = a.rscale[ch];
+            }
+        auto finish = [&](float v, int j, int e, float r, float o) {
+            float u = v * sv[j][e] + bv[j][e];
+            if (relu) u = fmaxf(u, 0.f);
+            if (has_res) u += r;
+            u *= a.scale;
+            if (acc_r) u += o;
+            if (a.post_div != 1.f) u = u / a.post_div;
+            return u;
+        };
+        if (bulk) {
+            if (pre) {                                          // waited for even after a failed wait: the copies always land
+#pragma unroll 1
+                for (int w = 0; w < 4; ++w) {
+                    const bool landed = mbar_wait(BAR(RES_FULL + 4 * wg + w), pr, a.err);
+                    ok = ok && landed;
+                }
+                pr ^= 1u;
+            } else {
+                named_bar_sync(5 + wg, 128);                    // every warp's previous bulk stores are done reading
+            }
+            if (ok) {
+#pragma unroll
+                for (int s = 0; s < TMS; ++s)
+#pragma unroll
+                    for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                float* p = rbuf + (8 * j + c0 + e) * P + 64 * s + t0 + 8 * h;
+                                const float r = has_res ? *p : 0.f;
+                                const float o = acc_r ? p[C * P] : 0.f;
+                                *p = finish(d[s][4 * j + 2 * h + e], j, e, r, o);
+                            }
+            }
+            fence_async_smem();                                 // the finished rows -> visible to the bulk copies (async proxy)
+            named_bar_sync(5 + wg, 128);
+            if (ok && lane == 0) {
+                for (int c = lq * CW; c < (lq + 1) * CW; ++c)
+                    bulk_s2g(a.y + (long long)b * a.y_bs + (long long)c * a.y_cs + qw, smem_u32(rbuf + c * P), HW * 4);
+                bulk_commit();
+            }
+        } else if (ok) {
+#pragma unroll
+            for (int s = 0; s < TMS; ++s)
+#pragma unroll
+                for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int ch = 8 * j + c0 + e, q = qw + 64 * s + t0 + 8 * h;
+                            if (q >= a.Tout) continue;
+                            float* yp = a.y + (long long)b * a.y_bs + (long long)ch * a.y_cs + q;
+                            const float r = has_res ? a.res[(long long)b * a.res_bs + (long long)ch * a.res_cs + q] : 0.f;
+                            const float o = acc_r ? *yp : 0.f;
+                            *yp = finish(d[s][4 * j + 2 * h + e], j, e, r, o);
+                        }
+        }
+    }
+    if (lane == 0) bulk_wait_all();                             // the bulk stores are complete before the dependent grid may read
+    __syncwarp();
+}
+
+template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false, bool NEAR = false, bool WG = false,
+          int TMC = 0, int TMS = 2>
+                                       // TMC: the time-major kernel's output channels (32 / 64; 0: off), TMS: its m64
+                                       // slices per warpgroup (tile width 128 * TMS), see tm_consumers;
                                        // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
                                        // plain-layer kernel (lean epilogue inline, general one out of line) -- false for the
                                        // WaveNet / masked / transposed layers (general epilogue inline); PREC: operand type;
@@ -538,19 +739,21 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     constexpr int SPC = KCH / RCH;               // raw stages per chunk (2 for X3)
     constexpr int NSL = B16 ? 2 : 4;             // 16-byte slabs per activation stage: two 16-bit slabs, or hi[2] + lo[2]
     constexpr int SLC = PREC != PREC_FP32 ? 8 : 4;   // channels per slab row
-    constexpr int NB = NB2;                      // weight ring depth
+    constexpr int NB = TMC ? tm_ring(TMC) : NB2; // weight ring depth
     constexpr bool SC = X3;                      // epilogues scale rows by rscale
-    constexpr bool BULK = GRP == 1 && LEAN;      // plain-layer kernel: whole interior tiles may take the bulk epilogue
+    constexpr bool TM = TMC != 0;                // time-major kernel (PREC_F16X3, 32 / 64 output channels)
+    constexpr bool BULK = GRP == 1 && LEAN && !TM;   // plain-layer kernel: whole interior tiles may take the bulk epilogue
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int ROWS = a.rows_pad, RAWW = a.raw_w, K = a.KJ;
     const uint32_t rawStage = (uint32_t)RCH * RAWS * 4;
     const uint32_t slabA = (uint32_t)ROWS * 16, stageA = NSL * slabA;
-    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = NSL * slabB;   // one tap block: [NSL slabs][128 rows][16 B]
+    // one tap block: [NSL slabs][128 rows][16 B]; time-major: {W_hs, W_lo, W_hi}[2 slabs][TMC rows][16 B]
+    const uint32_t slabB = (uint32_t)MROWS * 16, stageB = TM ? tm_block_bytes(TMC) : NSL * slabB;
     unsigned char* smRaw = smem;
     unsigned char* smA = smRaw + NRAW * rawStage;
     unsigned char* smB = smA + NA2 * stageA;
     float* accs = reinterpret_cast<float*>(smB + NB * stageB);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(accs) + ACC_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(accs) + (TM ? tm_epi_bytes(TMC, TMS) : ACC_BYTES));
     const int A_FULL = 0, A_EMPTY = NA2, B_FULL = 2 * NA2, B_EMPTY = 2 * NA2 + NB, RES_FULL = 2 * NA2 + 2 * NB;
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
@@ -844,6 +1047,9 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             }
         }
         __syncwarp();
+    } else if (TM && warp < W_PROD) {
+        if constexpr (TM)
+            tm_consumers<TMC, TMS>(a, smA, smB, accs, bar0, decode, my_tiles, nchunks, slabA, warp, lane);
     } else if (warp < W_PROD) {
         // ============================================================ consumers: MMA, then epilogue
         // Every lane runs the same loop (wgmma is warpgroup-collective); after a failed wait (`ok` false, the error flag
@@ -1072,16 +1278,30 @@ static inline Tc3Kernel plain_kernel(int prec, bool lean, bool reflect = false) 
     if (prec == PREC_F16X3) return lean ? conv1d_tc3_kernel<PREC_F16X3> : conv1d_tc3x_kernel<PREC_F16X3>;
     return lean ? conv1d_tc3_kernel<PREC_FP32> : conv1d_tc3x_kernel<PREC_FP32>;
 }
-// grouped kernel for 2 / 4 tap groups (any dilation with (GRP - 1) * dil <= 15)
+// grouped kernel for 2 / 4 tap groups (any dilation with (GRP - 1) * dil <= 15); 3xTF32 and 16-bit operands only
+// (PREC_F16X3 takes the time-major kernel)
 template <bool REFL>
 static inline Tc3Kernel grouped_kernel_t(int grp, int prec) {
     if (prec == PREC_BF16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_BF16, REFL> : conv1d_tc3g_kernel<4, PREC_BF16, REFL>;
     if (prec == PREC_FP16) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP16, REFL> : conv1d_tc3g_kernel<4, PREC_FP16, REFL>;
-    if (prec == PREC_F16X3) return grp == 2 ? conv1d_tc3g_kernel<2, PREC_F16X3, REFL> : conv1d_tc3g_kernel<4, PREC_F16X3, REFL>;
     return grp == 2 ? conv1d_tc3g_kernel<2, PREC_FP32, REFL> : conv1d_tc3g_kernel<4, PREC_FP32, REFL>;
 }
 static inline Tc3Kernel grouped_kernel(int grp, int prec = PREC_FP32, bool reflect = false) {
     return reflect ? grouped_kernel_t<true>(grp, prec) : grouped_kernel_t<false>(grp, prec);
+}
+
+// Time-major split-fp16 kernel for exactly C = 32 / 64 output rows, TMS m64 slices per warpgroup (tile width 128 * TMS)
+template <int C, int TMS, bool REFL>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3t_kernel(const __grid_constant__ Tc3Args a) {
+    tc3_body<1, true, PREC_F16X3, REFL, false, false, C, TMS>(a);
+}
+template <int C, bool REFL>
+static inline Tc3Kernel timemajor_kernel_t(int tms) {
+    return tms == 2 ? conv1d_tc3t_kernel<C, 2, REFL> : conv1d_tc3t_kernel<C, 1, REFL>;
+}
+static inline Tc3Kernel timemajor_kernel(int C, int tms, bool reflect) {
+    if (C == 64) return reflect ? timemajor_kernel_t<64, true>(tms) : timemajor_kernel_t<64, false>(tms);
+    return reflect ? timemajor_kernel_t<32, true>(tms) : timemajor_kernel_t<32, false>(tms);
 }
 
 }  // namespace tc3
