@@ -919,6 +919,77 @@ int b200tts_tacotron2_decode_loop(const b200tts_tacotron2* h, const int64_t* len
 int b200tts_tacotron2_postnet(const b200tts_tacotron2* h, const float* dec_out, const int32_t* frames, int B, int F,
                               int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Tacotron (1) inference (text -> spectrogram, autoregressive GRU attention decoder) ----------------------------
+ * Replaces Tacotron.inference (TTS/tts/models/tacotron.py:218-271) in three calls:
+ *   encode      - embedding (256) + Encoder (TTS/tts/layers/tacotron/tacotron.py:210-229): Prenet (Linear 256 -> 256 ->
+ *                 128 with bias, ReLU, no dropout at inference) and the CBHG (K = 16, projections [128, 128]); for the
+ *                 original attention also inputs_layer of every encoder output (step-invariant, hoisted out of the loop).
+ *   decode_loop - Decoder.inference (tacotron.py:457-485): Prenet (256, 128, with bias, "bn" folded), attention GRUCell
+ *                 (256), OriginalAttention or MonotonicDynamicConvolutionAttention, project_to_decoder_in, two residual
+ *                 GRUCells (256), proj_to_mel and the stopnet.  chunk_steps steps per CUDA graph replay, 2 + B words
+ *                 read after each chunk.
+ *   postnet     - last_linear(PostCBHG(decoder_outputs)) (K = 8, projections [256, C], pre_highway when C != 128).
+ * A CBHG's convs are BatchNormConv1d (no conv bias, eval BatchNorm with eps 1e-3 folded), padded [(k-1)/2, k/2].
+ * Batched, unlike the reference: row b computes the reference's inference(text[b:b+1, :lengths[b]]): every conv sees
+ * zeros past the row, the backward GRU starts at the row's last token or frame, outputs are zero past the row, and the
+ * stop rule is the reference's: with n steps taken, stop once n > lengths[b] / 4 and (sigmoid(stop logit) > 0.6 or the
+ * attention weight at token lengths[b] - 1 > 0.6), or once n > max_decoder_steps (so up to max_decoder_steps + 1 steps).
+ * The loop runs in FP32 on the FMA pipe.
+ * weights (host, PyTorch layouts), in this order (a CBHG: per bank conv k = 1..K conv1d.weight [128, Cin, k],
+ * bn.weight, .bias, .running_mean, .running_var; the same five for each of the two projections; pre_highway.weight
+ * [128, Cin] when Cin != 128; per highway H.weight, H.bias, T.weight, T.bias; gru weight_ih_l0 [384, 128],
+ * weight_hh_l0 [384, 128], bias_ih_l0, bias_hh_l0, then the four _reverse):
+ *   embedding.weight [n_vocab, 256]
+ *   encoder.prenet layer l < 2: linear_layer.weight, .bias
+ *   encoder CBHG (Cin 128, K 16, projections 128, 128)
+ *   decoder prenet layer l < 2: linear_layer.weight [out, in] (in = frame_channels * memory_size with a memory queue,
+ *     else frame_channels; then 256), .bias; prenet_bn: then batch_normalization.weight, .bias, .running_mean,
+ *     .running_var (eps 1e-5)
+ *   attention_rnn.weight_ih [768, 384], weight_hh [768, 256], bias_ih, bias_hh
+ *   attention as b200tts_tacotron2 (query width 256, inputs_layer [128, 256])
+ *   project_to_decoder_in.weight [256, 512], .bias
+ *   decoder_rnns.{0,1}.weight_ih [768, 256], weight_hh [768, 256], bias_ih, bias_hh
+ *   proj_to_mel.weight [C * r_init, 256], .bias; stopnet.linear.weight [1, 256 + C * r_init], .bias
+ *   postnet CBHG (Cin C, K 8, projections 256, C)
+ *   last_linear.weight [out_channels, 256], .bias
+ */
+typedef struct {
+    int n_vocab;
+    int frame_channels;        /* C: decoder_output_dim */
+    int out_channels;          /* last_linear rows */
+    int r_init;                /* proj_to_mel has C * r_init rows */
+    int memory_size;           /* <= 0: the prenet reads the last frame; else a queue of memory_size frames */
+    int attention_type;        /* 0: "original", 1: "dynamic_convolution" */
+    int location_attn;         /* original: location-sensitive */
+    int attention_norm;        /* original: 0 sigmoid, 1 softmax */
+    int prenet_bn;             /* prenet_type "bn" */
+    int prenet_dropout;        /* 0: no dropout layer; else p = 0.5 where decode_loop is given masks */
+} b200tts_tacotron_config;
+typedef struct b200tts_tacotron b200tts_tacotron;
+int b200tts_tacotron_create(const b200tts_tacotron_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_tacotron** out);
+void b200tts_tacotron_destroy(b200tts_tacotron* h);
+/* one workspace serves all three calls of an utterance batch: B rows of up to Tt tokens and up to F frames */
+size_t b200tts_tacotron_workspace_bytes(const b200tts_tacotron* h, int B, int Tt, int F);
+/* tokens int64 [B, Tt], lengths int64 [B] (1 .. Tt) -> enc_out [B, Tt, 256] (zero past lengths[b]); the hoisted
+ * inputs_layer term stays in the workspace for decode_loop() */
+int b200tts_tacotron_encode(const b200tts_tacotron* h, const int64_t* tokens, const int64_t* lengths, int B, int Tt,
+                            float* enc_out, void* workspace, size_t workspace_bytes, void* stream);
+/* the decoder loop on encode()'s state in the same workspace.  r: reduction rate (1 .. r_init); max_steps:
+ * max_decoder_steps (>= 1), so S = max_steps + 1 steps at most; drop (nullable; used with prenet_dropout only): uint8
+ * [B, S, 2, 256] (layer 1 reads the first 128 of its 256), nonzero keeps a unit (doubled); chunk_steps: steps per graph
+ * replay (even).  Out (device, zero past each row): dec_out [B, S * r, C], stop_tokens [B, S] (sigmoid values),
+ * alignments [B, S, Tt]; steps (host int32 [B]): decoder steps per row (frames = steps * r).  Synchronises the
+ * stream. */
+int b200tts_tacotron_decode_loop(const b200tts_tacotron* h, const int64_t* lengths, const float* enc_out, int B, int Tt,
+                                 int r, int max_steps, const uint8_t* drop, int chunk_steps, float* dec_out,
+                                 float* stop_tokens, float* alignments, int32_t* steps, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+/* dec_out [B, Fpitch, C], frames (device int32 [B]) -> out [B, F, out_channels] = last_linear(PostCBHG(dec_out)) below
+ * frames[b], zero past it */
+int b200tts_tacotron_postnet(const b200tts_tacotron* h, const float* dec_out, const int32_t* frames, int B, int F,
+                             int Fpitch, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -124,7 +124,8 @@ DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9:
                   11: "attn_fma", 12: "tc3w_tf32", 13: "tc3w_tf32_near", 14: "tc3w_f16x3", 15: "tc3w_f16x3_near",
                   16: "fma_wg", 17: "fma_wg_near", 18: "lstm_bi", 19: "lstm_cell", 20: "hmm_linear", 21: "hmm_step",
                   22: "pwgan_tc", 23: "pwgan_aux", 24: "taco_attn", 25: "taco_step", 26: "lstm_cell32",
-                  27: "univnet_predict", 28: "univnet_lvc"}
+                  27: "univnet_predict", 28: "univnet_lvc", 29: "gru_cell", 30: "gru_cell32", 31: "bigru",
+                  32: "highway", 33: "taco1_step"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}

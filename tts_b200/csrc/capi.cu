@@ -20,6 +20,7 @@ struct b200tts_forward_tts { ForwardTTS impl; };
 struct b200tts_wavegrad { Wavegrad impl; };
 struct b200tts_overflow { Overflow impl; };
 struct b200tts_tacotron2 { Tacotron2 impl; };
+struct b200tts_tacotron { Tacotron impl; };
 struct b200tts_pwgan { Pwgan impl; };
 struct b200tts_univnet { Univnet impl; };
 
@@ -39,6 +40,7 @@ static_assert(!std::is_copy_constructible_v<ForwardTTS>);
 static_assert(!std::is_copy_constructible_v<Wavegrad>);
 static_assert(!std::is_copy_constructible_v<Overflow>);
 static_assert(!std::is_copy_constructible_v<Tacotron2>);
+static_assert(!std::is_copy_constructible_v<Tacotron>);
 static_assert(!std::is_copy_constructible_v<Pwgan>);
 static_assert(!std::is_copy_constructible_v<Univnet>);
 
@@ -622,6 +624,41 @@ int b200tts_tacotron2_postnet(const b200tts_tacotron2* h, const float* dec_out, 
                               int Fpitch, float* mel, void* workspace, size_t workspace_bytes, void* stream) {
     if (!h) { set_error("tacotron2_postnet: null handle"); return 1; }
     return h->impl.postnet(dec_out, frames, B, F, Fpitch, mel, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200tts_tacotron_create(const b200tts_tacotron_config* cfg, const float* const* weights, int num_weights,
+                            b200tts_tacotron** out) {
+    if (!cfg || !weights || !out) { set_error("tacotron_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_tacotron* h = new (std::nothrow) b200tts_tacotron();
+    if (!h) { set_error("tacotron_create: out of host memory"); return 1; }
+    int rc = h->impl.init(*cfg, weights, num_weights);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+void b200tts_tacotron_destroy(b200tts_tacotron* h) { delete h; }
+size_t b200tts_tacotron_workspace_bytes(const b200tts_tacotron* h, int B, int Tt, int F) {
+    return h ? h->impl.workspace_bytes(B, Tt, F) : 0;
+}
+int b200tts_tacotron_encode(const b200tts_tacotron* h, const int64_t* tokens, const int64_t* lengths, int B, int Tt,
+                            float* enc_out, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("tacotron_encode: null handle"); return 1; }
+    return h->impl.encode((const long long*)tokens, (const long long*)lengths, B, Tt, enc_out, workspace,
+                          workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_tacotron_decode_loop(const b200tts_tacotron* h, const int64_t* lengths, const float* enc_out, int B, int Tt,
+                                 int r, int max_steps, const uint8_t* drop, int chunk_steps, float* dec_out,
+                                 float* stop_tokens, float* alignments, int32_t* steps, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("tacotron_decode_loop: null handle"); return 1; }
+    return h->impl.decode_loop((const long long*)lengths, enc_out, B, Tt, r, max_steps, drop, chunk_steps, dec_out,
+                               stop_tokens, alignments, steps, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int b200tts_tacotron_postnet(const b200tts_tacotron* h, const float* dec_out, const int32_t* frames, int B, int F,
+                             int Fpitch, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h) { set_error("tacotron_postnet: null handle"); return 1; }
+    return h->impl.postnet(dec_out, frames, B, F, Fpitch, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

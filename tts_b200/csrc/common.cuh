@@ -232,7 +232,11 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // Tacotron2 (tacotron2.cu): the attention step, the step epilogue; the LSTMCell with 32 rows per weight read
              DISPATCH_TACO_ATTN = 24, DISPATCH_TACO_STEP = 25, DISPATCH_LSTM_CELL32 = 26,
              // UnivNet (univnet.cu): the kernel-prediction GEMM, the fused LVC layer
-             DISPATCH_UNIVNET_PREDICT = 27, DISPATCH_UNIVNET_LVC = 28 };
+             DISPATCH_UNIVNET_PREDICT = 27, DISPATCH_UNIVNET_LVC = 28,
+             // Tacotron (tacotron.cu, recurrent.cu): the GRUCell (8 / 32 rows per weight read), the persistent biGRU,
+             // the highway stack, the step epilogue
+             DISPATCH_GRU_CELL = 29, DISPATCH_GRU_CELL32 = 30, DISPATCH_BIGRU = 31, DISPATCH_HIGHWAY = 32,
+             DISPATCH_TACO1_STEP = 33 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

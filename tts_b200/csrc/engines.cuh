@@ -279,6 +279,37 @@ struct LinArgs {
     int B = 0;
 };
 int launch_linear(const LinArgs& a, cudaStream_t st, bool note);
+// One GRUCell step (launch_gru): segments [0, nin) are the input x, [nin, nseg) the hidden state (torch rows r, z, n of
+// W_ih / W_hh, H each); bias [4][H] = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn); h_in [b * hin_bs + j] is the previous h.
+// h_out[b * h_bs + j] = h'; with x_out also x_out[b * xo_bs + j] = h' + res[b * res_bs + j].  Rows with done[b] skip.
+struct GruArgs {
+    LstmSeg seg[3]; int nseg = 0, nin = 0;
+    int H = 0;
+    const float* bias = nullptr;
+    const float* h_in = nullptr; int hin_bs = 0;
+    float* h_out = nullptr; int h_bs = 0;
+    const float* res = nullptr; int res_bs = 0;
+    float* x_out = nullptr; int xo_bs = 0;
+    const int* done = nullptr;
+    int B = 0;
+};
+// rows_per_block (8 or 32): batch rows served by one weight read; a row's result does not depend on it.
+int launch_gru(const GruArgs& a, int rows_per_block, cudaStream_t st, bool note);
+// A bidirectional GRU layer of hidden size GRU_H over whole sequences, one launch (launch_bigru, B x 2 CTAs):
+// pre[b * pre_bs + (d * 3H + row) * pre_cs + t] = W_ih x + b_ih, plus b_hr / b_hz on the r / z rows (direction d);
+// whh: both directions' W_hh as pack_bigru_whh lays them out; bhn [2][H].  out[b * out_bs + t * out_ts + (d * H + j) *
+// out_cs] = h_t of direction d for t < len_b (lens32 or lens64), zero for len_b <= t < T.
+constexpr int GRU_H = 128, BIGRU_THREADS = 4 * GRU_H;
+struct BiGruArgs {
+    const float* pre = nullptr; long long pre_bs = 0; int pre_cs = 0;
+    const float* whh = nullptr; const float* bhn = nullptr;
+    float* out = nullptr; long long out_bs = 0; int out_ts = 0, out_cs = 0;
+    const int* lens32 = nullptr; const long long* lens64 = nullptr;
+    int T = 0;
+};
+// one direction's W_hh [3H][H] (torch layout) -> dst [3 * 32][BIGRU_THREADS], the kernel's shared-memory image
+void pack_bigru_whh(const float* whh, float* dst);
+int launch_bigru(const BiGruArgs& a, int B, cudaStream_t st);
 // y[b, c, n] = x[b, n, c] for x [B, N, E]
 int launch_transpose(const float* x, float* y, int B, int N, int E, cudaStream_t st);
 // An autoregressive loop as CUDA-graph chunks: step(stream, parity, note) enqueues one step (parity = step index within
@@ -352,6 +383,72 @@ struct Tacotron2 {
     DevBuf<float> proj_w, proj_b, stop_w, stop_b;
     int init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw);
     size_t persist_bytes(int B, int Tt) const;
+    size_t workspace_bytes(int B, int Tt, int F) const;
+    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
+               size_t ws_bytes, cudaStream_t st) const;
+    int decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
+                    const unsigned char* drop, int chunk_steps, float* dec_out, float* stop_tokens, float* alignments,
+                    int* steps, void* ws, size_t ws_bytes, cudaStream_t st) const;
+    int postnet(const float* dec_out, const int* frames, int B, int F, int Fpitch, float* mel, void* ws,
+                size_t ws_bytes, cudaStream_t st) const;
+};
+
+// One attention step of the Tacotron models (tacotron2.cu; OriginalAttention / MonotonicDynamicConvolutionAttention
+// with mask None), one CTA per running row over its len_b tokens: the weights, the context and the alignment row of step
+// ctl[1].  Instantiated for query / encoder widths 1024 / 512 (Tacotron2) and 256 / 256 (Tacotron).
+struct AttnArgs {
+    const float* q = nullptr;                 // [B, Q] attention-RNN output
+    const float* enc = nullptr;               // [B, Tt, E] encoder outputs
+    const float* pin = nullptr;               // [B, A, Tt] inputs_layer(encoder outputs)
+    float* alpha = nullptr; float* cum = nullptr;   // [B, Tt] previous / cumulative weights
+    float* ctx = nullptr;                     // [B, E]
+    float* align = nullptr; int max_steps = 0;      // [B, max_steps, Tt]
+    const long long* lens = nullptr; const int* done = nullptr; const int* ctl = nullptr;
+    int Tt = 0, type = 0, location = 0, softmax = 0;
+    // original: Wq [A][Q], v [A], vb; location: Wc [F][2][K], Wd [A][F]
+    // DCA: Wq [A][Q], bq [A], Wk [F*K][A], Ws [F][K], Wsl [A][F], Wdl [A][F], bdl [A], v [A], prior [11]
+    const float *Wq = nullptr, *bq = nullptr, *v = nullptr, *Wc = nullptr, *Wd = nullptr;
+    const float *Wk = nullptr, *Ws = nullptr, *Wsl = nullptr, *Wdl = nullptr, *bdl = nullptr, *prior = nullptr;
+    float vb = 0.f;
+};
+// the dynamic shared memory of the attention step for Tt tokens (set as the kernel's limit on the current device;
+// fails past the opt-in maximum), then the launch itself (Q / E: 1024 / 512 or 256 / 256)
+int taco_attn_prepare(int Q, int E, int Tt, size_t* smem);
+int launch_taco_attn(const AttnArgs& a, int Q, int E, int B, size_t smem, cudaStream_t st, bool note);
+
+// Tacotron (1) inference (tacotron.cu).  encode: embedding, the encoder prenet and CBHG (K = 16) into the encoder
+// outputs [B, Tt, 256] and, for the original attention, inputs_layer of them.  decode_loop: the GRU attention decoder,
+// chunk_steps steps per CUDA graph replay.  postnet: the postnet CBHG (K = 8) and last_linear.  A CBHG is the conv bank
+// as one conv over the union tap window, the two projections (BatchNorm, eps 1e-3, folded; ReLU in the epilogue; masked
+// past each row), the fused highway stack, the biGRU input projection as a 1x1 conv and the persistent biGRU.
+struct Tacotron {
+    struct Cbhg {
+        int Cin = 0, K = 0, P1 = 0;
+        ConvLayer bank, proj1, proj2, gru_in;
+        DevBuf<float> pre_w;                   // pre_highway transposed [Cin][128] (empty: none)
+        DevBuf<float> hw_w, hw_b;              // per highway [H | T] transposed [128][256], bias [256]
+        DevBuf<float> whh, bhn;                // pack_bigru_whh images of both directions, b_hn [2][128]
+        int init(int Cin, int K, int P1, const float* const* w, int* consumed);
+        size_t scratch_bytes(int B, int T) const;
+        // x [B, Cin, T] (zero past each row) -> out as BiGruArgs describes it
+        int run(const float* x, const float* mask, const int* lens32, const long long* lens64, int B, int T, float* out,
+                long long out_bs, int out_ts, int out_cs, Arena& ar, cudaStream_t st) const;
+    };
+    b200tts_tacotron_config c;
+    int Cm = 0;                                // prenet input width: C * memory_size (memory queue) or C
+    DevBuf<float> emb;
+    ConvLayer eprenet[2];
+    Cbhg ecbhg, pcbhg;
+    ConvLayer inproj, last;
+    DevBuf<float> prenet_w[2], prenet_b[2];
+    DevBuf<float> arnn_wih, arnn_whh, arnn_b;   // [768][384], [768][256], bias as GruArgs
+    DevBuf<float> att_wq, att_bq, att_v, att_wc, att_wd;
+    DevBuf<float> att_prior, att_wk, att_ws, att_wsl, att_wdl, att_bdl;
+    float att_vb = 0.f;
+    DevBuf<float> pdi_w, pdi_b;                 // project_to_decoder_in [256][512]
+    DevBuf<float> drnn_wih[2], drnn_whh[2], drnn_b[2];
+    DevBuf<float> proj_w, proj_b, stop_w, stop_b;
+    int init(const b200tts_tacotron_config& cfg, const float* const* w, int nw);
     size_t workspace_bytes(int B, int Tt, int F) const;
     int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
                size_t ws_bytes, cudaStream_t st) const;

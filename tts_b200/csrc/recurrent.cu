@@ -1,6 +1,7 @@
-// Recurrent building blocks shared by the autoregressive text-to-mel models (Overflow / Neural-HMM, Tacotron2):
-// the Tacotron2-style text encoder (embedding, ConvBNBlocks, BiLSTM), the batch-amortised LSTM step, the GEMV layer with
-// the prenet dropout, and the driver that runs an autoregressive loop as CUDA-graph chunks of steps.
+// Recurrent building blocks shared by the autoregressive text-to-mel models (Overflow / Neural-HMM, Tacotron2, Tacotron):
+// the Tacotron2-style text encoder (embedding, ConvBNBlocks, BiLSTM), the batch-amortised LSTM and GRU steps, the
+// persistent bidirectional GRU, the GEMV layer with the prenet dropout, and the driver that runs an autoregressive loop
+// as CUDA-graph chunks of steps.
 // Everything is exact FP32 on the FMA pipe: the loops' stop decisions feed back through them, so they must not depend
 // on tensor-core rounding.
 #include <math.h>
@@ -122,6 +123,133 @@ __global__ void __launch_bounds__(256) lstm_kernel(LstmArgs a) {
     if (a.out) a.out[(size_t)b * a.out_bs + (size_t)t * a.out_ts + d * H + j] = h;
 }
 
+// Segment s of a GRU step: the (r, z, n) rows (j, H + j, 2H + j) of W times the staged columns, n into acc slot NS
+// (2: the input part W_in x, 3: the hidden part W_hn h, which the n gate scales by r).
+template <int NB, int NS>
+__device__ __forceinline__ void gru_seg_fma(float (&acc)[4 * NB], const float* W, int ldw, int H, int j, int k0,
+                                            const float* xs, int KC, int kc, int nb, int lane) {
+    for (int k = lane; k < kc; k += 32) {
+        float w[3];
+#pragma unroll
+        for (int g = 0; g < 3; ++g) w[g] = W[(size_t)(g * H + j) * ldw + k0 + k];
+#pragma unroll
+        for (int bb = 0; bb < NB; ++bb) {
+            const float xv = xs[(bb < nb ? bb : 0) * KC + k];
+            acc[bb * 4 + 0] = fmaf(w[0], xv, acc[bb * 4 + 0]);
+            acc[bb * 4 + 1] = fmaf(w[1], xv, acc[bb * 4 + 1]);
+            acc[bb * 4 + NS] = fmaf(w[2], xv, acc[bb * 4 + NS]);
+        }
+    }
+}
+
+// One GRUCell step for UNITS hidden units x NB batch rows per block, batch-amortised as lstm_kernel: warp w owns unit j,
+// segments [0, nin) are the input x and the rest the hidden state h, lane l sums columns l (mod 32) of each segment in
+// order, and the same reduction leaves lane l with row l % NB's four sums (r, z, n_x, n_h).
+//   r = sig(sum_r + b_r), z = sig(sum_z + b_z), n = tanh(n_x + b_in + r (n_h + b_hn)), h' = (1 - z) n + z h
+template <int NB>
+__global__ void __launch_bounds__(256) gru_kernel(GruArgs a) {
+    constexpr int KC = STAGE / NB;
+    __shared__ float xs[NB * KC];
+    const int H = a.H, b0 = blockIdx.z * NB, nb = min(NB, a.B - b0);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, j = blockIdx.x * UNITS + warp;
+    if (block_rows_done(a.done, b0, nb)) return;
+    float acc[4 * NB];   // [bb][r, z, n_x, n_h]
+#pragma unroll
+    for (int i = 0; i < 4 * NB; ++i) acc[i] = 0.f;
+    for (int s = 0; s < a.nseg; ++s) {
+        const LstmSeg& sg = a.seg[s];
+        for (int k0 = 0; k0 < sg.K; k0 += KC) {
+            const int kc = min(KC, sg.K - k0);
+            __syncthreads();
+            for (int i = threadIdx.x; i < nb * kc; i += blockDim.x) {
+                const int bb = i / kc, k = i - bb * kc;
+                xs[bb * KC + k] = sg.x[(size_t)(b0 + bb) * sg.x_bs + k0 + k];
+            }
+            __syncthreads();
+            if (j >= H) continue;
+            if (s < a.nin) gru_seg_fma<NB, 2>(acc, sg.W, sg.ldw, H, j, k0, xs, KC, kc, nb, lane);
+            else gru_seg_fma<NB, 3>(acc, sg.W, sg.ldw, H, j, k0, xs, KC, kc, nb, lane);
+        }
+    }
+    if (j >= H) return;
+    reduce_rows<16, NB>(acc, lane);
+    if (lane >= nb) return;
+    const int b = b0 + lane;
+    if (a.done[b]) return;
+    const float r = sigmoidf_(acc[0] + a.bias[j]);
+    const float z = sigmoidf_(acc[1] + a.bias[H + j]);
+    const float n = tanhf(acc[2] + a.bias[2 * H + j] + r * (acc[3] + a.bias[3 * H + j]));
+    const float h = (1.f - z) * n + z * a.h_in[(size_t)b * a.hin_bs + j];
+    a.h_out[(size_t)b * a.h_bs + j] = h;
+    if (a.x_out) a.x_out[(size_t)b * a.xo_bs + j] = h + a.res[(size_t)b * a.res_bs + j];
+}
+
+// A whole bidirectional GRU layer (H = 128) in one launch: CTA (b, d) runs direction d of row b over its len_b steps
+// (forward t = s, backward t = len_b - 1 - s) with W_hh resident in shared memory for the whole sequence.  Thread
+// tid = 4 j + q owns unit j and the columns k = 4 i + q (i < 32) of its three W_hh rows, stored at [(g * 32 + i) * 512 +
+// tid] so a warp reads 32 consecutive words; h is double-buffered in shared memory, so a step has one barrier.  The
+// four partial sums of a row are combined by the xor butterfly (the same two pairs in the same order for every row).
+// Past len_b the row's outputs are zero.
+__global__ void __launch_bounds__(BIGRU_THREADS, 1) bigru_kernel(BiGruArgs a) {
+    extern __shared__ float sm[];
+    float* Ws = sm;                              // [3 * 32][512]
+    float* hs = sm + 3 * 32 * BIGRU_THREADS;     // [2][128]
+    const int b = blockIdx.x, d = blockIdx.y, tid = threadIdx.x, j = tid >> 2, q = tid & 3;
+    const int len = a.lens64 ? (int)a.lens64[b] : a.lens32[b];
+    {
+        const float4* src = reinterpret_cast<const float4*>(a.whh + (size_t)d * 3 * 32 * BIGRU_THREADS);
+        float4* dst = reinterpret_cast<float4*>(Ws);
+        for (int i = tid; i < 3 * 32 * BIGRU_THREADS / 4; i += BIGRU_THREADS) dst[i] = src[i];
+    }
+    if (tid < 2 * GRU_H) hs[tid] = 0.f;
+    float* out = a.out + (size_t)b * a.out_bs + (size_t)(d * GRU_H) * a.out_cs;
+    for (int i = tid; i < (a.T - len) * GRU_H; i += BIGRU_THREADS) {
+        const int t = len + i / GRU_H, c = i % GRU_H;
+        out[(size_t)t * a.out_ts + (size_t)c * a.out_cs] = 0.f;
+    }
+    const float bhn = a.bhn[d * GRU_H + j];
+    const float* pre = a.pre + (size_t)b * a.pre_bs + (size_t)(d * 3 * GRU_H + j) * a.pre_cs;
+    float pr = 0.f, pz = 0.f, pn = 0.f;
+    if (q == 0 && len > 0) {
+        const int t = d ? len - 1 : 0;
+        pr = pre[t]; pz = pre[(size_t)GRU_H * a.pre_cs + t]; pn = pre[(size_t)2 * GRU_H * a.pre_cs + t];
+    }
+    __syncthreads();
+    for (int s = 0; s < len; ++s) {
+        const int t = d ? len - 1 - s : s;
+        const float* hc = hs + (s & 1) * GRU_H;
+        float* hn = hs + ((s & 1) ^ 1) * GRU_H;
+        float npr = 0.f, npz = 0.f, npn = 0.f;   // the next step's input projection, loaded under this step's sums
+        if (q == 0 && s + 1 < len) {
+            const int tn = d ? t - 1 : t + 1;
+            npr = pre[tn]; npz = pre[(size_t)GRU_H * a.pre_cs + tn]; npn = pre[(size_t)2 * GRU_H * a.pre_cs + tn];
+        }
+        float ar = 0.f, az = 0.f, an = 0.f;
+#pragma unroll 8
+        for (int i = 0; i < 32; ++i) {
+            const float hv = hc[4 * i + q];
+            ar = fmaf(Ws[(0 * 32 + i) * BIGRU_THREADS + tid], hv, ar);
+            az = fmaf(Ws[(1 * 32 + i) * BIGRU_THREADS + tid], hv, az);
+            an = fmaf(Ws[(2 * 32 + i) * BIGRU_THREADS + tid], hv, an);
+        }
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+            ar += __shfl_xor_sync(0xffffffffu, ar, o);
+            az += __shfl_xor_sync(0xffffffffu, az, o);
+            an += __shfl_xor_sync(0xffffffffu, an, o);
+        }
+        if (q == 0) {
+            const float r = sigmoidf_(pr + ar), z = sigmoidf_(pz + az);
+            const float n = tanhf(pn + r * (an + bhn));
+            const float h = (1.f - z) * n + z * hc[j];
+            hn[j] = h;
+            out[(size_t)t * a.out_ts + (size_t)j * a.out_cs] = h;
+        }
+        pr = npr; pz = npz; pn = npn;
+        __syncthreads();
+    }
+}
+
 // y[b, r] = act(W[r] . [x | x2][b] + bias[r] + add[b, r, state[b]]), then the prenet dropout (drop[b, f, layer, r] ?
 // 2v : 0 with f the loop's step counter ctl[1]); rows that are done skip.  One warp per row r, LIN_NB batch rows per
 // block; the input is staged in chunks of STAGE / LIN_NB columns (lane l sums columns l (mod 32) in order).
@@ -199,6 +327,47 @@ int launch_lstm(const LstmArgs& a, int dirs, int rows_per_block, int dispatch_id
     }
     count_launch();
     if (note) dispatch_note(dispatch_id);
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int launch_gru(const GruArgs& a, int rows_per_block, cudaStream_t st, bool note) {
+    B200_REQUIRE(a.nseg >= 1 && a.nseg <= 3 && a.nin >= 1 && a.nin < a.nseg && a.H > 0 && a.B >= 1 && a.done &&
+                 (!a.x_out || a.res), "gru: bad arguments");
+    const int nb = rows_per_block;
+    dim3 grid((a.H + UNITS - 1) / UNITS, 1, (a.B + nb - 1) / nb);
+    switch (nb) {
+        case 8: gru_kernel<8><<<grid, 256, 0, st>>>(a); break;
+        case 32: gru_kernel<32><<<grid, 256, 0, st>>>(a); break;
+        default: set_error("gru: rows_per_block must be 8 or 32, got %d", nb); return 1;
+    }
+    count_launch();
+    if (note) dispatch_note(nb == 32 ? DISPATCH_GRU_CELL32 : DISPATCH_GRU_CELL);
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+void pack_bigru_whh(const float* whh, float* dst) {
+    for (int g = 0; g < 3; ++g)
+        for (int i = 0; i < 32; ++i)
+            for (int t = 0; t < BIGRU_THREADS; ++t) {
+                const int j = t >> 2, q = t & 3;
+                dst[(size_t)(g * 32 + i) * BIGRU_THREADS + t] = whh[(size_t)(g * GRU_H + j) * GRU_H + 4 * i + q];
+            }
+}
+
+int launch_bigru(const BiGruArgs& a, int B, cudaStream_t st) {
+    B200_REQUIRE(a.pre && a.whh && a.bhn && a.out && (a.lens32 || a.lens64) && B >= 1 && a.T >= 1, "bigru: bad arguments");
+    constexpr int smem = sizeof(float) * (3 * 32 * BIGRU_THREADS + 2 * GRU_H);
+    static DeviceOnce once;
+    if (int rc = device_once(once, nullptr, [](int) -> int {
+            B200_CUDA_OK(cudaFuncSetAttribute(bigru_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            return 0;
+        }))
+        return rc;
+    bigru_kernel<<<dim3(B, 2), BIGRU_THREADS, smem, st>>>(a);
+    count_launch();
+    dispatch_note(DISPATCH_BIGRU);
     B200_CUDA_OK(cudaGetLastError());
     return 0;
 }

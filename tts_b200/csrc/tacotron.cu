@@ -1,0 +1,653 @@
+// Tacotron (1) inference: text -> spectrogram through the GRU attention decoder.
+// Reference: TTS/tts/models/tacotron.py:218-271 (inference), TTS/tts/layers/tacotron/tacotron.py (BatchNormConv1d,
+//            Highway, CBHG, Encoder, PostCBHG, Decoder), common_layers.py:63-119 (Prenet), attentions.py.
+// The decoder loop is exact FP32 on the FMA pipe (the stop decision feeds back through it).  Per step: two prenet GEMVs,
+// the attention GRUCell, one attention launch per row, project_to_decoder_in, the two residual GRUCells, proj_to_mel,
+// the stopnet and the step epilogue -- 10 launches, captured as CUDA-graph chunks.
+#include <math.h>
+
+#include "engines.cuh"
+
+namespace b200tts {
+
+namespace {
+
+constexpr int EMB = 256, E = 256, Q = 256, D = 256, A = 128, BANK = 128, HW = 128, NHW = 4;
+constexpr int PN0 = 256, PN1 = 128;      // decoder and encoder prenet widths
+constexpr int HW_TF = 16;                // frames per highway CTA
+constexpr int HW_MAX_CIN = 1024;         // widest pre_highway input the highway kernel stages
+
+__device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
+
+// The CBHG's highway stack over a tile of HW_TF frames of row blockIdx.y, held in shared memory for all four layers:
+// [pre_highway (x W_pre, no bias)], then per layer x = relu(H x + bH) sig(T x + bT) + x (1 - sig(T x + bT)).
+// x [B, Cin, T] channel-major -> y [B, 128, T].  Thread o < 256 computes row o of [H | T] for the tile's frames, summing
+// k in order; weights are transposed ([k][o]) so a warp reads consecutive words.
+struct HighwayArgs {
+    const float* x = nullptr; long long x_bs = 0; int Cin = 0, T = 0;
+    const float* pre = nullptr;                // [Cin][128] or null (Cin == 128)
+    const float* w = nullptr; const float* bias = nullptr;   // [NHW][128][256], [NHW][256]
+    float* y = nullptr; long long y_bs = 0;
+};
+
+__global__ void __launch_bounds__(256) highway_kernel(HighwayArgs a) {
+    extern __shared__ float sm[];
+    float* xs = sm;                      // [128][HW_TF]
+    float* hs = xs + HW * HW_TF;         // [256][HW_TF]
+    float* xin = hs + 2 * HW * HW_TF;    // [Cin][HW_TF] (pre_highway only)
+    const int b = blockIdx.y, t0 = blockIdx.x * HW_TF, tid = threadIdx.x;
+    const float* x = a.x + (size_t)b * a.x_bs;
+    float* dst = a.pre ? xin : xs;
+    for (int i = tid; i < a.Cin * HW_TF; i += blockDim.x) {
+        const int k = i / HW_TF, f = i - k * HW_TF, t = t0 + f;
+        dst[i] = t < a.T ? x[(size_t)k * a.T + t] : 0.f;
+    }
+    __syncthreads();
+    if (a.pre) {   // xs[j] = sum_k pre[k][j] xin[k]: thread (j, half) for 8 frames
+        const int j = tid & (HW - 1), f0 = (tid >> 7) * (HW_TF / 2);
+        float acc[HW_TF / 2];
+#pragma unroll
+        for (int f = 0; f < HW_TF / 2; ++f) acc[f] = 0.f;
+        for (int k = 0; k < a.Cin; ++k) {
+            const float wv = a.pre[(size_t)k * HW + j];
+            const float4* xv = reinterpret_cast<const float4*>(xin + k * HW_TF + f0);
+#pragma unroll
+            for (int v = 0; v < HW_TF / 8; ++v) {
+                const float4 q = xv[v];
+                acc[4 * v + 0] = fmaf(wv, q.x, acc[4 * v + 0]);
+                acc[4 * v + 1] = fmaf(wv, q.y, acc[4 * v + 1]);
+                acc[4 * v + 2] = fmaf(wv, q.z, acc[4 * v + 2]);
+                acc[4 * v + 3] = fmaf(wv, q.w, acc[4 * v + 3]);
+            }
+        }
+#pragma unroll
+        for (int f = 0; f < HW_TF / 2; ++f) xs[j * HW_TF + f0 + f] = acc[f];
+        __syncthreads();
+    }
+    for (int l = 0; l < NHW; ++l) {
+        const float* w = a.w + (size_t)l * HW * 2 * HW;
+        float acc[HW_TF];
+#pragma unroll
+        for (int f = 0; f < HW_TF; ++f) acc[f] = 0.f;
+        for (int k = 0; k < HW; ++k) {
+            const float wv = w[(size_t)k * 2 * HW + tid];
+            const float4* xv = reinterpret_cast<const float4*>(xs + k * HW_TF);
+#pragma unroll
+            for (int v = 0; v < HW_TF / 4; ++v) {
+                const float4 q = xv[v];
+                acc[4 * v + 0] = fmaf(wv, q.x, acc[4 * v + 0]);
+                acc[4 * v + 1] = fmaf(wv, q.y, acc[4 * v + 1]);
+                acc[4 * v + 2] = fmaf(wv, q.z, acc[4 * v + 2]);
+                acc[4 * v + 3] = fmaf(wv, q.w, acc[4 * v + 3]);
+            }
+        }
+        const float bo = a.bias[l * 2 * HW + tid];
+#pragma unroll
+        for (int f = 0; f < HW_TF; ++f) hs[tid * HW_TF + f] = acc[f] + bo;
+        __syncthreads();
+        for (int i = tid; i < HW * HW_TF; i += blockDim.x) {
+            const float h = fmaxf(hs[i], 0.f), g = sigm(hs[HW * HW_TF + i]);
+            xs[i] = h * g + xs[i] * (1.f - g);
+        }
+        __syncthreads();
+    }
+    float* y = a.y + (size_t)b * a.y_bs;
+    for (int i = tid; i < HW * HW_TF; i += blockDim.x) {
+        const int j = i / HW_TF, f = i - j * HW_TF, t = t0 + f;
+        if (t < a.T) y[(size_t)j * a.T + t] = xs[i];
+    }
+}
+
+// The step epilogue (Decoder.inference's loop body after decode, tacotron.py:470-482): for each running row b, the
+// first r frames of the projection -> dec_out[b, t*r .. t*r + r), the memory queue update (_update_memory_input) from
+// mem_in into mem_out, stop[b, t] = sigmoid(logit); with n = t + 1 steps taken, the row is done when n > len_b / 4 and
+// (sigmoid > 0.6 or its attention weight at token len_b - 1 > 0.6), or when n > max_decoder_steps (steps[b] = n);
+// then ctl = {running, t + 1}.
+struct Step1Args {
+    const float* proj = nullptr; int RC = 0; const float* logit = nullptr;
+    const float* alpha = nullptr; const long long* lens = nullptr; int Tt = 0;
+    int C = 0, r = 0, memory_size = 0, Cm = 0, max_decoder_steps = 0, S = 0;
+    const float* mem_in = nullptr; float* mem_out = nullptr;
+    float* dec_out = nullptr; float* stop = nullptr;
+    int* done = nullptr; int* ctl = nullptr; int B = 0;
+};
+
+__global__ void __launch_bounds__(256) taco1_step_kernel(Step1Args a) {
+    const int t = a.ctl[1], rc = a.r * a.C;
+    for (int i = threadIdx.x; i < a.B * rc; i += blockDim.x) {
+        const int b = i / rc, k = i - b * rc;
+        if (a.done[b]) continue;
+        a.dec_out[((size_t)b * a.S * a.r + (size_t)t * a.r) * a.C + k] = a.proj[(size_t)b * a.RC + k];
+    }
+    for (int i = threadIdx.x; i < a.B * a.Cm; i += blockDim.x) {
+        const int b = i / a.Cm, k = i - b * a.Cm;
+        if (a.done[b]) continue;
+        const float* pj = a.proj + (size_t)b * a.RC;
+        float v;
+        if (a.memory_size <= 0) v = pj[a.C * (a.r - 1) + k];                      // the last frame
+        else if (a.memory_size > a.r) v = k < rc ? pj[k] : a.mem_in[(size_t)b * a.Cm + k - rc];   // queue
+        else v = pj[k];                                                             // the first memory_size frames
+        a.mem_out[(size_t)b * a.Cm + k] = v;
+    }
+    __syncthreads();
+    for (int b = threadIdx.x; b < a.B; b += blockDim.x) {
+        if (a.done[b]) continue;
+        const float s = 1.f / (1.f + expf(-a.logit[b]));
+        a.stop[(size_t)b * a.S + t] = s;
+        const int n = t + 1, len = (int)a.lens[b];
+        const bool attn_end = a.alpha[(size_t)b * a.Tt + len - 1] > 0.6f;
+        if ((4 * n > len && (s > 0.6f || attn_end)) || n > a.max_decoder_steps) {
+            a.done[b] = 1;
+            a.ctl[2 + b] = n;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int b = 0; b < a.B; ++b) run += a.done[b] ? 0 : 1;
+        a.ctl[0] = run;
+        a.ctl[1] = t + 1;
+    }
+}
+
+// loop state at step 0: zero GRU states, context and go frame; alpha zero (original) or one-hot at token 0 (DCA)
+__global__ void taco1_reset_kernel(float* zero, size_t nzero, float* alpha, int Tt, int one_hot, int* done, int* ctl,
+                                   int B) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nzero; i += (size_t)gridDim.x * blockDim.x)
+        zero[i] = 0.f;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < B * Tt; i += gridDim.x * blockDim.x)
+        alpha[i] = (one_hot && i % Tt == 0) ? 1.f : 0.f;
+    if (blockIdx.x == 0)
+        for (int b = threadIdx.x; b < B; b += blockDim.x) {
+            done[b] = 0;
+            ctl[2 + b] = 0;
+            if (b == 0) { ctl[0] = B; ctl[1] = 0; }
+        }
+}
+
+// postnet input: x[b, c, t] = dec[b, t, c] below frames[b], else 0; mask[b, t] likewise
+__global__ void taco1_frames_in_kernel(const float* dec, int Fpitch, const int* frames, float* x, float* mask, int C,
+                                       int Tp) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, c = blockIdx.y, b = blockIdx.z;
+    if (t >= Tp) return;
+    const bool valid = t < frames[b];
+    x[((size_t)b * C + c) * Tp + t] = valid ? dec[((size_t)b * Fpitch + t) * C + c] : 0.f;
+    if (c == 0) mask[(size_t)b * Tp + t] = valid ? 1.f : 0.f;
+}
+
+// out[b, t, c] = y[b, c, t] for t < F
+__global__ void taco1_frames_out_kernel(const float* y, int Tp, float* out, int F, int C) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (i >= F * C) return;
+    const int t = i / C, c = i - t * C;
+    out[(size_t)b * F * C + i] = y[((size_t)b * C + c) * Tp + t];
+}
+
+// conv (no bias) -> BatchNorm (eval, eps 1e-3) folded into weight [Cout][Cin][K] and bias
+void fold_bn(const float* const* w, int Cout, int Cin, int K, std::vector<float>& wf, std::vector<float>& bf) {
+    wf.assign((size_t)Cout * Cin * K, 0.f);
+    bf.assign(Cout, 0.f);
+    for (int o = 0; o < Cout; ++o) {
+        const double s = (double)w[1][o] / sqrt((double)w[4][o] + 1e-3);
+        for (size_t k = 0; k < (size_t)Cin * K; ++k) wf[(size_t)o * Cin * K + k] = (float)(w[0][(size_t)o * Cin * K + k] * s);
+        bf[o] = (float)((double)w[2][o] - w[3][o] * s);
+    }
+}
+
+// the workspace that lives from encode to the end of the loop
+struct Persist {
+    float *pin, *alpha, *cum, *proj, *logit, *pb, *din, *x1, *x2;
+    float *mem, *q, *ctx, *dh1, *dh2;   // zeroed region: mem [2][B][Cm], q / dh1 / dh2 [2][B][256], ctx [B][256]
+    int *ctl, *done;
+    size_t nzero;
+};
+
+bool persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
+    const int RC = e.c.frame_channels * e.c.r_init;
+    p.pin = ar.f32((size_t)B * A * Tt);
+    p.ctl = (int*)ar.f32(2 + B);
+    p.done = (int*)ar.f32(B);
+    p.alpha = ar.f32((size_t)B * Tt);
+    p.cum = ar.f32((size_t)B * Tt);
+    p.proj = ar.f32((size_t)B * RC);
+    p.logit = ar.f32(B);
+    p.pb = ar.f32((size_t)B * (PN0 + PN1));
+    p.din = ar.f32((size_t)B * D);
+    p.x1 = ar.f32((size_t)B * D);
+    p.x2 = ar.f32((size_t)B * D);
+    p.nzero = (size_t)B * (2 * e.Cm + 2 * Q + E + 4 * D);
+    float* z = ar.f32(p.nzero);
+    if (!(p.pin && p.ctl && p.done && p.alpha && p.cum && p.proj && p.logit && p.pb && p.din && p.x1 && p.x2 && z))
+        return false;
+    p.mem = z;
+    p.q = p.mem + (size_t)2 * B * e.Cm;
+    p.ctx = p.q + (size_t)2 * B * Q;
+    p.dh1 = p.ctx + (size_t)B * E;
+    p.dh2 = p.dh1 + (size_t)2 * B * D;
+    return true;
+}
+
+// bytes an allocation sequence takes from an Arena (dry run over an unbounded one)
+template <class F> size_t arena_size(F&& f) {
+    Arena ar(nullptr, ~size_t(0) >> 1);
+    f(ar);
+    return ar.off;
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------ CBHG
+int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int* consumed) {
+    Cin = cin; K = k_max; P1 = p1;
+    B200_REQUIRE(Cin >= 1 && Cin <= HW_MAX_CIN && K >= 1, "tacotron: unsupported CBHG shape");
+    int rc, i = 0;
+    std::vector<float> wf, bf;
+    {   // the bank: conv k (taps [-(k-1)/2, k/2]) placed in the union window [-(K-1)/2, K/2] of K taps
+        const int padU = (K - 1) / 2;
+        std::vector<float> wb((size_t)K * BANK * Cin * K, 0.f), bb((size_t)K * BANK);
+        for (int k = 1; k <= K; ++k, i += 5) {
+            fold_bn(w + i, BANK, Cin, k, wf, bf);
+            const int off = padU - (k - 1) / 2;
+            for (int o = 0; o < BANK; ++o) {
+                const int row = (k - 1) * BANK + o;
+                bb[row] = bf[o];
+                for (int ci = 0; ci < Cin; ++ci)
+                    for (int j = 0; j < k; ++j)
+                        wb[((size_t)row * Cin + ci) * K + off + j] = wf[((size_t)o * Cin + ci) * k + j];
+            }
+        }
+        if ((rc = pack_conv(bank, wb.data(), bb.data(), K * BANK, Cin, K, 1, padU))) return rc;
+    }
+    fold_bn(w + i, P1, K * BANK, 3, wf, bf);
+    if ((rc = pack_conv(proj1, wf.data(), bf.data(), P1, K * BANK, 3, 1, 1))) return rc;
+    i += 5;
+    fold_bn(w + i, Cin, P1, 3, wf, bf);
+    if ((rc = pack_conv(proj2, wf.data(), bf.data(), Cin, P1, 3, 1, 1))) return rc;
+    i += 5;
+    if (Cin != HW) {   // pre_highway [128][Cin] -> [Cin][128]
+        std::vector<float> pt((size_t)Cin * HW);
+        for (int o = 0; o < HW; ++o)
+            for (int k = 0; k < Cin; ++k) pt[(size_t)k * HW + o] = w[i][(size_t)o * Cin + k];
+        if ((rc = upload(pre_w, pt.data(), pt.size()))) return rc;
+        ++i;
+    }
+    {   // highways: [H | T] rows transposed to [k][256]
+        std::vector<float> hw((size_t)NHW * HW * 2 * HW), hb((size_t)NHW * 2 * HW);
+        for (int l = 0; l < NHW; ++l, i += 4)
+            for (int o = 0; o < 2 * HW; ++o) {
+                const float* W = o < HW ? w[i] : w[i + 2];
+                const float* bsrc = o < HW ? w[i + 1] : w[i + 3];
+                const int oo = o % HW;
+                hb[(size_t)l * 2 * HW + o] = bsrc[oo];
+                for (int k = 0; k < HW; ++k) hw[((size_t)l * HW + k) * 2 * HW + o] = W[(size_t)oo * HW + k];
+            }
+        if ((rc = upload(hw_w, hw.data(), hw.size()))) return rc;
+        if ((rc = upload(hw_b, hb.data(), hb.size()))) return rc;
+    }
+    {   // GRU: both directions' input projections as one 1x1 conv (rows [fwd 3H | bwd 3H]), bias b_ih + (b_hr, b_hz, 0)
+        constexpr int H = GRU_H;
+        std::vector<float> wi((size_t)6 * H * HW), bi((size_t)6 * H), img((size_t)2 * 3 * 32 * BIGRU_THREADS), bn(2 * H);
+        for (int d = 0; d < 2; ++d) {
+            const float* const* p = w + i + 4 * d;
+            memcpy(wi.data() + (size_t)d * 3 * H * HW, p[0], sizeof(float) * 3 * H * HW);
+            for (int r = 0; r < 3 * H; ++r) bi[(size_t)d * 3 * H + r] = p[2][r] + (r < 2 * H ? p[3][r] : 0.f);
+            for (int j = 0; j < H; ++j) bn[d * H + j] = p[3][2 * H + j];
+            pack_bigru_whh(p[1], img.data() + (size_t)d * 3 * 32 * BIGRU_THREADS);
+        }
+        if ((rc = pack_conv(gru_in, wi.data(), bi.data(), 6 * H, HW, 1, 1, 0))) return rc;
+        if ((rc = upload(whh, img.data(), img.size()))) return rc;
+        if ((rc = upload(bhn, bn.data(), bn.size()))) return rc;
+        i += 8;
+    }
+    *consumed = i;
+    return 0;
+}
+
+static void cbhg_scratch(const Tacotron::Cbhg& c, Arena& ar, int B, int T, float** bank, float** y2, float** y3,
+                         float** hx, float** pre) {
+    *bank = ar.f32((size_t)B * c.K * BANK * T);
+    *y2 = ar.f32((size_t)B * c.P1 * T);
+    *y3 = ar.f32((size_t)B * c.Cin * T);
+    *hx = ar.f32((size_t)B * HW * T);
+    *pre = ar.f32((size_t)B * 6 * GRU_H * T);
+}
+
+size_t Tacotron::Cbhg::scratch_bytes(int B, int T) const {
+    return arena_size([&](Arena& ar) { float* p[5]; cbhg_scratch(*this, ar, B, T, p, p + 1, p + 2, p + 3, p + 4); });
+}
+
+int Tacotron::Cbhg::run(const float* x, const float* mask, const int* lens32, const long long* lens64, int B, int T,
+                        float* out, long long out_bs, int out_ts, int out_cs, Arena& ar, cudaStream_t st) const {
+    float *bk, *y2, *y3, *hx, *pre;
+    cbhg_scratch(*this, ar, B, T, &bk, &y2, &y3, &hx, &pre);
+    B200_REQUIRE(bk && y2 && y3 && hx && pre, "tacotron: arena exhausted");
+    int rc;
+    auto conv = [&](const ConvLayer& L, const float* in, int ci, float* o, int co, int act, const float* res) {
+        ConvIO io;
+        io.x = in; io.x_bs = (long long)ci * T; io.x_cs = T; io.Tin = T;
+        io.y = o; io.y_bs = (long long)co * T; io.y_cs = T; io.Tout = T; io.B = B;
+        io.act = act; io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+        if (res) { io.res = res; io.res_bs = (long long)co * T; io.res_cs = T; }
+        return launch_conv(L, io, st);
+    };
+    if ((rc = conv(bank, x, Cin, bk, K * BANK, ACT_RELU, nullptr))) return rc;
+    if ((rc = conv(proj1, bk, K * BANK, y2, P1, ACT_RELU, nullptr))) return rc;
+    if ((rc = conv(proj2, y2, P1, y3, Cin, ACT_NONE, x))) return rc;   // x += inputs
+    {
+        HighwayArgs a;
+        a.x = y3; a.x_bs = (long long)Cin * T; a.Cin = Cin; a.T = T; a.pre = pre_w; a.w = hw_w; a.bias = hw_b;
+        a.y = hx; a.y_bs = (long long)HW * T;
+        const size_t smem = sizeof(float) * HW_TF * (3 * HW + (Cin != HW ? Cin : 0));
+        static DeviceOnce once;
+        if ((rc = device_once(once, nullptr, [](int) -> int {
+                 B200_CUDA_OK(cudaFuncSetAttribute(highway_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)(sizeof(float) * HW_TF * (3 * HW + HW_MAX_CIN))));
+                 return 0;
+             })))
+            return rc;
+        highway_kernel<<<dim3((T + HW_TF - 1) / HW_TF, B), 256, smem, st>>>(a);
+        count_launch();
+        dispatch_note(DISPATCH_HIGHWAY);
+        B200_CUDA_OK(cudaGetLastError());
+    }
+    {
+        ConvIO io;
+        io.x = hx; io.x_bs = (long long)HW * T; io.x_cs = T; io.Tin = T;
+        io.y = pre; io.y_bs = (long long)6 * GRU_H * T; io.y_cs = T; io.Tout = T; io.B = B;
+        if ((rc = launch_conv(gru_in, io, st))) return rc;
+    }
+    BiGruArgs g;
+    g.pre = pre; g.pre_bs = (long long)6 * GRU_H * T; g.pre_cs = T; g.whh = whh; g.bhn = bhn;
+    g.out = out; g.out_bs = out_bs; g.out_ts = out_ts; g.out_cs = out_cs; g.lens32 = lens32; g.lens64 = lens64; g.T = T;
+    return launch_bigru(g, B, st);
+}
+
+// ------------------------------------------------------------------ the model
+int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, int nw) {
+    c = cfg;
+    const int C = c.frame_channels, RC = C * c.r_init;
+    B200_REQUIRE(c.n_vocab > 0 && C > 0 && C <= HW_MAX_CIN && c.out_channels > 0 && c.r_init >= 1 &&
+                 (c.attention_type == 0 || c.attention_type == 1), "tacotron: unsupported config");
+    Cm = c.memory_size > 0 ? C * c.memory_size : C;
+    const int cbhg_n_enc = 16 * 5 + 10 + 16 + 8, cbhg_n_post = 8 * 5 + 10 + (C != HW ? 1 : 0) + 16 + 8;
+    const int expect = 1 + 4 + cbhg_n_enc + 2 * (c.prenet_bn ? 6 : 2) + 4 +
+                       (c.attention_type == 1 ? 9 : 4 + (c.location_attn ? 2 : 0)) + 2 + 8 + 2 + 2 + cbhg_n_post + 2;
+    B200_REQUIRE(nw == expect, "tacotron: expected %d weight tensors, got %d", expect, nw);
+    int rc, i = 0, used = 0;
+    if ((rc = upload(emb, w[i++], (size_t)c.n_vocab * EMB))) return rc;
+    if ((rc = pack_conv(eprenet[0], w[i], w[i + 1], PN0, EMB, 1, 1, 0))) return rc;
+    if ((rc = pack_conv(eprenet[1], w[i + 2], w[i + 3], PN1, PN0, 1, 1, 0))) return rc;
+    i += 4;
+    if ((rc = ecbhg.init(PN1, 16, 128, w + i, &used))) return rc;
+    i += used;
+    for (int l = 0; l < 2; ++l) {   // decoder prenet (with bias); "bn": eval BatchNorm (eps 1e-5) folded into the layer
+        const int in = l ? PN0 : Cm, out = l ? PN1 : PN0;
+        if (!c.prenet_bn) {
+            if ((rc = upload(prenet_w[l], w[i], (size_t)out * in))) return rc;
+            if ((rc = upload(prenet_b[l], w[i + 1], out))) return rc;
+            i += 2;
+            continue;
+        }
+        std::vector<float> wf((size_t)out * in), bf(out);
+        for (int o = 0; o < out; ++o) {
+            const double s = (double)w[i + 2][o] / sqrt((double)w[i + 5][o] + 1e-5);
+            for (int k = 0; k < in; ++k) wf[(size_t)o * in + k] = (float)(w[i][(size_t)o * in + k] * s);
+            bf[o] = (float)(((double)w[i + 1][o] - w[i + 4][o]) * s + w[i + 3][o]);
+        }
+        if ((rc = upload(prenet_w[l], wf.data(), wf.size()))) return rc;
+        if ((rc = upload(prenet_b[l], bf.data(), bf.size()))) return rc;
+        i += 6;
+    }
+    // a GRUCell: W_ih, W_hh, bias [4][H] = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn)
+    auto gru = [&](DevBuf<float>& wih, DevBuf<float>& whh_, DevBuf<float>& bias, int in, int H) -> int {
+        int r;
+        if ((r = upload(wih, w[i], (size_t)3 * H * in))) return r;
+        if ((r = upload(whh_, w[i + 1], (size_t)3 * H * H))) return r;
+        std::vector<float> b((size_t)4 * H);
+        for (int k = 0; k < 2 * H; ++k) b[k] = w[i + 2][k] + w[i + 3][k];
+        for (int k = 0; k < H; ++k) { b[2 * H + k] = w[i + 2][2 * H + k]; b[3 * H + k] = w[i + 3][2 * H + k]; }
+        i += 4;
+        return upload(bias, b.data(), b.size());
+    };
+    if ((rc = gru(arnn_wih, arnn_whh, arnn_b, PN1 + E, Q))) return rc;
+    if (c.attention_type == 0) {
+        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
+        if ((rc = pack_conv(inproj, w[i++], nullptr, A, E, 1, 1, 0))) return rc;
+        if ((rc = upload(att_v, w[i++], A))) return rc;
+        att_vb = w[i++][0];
+        if (c.location_attn) {
+            if ((rc = upload(att_wc, w[i++], (size_t)32 * 2 * 31))) return rc;
+            if ((rc = upload(att_wd, w[i++], (size_t)A * 32))) return rc;
+        }
+    } else {
+        if ((rc = upload(att_prior, w[i++], 11))) return rc;
+        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
+        if ((rc = upload(att_bq, w[i++], A))) return rc;
+        if ((rc = upload(att_wk, w[i++], (size_t)8 * 21 * A))) return rc;
+        if ((rc = upload(att_ws, w[i++], (size_t)8 * 21))) return rc;
+        if ((rc = upload(att_wsl, w[i++], (size_t)A * 8))) return rc;
+        if ((rc = upload(att_wdl, w[i++], (size_t)A * 8))) return rc;
+        if ((rc = upload(att_bdl, w[i++], A))) return rc;
+        if ((rc = upload(att_v, w[i++], A))) return rc;
+    }
+    if ((rc = upload(pdi_w, w[i], (size_t)D * (Q + E)))) return rc;
+    if ((rc = upload(pdi_b, w[i + 1], D))) return rc;
+    i += 2;
+    for (int l = 0; l < 2; ++l)
+        if ((rc = gru(drnn_wih[l], drnn_whh[l], drnn_b[l], D, D))) return rc;
+    if ((rc = upload(proj_w, w[i], (size_t)RC * D))) return rc;
+    if ((rc = upload(proj_b, w[i + 1], RC))) return rc;
+    if ((rc = upload(stop_w, w[i + 2], (size_t)D + RC))) return rc;
+    if ((rc = upload(stop_b, w[i + 3], 1))) return rc;
+    i += 4;
+    if ((rc = pcbhg.init(C, 8, 256, w + i, &used))) return rc;
+    i += used;
+    if ((rc = pack_conv(last, w[i], w[i + 1], c.out_channels, 2 * GRU_H, 1, 1, 0))) return rc;
+    return 0;
+}
+
+static void encode_scratch(Arena& ar, int B, int Tt, float** x0, float** mask, float** x1, float** xin, float** encT) {
+    *x0 = ar.f32((size_t)B * EMB * Tt);
+    *mask = ar.f32((size_t)B * Tt);
+    *x1 = ar.f32((size_t)B * PN0 * Tt);
+    *xin = ar.f32((size_t)B * PN1 * Tt);
+    *encT = ar.f32((size_t)B * E * Tt);
+}
+
+static void postnet_scratch(const Tacotron& e, Arena& ar, int B, int Tp, float** x, float** mask, float** g, float** y) {
+    *x = ar.f32((size_t)B * e.c.frame_channels * Tp);
+    *mask = ar.f32((size_t)B * Tp);
+    *g = ar.f32((size_t)B * 2 * GRU_H * Tp);
+    *y = ar.f32((size_t)B * e.c.out_channels * Tp);
+}
+
+size_t Tacotron::workspace_bytes(int B, int Tt, int F) const {
+    const size_t encb = arena_size([&](Arena& ar) {
+        Persist p;
+        persist_layout(*this, ar, B, Tt, p);
+        float* q[5];
+        encode_scratch(ar, B, Tt, q, q + 1, q + 2, q + 3, q + 4);
+    }) + ecbhg.scratch_bytes(B, Tt);
+    const int Tp = (F + 3) / 4 * 4;
+    const size_t postb = arena_size([&](Arena& ar) {
+        float* q[4];
+        postnet_scratch(*this, ar, B, Tp, q, q + 1, q + 2, q + 3);
+    }) + pcbhg.scratch_bytes(B, Tp);
+    return std::max(encb, postb) + 1024;
+}
+
+int Tacotron::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
+                     size_t ws_bytes, cudaStream_t st) const {
+    B200_REQUIRE(tokens && lengths && enc_out && ws, "tacotron_encode: null pointer");
+    B200_REQUIRE(B >= 1 && Tt >= 1, "tacotron_encode: empty batch");
+    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron_encode: workspace too small");
+    Arena ar(ws, ws_bytes);
+    Persist p;
+    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron_encode: arena exhausted");
+    float *x0, *mask, *x1, *xin, *encT;
+    encode_scratch(ar, B, Tt, &x0, &mask, &x1, &xin, &encT);
+    B200_REQUIRE(x0 && mask && x1 && xin && encT, "tacotron_encode: arena exhausted");
+    int rc;
+    // emb(x), zero past each row's length (the reference runs each row at its own length)
+    if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, EMB, EMB, x0, mask, st, false))) return rc;
+    const float* in = x0;
+    for (int l = 0; l < 2; ++l) {   // encoder prenet: Linear -> ReLU (eval: no dropout), masked
+        const int ci = l ? PN0 : EMB, co = l ? PN1 : PN0;
+        float* o = l ? xin : x1;
+        ConvIO io;
+        io.x = in; io.x_bs = (long long)ci * Tt; io.x_cs = Tt; io.Tin = Tt;
+        io.y = o; io.y_bs = (long long)co * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
+        io.act = ACT_RELU; io.ymask = mask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
+        if ((rc = launch_conv(eprenet[l], io, st))) return rc;
+        in = o;
+    }
+    if ((rc = ecbhg.run(xin, mask, nullptr, lengths, B, Tt, enc_out, (long long)Tt * E, E, 1, ar, st))) return rc;
+    if (c.attention_type == 0) {   // inputs_layer, step-invariant: pin [B, A, Tt]
+        if ((rc = launch_transpose(enc_out, encT, B, Tt, E, st))) return rc;
+        ConvIO io;
+        io.x = encT; io.x_bs = (long long)E * Tt; io.x_cs = Tt; io.Tin = Tt;
+        io.y = p.pin; io.y_bs = (long long)A * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
+        if ((rc = launch_conv(inproj, io, st))) return rc;
+    }
+    return 0;
+}
+
+int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
+                          const unsigned char* drop, int chunk_steps, float* dec_out, float* stop_tokens,
+                          float* alignments, int* steps, void* ws, size_t ws_bytes, cudaStream_t st) const {
+    B200_REQUIRE(lengths && enc_out && dec_out && stop_tokens && alignments && steps && ws,
+                 "tacotron_decode_loop: null pointer");
+    B200_REQUIRE(B >= 1 && Tt >= 1 && max_steps >= 1, "tacotron_decode_loop: B, Tt and max_steps must be >= 1");
+    B200_REQUIRE(r >= 1 && r <= c.r_init, "tacotron_decode_loop: r must be in [1, r_init = %d]", c.r_init);
+    B200_REQUIRE(chunk_steps >= 2 && chunk_steps % 2 == 0, "tacotron_decode_loop: chunk_steps must be even and >= 2");
+    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron_decode_loop: workspace too small");
+    const int C = c.frame_channels, RC = C * c.r_init, S = max_steps + 1;   // a row emits at most max_steps + 1 steps
+    Arena ar(ws, ws_bytes);
+    Persist p;
+    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron_decode_loop: arena exhausted");
+    B200_CUDA_OK(cudaMemsetAsync(dec_out, 0, sizeof(float) * (size_t)B * S * r * C, st));
+    B200_CUDA_OK(cudaMemsetAsync(stop_tokens, 0, sizeof(float) * (size_t)B * S, st));
+    B200_CUDA_OK(cudaMemsetAsync(alignments, 0, sizeof(float) * (size_t)B * S * Tt, st));
+    B200_CUDA_OK(cudaMemsetAsync(p.cum, 0, sizeof(float) * (size_t)B * Tt, st));
+    taco1_reset_kernel<<<64, 256, 0, st>>>(p.mem, p.nzero, p.alpha, Tt, c.attention_type == 1, p.done, p.ctl, B);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    int rc;
+    size_t attn_smem = 0;
+    if ((rc = taco_attn_prepare(Q, E, Tt, &attn_smem))) return rc;
+    const int nb = B > 8 ? 32 : 8;
+    // one step; parity = step index within the chunk (memory, query and both decoder h are double-buffered)
+    auto step = [&](cudaStream_t cs, int par, bool note) -> int {
+        int rc;
+        const float* mem_in = p.mem + (size_t)par * B * Cm;
+        float* mem_out = p.mem + (size_t)(par ^ 1) * B * Cm;
+        float* pb0 = p.pb;
+        float* pb1 = p.pb + (size_t)B * PN0;
+        for (int l = 0; l < 2; ++l) {   // prenet: Linear -> ReLU -> dropout; drop is [B, S, 2, 256], layer 1 uses 128
+            LinArgs a;
+            a.W = prenet_w[l]; a.bias = prenet_b[l]; a.K = l ? PN0 : Cm; a.R = l ? PN1 : PN0;
+            a.x = l ? pb0 : mem_in; a.x_bs = a.K; a.y = l ? pb1 : pb0; a.y_bs = a.R; a.relu = 1;
+            a.drop = c.prenet_dropout ? drop : nullptr; a.drop_layer = l ? 2 : 0; a.drop_L = l ? 4 : 2; a.drop_F = S;
+            a.ctl = p.ctl; a.done = p.done; a.B = B;
+            if ((rc = launch_linear(a, cs, note))) return rc;
+        }
+        float* q_in = p.q + (size_t)par * B * Q;
+        float* q_out = p.q + (size_t)(par ^ 1) * B * Q;
+        {   // attention RNN on [prenet | context], h
+            GruArgs a;
+            a.seg[0] = {arnn_wih, PN1 + E, 0, pb1, PN1, 0, PN1};
+            a.seg[1] = {arnn_wih + PN1, PN1 + E, 0, p.ctx, E, 0, E};
+            a.seg[2] = {arnn_whh, Q, 0, q_in, Q, 0, Q};
+            a.nseg = 3; a.nin = 2;
+            a.H = Q; a.bias = arnn_b; a.h_in = q_in; a.hin_bs = Q; a.h_out = q_out; a.h_bs = Q; a.done = p.done; a.B = B;
+            if ((rc = launch_gru(a, nb, cs, note))) return rc;
+        }
+        {
+            AttnArgs a;
+            a.q = q_out; a.enc = enc_out; a.pin = p.pin; a.alpha = p.alpha;
+            a.cum = (c.attention_type == 0 && c.location_attn) ? p.cum : nullptr;
+            a.ctx = p.ctx; a.align = alignments; a.max_steps = S; a.lens = lengths; a.done = p.done;
+            a.ctl = p.ctl; a.Tt = Tt; a.type = c.attention_type; a.location = c.location_attn;
+            a.softmax = c.attention_norm; a.Wq = att_wq; a.bq = att_bq; a.v = att_v; a.vb = att_vb; a.Wc = att_wc;
+            a.Wd = att_wd; a.Wk = att_wk; a.Ws = att_ws; a.Wsl = att_wsl; a.Wdl = att_wdl; a.bdl = att_bdl;
+            a.prior = att_prior;
+            if ((rc = launch_taco_attn(a, Q, E, B, attn_smem, cs, note))) return rc;
+        }
+        {   // project_to_decoder_in([query | context])
+            LinArgs a;
+            a.W = pdi_w; a.bias = pdi_b; a.K = Q; a.R = D; a.x = q_out; a.x_bs = Q; a.x2 = p.ctx; a.x2_bs = E; a.K2 = E;
+            a.y = p.din; a.y_bs = D; a.done = p.done; a.B = B;
+            if ((rc = launch_linear(a, cs, note))) return rc;
+        }
+        const float* xin = p.din;
+        float* xo[2] = {p.x1, p.x2};
+        float* dh[2] = {p.dh1, p.dh2};
+        for (int l = 0; l < 2; ++l) {   // decoder RNN l, then the residual x = h + x
+            GruArgs a;
+            a.seg[0] = {drnn_wih[l], D, 0, xin, D, 0, D};
+            a.seg[1] = {drnn_whh[l], D, 0, dh[l] + (size_t)par * B * D, D, 0, D};
+            a.nseg = 2; a.nin = 1;
+            a.H = D; a.bias = drnn_b[l]; a.h_in = a.seg[1].x; a.hin_bs = D;
+            a.h_out = dh[l] + (size_t)(par ^ 1) * B * D; a.h_bs = D;
+            a.res = xin; a.res_bs = D; a.x_out = xo[l]; a.xo_bs = D; a.done = p.done; a.B = B;
+            if ((rc = launch_gru(a, nb, cs, note))) return rc;
+            xin = xo[l];
+        }
+        {   // proj_to_mel, all C * r_init rows
+            LinArgs a;
+            a.W = proj_w; a.bias = proj_b; a.K = D; a.R = RC; a.x = p.x2; a.x_bs = D; a.y = p.proj; a.y_bs = RC;
+            a.done = p.done; a.B = B;
+            if ((rc = launch_linear(a, cs, note))) return rc;
+        }
+        {   // stopnet([decoder output | full projection])
+            LinArgs a;
+            a.W = stop_w; a.bias = stop_b; a.K = D; a.R = 1; a.x = p.x2; a.x_bs = D; a.x2 = p.proj; a.x2_bs = RC;
+            a.K2 = RC; a.y = p.logit; a.y_bs = 1; a.done = p.done; a.B = B;
+            if ((rc = launch_linear(a, cs, note))) return rc;
+        }
+        Step1Args s;
+        s.proj = p.proj; s.RC = RC; s.logit = p.logit; s.alpha = p.alpha; s.lens = lengths; s.Tt = Tt;
+        s.C = C; s.r = r; s.memory_size = c.memory_size; s.Cm = Cm; s.max_decoder_steps = max_steps; s.S = S;
+        s.mem_in = mem_in; s.mem_out = mem_out; s.dec_out = dec_out; s.stop = stop_tokens;
+        s.done = p.done; s.ctl = p.ctl; s.B = B;
+        taco1_step_kernel<<<1, 256, 0, cs>>>(s);
+        if (note) dispatch_note(DISPATCH_TACO1_STEP);
+        B200_CUDA_OK(cudaGetLastError());
+        return 0;
+    };
+    std::vector<int> host;
+    if ((rc = run_step_graph("tacotron_decode_loop", chunk_steps, S, 10, step, p.ctl, B, host, st))) return rc;
+    for (int b = 0; b < B; ++b) steps[b] = host[2 + b];
+    return 0;
+}
+
+int Tacotron::postnet(const float* dec_out, const int* frames, int B, int F, int Fpitch, float* out, void* ws,
+                      size_t ws_bytes, cudaStream_t st) const {
+    B200_REQUIRE(dec_out && frames && out && ws, "tacotron_postnet: null pointer");
+    B200_REQUIRE(B >= 1 && F >= 1 && F <= Fpitch, "tacotron_postnet: need B >= 1 and 1 <= F <= Fpitch");
+    B200_REQUIRE(ws_bytes >= workspace_bytes(B, 1, F), "tacotron_postnet: workspace too small");
+    const int C = c.frame_channels, O = c.out_channels, Tp = (F + 3) / 4 * 4;
+    Arena ar(ws, ws_bytes);
+    float *x, *mask, *g, *y;
+    postnet_scratch(*this, ar, B, Tp, &x, &mask, &g, &y);
+    B200_REQUIRE(x && mask && g && y, "tacotron_postnet: arena exhausted");
+    taco1_frames_in_kernel<<<dim3((Tp + 127) / 128, C, B), 128, 0, st>>>(dec_out, Fpitch, frames, x, mask, C, Tp);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    int rc;
+    // the biGRU writes channel-major [B, 256, Tp] for last_linear on the conv engine
+    if ((rc = pcbhg.run(x, mask, frames, nullptr, B, Tp, g, (long long)2 * GRU_H * Tp, 1, Tp, ar, st))) return rc;
+    {
+        ConvIO io;
+        io.x = g; io.x_bs = (long long)2 * GRU_H * Tp; io.x_cs = Tp; io.Tin = Tp;
+        io.y = y; io.y_bs = (long long)O * Tp; io.y_cs = Tp; io.Tout = Tp; io.B = B;
+        io.ymask = mask; io.ymask_bs = Tp; io.flags = EPI_MASK_POST;
+        if ((rc = launch_conv(last, io, st))) return rc;
+    }
+    taco1_frames_out_kernel<<<dim3((F * O + 255) / 256, B), 256, 0, st>>>(y, Tp, out, F, O);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+}  // namespace b200tts

@@ -37,24 +37,10 @@ __device__ __forceinline__ float warp_sum1(float v) {
     return v;
 }
 
-struct AttnArgs {
-    const float* q = nullptr;                 // [B, Q] attention-RNN output
-    const float* enc = nullptr;               // [B, Tt, E] encoder outputs
-    const float* pin = nullptr;               // [B, A, Tt] inputs_layer(encoder outputs)
-    float* alpha = nullptr; float* cum = nullptr;   // [B, Tt] previous / cumulative weights
-    float* ctx = nullptr;                     // [B, E]
-    float* align = nullptr; int max_steps = 0;      // [B, max_steps, Tt]
-    const long long* lens = nullptr; const int* done = nullptr; const int* ctl = nullptr;
-    int Tt = 0, type = 0, location = 0, softmax = 0;
-    // original: Wq [A][Q], v [A], vb; location: Wc [F][2][K], Wd [A][F]
-    // DCA: Wq [A][Q], bq [A], Wk [F*K][A], Ws [F][K], Wsl [A][F], Wdl [A][F], bdl [A], v [A], prior [11]
-    const float *Wq = nullptr, *bq = nullptr, *v = nullptr, *Wc = nullptr, *Wd = nullptr;
-    const float *Wk = nullptr, *Ws = nullptr, *Wsl = nullptr, *Wdl = nullptr, *bdl = nullptr, *prior = nullptr;
-    float vb = 0.f;
-};
-
 // One attention step for row b = blockIdx.x over its len_b tokens (OriginalAttention.forward with mask None /
-// MonotonicDynamicConvolutionAttention.forward), then the context and the alignment row of step ctl[1].
+// MonotonicDynamicConvolutionAttention.forward), then the context and the alignment row of step ctl[1].  Q / E: the
+// query and encoder widths.
+template <int Q, int E>
 __global__ void __launch_bounds__(256) taco_attn_kernel(AttnArgs a) {
     extern __shared__ float sm[];
     const int b = blockIdx.x;
@@ -273,7 +259,34 @@ struct Persist {   // the part of the workspace that lives from encode to the en
     int *ctl, *done;
 };
 
+size_t attn_smem_bytes(int Qd, int Tt) {
+    return sizeof(float) * (Qd + 2 * A + DCA_F * DCA_K + 32 + 3 * (size_t)Tt + 4 * PADL + LOC_F * A + LOC_F * 2 * LOC_K);
+}
+
 }  // namespace
+
+int taco_attn_prepare(int Qd, int Ed, int Tt, size_t* smem) {
+    B200_REQUIRE((Qd == 1024 && Ed == 512) || (Qd == 256 && Ed == 256), "taco_attn: no kernel for Q %d / E %d", Qd, Ed);
+    const size_t n = attn_smem_bytes(Qd, Tt);
+    B200_REQUIRE(n <= 200 * 1024, "taco_attn: %d tokens exceed the attention kernel's shared memory", Tt);
+    if (n > 48 * 1024) {
+        if (Qd == 1024)
+            B200_CUDA_OK(cudaFuncSetAttribute(taco_attn_kernel<1024, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
+        else
+            B200_CUDA_OK(cudaFuncSetAttribute(taco_attn_kernel<256, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)n));
+    }
+    *smem = n;
+    return 0;
+}
+
+int launch_taco_attn(const AttnArgs& a, int Qd, int Ed, int B, size_t smem, cudaStream_t st, bool note) {
+    if (Qd == 1024 && Ed == 512) taco_attn_kernel<1024, 512><<<B, 256, smem, st>>>(a);
+    else if (Qd == 256 && Ed == 256) taco_attn_kernel<256, 256><<<B, 256, smem, st>>>(a);
+    else { set_error("taco_attn: no kernel for Q %d / E %d", Qd, Ed); return 1; }
+    if (note) dispatch_note(DISPATCH_TACO_ATTN);
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
 
 static bool persist_layout(const Tacotron2& e, Arena& ar, int B, int Tt, Persist& p) {
     const int C = e.c.out_channels;
@@ -428,17 +441,15 @@ int Tacotron2::decode_loop(const long long* lengths, const float* enc_out, int B
     B200_CUDA_OK(cudaMemsetAsync(stop_tokens, 0, sizeof(float) * (size_t)B * max_steps, st));
     B200_CUDA_OK(cudaMemsetAsync(alignments, 0, sizeof(float) * (size_t)B * max_steps * Tt, st));
     B200_CUDA_OK(cudaMemsetAsync(p.cum, 0, sizeof(float) * (size_t)B * Tt, st));
+    int rc;
     taco_reset_kernel<<<64, 256, 0, st>>>(p.mem, (size_t)B * (C + 2 * Q + Q + E + 2 * D + D), p.alpha, Tt,
                                           c.attention_type == 1, p.done, p.ctl, B);
     count_launch();
     B200_CUDA_OK(cudaGetLastError());
     const int nb = B > 8 ? 32 : 8;
     const int lstm_id = nb == 32 ? DISPATCH_LSTM_CELL32 : DISPATCH_LSTM_CELL;
-    const size_t attn_smem =
-        sizeof(float) * (Q + 2 * A + DCA_F * DCA_K + 32 + 3 * (size_t)Tt + 4 * PADL + LOC_F * A + LOC_F * 2 * LOC_K);
-    B200_REQUIRE(attn_smem <= 200 * 1024, "tacotron2_decode_loop: %d tokens exceed the attention kernel's shared memory", Tt);
-    if (attn_smem > 48 * 1024)
-        B200_CUDA_OK(cudaFuncSetAttribute(taco_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_smem));
+    size_t attn_smem = 0;
+    if ((rc = taco_attn_prepare(Q, E, Tt, &attn_smem))) return rc;
     // one step; parity = step index within the chunk (query and decoder h are double-buffered)
     auto step = [&](cudaStream_t cs, int par, bool note) -> int {
         int rc;
@@ -472,9 +483,7 @@ int Tacotron2::decode_loop(const long long* lengths, const float* enc_out, int B
             a.softmax = c.attention_norm; a.Wq = att_wq; a.bq = att_bq; a.v = att_v; a.vb = att_vb; a.Wc = att_wc;
             a.Wd = att_wd; a.Wk = att_wk; a.Ws = att_ws; a.Wsl = att_wsl; a.Wdl = att_wdl; a.bdl = att_bdl;
             a.prior = att_prior;
-            taco_attn_kernel<<<B, 256, attn_smem, cs>>>(a);
-            if (note) dispatch_note(DISPATCH_TACO_ATTN);
-            B200_CUDA_OK(cudaGetLastError());
+            if ((rc = launch_taco_attn(a, Q, E, B, attn_smem, cs, note))) return rc;
         }
         float* dh_in = p.dh + (size_t)par * B * D;
         float* dh_out = p.dh + (size_t)(par ^ 1) * B * D;
@@ -508,7 +517,6 @@ int Tacotron2::decode_loop(const long long* lengths, const float* enc_out, int B
         return 0;
     };
     std::vector<int> host;
-    int rc;
     if ((rc = run_step_graph("tacotron2_decode_loop", chunk_steps, max_steps, 8, step, p.ctl, B, host, st))) return rc;
     for (int b = 0; b < B; ++b) steps[b] = host[2 + b];
     return 0;

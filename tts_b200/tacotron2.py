@@ -25,7 +25,7 @@ Differences from the reference, on purpose:
 
 Out of scope (construction raises ``NotImplementedError``): graves attention, attention windowing, forward attention
 and the transition agent, GST and Capacitron, speaker embeddings and d-vectors, the bidirectional decoder, encoder /
-decoder widths other than 512, the Tacotron (1) model, and training (``forward``).
+decoder widths other than 512, the Tacotron (1) model (``tts_b200.tacotron.Tacotron``), and training (``forward``).
 """
 import ctypes
 from dataclasses import dataclass
@@ -117,13 +117,13 @@ class _LinearBN(nn.Module):
 
 
 class _Prenet(nn.Module):
-    """Parameters of common_layers.py:63-119 (bias=False, as the decoder builds it)."""
+    """Parameters of common_layers.py:63-119 (bias=False, as the Tacotron2 decoder builds it; Tacotron's with bias)."""
 
-    def __init__(self, in_features, prenet_type, out_features):
+    def __init__(self, in_features, prenet_type, out_features, bias=False):
         super().__init__()
         ins = [in_features] + out_features[:-1]
         layer = _LinearBN if prenet_type == "bn" else _Linear
-        self.linear_layers = nn.ModuleList([layer(i, o, bias=False) for i, o in zip(ins, out_features)])
+        self.linear_layers = nn.ModuleList([layer(i, o, bias=bias) for i, o in zip(ins, out_features)])
 
 
 class _LocationLayer(nn.Module):
@@ -221,7 +221,7 @@ def _check_config(cfg):
         raise NotImplementedError(f"tts_b200: Tacotron2 with {what} is not built")
 
     if getattr(cfg, "model", "tacotron2") != "tacotron2":
-        no(f"model {cfg.model!r} (only Tacotron2; the Tacotron 1 model is out of scope)")
+        no(f"model {cfg.model!r} (only Tacotron2; the Tacotron 1 model is tts_b200.tacotron.Tacotron)")
     if cfg.attention_type not in ("original", "dynamic_convolution"):
         no(f"attention_type {cfg.attention_type!r}")
     if cfg.attention_win or cfg.windowing:
