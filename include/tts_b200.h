@@ -424,6 +424,36 @@ int b200tts_stft_magnitude(const b200tts_stft* h, const float* wav, int B, int T
 int b200tts_stft_mel_project(const b200tts_stft* h, const float* spec, int B, int n_frames, float log_clamp,
                              float* mel, void* stream);
 
+/* ---- Griffin-Lim: spectrogram -> waveform ---------------------------------------------------------
+ * Replaces AudioProcessor.inv_spectrogram / inv_melspectrogram, TTS/utils/audio/processor.py:444-458, with
+ * numpy_transforms.griffin_lim (:220-230; librosa stft / istft, center=True, reflect padding) and the inverse
+ * preemphasis (scipy.signal.lfilter([1], [1, -preemphasis])), batched; the reference runs one row at a time on the host.
+ * create: window [n_fft] (host; the periodic analysis window already centred and zero-padded to n_fft), n_fft a power
+ *   of two in [32, 8192], 1 <= hop_length <= n_fft.  pinv (host, [n_fft/2+1, n_mels], np.linalg.pinv(mel_basis)) makes
+ *   a mel handle (C == n_mels); NULL makes a linear one (C == n_fft/2+1).
+ * forward: x is addressed as x[b*x_batch_stride + c*x_channel_stride + t*x_time_stride] ([B,C,T] or [B,T,C]);
+ *   lengths (DEVICE int32 [B], each in [2, T]; NULL: all T) are the rows' frame counts.  Per row:
+ *     S = denormalize(x) (norm; scaler_mean / scaler_scale as for b200tts_vocoder_input)
+ *     S = base ** (S / spec_gain)            (base 10 or e; base 0: x is already a magnitude, norm must be identity)
+ *     S = max(1e-10, pinv @ S)               (mel handles)
+ *     S = |S| ** power
+ *     y = istft(S exp(2 pi i angles)), then num_iter times y = istft(S exp(i angle(stft(y))))
+ *     wav = lfilter([1], [1, -preemphasis], y)   (preemphasis 0: wav = y)
+ *   angles: DEVICE [B, n_fft/2+1, T] draws in [0, 1).  wav: [B, wav_pitch] with wav_pitch >= hop_length * (T - 1); row
+ *   b holds wav_lengths[b] = hop_length * (lengths[b] - 1) samples and zeros after them, or, when the first istft of
+ *   the row is not finite everywhere, the reference's single 0.0 sample (wav_lengths[b] = 1).  No host synchronisation.
+ */
+typedef struct b200tts_griffin_lim b200tts_griffin_lim;
+int b200tts_griffin_lim_create(int n_fft, int hop_length, const float* window, const float* pinv, int n_mels,
+                               b200tts_griffin_lim** out);
+void b200tts_griffin_lim_destroy(b200tts_griffin_lim* h);
+size_t b200tts_griffin_lim_workspace_bytes(const b200tts_griffin_lim* h, int B, int T);
+int b200tts_griffin_lim_forward(const b200tts_griffin_lim* h, const float* x, long long x_batch_stride,
+                                int x_channel_stride, int x_time_stride, int B, int C, int T, const int32_t* lengths,
+                                const b200tts_audio_norm* norm, float base, float spec_gain, float power, int num_iter,
+                                float preemphasis, const float* angles, float* wav, long long wav_pitch,
+                                int32_t* wav_lengths, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- H/ASP ResNet speaker encoder (d-vectors) --------------------------------------------------
  * Replaces ResNetSpeakerEncoder.forward, TTS/encoder/models/resnet.py:153-198, with the front end of
  * BaseEncoder.get_torch_mel_spectrogram_class, TTS/encoder/models/base_encoder.py:12-61 (PreEmphasis, then

@@ -125,7 +125,7 @@ DISPATCH_NAMES = {0: "fma", 3: "tc3", 5: "tc3_grouped", 6: "row1", 8: "tc16", 9:
                   16: "fma_wg", 17: "fma_wg_near", 18: "lstm_bi", 19: "lstm_cell", 20: "hmm_linear", 21: "hmm_step",
                   22: "pwgan_tc", 23: "pwgan_aux", 24: "taco_attn", 25: "taco_step", 26: "lstm_cell32",
                   27: "univnet_predict", 28: "univnet_lvc", 29: "gru_cell", 30: "gru_cell32", 31: "bigru",
-                  32: "highway", 33: "taco1_step"}
+                  32: "highway", 33: "taco1_step", 34: "gl_prepare", 35: "gl_iter", 36: "gl_deemphasis"}
 
 # tensor-core operand precision (B200TTS_PRECISION_* in include/tts_b200.h)
 PRECISIONS = {"fp32": 0, "bf16": 1, "fp16": 2, "tf32x3": 3, "f16x3": 4}
@@ -319,6 +319,16 @@ def _declare(lib):
     lib.b200tts_stft_magnitude.argtypes = [vp, vp, ci, ci, ci, ci, ci, cf, vp, ci, vp]
     lib.b200tts_stft_mel_project.restype = ci
     lib.b200tts_stft_mel_project.argtypes = [vp, vp, ci, ci, cf, vp, vp]
+    lib.b200tts_griffin_lim_create.restype = ci
+    lib.b200tts_griffin_lim_create.argtypes = [ci, ci, vp, vp, ci, ctypes.POINTER(vp)]
+    lib.b200tts_griffin_lim_destroy.restype = None
+    lib.b200tts_griffin_lim_destroy.argtypes = [vp]
+    lib.b200tts_griffin_lim_workspace_bytes.restype = sz
+    lib.b200tts_griffin_lim_workspace_bytes.argtypes = [vp, ci, ci]
+    lib.b200tts_griffin_lim_forward.restype = ci
+    lib.b200tts_griffin_lim_forward.argtypes = [vp, vp, ctypes.c_longlong, ci, ci, ci, ci, ci, vp,
+                                                ctypes.POINTER(AudioNormC), cf, cf, cf, ci, cf, vp, vp,
+                                                ctypes.c_longlong, vp, vp, sz, vp]
     lib.b200tts_flow_create_forward.restype = ci
     lib.b200tts_flow_create_forward.argtypes = [ctypes.POINTER(FlowConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
     lib.b200tts_posterior_forward.restype = ci

@@ -23,6 +23,7 @@ struct b200tts_tacotron2 { Tacotron2 impl; };
 struct b200tts_tacotron { Tacotron impl; };
 struct b200tts_pwgan { Pwgan impl; };
 struct b200tts_univnet { Univnet impl; };
+struct b200tts_griffin_lim { GriffinLim impl; };
 
 // A handle owns its device buffers through DevBuf members: copying one would free them twice, so it must not compile.
 static_assert(!std::is_copy_constructible_v<ConvLayer>);
@@ -43,6 +44,7 @@ static_assert(!std::is_copy_constructible_v<Tacotron2>);
 static_assert(!std::is_copy_constructible_v<Tacotron>);
 static_assert(!std::is_copy_constructible_v<Pwgan>);
 static_assert(!std::is_copy_constructible_v<Univnet>);
+static_assert(!std::is_copy_constructible_v<GriffinLim>);
 
 extern "C" {
 
@@ -364,6 +366,32 @@ int b200tts_stft_mel_project(const b200tts_stft* h, const float* spec, int B, in
                              float* mel, void* stream) {
     if (!h) { set_error("stft_mel_project: null handle"); return 1; }
     return h->impl.mel_project(spec, B, n_frames, log_clamp, mel, (cudaStream_t)stream);
+}
+
+int b200tts_griffin_lim_create(int n_fft, int hop_length, const float* window, const float* pinv, int n_mels,
+                               b200tts_griffin_lim** out) {
+    if (!out) { set_error("griffin_lim_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_griffin_lim* h = new (std::nothrow) b200tts_griffin_lim();
+    if (!h) { set_error("griffin_lim_create: out of host memory"); return 1; }
+    int rc = h->impl.init(n_fft, hop_length, window, pinv, n_mels);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+void b200tts_griffin_lim_destroy(b200tts_griffin_lim* h) { delete h; }
+size_t b200tts_griffin_lim_workspace_bytes(const b200tts_griffin_lim* h, int B, int T) {
+    return h ? h->impl.workspace_bytes(B, T) : 0;
+}
+int b200tts_griffin_lim_forward(const b200tts_griffin_lim* h, const float* x, long long x_batch_stride,
+                                int x_channel_stride, int x_time_stride, int B, int C, int T, const int32_t* lengths,
+                                const b200tts_audio_norm* norm, float base, float spec_gain, float power, int num_iter,
+                                float preemphasis, const float* angles, float* wav, long long wav_pitch,
+                                int32_t* wav_lengths, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!h || !norm) { set_error("griffin_lim_forward: null handle / norm"); return 1; }
+    return h->impl.forward(x, x_batch_stride, x_channel_stride, x_time_stride, B, C, T, lengths, *norm, base, spec_gain,
+                           power, num_iter, preemphasis, angles, wav, wav_pitch, wav_lengths, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
 }
 
 #define B200_HANDLE_API(NAME, TYPE, CFG)                                                                        \

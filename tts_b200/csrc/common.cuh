@@ -236,7 +236,9 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              // Tacotron (tacotron.cu, recurrent.cu): the GRUCell (8 / 32 rows per weight read), the persistent biGRU,
              // the highway stack, the step epilogue
              DISPATCH_GRU_CELL = 29, DISPATCH_GRU_CELL32 = 30, DISPATCH_BIGRU = 31, DISPATCH_HIGHWAY = 32,
-             DISPATCH_TACO1_STEP = 33 };
+             DISPATCH_TACO1_STEP = 33,
+             // Griffin-Lim (griffin_lim.cu): the magnitude preparation, one iteration, the deemphasis / output pass
+             DISPATCH_GL_PREPARE = 34, DISPATCH_GL_ITER = 35, DISPATCH_GL_DEEMPHASIS = 36 };
 void dispatch_begin();
 int dispatch_end(int* ids, int cap);
 void dispatch_note(int id);

@@ -166,6 +166,21 @@ struct Stft {
     int mel_project(const float* spec, int B, int n_frames, float log_clamp, float* out, cudaStream_t st) const;
 };
 
+// Griffin-Lim (griffin_lim.cu): a normalised [B, C, T] linear or mel spectrogram -> waveform [B, hop (T_b - 1)].
+struct GriffinLim {
+    int n_fft = 0, hop = 0, log2n = 0, n_mels = 0;   // n_mels > 0: mel input through the pseudo-inverse
+    int win_lo = 0, win_hi = 0;                      // the window's nonzero span in [0, n_fft)
+    DevBuf<float> window;                            // [n_fft], the analysis window centred in the frame
+    DevBuf<float2> twiddle;                          // n_fft / 2 (cos, sin) pairs
+    ConvLayer pinv;                                  // [F, n_mels] pinv(mel_basis) as a 1x1 conv
+    int init(int n_fft, int hop, const float* window_host, const float* pinv_host, int n_mels);
+    size_t workspace_bytes(int B, int T) const;
+    int forward(const float* x, long long x_bs, int x_cs, int x_ts, int B, int C, int T, const int* lens,
+                const b200tts_audio_norm& norm, float base, float spec_gain, float power, int num_iter, float preemphasis,
+                const float* u, float* wav, long long wav_pitch, int* wav_lengths, void* ws, size_t ws_bytes,
+                cudaStream_t st) const;
+};
+
 // H/ASP ResNet speaker encoder (speaker_encoder.cu).  Activations are freq-major with one zero row above and below,
 // [H + 2][C][L]: the B windows sit side by side on the time axis, window b in columns [b*P, b*P + T) of its stage, with
 // zero columns up to (b+1)*P; a 3x3 conv is then a 1D conv over the 3C channel rows of three adjacent freq rows.

@@ -3,12 +3,13 @@
 //            sqrt(re^2+im^2+1e-6)), :141-157 (spec_to_mel: mel_basis @ spec, log(clamp(.,1e-5))), :160-208 (wav_to_mel);
 //            TTS/utils/audio/torch_transforms.py:104-145 (TorchSTFT.__call__: center=True, sqrt(clamp(.,1e-8))).
 // One CTA transforms FR consecutive frames of one utterance: windowed frame -> shared memory (bit-reversed),
-// radix-2 FFT in shared memory with a precomputed twiddle table, magnitudes staged in shared memory and written
+// radix-2 FFT in shared memory with a precomputed twiddle table (fft.cuh), magnitudes staged in shared memory and written
 // as FR-wide runs per frequency bin (the [B, F, frames] layout is frame-contiguous).  The mel projection is a
 // 1x1 "conv" over the frequency axis through the fused conv1d kernel with a log-clamp epilogue.
 #include <math.h>
 
 #include "engines.cuh"
+#include "fft.cuh"
 
 namespace b200tts {
 
@@ -16,14 +17,6 @@ namespace {
 
 constexpr int STFT_FR = 8;
 constexpr int STFT_NT = 256;
-
-__device__ __forceinline__ int reflect_index(int i, int n) {   // torch 'reflect' padding (no edge repeat)
-    if (n == 1) return 0;
-    const int period = 2 * (n - 1);
-    i %= period;
-    if (i < 0) i += period;
-    return (i < n) ? i : period - i;
-}
 
 __global__ void __launch_bounds__(STFT_NT) stft_mag_kernel(const float* wav, const float* window, const float2* twiddle,
                                                           float* spec, int T, int n_fft, int log2n, int hop, int pad1,
@@ -45,23 +38,13 @@ __global__ void __launch_bounds__(STFT_NT) stft_mag_kernel(const float* wav, con
             i -= pad1;                                  // index into the raw signal
             if (pad1 > 0) i = reflect_index(i, T);
             const float v = (i >= 0 && i < T) ? wb[i] * window[n] : 0.f;
-            const int r = (int)(__brev((unsigned)n) >> (32 - log2n));
+            const int r = fft_brev(n, log2n);
             re[r] = v;
             im[r] = 0.f;
         }
         __syncthreads();
         for (int s = 1; s <= log2n; ++s) {
-            const int half = 1 << (s - 1), tstride = n_fft >> s;
-            for (int k = tid; k < n_fft / 2; k += STFT_NT) {
-                const int j = k & (half - 1);
-                const int i0 = ((k >> (s - 1)) << s) + j, i1 = i0 + half;
-                const float2 w = twiddle[j * tstride];  // (cos, -sin)(2 pi j tstride / n_fft)
-                const float xr = re[i1], xi = im[i1];
-                const float tr = w.x * xr - w.y * xi, ti = w.x * xi + w.y * xr;
-                const float ur = re[i0], ui = im[i0];
-                re[i0] = ur + tr; im[i0] = ui + ti;
-                re[i1] = ur - tr; im[i1] = ui - ti;
-            }
+            fft_dit_radix2(re, im, twiddle, n_fft, s, tid, STFT_NT);
             __syncthreads();
         }
         for (int f = tid; f < F; f += STFT_NT) {
@@ -89,11 +72,7 @@ int Stft::init(int n_fft_, int hop_, const float* window_host, const float* mel_
     B200_REQUIRE(hop >= 1 && window_host, "stft: bad arguments");
     int rc;
     if ((rc = upload(window, window_host, n_fft))) return rc;
-    std::vector<float2> tw(n_fft / 2);
-    for (int k = 0; k < n_fft / 2; ++k) {
-        const double a = -2.0 * M_PI * (double)k / (double)n_fft;
-        tw[k] = make_float2((float)cos(a), (float)sin(a));
-    }
+    const std::vector<float2> tw = fft_twiddles(n_fft);
     if ((rc = upload(twiddle, tw.data(), tw.size()))) return rc;
     if (mel_basis_host && n_mels > 0) {
         // mel = basis [n_mels, F] @ spec [F, frames]  ==  1x1 conv with Cin = F

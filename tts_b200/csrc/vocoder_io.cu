@@ -10,47 +10,12 @@
 //  absmax / to_int16    : save_wav's peak normalisation, wav * (32767 / max(0.01, max|wav|)) truncated to int16
 //      (TTS/utils/audio/numpy_transforms.py:439-441), on the device: the conv_post kernel already folds max|wav| into a
 //      device word while it stores the waveform (conv1d.cu), to_int16 scales and converts.
+#include "audio_norm.cuh"
 #include "engines.cuh"
 
 namespace b200tts {
 
 namespace {
-
-struct NormParams {          // one AudioProcessor's normalisation settings
-    int signal_norm, symmetric_norm, clip_norm, has_scaler;
-    float max_norm, min_level_db, ref_level_db;
-    const float* mean;       // [C] (mean-var scaler) or null
-    const float* scale;      // [C]
-};
-
-__device__ __forceinline__ float denorm_one(const NormParams& p, float s, int c) {
-    if (!p.signal_norm) return s;
-    if (p.has_scaler) return __fadd_rn(__fmul_rn(s, p.scale[c]), p.mean[c]);     // StandardScaler.inverse_transform
-    if (p.symmetric_norm) {
-        if (p.clip_norm) s = fminf(fmaxf(s, -p.max_norm), p.max_norm);
-        // ((S + max_norm) * -min_level_db / (2 * max_norm)) + min_level_db   evaluated left to right like numpy
-        s = __fadd_rn(__fdiv_rn(__fmul_rn(__fadd_rn(s, p.max_norm), -p.min_level_db), __fmul_rn(2.f, p.max_norm)), p.min_level_db);
-        return __fadd_rn(s, p.ref_level_db);
-    }
-    if (p.clip_norm) s = fminf(fmaxf(s, 0.f), p.max_norm);
-    s = __fadd_rn(__fdiv_rn(__fmul_rn(s, -p.min_level_db), p.max_norm), p.min_level_db);
-    return __fadd_rn(s, p.ref_level_db);
-}
-
-__device__ __forceinline__ float norm_one(const NormParams& p, float s, int c) {
-    if (!p.signal_norm) return s;
-    if (p.has_scaler) return __fdiv_rn(__fsub_rn(s, p.mean[c]), p.scale[c]);     // StandardScaler.transform
-    s = __fsub_rn(s, p.ref_level_db);
-    float n = __fdiv_rn(__fsub_rn(s, p.min_level_db), -p.min_level_db);
-    if (p.symmetric_norm) {
-        n = __fsub_rn(__fmul_rn(__fmul_rn(2.f, p.max_norm), n), p.max_norm);
-        if (p.clip_norm) n = fminf(fmaxf(n, -p.max_norm), p.max_norm);
-        return n;
-    }
-    n = __fmul_rn(p.max_norm, n);
-    if (p.clip_norm) n = fminf(fmaxf(n, 0.f), p.max_norm);
-    return n;
-}
 
 // out[b, c, j] for j in [0, Tmid + 2*pad): source column jj = clamp(j - pad, 0, Tmid - 1) of the interpolated
 // spectrogram; interpolation (Tmid != T): src = (jj + 0.5) * (T / Tmid) - 0.5 clamped at 0, neighbours t0, min(t0+1, T-1).
@@ -110,15 +75,6 @@ __global__ void to_int16_kernel(const float* __restrict__ x, long long n, const 
     const float s = __fdiv_rn(32767.f, fmaxf(0.01f, peak));
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
         out[i] = (short)__float2int_rz(__fmul_rn(x[i], s));
-}
-
-static NormParams to_params(const b200tts_audio_norm& a) {
-    NormParams p;
-    p.signal_norm = a.signal_norm; p.symmetric_norm = a.symmetric_norm; p.clip_norm = a.clip_norm;
-    p.has_scaler = (a.scaler_mean && a.scaler_scale) ? 1 : 0;
-    p.max_norm = a.max_norm; p.min_level_db = a.min_level_db; p.ref_level_db = a.ref_level_db;
-    p.mean = a.scaler_mean; p.scale = a.scaler_scale;
-    return p;
 }
 
 }  // namespace

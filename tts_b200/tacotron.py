@@ -26,7 +26,8 @@ Differences from the reference, on purpose:
 Out of scope (construction or the call raises ``NotImplementedError``): GST and Capacitron, speaker embeddings and
 d-vectors, graves attention, windowing, forward attention and the transition agent, the bidirectional decoder,
 encoder / decoder widths other than 256, inference in training mode (the encoder prenet's dropout), and training
-(``forward``).  Also not built: Griffin-Lim (``ap.inv_spectrogram``, a CPU utility), streaming and 16-bit precision.
+(``forward``).  Also not built: streaming and 16-bit precision.
+A linear output reaches audio through ``tts_b200.audio.AudioProcessor.inv_spectrogram`` (Griffin-Lim on the device).
 """
 import ctypes
 from dataclasses import dataclass
