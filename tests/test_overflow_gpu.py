@@ -78,7 +78,6 @@ def test_bilstm_against_float64_ragged():
     states = torch.empty(len(lens), 200 * 2, 512, device=DEV)
     h = model.handle(DEV)
     L = _lib.lib()
-    OV._declare(L)
     ws = torch.full((L.b200tts_overflow_workspace_bytes(h, len(lens), 200, 1) // 4,), float("nan"), device=DEV)
     tok, ln = text.to(DEV), lt.to(DEV)   # held: the call is asynchronous
     with _lib.dispatch_log() as log:

@@ -110,6 +110,27 @@ class UnivnetConfigC(ctypes.Structure):
                [(n, ctypes.c_int) for n in ("lvc_layers", "lvc_kernel_size", "kpnet_hidden_channels", "kpnet_conv_size")]
 
 
+class OverflowConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "encoder_dim", "n_convs", "state_per_phone", "out_channels",
+                                            "ar_order", "prenet_dim", "prenet_n_layers", "prenet_dropout",
+                                            "memory_rnn_dim", "outputnet_n_layers")] + \
+               [("outputnet_size", ctypes.c_int * 8), ("std_floor", ctypes.c_float)] + \
+               [(n, ctypes.c_int) for n in ("has_decoder", "hidden_channels_dec", "kernel_size_dec", "dilation_rate",
+                                            "num_flow_blocks", "num_block_layers", "num_splits", "num_squeeze",
+                                            "sigmoid_scale")]
+
+
+class Tacotron2ConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "out_channels", "r_init", "attention_type", "location_attn",
+                                            "attention_norm", "prenet_bn", "prenet_dropout")]
+
+
+class TacotronConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "frame_channels", "out_channels", "r_init", "memory_size",
+                                            "attention_type", "location_attn", "attention_norm", "prenet_bn",
+                                            "prenet_dropout")]
+
+
 # padding modes of b200tts_conv1d_create_padded (B200TTS_PAD_* in include/tts_b200.h)
 PADDING_MODES = {"zeros": 0, "reflect": 1}
 
@@ -347,6 +368,30 @@ def _declare(lib):
     lib.b200tts_durations.argtypes = [vp, vp, cf, ci, ci, vp, vp, vp, vp, vp, vp]
     lib.b200tts_expand_prior.restype = ci
     lib.b200tts_expand_prior.argtypes = [vp, vp, vp, vp, vp, cf, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
+    for name, cfgt in (("overflow", OverflowConfigC), ("tacotron2", Tacotron2ConfigC), ("tacotron", TacotronConfigC)):
+        f = getattr(lib, f"b200tts_{name}_create")
+        f.restype = ci
+        f.argtypes = [ctypes.POINTER(cfgt), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
+        f = getattr(lib, f"b200tts_{name}_destroy")
+        f.restype = None
+        f.argtypes = [vp]
+        f = getattr(lib, f"b200tts_{name}_workspace_bytes")
+        f.restype = sz
+        f.argtypes = [vp, ci, ci, ci]
+        f = getattr(lib, f"b200tts_{name}_encode")
+        f.restype = ci
+        f.argtypes = [vp, vp, vp, ci, ci, vp, vp, sz, vp]
+    lib.b200tts_overflow_sample.restype = ci
+    lib.b200tts_overflow_sample.argtypes = [vp, vp, ci, ci, cf, ci, cf, vp, vp, ci, vp, vp, vp, vp, sz, vp]
+    lib.b200tts_overflow_decode.restype = ci
+    lib.b200tts_overflow_decode.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
+    for name in ("tacotron2", "tacotron"):
+        f = getattr(lib, f"b200tts_{name}_decode_loop")
+        f.restype = ci
+        f.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, vp, vp, sz, vp]
+        f = getattr(lib, f"b200tts_{name}_postnet")
+        f.restype = ci
+        f.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
 
 
 def lib():

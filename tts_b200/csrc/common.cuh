@@ -229,7 +229,7 @@ enum : int { DISPATCH_FMA = 0, DISPATCH_TC3 = 3, DISPATCH_TC3_GROUPED = 5, DISPA
              DISPATCH_LSTM_BI = 18, DISPATCH_LSTM_CELL = 19, DISPATCH_HMM_LINEAR = 20, DISPATCH_HMM_STEP = 21,
              // Parallel WaveGAN (pwgan.cu): the fused residual layer, the folded conditioning conv
              DISPATCH_PWGAN_TC = 22, DISPATCH_PWGAN_AUX = 23,
-             // Tacotron2 (tacotron2.cu): the attention step, the step epilogue; the LSTMCell with 32 rows per weight read
+             // Tacotron2 (taco_decoder.cu, tacotron2.cu): the attention step, the step epilogue; the LSTMCell with 32 rows per weight read
              DISPATCH_TACO_ATTN = 24, DISPATCH_TACO_STEP = 25, DISPATCH_LSTM_CELL32 = 26,
              // UnivNet (univnet.cu): the kernel-prediction GEMM, the fused LVC layer
              DISPATCH_UNIVNET_PREDICT = 27, DISPATCH_UNIVNET_LVC = 28,
@@ -259,5 +259,13 @@ struct Arena {
     }
 };
 inline size_t arena_bytes(size_t n_floats) { return (n_floats * sizeof(float) + 255) & ~size_t(255); }
+// bytes an allocation sequence f(Arena&) takes from an Arena (a dry run over an unbounded one), so a workspace is sized
+// by the code that lays it out.  The dry run's first allocation is null: f must make every allocation before it checks
+// any of them.
+template <class F> size_t arena_size(F&& f) {
+    Arena ar(nullptr, ~size_t(0) >> 1);
+    f(ar);
+    return ar.off;
+}
 
 }  // namespace b200tts

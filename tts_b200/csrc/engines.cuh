@@ -334,6 +334,12 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
                    const std::function<int(cudaStream_t, int, bool)>& step, const int* ctl, int B, std::vector<int>& host,
                    cudaStream_t st);
 
+// An eval-mode BatchNorm folded into the layer before it (recurrent.cu): w [Cout][row] (row = Cin * K), bias [Cout] or
+// null, bn -> {gamma, beta, running_mean, running_var} [Cout].  wf = w * s, bf = beta - mean * s (no bias) or
+// (bias - mean) * s + beta, s = gamma / sqrt(var + eps), in double.
+void fold_bn(const float* w, const float* bias, const float* const* bn, double eps, int Cout, size_t row,
+             std::vector<float>& wf, std::vector<float>& bf);
+
 // The Tacotron2 text encoder (TTS/tts/layers/tacotron/tacotron2.py:73-112, also Overflow's encoder): embedding,
 // n_convs x (conv k5 with BatchNorm folded -> ReLU), the LSTM input projection of both directions as one 1x1 conv, then
 // one BiLSTM launch per time step (lstm_bi), each row at its own length.
@@ -369,7 +375,6 @@ struct Overflow {
     GlowDecoder dec;
     int init(const b200tts_overflow_config& cfg, const float* const* w, int nw);
     int tq(int F) const { return (F / c.num_squeeze + 3) / 4 * 4; }
-    size_t persist_bytes(int B, int Tt) const;     // zc and the loop state, kept from encode to sample
     size_t workspace_bytes(int B, int Tt, int F) const;
     int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* states, void* ws,
                size_t ws_bytes, cudaStream_t st) const;
@@ -380,24 +385,67 @@ struct Overflow {
                cudaStream_t st) const;
 };
 
-// Tacotron2 inference (tacotron2.cu).  encode: the SeqEncoder (hidden 256 per direction) into the encoder outputs
+// ---- the decoder plumbing of the Tacotron models (taco_decoder.cu)
+// The loop state both models keep at the start of the workspace from encode to the end of the loop: inputs_layer of
+// the encoder outputs pin [B, 128, Tt], the loop control ctl [2 + B] ({rows running, step, steps per row}), done [B],
+// the attention weights alpha and their running sum cum [B, Tt], the projection proj [B, RC], the stop logit [B], then
+// nzero floats zeroed at the start of the loop, out of which each model slices its RNN states, context and go frame.
+struct TacoLoop {
+    float *pin, *alpha, *cum, *proj, *logit, *zero;
+    int *ctl, *done;
+    size_t nzero;
+};
+// lays the state out from the arena's current offset; false when the arena runs out
+bool taco_loop_layout(Arena& ar, int B, int Tt, int RC, size_t nzero, TacoLoop& p);
+// the loop's start: zeroes dec_out [B, S, rC], stop [B, S], align [B, S, Tt], cum and the zeroed region; alpha zero
+// (original attention) or one-hot at token 0 (one_hot: DCA); no row done, step 0
+int taco_loop_start(const TacoLoop& p, int B, int Tt, int S, int rC, int one_hot, float* dec_out, float* stop,
+                    float* align, cudaStream_t st);
+// The attention step (OriginalAttention, optionally location-sensitive, or MonotonicDynamicConvolutionAttention, with
+// mask None), one CTA per running row over its len_b tokens: the weights, the context and the alignment row of step
+// ctl[1].  Query / encoder widths 1024 / 512 (Tacotron2) or 256 / 256 (Tacotron); attention dim 128.
+struct TacoAttention {
+    int Q = 0, E = 0, type = 0, location = 0, softmax = 0;   // type 0: original, 1: dynamic convolution
+    ConvLayer inproj;                          // inputs_layer as a 1x1 conv (original attention)
+    DevBuf<float> wq, bq, v, wc, wd;           // query_layer, its bias (DCA), v, location conv and dense
+    DevBuf<float> prior, wk, ws, wsl, wdl, bdl;   // DCA: prior, key_layer, static conv / layer, dynamic layer
+    float vb = 0.f;                            // v's bias (original attention)
+    // the number of weight tensors init reads
+    static int n_weights(int type, int location);
+    // w, original: query_layer, inputs_layer, v.weight, v.bias[, location_conv1d, location_dense]; DCA: prior,
+    // query_layer.weight, .bias, key_layer, static_filter_conv, static_filter_layer, dynamic_filter_layer.weight, .bias,
+    // v; *consumed = n_weights(type, location)
+    int init(int Q, int E, int type, int location, int softmax, const float* const* w, int* consumed);
+    // the step-invariant keys pin [B, 128, Tt] = inputs_layer(enc) for every token (original attention; DCA: nothing),
+    // through encT [B, E, Tt]
+    int keys(const float* enc, float* encT, float* pin, int B, int Tt, cudaStream_t st) const;
+    // the dynamic shared memory of the step for Tt tokens (set as the kernel's limit on the current device; fails past
+    // the opt-in maximum)
+    int prepare(int Tt, size_t* smem) const;
+    // one step from q [B, Q] and enc [B, Tt, E] into ctx [B, E], p's alpha / cum and align [B, S, Tt]
+    int launch(const TacoLoop& p, const float* q, float* ctx, const float* enc, float* align, int S,
+               const long long* lens, int B, int Tt, size_t smem, cudaStream_t st, bool note) const;
+};
+// the postnet input: x [B, C, Tp] = dec [B, Fpitch, C] transposed below frames[b], else 0; mask [B, Tp] likewise
+int launch_frames_in(const float* dec, int Fpitch, const int* frames, float* x, float* mask, int B, int C, int Tp,
+                     cudaStream_t st);
+// out [B, F, C] = y [B, C, Tp] transposed, t < F
+int launch_frames_out(const float* y, int Tp, float* out, int B, int F, int C, cudaStream_t st);
+
+// Tacotron2 inference (tacotron2.cu, on the plumbing above).  encode: the SeqEncoder (hidden 256 per direction) into the encoder outputs
 // [B, Tt, 512] and, for the original attention, inputs_layer of them for every token as one 1x1 conv.  decode_loop: the
 // attention decoder, chunk_steps steps per CUDA graph replay, one host read per chunk.  postnet: the 5 ConvBNBlocks
 // (BatchNorm folded) on the conv engine, masked past each row's frames, plus the decoder output.
 struct Tacotron2 {
     b200tts_tacotron2_config c;
     SeqEncoder enc;
-    ConvLayer inproj;                  // attention.inputs_layer as a 1x1 conv (original attention)
+    TacoAttention att;
     ConvLayer post[5];
     DevBuf<float> prenet_w[2], prenet_b[2];     // bias: the folded "bn" prenet only
     DevBuf<float> arnn_wih, arnn_whh, arnn_b;   // [4096][768], [4096][1024], b_ih + b_hh
     DevBuf<float> drnn_wih, drnn_whh, drnn_b;   // [4096][1536], [4096][1024], b_ih + b_hh
-    DevBuf<float> att_wq, att_bq, att_v, att_wc, att_wd;
-    DevBuf<float> att_prior, att_wk, att_ws, att_wsl, att_wdl, att_bdl;
-    float att_vb = 0.f;
     DevBuf<float> proj_w, proj_b, stop_w, stop_b;
     int init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw);
-    size_t persist_bytes(int B, int Tt) const;
     size_t workspace_bytes(int B, int Tt, int F) const;
     int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
                size_t ws_bytes, cudaStream_t st) const;
@@ -408,30 +456,7 @@ struct Tacotron2 {
                 size_t ws_bytes, cudaStream_t st) const;
 };
 
-// One attention step of the Tacotron models (tacotron2.cu; OriginalAttention / MonotonicDynamicConvolutionAttention
-// with mask None), one CTA per running row over its len_b tokens: the weights, the context and the alignment row of step
-// ctl[1].  Instantiated for query / encoder widths 1024 / 512 (Tacotron2) and 256 / 256 (Tacotron).
-struct AttnArgs {
-    const float* q = nullptr;                 // [B, Q] attention-RNN output
-    const float* enc = nullptr;               // [B, Tt, E] encoder outputs
-    const float* pin = nullptr;               // [B, A, Tt] inputs_layer(encoder outputs)
-    float* alpha = nullptr; float* cum = nullptr;   // [B, Tt] previous / cumulative weights
-    float* ctx = nullptr;                     // [B, E]
-    float* align = nullptr; int max_steps = 0;      // [B, max_steps, Tt]
-    const long long* lens = nullptr; const int* done = nullptr; const int* ctl = nullptr;
-    int Tt = 0, type = 0, location = 0, softmax = 0;
-    // original: Wq [A][Q], v [A], vb; location: Wc [F][2][K], Wd [A][F]
-    // DCA: Wq [A][Q], bq [A], Wk [F*K][A], Ws [F][K], Wsl [A][F], Wdl [A][F], bdl [A], v [A], prior [11]
-    const float *Wq = nullptr, *bq = nullptr, *v = nullptr, *Wc = nullptr, *Wd = nullptr;
-    const float *Wk = nullptr, *Ws = nullptr, *Wsl = nullptr, *Wdl = nullptr, *bdl = nullptr, *prior = nullptr;
-    float vb = 0.f;
-};
-// the dynamic shared memory of the attention step for Tt tokens (set as the kernel's limit on the current device;
-// fails past the opt-in maximum), then the launch itself (Q / E: 1024 / 512 or 256 / 256)
-int taco_attn_prepare(int Q, int E, int Tt, size_t* smem);
-int launch_taco_attn(const AttnArgs& a, int Q, int E, int B, size_t smem, cudaStream_t st, bool note);
-
-// Tacotron (1) inference (tacotron.cu).  encode: embedding, the encoder prenet and CBHG (K = 16) into the encoder
+// Tacotron (1) inference (tacotron.cu, on the plumbing above).  encode: embedding, the encoder prenet and CBHG (K = 16) into the encoder
 // outputs [B, Tt, 256] and, for the original attention, inputs_layer of them.  decode_loop: the GRU attention decoder,
 // chunk_steps steps per CUDA graph replay.  postnet: the postnet CBHG (K = 8) and last_linear.  A CBHG is the conv bank
 // as one conv over the union tap window, the two projections (BatchNorm, eps 1e-3, folded; ReLU in the epilogue; masked
@@ -454,12 +479,10 @@ struct Tacotron {
     DevBuf<float> emb;
     ConvLayer eprenet[2];
     Cbhg ecbhg, pcbhg;
-    ConvLayer inproj, last;
+    ConvLayer last;
+    TacoAttention att;
     DevBuf<float> prenet_w[2], prenet_b[2];
     DevBuf<float> arnn_wih, arnn_whh, arnn_b;   // [768][384], [768][256], bias as GruArgs
-    DevBuf<float> att_wq, att_bq, att_v, att_wc, att_wd;
-    DevBuf<float> att_prior, att_wk, att_ws, att_wsl, att_wdl, att_bdl;
-    float att_vb = 0.f;
     DevBuf<float> pdi_w, pdi_b;                 // project_to_decoder_in [256][512]
     DevBuf<float> drnn_wih[2], drnn_whh[2], drnn_b[2];
     DevBuf<float> proj_w, proj_b, stop_w, stop_b;

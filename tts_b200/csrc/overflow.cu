@@ -129,6 +129,13 @@ static bool persist_layout(const Overflow& e, Arena& ar, int B, int Tt, Persist&
     return p.zc && p.ctl && p.state && p.done && p.quant && p.hm && p.cm && p.pin && p.pb && p.hid && p.outp;
 }
 
+static void decode_scratch(const Overflow& e, Arena& ar, int B, int Tq, float** za, float** msk, float** melc) {
+    const int C = e.c.out_channels, nsq = e.c.num_squeeze;
+    *za = ar.f32((size_t)B * C * nsq * Tq);
+    *msk = ar.f32((size_t)B * Tq);
+    *melc = ar.f32((size_t)B * C * Tq * nsq);
+}
+
 int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, int nw) {
     c = cfg;
     const int E = c.encoder_dim, C = c.out_channels, P = c.prenet_dim, M = c.memory_rnn_dim, nL = c.outputnet_n_layers;
@@ -191,24 +198,20 @@ int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, in
     return 0;
 }
 
-size_t Overflow::persist_bytes(int B, int Tt) const {
-    int omax = 0;
-    for (int l = 0; l < c.outputnet_n_layers; ++l) omax = std::max(omax, c.outputnet_size[l]);
-    const int N = Tt * c.state_per_phone, M = c.memory_rnn_dim;
-    return arena_bytes((size_t)B * O1 * N) + 3 * arena_bytes(B) + arena_bytes(2 + B) + arena_bytes((size_t)2 * B * M) +
-           arena_bytes((size_t)B * M) + arena_bytes((size_t)B * c.ar_order * c.out_channels) +
-           arena_bytes((size_t)2 * B * c.prenet_dim) + arena_bytes((size_t)2 * B * omax) +
-           arena_bytes((size_t)B * (2 * c.out_channels + 1));
-}
-
 size_t Overflow::workspace_bytes(int B, int Tt, int F) const {
     const int E = c.encoder_dim, N = Tt * c.state_per_phone;
-    const size_t encb = persist_bytes(B, Tt) + enc.workspace_bytes(B, Tt) + arena_bytes((size_t)B * E * N);
+    const size_t encb = arena_size([&](Arena& ar) {
+        Persist p;
+        persist_layout(*this, ar, B, Tt, p);
+        ar.f32((size_t)B * E * N);   // encode's transposed encoder states
+    }) + enc.workspace_bytes(B, Tt);
     size_t decb = 0;
     if (c.has_decoder && F > 0) {
-        const int Tq = tq(F), Cs = c.out_channels * c.num_squeeze;
-        decb = arena_bytes((size_t)B * Cs * Tq) + arena_bytes((size_t)B * Tq) +
-               arena_bytes((size_t)B * c.out_channels * Tq * c.num_squeeze) + dec.workspace_bytes(B, Tq);
+        const int Tq = tq(F);
+        decb = arena_size([&](Arena& ar) {
+            float* q[3];
+            decode_scratch(*this, ar, B, Tq, q, q + 1, q + 2);
+        }) + dec.workspace_bytes(B, Tq);
     }
     return std::max(encb, decb) + 1024;
 }
@@ -333,9 +336,8 @@ int Overflow::decode(const float* hmm_out, const int* frames, int B, int F, int 
     const int nsq = c.num_squeeze, Tv = F / nsq, Tq = tq(F), Cs = C * nsq;
     if (Tv == 0) return 0;
     Arena ar(ws, ws_bytes);
-    float* za = ar.f32((size_t)B * Cs * Tq);
-    float* msk = ar.f32((size_t)B * Tq);
-    float* melc = ar.f32((size_t)B * C * Tq * nsq);
+    float *za, *msk, *melc;
+    decode_scratch(*this, ar, B, Tq, &za, &msk, &melc);
     B200_REQUIRE(za && msk && melc, "overflow_decode: arena exhausted");
     {
         dim3 grid((Tq + 127) / 128, Cs, B);

@@ -441,19 +441,27 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
     return 0;
 }
 
+void fold_bn(const float* w, const float* bias, const float* const* bn, double eps, int Cout, size_t row,
+             std::vector<float>& wf, std::vector<float>& bf) {
+    const float *gamma = bn[0], *beta = bn[1], *mean = bn[2], *var = bn[3];
+    wf.assign((size_t)Cout * row, 0.f);
+    bf.assign(Cout, 0.f);
+    for (int o = 0; o < Cout; ++o) {
+        const double s = (double)gamma[o] / sqrt((double)var[o] + eps);
+        for (size_t k = 0; k < row; ++k) wf[(size_t)o * row + k] = (float)(w[(size_t)o * row + k] * s);
+        bf[o] = bias ? (float)(((double)bias[o] - mean[o]) * s + beta[o]) : (float)((double)beta[o] - mean[o] * s);
+    }
+}
+
 // ------------------------------------------------------------------ the text encoder
 int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, const float* const* w, int* consumed) {
     n_vocab = vocab; E = dim; H = hidden; n_convs = convs_n;
     B200_REQUIRE(n_vocab > 0 && E > 0 && H > 0 && n_convs >= 1 && n_convs <= 8, "encoder: unsupported config");
     int rc, i = 0;
     if ((rc = upload(emb, w[i++], (size_t)n_vocab * E))) return rc;
+    std::vector<float> wf, bf;
     for (int l = 0; l < n_convs; ++l, i += 6) {   // ConvBNBlock: BatchNorm1d (eps 1e-5) folded into the conv
-        std::vector<float> wf((size_t)E * E * 5), bf(E);
-        for (int o = 0; o < E; ++o) {
-            const double s = (double)w[i + 2][o] / sqrt((double)w[i + 5][o] + 1e-5);
-            for (size_t k = 0; k < (size_t)E * 5; ++k) wf[(size_t)o * E * 5 + k] = (float)(w[i][(size_t)o * E * 5 + k] * s);
-            bf[o] = (float)(((double)w[i + 1][o] - w[i + 4][o]) * s + w[i + 3][o]);
-        }
+        fold_bn(w[i], w[i + 1], w + i + 2, 1e-5, E, (size_t)E * 5, wf, bf);
         if ((rc = pack_conv(convs[l], wf.data(), bf.data(), E, E, 5, 1, 2))) return rc;
     }
     {   // LSTM: both directions' input projections as one 1x1 conv (rows [fwd 4H | bwd 4H]), bias b_ih + b_hh

@@ -12,7 +12,7 @@ namespace b200tts {
 
 namespace {
 
-constexpr int EMB = 256, E = 256, Q = 256, D = 256, A = 128, BANK = 128, HW = 128, NHW = 4;
+constexpr int EMB = 256, E = 256, Q = 256, D = 256, BANK = 128, HW = 128, NHW = 4;
 constexpr int PN0 = 256, PN1 = 128;      // decoder and encoder prenet widths
 constexpr int HW_TF = 16;                // frames per highway CTA
 constexpr int HW_MAX_CIN = 1024;         // widest pre_highway input the highway kernel stages
@@ -150,88 +150,26 @@ __global__ void __launch_bounds__(256) taco1_step_kernel(Step1Args a) {
     }
 }
 
-// loop state at step 0: zero GRU states, context and go frame; alpha zero (original) or one-hot at token 0 (DCA)
-__global__ void taco1_reset_kernel(float* zero, size_t nzero, float* alpha, int Tt, int one_hot, int* done, int* ctl,
-                                   int B) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nzero; i += (size_t)gridDim.x * blockDim.x)
-        zero[i] = 0.f;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < B * Tt; i += gridDim.x * blockDim.x)
-        alpha[i] = (one_hot && i % Tt == 0) ? 1.f : 0.f;
-    if (blockIdx.x == 0)
-        for (int b = threadIdx.x; b < B; b += blockDim.x) {
-            done[b] = 0;
-            ctl[2 + b] = 0;
-            if (b == 0) { ctl[0] = B; ctl[1] = 0; }
-        }
-}
-
-// postnet input: x[b, c, t] = dec[b, t, c] below frames[b], else 0; mask[b, t] likewise
-__global__ void taco1_frames_in_kernel(const float* dec, int Fpitch, const int* frames, float* x, float* mask, int C,
-                                       int Tp) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x, c = blockIdx.y, b = blockIdx.z;
-    if (t >= Tp) return;
-    const bool valid = t < frames[b];
-    x[((size_t)b * C + c) * Tp + t] = valid ? dec[((size_t)b * Fpitch + t) * C + c] : 0.f;
-    if (c == 0) mask[(size_t)b * Tp + t] = valid ? 1.f : 0.f;
-}
-
-// out[b, t, c] = y[b, c, t] for t < F
-__global__ void taco1_frames_out_kernel(const float* y, int Tp, float* out, int F, int C) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
-    if (i >= F * C) return;
-    const int t = i / C, c = i - t * C;
-    out[(size_t)b * F * C + i] = y[((size_t)b * C + c) * Tp + t];
-}
-
-// conv (no bias) -> BatchNorm (eval, eps 1e-3) folded into weight [Cout][Cin][K] and bias
-void fold_bn(const float* const* w, int Cout, int Cin, int K, std::vector<float>& wf, std::vector<float>& bf) {
-    wf.assign((size_t)Cout * Cin * K, 0.f);
-    bf.assign(Cout, 0.f);
-    for (int o = 0; o < Cout; ++o) {
-        const double s = (double)w[1][o] / sqrt((double)w[4][o] + 1e-3);
-        for (size_t k = 0; k < (size_t)Cin * K; ++k) wf[(size_t)o * Cin * K + k] = (float)(w[0][(size_t)o * Cin * K + k] * s);
-        bf[o] = (float)((double)w[2][o] - w[3][o] * s);
-    }
-}
-
-// the workspace that lives from encode to the end of the loop
-struct Persist {
-    float *pin, *alpha, *cum, *proj, *logit, *pb, *din, *x1, *x2;
-    float *mem, *q, *ctx, *dh1, *dh2;   // zeroed region: mem [2][B][Cm], q / dh1 / dh2 [2][B][256], ctx [B][256]
-    int *ctl, *done;
-    size_t nzero;
+// the loop state plus Tacotron's own: the prenet outputs, the decoder input, the residual GRU outputs and, zeroed,
+// mem [2][B][Cm], q / dh1 / dh2 [2][B][256] and ctx [B][256]
+struct Persist : TacoLoop {
+    float *pb, *din, *x1, *x2;
+    float *mem, *q, *ctx, *dh1, *dh2;
 };
 
 bool persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
-    const int RC = e.c.frame_channels * e.c.r_init;
-    p.pin = ar.f32((size_t)B * A * Tt);
-    p.ctl = (int*)ar.f32(2 + B);
-    p.done = (int*)ar.f32(B);
-    p.alpha = ar.f32((size_t)B * Tt);
-    p.cum = ar.f32((size_t)B * Tt);
-    p.proj = ar.f32((size_t)B * RC);
-    p.logit = ar.f32(B);
+    const size_t nzero = (size_t)B * (2 * e.Cm + 2 * Q + E + 4 * D);
+    const bool ok = taco_loop_layout(ar, B, Tt, e.c.frame_channels * e.c.r_init, nzero, p);
     p.pb = ar.f32((size_t)B * (PN0 + PN1));
     p.din = ar.f32((size_t)B * D);
     p.x1 = ar.f32((size_t)B * D);
     p.x2 = ar.f32((size_t)B * D);
-    p.nzero = (size_t)B * (2 * e.Cm + 2 * Q + E + 4 * D);
-    float* z = ar.f32(p.nzero);
-    if (!(p.pin && p.ctl && p.done && p.alpha && p.cum && p.proj && p.logit && p.pb && p.din && p.x1 && p.x2 && z))
-        return false;
-    p.mem = z;
+    p.mem = p.zero;
     p.q = p.mem + (size_t)2 * B * e.Cm;
     p.ctx = p.q + (size_t)2 * B * Q;
     p.dh1 = p.ctx + (size_t)B * E;
     p.dh2 = p.dh1 + (size_t)2 * B * D;
-    return true;
-}
-
-// bytes an allocation sequence takes from an Arena (dry run over an unbounded one)
-template <class F> size_t arena_size(F&& f) {
-    Arena ar(nullptr, ~size_t(0) >> 1);
-    f(ar);
-    return ar.off;
+    return ok && p.pb && p.din && p.x1 && p.x2;
 }
 
 }  // namespace
@@ -246,7 +184,7 @@ int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int*
         const int padU = (K - 1) / 2;
         std::vector<float> wb((size_t)K * BANK * Cin * K, 0.f), bb((size_t)K * BANK);
         for (int k = 1; k <= K; ++k, i += 5) {
-            fold_bn(w + i, BANK, Cin, k, wf, bf);
+            fold_bn(w[i], nullptr, w + i + 1, 1e-3, BANK, (size_t)Cin * k, wf, bf);
             const int off = padU - (k - 1) / 2;
             for (int o = 0; o < BANK; ++o) {
                 const int row = (k - 1) * BANK + o;
@@ -258,10 +196,10 @@ int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int*
         }
         if ((rc = pack_conv(bank, wb.data(), bb.data(), K * BANK, Cin, K, 1, padU))) return rc;
     }
-    fold_bn(w + i, P1, K * BANK, 3, wf, bf);
+    fold_bn(w[i], nullptr, w + i + 1, 1e-3, P1, (size_t)K * BANK * 3, wf, bf);
     if ((rc = pack_conv(proj1, wf.data(), bf.data(), P1, K * BANK, 3, 1, 1))) return rc;
     i += 5;
-    fold_bn(w + i, Cin, P1, 3, wf, bf);
+    fold_bn(w[i], nullptr, w + i + 1, 1e-3, Cin, (size_t)P1 * 3, wf, bf);
     if ((rc = pack_conv(proj2, wf.data(), bf.data(), Cin, P1, 3, 1, 1))) return rc;
     i += 5;
     if (Cin != HW) {   // pre_highway [128][Cin] -> [Cin][128]
@@ -371,7 +309,7 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
     Cm = c.memory_size > 0 ? C * c.memory_size : C;
     const int cbhg_n_enc = 16 * 5 + 10 + 16 + 8, cbhg_n_post = 8 * 5 + 10 + (C != HW ? 1 : 0) + 16 + 8;
     const int expect = 1 + 4 + cbhg_n_enc + 2 * (c.prenet_bn ? 6 : 2) + 4 +
-                       (c.attention_type == 1 ? 9 : 4 + (c.location_attn ? 2 : 0)) + 2 + 8 + 2 + 2 + cbhg_n_post + 2;
+                       TacoAttention::n_weights(c.attention_type, c.location_attn) + 2 + 8 + 2 + 2 + cbhg_n_post + 2;
     B200_REQUIRE(nw == expect, "tacotron: expected %d weight tensors, got %d", expect, nw);
     int rc, i = 0, used = 0;
     if ((rc = upload(emb, w[i++], (size_t)c.n_vocab * EMB))) return rc;
@@ -380,6 +318,7 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
     i += 4;
     if ((rc = ecbhg.init(PN1, 16, 128, w + i, &used))) return rc;
     i += used;
+    std::vector<float> wf, bf;
     for (int l = 0; l < 2; ++l) {   // decoder prenet (with bias); "bn": eval BatchNorm (eps 1e-5) folded into the layer
         const int in = l ? PN0 : Cm, out = l ? PN1 : PN0;
         if (!c.prenet_bn) {
@@ -388,12 +327,7 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
             i += 2;
             continue;
         }
-        std::vector<float> wf((size_t)out * in), bf(out);
-        for (int o = 0; o < out; ++o) {
-            const double s = (double)w[i + 2][o] / sqrt((double)w[i + 5][o] + 1e-5);
-            for (int k = 0; k < in; ++k) wf[(size_t)o * in + k] = (float)(w[i][(size_t)o * in + k] * s);
-            bf[o] = (float)(((double)w[i + 1][o] - w[i + 4][o]) * s + w[i + 3][o]);
-        }
+        fold_bn(w[i], w[i + 1], w + i + 2, 1e-5, out, in, wf, bf);
         if ((rc = upload(prenet_w[l], wf.data(), wf.size()))) return rc;
         if ((rc = upload(prenet_b[l], bf.data(), bf.size()))) return rc;
         i += 6;
@@ -410,26 +344,8 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
         return upload(bias, b.data(), b.size());
     };
     if ((rc = gru(arnn_wih, arnn_whh, arnn_b, PN1 + E, Q))) return rc;
-    if (c.attention_type == 0) {
-        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
-        if ((rc = pack_conv(inproj, w[i++], nullptr, A, E, 1, 1, 0))) return rc;
-        if ((rc = upload(att_v, w[i++], A))) return rc;
-        att_vb = w[i++][0];
-        if (c.location_attn) {
-            if ((rc = upload(att_wc, w[i++], (size_t)32 * 2 * 31))) return rc;
-            if ((rc = upload(att_wd, w[i++], (size_t)A * 32))) return rc;
-        }
-    } else {
-        if ((rc = upload(att_prior, w[i++], 11))) return rc;
-        if ((rc = upload(att_wq, w[i++], (size_t)A * Q))) return rc;
-        if ((rc = upload(att_bq, w[i++], A))) return rc;
-        if ((rc = upload(att_wk, w[i++], (size_t)8 * 21 * A))) return rc;
-        if ((rc = upload(att_ws, w[i++], (size_t)8 * 21))) return rc;
-        if ((rc = upload(att_wsl, w[i++], (size_t)A * 8))) return rc;
-        if ((rc = upload(att_wdl, w[i++], (size_t)A * 8))) return rc;
-        if ((rc = upload(att_bdl, w[i++], A))) return rc;
-        if ((rc = upload(att_v, w[i++], A))) return rc;
-    }
+    if ((rc = att.init(Q, E, c.attention_type, c.location_attn, c.attention_norm, w + i, &used))) return rc;
+    i += used;
     if ((rc = upload(pdi_w, w[i], (size_t)D * (Q + E)))) return rc;
     if ((rc = upload(pdi_b, w[i + 1], D))) return rc;
     i += 2;
@@ -502,14 +418,7 @@ int Tacotron::encode(const long long* tokens, const long long* lengths, int B, i
         in = o;
     }
     if ((rc = ecbhg.run(xin, mask, nullptr, lengths, B, Tt, enc_out, (long long)Tt * E, E, 1, ar, st))) return rc;
-    if (c.attention_type == 0) {   // inputs_layer, step-invariant: pin [B, A, Tt]
-        if ((rc = launch_transpose(enc_out, encT, B, Tt, E, st))) return rc;
-        ConvIO io;
-        io.x = encT; io.x_bs = (long long)E * Tt; io.x_cs = Tt; io.Tin = Tt;
-        io.y = p.pin; io.y_bs = (long long)A * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        if ((rc = launch_conv(inproj, io, st))) return rc;
-    }
-    return 0;
+    return att.keys(enc_out, encT, p.pin, B, Tt, st);
 }
 
 int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
@@ -525,16 +434,11 @@ int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B,
     Arena ar(ws, ws_bytes);
     Persist p;
     B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron_decode_loop: arena exhausted");
-    B200_CUDA_OK(cudaMemsetAsync(dec_out, 0, sizeof(float) * (size_t)B * S * r * C, st));
-    B200_CUDA_OK(cudaMemsetAsync(stop_tokens, 0, sizeof(float) * (size_t)B * S, st));
-    B200_CUDA_OK(cudaMemsetAsync(alignments, 0, sizeof(float) * (size_t)B * S * Tt, st));
-    B200_CUDA_OK(cudaMemsetAsync(p.cum, 0, sizeof(float) * (size_t)B * Tt, st));
-    taco1_reset_kernel<<<64, 256, 0, st>>>(p.mem, p.nzero, p.alpha, Tt, c.attention_type == 1, p.done, p.ctl, B);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
     int rc;
+    if ((rc = taco_loop_start(p, B, Tt, S, r * C, c.attention_type == 1, dec_out, stop_tokens, alignments, st)))
+        return rc;
     size_t attn_smem = 0;
-    if ((rc = taco_attn_prepare(Q, E, Tt, &attn_smem))) return rc;
+    if ((rc = att.prepare(Tt, &attn_smem))) return rc;
     const int nb = B > 8 ? 32 : 8;
     // one step; parity = step index within the chunk (memory, query and both decoder h are double-buffered)
     auto step = [&](cudaStream_t cs, int par, bool note) -> int {
@@ -562,17 +466,7 @@ int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B,
             a.H = Q; a.bias = arnn_b; a.h_in = q_in; a.hin_bs = Q; a.h_out = q_out; a.h_bs = Q; a.done = p.done; a.B = B;
             if ((rc = launch_gru(a, nb, cs, note))) return rc;
         }
-        {
-            AttnArgs a;
-            a.q = q_out; a.enc = enc_out; a.pin = p.pin; a.alpha = p.alpha;
-            a.cum = (c.attention_type == 0 && c.location_attn) ? p.cum : nullptr;
-            a.ctx = p.ctx; a.align = alignments; a.max_steps = S; a.lens = lengths; a.done = p.done;
-            a.ctl = p.ctl; a.Tt = Tt; a.type = c.attention_type; a.location = c.location_attn;
-            a.softmax = c.attention_norm; a.Wq = att_wq; a.bq = att_bq; a.v = att_v; a.vb = att_vb; a.Wc = att_wc;
-            a.Wd = att_wd; a.Wk = att_wk; a.Ws = att_ws; a.Wsl = att_wsl; a.Wdl = att_wdl; a.bdl = att_bdl;
-            a.prior = att_prior;
-            if ((rc = launch_taco_attn(a, Q, E, B, attn_smem, cs, note))) return rc;
-        }
+        if ((rc = att.launch(p, q_out, p.ctx, enc_out, alignments, S, lengths, B, Tt, attn_smem, cs, note))) return rc;
         {   // project_to_decoder_in([query | context])
             LinArgs a;
             a.W = pdi_w; a.bias = pdi_b; a.K = Q; a.R = D; a.x = q_out; a.x_bs = Q; a.x2 = p.ctx; a.x2_bs = E; a.K2 = E;
@@ -631,10 +525,8 @@ int Tacotron::postnet(const float* dec_out, const int* frames, int B, int F, int
     float *x, *mask, *g, *y;
     postnet_scratch(*this, ar, B, Tp, &x, &mask, &g, &y);
     B200_REQUIRE(x && mask && g && y, "tacotron_postnet: arena exhausted");
-    taco1_frames_in_kernel<<<dim3((Tp + 127) / 128, C, B), 128, 0, st>>>(dec_out, Fpitch, frames, x, mask, C, Tp);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
     int rc;
+    if ((rc = launch_frames_in(dec_out, Fpitch, frames, x, mask, B, C, Tp, st))) return rc;
     // the biGRU writes channel-major [B, 256, Tp] for last_linear on the conv engine
     if ((rc = pcbhg.run(x, mask, frames, nullptr, B, Tp, g, (long long)2 * GRU_H * Tp, 1, Tp, ar, st))) return rc;
     {
@@ -644,10 +536,7 @@ int Tacotron::postnet(const float* dec_out, const int* frames, int B, int F, int
         io.ymask = mask; io.ymask_bs = Tp; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(last, io, st))) return rc;
     }
-    taco1_frames_out_kernel<<<dim3((F * O + 255) / 256, B), 256, 0, st>>>(y, Tp, out, F, O);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_frames_out(y, Tp, out, B, F, O, st);
 }
 
 }  // namespace b200tts

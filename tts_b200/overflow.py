@@ -224,35 +224,6 @@ class _OverflowDecoder(nn.Module):
                 f.store_inverse()
 
 
-class OverflowConfigC(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "encoder_dim", "n_convs", "state_per_phone", "out_channels",
-                                            "ar_order", "prenet_dim", "prenet_n_layers", "prenet_dropout",
-                                            "memory_rnn_dim", "outputnet_n_layers")] + \
-               [("outputnet_size", ctypes.c_int * 8), ("std_floor", ctypes.c_float)] + \
-               [(n, ctypes.c_int) for n in ("has_decoder", "hidden_channels_dec", "kernel_size_dec", "dilation_rate",
-                                            "num_flow_blocks", "num_block_layers", "num_splits", "num_squeeze",
-                                            "sigmoid_scale")]
-
-
-def _declare(L):
-    if getattr(L, "_overflow_declared", False):
-        return
-    vp, sz, ci, cf = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_float
-    L.b200tts_overflow_create.restype = ci
-    L.b200tts_overflow_create.argtypes = [ctypes.POINTER(OverflowConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
-    L.b200tts_overflow_destroy.restype = None
-    L.b200tts_overflow_destroy.argtypes = [vp]
-    L.b200tts_overflow_workspace_bytes.restype = sz
-    L.b200tts_overflow_workspace_bytes.argtypes = [vp, ci, ci, ci]
-    L.b200tts_overflow_encode.restype = ci
-    L.b200tts_overflow_encode.argtypes = [vp, vp, vp, ci, ci, vp, vp, sz, vp]
-    L.b200tts_overflow_sample.restype = ci
-    L.b200tts_overflow_sample.argtypes = [vp, vp, ci, ci, cf, ci, cf, vp, vp, ci, vp, vp, vp, vp, sz, vp]
-    L.b200tts_overflow_decode.restype = ci
-    L.b200tts_overflow_decode.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
-    L._overflow_declared = True
-
-
 def _format_aux_input(defaults, aux_input):
     """TTS/utils/generic_utils.py format_aux_input: a missing or None entry takes the default."""
     out = dict(aux_input or {})
@@ -325,7 +296,7 @@ class NeuralhmmTTS(EngineModule):
         dec = [self.hidden_channels_dec, self.kernel_size_dec, self.dilation_rate, self.num_flow_blocks_dec,
                self.num_block_layers, self.num_splits, self.num_squeeze, int(self.sigmoid_scale)] \
             if self._has_decoder else [0] * 8
-        cfg = OverflowConfigC(self.num_chars, self.encoder_in_out_features, self.encoder_n_convolutions,
+        cfg = _lib.OverflowConfigC(self.num_chars, self.encoder_in_out_features, self.encoder_n_convolutions,
                               self.state_per_phone, c, self.ar_order, self.prenet_dim, self.prenet_n_layers,
                               int(bool(self.prenet_dropout)), self.memory_rnn_dim, len(self.outputnet_size), sizes,
                               float(self.std_floor), int(self._has_decoder), *dec)
@@ -352,7 +323,6 @@ class NeuralhmmTTS(EngineModule):
                 t += [_host(an.logs.reshape(-1)), _host(an.bias.reshape(-1)), ic.inverse().contiguous()]
                 t += [_host(cb.start.weight), _host(cb.start.bias)] + cb.wn.ordered_weights() + \
                      [_host(cb.end.weight), _host(cb.end.bias)]
-        _declare(_lib.lib())
         return self._make("b200tts_overflow_create", cfg, t)
 
     # ------------------------------------------------------------------ inference
@@ -413,7 +383,6 @@ class NeuralhmmTTS(EngineModule):
         frames = (ctypes.c_int32 * b)()
         h = self.handle(dev)
         L = _lib.lib()
-        _declare(L)
         s = _lib.stream_ptr(dev)
         with torch.cuda.device(dev):
             ws = _lib.workspace(dev, L.b200tts_overflow_workspace_bytes(h, b, tt, max_t), "overflow")

@@ -191,37 +191,21 @@ class _Postnet(nn.Module):
         self.convolutions = nn.ModuleList([_ConvBNBlock(chans[i], chans[i + 1]) for i in range(num_convs)])
 
 
-class Tacotron2ConfigC(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "out_channels", "r_init", "attention_type", "location_attn",
-                                            "attention_norm", "prenet_bn", "prenet_dropout")]
+# config.model -> the class name and where the other model of the family is
+_MODELS = {"tacotron": ("Tacotron", "Tacotron2 is tts_b200.tacotron2.Tacotron2"),
+           "tacotron2": ("Tacotron2", "the Tacotron 1 model is tts_b200.tacotron.Tacotron")}
 
 
-def _declare(L):
-    if getattr(L, "_tacotron2_declared", False):
-        return
-    vp, sz, ci = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
-    L.b200tts_tacotron2_create.restype = ci
-    L.b200tts_tacotron2_create.argtypes = [ctypes.POINTER(Tacotron2ConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
-    L.b200tts_tacotron2_destroy.restype = None
-    L.b200tts_tacotron2_destroy.argtypes = [vp]
-    L.b200tts_tacotron2_workspace_bytes.restype = sz
-    L.b200tts_tacotron2_workspace_bytes.argtypes = [vp, ci, ci, ci]
-    L.b200tts_tacotron2_encode.restype = ci
-    L.b200tts_tacotron2_encode.argtypes = [vp, vp, vp, ci, ci, vp, vp, sz, vp]
-    L.b200tts_tacotron2_decode_loop.restype = ci
-    L.b200tts_tacotron2_decode_loop.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, vp, vp, sz, vp]
-    L.b200tts_tacotron2_postnet.restype = ci
-    L.b200tts_tacotron2_postnet.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, sz, vp]
-    L._tacotron2_declared = True
+def _check_config(cfg, model, width):
+    """NotImplementedError for every option this drop-in of ``model`` ("tacotron" / "tacotron2", encoder and decoder
+    widths ``width``) does not build."""
+    name, other = _MODELS[model]
 
-
-def _check_config(cfg):
-    """NotImplementedError for every option this drop-in does not build."""
     def no(what):
-        raise NotImplementedError(f"tts_b200: Tacotron2 with {what} is not built")
+        raise NotImplementedError(f"tts_b200: {name} with {what} is not built")
 
-    if getattr(cfg, "model", "tacotron2") != "tacotron2":
-        no(f"model {cfg.model!r} (only Tacotron2; the Tacotron 1 model is tts_b200.tacotron.Tacotron)")
+    if getattr(cfg, "model", model) != model:
+        no(f"model {cfg.model!r} (only {name}; {other})")
     if cfg.attention_type not in ("original", "dynamic_convolution"):
         no(f"attention_type {cfg.attention_type!r}")
     if cfg.attention_win or cfg.windowing:
@@ -236,90 +220,48 @@ def _check_config(cfg):
         no("speaker embeddings / d-vectors")
     if cfg.bidirectional_decoder:
         no("the bidirectional decoder")
-    if cfg.encoder_in_features != 512 or cfg.decoder_in_features != 512:
-        no("encoder / decoder widths other than 512 (the reference's embedding is fixed at 512)")
+    if cfg.encoder_in_features != width or cfg.decoder_in_features != width:
+        no(f"encoder / decoder widths other than {width} (the reference's embedding is fixed at {width})")
     if cfg.prenet_type not in ("original", "bn"):
         no(f"prenet_type {cfg.prenet_type!r}")
     if cfg.attention_norm not in ("sigmoid", "softmax"):
         raise ValueError("Unknown value for attention norm type")
 
 
-# ----------------------------------------------------------------------------- model
-class Tacotron2(EngineModule):
-    """Tacotron2 text -> mel synthesiser, inference path on sm_90a kernels."""
+# ----------------------------------------------------------------------------- models
+class _TacotronBase(EngineModule):
+    """What Tacotron and Tacotron2 share: the inference driver over the library's encode / decode_loop / postnet calls,
+    the attention's weight list, the config check, construction from a config and checkpoints.  A subclass sets
+    ``_model`` (the C-ABI prefix and ``config.model``), ``_width`` (encoder output width) and ``_extra_steps``."""
 
-    _destroy = "b200tts_tacotron2_destroy"
-
-    def __init__(self, config, ap=None, tokenizer=None, speaker_manager=None):
-        super().__init__()
-        _check_config(config)
-        self.config, self.ap, self.tokenizer, self.speaker_manager = config, ap, tokenizer, speaker_manager
-        for key in config:
-            setattr(self, key, config[key])
-        if tokenizer is not None:   # BaseTTS._set_model_args
-            self.num_chars = tokenizer.characters.num_chars
-        self.decoder_output_dim = self.out_channels
-        self.embedding = nn.Embedding(self.num_chars, 512, padding_idx=0)
-        self.encoder = _Encoder(self.encoder_in_features)
-        self.decoder = _Decoder(self.decoder_in_features, self.out_channels, self.r, self.attention_type,
-                                self.prenet_type, self.location_attn)
-        self.postnet = _Postnet(self.out_channels)
-        if self.double_decoder_consistency:
-            self.coarse_decoder = _Decoder(self.decoder_in_features, self.out_channels, self.ddc_r,
-                                           self.attention_type, self.prenet_type, self.location_attn)
+    _model = None
+    _width = None
+    _extra_steps = 0      # decoder steps a row may run past max_decoder_steps
 
     @classmethod
     def init_from_config(cls, config, samples=None, verbose=True):  # pylint: disable=unused-argument
         """base_tacotron.py init_from_config without the host-side managers (built by the caller)."""
         return cls(config)
 
-    # ------------------------------------------------------------------ packing
-    def _create(self, device):
-        d = self.decoder
-        dca = self.attention_type == "dynamic_convolution"
-        cfg = Tacotron2ConfigC(self.num_chars, self.out_channels, d.r_init, int(dca), int(bool(self.location_attn)),
-                               int(self.attention_norm == "softmax"), int(self.prenet_type == "bn"),
-                               int(bool(self.prenet_dropout)))
-        t = [_host(self.embedding.weight)]
-        for blk in list(self.encoder.convolutions):
-            t += self._conv_bn(blk)
-        for sfx in ("", "_reverse"):
-            t += [_host(getattr(self.encoder.lstm, f"{n}_l0{sfx}")) for n in ("weight_ih", "weight_hh", "bias_ih",
-                                                                              "bias_hh")]
-        for lin in d.prenet.linear_layers:
-            t += [_host(lin.linear_layer.weight)]
-            if self.prenet_type == "bn":
-                bn = lin.batch_normalization
-                t += [_host(bn.weight), _host(bn.bias), _host(bn.running_mean), _host(bn.running_var)]
-        t += self._cell(d.attention_rnn)
-        a = d.attention
-        if dca:
-            t += [_host(a.prior), _host(a.query_layer.weight), _host(a.query_layer.bias), _host(a.key_layer.weight),
-                  _host(a.static_filter_conv.weight), _host(a.static_filter_layer.weight),
-                  _host(a.dynamic_filter_layer.weight), _host(a.dynamic_filter_layer.bias), _host(a.v.weight)]
-        else:
-            t += [_host(a.query_layer.linear_layer.weight), _host(a.inputs_layer.linear_layer.weight),
-                  _host(a.v.linear_layer.weight), _host(a.v.linear_layer.bias)]
-            if self.location_attn:
-                t += [_host(a.location_layer.location_conv1d.weight),
-                      _host(a.location_layer.location_dense.linear_layer.weight)]
-        t += self._cell(d.decoder_rnn)
-        t += [_host(d.linear_projection.linear_layer.weight), _host(d.linear_projection.linear_layer.bias),
-              _host(d.stopnet[1].linear_layer.weight), _host(d.stopnet[1].linear_layer.bias)]
-        for blk in self.postnet.convolutions:
-            t += self._conv_bn(blk)
-        _declare(_lib.lib())
-        return self._make("b200tts_tacotron2_create", cfg, t)
-
-    @staticmethod
-    def _conv_bn(blk):
-        bn = blk.batch_normalization
-        return [_host(blk.convolution1d.weight), _host(blk.convolution1d.bias), _host(bn.weight), _host(bn.bias),
-                _host(bn.running_mean), _host(bn.running_var)]
+    def _check_call(self):
+        _check_config(self, self._model, self._width)
 
     @staticmethod
     def _cell(m):
         return [_host(m.weight_ih), _host(m.weight_hh), _host(m.bias_ih), _host(m.bias_hh)]
+
+    def _attention_weights(self, a):
+        """The attention's tensors in the order TacoAttention::init reads them."""
+        if self.attention_type == "dynamic_convolution":
+            return [_host(a.prior), _host(a.query_layer.weight), _host(a.query_layer.bias), _host(a.key_layer.weight),
+                    _host(a.static_filter_conv.weight), _host(a.static_filter_layer.weight),
+                    _host(a.dynamic_filter_layer.weight), _host(a.dynamic_filter_layer.bias), _host(a.v.weight)]
+        t = [_host(a.query_layer.linear_layer.weight), _host(a.inputs_layer.linear_layer.weight),
+             _host(a.v.linear_layer.weight), _host(a.v.linear_layer.bias)]
+        if self.location_attn:
+            t += [_host(a.location_layer.location_conv1d.weight),
+                  _host(a.location_layer.location_dense.linear_layer.weight)]
+        return t
 
     def _dropout_active(self):
         return bool(self.prenet_dropout) and (self.training or bool(self.prenet_dropout_at_inference))
@@ -327,10 +269,10 @@ class Tacotron2(EngineModule):
     # ------------------------------------------------------------------ inference
     @torch.no_grad()
     def inference(self, text, aux_input=None, *, draws=None):
-        """text int64 [B, T] (CUDA) -> dict(model_outputs [B, T_mel, C], decoder_outputs [B, T_mel, C], alignments
-        [B, T_dec, T], stop_tokens [B, T_dec, 1], model_outputs_len [B]).  ``draws`` (optional): the prenet dropout
-        masks, see the module docstring.  One host read per chunk of 32 decoder steps drives the loop."""
-        _check_config(self)
+        """text int64 [B, T] (CUDA) -> dict(model_outputs [B, T_out, out_channels], decoder_outputs [B, T_out, C],
+        alignments [B, T_dec, T], stop_tokens [B, T_dec, 1], model_outputs_len [B]).  ``draws`` (optional): the prenet
+        dropout masks, see the module docstring.  One host read per chunk of 32 decoder steps drives the loop."""
+        self._check_call()
         _lib.require_cuda(text, "text")
         dev = text.device
         tok = text.to(torch.int64).contiguous()
@@ -345,53 +287,54 @@ class Tacotron2(EngineModule):
         max_steps = int(self.max_decoder_steps)
         if max_steps < 1:
             raise ValueError("tts_b200: max_decoder_steps must be >= 1")
-        r, c = int(self.decoder.r), self.out_channels
+        steps_cap = max_steps + self._extra_steps
+        r, c = int(self.decoder.r), self.decoder_output_dim
         if not 1 <= r <= self.decoder.r_init:
             raise ValueError(f"tts_b200: r must be in [1, {self.decoder.r_init}], got {r}")
         drop = None
         if self._dropout_active():
             drop = (draws or {}).get("dropout", None)
             if drop is None:
-                drop = torch.empty((b, max_steps, 2, PRENET_DIM), dtype=torch.uint8, device=dev).bernoulli_(0.5)
+                drop = torch.empty((b, steps_cap, 2, PRENET_DIM), dtype=torch.uint8, device=dev).bernoulli_(0.5)
             else:
-                if drop.shape[0] != b or drop.shape[1] < max_steps or tuple(drop.shape[2:]) != (2, PRENET_DIM):
-                    raise ValueError(f"tts_b200: draws['dropout'] must be [{b}, >= {max_steps}, 2, {PRENET_DIM}], "
+                if drop.shape[0] != b or drop.shape[1] < steps_cap or tuple(drop.shape[2:]) != (2, PRENET_DIM):
+                    raise ValueError(f"tts_b200: draws['dropout'] must be [{b}, >= {steps_cap}, 2, {PRENET_DIM}], "
                                      f"got {tuple(drop.shape)}")
-                drop = drop[:, :max_steps].to(dev, torch.uint8).contiguous()
+                drop = drop[:, :steps_cap].to(dev, torch.uint8).contiguous()
         f32 = dict(dtype=torch.float32, device=dev)
-        enc = torch.empty((b, tt, 512), **f32)
-        dec = torch.empty((b, max_steps * r, c), **f32)
-        stop = torch.empty((b, max_steps), **f32)
-        align = torch.empty((b, max_steps, tt), **f32)
+        enc = torch.empty((b, tt, self._width), **f32)
+        dec = torch.empty((b, steps_cap * r, c), **f32)
+        stop = torch.empty((b, steps_cap), **f32)
+        align = torch.empty((b, steps_cap, tt), **f32)
         steps = (ctypes.c_int32 * b)()
         h = self.handle(dev)
-        L = _lib.lib()
-        _declare(L)
+        L, m = _lib.lib(), self._model
         s = _lib.stream_ptr(dev)
         with torch.cuda.device(dev):
             # the encoder and the loop; the postnet's scratch is sized below from the frames the loop produced
-            ws = _lib.workspace(dev, L.b200tts_tacotron2_workspace_bytes(h, b, tt, 0), "tacotron2")
+            ws = _lib.workspace(dev, getattr(L, f"b200tts_{m}_workspace_bytes")(h, b, tt, 0), m)
             wsp, wsn = _lib.ptr(ws), ctypes.c_size_t(ws.numel())
-            _lib.check(L.b200tts_tacotron2_encode(h, _lib.ptr(tok), _lib.ptr(lens), b, tt, _lib.ptr(enc), wsp, wsn, s),
-                       "tacotron2_encode")
-            _lib.check(L.b200tts_tacotron2_decode_loop(h, _lib.ptr(lens), _lib.ptr(enc), b, tt, r, max_steps,
-                                                       _lib.ptr(drop), CHUNK_STEPS, _lib.ptr(dec), _lib.ptr(stop),
-                                                       _lib.ptr(align), steps, wsp, wsn, s), "tacotron2_decode_loop")
+            _lib.check(getattr(L, f"b200tts_{m}_encode")(h, _lib.ptr(tok), _lib.ptr(lens), b, tt, _lib.ptr(enc), wsp,
+                                                         wsn, s), f"{m}_encode")
+            _lib.check(getattr(L, f"b200tts_{m}_decode_loop")(h, _lib.ptr(lens), _lib.ptr(enc), b, tt, r, max_steps,
+                                                              _lib.ptr(drop), CHUNK_STEPS, _lib.ptr(dec),
+                                                              _lib.ptr(stop), _lib.ptr(align), steps, wsp, wsn, s),
+                       f"{m}_decode_loop")
             n_steps = torch.tensor(list(steps), dtype=torch.int32)
             t_dec = int(n_steps.max())
             frames = (n_steps * r).to(dev)
-            mel = torch.empty((b, t_dec * r, c), **f32)
-            ws = _lib.workspace(dev, L.b200tts_tacotron2_workspace_bytes(h, b, tt, t_dec * r), "tacotron2")
+            out = torch.empty((b, t_dec * r, self.out_channels), **f32)
+            ws = _lib.workspace(dev, getattr(L, f"b200tts_{m}_workspace_bytes")(h, b, tt, t_dec * r), m)
             wsp, wsn = _lib.ptr(ws), ctypes.c_size_t(ws.numel())
-            _lib.check(L.b200tts_tacotron2_postnet(h, _lib.ptr(dec), _lib.ptr(frames), b, t_dec * r, max_steps * r,
-                                                   _lib.ptr(mel), wsp, wsn, s), "tacotron2_postnet")
-        return {"model_outputs": mel, "decoder_outputs": dec[:, :t_dec * r], "alignments": align[:, :t_dec],
+            _lib.check(getattr(L, f"b200tts_{m}_postnet")(h, _lib.ptr(dec), _lib.ptr(frames), b, t_dec * r,
+                                                          steps_cap * r, _lib.ptr(out), wsp, wsn, s), f"{m}_postnet")
+        return {"model_outputs": out, "decoder_outputs": dec[:, :t_dec * r], "alignments": align[:, :t_dec],
                 "stop_tokens": stop[:, :t_dec].unsqueeze(-1),
                 "model_outputs_len": (n_steps * r).to(device=dev, dtype=x_lengths.dtype)}
 
     # ------------------------------------------------------------------ out of scope
     def forward(self, *args, **kwargs):
-        raise NotImplementedError("tts_b200: Tacotron2 implements inference only; training (forward) is out of scope")
+        raise NotImplementedError(f"tts_b200: {_MODELS[self._model][0]} implements inference only; training (forward) is out of scope")
 
     # ------------------------------------------------------------------ checkpoints (base_tacotron.py:94-120)
     def load_checkpoint(self, config, checkpoint_path, eval=False, cache=False):  # pylint: disable=unused-argument, redefined-builtin
@@ -407,3 +350,62 @@ class Tacotron2(EngineModule):
         if eval:
             self.eval()
             assert not self.training
+
+
+class Tacotron2(_TacotronBase):
+    """Tacotron2 text -> mel synthesiser, inference path on sm_90a kernels."""
+
+    _destroy = "b200tts_tacotron2_destroy"
+    _model = "tacotron2"
+    _width = 512
+
+    def __init__(self, config, ap=None, tokenizer=None, speaker_manager=None):
+        super().__init__()
+        _check_config(config, self._model, self._width)
+        self.config, self.ap, self.tokenizer, self.speaker_manager = config, ap, tokenizer, speaker_manager
+        for key in config:
+            setattr(self, key, config[key])
+        if tokenizer is not None:   # BaseTTS._set_model_args
+            self.num_chars = tokenizer.characters.num_chars
+        self.decoder_output_dim = self.out_channels
+        self.embedding = nn.Embedding(self.num_chars, 512, padding_idx=0)
+        self.encoder = _Encoder(self.encoder_in_features)
+        self.decoder = _Decoder(self.decoder_in_features, self.out_channels, self.r, self.attention_type,
+                                self.prenet_type, self.location_attn)
+        self.postnet = _Postnet(self.out_channels)
+        if self.double_decoder_consistency:
+            self.coarse_decoder = _Decoder(self.decoder_in_features, self.out_channels, self.ddc_r,
+                                           self.attention_type, self.prenet_type, self.location_attn)
+
+    # ------------------------------------------------------------------ packing
+    def _create(self, device):
+        d = self.decoder
+        cfg = _lib.Tacotron2ConfigC(self.num_chars, self.out_channels, d.r_init,
+                                    int(self.attention_type == "dynamic_convolution"), int(bool(self.location_attn)),
+                                    int(self.attention_norm == "softmax"), int(self.prenet_type == "bn"),
+                                    int(bool(self.prenet_dropout)))
+        t = [_host(self.embedding.weight)]
+        for blk in list(self.encoder.convolutions):
+            t += self._conv_bn(blk)
+        for sfx in ("", "_reverse"):
+            t += [_host(getattr(self.encoder.lstm, f"{n}_l0{sfx}")) for n in ("weight_ih", "weight_hh", "bias_ih",
+                                                                              "bias_hh")]
+        for lin in d.prenet.linear_layers:
+            t += [_host(lin.linear_layer.weight)]
+            if self.prenet_type == "bn":
+                bn = lin.batch_normalization
+                t += [_host(bn.weight), _host(bn.bias), _host(bn.running_mean), _host(bn.running_var)]
+        t += self._cell(d.attention_rnn)
+        t += self._attention_weights(d.attention)
+        t += self._cell(d.decoder_rnn)
+        t += [_host(d.linear_projection.linear_layer.weight), _host(d.linear_projection.linear_layer.bias),
+              _host(d.stopnet[1].linear_layer.weight), _host(d.stopnet[1].linear_layer.bias)]
+        for blk in self.postnet.convolutions:
+            t += self._conv_bn(blk)
+        return self._make("b200tts_tacotron2_create", cfg, t)
+
+    @staticmethod
+    def _conv_bn(blk):
+        bn = blk.batch_normalization
+        return [_host(blk.convolution1d.weight), _host(blk.convolution1d.bias), _host(bn.weight), _host(bn.bias),
+                _host(bn.running_mean), _host(bn.running_var)]
