@@ -247,21 +247,25 @@ inline int conv_transpose_out_len(const ConvLayer& L, int Tin) {
 }
 
 // ------------------------------------------------------------------ bump allocator over a caller workspace
+// Every engine lays its scratch out with one carve, a function of (Arena&, shape); its workspace size is arena_size over
+// that same carve, so the layout is written once.  Blocks are 256-byte aligned.  ok() turns false at the first
+// allocation that does not fit and stays false, so a carve is checked once, after its last allocation.
 struct Arena {
     char* base; size_t cap; size_t off;
+    bool good = true;
     Arena(void* p, size_t bytes) : base((char*)p), cap(bytes), off(0) {}
-    float* f32(size_t n) {
-        size_t bytes = (n * sizeof(float) + 255) & ~size_t(255);
-        if (off + bytes > cap) return nullptr;
-        float* r = (float*)(base + off);
-        off += bytes;
+    // n raw bytes (a child component's workspace)
+    void* bytes(size_t n) {
+        const size_t b = (n + 255) & ~size_t(255);
+        if (!good || off + b > cap) { good = false; return nullptr; }
+        void* r = base + off;
+        off += b;
         return r;
     }
+    float* f32(size_t n) { return (float*)bytes(n * sizeof(float)); }
+    bool ok() const { return good; }
 };
-inline size_t arena_bytes(size_t n_floats) { return (n_floats * sizeof(float) + 255) & ~size_t(255); }
-// bytes an allocation sequence f(Arena&) takes from an Arena (a dry run over an unbounded one), so a workspace is sized
-// by the code that lays it out.  The dry run's first allocation is null: f must make every allocation before it checks
-// any of them.
+// bytes an allocation sequence f(Arena&) takes from an Arena (a dry run over an unbounded one)
 template <class F> size_t arena_size(F&& f) {
     Arena ar(nullptr, ~size_t(0) >> 1);
     f(ar);

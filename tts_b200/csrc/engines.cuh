@@ -46,7 +46,6 @@ struct WaveNet {
     std::vector<ConvLayer> in_layers, res_skip;
     int init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels,
              const float* const* w, int* consumed);
-    size_t scratch_floats(int B, int T) const;
     int forward(float* h, float* out, const float* mask, const float* g, int B, int T, float* acts, float* condv,
                 cudaStream_t st, const int* lens = nullptr) const;
 };
@@ -351,9 +350,12 @@ struct SeqEncoder {
     // w: emb [n_vocab, E]; per conv: weight [E, E, 5], bias, BN weight, bias, running_mean, running_var;
     // lstm weight_ih, weight_hh, bias_ih, bias_hh, then the same four _reverse
     int init(int n_vocab, int E, int H, int n_convs, const float* const* w, int* consumed);
-    size_t workspace_bytes(int B, int Tt) const;
-    // out [B, Tt, 2H], zero past each row's length; scratch from ar
-    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* out, Arena& ar,
+    // encode's scratch, carved by the parent model: the conv stack's two tensors and mask, the LSTM input projection,
+    // h (double-buffered) and c
+    struct Scratch { float *x, *y, *xmask, *pre, *hb, *cb; };
+    Scratch carve(Arena& ar, int B, int Tt) const;
+    // out [B, Tt, 2H], zero past each row's length
+    int encode(const long long* tokens, const long long* lengths, int B, int Tt, float* out, const Scratch& s,
                cudaStream_t st) const;
 };
 
@@ -395,8 +397,8 @@ struct TacoLoop {
     int *ctl, *done;
     size_t nzero;
 };
-// lays the state out from the arena's current offset; false when the arena runs out
-bool taco_loop_layout(Arena& ar, int B, int Tt, int RC, size_t nzero, TacoLoop& p);
+// lays the state out from the arena's current offset
+void taco_loop_layout(Arena& ar, int B, int Tt, int RC, size_t nzero, TacoLoop& p);
 // the loop's start: zeroes dec_out [B, S, rC], stop [B, S], align [B, S, Tt], cum and the zeroed region; alpha zero
 // (original attention) or one-hot at token 0 (one_hot: DCA); no row done, step 0
 int taco_loop_start(const TacoLoop& p, int B, int Tt, int S, int rC, int one_hot, float* dec_out, float* stop,
@@ -469,10 +471,12 @@ struct Tacotron {
         DevBuf<float> hw_w, hw_b;              // per highway [H | T] transposed [128][256], bias [256]
         DevBuf<float> whh, bhn;                // pack_bigru_whh images of both directions, b_hn [2][128]
         int init(int Cin, int K, int P1, const float* const* w, int* consumed);
-        size_t scratch_bytes(int B, int T) const;
+        // run's scratch, carved by the model: the bank and projection outputs, the highway output, the biGRU input
+        struct Scratch { float *bank, *y2, *y3, *hx, *pre; };
+        Scratch carve(Arena& ar, int B, int T) const;
         // x [B, Cin, T] (zero past each row) -> out as BiGruArgs describes it
         int run(const float* x, const float* mask, const int* lens32, const long long* lens64, int B, int T, float* out,
-                long long out_bs, int out_ts, int out_cs, Arena& ar, cudaStream_t st) const;
+                long long out_bs, int out_ts, int out_cs, const Scratch& s, cudaStream_t st) const;
     };
     b200tts_tacotron_config c;
     int Cm = 0;                                // prenet input width: C * memory_size (memory queue) or C

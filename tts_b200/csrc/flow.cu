@@ -38,10 +38,6 @@ int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers
     return 0;
 }
 
-size_t WaveNet::scratch_floats(int B, int T) const {
-    return (size_t)B * H * T + (size_t)B * cond.RowsPad + 64;  // acts + per-utterance cond vector
-}
-
 // h [B,H,T] (masked, updated in place), out [B,H,T] <- WN(h) * mask
 int WaveNet::forward(float* h, float* out, const float* mask, const float* g, int B, int T, float* acts,
                      float* condv, cudaStream_t st, const int* lens) const {
@@ -113,9 +109,20 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
     return 0;
 }
 
+// the scratch of a hidden-width stage around one WaveNet (Flow, PosteriorEnc): its input h, the gated activations, its
+// output and the per-utterance cond vector
+struct WnWs { float *h, *acts, *out, *condv; };
+static WnWs wn_carve(const WaveNet& wn, Arena& ar, int B, int T) {
+    WnWs w;
+    w.h = ar.f32((size_t)B * wn.H * T);
+    w.acts = ar.f32((size_t)B * wn.H * T);
+    w.out = ar.f32((size_t)B * wn.H * T);
+    w.condv = ar.f32((size_t)B * wn.cond.RowsPad + 64);
+    return w;
+}
+
 size_t Flow::workspace_bytes(int B, int T) const {
-    const size_t hb = arena_bytes((size_t)B * c.hidden_channels * T);
-    return 3 * hb + arena_bytes((size_t)B * blocks[0].wn.cond.RowsPad + 64) + 1024;
+    return arena_size([&](Arena& ar) { wn_carve(blocks[0].wn, ar, B, T); });
 }
 
 int Flow::reverse(float* z, const float* mask, const float* g, int B, int T, void* ws, size_t ws_bytes,
@@ -125,15 +132,13 @@ int Flow::reverse(float* z, const float* mask, const float* g, int B, int T, voi
     //  x1 = m + x1*mask instead of x1 = (x1 - m)*mask)
     B200_REQUIRE(c.cond_channels == 0 || g != nullptr, "flow_reverse: model has cond_channels=%d but g is null",
                  c.cond_channels);
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "flow_reverse: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "flow_reverse: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
     Arena ar(ws, ws_bytes);
+    const WnWs w = wn_carve(blocks[0].wn, ar, B, T);
+    float *h = w.h, *acts = w.acts, *out = w.out, *condv = w.condv;
     const int H = c.hidden_channels, half = c.channels / 2;
-    float* h = ar.f32((size_t)B * H * T);
-    float* acts = ar.f32((size_t)B * H * T);
-    float* out = ar.f32((size_t)B * H * T);
-    float* condv = ar.f32((size_t)B * blocks[0].wn.cond.RowsPad + 64);
-    B200_REQUIRE(h && acts && out && condv, "flow_reverse: arena exhausted");
     const long long zbs = (long long)c.channels * T;
     int rc;
     for (int step = 0; step < c.num_flows; ++step) {
@@ -193,22 +198,20 @@ int PosteriorEnc::init(const b200tts_posterior_config& cfg, const float* const* 
 }
 
 size_t PosteriorEnc::workspace_bytes(int B, int T) const {
-    return 3 * arena_bytes((size_t)B * c.hidden_channels * T) + arena_bytes((size_t)B * wn.cond.RowsPad + 64) + 1024;
+    return arena_size([&](Arena& ar) { wn_carve(wn, ar, B, T); });
 }
 
 int PosteriorEnc::forward(const float* x, const float* mask, const float* g, const float* noise, int B, int T, float* z,
                           float* stats, void* ws, size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(x && mask && noise && z && stats && ws, "posterior_encoder: null pointer");
     B200_REQUIRE(c.cond_channels == 0 || g != nullptr, "posterior_encoder: model has cond_channels=%d but g is null", c.cond_channels);
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "posterior_encoder: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "posterior_encoder: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
     Arena ar(ws, ws_bytes);
+    const WnWs w = wn_carve(wn, ar, B, T);
+    float *h = w.h, *acts = w.acts, *out = w.out, *condv = w.condv;
     const int H = c.hidden_channels;
-    float* h = ar.f32((size_t)B * H * T);
-    float* acts = ar.f32((size_t)B * H * T);
-    float* out = ar.f32((size_t)B * H * T);
-    float* condv = ar.f32((size_t)B * wn.cond.RowsPad + 64);
-    B200_REQUIRE(h && acts && out && condv, "posterior_encoder: arena exhausted");
     int rc;
     {
         ConvIO io;

@@ -197,22 +197,45 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
     return pack_conv(postnet, w[i], w[i + 1], c.out_channels, C, 1, 1, 0);
 }
 
+// the encoder layers' scratch, the projected speaker vector and one block the duration, pitch and energy predictors
+// take in turn
+struct FttsEncWs { float *qkv, *att, *yb, *hb, *gp; void* dp; size_t dp_bytes; };
+static FttsEncWs ftts_encode_carve(const ForwardTTS& m, Arena& ar, int B, int Tt) {
+    const int C = m.c.hidden_channels;
+    FttsEncWs w;
+    w.qkv = ar.f32((size_t)B * 3 * C * Tt);
+    w.att = ar.f32((size_t)B * C * Tt);
+    w.yb = ar.f32((size_t)B * C * Tt);
+    w.hb = ar.f32((size_t)B * m.c.enc_ffn * Tt);
+    w.gp = ar.f32((size_t)B * C);
+    w.dp_bytes = m.dp.workspace_bytes(B, Tt);
+    if (m.c.use_pitch) w.dp_bytes = std::max(w.dp_bytes, m.pitch_dp.workspace_bytes(B, Tt));
+    if (m.c.use_energy) w.dp_bytes = std::max(w.dp_bytes, m.energy_dp.workspace_bytes(B, Tt));
+    w.dp = ar.bytes(w.dp_bytes);
+    return w;
+}
+
 size_t ForwardTTS::encode_bytes(int B, int Tt) const {
-    const int C = c.hidden_channels;
-    size_t dpb = dp.workspace_bytes(B, Tt);
-    if (c.use_pitch) dpb = std::max(dpb, pitch_dp.workspace_bytes(B, Tt));
-    if (c.use_energy) dpb = std::max(dpb, energy_dp.workspace_bytes(B, Tt));
-    return arena_bytes((size_t)B * 3 * C * Tt) + 2 * arena_bytes((size_t)B * C * Tt) +
-           arena_bytes((size_t)B * c.enc_ffn * Tt) + arena_bytes((size_t)B * C) + arena_bytes(dpb / sizeof(float) + 1) +
-           1024;
+    return arena_size([&](Arena& ar) { ftts_encode_carve(*this, ar, B, Tt); });
+}
+
+struct FttsDecWs { float *x, *qkv, *att, *yb, *hb, *pm, *ymask; int* lens; };
+static FttsDecWs ftts_decode_carve(const ForwardTTS& m, Arena& ar, int B, int Ty) {
+    const size_t C = m.c.hidden_channels, Tp = ForwardTTS::tp(Ty);
+    FttsDecWs w;
+    w.x = ar.f32(B * C * Tp);
+    w.qkv = ar.f32(B * 3 * C * Tp);
+    w.att = ar.f32(B * C * Tp);
+    w.yb = ar.f32(B * C * Tp);
+    w.hb = ar.f32(B * m.c.dec_ffn * Tp);
+    w.pm = ar.f32(B * m.c.out_channels * Tp);
+    w.ymask = ar.f32(B * Tp);
+    w.lens = reinterpret_cast<int*>(ar.f32((size_t)B));
+    return w;
 }
 
 size_t ForwardTTS::decode_bytes(int B, int Ty) const {
-    const int C = c.hidden_channels;
-    const size_t Tp = (size_t)tp(Ty);
-    return 3 * arena_bytes((size_t)B * C * Tp) + arena_bytes((size_t)B * 3 * C * Tp) +
-           arena_bytes((size_t)B * c.dec_ffn * Tp) + arena_bytes((size_t)B * c.out_channels * Tp) +
-           arena_bytes((size_t)B * Tp) + arena_bytes((size_t)B) + 1024;
+    return arena_size([&](Arena& ar) { ftts_decode_carve(*this, ar, B, Ty); });
 }
 
 int ForwardTTS::encode(const long long* tokens, const long long* lengths, const float* g, float length_scale, int B,
@@ -223,20 +246,13 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
                  "forward_tts_encode: null pointer");
     B200_REQUIRE(!c.use_pitch || pitch, "forward_tts_encode: the pitch predictor needs a pitch output");
     B200_REQUIRE(!c.use_energy || energy, "forward_tts_encode: the energy predictor needs an energy output");
-    B200_REQUIRE(ws_bytes >= encode_bytes(B, Tt), "forward_tts_encode: workspace too small");
+    const size_t need = encode_bytes(B, Tt);
+    B200_REQUIRE(ws_bytes >= need, "forward_tts_encode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || Tt == 0) return 0;
     const int C = c.hidden_channels, F = c.enc_ffn;
     Arena ar(ws, ws_bytes);
-    float* qkv = ar.f32((size_t)B * 3 * C * Tt);
-    float* att = ar.f32((size_t)B * C * Tt);
-    float* yb = ar.f32((size_t)B * C * Tt);
-    float* hb = ar.f32((size_t)B * F * Tt);
-    float* gp = ar.f32((size_t)B * C);
-    size_t dpb = dp.workspace_bytes(B, Tt);
-    if (c.use_pitch) dpb = std::max(dpb, pitch_dp.workspace_bytes(B, Tt));
-    if (c.use_energy) dpb = std::max(dpb, energy_dp.workspace_bytes(B, Tt));
-    float* dpws = ar.f32(dpb / sizeof(float) + 1);
-    B200_REQUIRE(qkv && att && yb && hb && gp && dpws, "forward_tts_encode: arena exhausted");
+    const FttsEncWs w = ftts_encode_carve(*this, ar, B, Tt);
+    float *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb, *gp = w.gp;
     const long long bs = (long long)C * Tt;
     float* x = o_en;
     int rc;
@@ -289,14 +305,14 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
         B200_CUDA_OK(cudaGetLastError());
     }
     // the duration predictor sees o_en with g, before any pitch (forward_tts.py:691)
-    if ((rc = dp.forward(x, x_mask, nullptr, nullptr, B, Tt, logw, dpws, dpb, st))) return rc;
+    if ((rc = dp.forward(x, x_mask, nullptr, nullptr, B, Tt, logw, w.dp, w.dp_bytes, st))) return rc;
     // pitch, then energy on o_en that already holds the pitch embedding: o_en += emb(pred) (:697-704)
     const DurPred* preds[2] = {c.use_pitch ? &pitch_dp : nullptr, c.use_energy ? &energy_dp : nullptr};
     const ConvLayer* embs[2] = {&pitch_emb, &energy_emb};
     float* outs[2] = {pitch, energy};
     for (int p = 0; p < 2; ++p) {
         if (!preds[p]) continue;
-        if ((rc = preds[p]->forward(x, x_mask, nullptr, nullptr, B, Tt, outs[p], dpws, dpb, st))) return rc;
+        if ((rc = preds[p]->forward(x, x_mask, nullptr, nullptr, B, Tt, outs[p], w.dp, w.dp_bytes, st))) return rc;
         ConvIO io;
         io.x = outs[p]; io.x_bs = Tt; io.x_cs = Tt; io.Tin = Tt;
         io.y = x; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
@@ -311,19 +327,14 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
     B200_REQUIRE(o_en && x_mask && cum && y_lengths && mel && ws, "forward_tts_decode: null pointer");
     B200_REQUIRE(c.pe_len == 0 || Ty <= c.pe_len,
                  "forward_tts_decode: sequence is %d frames but the positional encoding is limited to %d", Ty, c.pe_len);
-    B200_REQUIRE(ws_bytes >= decode_bytes(B, Ty), "forward_tts_decode: workspace too small");
+    const size_t need = decode_bytes(B, Ty);
+    B200_REQUIRE(ws_bytes >= need, "forward_tts_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || Ty == 0) return 0;
     const int C = c.hidden_channels, F = c.dec_ffn, Co = c.out_channels, Tp = tp(Ty);
     Arena ar(ws, ws_bytes);
-    float* x = ar.f32((size_t)B * C * Tp);
-    float* qkv = ar.f32((size_t)B * 3 * C * Tp);
-    float* att = ar.f32((size_t)B * C * Tp);
-    float* yb = ar.f32((size_t)B * C * Tp);
-    float* hb = ar.f32((size_t)B * F * Tp);
-    float* pm = ar.f32((size_t)B * Co * Tp);
-    float* ymask = ar.f32((size_t)B * Tp);
-    int* lens = reinterpret_cast<int*>(ar.f32((size_t)B));
-    B200_REQUIRE(x && qkv && att && yb && hb && pm && ymask && lens, "forward_tts_decode: arena exhausted");
+    const FttsDecWs w = ftts_decode_carve(*this, ar, B, Ty);
+    float *x = w.x, *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb, *pm = w.pm, *ymask = w.ymask;
+    int* lens = w.lens;
     int rc;
     {
         dim3 grid((Tp + 127) / 128, B);

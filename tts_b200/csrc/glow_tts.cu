@@ -133,21 +133,28 @@ int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilatio
     return 0;
 }
 
+struct GlowDecWs { float *zb, *eo, *h, *acts, *out, *condv; };
+static GlowDecWs glowdec_carve(const GlowDecoder& m, Arena& ar, int B, int Tq) {
+    GlowDecWs w;
+    w.zb = ar.f32((size_t)B * m.Cs * Tq);
+    w.eo = ar.f32((size_t)B * m.Cs * Tq);
+    w.h = ar.f32((size_t)B * m.Hd * Tq);
+    w.acts = ar.f32((size_t)B * m.Hd * Tq);
+    w.out = ar.f32((size_t)B * m.Hd * Tq);
+    w.condv = ar.f32((size_t)B * m.blocks[0].wn.cond.RowsPad + 64);
+    return w;
+}
+
 size_t GlowDecoder::workspace_bytes(int B, int Tq) const {
-    return 2 * arena_bytes((size_t)B * Cs * Tq) + 3 * arena_bytes((size_t)B * Hd * Tq) +
-           arena_bytes((size_t)B * blocks[0].wn.cond.RowsPad + 64);
+    return arena_size([&](Arena& ar) { glowdec_carve(*this, ar, B, Tq); });
 }
 
 int GlowDecoder::reverse(float* z, const float* msk, const float* g, int B, int Tq, int Tv, float* mel, void* ws,
                          size_t ws_bytes, cudaStream_t st) const {
     Arena ar(ws, ws_bytes);
-    float* zb = ar.f32((size_t)B * Cs * Tq);
-    float* eo = ar.f32((size_t)B * Cs * Tq);
-    float* h = ar.f32((size_t)B * Hd * Tq);
-    float* acts = ar.f32((size_t)B * Hd * Tq);
-    float* out = ar.f32((size_t)B * Hd * Tq);
-    float* condv = ar.f32((size_t)B * blocks[0].wn.cond.RowsPad + 64);
-    B200_REQUIRE(zb && eo && h && acts && out && condv, "glow decoder: arena exhausted");
+    const GlowDecWs w = glowdec_carve(*this, ar, B, Tq);
+    B200_REQUIRE(ar.ok(), "glow decoder: workspace of %zu bytes is too small", ws_bytes);
+    float *zb = w.zb, *eo = w.eo, *h = w.h, *acts = w.acts, *out = w.out, *condv = w.condv;
     int rc;
     const long long zbs = (long long)Cs * Tq, hbs = (long long)Hd * Tq;
     float* cur = z;
@@ -237,15 +244,41 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
     return 0;
 }
 
+// x, cat(x, g), the duration predictor's and the transformer's blocks; the prenet runs before the transformer, so its
+// two buffers are the transformer's scratch (which holds q|k|v alone, 3 B H Tt floats)
+struct GlowEncWs { float *x, *xdp, *pre[2]; void *dp, *tf; size_t dp_bytes, tf_bytes; };
+static GlowEncWs glow_encode_carve(const GlowTTS& m, Arena& ar, int B, int Tt) {
+    const int H = m.c.hidden_channels_enc;
+    GlowEncWs w;
+    w.x = ar.f32((size_t)B * H * Tt);
+    w.xdp = ar.f32((size_t)B * (H + m.c.c_in_channels) * Tt);
+    w.dp_bytes = m.dp.workspace_bytes(B, Tt);
+    w.dp = ar.bytes(w.dp_bytes);
+    w.tf_bytes = m.tf.workspace_bytes(B, Tt);
+    w.tf = ar.bytes(w.tf_bytes);
+    Arena pa(w.tf, w.tf_bytes);
+    w.pre[0] = pa.f32((size_t)B * H * Tt);
+    w.pre[1] = pa.f32((size_t)B * H * Tt);
+    return w;
+}
+
 size_t GlowTTS::encode_bytes(int B, int Tt) const {
-    const int H = c.hidden_channels_enc, Cg = H + c.c_in_channels;
-    return arena_bytes((size_t)B * H * Tt) + arena_bytes((size_t)B * Cg * Tt) +
-           arena_bytes(dp.workspace_bytes(B, Tt) / sizeof(float) + 1) + tf.workspace_bytes(B, Tt) + 1024;
+    return arena_size([&](Arena& ar) { glow_encode_carve(*this, ar, B, Tt); });
+}
+
+// the squeezed latent, its mask and the Glow decoder's block
+struct GlowDecodeWs { float *za, *msk; void* dec; size_t dec_bytes; };
+static GlowDecodeWs glow_decode_carve(const GlowTTS& m, Arena& ar, int B, int Tq) {
+    GlowDecodeWs w;
+    w.za = ar.f32((size_t)B * m.Cs * Tq);
+    w.msk = ar.f32((size_t)B * Tq);
+    w.dec_bytes = m.dec.workspace_bytes(B, Tq);
+    w.dec = ar.bytes(w.dec_bytes);
+    return w;
 }
 
 size_t GlowTTS::decode_bytes(int B, int Ty) const {
-    const int Tq = tq(Ty);
-    return arena_bytes((size_t)B * Cs * Tq) + arena_bytes((size_t)B * Tq) + dec.workspace_bytes(B, Tq) + 1024;
+    return arena_size([&](Arena& ar) { glow_decode_carve(*this, ar, B, tq(Ty)); });
 }
 
 int GlowTTS::encode(const long long* tokens, const long long* lengths, const float* g, float length_scale, int B,
@@ -254,27 +287,21 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
     B200_REQUIRE(tokens && lengths && o_stats && logw && x_mask && w_ceil && cum && dur_log && y_lengths && ws,
                  "glow_tts_encode: null pointer");
     B200_REQUIRE((c.c_in_channels > 0) == (g != nullptr), "glow_tts_encode: g must be given iff c_in_channels > 0");
-    B200_REQUIRE(ws_bytes >= encode_bytes(B, Tt), "glow_tts_encode: workspace too small");
+    const size_t need = encode_bytes(B, Tt);
+    B200_REQUIRE(ws_bytes >= need, "glow_tts_encode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || Tt == 0) return 0;
     const int H = c.hidden_channels_enc, Cg = H + c.c_in_channels;
     Arena ar(ws, ws_bytes);
-    float* x = ar.f32((size_t)B * H * Tt);
-    float* xdp = ar.f32((size_t)B * Cg * Tt);
-    const size_t dp_bytes = dp.workspace_bytes(B, Tt);
-    float* dpws = ar.f32(dp_bytes / sizeof(float) + 1);
-    const size_t tf_bytes = tf.workspace_bytes(B, Tt);
-    float* tfws = ar.f32(tf_bytes / sizeof(float));
-    B200_REQUIRE(x && xdp && dpws && tfws, "glow_tts_encode: arena exhausted");
+    const GlowEncWs w = glow_encode_carve(*this, ar, B, Tt);
+    float *x = w.x, *xdp = w.xdp;
     const long long bs = (long long)H * Tt;
     int rc;
     // x = emb(tokens) * sqrt(H), masked: the prenet and the transformer both start with x * x_mask
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, H, H, x, x_mask, st))) return rc;
     if (c.use_prenet) {   // glow.py:55-67: 3 x (conv(x * mask) -> LayerNorm(. * mask) -> ReLU), x = (x + proj(.)) * mask
-        Arena pa(tfws, tf_bytes);   // the prenet runs before the transformer: its buffers are the transformer's scratch
         const float* in = x;
-        float* bufs[2] = {pa.f32((size_t)B * H * Tt), pa.f32((size_t)B * H * Tt)};
         for (int l = 0; l < 3; ++l) {
-            float* out = bufs[l & 1];
+            float* out = w.pre[l & 1];
             ConvIO io;
             io.x = in; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
             if (l > 0) io.in_slope = 0.f;   // the previous layer's ReLU, applied to its masked output
@@ -291,7 +318,7 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
         io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_ACCUM | EPI_MASK_POST;
         if ((rc = launch_conv(prenet_proj, io, st))) return rc;
     }
-    if ((rc = tf.forward(x, x_mask, B, Tt, tfws, tf_bytes, st))) return rc;
+    if ((rc = tf.forward(x, x_mask, B, Tt, w.tf, w.tf_bytes, st))) return rc;
     {   // o_mean = proj_m(x) * mask, o_log_scale = proj_s(x) * mask (encoder.py:172-176)
         ConvIO io;
         io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
@@ -307,7 +334,7 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
         B200_CUDA_OK(cudaGetLastError());
         dp_in = xdp;
     }
-    if ((rc = dp.forward(dp_in, x_mask, nullptr, nullptr, B, Tt, logw, dpws, dp_bytes, st))) return rc;
+    if ((rc = dp.forward(dp_in, x_mask, nullptr, nullptr, B, Tt, logw, w.dp, w.dp_bytes, st))) return rc;
     return launch_durations_glow(logw, x_mask, length_scale, B, Tt, w_ceil, cum, y_lengths, dur_log, meta, st);
 }
 
@@ -317,28 +344,27 @@ int GlowTTS::decode(const float* o_stats, const float* x_mask, const float* cum,
     B200_REQUIRE(o_stats && x_mask && cum && y_lengths && y_mean && y_log_scale && mel && ws,
                  "glow_tts_decode: null pointer");
     B200_REQUIRE((c.c_in_channels > 0) == (g != nullptr), "glow_tts_decode: g must be given iff c_in_channels > 0");
-    B200_REQUIRE(ws_bytes >= decode_bytes(B, Ty), "glow_tts_decode: workspace too small");
+    const size_t need = decode_bytes(B, Ty);
+    B200_REQUIRE(ws_bytes >= need, "glow_tts_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || Ty == 0) return 0;
     const int C = c.out_channels, nsq = c.num_squeeze;
+    const int Tv = Ty / nsq, Tq = tq(Ty);
+    Arena ar(ws, ws_bytes);
+    const GlowDecodeWs w = glow_decode_carve(*this, ar, B, Tq);
     int rc;
     // path and expanded prior (:355-359): attn, y_mean = attn^T o_mean, y_log_scale = attn^T o_log_scale
     if ((rc = launch_expand_prior(cum, x_mask, y_lengths, o_stats, nullptr, 0.f, B, Tt, Ty, C, attn, y_mean, y_log_scale,
                                   nullptr, nullptr, st)))
         return rc;
-    const int Tv = Ty / nsq, Tq = tq(Ty);
     if (Tv == 0) return 0;
-    Arena ar(ws, ws_bytes);
-    float* za = ar.f32((size_t)B * Cs * Tq);
-    float* msk = ar.f32((size_t)B * Tq);
-    B200_REQUIRE(za && msk, "glow_tts_decode: arena exhausted");
     {
         dim3 grid((Tq + 127) / 128, Cs, B);
         squeeze_prior_kernel<<<grid, 128, 0, st>>>(y_mean, y_log_scale, noise_scale != 0.f ? noise : nullptr,
-                                                   noise_scale, y_lengths, za, msk, C, Ty, nsq, Tv, Tq);
+                                                   noise_scale, y_lengths, w.za, w.msk, C, Ty, nsq, Tv, Tq);
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
     }
-    return dec.reverse(za, msk, g, B, Tq, Tv, mel, ar.base + ar.off, ar.cap - ar.off, st);
+    return dec.reverse(w.za, w.msk, g, B, Tq, Tv, mel, w.dec, w.dec_bytes, st);
 }
 
 }  // namespace b200tts

@@ -269,11 +269,25 @@ int GriffinLim::init(int n_fft_, int hop_, const float* window_host, const float
     return 0;
 }
 
+// the magnitudes, two waveforms, the non-finite row flags; mel input also takes the denormalised mel (amp) and its
+// linear projection (lin)
+struct GlWs { float *mag, *y[2], *amp, *lin; int* bad; };
+static GlWs gl_carve(const GriffinLim& m, Arena& ar, int B, int T) {
+    const size_t F = m.n_fft / 2 + 1, BT = (size_t)B * T, L = (size_t)m.hop * (size_t)std::max(T - 1, 0);
+    GlWs w{};
+    w.mag = ar.f32(BT * F);
+    w.y[0] = ar.f32((size_t)B * L);
+    w.y[1] = ar.f32((size_t)B * L);
+    w.bad = (int*)ar.f32(B);
+    if (m.n_mels) {
+        w.amp = ar.f32(BT * m.n_mels);
+        w.lin = ar.f32(BT * F);
+    }
+    return w;
+}
+
 size_t GriffinLim::workspace_bytes(int B, int T) const {
-    const size_t F = n_fft / 2 + 1, BT = (size_t)B * T, L = (size_t)hop * (size_t)std::max(T - 1, 0);
-    size_t n = arena_bytes(BT * F) + 2 * arena_bytes((size_t)B * L) + arena_bytes(B);
-    if (n_mels) n += arena_bytes(BT * n_mels) + arena_bytes(BT * F);
-    return n;
+    return arena_size([&](Arena& ar) { gl_carve(*this, ar, B, T); });
 }
 
 int GriffinLim::forward(const float* x, long long x_bs, int x_cs, int x_ts, int B, int C, int T, const int* lens,
@@ -290,13 +304,14 @@ int GriffinLim::forward(const float* x, long long x_bs, int x_cs, int x_ts, int 
                  "griffin_lim_forward: output pitch %lld < %lld samples", wav_pitch, (long long)hop * (T - 1));
     B200_REQUIRE(base >= 0.f && spec_gain != 0.f, "griffin_lim_forward: base=%f spec_gain=%f", (double)base,
                  (double)spec_gain);
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "griffin_lim_forward: workspace %zu < %zu bytes", ws_bytes,
-                 workspace_bytes(B, T));
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "griffin_lim_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const long long L = (long long)hop * (T - 1);
     Arena ar(ws, ws_bytes);
-    float* mag = ar.f32((size_t)B * T * F);
-    float* y[2] = {ar.f32((size_t)B * L), ar.f32((size_t)B * L)};
-    int* bad = (int*)ar.f32(B);
+    const GlWs w = gl_carve(*this, ar, B, T);
+    float *mag = w.mag, *amp = w.amp, *lin = w.lin;
+    float* const* y = w.y;
+    int* bad = w.bad;
     const NormParams np = to_params(norm);
     const dim3 tblk(32, 8);
     if (!n_mels) {
@@ -306,8 +321,6 @@ int GriffinLim::forward(const float* x, long long x_bs, int x_cs, int x_ts, int 
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
     } else {
-        float* amp = ar.f32((size_t)B * T * n_mels);
-        float* lin = ar.f32((size_t)B * T * F);
         dispatch_note(DISPATCH_GL_PREPARE);
         gl_prepare_kernel<<<dim3((T + 31) / 32, (C + 31) / 32, B), tblk, 0, st>>>(
             x, x_bs, x_cs, x_ts, C, T, lens, np, base, spec_gain, power, GL_DENORM_AMP, amp, (long long)n_mels * T, T, 1);

@@ -125,17 +125,28 @@ void Hifigan::stage_dims(int T, std::vector<int>& C, std::vector<int>& L) const 
     }
 }
 
-size_t Hifigan::workspace_bytes(int B, int T) const {
+struct HifiganWs { float *P, *Xp, *U, *T1, *R, *OUT, *condv; };
+
+// P: conv_pre's output, Xp: the re-pitched input, U / T1 / R / OUT: the stage tensors (the largest stage each)
+static HifiganWs hifigan_carve(const Hifigan& m, Arena& ar, int B, int T) {
     std::vector<int> C, L;
-    stage_dims(T, C, L);
+    m.stage_dims(T, C, L);
     size_t mx = 0;
     for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)L[s]);
     const size_t Tp = (size_t)(T + 3) / 4 * 4;    // 16-byte aligned row pitch for the stage-0 tensors
-    size_t tot = arena_bytes((size_t)B * c.upsample_initial_channel * Tp);
-    tot += arena_bytes((size_t)B * c.in_channels * Tp);
-    tot += 4 * arena_bytes((size_t)B * mx);
-    tot += arena_bytes((size_t)B * cond.RowsPad + 64);
-    return tot;
+    HifiganWs w;
+    w.P = ar.f32((size_t)B * m.c.upsample_initial_channel * Tp);
+    w.Xp = ar.f32((size_t)B * m.c.in_channels * Tp);
+    w.U = ar.f32((size_t)B * mx);
+    w.T1 = ar.f32((size_t)B * mx);
+    w.R = ar.f32((size_t)B * mx);
+    w.OUT = ar.f32((size_t)B * mx);
+    w.condv = ar.f32((size_t)B * m.cond.RowsPad + 64);
+    return w;
+}
+
+size_t Hifigan::workspace_bytes(int B, int T) const {
+    return arena_size([&](Arena& ar) { hifigan_carve(*this, ar, B, T); });
 }
 
 int Hifigan::out_len(int T) const {
@@ -161,7 +172,8 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
     B200_REQUIRE(x && wav && ws, "hifigan_forward: null pointer");
     B200_REQUIRE((c.cond_channels > 0) == (g != nullptr) || c.cond_channels == 0,
                  "hifigan_forward: model has cond_channels=%d but g is null", c.cond_channels);
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "hifigan_forward: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "hifigan_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (frame_end < 0) frame_end = T;
     const bool windowed = frame_begin != 0 || frame_end != T;
     B200_REQUIRE(!windowed || (0 <= frame_begin && frame_begin < frame_end && frame_end <= T),
@@ -183,22 +195,14 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
         io.in_lo = (int)std::max(0LL, fb * io.rate_in - io.need_in);
         io.in_hi = (int)std::min(0x7fffffffLL, fe * io.rate_in + io.need_in);
     };
-    size_t mx = 0;
-    for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)L[s]);
     Arena ar(ws, ws_bytes);
+    const HifiganWs w = hifigan_carve(*this, ar, B, T);
+    float *P = w.P, *Xp = w.Xp, *U = w.U, *T1 = w.T1, *R = w.R, *OUT = w.OUT, *condv = w.condv;
     const int C0 = c.upsample_initial_channel;
     // The tensor-core kernels stage activation rows with 16-byte cp.async: rows must start 16-byte aligned.  T (decoder frames)
     // is arbitrary, so the stage-0 tensors use a row pitch rounded up to 4 floats and an unaligned input is re-pitched
     // once (B x Cin x T floats, tiny) -- otherwise conv_pre / ups[0] would silently take the FP32-FMA kernel for 3 of 4 T.
     const int Tp = (T + 3) / 4 * 4;
-    float* P = ar.f32((size_t)B * C0 * Tp);
-    float* Xp = ar.f32((size_t)B * c.in_channels * Tp);
-    float* U = ar.f32((size_t)B * mx);
-    float* T1 = ar.f32((size_t)B * mx);
-    float* R = ar.f32((size_t)B * mx);
-    float* OUT = ar.f32((size_t)B * mx);
-    float* condv = ar.f32((size_t)B * cond.RowsPad + 64);
-    B200_REQUIRE(P && Xp && U && T1 && R && OUT && condv, "hifigan_forward: arena exhausted");
     const float* xin0 = x;
     int x_pitch = T;
     if (Tp != T || (reinterpret_cast<uintptr_t>(x) & 15) != 0) {

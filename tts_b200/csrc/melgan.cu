@@ -153,14 +153,26 @@ int Melgan::out_len(int T) const {
     return L.back();
 }
 
-size_t Melgan::workspace_bytes(int B, int T) const {
+// Xp: the re-pitched input, P: conv_pre's output, X / Y: the stage tensors (the largest stage each), H: the residual
+// stacks' hidden tensors
+struct MelganWs { float *Xp, *P, *X, *Y, *H; };
+static MelganWs melgan_carve(const Melgan& m, Arena& ar, int B, int T) {
     std::vector<int> C, L;
-    stage_dims(T, C, L);
+    m.stage_dims(T, C, L);
     size_t mx = 0;
     for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)round4(L[s]));
     const size_t Tp = (size_t)round4(T);
-    return arena_bytes((size_t)B * c.in_channels * Tp) + arena_bytes((size_t)B * c.base_channels * Tp) +
-           2 * arena_bytes((size_t)B * mx) + arena_bytes((size_t)B * h_floats(c, C, L));
+    MelganWs w;
+    w.Xp = ar.f32((size_t)B * m.c.in_channels * Tp);
+    w.P = ar.f32((size_t)B * m.c.base_channels * Tp);
+    w.X = ar.f32((size_t)B * mx);
+    w.Y = ar.f32((size_t)B * mx);
+    w.H = ar.f32((size_t)B * h_floats(m.c, C, L));
+    return w;
+}
+
+size_t Melgan::workspace_bytes(int B, int T) const {
+    return arena_size([&](Arena& ar) { melgan_carve(*this, ar, B, T); });
 }
 
 int Melgan::check_len(int T) const {
@@ -187,19 +199,14 @@ int Melgan::forward(const float* x, int B, int T, int synthesize, float* out, un
     B200_REQUIRE(B >= 0, "melgan_forward: B = %d", B);
     if (B == 0) return 0;
     if (int rc = check_len(T)) return rc;
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "melgan_forward: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "melgan_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
     std::vector<int> C, L;
     stage_dims(T, C, L);
-    size_t mx = 0;
-    for (size_t s = 0; s < C.size(); ++s) mx = std::max(mx, (size_t)C[s] * (size_t)round4(L[s]));
     const int Tp = round4(T), C0 = c.base_channels;
     Arena ar(ws, ws_bytes);
-    float* Xp = ar.f32((size_t)B * c.in_channels * Tp);
-    float* P = ar.f32((size_t)B * C0 * Tp);
-    float* X = ar.f32((size_t)B * mx);
-    float* Y = ar.f32((size_t)B * mx);
-    float* H = ar.f32((size_t)B * h_floats(c, C, L));
-    B200_REQUIRE(Xp && P && X && Y && H, "melgan_forward: arena exhausted");
+    const MelganWs w = melgan_carve(*this, ar, B, T);
+    float *Xp = w.Xp, *P = w.P, *X = w.X, *Y = w.Y, *H = w.H;
     // 16-byte aligned input rows for the tensor-core producers: re-pitch an unaligned input once (B x in x T floats)
     const float* xin = x;
     int x_pitch = T;

@@ -110,7 +110,7 @@ struct Persist {   // the part of the workspace that lives from encode to sample
 
 }  // namespace
 
-static bool persist_layout(const Overflow& e, Arena& ar, int B, int Tt, Persist& p) {
+static void persist_layout(const Overflow& e, Arena& ar, int B, int Tt, Persist& p) {
     const auto& c = e.c;
     int omax = 0;
     for (int l = 0; l < c.outputnet_n_layers; ++l) omax = std::max(omax, c.outputnet_size[l]);
@@ -126,14 +126,30 @@ static bool persist_layout(const Overflow& e, Arena& ar, int B, int Tt, Persist&
     p.pb = ar.f32((size_t)2 * B * c.prenet_dim);
     p.hid = ar.f32((size_t)2 * B * omax);
     p.outp = ar.f32((size_t)B * (2 * c.out_channels + 1));
-    return p.zc && p.ctl && p.state && p.done && p.quant && p.hm && p.cm && p.pin && p.pb && p.hid && p.outp;
 }
 
-static void decode_scratch(const Overflow& e, Arena& ar, int B, int Tq, float** za, float** msk, float** melc) {
+// encode: the state kept until sample() ends, the encoder's scratch and the transposed encoder states
+struct EncodeWs { Persist p; SeqEncoder::Scratch enc; float* encT; };
+static EncodeWs encode_carve(const Overflow& e, Arena& ar, int B, int Tt) {
+    EncodeWs w;
+    persist_layout(e, ar, B, Tt, w.p);
+    w.enc = e.enc.carve(ar, B, Tt);
+    w.encT = ar.f32((size_t)B * e.c.encoder_dim * Tt * e.c.state_per_phone);
+    return w;
+}
+
+// decode (Overflow only), from the start of the workspace once sampling is done: the squeezed latent, its mask, the
+// decoder's mel and the Glow decoder's block
+struct DecodeWs { float *za, *msk, *melc; void* dec; size_t dec_bytes; };
+static DecodeWs decode_carve(const Overflow& e, Arena& ar, int B, int Tq) {
     const int C = e.c.out_channels, nsq = e.c.num_squeeze;
-    *za = ar.f32((size_t)B * C * nsq * Tq);
-    *msk = ar.f32((size_t)B * Tq);
-    *melc = ar.f32((size_t)B * C * Tq * nsq);
+    DecodeWs w;
+    w.za = ar.f32((size_t)B * C * nsq * Tq);
+    w.msk = ar.f32((size_t)B * Tq);
+    w.melc = ar.f32((size_t)B * C * Tq * nsq);
+    w.dec_bytes = e.dec.workspace_bytes(B, Tq);
+    w.dec = ar.bytes(w.dec_bytes);
+    return w;
 }
 
 int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, int nw) {
@@ -199,37 +215,25 @@ int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, in
 }
 
 size_t Overflow::workspace_bytes(int B, int Tt, int F) const {
-    const int E = c.encoder_dim, N = Tt * c.state_per_phone;
-    const size_t encb = arena_size([&](Arena& ar) {
-        Persist p;
-        persist_layout(*this, ar, B, Tt, p);
-        ar.f32((size_t)B * E * N);   // encode's transposed encoder states
-    }) + enc.workspace_bytes(B, Tt);
-    size_t decb = 0;
-    if (c.has_decoder && F > 0) {
-        const int Tq = tq(F);
-        decb = arena_size([&](Arena& ar) {
-            float* q[3];
-            decode_scratch(*this, ar, B, Tq, q, q + 1, q + 2);
-        }) + dec.workspace_bytes(B, Tq);
-    }
-    return std::max(encb, decb) + 1024;
+    const size_t encb = arena_size([&](Arena& ar) { encode_carve(*this, ar, B, Tt); });
+    if (!c.has_decoder || F <= 0) return encb;
+    return std::max(encb, arena_size([&](Arena& ar) { decode_carve(*this, ar, B, tq(F)); }));
 }
 
 int Overflow::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* states, void* ws,
                      size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(tokens && lengths && states && ws, "overflow_encode: null pointer");
     B200_REQUIRE(B >= 1 && Tt >= 1, "overflow_encode: empty batch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "overflow_encode: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "overflow_encode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int E = c.encoder_dim, N = Tt * c.state_per_phone;
     Arena ar(ws, ws_bytes);
-    Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "overflow_encode: arena exhausted");
+    const EncodeWs w = encode_carve(*this, ar, B, Tt);
+    const Persist& p = w.p;
+    float* encT = w.encT;
     int rc;
     // the [B, Tt, 2H] LSTM output is the [B, Tt*spp, E] state tensor
-    if ((rc = enc.encode(tokens, lengths, B, Tt, states, ar, st))) return rc;
-    float* encT = ar.f32((size_t)B * E * N);
-    B200_REQUIRE(encT, "overflow_encode: arena exhausted");
+    if ((rc = enc.encode(tokens, lengths, B, Tt, states, w.enc, st))) return rc;
     if ((rc = launch_transpose(states, encT, B, N, E, st))) return rc;
     {   // hoisted: zc[b, r, n] = W_z[r] . state[b, n] + b_0[r] for every state n
         ConvIO io;
@@ -247,12 +251,13 @@ int Overflow::sample(const long long* lengths, int B, int Tt, float temp, int ma
     B200_REQUIRE(B >= 1 && Tt >= 1 && max_frames >= 1, "overflow_sample: B, Tt and max_frames must be >= 1");
     B200_REQUIRE(temp <= 0.f || noise, "overflow_sample: sampling_temp > 0 needs noise");
     B200_REQUIRE(chunk_frames >= 2 && chunk_frames % 2 == 0, "overflow_sample: chunk_frames must be even and >= 2");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "overflow_sample: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "overflow_sample: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int C = c.out_channels, P = c.prenet_dim, M = c.memory_rnn_dim, nL = c.outputnet_n_layers;
     const int N = Tt * c.state_per_phone;
     Arena ar(ws, ws_bytes);
     Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "overflow_sample: arena exhausted");
+    persist_layout(*this, ar, B, Tt, p);
     int omax = 0;
     for (int l = 0; l < nL; ++l) omax = std::max(omax, c.outputnet_size[l]);
     B200_CUDA_OK(cudaMemsetAsync(hmm_out, 0, sizeof(float) * (size_t)B * max_frames * C, st));
@@ -332,13 +337,13 @@ int Overflow::decode(const float* hmm_out, const int* frames, int B, int F, int 
         B200_CUDA_OK(cudaGetLastError());
         return 0;
     }
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, 1, F), "overflow_decode: workspace too small");
+    const size_t need = workspace_bytes(B, 1, F);
+    B200_REQUIRE(ws_bytes >= need, "overflow_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int nsq = c.num_squeeze, Tv = F / nsq, Tq = tq(F), Cs = C * nsq;
     if (Tv == 0) return 0;
     Arena ar(ws, ws_bytes);
-    float *za, *msk, *melc;
-    decode_scratch(*this, ar, B, Tq, &za, &msk, &melc);
-    B200_REQUIRE(za && msk && melc, "overflow_decode: arena exhausted");
+    const DecodeWs w = decode_carve(*this, ar, B, Tq);
+    float *za = w.za, *msk = w.msk, *melc = w.melc;
     {
         dim3 grid((Tq + 127) / 128, Cs, B);
         squeeze_hmm_kernel<<<grid, 128, 0, st>>>(hmm_out, Fpitch, frames, za, msk, C, nsq, Tq);
@@ -346,7 +351,7 @@ int Overflow::decode(const float* hmm_out, const int* frames, int B, int F, int 
         B200_CUDA_OK(cudaGetLastError());
     }
     int rc;
-    if ((rc = dec.reverse(za, msk, nullptr, B, Tq, Tv, melc, ar.base + ar.off, ar.cap - ar.off, st))) return rc;
+    if ((rc = dec.reverse(za, msk, nullptr, B, Tq, Tv, melc, w.dec, w.dec_bytes, st))) return rc;
     const int T = Tv * nsq;
     dim3 grid((T * C + 255) / 256, B);
     denorm_kernel<<<grid, 256, 0, st>>>(melc, (long long)C * T, 1, T, mean, std_, mel, T, C);

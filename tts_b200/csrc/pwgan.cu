@@ -540,9 +540,23 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
     return build_u(fir);
 }
 
+// A: the conditioning of every layer (forward) or of one (layer); forward() also takes X0 / X1 (the residual stream)
+// and S (the skip sum)
+struct PwganWs { float *A, *X0, *X1, *S; };
+static PwganWs pwgan_carve(const Pwgan& m, Arena& ar, int B, int Tf, bool whole) {
+    const size_t bs = (size_t)pw::RES * round4(Tf * m.P);
+    PwganWs w{};
+    w.A = ar.f32((size_t)B * (whole ? m.c.num_res_blocks : 1) * pw::GATE * Tf);
+    if (whole) {
+        w.X0 = ar.f32(B * bs);
+        w.X1 = ar.f32(B * bs);
+        w.S = ar.f32(B * bs);
+    }
+    return w;
+}
+
 size_t Pwgan::workspace_bytes(int B, int Tf) const {
-    const size_t pitch = (size_t)round4(Tf * P);
-    return arena_bytes((size_t)B * c.num_res_blocks * pw::GATE * Tf) + 3 * arena_bytes((size_t)B * pw::RES * pitch);
+    return arena_size([&](Arena& ar) { pwgan_carve(*this, ar, B, Tf, true); });
 }
 
 UTab Pwgan::utab() const { return UTab{ucoef, P, uE0, uE1, uTW, uoff}; }
@@ -625,18 +639,16 @@ int Pwgan::forward(const float* mel, const float* noise, int B, int T, int pad, 
     int Tf = 0;
     if (int rc = check_call("pwgan_forward", B, T, pad, &Tf)) return rc;
     if (B == 0) return 0;
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tf), "pwgan_forward: workspace too small");
+    const size_t need = workspace_bytes(B, Tf);
+    B200_REQUIRE(ws_bytes >= need, "pwgan_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    const PwganWs w = pwgan_carve(*this, ar, B, Tf, true);
+    float *A = w.A, *X0 = w.X0, *S = w.S;
     int* err = nullptr;
     int num_sms = 0;
     if (int rc = layer_device(&err, &num_sms)) return rc;
     const int L = c.num_res_blocks, Ts = Tf * P, pitch = round4(Ts);
     const long long bs = (long long)RES * pitch;
-    Arena ar(ws, ws_bytes);
-    float* A = ar.f32((size_t)B * L * GATE * Tf);
-    float* X0 = ar.f32((size_t)B * bs);
-    float* X1 = ar.f32((size_t)B * bs);
-    float* S = ar.f32((size_t)B * bs);
-    B200_REQUIRE(A && X0 && X1 && S, "pwgan_forward: arena exhausted");
     if (int rc = launch_aux(mel, B, T, pad, 0, L, A, st)) return rc;
     {
         const long long n = (long long)B * Ts;
@@ -644,7 +656,7 @@ int Pwgan::forward(const float* mel, const float* noise, int B, int T, int pad, 
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
     }
-    float *x = X0, *xn = X1;
+    float *x = X0, *xn = w.X1;
     for (int l = 0; l < L; ++l) {
         if (int rc = launch_layer(l, x, xn, S, B, pitch, Tf, A + (size_t)l * GATE * Tf, (long long)L * GATE * Tf, err,
                                   num_sms, st))
@@ -670,11 +682,13 @@ int Pwgan::layer(int l, const float* mel, int B, int T, int pad, const float* x,
     if (int rc = check_call("pwgan_layer", B, T, pad, &Tf)) return rc;
     B200_REQUIRE(pitch >= Tf * P, "pwgan_layer: row pitch %d < %d samples", pitch, Tf * P);
     if (B == 0) return 0;
-    B200_REQUIRE(ws_bytes >= arena_bytes((size_t)B * GATE * Tf), "pwgan_layer: workspace too small");
+    const size_t need = arena_size([&](Arena& ar) { pwgan_carve(*this, ar, B, Tf, false); });
+    B200_REQUIRE(ws_bytes >= need, "pwgan_layer: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    float* A = pwgan_carve(*this, ar, B, Tf, false).A;
     int* err = nullptr;
     int num_sms = 0;
     if (int rc = layer_device(&err, &num_sms)) return rc;
-    float* A = static_cast<float*>(ws);
     if (int rc = launch_aux(mel, B, T, pad, l, 1, A, st)) return rc;
     return launch_layer(l, x, x_new, skip, B, pitch, Tf, A, (long long)GATE * Tf, err, num_sms, st);
 }

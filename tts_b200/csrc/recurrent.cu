@@ -480,20 +480,20 @@ int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, const float* c
     return 0;
 }
 
-size_t SeqEncoder::workspace_bytes(int B, int Tt) const {
-    return 2 * arena_bytes((size_t)B * E * Tt) + arena_bytes((size_t)B * Tt) + arena_bytes((size_t)B * 8 * H * Tt) +
-           arena_bytes((size_t)4 * B * H) + arena_bytes((size_t)2 * B * H);
+SeqEncoder::Scratch SeqEncoder::carve(Arena& ar, int B, int Tt) const {
+    Scratch s;
+    s.x = ar.f32((size_t)B * E * Tt);
+    s.y = ar.f32((size_t)B * E * Tt);
+    s.xmask = ar.f32((size_t)B * Tt);
+    s.pre = ar.f32((size_t)B * 8 * H * Tt);
+    s.hb = ar.f32((size_t)4 * B * H);
+    s.cb = ar.f32((size_t)2 * B * H);
+    return s;
 }
 
-int SeqEncoder::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* out, Arena& ar,
+int SeqEncoder::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* out, const Scratch& s,
                        cudaStream_t st) const {
-    float* x = ar.f32((size_t)B * E * Tt);
-    float* y = ar.f32((size_t)B * E * Tt);
-    float* xmask = ar.f32((size_t)B * Tt);
-    float* pre = ar.f32((size_t)B * 8 * H * Tt);
-    float* hb = ar.f32((size_t)4 * B * H);
-    float* cb = ar.f32((size_t)2 * B * H);
-    B200_REQUIRE(x && y && xmask && pre && hb && cb, "encoder: arena exhausted");
+    float *x = s.x, *y = s.y, *xmask = s.xmask, *pre = s.pre, *hb = s.hb, *cb = s.cb;
     int rc;
     // emb(x) without a scale, zero past each row's length (the reference runs each row at its own length)
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, E, E, x, xmask, st, false))) return rc;

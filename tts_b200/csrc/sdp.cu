@@ -249,25 +249,33 @@ int DurPred::init(const b200tts_duration_predictor_config& cfg, const float* con
     return 0;
 }
 
+// the conditioned input, the two hidden tensors and the per-utterance bias (row pitch cpad)
+struct DurPredWs { float *xin, *h1, *h2, *cv; int cpad; };
+static DurPredWs durpred_carve(const DurPred& m, Arena& ar, int B, int T) {
+    DurPredWs w;
+    w.xin = ar.f32((size_t)B * (m.c.in_channels + m.c.language_emb_dim) * T);
+    w.h1 = ar.f32((size_t)B * m.c.hidden_channels * T);
+    w.h2 = ar.f32((size_t)B * m.c.hidden_channels * T);
+    w.cpad = std::max(std::max(m.cond.RowsPad, m.cond_lang.RowsPad), 64);
+    w.cv = ar.f32((size_t)B * w.cpad + 64);
+    return w;
+}
+
 size_t DurPred::workspace_bytes(int B, int T) const {
-    const int Cin = c.in_channels + c.language_emb_dim;
-    return arena_bytes((size_t)B * Cin * T) + 2 * arena_bytes((size_t)B * c.hidden_channels * T) +
-           arena_bytes((size_t)B * std::max(std::max(cond.RowsPad, cond_lang.RowsPad), 64) + 64) + 1024;
+    return arena_size([&](Arena& ar) { durpred_carve(*this, ar, B, T); });
 }
 
 int DurPred::forward(const float* x, const float* mask, const float* g, const float* lang_emb, int B, int T,
                      float* logw, void* ws, size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(x && mask && logw && ws, "duration_predictor: null pointer");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "duration_predictor: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "duration_predictor: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
     const int Cin = c.in_channels + c.language_emb_dim, F = c.hidden_channels;
     Arena ar(ws, ws_bytes);
-    float* xin = ar.f32((size_t)B * Cin * T);
-    float* h1 = ar.f32((size_t)B * F * T);
-    float* h2 = ar.f32((size_t)B * F * T);
-    const int cpad = std::max(std::max(cond.RowsPad, cond_lang.RowsPad), 64);
-    float* cv = ar.f32((size_t)B * cpad + 64);
-    B200_REQUIRE(xin && h1 && h2 && cv, "duration_predictor: arena exhausted");
+    const DurPredWs w = durpred_carve(*this, ar, B, T);
+    float *xin = w.xin, *h1 = w.h1, *h2 = w.h2, *cv = w.cv;
+    const int cpad = w.cpad;
     int rc;
     const float* cur = x;
     const bool has_g = c.cond_channels > 0 && g, has_l = c.language_emb_dim > 0 && lang_emb;
@@ -387,30 +395,36 @@ int SDP::init(const b200tts_sdp_config& cfg, const float* const* w, int nw) {
     return 0;
 }
 
+struct SdpWs { float *xc, *h, *y1, *y2, *z, *hp, *condv; };
+static SdpWs sdp_carve(const SDP& m, Arena& ar, int B, int T) {
+    const size_t bh = (size_t)B * m.c.hidden_channels * T;
+    SdpWs w;
+    w.xc = ar.f32(bh);
+    w.h = ar.f32(bh);
+    w.y1 = ar.f32(bh);
+    w.y2 = ar.f32(bh);
+    w.z = ar.f32((size_t)B * 2 * T);
+    w.hp = ar.f32((size_t)B * (3 * m.c.num_bins - 1) * T);
+    w.condv = ar.f32((size_t)B * std::max(std::max(m.cond.RowsPad, m.cond_lang.RowsPad), 64) + 64);
+    return w;
+}
+
 size_t SDP::workspace_bytes(int B, int T) const {
-    const size_t hb = arena_bytes((size_t)B * c.hidden_channels * T);
-    return 4 * hb + arena_bytes((size_t)B * 2 * T) + arena_bytes((size_t)B * (3 * c.num_bins - 1) * T) +
-           arena_bytes((size_t)B * std::max(std::max(cond.RowsPad, cond_lang.RowsPad), 64) + 64) + 1024;
+    return arena_size([&](Arena& ar) { sdp_carve(*this, ar, B, T); });
 }
 
 int SDP::reverse(const float* x, const float* mask, const float* noise, const float* g, const float* lang_emb,
                  float noise_scale, int B, int T, float* logw, int* err_flag, void* ws, size_t ws_bytes,
                  cudaStream_t st) const {
     B200_REQUIRE(x && mask && noise && logw && ws, "sdp_reverse: null pointer");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "sdp_reverse: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "sdp_reverse: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
     const int H = c.hidden_channels, nproj = 3 * c.num_bins - 1;
     Arena ar(ws, ws_bytes);
-    float* xc = ar.f32((size_t)B * H * T);
-    float* h = ar.f32((size_t)B * H * T);
-    float* y1 = ar.f32((size_t)B * H * T);
-    float* y2 = ar.f32((size_t)B * H * T);
-    float* z = ar.f32((size_t)B * 2 * T);
-    float* hp = ar.f32((size_t)B * nproj * T);
-    const int cpad = std::max(std::max(cond.RowsPad, cond_lang.RowsPad), 64);
-    float* condv = ar.f32((size_t)B * cpad + 64);
+    const SdpWs w = sdp_carve(*this, ar, B, T);
+    float *xc = w.xc, *h = w.h, *y1 = w.y1, *y2 = w.y2, *z = w.z, *hp = w.hp, *condv = w.condv;
     float* cv = nullptr;
-    B200_REQUIRE(xc && h && y1 && y2 && z && hp && condv, "sdp_reverse: arena exhausted");
     const long long bs = (long long)H * T;
     int rc;
     const bool has_g = c.cond_channels > 0 && g != nullptr;

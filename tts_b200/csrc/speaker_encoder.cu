@@ -325,7 +325,7 @@ struct Ws {
     float *pre, *spec, *mel, *x0, *buf[4], *part, *scale, *atth, *logits, *pooled, *fco;
     int Bp;
 };
-size_t ws_layout(const b200tts_speaker_encoder_config& c, int B, int T, Ws* out, void* base, size_t cap) {
+Ws ws_carve(const b200tts_speaker_encoder_config& c, Arena& a, int B, int T) {
     const Geo g = geometry(c, B, frames_of(c, T));
     const int F = c.fft_size / 2 + 1, T1 = g.T[1];
     size_t big = 0, part = 0;
@@ -336,25 +336,20 @@ size_t ws_layout(const b200tts_speaker_encoder_config& c, int B, int T, Ws* out,
     }
     const int Hf = c.input_dim / 8, C4 = c.num_filters[3], Bp = (B + 3) / 4 * 4;
     const int out_dim = (c.encoder_type ? 2 : 1) * Hf * C4;
-    const size_t n[] = {c.use_torch_spec ? (size_t)B * T : 0, c.use_torch_spec ? (size_t)B * F * T1 : 0,
-                        c.use_torch_spec ? (size_t)B * c.input_dim * T1 : 0, (size_t)(g.H[0] + 2) * g.L[0],
-                        big, big, big, big, part, (size_t)B * 256 * 4 /* C <= 1024 */,
-                        (size_t)128 * g.L[4], (size_t)Hf * C4 * g.L[4], (size_t)out_dim * Bp,
-                        (size_t)c.proj_dim * Bp};
-    Arena a(base, cap);
-    size_t total = 0;
-    float* p[14];
-    for (int i = 0; i < 14; ++i) {
-        total += arena_bytes(n[i]);
-        p[i] = base ? a.f32(n[i]) : nullptr;
-    }
-    if (out) {
-        out->pre = p[0]; out->spec = p[1]; out->mel = p[2]; out->x0 = p[3];
-        for (int i = 0; i < 4; ++i) out->buf[i] = p[4 + i];
-        out->part = p[8]; out->scale = p[9]; out->atth = p[10]; out->logits = p[11]; out->pooled = p[12]; out->fco = p[13];
-        out->Bp = Bp;
-    }
-    return total;
+    Ws w;
+    w.pre = a.f32(c.use_torch_spec ? (size_t)B * T : 0);
+    w.spec = a.f32(c.use_torch_spec ? (size_t)B * F * T1 : 0);
+    w.mel = a.f32(c.use_torch_spec ? (size_t)B * c.input_dim * T1 : 0);
+    w.x0 = a.f32((size_t)(g.H[0] + 2) * g.L[0]);
+    for (int i = 0; i < 4; ++i) w.buf[i] = a.f32(big);
+    w.part = a.f32(part);
+    w.scale = a.f32((size_t)B * 256 * 4);   // C <= 1024
+    w.atth = a.f32((size_t)128 * g.L[4]);
+    w.logits = a.f32((size_t)Hf * C4 * g.L[4]);
+    w.pooled = a.f32((size_t)out_dim * Bp);
+    w.fco = a.f32((size_t)c.proj_dim * Bp);
+    w.Bp = Bp;
+    return w;
 }
 
 int zero_rows(float* buf, int H, size_t row, cudaStream_t st) {   // rows 0 and H + 1 of [H + 2][row]
@@ -491,7 +486,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
 
 size_t SpeakerEncoder::workspace_bytes(int B, int T) const {
     if (B <= 0 || T <= 0) return 0;
-    return ws_layout(c, B, T, nullptr, nullptr, 0);
+    return arena_size([&](Arena& ar) { ws_carve(c, ar, B, T); });
 }
 
 int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int groups, int l2_norm, float* emb, int stop,
@@ -501,10 +496,10 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
     B200_REQUIRE(stop <= 4, "speaker_encoder: stage %d does not exist", stop);
     B200_REQUIRE(stop >= 0 ? feat != nullptr : (emb && groups >= 1 && B % groups == 0 && B / groups <= 8192),
                  "speaker_encoder: B=%d windows do not split into %d groups of at most 8192 (or null output)", B, groups);
-    const size_t need = ws_layout(c, B, T, nullptr, nullptr, 0);
+    const size_t need = workspace_bytes(B, T);
     B200_REQUIRE(ws_bytes >= need, "speaker_encoder: workspace of %zu bytes, %zu needed", ws_bytes, need);
-    Ws W;
-    ws_layout(c, B, T, &W, ws, ws_bytes);
+    Arena ar(ws, ws_bytes);
+    const Ws W = ws_carve(c, ar, B, T);
     const int T1 = frames_of(c, T);
     const Geo g = geometry(c, B, T1);
     // ---- front end -> stem input [H0 + 2][1][L1]

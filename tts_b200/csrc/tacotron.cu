@@ -157,9 +157,9 @@ struct Persist : TacoLoop {
     float *mem, *q, *ctx, *dh1, *dh2;
 };
 
-bool persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
+void persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
     const size_t nzero = (size_t)B * (2 * e.Cm + 2 * Q + E + 4 * D);
-    const bool ok = taco_loop_layout(ar, B, Tt, e.c.frame_channels * e.c.r_init, nzero, p);
+    taco_loop_layout(ar, B, Tt, e.c.frame_channels * e.c.r_init, nzero, p);
     p.pb = ar.f32((size_t)B * (PN0 + PN1));
     p.din = ar.f32((size_t)B * D);
     p.x1 = ar.f32((size_t)B * D);
@@ -169,7 +169,6 @@ bool persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
     p.ctx = p.q + (size_t)2 * B * Q;
     p.dh1 = p.ctx + (size_t)B * E;
     p.dh2 = p.dh1 + (size_t)2 * B * D;
-    return ok && p.pb && p.din && p.x1 && p.x2;
 }
 
 }  // namespace
@@ -241,24 +240,19 @@ int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int*
     return 0;
 }
 
-static void cbhg_scratch(const Tacotron::Cbhg& c, Arena& ar, int B, int T, float** bank, float** y2, float** y3,
-                         float** hx, float** pre) {
-    *bank = ar.f32((size_t)B * c.K * BANK * T);
-    *y2 = ar.f32((size_t)B * c.P1 * T);
-    *y3 = ar.f32((size_t)B * c.Cin * T);
-    *hx = ar.f32((size_t)B * HW * T);
-    *pre = ar.f32((size_t)B * 6 * GRU_H * T);
-}
-
-size_t Tacotron::Cbhg::scratch_bytes(int B, int T) const {
-    return arena_size([&](Arena& ar) { float* p[5]; cbhg_scratch(*this, ar, B, T, p, p + 1, p + 2, p + 3, p + 4); });
+Tacotron::Cbhg::Scratch Tacotron::Cbhg::carve(Arena& ar, int B, int T) const {
+    Scratch s;
+    s.bank = ar.f32((size_t)B * K * BANK * T);
+    s.y2 = ar.f32((size_t)B * P1 * T);
+    s.y3 = ar.f32((size_t)B * Cin * T);
+    s.hx = ar.f32((size_t)B * HW * T);
+    s.pre = ar.f32((size_t)B * 6 * GRU_H * T);
+    return s;
 }
 
 int Tacotron::Cbhg::run(const float* x, const float* mask, const int* lens32, const long long* lens64, int B, int T,
-                        float* out, long long out_bs, int out_ts, int out_cs, Arena& ar, cudaStream_t st) const {
-    float *bk, *y2, *y3, *hx, *pre;
-    cbhg_scratch(*this, ar, B, T, &bk, &y2, &y3, &hx, &pre);
-    B200_REQUIRE(bk && y2 && y3 && hx && pre, "tacotron: arena exhausted");
+                        float* out, long long out_bs, int out_ts, int out_cs, const Scratch& s, cudaStream_t st) const {
+    float *bk = s.bank, *y2 = s.y2, *y3 = s.y3, *hx = s.hx, *pre = s.pre;
     int rc;
     auto conv = [&](const ConvLayer& L, const float* in, int ci, float* o, int co, int act, const float* res) {
         ConvIO io;
@@ -362,47 +356,47 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
     return 0;
 }
 
-static void encode_scratch(Arena& ar, int B, int Tt, float** x0, float** mask, float** x1, float** xin, float** encT) {
-    *x0 = ar.f32((size_t)B * EMB * Tt);
-    *mask = ar.f32((size_t)B * Tt);
-    *x1 = ar.f32((size_t)B * PN0 * Tt);
-    *xin = ar.f32((size_t)B * PN1 * Tt);
-    *encT = ar.f32((size_t)B * E * Tt);
+// encode: the loop state (kept until the loop ends), the embedding and its mask, the prenet outputs, the transposed
+// encoder outputs and the encoder CBHG's scratch
+struct EncodeWs { Persist p; float *x0, *mask, *x1, *xin, *encT; Tacotron::Cbhg::Scratch cbhg; };
+static EncodeWs encode_carve(const Tacotron& e, Arena& ar, int B, int Tt) {
+    EncodeWs w;
+    persist_layout(e, ar, B, Tt, w.p);
+    w.x0 = ar.f32((size_t)B * EMB * Tt);
+    w.mask = ar.f32((size_t)B * Tt);
+    w.x1 = ar.f32((size_t)B * PN0 * Tt);
+    w.xin = ar.f32((size_t)B * PN1 * Tt);
+    w.encT = ar.f32((size_t)B * E * Tt);
+    w.cbhg = e.ecbhg.carve(ar, B, Tt);
+    return w;
 }
 
-static void postnet_scratch(const Tacotron& e, Arena& ar, int B, int Tp, float** x, float** mask, float** g, float** y) {
-    *x = ar.f32((size_t)B * e.c.frame_channels * Tp);
-    *mask = ar.f32((size_t)B * Tp);
-    *g = ar.f32((size_t)B * 2 * GRU_H * Tp);
-    *y = ar.f32((size_t)B * e.c.out_channels * Tp);
+// postnet, from the start of the workspace once the loop is done: its input and mask, the CBHG output and scratch
+struct PostnetWs { float *x, *mask, *g, *y; Tacotron::Cbhg::Scratch cbhg; };
+static PostnetWs postnet_carve(const Tacotron& e, Arena& ar, int B, int Tp) {
+    PostnetWs w;
+    w.x = ar.f32((size_t)B * e.c.frame_channels * Tp);
+    w.mask = ar.f32((size_t)B * Tp);
+    w.g = ar.f32((size_t)B * 2 * GRU_H * Tp);
+    w.y = ar.f32((size_t)B * e.c.out_channels * Tp);
+    w.cbhg = e.pcbhg.carve(ar, B, Tp);
+    return w;
 }
 
 size_t Tacotron::workspace_bytes(int B, int Tt, int F) const {
-    const size_t encb = arena_size([&](Arena& ar) {
-        Persist p;
-        persist_layout(*this, ar, B, Tt, p);
-        float* q[5];
-        encode_scratch(ar, B, Tt, q, q + 1, q + 2, q + 3, q + 4);
-    }) + ecbhg.scratch_bytes(B, Tt);
-    const int Tp = (F + 3) / 4 * 4;
-    const size_t postb = arena_size([&](Arena& ar) {
-        float* q[4];
-        postnet_scratch(*this, ar, B, Tp, q, q + 1, q + 2, q + 3);
-    }) + pcbhg.scratch_bytes(B, Tp);
-    return std::max(encb, postb) + 1024;
+    return std::max(arena_size([&](Arena& ar) { encode_carve(*this, ar, B, Tt); }),
+                    arena_size([&](Arena& ar) { postnet_carve(*this, ar, B, (F + 3) / 4 * 4); }));
 }
 
 int Tacotron::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,
                      size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(tokens && lengths && enc_out && ws, "tacotron_encode: null pointer");
     B200_REQUIRE(B >= 1 && Tt >= 1, "tacotron_encode: empty batch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron_encode: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "tacotron_encode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     Arena ar(ws, ws_bytes);
-    Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron_encode: arena exhausted");
-    float *x0, *mask, *x1, *xin, *encT;
-    encode_scratch(ar, B, Tt, &x0, &mask, &x1, &xin, &encT);
-    B200_REQUIRE(x0 && mask && x1 && xin && encT, "tacotron_encode: arena exhausted");
+    const EncodeWs w = encode_carve(*this, ar, B, Tt);
+    float *x0 = w.x0, *mask = w.mask, *x1 = w.x1, *xin = w.xin;
     int rc;
     // emb(x), zero past each row's length (the reference runs each row at its own length)
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, EMB, EMB, x0, mask, st, false))) return rc;
@@ -417,8 +411,8 @@ int Tacotron::encode(const long long* tokens, const long long* lengths, int B, i
         if ((rc = launch_conv(eprenet[l], io, st))) return rc;
         in = o;
     }
-    if ((rc = ecbhg.run(xin, mask, nullptr, lengths, B, Tt, enc_out, (long long)Tt * E, E, 1, ar, st))) return rc;
-    return att.keys(enc_out, encT, p.pin, B, Tt, st);
+    if ((rc = ecbhg.run(xin, mask, nullptr, lengths, B, Tt, enc_out, (long long)Tt * E, E, 1, w.cbhg, st))) return rc;
+    return att.keys(enc_out, w.encT, w.p.pin, B, Tt, st);
 }
 
 int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
@@ -429,11 +423,12 @@ int Tacotron::decode_loop(const long long* lengths, const float* enc_out, int B,
     B200_REQUIRE(B >= 1 && Tt >= 1 && max_steps >= 1, "tacotron_decode_loop: B, Tt and max_steps must be >= 1");
     B200_REQUIRE(r >= 1 && r <= c.r_init, "tacotron_decode_loop: r must be in [1, r_init = %d]", c.r_init);
     B200_REQUIRE(chunk_steps >= 2 && chunk_steps % 2 == 0, "tacotron_decode_loop: chunk_steps must be even and >= 2");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron_decode_loop: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "tacotron_decode_loop: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int C = c.frame_channels, RC = C * c.r_init, S = max_steps + 1;   // a row emits at most max_steps + 1 steps
     Arena ar(ws, ws_bytes);
     Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron_decode_loop: arena exhausted");
+    persist_layout(*this, ar, B, Tt, p);
     int rc;
     if ((rc = taco_loop_start(p, B, Tt, S, r * C, c.attention_type == 1, dec_out, stop_tokens, alignments, st)))
         return rc;
@@ -519,16 +514,16 @@ int Tacotron::postnet(const float* dec_out, const int* frames, int B, int F, int
                       size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(dec_out && frames && out && ws, "tacotron_postnet: null pointer");
     B200_REQUIRE(B >= 1 && F >= 1 && F <= Fpitch, "tacotron_postnet: need B >= 1 and 1 <= F <= Fpitch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, 1, F), "tacotron_postnet: workspace too small");
+    const size_t need = workspace_bytes(B, 1, F);
+    B200_REQUIRE(ws_bytes >= need, "tacotron_postnet: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int C = c.frame_channels, O = c.out_channels, Tp = (F + 3) / 4 * 4;
     Arena ar(ws, ws_bytes);
-    float *x, *mask, *g, *y;
-    postnet_scratch(*this, ar, B, Tp, &x, &mask, &g, &y);
-    B200_REQUIRE(x && mask && g && y, "tacotron_postnet: arena exhausted");
+    const PostnetWs w = postnet_carve(*this, ar, B, Tp);
+    float *x = w.x, *mask = w.mask, *g = w.g, *y = w.y;
     int rc;
     if ((rc = launch_frames_in(dec_out, Fpitch, frames, x, mask, B, C, Tp, st))) return rc;
     // the biGRU writes channel-major [B, 256, Tp] for last_linear on the conv engine
-    if ((rc = pcbhg.run(x, mask, frames, nullptr, B, Tp, g, (long long)2 * GRU_H * Tp, 1, Tp, ar, st))) return rc;
+    if ((rc = pcbhg.run(x, mask, frames, nullptr, B, Tp, g, (long long)2 * GRU_H * Tp, 1, Tp, w.cbhg, st))) return rc;
     {
         ConvIO io;
         io.x = g; io.x_bs = (long long)2 * GRU_H * Tp; io.x_cs = Tp; io.Tin = Tp;

@@ -60,9 +60,9 @@ struct Persist : TacoLoop {
     float *pb, *mem, *q, *qc, *ctx, *dh, *dc;
 };
 
-bool persist_layout(const Tacotron2& e, Arena& ar, int B, int Tt, Persist& p) {
+void persist_layout(const Tacotron2& e, Arena& ar, int B, int Tt, Persist& p) {
     const int C = e.c.out_channels;
-    const bool ok = taco_loop_layout(ar, B, Tt, C * e.c.r_init, (size_t)B * (C + 2 * Q + Q + E + 2 * D + D), p);
+    taco_loop_layout(ar, B, Tt, C * e.c.r_init, (size_t)B * (C + 2 * Q + Q + E + 2 * D + D), p);
     p.pb = ar.f32((size_t)2 * B * PN);
     p.mem = p.zero;
     p.q = p.mem + (size_t)B * C;
@@ -70,30 +70,35 @@ bool persist_layout(const Tacotron2& e, Arena& ar, int B, int Tt, Persist& p) {
     p.ctx = p.qc + (size_t)B * Q;
     p.dh = p.ctx + (size_t)B * E;
     p.dc = p.dh + (size_t)2 * B * D;
-    return ok && p.pb;
 }
 
-void postnet_scratch(Arena& ar, int B, int C, int Tp, float** x, float** y, float** h1, float** h2, float** mask) {
-    *x = ar.f32((size_t)B * C * Tp);
-    *y = ar.f32((size_t)B * C * Tp);
-    *h1 = ar.f32((size_t)B * 512 * Tp);
-    *h2 = ar.f32((size_t)B * 512 * Tp);
-    *mask = ar.f32((size_t)B * Tp);
+// encode: the loop state (kept until the loop ends), the encoder's scratch and the transposed encoder outputs
+struct EncodeWs { Persist p; SeqEncoder::Scratch enc; float* encT; };
+EncodeWs encode_carve(const Tacotron2& e, Arena& ar, int B, int Tt) {
+    EncodeWs w;
+    persist_layout(e, ar, B, Tt, w.p);
+    w.enc = e.enc.carve(ar, B, Tt);
+    w.encT = ar.f32((size_t)B * E * Tt);
+    return w;
+}
+
+// postnet, from the start of the workspace once the loop is done
+struct PostnetWs { float *x, *y, *h1, *h2, *mask; };
+PostnetWs postnet_carve(Arena& ar, int B, int C, int Tp) {
+    PostnetWs w;
+    w.x = ar.f32((size_t)B * C * Tp);
+    w.y = ar.f32((size_t)B * C * Tp);
+    w.h1 = ar.f32((size_t)B * 512 * Tp);
+    w.h2 = ar.f32((size_t)B * 512 * Tp);
+    w.mask = ar.f32((size_t)B * Tp);
+    return w;
 }
 
 }  // namespace
 
 size_t Tacotron2::workspace_bytes(int B, int Tt, int F) const {
-    const size_t encb = arena_size([&](Arena& ar) {
-        Persist p;
-        persist_layout(*this, ar, B, Tt, p);
-        ar.f32((size_t)B * E * Tt);   // encode's transposed encoder outputs
-    }) + enc.workspace_bytes(B, Tt);
-    const size_t postb = arena_size([&](Arena& ar) {
-        float* q[5];
-        postnet_scratch(ar, B, c.out_channels, (F + 3) / 4 * 4, q, q + 1, q + 2, q + 3, q + 4);
-    });
-    return std::max(encb, postb) + 1024;
+    return std::max(arena_size([&](Arena& ar) { encode_carve(*this, ar, B, Tt); }),
+                    arena_size([&](Arena& ar) { postnet_carve(ar, B, c.out_channels, (F + 3) / 4 * 4); }));
 }
 
 int Tacotron2::init(const b200tts_tacotron2_config& cfg, const float* const* w, int nw) {
@@ -149,15 +154,13 @@ int Tacotron2::encode(const long long* tokens, const long long* lengths, int B, 
                       size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(tokens && lengths && enc_out && ws, "tacotron2_encode: null pointer");
     B200_REQUIRE(B >= 1 && Tt >= 1, "tacotron2_encode: empty batch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron2_encode: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "tacotron2_encode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     Arena ar(ws, ws_bytes);
-    Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron2_encode: arena exhausted");
+    const EncodeWs w = encode_carve(*this, ar, B, Tt);
     int rc;
-    if ((rc = enc.encode(tokens, lengths, B, Tt, enc_out, ar, st))) return rc;
-    float* encT = ar.f32((size_t)B * E * Tt);
-    B200_REQUIRE(encT, "tacotron2_encode: arena exhausted");
-    return att.keys(enc_out, encT, p.pin, B, Tt, st);
+    if ((rc = enc.encode(tokens, lengths, B, Tt, enc_out, w.enc, st))) return rc;
+    return att.keys(enc_out, w.encT, w.p.pin, B, Tt, st);
 }
 
 int Tacotron2::decode_loop(const long long* lengths, const float* enc_out, int B, int Tt, int r, int max_steps,
@@ -168,11 +171,12 @@ int Tacotron2::decode_loop(const long long* lengths, const float* enc_out, int B
     B200_REQUIRE(B >= 1 && Tt >= 1 && max_steps >= 1, "tacotron2_decode_loop: B, Tt and max_steps must be >= 1");
     B200_REQUIRE(r >= 1 && r <= c.r_init, "tacotron2_decode_loop: r must be in [1, r_init = %d]", c.r_init);
     B200_REQUIRE(chunk_steps >= 2 && chunk_steps % 2 == 0, "tacotron2_decode_loop: chunk_steps must be even and >= 2");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, Tt, 0), "tacotron2_decode_loop: workspace too small");
+    const size_t need = workspace_bytes(B, Tt, 0);
+    B200_REQUIRE(ws_bytes >= need, "tacotron2_decode_loop: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int C = c.out_channels, RC = C * c.r_init;
     Arena ar(ws, ws_bytes);
     Persist p;
-    B200_REQUIRE(persist_layout(*this, ar, B, Tt, p), "tacotron2_decode_loop: arena exhausted");
+    persist_layout(*this, ar, B, Tt, p);
     int rc;
     if ((rc = taco_loop_start(p, B, Tt, max_steps, r * C, c.attention_type == 1, dec_out, stop_tokens, alignments, st)))
         return rc;
@@ -247,12 +251,12 @@ int Tacotron2::postnet(const float* dec_out, const int* frames, int B, int F, in
                        size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(dec_out && frames && mel && ws, "tacotron2_postnet: null pointer");
     B200_REQUIRE(B >= 1 && F >= 1 && F <= Fpitch, "tacotron2_postnet: need B >= 1 and 1 <= F <= Fpitch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, 1, F), "tacotron2_postnet: workspace too small");
+    const size_t need = workspace_bytes(B, 1, F);
+    B200_REQUIRE(ws_bytes >= need, "tacotron2_postnet: workspace of %zu bytes, %zu needed", ws_bytes, need);
     const int C = c.out_channels, Tp = (F + 3) / 4 * 4;
     Arena ar(ws, ws_bytes);
-    float *x, *y, *h1, *h2, *mask;
-    postnet_scratch(ar, B, C, Tp, &x, &y, &h1, &h2, &mask);
-    B200_REQUIRE(x && y && h1 && h2 && mask, "tacotron2_postnet: arena exhausted");
+    const PostnetWs w = postnet_carve(ar, B, C, Tp);
+    float *x = w.x, *y = w.y, *h1 = w.h1, *h2 = w.h2, *mask = w.mask;
     int rc;
     if ((rc = launch_frames_in(dec_out, Fpitch, frames, x, mask, B, C, Tp, st))) return rc;
     const float* in = x;

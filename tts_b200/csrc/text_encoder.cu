@@ -301,18 +301,26 @@ int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int
     return 0;
 }
 
+struct RelPosWs { float *qkv, *att, *yb, *hb; };
+static RelPosWs relpos_carve(const RelPosTransformer& m, Arena& ar, int B, int T) {
+    RelPosWs w;
+    w.qkv = ar.f32((size_t)B * 3 * m.C * T);
+    w.att = ar.f32((size_t)B * m.C * T);
+    w.yb = ar.f32((size_t)B * m.C * T);
+    w.hb = ar.f32((size_t)B * m.F * T);
+    return w;
+}
+
 size_t RelPosTransformer::workspace_bytes(int B, int T) const {
-    return arena_bytes((size_t)B * 3 * C * T) + 2 * arena_bytes((size_t)B * C * T) + arena_bytes((size_t)B * F * T);
+    return arena_size([&](Arena& ar) { relpos_carve(*this, ar, B, T); });
 }
 
 int RelPosTransformer::forward(float* x, const float* x_mask, int B, int T, void* ws, size_t ws_bytes,
                                cudaStream_t st) const {
     Arena ar(ws, ws_bytes);
-    float* qkv = ar.f32((size_t)B * 3 * C * T);
-    float* att = ar.f32((size_t)B * C * T);
-    float* yb = ar.f32((size_t)B * C * T);
-    float* hb = ar.f32((size_t)B * F * T);
-    B200_REQUIRE(qkv && att && yb && hb, "rel_pos_transformer: arena exhausted");
+    const RelPosWs w = relpos_carve(*this, ar, B, T);
+    B200_REQUIRE(ar.ok(), "rel_pos_transformer: workspace of %zu bytes is too small", ws_bytes);
+    float *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb;
     const long long bs = (long long)C * T;
     int rc;
     for (const Layer& L : layers) {
@@ -373,13 +381,15 @@ int TextEncoder::init(const b200tts_text_encoder_config& cfg, const float* const
     return pack_conv(proj, p[0], p[1], 2 * c.out_channels, C, 1, 1, 0);
 }
 
-size_t TextEncoder::workspace_bytes(int B, int T) const { return tf.workspace_bytes(B, T) + 1024; }
+// the whole workspace is the transformer's
+size_t TextEncoder::workspace_bytes(int B, int T) const { return tf.workspace_bytes(B, T); }
 
 int TextEncoder::forward(const long long* tokens, const long long* lengths, const float* lang_emb, int B, int T,
                          float* x, float* stats, float* x_mask, void* ws, size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(tokens && lengths && x && stats && x_mask && ws, "text_encoder_forward: null pointer");
     B200_REQUIRE((c.language_emb_dim > 0) == (lang_emb != nullptr), "text_encoder_forward: lang_emb mismatch");
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "text_encoder_forward: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "text_encoder_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
     const long long bs = (long long)C * T;
     int rc;

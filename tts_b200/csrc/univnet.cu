@@ -377,11 +377,23 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
     return pack_conv(last, w[i], w[i + 1], c.out_channels, C, 7, 1, 3);
 }
 
-// scratch: the predicted kernels of one block, the KPnet hidden state (3 tensors), two x tensors at the final rate
+// the KPnet hidden state (3 tensors); forward() also takes the predicted kernels of one block (P) and two x tensors at
+// the final rate
+struct UnivnetWs { float *P, *H[3], *X0, *X1; };
+static UnivnetWs univnet_carve(const Univnet& m, Arena& ar, int B, int T, bool whole) {
+    const size_t Tp = (size_t)round4(T), Ts = (size_t)round4(T * m.hop_total);
+    UnivnetWs w{};
+    if (whole) w.P = ar.f32((size_t)B * T * m.MP);
+    for (float*& h : w.H) h = ar.f32((size_t)B * m.c.kpnet_hidden_channels * Tp);
+    if (whole) {
+        w.X0 = ar.f32((size_t)B * uv::C * Ts);
+        w.X1 = ar.f32((size_t)B * uv::C * Ts);
+    }
+    return w;
+}
+
 size_t Univnet::workspace_bytes(int B, int T) const {
-    const size_t Tp = (size_t)round4(T), Ts = (size_t)round4(T * hop_total);
-    return arena_bytes((size_t)B * T * MP) + 3 * arena_bytes((size_t)B * c.kpnet_hidden_channels * Tp) +
-           2 * arena_bytes((size_t)B * uv::C * Ts);
+    return arena_size([&](Arena& ar) { univnet_carve(*this, ar, B, T, true); });
 }
 
 int Univnet::check_call(const char* who, int B, int T) const {
@@ -460,18 +472,14 @@ int Univnet::forward(const float* mel, const float* noise, int B, int T, float* 
     B200_REQUIRE(mel && noise && out && ws, "univnet_forward: null pointer");
     if (int rc = check_call("univnet_forward", B, T)) return rc;
     if (B == 0) return 0;
-    B200_REQUIRE(ws_bytes >= workspace_bytes(B, T), "univnet_forward: workspace too small");
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws_bytes >= need, "univnet_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    const UnivnetWs w = univnet_carve(*this, ar, B, T, true);
+    float *P = w.P, *X0 = w.X0, *X1 = w.X1;
     int* err = nullptr;
     if (int rc = uv_device(&err)) return rc;
-    const int Ch = c.kpnet_hidden_channels, Tp = round4(T);
-    Arena ar(ws, ws_bytes);
-    float* P = ar.f32((size_t)B * T * MP);
-    float* H0 = ar.f32((size_t)B * Ch * Tp);
-    float* H1 = ar.f32((size_t)B * Ch * Tp);
-    float* H2 = ar.f32((size_t)B * Ch * Tp);
-    float* X0 = ar.f32((size_t)B * C * round4(T * hop_total));
-    float* X1 = ar.f32((size_t)B * C * round4(T * hop_total));
-    B200_REQUIRE(P && H0 && H1 && H2 && X0 && X1, "univnet_forward: arena exhausted");
+    const int Tp = round4(T);
     int rc;
     {   // first_conv(noise)
         ConvIO io;
@@ -483,7 +491,7 @@ int Univnet::forward(const float* mel, const float* noise, int B, int T, float* 
     int len = T, pitch = Tp;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const Block& bl = blocks[s];
-        if ((rc = launch_predict(s, mel, B, T, P, H0, H1, H2, err, st))) return rc;
+        if ((rc = launch_predict(s, mel, B, T, P, w.H[0], w.H[1], w.H[2], err, st))) return rc;
         const int Ls = T * bl.hop, Lp = round4(Ls);
         {   // x = upsample(lrelu(x, 0.2))
             ConvIO io;
@@ -510,15 +518,13 @@ int Univnet::predict(int blk, const float* mel, int B, int T, float* P, void* ws
     B200_REQUIRE(blk >= 0 && blk < c.num_upsamples, "univnet_predict: block %d of %d", blk, c.num_upsamples);
     if (int rc = check_call("univnet_predict", B, T)) return rc;
     if (B == 0) return 0;
-    const size_t hb = (size_t)B * c.kpnet_hidden_channels * round4(T);
-    B200_REQUIRE(ws_bytes >= 3 * arena_bytes(hb), "univnet_predict: workspace too small");
+    const size_t need = arena_size([&](Arena& ar) { univnet_carve(*this, ar, B, T, false); });
+    B200_REQUIRE(ws_bytes >= need, "univnet_predict: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    const UnivnetWs w = univnet_carve(*this, ar, B, T, false);
     int* err = nullptr;
     if (int rc = uv_device(&err)) return rc;
-    Arena ar(ws, ws_bytes);
-    float* H0 = ar.f32(hb);
-    float* H1 = ar.f32(hb);
-    float* H2 = ar.f32(hb);
-    return launch_predict(blk, mel, B, T, P, H0, H1, H2, err, st);
+    return launch_predict(blk, mel, B, T, P, w.H[0], w.H[1], w.H[2], err, st);
 }
 
 int Univnet::lvc_layer(int blk, int l, const float* x, const float* P, int B, int T, float* x_new, int pitch,

@@ -163,32 +163,23 @@ static void wg_sizes(const Wavegrad& m, int T, std::vector<size_t>& s) {
     s[n + 1] = mx;
 }
 
-size_t Wavegrad::workspace_bytes(int B, int T) const {
-    std::vector<size_t> s;
-    wg_sizes(*this, T, s);
-    size_t total = 0;
-    for (size_t i = 0; i + 1 < s.size(); ++i) total += arena_bytes((size_t)B * s[i]);
-    return total + 5 * arena_bytes((size_t)B * s.back());
-}
-
 namespace {
 struct WgBufs {
     float* xc = nullptr;
     std::vector<float*> F;
     float* P[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
 };
-int wg_carve(const Wavegrad& m, int B, int T, void* ws, size_t ws_bytes, WgBufs& o) {
+// x_conv's output comes first, so condition() and step() find it at the same offset
+WgBufs wg_carve(const Wavegrad& m, Arena& ar, int B, int T) {
     std::vector<size_t> s;
     wg_sizes(m, T, s);
     const int n = m.c.num_upsamples;
-    B200_REQUIRE(ws && ws_bytes >= m.workspace_bytes(B, T), "wavegrad: workspace too small (%zu < %zu bytes)", ws_bytes,
-                 m.workspace_bytes(B, T));
-    Arena ar(ws, ws_bytes);
+    WgBufs o;
     o.xc = ar.f32((size_t)B * s[0]);
     o.F.resize(n);
     for (int i = 0; i < n; ++i) o.F[i] = ar.f32((size_t)B * s[1 + i]);
     for (auto& p : o.P) p = ar.f32((size_t)B * s[n + 1]);
-    return 0;
+    return o;
 }
 // a stage buffer that is none of the given ones
 float* wg_pick(const WgBufs& o, const float* a, const float* b = nullptr, const float* c = nullptr, const float* d = nullptr) {
@@ -205,11 +196,17 @@ ConvIO wg_io(const float* x, int Cin, int xp, int Tin, float* y, int Cout, int y
 }
 }  // namespace
 
+size_t Wavegrad::workspace_bytes(int B, int T) const {
+    return arena_size([&](Arena& ar) { wg_carve(*this, ar, B, T); });
+}
+
 int Wavegrad::condition(const float* x, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const {
     B200_REQUIRE(x, "wavegrad_condition: null input");
     B200_REQUIRE(B >= 1 && T >= 1, "wavegrad_condition: B = %d, T = %d", B, T);
-    WgBufs o;
-    if (int rc = wg_carve(*this, B, T, ws, ws_bytes, o)) return rc;
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws && ws_bytes >= need, "wavegrad: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    const WgBufs o = wg_carve(*this, ar, B, T);
     ConvIO io = wg_io(x, c.in_channels, T, T, o.xc, c.x_conv_channels, round4(T), T, B);   // x_conv (wavegrad.py:115)
     return launch_conv(x_conv, io, st);
 }
@@ -222,8 +219,10 @@ int Wavegrad::network(const float* y, const float* noise_level, const float* con
     B200_REQUIRE(pe_frames >= T, "wavegrad: positional-encoding tables for %d frames, the input has %d", pe_frames, T);
     const int n = c.num_upsamples;
     for (int i = 0; i < n; ++i) B200_REQUIRE(pe[i], "wavegrad: null positional-encoding table %d", i);
-    WgBufs o;
-    if (int rc = wg_carve(*this, B, T, ws, ws_bytes, o)) return rc;
+    const size_t need = workspace_bytes(B, T);
+    B200_REQUIRE(ws && ws_bytes >= need, "wavegrad: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    Arena ar(ws, ws_bytes);
+    const WgBufs o = wg_carve(*this, ar, B, T);
     std::vector<int> L, Lpe;
     lengths(T, L);
     lengths(pe_frames, Lpe);
