@@ -116,6 +116,53 @@ int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, lon
                                     const float* film, long long film_batch_stride, int film_channel_stride, int film_half,
                                     float* y, long long y_batch_stride, int y_channel_stride, float* y2, void* stream);
 
+/* Debug / test aids: one conv layer with every prologue / epilogue option the engines use internally (the WaveNet gate
+ * and res/skip split, masks, per-row conditioning, ReLU / log-clamp, ragged rows, column windows), so that each option
+ * can be checked on its own against a float64 reference.  Not a stable interface.
+ *   create: b200tts_conv1d_create_padded plus the packing options of the engines: gate_half > 0 (= out_channels / 2)
+ *     interleaves rows (p, p + gate_half) into one (tanh, sigmoid) GEMM row pair; in_perm / out_perm (host int32,
+ *     nullable, in_channels / out_channels entries) put logical channel c at physical channel perm[c] (the flow's channel
+ *     flips).  Not for transposed convs.  The handle is a b200tts_conv1d (destroy, out_len and the forward calls apply).
+ *   launch: y[b, r, t] (t < out_len(T)) in the documented order
+ *     prologue  x *= xmask[b, t] (xmask nullable); x = leaky_relu(x, in_slope)
+ *     v = conv + bias[r] + cond[b, r]   (cond nullable, indexed by GEMM row: gate layers take it interleaved)
+ *     gate      (EPI_GATE 1): v = tanh(v[2p]) * sigmoid(v[2p + 1]) -> output row p; takes no other epilogue option
+ *     act       0 none, 1 relu, 2 tanh, 3 log(max(v, act_param))
+ *     mask_pre  (EPI_MASK_PRE 2): v *= ymask[b, t]
+ *     v += res[b, r, t] (nullable); v *= scale; accumulate (EPI_ACCUM 8): v += y_old; v /= post_div
+ *     mask_post (EPI_MASK_POST 4): v *= ymask[b, t]
+ *     split     (EPI_SPLIT 16, WaveNet res/skip): rows r < split go to y[b, r] with accumulate and mask_post forced on,
+ *               rows r >= split to y2[b, r - split], accumulating only with EPI_ACCUM2 (32), never masked
+ *   ymask needs EPI_MASK_PRE, EPI_MASK_POST or EPI_SPLIT (status 1 otherwise).  lens (device int32 [B], nullable): row b
+ *   is computed below lens[b] * rate_out + need_out and reads its input as zero from lens[b] * rate_in + need_in on (the
+ *   FP32-FMA kernel computes every column).  [q_lo, q_hi): the output columns to produce (the tensor-core kernels may
+ *   write other columns of their tiles too); [in_lo, in_hi): the input columns that hold data.  Returns the engine's
+ *   status. */
+enum { B200TTS_DEBUG_EPI_GATE = 1, B200TTS_DEBUG_EPI_MASK_PRE = 2, B200TTS_DEBUG_EPI_MASK_POST = 4,
+       B200TTS_DEBUG_EPI_ACCUM = 8, B200TTS_DEBUG_EPI_SPLIT = 16, B200TTS_DEBUG_EPI_ACCUM2 = 32 };
+enum { B200TTS_DEBUG_ACT_NONE = 0, B200TTS_DEBUG_ACT_RELU = 1, B200TTS_DEBUG_ACT_TANH = 2, B200TTS_DEBUG_ACT_LOGCLAMP = 3 };
+typedef struct {
+    const float* x; long long x_batch_stride; int x_channel_stride; int T;
+    const float* xmask; long long xmask_batch_stride;
+    float in_slope;
+    const float* cond; long long cond_batch_stride;
+    float* y; long long y_batch_stride; int y_channel_stride;
+    const float* res; long long res_batch_stride; int res_channel_stride;
+    const float* ymask; long long ymask_batch_stride;
+    float* y2; long long y2_batch_stride; int y2_channel_stride;
+    int split;
+    float scale, post_div;
+    int act; float act_param;
+    int flags;
+    int B;
+    const int32_t* lens; int rate_out, need_out, rate_in, need_in;
+    int q_lo, q_hi, in_lo, in_hi;
+} b200tts_debug_conv_io;
+int b200tts_debug_conv1d_create(const b200tts_conv1d_config* cfg, const float* weight, const float* bias,
+                                int allow_tensor_cores, int precision, int padding_mode, int gate_half,
+                                const int32_t* in_perm, const int32_t* out_perm, b200tts_conv1d** out);
+int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* io, void* stream);
+
 /* ---- monotonic alignment search ------------------------------------------------------------
  * Replaces maximum_path_c / maximum_path_each, TTS/tts/utils/monotonic_align/core.pyx:11-47
  * (called through TTS/tts/utils/helpers.py:172-194 from Vits.forward_mas, vits.py:919).

@@ -49,6 +49,90 @@ def epilogue(c, *, residual=None, scale=1.0, y_old=None, post_div=1.0, tanh=Fals
     return c
 
 
+ACT_NONE, ACT_RELU, ACT_TANH, ACT_LOGCLAMP = 0, 1, 2, 3
+EPI_GATE, EPI_MASK_PRE, EPI_MASK_POST, EPI_ACCUM, EPI_SPLIT, EPI_ACCUM2 = 1, 2, 4, 8, 16, 32
+
+
+def engine_prologue(x, xmask=None, in_slope=1.0, dtype=torch.float64):
+    """The engine's conv prologue in ``dtype``: x *= xmask[b, t] (xmask [B, T]), then leaky ReLU."""
+    x = x.to(dtype)
+    if xmask is not None:
+        x = x * xmask.to(dtype)[:, None, :]
+    return F.leaky_relu(x, in_slope)
+
+
+def engine_epilogue(c, *, cond=None, act=ACT_NONE, act_param=0.0, ymask=None, flags=0, residual=None, scale=1.0,
+                    y_old=None, post_div=1.0, split=0, y2_old=None):
+    """The engine's epilogue (common.cuh, launch_conv) on a conv result ``c`` [B, R, T] with its bias, in c's dtype and
+    in the documented order; returns (y, y2).  Rows are logical rows (a gate layer's first R/2 rows are the tanh half);
+    cond [B, R] in the same order; ymask [B, T]; y_old / y2_old are the destinations' previous contents.
+      v = c + cond;  gate: tanh(v[:H]) * sigmoid(v[H:]) (nothing else applies)  |  act
+      mask_pre; + residual; * scale; + y_old (ACCUM); / post_div; mask_post
+      split: rows < split -> y with ACCUM and MASK_POST forced on, rows >= split -> y2 (+ y2_old with ACCUM2, no mask)"""
+    dt = c.dtype
+    v = c if cond is None else c + cond.to(dt)[:, :, None]
+    if flags & EPI_GATE:
+        h = v.shape[1] // 2
+        return torch.tanh(v[:, :h]) * torch.sigmoid(v[:, h:]), None
+    if act == ACT_RELU:
+        v = torch.relu(v)
+    elif act == ACT_TANH:
+        v = torch.tanh(v)
+    elif act == ACT_LOGCLAMP:
+        v = torch.log(torch.clamp_min(v, act_param))
+    m = None if ymask is None else ymask.to(dt)[:, None, :]
+    rows = v.shape[1]
+    n_y = split if flags & EPI_SPLIT else rows
+    accum = torch.zeros(rows, dtype=torch.bool)
+    mpost = torch.zeros(rows, dtype=torch.bool)
+    accum[:n_y], mpost[:n_y] = bool(flags & EPI_ACCUM) or n_y < rows, bool(flags & EPI_MASK_POST) or n_y < rows
+    accum[n_y:] = bool(flags & EPI_ACCUM2)
+    if flags & EPI_MASK_PRE:
+        v = v * m
+    if residual is not None:
+        v = v + residual.to(dt)
+    v = v * scale
+    old = torch.zeros_like(v)
+    if y_old is not None:
+        old[:, :n_y] = y_old.to(dt)[:, :n_y]
+    if y2_old is not None and n_y < rows:
+        old[:, n_y:] = y2_old.to(dt)
+    v = torch.where(accum[None, :, None].to(v.device), v + old, v)
+    v = v / post_div
+    if m is not None:
+        v = torch.where(mpost[None, :, None].to(v.device), v * m, v)
+    return v[:, :n_y], (v[:, n_y:] if n_y < rows else None)
+
+
+def engine_layer(x, w, bias, *, dilation=1, padding=0, reflect=False, xmask=None, in_slope=1.0, dtype=torch.float64,
+                 conv_fn=None, **epi):
+    """One engine layer: engine_prologue, conv1d (w [R, Cin, K], logical rows; reflect: ReflectionPad1d(padding) and no
+    zero padding) + bias, engine_epilogue(**epi); returns (y, y2).  ``conv_fn(x, in_slope, padding)`` replaces the
+    leaky ReLU and the conv (lowp_reference for 16-bit operands); it gets x after the input mask and any reflection."""
+    if conv_fn is not None:
+        xm = x if xmask is None else x * xmask.to(x.dtype)[:, None, :]
+    else:
+        xm = engine_prologue(x, xmask, in_slope, dtype)
+    if reflect and padding:
+        xm = F.pad(xm, (padding, padding), mode="reflect")
+        padding = 0
+    if conv_fn is None:
+        c = F.conv1d(xm, w.to(dtype), None if bias is None else bias.to(dtype), dilation=dilation, padding=padding)
+    else:
+        c = conv_fn(xm, in_slope, padding)
+    return engine_epilogue(c, **epi)
+
+
+def ragged_extent(lens, rate, need, limit):
+    """ConvIO's ragged extent per row: min(limit, max(0, lens[b] * rate + need)), as a CPU int64 tensor"""
+    return (lens.to(torch.int64).cpu() * rate + need).clamp(0, limit)
+
+
+def columns_below(ext, T):
+    """[B, T] bool: column t of row b is below ext[b]"""
+    return torch.arange(T)[None, :] < ext[:, None]
+
+
 def measure(got, want):
     """Relative errors of ``got`` [B, R, T] against ``want``: whole tensor, worst (batch, column), worst (batch, row)
     (RMS over the other axis, relative to the whole tensor's RMS) and worst element (relative to max |want|)."""

@@ -36,6 +36,24 @@ def test_library_exports_the_device_buffer_counter():
     assert lib.b200tts_debug_device_buffers() >= 0
 
 
+def test_library_exports_the_debug_conv_layer():
+    """the per-option conv aid (b200tts_debug_conv1d_*) is declared, exported and bound with its argument struct"""
+    from tts_b200 import _lib
+
+    syms = declared_symbols()
+    assert "b200tts_debug_conv1d_create" in syms and "b200tts_debug_conv1d_launch" in syms
+    lib = _lib.lib()
+    assert lib.b200tts_debug_conv1d_create.restype is ctypes.c_int
+    assert len(lib.b200tts_debug_conv1d_create.argtypes) == 10
+    assert lib.b200tts_debug_conv1d_launch.argtypes[1] is ctypes.POINTER(_lib.DebugConvIOC)
+    # the struct mirrors include/tts_b200.h field for field (x64 alignment: 8-byte pointers and long longs)
+    src = open(os.path.join(ROOT, "include", "tts_b200.h")).read()
+    body = re.search(r"typedef struct \{([^{}]*)\} b200tts_debug_conv_io;", src).group(1)
+    names = re.findall(r"\*?\s*(\w+)\s*[,;]", re.sub(r"/\*.*?\*/", "", body, flags=re.S))
+    assert names == [f[0] for f in _lib.DebugConvIOC._fields_]
+    assert ctypes.sizeof(_lib.DebugConvIOC) == 216    # static_assert in capi.cu
+
+
 def test_product_fails_loudly_without_cuda():
     import pytest
     import torch

@@ -126,3 +126,118 @@ def test_fp32_calibrated_check(shape):
     bumped[-1, :, col // 2] *= 1 + 1e-3
     for got in bad + [shifted, bumped]:
         assert CC.fp32_calibrated_failures(got, want, cpu32)
+
+
+# ----------------------------------------------------------------------------- the engine-option reference
+# engine_epilogue / engine_layer (conv_check.py) restate launch_conv's documented order; test_conv_engine_epilogues_gpu.py
+# holds the kernels to them.  Here they are pinned to plain restatements of the model code they stand for, and the
+# checker is shown to reject each option applied wrongly.
+H_WN, T_WN = 96, 131
+
+
+def _wn_inputs(seed=3):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(2, H_WN, T_WN, generator=g, dtype=torch.float64)
+    w_in = torch.randn(2 * H_WN, H_WN, 5, generator=g, dtype=torch.float64) / (5 * H_WN) ** 0.5
+    b_in = torch.randn(2 * H_WN, generator=g, dtype=torch.float64) * 0.1
+    w_rs = torch.randn(2 * H_WN, H_WN, 1, generator=g, dtype=torch.float64) / H_WN ** 0.5
+    b_rs = torch.randn(2 * H_WN, generator=g, dtype=torch.float64) * 0.1
+    cond = torch.randn(2, 2 * H_WN, generator=g, dtype=torch.float64)
+    out_old = torch.randn(2, H_WN, T_WN, generator=g, dtype=torch.float64)
+    mask = torch.ones(2, T_WN, dtype=torch.float64)
+    mask[0, 100:] = 0
+    mask[1, 7:11] = 0            # zeros inside the row too
+    return x, w_in, b_in, w_rs, b_rs, cond, out_old, mask
+
+
+def _wn_layer_plain(x, w_in, b_in, w_rs, b_rs, cond, out_old, mask, dil):
+    """one WaveNet layer as wavenet.py writes it (:6-13, :98-113), not the last one"""
+    x_in = F.conv1d(x, w_in, b_in, dilation=dil, padding=2 * dil)
+    in_act = x_in + cond[:, :, None]
+    acts = torch.tanh(in_act[:, :H_WN]) * torch.sigmoid(in_act[:, H_WN:])
+    rs = F.conv1d(acts, w_rs, b_rs)
+    return acts, (x + rs[:, :H_WN]) * mask[:, None], out_old + rs[:, H_WN:]
+
+
+def _wn_layer_engine(x, w_in, b_in, w_rs, b_rs, cond, out_old, mask, dil, **mutate):
+    acts, _ = CC.engine_layer(x, w_in, b_in, dilation=dil, padding=2 * dil, cond=mutate.get("cond_override", cond),
+                              flags=CC.EPI_GATE)
+    if mutate.get("swap_gate"):
+        c = F.conv1d(x, w_in, b_in, dilation=dil, padding=2 * dil) + cond[:, :, None]
+        acts = torch.sigmoid(c[:, :H_WN]) * torch.tanh(c[:, H_WN:])
+    h, out = CC.engine_layer(acts, w_rs, b_rs, ymask=mask, flags=CC.EPI_SPLIT | CC.EPI_ACCUM2, split=H_WN,
+                             y_old=x, y2_old=out_old)
+    if mutate.get("mask_y2"):
+        out = out * mask[:, None]
+    return acts, h, out
+
+
+@pytest.mark.parametrize("dil", [1, 2])
+def test_engine_reference_is_one_wavenet_layer(dil):
+    args = _wn_inputs()
+    want = _wn_layer_plain(*args, dil)
+    got = _wn_layer_engine(*args, dil)
+    for g, w in zip(got, want):
+        torch.testing.assert_close(g, w, rtol=1e-12, atol=1e-12)
+
+
+def test_engine_reference_is_the_last_wavenet_layer_and_the_coupling_post():
+    x, w_in, b_in, w_rs, b_rs, cond, out_old, mask = _wn_inputs()
+    w_last, b_last = w_rs[:H_WN], b_rs[:H_WN]
+    # last layer: output = (output + res_skip(acts)) * x_mask
+    y, _ = CC.engine_layer(x, w_last, b_last, ymask=mask, flags=CC.EPI_MASK_POST | CC.EPI_ACCUM, y_old=out_old)
+    torch.testing.assert_close(y, (out_old + F.conv1d(x, w_last, b_last)) * mask[:, None], rtol=1e-12, atol=1e-12)
+    # coupling post (networks.py:151-164, mean_only): m = post(h) * mask; reverse x1 = (x1 - m) * mask, forward
+    # x1 = m + x1 * mask
+    x1 = out_old[:, : H_WN // 2]
+    w_post, b_post = w_rs[: H_WN // 2], b_rs[: H_WN // 2]
+    m = F.conv1d(x, w_post, b_post) * mask[:, None]
+    for scale, want in ((-1.0, (x1 - m) * mask[:, None]), (1.0, m + x1 * mask[:, None])):
+        y, _ = CC.engine_layer(x, w_post, b_post, ymask=mask, scale=scale, y_old=x1,
+                               flags=CC.EPI_MASK_PRE | CC.EPI_ACCUM | CC.EPI_MASK_POST)
+        torch.testing.assert_close(y, want, rtol=1e-12, atol=1e-12)
+
+
+def test_checker_rejects_swapped_gate_halves():
+    args = _wn_inputs()
+    want, got = _wn_layer_engine(*args, 1), _wn_layer_engine(*args, 1, swap_gate=True)
+    assert _rejected(got[0], want[0])
+
+
+def test_checker_rejects_a_dropped_cond_on_one_row():
+    args = _wn_inputs()
+    cond = args[5].clone()
+    r = H_WN + 17                                  # one row of the sigmoid half
+    cond[1, r] = 0
+    want, got = _wn_layer_engine(*args, 1), _wn_layer_engine(*args, 1, cond_override=cond)
+    fails = _rejected(got[0], want[0])
+    assert any("per-row" in f for f in fails), fails
+
+
+def test_checker_rejects_the_mask_on_y2_rows():
+    args = _wn_inputs()
+    want, got = _wn_layer_engine(*args, 1), _wn_layer_engine(*args, 1, mask_y2=True)
+    assert torch.equal(got[1], want[1])
+    assert _rejected(got[2], want[2])
+
+
+def test_checker_rejects_mask_pre_after_the_residual():
+    x, _, _, w_rs, b_rs, _, out_old, mask = _wn_inputs()
+    w, b = w_rs[: H_WN // 2], b_rs[: H_WN // 2]
+    res = out_old[:, H_WN // 2:]
+    want, _ = CC.engine_layer(x, w, b, ymask=mask, residual=res, flags=CC.EPI_MASK_PRE)
+    got = (F.conv1d(x, w, b) + res) * mask[:, None]
+    assert _rejected(got, want)
+
+
+def test_checker_rejects_a_ragged_row_one_column_short():
+    x, w_in, b_in, _, _, _, _, _ = _wn_inputs()
+    lens, rate, need = torch.tensor([T_WN, 57]), 2, 3
+    want, _ = CC.engine_layer(x, w_in[:H_WN], b_in[:H_WN], padding=2)
+    ext = CC.ragged_extent(lens, rate, need, T_WN)
+    valid = CC.columns_below(ext, T_WN)
+    got = want.clone()
+    got[1, :, int(ext[1]) - 1] = 0                 # the row's last column not computed (a zeroed buffer)
+    assert int(ext[1]) == 117
+    assert not CC.failures(torch.where(valid[:, None], want, want), want, LAYER_REL_TOL)[0]
+    assert _rejected(torch.where(valid[:, None], got, want), want)

@@ -135,6 +135,31 @@ class TacotronConfigC(ctypes.Structure):
 PADDING_MODES = {"zeros": 0, "reflect": 1}
 
 
+# b200tts_debug_conv1d_launch's arguments and its flag / activation values (B200TTS_DEBUG_* in include/tts_b200.h)
+EPI_GATE, EPI_MASK_PRE, EPI_MASK_POST, EPI_ACCUM, EPI_SPLIT, EPI_ACCUM2 = 1, 2, 4, 8, 16, 32
+ACT_NONE, ACT_RELU, ACT_TANH, ACT_LOGCLAMP = 0, 1, 2, 3
+
+
+class DebugConvIOC(ctypes.Structure):
+    _fields_ = [("x", ctypes.c_void_p), ("x_batch_stride", ctypes.c_longlong), ("x_channel_stride", ctypes.c_int),
+                ("T", ctypes.c_int),
+                ("xmask", ctypes.c_void_p), ("xmask_batch_stride", ctypes.c_longlong),
+                ("in_slope", ctypes.c_float),
+                ("cond", ctypes.c_void_p), ("cond_batch_stride", ctypes.c_longlong),
+                ("y", ctypes.c_void_p), ("y_batch_stride", ctypes.c_longlong), ("y_channel_stride", ctypes.c_int),
+                ("res", ctypes.c_void_p), ("res_batch_stride", ctypes.c_longlong), ("res_channel_stride", ctypes.c_int),
+                ("ymask", ctypes.c_void_p), ("ymask_batch_stride", ctypes.c_longlong),
+                ("y2", ctypes.c_void_p), ("y2_batch_stride", ctypes.c_longlong), ("y2_channel_stride", ctypes.c_int),
+                ("split", ctypes.c_int),
+                ("scale", ctypes.c_float), ("post_div", ctypes.c_float),
+                ("act", ctypes.c_int), ("act_param", ctypes.c_float),
+                ("flags", ctypes.c_int),
+                ("B", ctypes.c_int),
+                ("lens", ctypes.c_void_p), ("rate_out", ctypes.c_int), ("need_out", ctypes.c_int), ("rate_in", ctypes.c_int),
+                ("need_in", ctypes.c_int),
+                ("q_lo", ctypes.c_int), ("q_hi", ctypes.c_int), ("in_lo", ctypes.c_int), ("in_hi", ctypes.c_int)]
+
+
 class AudioNormC(ctypes.Structure):
     _fields_ = [("signal_norm", ctypes.c_int), ("symmetric_norm", ctypes.c_int), ("clip_norm", ctypes.c_int),
                 ("max_norm", ctypes.c_float), ("min_level_db", ctypes.c_float), ("ref_level_db", ctypes.c_float),
@@ -179,6 +204,11 @@ def _declare(lib):
     lib.b200tts_conv1d_forward_strided.restype = ci
     lib.b200tts_conv1d_forward_strided.argtypes = [vp, vp, ctypes.c_longlong, ci, ci, ci, ctypes.c_float, vp,
                                                    ctypes.c_float, ci, ctypes.c_float, ci, vp, vp, vp]
+    lib.b200tts_debug_conv1d_create.restype = ci
+    lib.b200tts_debug_conv1d_create.argtypes = [ctypes.POINTER(Conv1dConfigC), vp, vp, ci, ci, ci, ci, vp, vp,
+                                                ctypes.POINTER(vp)]
+    lib.b200tts_debug_conv1d_launch.restype = ci
+    lib.b200tts_debug_conv1d_launch.argtypes = [vp, ctypes.POINTER(DebugConvIOC), vp]
     lib.b200tts_melgan_create.restype = ci
     lib.b200tts_melgan_create.argtypes = [ctypes.POINTER(MelganConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
     lib.b200tts_melgan_destroy.restype = None

@@ -66,9 +66,14 @@ static bool valid_precision(int p) {
 }
 
 static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* weight, const float* bias, int allow_tensor_cores,
-                              int precision, b200tts_conv1d** out, int padding_mode = B200TTS_PAD_ZEROS) {
+                              int precision, b200tts_conv1d** out, int padding_mode = B200TTS_PAD_ZEROS, int gate_half = 0,
+                              const int* in_perm = nullptr, const int* out_perm = nullptr) {
     if (!cfg || !weight || !out) { set_error("conv1d_create: null argument"); return 1; }
     *out = nullptr;
+    if (cfg->transposed && (gate_half || in_perm || out_perm)) {
+        set_error("conv1d_create: gate / channel permutations need a non-transposed conv");
+        return 1;
+    }
     if (!valid_precision(precision)) { set_error("conv1d_create: unknown precision %d", precision); return 1; }
     if (padding_mode != B200TTS_PAD_ZEROS && padding_mode != B200TTS_PAD_REFLECT) {
         set_error("conv1d_create: unknown padding mode %d", padding_mode);
@@ -89,7 +94,7 @@ static int conv1d_create_impl(const b200tts_conv1d_config* cfg, const float* wei
                  ? pack_conv_transpose(h->L, weight, bias, cfg->in_channels, cfg->out_channels, cfg->kernel_size,
                                        cfg->stride, cfg->padding)
                  : pack_conv(h->L, weight, bias, cfg->out_channels, cfg->in_channels, cfg->kernel_size, cfg->dilation,
-                             cfg->padding);
+                             cfg->padding, gate_half, in_perm, out_perm);
     if (rc) { delete h; return rc; }
     *out = h;
     return 0;
@@ -160,6 +165,50 @@ int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, lon
     if (lrelu) { io.act = ACT_LRELU; io.act_param = 0.2f; }
     io.act_add = act_add;
     io.film = film; io.film_bs = film_batch_stride; io.film_cs = film_channel_stride; io.film_half = film_half;
+    return launch_conv(h->L, io, (cudaStream_t)stream);
+}
+
+int b200tts_debug_conv1d_create(const b200tts_conv1d_config* cfg, const float* weight, const float* bias,
+                                int allow_tensor_cores, int precision, int padding_mode, int gate_half,
+                                const int32_t* in_perm, const int32_t* out_perm, b200tts_conv1d** out) {
+    if (!cfg || !out) { set_error("debug_conv1d_create: null argument"); return 1; }
+    *out = nullptr;
+    auto is_perm = [](const int32_t* p, int n) {   // pack_conv writes through the permutation: it must be one
+        std::vector<char> seen(n > 0 ? n : 0, 0);
+        for (int i = 0; i < n; ++i) {
+            if (p[i] < 0 || p[i] >= n || seen[p[i]]) return false;
+            seen[p[i]] = 1;
+        }
+        return true;
+    };
+    if ((in_perm && !is_perm(in_perm, cfg->in_channels)) || (out_perm && !is_perm(out_perm, cfg->out_channels))) {
+        set_error("debug_conv1d_create: in_perm / out_perm must be permutations of the channels");
+        return 1;
+    }
+    return conv1d_create_impl(cfg, weight, bias, allow_tensor_cores, precision, out, padding_mode, gate_half, in_perm,
+                              out_perm);
+}
+static_assert(sizeof(b200tts_debug_conv_io) == 216, "tts_b200/_lib.py DebugConvIOC mirrors this layout");
+int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, void* stream) {
+    if (!h || !d) { set_error("debug_conv1d_launch: null argument"); return 1; }
+    ConvIO io;
+    io.x = d->x; io.x_bs = d->x_batch_stride; io.x_cs = d->x_channel_stride; io.Tin = d->T;
+    io.xmask = d->xmask; io.xmask_bs = d->xmask_batch_stride; io.in_slope = d->in_slope;
+    io.cond = d->cond; io.cond_bs = d->cond_batch_stride;
+    io.y = d->y; io.y_bs = d->y_batch_stride; io.y_cs = d->y_channel_stride; io.Tout = b200tts_conv1d_out_len(h, d->T);
+    io.res = d->res; io.res_bs = d->res_batch_stride; io.res_cs = d->res_channel_stride;
+    io.ymask = d->ymask; io.ymask_bs = d->ymask_batch_stride;
+    io.y2 = d->y2; io.y2_bs = d->y2_batch_stride; io.y2_cs = d->y2_channel_stride;
+    io.split = d->split; io.scale = d->scale; io.post_div = d->post_div;
+    io.act = d->act; io.act_param = d->act_param; io.flags = d->flags; io.B = d->B;
+    io.lens = d->lens; io.rate_out = d->rate_out; io.need_out = d->need_out; io.rate_in = d->rate_in; io.need_in = d->need_in;
+    io.q_lo = d->q_lo; io.q_hi = d->q_hi; io.in_lo = d->in_lo; io.in_hi = d->in_hi;
+    io.reflect = h->reflect;
+    if (io.flags & ~(EPI_GATE | EPI_MASK_PRE | EPI_MASK_POST | EPI_ACCUM | EPI_SPLIT | EPI_ACCUM2) ||
+        !(io.act >= ACT_NONE && io.act <= ACT_LOGCLAMP)) {
+        set_error("debug_conv1d_launch: unknown flags 0x%x or act %d", io.flags, io.act);
+        return 1;
+    }
     return launch_conv(h->L, io, (cudaStream_t)stream);
 }
 

@@ -81,6 +81,8 @@ inline void count_launch(int n = 1) { g_launch_count += (unsigned long long)n; }
 //            SPLIT (WN res/skip): rows <  split -> (y , accum=1, mask_post=1)
 //                                 rows >= split -> (y2, accum=accum2, no mask), row index -= split
 //            ups > 1 (polyphase transposed conv): row r -> channel r/ups, time q*ups + r%ups
+//            launch_conv rejects what some kernel family would silently ignore: ymask without MASK_PRE / MASK_POST /
+//            SPLIT, and GATE with ymask, another flag, a residual, an act, scale or post_div (no engine sends these)
 //            WAVEGRAD (EPI_WAVEGRAD / ConvIO::near_src): v = acc + bias; [lrelu(v, act_param)]; [+ act_add[b]]; [+ res];
 //                       [y2 <- v]; [v = shift + scale * v]; y <- v   (own kernel variants, see ConvIO)
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3,   // LOGCLAMP: log(max(v, act_param))

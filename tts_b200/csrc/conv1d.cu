@@ -1044,8 +1044,13 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
                  "launch_conv: masked/split epilogue needs ymask");
     B200_REQUIRE(!(a.flags & EPI_SPLIT) || io.y2, "launch_conv: split epilogue needs y2");
     B200_REQUIRE(!(io.ymask && L.ups > 1), "launch_conv: output mask with an upsampling layer is not supported");
+    // a mask without a flag saying where it applies: the FMA plain epilogue would apply it, the others would not
+    B200_REQUIRE(!io.ymask || (a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)),
+                 "launch_conv: ymask needs EPI_MASK_PRE, EPI_MASK_POST or EPI_SPLIT");
     if (a.flags & EPI_GATE) {
-        B200_REQUIRE(L.ups == 1 && !io.res && a.act == ACT_NONE, "launch_conv: gate epilogue takes no other options");
+        B200_REQUIRE(L.ups == 1 && !io.res && !io.ymask && a.act == ACT_NONE && a.flags == EPI_GATE && a.scale == 1.f &&
+                         a.post_div == 1.f,
+                     "launch_conv: gate epilogue takes no other options");
         if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;
         return launch_cic<KEPI_GATE>(a, L.co_tile, io.B, L.RowsPad, st);
     }
