@@ -131,6 +131,7 @@ template <class T> class DevBuf {
 template <class T> inline int upload(DevBuf<T>& dst, const T* src, size_t n) {
     dst = DevBuf<T>();
     if (n == 0) return 0;
+    B200_REQUIRE(src, "upload: null host array of %zu elements", n);
     B200_CUDA_OK(dst.alloc(n));
     B200_CUDA_OK(cudaMemcpy(dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
     return 0;
@@ -273,5 +274,21 @@ template <class F> size_t arena_size(F&& f) {
     f(ar);
     return ar.off;
 }
+
+// ------------------------------------------------------------------ cursor over an engine's weight list
+// Every engine's init reads its flat weight list (order: include/tts_b200.h) front to back through one cursor, which its
+// components take by reference, so the reads are the only description of the order.  Past the end take() returns null
+// and keeps counting; whatever reads a taken pointer on the host refuses a null it cannot accept.  finish() then checks
+// the list's length against the reads.
+struct WeightList {
+    const float* const* w; int n; int pos = 0;   // pos > n: the reads ran past the end
+    WeightList(const float* const* list, int count) : w(list), n(count) {}
+    const float* take() { const int i = pos++; return i < n ? w[i] : nullptr; }
+    int finish(const char* who) const {
+        B200_REQUIRE(pos <= n, "%s: the weight list ends after %d tensors; the config reads more", who, n);
+        B200_REQUIRE(pos == n, "%s: expected %d weight tensors, got %d", who, pos, n);
+        return 0;
+    }
+};
 
 }  // namespace b200tts

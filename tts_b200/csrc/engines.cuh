@@ -45,7 +45,7 @@ struct WaveNet {
     ConvLayer cond;
     std::vector<ConvLayer> in_layers, res_skip;
     int init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels,
-             const float* const* w, int* consumed);
+             WeightList& wl);
     int forward(float* h, float* out, const float* mask, const float* g, int B, int T, float* acts, float* condv,
                 cudaStream_t st, const int* lens = nullptr) const;
 };
@@ -83,6 +83,7 @@ struct DurPred {
     ConvLayer conv1, conv2, proj, cond, cond_lang;
     DevBuf<float> g1, b1, g2, b2;
     int init(const b200tts_duration_predictor_config& cfg, const float* const* w, int nw);
+    int init(const b200tts_duration_predictor_config& cfg, WeightList& wl);   // as a component of a larger model
     size_t workspace_bytes(int B, int T) const;
     int forward(const float* x, const float* mask, const float* g, const float* lang_emb, int B, int T, float* logw,
                 void* ws, size_t ws_bytes, cudaStream_t st) const;
@@ -111,10 +112,10 @@ struct RelPosTransformer {
     int C = 0, F = 0, heads = 0, window = -1;   // window < 0: no relative-position terms
     float eps = 0.f;
     std::vector<Layer> layers;
-    // w per layer: emb_rel_k [1,2w+1,d], emb_rel_v (window >= 0 only), conv_q.w/.b, conv_k.w/.b, conv_v.w/.b,
+    // wl per layer: emb_rel_k [1,2w+1,d], emb_rel_v (window >= 0 only), conv_q.w/.b, conv_k.w/.b, conv_v.w/.b,
     // conv_o.w/.b, norm_1.gamma/.beta, ffn.conv_1.w/.b, ffn.conv_2.w/.b, norm_2.gamma/.beta
     int init(int channels, int ffn_channels, int kernel_size, int num_heads, int window, float eps, int num_layers,
-             const float* const* w, int* consumed);
+             WeightList& wl);
     size_t workspace_bytes(int B, int T) const;   // q|k|v, attention output, y, FFN hidden
     // x [B, C, T], already masked: every layer in place; x is left masked
     int forward(float* x, const float* x_mask, int B, int T, void* ws, size_t ws_bytes, cudaStream_t st) const;
@@ -136,7 +137,7 @@ struct DDSConv {
     int C = 0, K = 0, L = 0;
     std::vector<ConvLayer> conv1x1;
     std::vector<DevBuf<float>> sep_w, sep_b, g1, b1, g2, b2;
-    int init(int channels, int kernel_size, int num_layers, const float* const* w, int* consumed);
+    int init(int channels, int kernel_size, int num_layers, WeightList& wl);
     int forward(float* x, const float* mask, int B, int T, float* y1, float* y2, cudaStream_t st) const;
 };
 
@@ -218,9 +219,9 @@ struct GlowDecoder {
     };
     int Cs = 0, Hd = 0, ns = 0, nsq = 0, sigmoid_scale = 0;   // Cs: squeezed channels out_channels * num_squeeze
     std::vector<Block> blocks;
-    // w: per block ActNorm logs, bias, InvConvNear^-1, start.w, .b, WaveNet, end.w, .b (see b200tts_glow_tts_config)
+    // wl: per block ActNorm logs, bias, InvConvNear^-1, start.w, .b, WaveNet, end.w, .b (see b200tts_glow_tts_config)
     int init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
-             int cond_channels, int num_splits, int num_squeeze, int sigmoid_scale, const float* const* w, int* consumed);
+             int cond_channels, int num_splits, int num_squeeze, int sigmoid_scale, WeightList& wl);
     size_t workspace_bytes(int B, int Tq) const;
     // z [B, Cs, Tq] (overwritten), msk [B, Tq] -> mel [B, C, Tv * num_squeeze]
     int reverse(float* z, const float* msk, const float* g, int B, int Tq, int Tv, float* mel, void* ws, size_t ws_bytes,
@@ -322,7 +323,7 @@ struct BiGruArgs {
     int T = 0;
 };
 // one direction's W_hh [3H][H] (torch layout) -> dst [3 * 32][BIGRU_THREADS], the kernel's shared-memory image
-void pack_bigru_whh(const float* whh, float* dst);
+int pack_bigru_whh(const float* whh, float* dst);
 int launch_bigru(const BiGruArgs& a, int B, cudaStream_t st);
 // y[b, c, n] = x[b, n, c] for x [B, N, E]
 int launch_transpose(const float* x, float* y, int B, int N, int E, cudaStream_t st);
@@ -333,11 +334,11 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
                    const std::function<int(cudaStream_t, int, bool)>& step, const int* ctl, int B, std::vector<int>& host,
                    cudaStream_t st);
 
-// An eval-mode BatchNorm folded into the layer before it (recurrent.cu): w [Cout][row] (row = Cin * K), bias [Cout] or
-// null, bn -> {gamma, beta, running_mean, running_var} [Cout].  wf = w * s, bf = beta - mean * s (no bias) or
-// (bias - mean) * s + beta, s = gamma / sqrt(var + eps), in double.
-void fold_bn(const float* w, const float* bias, const float* const* bn, double eps, int Cout, size_t row,
-             std::vector<float>& wf, std::vector<float>& bf);
+// An eval-mode BatchNorm folded into the layer before it (recurrent.cu), taking from wl: w [Cout][row] (row = Cin * K),
+// bias [Cout] when has_bias, then gamma, beta, running_mean, running_var [Cout].  wf = w * s, bf = beta - mean * s (no
+// bias) or (bias - mean) * s + beta, s = gamma / sqrt(var + eps), in double.
+int fold_bn(WeightList& wl, bool has_bias, double eps, int Cout, size_t row, std::vector<float>& wf,
+            std::vector<float>& bf);
 
 // The Tacotron2 text encoder (TTS/tts/layers/tacotron/tacotron2.py:73-112, also Overflow's encoder): embedding,
 // n_convs x (conv k5 with BatchNorm folded -> ReLU), the LSTM input projection of both directions as one 1x1 conv, then
@@ -347,9 +348,9 @@ struct SeqEncoder {
     DevBuf<float> emb;
     ConvLayer convs[8], lstm_in;
     DevBuf<float> whh;                            // [2][4H][H]
-    // w: emb [n_vocab, E]; per conv: weight [E, E, 5], bias, BN weight, bias, running_mean, running_var;
+    // wl: emb [n_vocab, E]; per conv: weight [E, E, 5], bias, BN weight, bias, running_mean, running_var;
     // lstm weight_ih, weight_hh, bias_ih, bias_hh, then the same four _reverse
-    int init(int n_vocab, int E, int H, int n_convs, const float* const* w, int* consumed);
+    int init(int n_vocab, int E, int H, int n_convs, WeightList& wl);
     // encode's scratch, carved by the parent model: the conv stack's two tensors and mask, the LSTM input projection,
     // h (double-buffered) and c
     struct Scratch { float *x, *y, *xmask, *pre, *hb, *cb; };
@@ -412,12 +413,9 @@ struct TacoAttention {
     DevBuf<float> wq, bq, v, wc, wd;           // query_layer, its bias (DCA), v, location conv and dense
     DevBuf<float> prior, wk, ws, wsl, wdl, bdl;   // DCA: prior, key_layer, static conv / layer, dynamic layer
     float vb = 0.f;                            // v's bias (original attention)
-    // the number of weight tensors init reads
-    static int n_weights(int type, int location);
-    // w, original: query_layer, inputs_layer, v.weight, v.bias[, location_conv1d, location_dense]; DCA: prior,
-    // query_layer.weight, .bias, key_layer, static_filter_conv, static_filter_layer, dynamic_filter_layer.weight, .bias,
-    // v; *consumed = n_weights(type, location)
-    int init(int Q, int E, int type, int location, int softmax, const float* const* w, int* consumed);
+    // wl, original: query_layer, inputs_layer, v.weight, v.bias[, location_conv1d, location_dense]; DCA: prior,
+    // query_layer.weight, .bias, key_layer, static_filter_conv, static_filter_layer, dynamic_filter_layer.weight, .bias, v
+    int init(int Q, int E, int type, int location, int softmax, WeightList& wl);
     // the step-invariant keys pin [B, 128, Tt] = inputs_layer(enc) for every token (original attention; DCA: nothing),
     // through encT [B, E, Tt]
     int keys(const float* enc, float* encT, float* pin, int B, int Tt, cudaStream_t st) const;
@@ -470,7 +468,7 @@ struct Tacotron {
         DevBuf<float> pre_w;                   // pre_highway transposed [Cin][128] (empty: none)
         DevBuf<float> hw_w, hw_b;              // per highway [H | T] transposed [128][256], bias [256]
         DevBuf<float> whh, bhn;                // pack_bigru_whh images of both directions, b_hn [2][128]
-        int init(int Cin, int K, int P1, const float* const* w, int* consumed);
+        int init(int Cin, int K, int P1, WeightList& wl);
         // run's scratch, carved by the model: the bank and projection outputs, the highway output, the biGRU input
         struct Scratch { float *bank, *y2, *y3, *hx, *pre; };
         Scratch carve(Arena& ar, int B, int T) const;

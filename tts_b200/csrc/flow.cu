@@ -8,33 +8,30 @@
 
 namespace b200tts {
 
-// w: [cond.w, cond.b] (if cond_channels) then per layer: in.w, in.b, rs.w, rs.b.  Returns tensors consumed.
-int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels,
-                  const float* const* w, int* consumed) {
+// wl: [cond.w, cond.b] (if cond_channels) then per layer: in.w, in.b, rs.w, rs.b
+int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers, int cond_channels, WeightList& wl) {
     H = hidden; K = kernel_size; L = num_layers; cond_ch = cond_channels;
-    int i = 0;
     int rc;
     if (cond_ch > 0) {
         // rows of cond_layer are sliced per layer (wavenet.py:104-105) and must follow the gate interleave
         std::vector<int> perm(2 * H * L);
         for (int l = 0; l < L; ++l)
             for (int r = 0; r < 2 * H; ++r) perm[l * 2 * H + r] = l * 2 * H + (r < H ? 2 * r : 2 * (r - H) + 1);
-        if ((rc = pack_conv(cond, w[i], w[i + 1], 2 * H * L, cond_ch, 1, 1, 0, 0, nullptr, perm.data()))) return rc;
-        i += 2;
+        const float *cw = wl.take(), *cb = wl.take();
+        if ((rc = pack_conv(cond, cw, cb, 2 * H * L, cond_ch, 1, 1, 0, 0, nullptr, perm.data()))) return rc;
     }
     in_layers.resize(L);
     res_skip.resize(L);
     int d = 1;
     for (int l = 0; l < L; ++l) {
         in_layers[l].tc_prec = res_skip[l].tc_prec = B200TTS_PRECISION_FP32;   // ~85% of the flow FLOPs (k5, 192 -> 384)
-        if ((rc = pack_conv(in_layers[l], w[i], w[i + 1], 2 * H, H, K, d, (K * d - d) / 2, /*gate_half=*/H))) return rc;
-        i += 2;
+        const float *iw = wl.take(), *ib = wl.take();
+        if ((rc = pack_conv(in_layers[l], iw, ib, 2 * H, H, K, d, (K * d - d) / 2, /*gate_half=*/H))) return rc;
         const int rows = (l < L - 1) ? 2 * H : H;
-        if ((rc = pack_conv(res_skip[l], w[i], w[i + 1], rows, H, 1, 1, 0))) return rc;
-        i += 2;
+        const float *rw = wl.take(), *rb = wl.take();
+        if ((rc = pack_conv(res_skip[l], rw, rb, rows, H, 1, 1, 0))) return rc;
         d *= dilation_rate;
     }
-    *consumed = i;
     return 0;
 }
 
@@ -82,8 +79,7 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
     c = cfg;
     fwd = forward_direction != 0;
     B200_REQUIRE(c.channels % 2 == 0 && c.num_flows >= 1 && c.num_layers >= 1, "flow: unsupported config");
-    const int per = 2 + (c.cond_channels > 0 ? 2 : 0) + 4 * c.num_layers + 2;
-    B200_REQUIRE(nw == per * c.num_flows, "flow: expected %d weight tensors, got %d", per * c.num_flows, nw);
+    WeightList wl(w, nw);
     const int half = c.channels / 2;
     std::vector<int> rev(half);
     for (int i = 0; i < half; ++i) rev[i] = half - 1 - i;
@@ -93,20 +89,18 @@ int Flow::init(const b200tts_flow_config& cfg, const float* const* w, int nw, in
         // reverse pass applies flows F-1 .. 0, each after one more flip: block n sees (F - n) flips;
         // the forward pass (networks.py:223-227) flips after each block: block n sees n flips
         b.odd = fwd ? (n % 2) == 1 : ((c.num_flows - n) % 2) == 1;
-        const float* const* wn = w + (size_t)n * per;
-        int rc, used = 0;
+        int rc;
         b.pre.tc_prec = b.post.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(b.pre, wn[0], wn[1], c.hidden_channels, half, 1, 1, 0, 0, b.odd ? rev.data() : nullptr,
-                            nullptr)))
+        const float *pw = wl.take(), *pb = wl.take();
+        if ((rc = pack_conv(b.pre, pw, pb, c.hidden_channels, half, 1, 1, 0, 0, b.odd ? rev.data() : nullptr, nullptr)))
             return rc;
-        if ((rc = b.wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, wn + 2,
-                             &used)))
+        if ((rc = b.wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, wl)))
             return rc;
-        if ((rc = pack_conv(b.post, wn[2 + used], wn[3 + used], half, c.hidden_channels, 1, 1, 0, 0, nullptr,
-                            b.odd ? rev.data() : nullptr)))
+        const float *qw = wl.take(), *qb = wl.take();
+        if ((rc = pack_conv(b.post, qw, qb, half, c.hidden_channels, 1, 1, 0, 0, nullptr, b.odd ? rev.data() : nullptr)))
             return rc;
     }
-    return 0;
+    return wl.finish("flow");
 }
 
 // the scratch of a hidden-width stage around one WaveNet (Flow, PosteriorEnc): its input h, the gated activations, its
@@ -187,14 +181,15 @@ __global__ void sample_posterior_kernel(const float* stats, const float* noise, 
 // weights: pre.w [H,Cin,1], pre.b, enc.* (WaveNet order), proj.w [2*out,H,1], proj.b
 int PosteriorEnc::init(const b200tts_posterior_config& cfg, const float* const* w, int nw) {
     c = cfg;
-    const int expect = 2 + (c.cond_channels > 0 ? 2 : 0) + 4 * c.num_layers + 2;
-    B200_REQUIRE(nw == expect, "posterior_encoder: expected %d weight tensors, got %d", expect, nw);
-    int rc, used = 0;
+    WeightList wl(w, nw);
+    int rc;
     pre.tc_prec = proj.tc_prec = B200TTS_PRECISION_FP32;
-    if ((rc = pack_conv(pre, w[0], w[1], c.hidden_channels, c.in_channels, 1, 1, 0))) return rc;
-    if ((rc = wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, w + 2, &used))) return rc;
-    if ((rc = pack_conv(proj, w[2 + used], w[3 + used], 2 * c.out_channels, c.hidden_channels, 1, 1, 0))) return rc;
-    return 0;
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(pre, pw, pb, c.hidden_channels, c.in_channels, 1, 1, 0))) return rc;
+    if ((rc = wn.init(c.hidden_channels, c.kernel_size, c.dilation_rate, c.num_layers, c.cond_channels, wl))) return rc;
+    const float *qw = wl.take(), *qb = wl.take();
+    if ((rc = pack_conv(proj, qw, qb, 2 * c.out_channels, c.hidden_channels, 1, 1, 0))) return rc;
+    return wl.finish("posterior_encoder");
 }
 
 size_t PosteriorEnc::workspace_bytes(int B, int T) const {

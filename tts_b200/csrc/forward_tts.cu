@@ -123,20 +123,20 @@ int launch_add_norm(const float* x, const float* y, bool twice, const float* g, 
     return 0;
 }
 
-int pack_layer(ForwardTTS::Layer& L, const float* const* p, int C, int F, int prec) {
+int pack_layer(ForwardTTS::Layer& L, WeightList& wl, int C, int F, int prec) {
     int rc;
     L.qkv.tc_prec = L.o.tc_prec = L.ffn1.tc_prec = L.ffn2.tc_prec = prec;
-    if ((rc = pack_conv(L.qkv, p[0], p[1], 3 * C, C, 1, 1, 0))) return rc;   // in_proj rows q | k | v
-    if ((rc = pack_conv(L.o, p[2], p[3], C, C, 1, 1, 0))) return rc;
-    if ((rc = pack_conv(L.ffn1, p[4], p[5], F, C, 3, 1, 1))) return rc;
-    if ((rc = pack_conv(L.ffn2, p[6], p[7], C, F, 3, 1, 1))) return rc;
-    if ((rc = upload(L.ln1_g, p[8], C))) return rc;
-    if ((rc = upload(L.ln1_b, p[9], C))) return rc;
-    if ((rc = upload(L.ln2_g, p[10], C))) return rc;
-    return upload(L.ln2_b, p[11], C);
+    const float *qw = wl.take(), *qb = wl.take(), *ow = wl.take(), *ob = wl.take(), *f1w = wl.take(), *f1b = wl.take(),
+                *f2w = wl.take(), *f2b = wl.take();
+    if ((rc = pack_conv(L.qkv, qw, qb, 3 * C, C, 1, 1, 0))) return rc;   // in_proj rows q | k | v
+    if ((rc = pack_conv(L.o, ow, ob, C, C, 1, 1, 0))) return rc;
+    if ((rc = pack_conv(L.ffn1, f1w, f1b, F, C, 3, 1, 1))) return rc;
+    if ((rc = pack_conv(L.ffn2, f2w, f2b, C, F, 3, 1, 1))) return rc;
+    if ((rc = upload(L.ln1_g, wl.take(), C))) return rc;
+    if ((rc = upload(L.ln1_b, wl.take(), C))) return rc;
+    if ((rc = upload(L.ln2_g, wl.take(), C))) return rc;
+    return upload(L.ln2_b, wl.take(), C);
 }
-
-constexpr int PER_LAYER = 12;
 
 }  // namespace
 
@@ -154,47 +154,42 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
                  "forward_tts: bad pitch predictor config");
     B200_REQUIRE(!c.use_energy || (c.energy_hidden > 0 && c.energy_kernel >= 1 && c.energy_emb_kernel % 2 == 1),
                  "forward_tts: bad energy predictor config");
-    const int expect = 1 + PER_LAYER * c.enc_layers + (c.proj_g_in > 0 ? 2 : 0) + 10 + (c.use_pitch ? 12 : 0) +
-                       (c.use_energy ? 12 : 0) + (c.pe_len > 0 ? 1 : 0) + PER_LAYER * c.dec_layers + 2;
-    B200_REQUIRE(nw == expect, "forward_tts: expected %d weight tensors, got %d", expect, nw);
+    WeightList wl(w, nw);
     int rc;
-    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * C))) return rc;
-    int i = 1;
+    if ((rc = upload(emb, wl.take(), (size_t)c.n_vocab * C))) return rc;
     enc.resize(c.enc_layers);
-    for (int l = 0; l < c.enc_layers; ++l, i += PER_LAYER)
-        if ((rc = pack_layer(enc[l], w + i, C, c.enc_ffn, TC_NONE))) return rc;
+    for (int l = 0; l < c.enc_layers; ++l)
+        if ((rc = pack_layer(enc[l], wl, C, c.enc_ffn, TC_NONE))) return rc;
     if (c.proj_g_in > 0) {   // nn.Linear(d_vector_dim, C) as a 1x1 conv over a one-column input
-        if ((rc = pack_conv(proj_g, w[i], w[i + 1], C, c.proj_g_in, 1, 1, 0))) return rc;
-        i += 2;
+        const float *gw = wl.take(), *gb = wl.take();
+        if ((rc = pack_conv(proj_g, gw, gb, C, c.proj_g_in, 1, 1, 0))) return rc;
     }
     {
         b200tts_duration_predictor_config dc{C, c.dp_hidden, c.dp_kernel, 0, 0};
-        if ((rc = dp.init(dc, w + i, 10))) return rc;
-        i += 10;
+        if ((rc = dp.init(dc, wl))) return rc;
     }
     if (c.use_pitch) {
         b200tts_duration_predictor_config dc{C, c.pitch_hidden, c.pitch_kernel, 0, 0};
-        if ((rc = pitch_dp.init(dc, w + i, 10))) return rc;
+        if ((rc = pitch_dp.init(dc, wl))) return rc;
         const int k = c.pitch_emb_kernel;
-        if ((rc = pack_conv(pitch_emb, w[i + 10], w[i + 11], C, 1, k, 1, (k - 1) / 2))) return rc;
-        i += 12;
+        const float *ew = wl.take(), *eb = wl.take();
+        if ((rc = pack_conv(pitch_emb, ew, eb, C, 1, k, 1, (k - 1) / 2))) return rc;
     }
     if (c.use_energy) {
         b200tts_duration_predictor_config dc{C, c.energy_hidden, c.energy_kernel, 0, 0};
-        if ((rc = energy_dp.init(dc, w + i, 10))) return rc;
+        if ((rc = energy_dp.init(dc, wl))) return rc;
         const int k = c.energy_emb_kernel;
-        if ((rc = pack_conv(energy_emb, w[i + 10], w[i + 11], C, 1, k, 1, (k - 1) / 2))) return rc;
-        i += 12;
+        const float *ew = wl.take(), *eb = wl.take();
+        if ((rc = pack_conv(energy_emb, ew, eb, C, 1, k, 1, (k - 1) / 2))) return rc;
     }
-    if (c.pe_len > 0) {
-        if ((rc = upload(pe, w[i], (size_t)C * c.pe_len))) return rc;
-        i += 1;
-    }
+    if (c.pe_len > 0 && (rc = upload(pe, wl.take(), (size_t)C * c.pe_len))) return rc;
     dec.resize(c.dec_layers);
-    for (int l = 0; l < c.dec_layers; ++l, i += PER_LAYER)
-        if ((rc = pack_layer(dec[l], w + i, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
+    for (int l = 0; l < c.dec_layers; ++l)
+        if ((rc = pack_layer(dec[l], wl, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
     postnet.tc_prec = B200TTS_PRECISION_FP32;
-    return pack_conv(postnet, w[i], w[i + 1], c.out_channels, C, 1, 1, 0);
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(postnet, pw, pb, c.out_channels, C, 1, 1, 0))) return rc;
+    return wl.finish("forward_tts");
 }
 
 // the encoder layers' scratch, the projected speaker vector and one block the duration, pitch and energy predictors

@@ -107,29 +107,26 @@ __global__ void flow_step_kernel(const float* __restrict__ x, const float* __res
 }  // namespace
 
 int GlowDecoder::init(int out_channels, int hidden, int kernel_size, int dilation_rate, int num_blocks, int num_layers,
-                      int cond_channels, int num_splits, int num_squeeze, int sigmoid, const float* const* w,
-                      int* consumed) {
+                      int cond_channels, int num_splits, int num_squeeze, int sigmoid, WeightList& wl) {
     Cs = out_channels * num_squeeze;
     Hd = hidden; ns = num_splits; nsq = num_squeeze; sigmoid_scale = sigmoid;
     B200_REQUIRE(ns >= 2 && ns % 2 == 0 && ns <= MAX_SPLITS && Cs % ns == 0,
                  "glow decoder: num_splits %d must be even, <= %d and divide out_channels * num_squeeze = %d", ns,
                  MAX_SPLITS, Cs);
-    const int per_block = 3 + 2 + (cond_channels > 0 ? 2 : 0) + 4 * num_layers + 2;
     int rc;
     blocks.resize(num_blocks);
     for (int n = 0; n < num_blocks; ++n) {
-        const float* const* p = w + n * per_block;
         Block& b = blocks[n];
-        if ((rc = upload(b.an_logs, p[0], Cs))) return rc;
-        if ((rc = upload(b.an_bias, p[1], Cs))) return rc;
-        if ((rc = upload(b.mix, p[2], (size_t)ns * ns))) return rc;
+        if ((rc = upload(b.an_logs, wl.take(), Cs))) return rc;
+        if ((rc = upload(b.an_bias, wl.take(), Cs))) return rc;
+        if ((rc = upload(b.mix, wl.take(), (size_t)ns * ns))) return rc;
         b.start.tc_prec = b.end.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(b.start, p[3], p[4], Hd, Cs / 2, 1, 1, 0))) return rc;
-        int used = 0;
-        if ((rc = b.wn.init(Hd, kernel_size, dilation_rate, num_layers, cond_channels, p + 5, &used))) return rc;
-        if ((rc = pack_conv(b.end, p[5 + used], p[6 + used], Cs, Hd, 1, 1, 0))) return rc;
+        const float *sw = wl.take(), *sb = wl.take();
+        if ((rc = pack_conv(b.start, sw, sb, Hd, Cs / 2, 1, 1, 0))) return rc;
+        if ((rc = b.wn.init(Hd, kernel_size, dilation_rate, num_layers, cond_channels, wl))) return rc;
+        const float *ew = wl.take(), *eb = wl.take();
+        if ((rc = pack_conv(b.end, ew, eb, Cs, Hd, 1, 1, 0))) return rc;
     }
-    *consumed = per_block * num_blocks;
     return 0;
 }
 
@@ -199,49 +196,39 @@ int GlowTTS::init(const b200tts_glow_tts_config& cfg, const float* const* w, int
     B200_REQUIRE(ns >= 2 && ns % 2 == 0 && ns <= MAX_SPLITS && Cs % ns == 0,
                  "glow_tts: num_splits %d must be even, <= %d and divide out_channels * num_squeeze = %d", ns, MAX_SPLITS,
                  Cs);
-    const int per_layer = 16;
-    const int per_block = 3 + 2 + (cin > 0 ? 2 : 0) + 4 * c.num_block_layers + 2;
-    const int expect = 1 + (c.use_prenet ? 14 : 0) + per_layer * c.num_layers_enc + (c.mean_only ? 2 : 4) + 10 +
-                       per_block * c.num_flow_blocks;
-    B200_REQUIRE(nw == expect, "glow_tts: expected %d weight tensors, got %d", expect, nw);
+    WeightList wl(w, nw);
     int rc;
-    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * H))) return rc;
-    int i = 1;
+    if ((rc = upload(emb, wl.take(), (size_t)c.n_vocab * H))) return rc;
     if (c.use_prenet) {   // ResidualConv1dLayerNormBlock(H, H, H, kernel_size=5, num_layers=3), encoder.py:107-110
         prenet.resize(3);
         for (auto& p : prenet) {
-            if ((rc = pack_conv(p.conv, w[i], w[i + 1], H, H, 5, 1, 2))) return rc;
-            if ((rc = upload(p.g, w[i + 2], H))) return rc;
-            if ((rc = upload(p.b, w[i + 3], H))) return rc;
-            i += 4;
+            const float *pw = wl.take(), *pb = wl.take();
+            if ((rc = pack_conv(p.conv, pw, pb, H, H, 5, 1, 2))) return rc;
+            if ((rc = upload(p.g, wl.take(), H))) return rc;
+            if ((rc = upload(p.b, wl.take(), H))) return rc;
         }
-        if ((rc = pack_conv(prenet_proj, w[i], w[i + 1], H, H, 1, 1, 0))) return rc;
-        i += 2;
+        const float *pw = wl.take(), *pb = wl.take();
+        if ((rc = pack_conv(prenet_proj, pw, pb, H, H, 1, 1, 0))) return rc;
     }
-    int used = 0;
-    if ((rc = tf.init(H, F, K, c.num_heads, -1, 1e-4f, c.num_layers_enc, w + i, &used))) return rc;
-    i += used;
+    if ((rc = tf.init(H, F, K, c.num_heads, -1, 1e-4f, c.num_layers_enc, wl))) return rc;
     {   // [proj_m | proj_s]: with mean_only the log-scale rows are zero weights and bias, i.e. zeros_like(x_m) (:176)
         std::vector<float> wp((size_t)2 * C * H, 0.f), bp((size_t)2 * C, 0.f);
-        memcpy(wp.data(), w[i], sizeof(float) * C * H);
-        memcpy(bp.data(), w[i + 1], sizeof(float) * C);
-        i += 2;
-        if (!c.mean_only) {
-            memcpy(wp.data() + (size_t)C * H, w[i], sizeof(float) * C * H);
-            memcpy(bp.data() + C, w[i + 1], sizeof(float) * C);
-            i += 2;
+        for (int s = 0; s < (c.mean_only ? 1 : 2); ++s) {
+            const float *sw = wl.take(), *sb = wl.take();
+            B200_REQUIRE(sw && sb, "glow_tts: null proj_m / proj_s weight or bias");
+            memcpy(wp.data() + (size_t)s * C * H, sw, sizeof(float) * C * H);
+            memcpy(bp.data() + (size_t)s * C, sb, sizeof(float) * C);
         }
         if ((rc = pack_conv(proj, wp.data(), bp.data(), 2 * C, H, 1, 1, 0))) return rc;
     }
     {   // DurationPredictor(H + c_in, hidden_channels_dp, 3): the speaker vector is concatenated, not added (:139-141)
         b200tts_duration_predictor_config dc{H + cin, c.hidden_channels_dp, 3, 0, 0};
-        if ((rc = dp.init(dc, w + i, 10))) return rc;
-        i += 10;
+        if ((rc = dp.init(dc, wl))) return rc;
     }
     if ((rc = dec.init(C, Hd, c.kernel_size_dec, c.dilation_rate, c.num_flow_blocks, c.num_block_layers, cin, ns, nsq,
-                       c.sigmoid_scale, w + i, &used)))
+                       c.sigmoid_scale, wl)))
         return rc;
-    return 0;
+    return wl.finish("glow_tts");
 }
 
 // x, cat(x, g), the duration predictor's and the transformer's blocks; the prenet runs before the transformer, so its

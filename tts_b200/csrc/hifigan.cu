@@ -24,18 +24,15 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
                      c.num_dilations >= 1 && c.num_dilations <= 8,
                  "hifigan: unsupported config");
     const int type1 = (c.resblock_type == 1);
-    const int expect = 2 + (c.cond_channels > 0 ? 2 : 0) + 2 * c.num_upsamples +
-                       c.num_upsamples * c.num_kernels * c.num_dilations * (type1 ? 4 : 2) + 2;
-    B200_REQUIRE(nw == expect, "hifigan: expected %d weight tensors, got %d", expect, nw);
-    int i = 0;
+    WeightList wl(w, nw);
     conv_pre.tc_prec = lp;
-    int rc = pack_conv(conv_pre, w[i], w[i + 1], c.upsample_initial_channel, c.in_channels, 7, 1, 3);
+    const float *pw = wl.take(), *pb = wl.take();
+    int rc = pack_conv(conv_pre, pw, pb, c.upsample_initial_channel, c.in_channels, 7, 1, 3);
     if (rc) return rc;
-    i += 2;
     if (c.cond_channels > 0) {
-        rc = pack_conv(cond, w[i], w[i + 1], c.upsample_initial_channel, c.cond_channels, 1, 1, 0);
+        const float *cw = wl.take(), *cb = wl.take();
+        rc = pack_conv(cond, cw, cb, c.upsample_initial_channel, c.cond_channels, 1, 1, 0);
         if (rc) return rc;
-        i += 2;
     }
     ups.resize(c.num_upsamples);
     rb_c1.resize(c.num_upsamples * c.num_kernels);
@@ -44,9 +41,9 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int u = c.upsample_factors[s], k = c.upsample_kernel_sizes[s];
         ups[s].tc_prec = lp;
-        rc = pack_conv_transpose(ups[s], w[i], w[i + 1], ch, ch / 2, k, u, (k - u) / 2);
+        const float *uw = wl.take(), *ub = wl.take();
+        rc = pack_conv_transpose(ups[s], uw, ub, ch, ch / 2, k, u, (k - u) / 2);
         if (rc) return rc;
-        i += 2;
         ch /= 2;
         for (int j = 0; j < c.num_kernels; ++j) {
             const int rk = c.resblock_kernel_sizes[j];
@@ -57,19 +54,21 @@ int Hifigan::init(const b200tts_hifigan_config& cfg, const float* const* w, int 
             for (int n = 0; n < c.num_dilations; ++n) {
                 const int d = c.resblock_dilations[j][n];
                 v1[n].tc_prec = lp;
-                rc = pack_conv(v1[n], w[i], w[i + 1], ch, ch, rk, d, (rk * d - d) / 2);
+                const float *w1 = wl.take(), *b1 = wl.take();
+                rc = pack_conv(v1[n], w1, b1, ch, ch, rk, d, (rk * d - d) / 2);
                 if (rc) return rc;
-                i += 2;
                 if (type1) {
                     v2[n].tc_prec = lp;
-                    rc = pack_conv(v2[n], w[i], w[i + 1], ch, ch, rk, 1, (rk - 1) / 2);
+                    const float *w2 = wl.take(), *b2 = wl.take();
+                    rc = pack_conv(v2[n], w2, b2, ch, ch, rk, 1, (rk - 1) / 2);
                     if (rc) return rc;
-                    i += 2;
                 }
             }
         }
     }
-    rc = pack_conv(conv_post, w[i], w[i + 1], c.out_channels, ch, 7, 1, 3);
+    const float *qw = wl.take(), *qb = wl.take();
+    rc = pack_conv(conv_post, qw, qb, c.out_channels, ch, 7, 1, 3);
+    if (rc == 0) rc = wl.finish("hifigan");
     if (rc == 0) plan_margins();
     return rc;
 }

@@ -91,40 +91,37 @@ int Melgan::init(const b200tts_melgan_config& cfg, const float* const* w, int nw
     for (int s = 0; s < S; ++s) B200_REQUIRE(c.upsample_factors[s] >= 1, "melgan: upsample factor %d", c.upsample_factors[s]);
     B200_REQUIRE(c.pqmf_bands == 0 || (c.pqmf_bands == c.out_channels && c.pqmf_taps >= 0 && c.pqmf_taps <= 1024),
                  "melgan: pqmf_bands must be 0 or equal out_channels (%d), with pqmf_taps >= 0", c.out_channels);
-    const int expect = 2 + S * (2 + 6 * nb) + 2 + (c.pqmf_bands > 0 ? 1 : 0);
-    B200_REQUIRE(nw == expect, "melgan: expected %d weight tensors, got %d", expect, nw);
-    int i = 0, rc;
+    WeightList wl(w, nw);
+    int rc;
     const int ppad = (c.proj_kernel - 1) / 2;
     conv_pre.tc_prec = B200TTS_PRECISION_FP32;
-    if ((rc = pack_conv(conv_pre, w[i], w[i + 1], c.base_channels, c.in_channels, c.proj_kernel, 1, ppad))) return rc;
-    i += 2;
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(conv_pre, pw, pb, c.base_channels, c.in_channels, c.proj_kernel, 1, ppad))) return rc;
     ups.resize(S);
     blocks.resize(S);
     int ch = c.base_channels;
     for (int s = 0; s < S; ++s) {
         const int u = c.upsample_factors[s], Cs = ch / 2;
         ups[s].tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv_transpose(ups[s], w[i], w[i + 1], ch, Cs, 2 * u, u, u / 2 + u % 2, u % 2))) return rc;
-        i += 2;
+        const float *uw = wl.take(), *ub = wl.take();
+        if ((rc = pack_conv_transpose(ups[s], uw, ub, ch, Cs, 2 * u, u, u / 2 + u % 2, u % 2))) return rc;
         int d = 1;
         blocks[s].resize(nb);
         for (int m = 0; m < nb; ++m, d *= c.res_kernel) {
             Block& bl = blocks[s][m];
             bl.dil.tc_prec = bl.c1x1.tc_prec = bl.shortcut.tc_prec = B200TTS_PRECISION_FP32;
-            if ((rc = pack_conv(bl.dil, w[i], w[i + 1], Cs, Cs, c.res_kernel, d, (c.res_kernel - 1) / 2 * d))) return rc;
-            if ((rc = pack_conv(bl.c1x1, w[i + 2], w[i + 3], Cs, Cs, 1, 1, 0))) return rc;
-            if ((rc = pack_conv(bl.shortcut, w[i + 4], w[i + 5], Cs, Cs, 1, 1, 0))) return rc;
-            i += 6;
+            const float *dw = wl.take(), *db = wl.take(), *cw = wl.take(), *cb = wl.take(), *sw = wl.take(),
+                        *sb = wl.take();
+            if ((rc = pack_conv(bl.dil, dw, db, Cs, Cs, c.res_kernel, d, (c.res_kernel - 1) / 2 * d))) return rc;
+            if ((rc = pack_conv(bl.c1x1, cw, cb, Cs, Cs, 1, 1, 0))) return rc;
+            if ((rc = pack_conv(bl.shortcut, sw, sb, Cs, Cs, 1, 1, 0))) return rc;
         }
         ch = Cs;
     }
-    if ((rc = pack_conv(conv_post, w[i], w[i + 1], c.out_channels, ch, c.proj_kernel, 1, ppad))) return rc;
-    i += 2;
-    if (c.pqmf_bands > 0) {
-        B200_REQUIRE(w[i] != nullptr, "melgan: null PQMF filter");
-        if (upload(G, w[i], (size_t)c.pqmf_bands * (c.pqmf_taps + 1))) return 2;
-    }
-    return 0;
+    const float *qw = wl.take(), *qb = wl.take();
+    if ((rc = pack_conv(conv_post, qw, qb, c.out_channels, ch, c.proj_kernel, 1, ppad))) return rc;
+    if (c.pqmf_bands > 0 && (rc = upload(G, wl.take(), (size_t)c.pqmf_bands * (c.pqmf_taps + 1)))) return rc;
+    return wl.finish("melgan");
 }
 
 void Melgan::stage_dims(int T, std::vector<int>& C, std::vector<int>& L) const {

@@ -163,55 +163,53 @@ int Overflow::init(const b200tts_overflow_config& cfg, const float* const* w, in
     O1 = c.outputnet_size[0];
     for (int l = 0; l < nL; ++l)
         B200_REQUIRE(c.outputnet_size[l] > 0, "overflow: outputnet_size[%d] = %d", l, c.outputnet_size[l]);
-    const int per_block = 3 + 2 + 4 * c.num_block_layers + 2;
-    const int expect = 1 + 6 * c.n_convs + 8 + 1 + c.prenet_n_layers + 4 + 2 * nL + 2 + 2 +
-                       (c.has_decoder ? per_block * c.num_flow_blocks : 0);
-    B200_REQUIRE(nw == expect, "overflow: expected %d weight tensors, got %d", expect, nw);
-    int rc, i = 0;
-    if ((rc = enc.init(c.n_vocab, E, H, c.n_convs, w, &i))) return rc;
-    if ((rc = upload(go, w[i++], (size_t)c.ar_order))) return rc;
+    WeightList wl(w, nw);
+    int rc;
+    if ((rc = enc.init(c.n_vocab, E, H, c.n_convs, wl))) return rc;
+    if ((rc = upload(go, wl.take(), (size_t)c.ar_order))) return rc;
     prenet_w.resize(c.prenet_n_layers);
     for (int l = 0; l < c.prenet_n_layers; ++l)
-        if ((rc = upload(prenet_w[l], w[i++], (size_t)P * (l ? P : c.ar_order * C)))) return rc;
-    if ((rc = upload(mem_wih, w[i], (size_t)4 * M * P))) return rc;
-    if ((rc = upload(mem_whh, w[i + 1], (size_t)4 * M * M))) return rc;
+        if ((rc = upload(prenet_w[l], wl.take(), (size_t)P * (l ? P : c.ar_order * C)))) return rc;
+    if ((rc = upload(mem_wih, wl.take(), (size_t)4 * M * P))) return rc;
+    if ((rc = upload(mem_whh, wl.take(), (size_t)4 * M * M))) return rc;
     {
+        const float *b_ih = wl.take(), *b_hh = wl.take();
+        B200_REQUIRE(b_ih && b_hh, "overflow: null memory LSTM bias");
         std::vector<float> b((size_t)4 * M);
-        for (int r = 0; r < 4 * M; ++r) b[r] = w[i + 2][r] + w[i + 3][r];
+        for (int r = 0; r < 4 * M; ++r) b[r] = b_ih[r] + b_hh[r];
         if ((rc = upload(mem_b, b.data(), b.size()))) return rc;
     }
-    i += 4;
     out_w.resize(nL + 1);
     out_b.resize(nL + 1);
-    for (int l = 0; l <= nL; ++l, i += 2) {
+    for (int l = 0; l <= nL; ++l) {
         const int rows = l < nL ? c.outputnet_size[l] : 2 * C + 1;
         const int in = l == 0 ? M + E : c.outputnet_size[l - 1];
+        const float *ow = wl.take(), *ob = wl.take();
         if (l == 0) {   // cat(h, z): the h columns per frame, the z columns hoisted into zproj (with the bias)
+            B200_REQUIRE(ow, "overflow: null output net weight");
             std::vector<float> wh((size_t)rows * M), wz((size_t)rows * E);
             for (int r = 0; r < rows; ++r) {
-                memcpy(wh.data() + (size_t)r * M, w[i] + (size_t)r * in, sizeof(float) * M);
-                memcpy(wz.data() + (size_t)r * E, w[i] + (size_t)r * in + M, sizeof(float) * E);
+                memcpy(wh.data() + (size_t)r * M, ow + (size_t)r * in, sizeof(float) * M);
+                memcpy(wz.data() + (size_t)r * E, ow + (size_t)r * in + M, sizeof(float) * E);
             }
             if ((rc = upload(out_w[l], wh.data(), wh.size()))) return rc;
-            if ((rc = pack_conv(zproj, wz.data(), w[i + 1], rows, E, 1, 1, 0))) return rc;
+            if ((rc = pack_conv(zproj, wz.data(), ob, rows, E, 1, 1, 0))) return rc;
         } else {
-            if ((rc = upload(out_w[l], w[i], (size_t)rows * in))) return rc;
-            if ((rc = upload(out_b[l], w[i + 1], (size_t)rows))) return rc;
+            if ((rc = upload(out_w[l], ow, (size_t)rows * in))) return rc;
+            if ((rc = upload(out_b[l], ob, (size_t)rows))) return rc;
         }
     }
-    if ((rc = upload(mean, w[i], (size_t)C))) return rc;
-    if ((rc = upload(std_, w[i + 1], (size_t)C))) return rc;
-    i += 2;
+    if ((rc = upload(mean, wl.take(), (size_t)C))) return rc;
+    if ((rc = upload(std_, wl.take(), (size_t)C))) return rc;
     if (c.has_decoder) {
         B200_REQUIRE(c.num_squeeze >= 1 && c.hidden_channels_dec > 0 && c.kernel_size_dec % 2 == 1 &&
                          c.num_flow_blocks >= 1 && c.num_block_layers >= 1 && c.dilation_rate >= 1,
                      "overflow: unsupported decoder config");
-        int used = 0;
         if ((rc = dec.init(C, c.hidden_channels_dec, c.kernel_size_dec, c.dilation_rate, c.num_flow_blocks,
-                           c.num_block_layers, 0, c.num_splits, c.num_squeeze, c.sigmoid_scale, w + i, &used)))
+                           c.num_block_layers, 0, c.num_splits, c.num_squeeze, c.sigmoid_scale, wl)))
             return rc;
     }
-    return 0;
+    return wl.finish("overflow");
 }
 
 size_t Overflow::workspace_bytes(int B, int Tt, int F) const {

@@ -496,20 +496,25 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
         P *= c.upsample_factors[s];
     }
     B200_REQUIRE(P <= 4096, "pwgan: upsampling %d samples per frame (at most 4096)", P);
-    const int expect = 2 + 1 + S + 7 * L + 4;
-    B200_REQUIRE(nw == expect, "pwgan: expected %d weight tensors, got %d", expect, nw);
     for (int i = 0; i < nw; ++i) B200_REQUIRE(w[i] != nullptr, "pwgan: weight tensor %d is null", i);
-    if (upload(first_w, w[0], RES) || upload(first_b, w[1], RES)) return 2;
-    const float* W_in = w[2];                                          // conv_in [80][80]
+    WeightList wl(w, nw);
+    int rc;
+    if ((rc = upload(first_w, wl.take(), RES)) || (rc = upload(first_b, wl.take(), RES))) return rc;
+    const float* W_in = wl.take();                                     // conv_in [80][80]
     std::vector<std::vector<double>> fir(S);
-    for (int s = 0; s < S; ++s) fir[s].assign(w[3 + s], w[3 + s] + 2 * c.upsample_factors[s] + 1);
-    int i = 3 + S;
+    for (int s = 0; s < S; ++s) {
+        const float* f = wl.take();
+        B200_REQUIRE(W_in && f, "pwgan: null conv_in or upsampler filter");
+        fir[s].assign(f, f + 2 * c.upsample_factors[s] + 1);
+    }
     // MMA row m of the gate: tanh row 8g + (m % 16) for m % 16 < 8, else sigmoid row 64 + 8g + (m % 16 - 8), g = m / 16
     auto gate_row = [](int m) { const int g = m / 16, q = m % 16; return q < 8 ? 8 * g + q : 64 + 8 * g + q - 8; };
     std::vector<float> aux((size_t)L * GATE * AUX), bias1((size_t)L * GATE), bias2((size_t)L * GATE);
     w1.resize(L); w2.resize(L); rs1.resize(L); rs2.resize(L);
-    for (int l = 0; l < L; ++l, i += 7) {
-        const float *cw = w[i], *cb = w[i + 1], *aw = w[i + 2], *ow = w[i + 3], *ob = w[i + 4], *sw = w[i + 5], *sb = w[i + 6];
+    for (int l = 0; l < L; ++l) {
+        const float *cw = wl.take(), *cb = wl.take(), *aw = wl.take(), *ow = wl.take(), *ob = wl.take(), *sw = wl.take(),
+                    *sb = wl.take();
+        B200_REQUIRE(cw && cb && aw && ow && ob && sw && sb, "pwgan: null residual layer weight or bias");
         std::vector<float> W1((size_t)GATE * RES * 3), W2((size_t)GATE * RES);
         for (int m = 0; m < GATE; ++m) {
             const int r = gate_row(m);
@@ -534,9 +539,10 @@ int Pwgan::init(const b200tts_pwgan_config& cfg, const float* const* w, int nw) 
         upload(b2, bias2.data(), bias2.size()))
         return 2;
     tail1.tc_prec = B200TTS_PRECISION_FP32;
-    int rc;
-    if ((rc = pack_conv(tail1, w[i], w[i + 1], RES, RES, 1, 1, 0))) return rc;
-    if ((rc = pack_conv(tail2, w[i + 2], w[i + 3], 1, RES, 1, 1, 0))) return rc;
+    const float *t1w = wl.take(), *t1b = wl.take(), *t2w = wl.take(), *t2b = wl.take();
+    if ((rc = pack_conv(tail1, t1w, t1b, RES, RES, 1, 1, 0))) return rc;
+    if ((rc = pack_conv(tail2, t2w, t2b, 1, RES, 1, 1, 0))) return rc;
+    if ((rc = wl.finish("pwgan"))) return rc;
     return build_u(fir);
 }
 

@@ -347,13 +347,15 @@ int launch_gru(const GruArgs& a, int rows_per_block, cudaStream_t st, bool note)
     return 0;
 }
 
-void pack_bigru_whh(const float* whh, float* dst) {
+int pack_bigru_whh(const float* whh, float* dst) {
+    B200_REQUIRE(whh, "pack_bigru_whh: null W_hh");
     for (int g = 0; g < 3; ++g)
         for (int i = 0; i < 32; ++i)
             for (int t = 0; t < BIGRU_THREADS; ++t) {
                 const int j = t >> 2, q = t & 3;
                 dst[(size_t)(g * 32 + i) * BIGRU_THREADS + t] = whh[(size_t)(g * GRU_H + j) * GRU_H + 4 * i + q];
             }
+    return 0;
 }
 
 int launch_bigru(const BiGruArgs& a, int B, cudaStream_t st) {
@@ -441,9 +443,12 @@ int run_step_graph(const char* who, int chunk, int max_steps, int launches_per_s
     return 0;
 }
 
-void fold_bn(const float* w, const float* bias, const float* const* bn, double eps, int Cout, size_t row,
-             std::vector<float>& wf, std::vector<float>& bf) {
-    const float *gamma = bn[0], *beta = bn[1], *mean = bn[2], *var = bn[3];
+int fold_bn(WeightList& wl, bool has_bias, double eps, int Cout, size_t row, std::vector<float>& wf,
+            std::vector<float>& bf) {
+    const float* w = wl.take();
+    const float* bias = has_bias ? wl.take() : nullptr;
+    const float *gamma = wl.take(), *beta = wl.take(), *mean = wl.take(), *var = wl.take();
+    B200_REQUIRE(w && (bias || !has_bias) && gamma && beta && mean && var, "fold_bn: null weight or BatchNorm tensor");
     wf.assign((size_t)Cout * row, 0.f);
     bf.assign(Cout, 0.f);
     for (int o = 0; o < Cout; ++o) {
@@ -451,32 +456,32 @@ void fold_bn(const float* w, const float* bias, const float* const* bn, double e
         for (size_t k = 0; k < row; ++k) wf[(size_t)o * row + k] = (float)(w[(size_t)o * row + k] * s);
         bf[o] = bias ? (float)(((double)bias[o] - mean[o]) * s + beta[o]) : (float)((double)beta[o] - mean[o] * s);
     }
+    return 0;
 }
 
 // ------------------------------------------------------------------ the text encoder
-int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, const float* const* w, int* consumed) {
+int SeqEncoder::init(int vocab, int dim, int hidden, int convs_n, WeightList& wl) {
     n_vocab = vocab; E = dim; H = hidden; n_convs = convs_n;
     B200_REQUIRE(n_vocab > 0 && E > 0 && H > 0 && n_convs >= 1 && n_convs <= 8, "encoder: unsupported config");
-    int rc, i = 0;
-    if ((rc = upload(emb, w[i++], (size_t)n_vocab * E))) return rc;
+    int rc;
+    if ((rc = upload(emb, wl.take(), (size_t)n_vocab * E))) return rc;
     std::vector<float> wf, bf;
-    for (int l = 0; l < n_convs; ++l, i += 6) {   // ConvBNBlock: BatchNorm1d (eps 1e-5) folded into the conv
-        fold_bn(w[i], w[i + 1], w + i + 2, 1e-5, E, (size_t)E * 5, wf, bf);
+    for (int l = 0; l < n_convs; ++l) {   // ConvBNBlock: BatchNorm1d (eps 1e-5) folded into the conv
+        if ((rc = fold_bn(wl, true, 1e-5, E, (size_t)E * 5, wf, bf))) return rc;
         if ((rc = pack_conv(convs[l], wf.data(), bf.data(), E, E, 5, 1, 2))) return rc;
     }
     {   // LSTM: both directions' input projections as one 1x1 conv (rows [fwd 4H | bwd 4H]), bias b_ih + b_hh
         std::vector<float> wi((size_t)8 * H * E), bi((size_t)8 * H), wh((size_t)8 * H * H);
         for (int d = 0; d < 2; ++d) {
-            const float* const* p = w + i + 4 * d;
-            memcpy(wi.data() + (size_t)d * 4 * H * E, p[0], sizeof(float) * 4 * H * E);
-            memcpy(wh.data() + (size_t)d * 4 * H * H, p[1], sizeof(float) * 4 * H * H);
-            for (int r = 0; r < 4 * H; ++r) bi[(size_t)d * 4 * H + r] = p[2][r] + p[3][r];
+            const float *w_ih = wl.take(), *w_hh = wl.take(), *b_ih = wl.take(), *b_hh = wl.take();
+            B200_REQUIRE(w_ih && w_hh && b_ih && b_hh, "encoder: null LSTM weight or bias");
+            memcpy(wi.data() + (size_t)d * 4 * H * E, w_ih, sizeof(float) * 4 * H * E);
+            memcpy(wh.data() + (size_t)d * 4 * H * H, w_hh, sizeof(float) * 4 * H * H);
+            for (int r = 0; r < 4 * H; ++r) bi[(size_t)d * 4 * H + r] = b_ih[r] + b_hh[r];
         }
         if ((rc = pack_conv(lstm_in, wi.data(), bi.data(), 8 * H, E, 1, 1, 0))) return rc;
         if ((rc = upload(whh, wh.data(), wh.size()))) return rc;
-        i += 8;
     }
-    *consumed = i;
     return 0;
 }
 

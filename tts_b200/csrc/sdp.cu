@@ -231,21 +231,33 @@ __global__ void add_chan_bias_kernel(const float* x, const float* cb, long long 
 // weights: conv_1.w [F,Cin,k], .b, norm_1.gamma [1,F,1], .beta, conv_2.w [F,F,k], .b, norm_2.gamma, .beta,
 //          proj.w [1,F,1], .b, [cond.w [Cin,cond,1], .b], [cond_lang.w, .b]
 int DurPred::init(const b200tts_duration_predictor_config& cfg, const float* const* w, int nw) {
+    WeightList wl(w, nw);
+    if (int rc = init(cfg, wl)) return rc;
+    return wl.finish("duration_predictor");
+}
+
+int DurPred::init(const b200tts_duration_predictor_config& cfg, WeightList& wl) {
     c = cfg;
     const int Cin = c.in_channels + c.language_emb_dim, F = c.hidden_channels, K = c.kernel_size;
-    const int expect = 10 + (c.cond_channels > 0 ? 2 : 0) + (c.language_emb_dim > 0 ? 2 : 0);
-    B200_REQUIRE(nw == expect, "duration_predictor: expected %d weight tensors, got %d", expect, nw);
     int rc;
-    if ((rc = pack_conv(conv1, w[0], w[1], F, Cin, K, 1, K / 2))) return rc;
-    if ((rc = upload(g1, w[2], F))) return rc;
-    if ((rc = upload(b1, w[3], F))) return rc;
-    if ((rc = pack_conv(conv2, w[4], w[5], F, F, K, 1, K / 2))) return rc;
-    if ((rc = upload(g2, w[6], F))) return rc;
-    if ((rc = upload(b2, w[7], F))) return rc;
-    if ((rc = pack_conv(proj, w[8], w[9], 1, F, 1, 1, 0))) return rc;
-    int i = 10;
-    if (c.cond_channels > 0) { if ((rc = pack_conv(cond, w[i], w[i + 1], Cin, c.cond_channels, 1, 1, 0))) return rc; i += 2; }
-    if (c.language_emb_dim > 0) { if ((rc = pack_conv(cond_lang, w[i], w[i + 1], Cin, c.language_emb_dim, 1, 1, 0))) return rc; }
+    const float *c1w = wl.take(), *c1b = wl.take();
+    if ((rc = pack_conv(conv1, c1w, c1b, F, Cin, K, 1, K / 2))) return rc;
+    if ((rc = upload(g1, wl.take(), F))) return rc;
+    if ((rc = upload(b1, wl.take(), F))) return rc;
+    const float *c2w = wl.take(), *c2b = wl.take();
+    if ((rc = pack_conv(conv2, c2w, c2b, F, F, K, 1, K / 2))) return rc;
+    if ((rc = upload(g2, wl.take(), F))) return rc;
+    if ((rc = upload(b2, wl.take(), F))) return rc;
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(proj, pw, pb, 1, F, 1, 1, 0))) return rc;
+    if (c.cond_channels > 0) {
+        const float *gw = wl.take(), *gb = wl.take();
+        if ((rc = pack_conv(cond, gw, gb, Cin, c.cond_channels, 1, 1, 0))) return rc;
+    }
+    if (c.language_emb_dim > 0) {
+        const float *lw = wl.take(), *lb = wl.take();
+        if ((rc = pack_conv(cond_lang, lw, lb, Cin, c.language_emb_dim, 1, 1, 0))) return rc;
+    }
     return 0;
 }
 
@@ -319,22 +331,21 @@ int DurPred::forward(const float* x, const float* mask, const float* g, const fl
 }
 
 // per layer: sep.w [C,1,K], sep.b, 1x1.w [C,C,1], 1x1.b, norm1.gamma, norm1.beta, norm2.gamma, norm2.beta
-int DDSConv::init(int channels, int kernel_size, int num_layers, const float* const* w, int* consumed) {
+int DDSConv::init(int channels, int kernel_size, int num_layers, WeightList& wl) {
     C = channels; K = kernel_size; L = num_layers;
     conv1x1.resize(L);
     sep_w.resize(L); sep_b.resize(L); g1.resize(L); b1.resize(L); g2.resize(L); b2.resize(L);
     int rc;
     for (int l = 0; l < L; ++l) {
-        const float* const* p = w + 8 * l;
-        if ((rc = upload(sep_w[l], p[0], (size_t)C * K))) return rc;
-        if ((rc = upload(sep_b[l], p[1], C))) return rc;
-        if ((rc = pack_conv(conv1x1[l], p[2], p[3], C, C, 1, 1, 0))) return rc;
-        if ((rc = upload(g1[l], p[4], C))) return rc;
-        if ((rc = upload(b1[l], p[5], C))) return rc;
-        if ((rc = upload(g2[l], p[6], C))) return rc;
-        if ((rc = upload(b2[l], p[7], C))) return rc;
+        if ((rc = upload(sep_w[l], wl.take(), (size_t)C * K))) return rc;
+        if ((rc = upload(sep_b[l], wl.take(), C))) return rc;
+        const float *pw = wl.take(), *pb = wl.take();
+        if ((rc = pack_conv(conv1x1[l], pw, pb, C, C, 1, 1, 0))) return rc;
+        if ((rc = upload(g1[l], wl.take(), C))) return rc;
+        if ((rc = upload(b1[l], wl.take(), C))) return rc;
+        if ((rc = upload(g2[l], wl.take(), C))) return rc;
+        if ((rc = upload(b2[l], wl.take(), C))) return rc;
     }
-    *consumed = 8 * L;
     return 0;
 }
 
@@ -366,33 +377,33 @@ int SDP::init(const b200tts_sdp_config& cfg, const float* const* w, int nw) {
     c = cfg;
     B200_REQUIRE(c.num_bins >= 1 && c.num_bins <= NB_MAX, "sdp: num_bins %d unsupported", c.num_bins);
     const int H = c.hidden_channels;
-    const int expect = 2 + (c.cond_channels > 0 ? 2 : 0) + (c.language_emb_dim > 0 ? 2 : 0) + 24 + 2 + 2 +
-                       c.num_flows * (2 + 24 + 2);
-    B200_REQUIRE(nw == expect, "sdp: expected %d weight tensors, got %d", expect, nw);
-    int i = 0, rc, used;
-    if ((rc = pack_conv(pre, w[i], w[i + 1], H, c.in_channels + c.language_emb_dim, 1, 1, 0))) return rc;
-    i += 2;
-    if (c.cond_channels > 0) { if ((rc = pack_conv(cond, w[i], w[i + 1], H, c.cond_channels, 1, 1, 0))) return rc; i += 2; }
-    if (c.language_emb_dim > 0) { if ((rc = pack_conv(cond_lang, w[i], w[i + 1], H, c.language_emb_dim, 1, 1, 0))) return rc; i += 2; }
-    if ((rc = convs.init(H, c.kernel_size, 3, w + i, &used))) return rc;
-    i += used;
-    if ((rc = pack_conv(proj, w[i], w[i + 1], H, H, 1, 1, 0))) return rc;
-    i += 2;
-    if ((rc = upload(ea_t, w[i], 2))) return rc;
-    if ((rc = upload(ea_ls, w[i + 1], 2))) return rc;
-    i += 2;
+    WeightList wl(w, nw);
+    int rc;
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(pre, pw, pb, H, c.in_channels + c.language_emb_dim, 1, 1, 0))) return rc;
+    if (c.cond_channels > 0) {
+        const float *gw = wl.take(), *gb = wl.take();
+        if ((rc = pack_conv(cond, gw, gb, H, c.cond_channels, 1, 1, 0))) return rc;
+    }
+    if (c.language_emb_dim > 0) {
+        const float *lw = wl.take(), *lb = wl.take();
+        if ((rc = pack_conv(cond_lang, lw, lb, H, c.language_emb_dim, 1, 1, 0))) return rc;
+    }
+    if ((rc = convs.init(H, c.kernel_size, 3, wl))) return rc;
+    const float *qw = wl.take(), *qb = wl.take();
+    if ((rc = pack_conv(proj, qw, qb, H, H, 1, 1, 0))) return rc;
+    if ((rc = upload(ea_t, wl.take(), 2))) return rc;
+    if ((rc = upload(ea_ls, wl.take(), 2))) return rc;
     flows.resize(c.num_flows);
     for (int f = 0; f < c.num_flows; ++f) {
         CFlow& F = flows[f];
-        if ((rc = upload(F.pre_w, w[i], H))) return rc;
-        if ((rc = upload(F.pre_b, w[i + 1], H))) return rc;
-        i += 2;
-        if ((rc = F.convs.init(H, c.kernel_size, 3, w + i, &used))) return rc;
-        i += used;
-        if ((rc = pack_conv(F.proj, w[i], w[i + 1], 3 * c.num_bins - 1, H, 1, 1, 0))) return rc;
-        i += 2;
+        if ((rc = upload(F.pre_w, wl.take(), H))) return rc;
+        if ((rc = upload(F.pre_b, wl.take(), H))) return rc;
+        if ((rc = F.convs.init(H, c.kernel_size, 3, wl))) return rc;
+        const float *fw = wl.take(), *fb = wl.take();
+        if ((rc = pack_conv(F.proj, fw, fb, 3 * c.num_bins - 1, H, 1, 1, 0))) return rc;
     }
-    return 0;
+    return wl.finish("sdp");
 }
 
 struct SdpWs { float *xc, *h, *y1, *y2, *z, *hp, *condv; };

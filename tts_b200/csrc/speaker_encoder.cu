@@ -367,14 +367,13 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
     for (int s = 0; s < 4; ++s)
         B200_REQUIRE(c.layers[s] >= 1 && c.num_filters[s] >= 8 && c.num_filters[s] <= 1024,
                      "speaker_encoder: stage %d needs >= 1 block and 8..1024 filters", s + 1);
-    int i = 0;
-    auto next = [&]() -> const float* { return i < nw ? w[i++] : nullptr; };
+    WeightList wl(w, nw);
     int rc;
     if (c.use_torch_spec) {
         B200_REQUIRE(c.win_length >= 1 && c.win_length <= c.fft_size && c.hop_length >= 1, "speaker_encoder: bad STFT sizes");
-        const float* filt = next();
-        const float* win = next();
-        const float* fb = next();
+        const float* filt = wl.take();
+        const float* win = wl.take();
+        const float* fb = wl.take();
         B200_REQUIRE(filt && win && fb, "speaker_encoder: missing front-end weights");
         pre0 = filt[0]; pre1 = filt[1];
         const int F = c.fft_size / 2 + 1, left = (c.fft_size - c.win_length) / 2;
@@ -385,7 +384,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
         if ((rc = stft.init(c.fft_size, c.hop_length, wp.data(), basis.data(), c.input_dim))) return rc;
     }
     auto bn = [&](int C, BN& out) -> int {
-        const float *bw = next(), *bb = next(), *bm = next(), *bv = next();
+        const float *bw = wl.take(), *bb = wl.take(), *bm = wl.take(), *bv = wl.take();
         B200_REQUIRE(bw && bb && bm && bv, "speaker_encoder: missing BatchNorm tensors");
         out = bn_affine(bw, bb, bm, bv, C);
         return 0;
@@ -393,7 +392,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
     // stem: conv1 (1 -> F0, bias) -> ReLU -> bn1
     const int F0 = c.num_filters[0];
     {
-        const float *cw = next(), *cb = next();
+        const float *cw = wl.take(), *cb = wl.take();
         B200_REQUIRE(cw && cb, "speaker_encoder: missing conv1");
         BN b;
         if ((rc = bn(F0, b))) return rc;
@@ -410,12 +409,12 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
             blocks.emplace_back();
             Block& b = blocks.back();
             b.C = c.num_filters[s]; b.Cin = (k == 0) ? Cprev : b.C; b.Cr = b.C / 8; b.down = (k == 0 && s > 0);
-            const float* w1 = next();
+            const float* w1 = wl.take();
             BN b1, b2;
             if ((rc = bn(b.C, b1))) return rc;
-            const float* w2 = next();
+            const float* w2 = wl.take();
             if ((rc = bn(b.C, b2))) return rc;
-            const float *f1w = next(), *f1b = next(), *f2w = next(), *f2b = next();
+            const float *f1w = wl.take(), *f1b = wl.take(), *f2w = wl.take(), *f2b = wl.take();
             B200_REQUIRE(w1 && w2 && f1w && f1b && f2w && f2b, "speaker_encoder: missing block weights");
             b.c1.tc_prec = b.c2.tc_prec = B200TTS_PRECISION_FP32;
             if (b.down) {
@@ -435,7 +434,7 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
                 (rc = upload(b.fc2w, f2w, (size_t)b.C * b.Cr)) || (rc = upload(b.fc2b, f2b, b.C)))
                 return rc;
             if (b.down) {
-                const float* dw = next();
+                const float* dw = wl.take();
                 B200_REQUIRE(dw, "speaker_encoder: missing downsample weight");
                 BN bd;
                 if ((rc = bn(b.C, bd))) return rc;
@@ -452,10 +451,10 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
     // head: attention conv 1x1 (input channels permuted from the reference's c*Hf + h to this layout's h*C + c)
     const int Hf = c.input_dim / 8, C4 = c.num_filters[3], Ca = Hf * C4;
     {
-        const float *aw = next(), *ab = next();
+        const float *aw = wl.take(), *ab = wl.take();
         BN ba;
         if ((rc = bn(128, ba))) return rc;
-        const float *a3w = next(), *a3b = next();
+        const float *a3w = wl.take(), *a3b = wl.take();
         B200_REQUIRE(aw && ab && a3w && a3b, "speaker_encoder: missing attention weights");
         std::vector<int> perm(Ca);
         for (int cc = 0; cc < C4; ++cc)
@@ -475,13 +474,12 @@ int SpeakerEncoder::init(const b200tts_speaker_encoder_config& cfg, const float*
         if ((rc = pack_conv(att2, r.data(), bias.data(), Ca, 128, 1, 1, 0))) return rc;
     }
     {
-        const float *fw = next(), *fb = next();
+        const float *fw = wl.take(), *fb = wl.take();
         B200_REQUIRE(fw && fb, "speaker_encoder: missing fc");
         fc.tc_prec = B200TTS_PRECISION_FP32;
         if ((rc = pack_conv(fc, fw, fb, c.proj_dim, (c.encoder_type ? 2 : 1) * Ca, 1, 1, 0))) return rc;
     }
-    B200_REQUIRE(i == nw, "speaker_encoder: expected %d weight tensors, got %d", i, nw);
-    return 0;
+    return wl.finish("speaker_encoder");
 }
 
 size_t SpeakerEncoder::workspace_bytes(int B, int T) const {

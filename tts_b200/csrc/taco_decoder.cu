@@ -240,34 +240,33 @@ size_t attn_smem_bytes(int Qd, int Tt) {
 }  // namespace
 
 // ------------------------------------------------------------------ the attention
-int TacoAttention::n_weights(int type, int location) { return type == 1 ? 9 : 4 + (location ? 2 : 0); }
-
 int TacoAttention::init(int q_dim, int e_dim, int attention_type, int location_attn, int attention_softmax,
-                        const float* const* w, int* consumed) {
+                        WeightList& wl) {
     Q = q_dim; E = e_dim; type = attention_type; location = location_attn; softmax = attention_softmax;
     B200_REQUIRE((Q == 1024 && E == 512) || (Q == 256 && E == 256), "taco_attn: no kernel for Q %d / E %d", Q, E);
-    int rc, i = 0;
+    int rc;
     if (type == 0) {
-        if ((rc = upload(wq, w[i++], (size_t)A * Q))) return rc;
-        if ((rc = pack_conv(inproj, w[i++], nullptr, A, E, 1, 1, 0))) return rc;
-        if ((rc = upload(v, w[i++], A))) return rc;
-        vb = w[i++][0];
+        if ((rc = upload(wq, wl.take(), (size_t)A * Q))) return rc;
+        if ((rc = pack_conv(inproj, wl.take(), nullptr, A, E, 1, 1, 0))) return rc;
+        if ((rc = upload(v, wl.take(), A))) return rc;
+        const float* v_bias = wl.take();
+        B200_REQUIRE(v_bias, "taco_attn: null v.bias");
+        vb = v_bias[0];
         if (location) {
-            if ((rc = upload(wc, w[i++], (size_t)LOC_F * 2 * LOC_K))) return rc;
-            if ((rc = upload(wd, w[i++], (size_t)A * LOC_F))) return rc;
+            if ((rc = upload(wc, wl.take(), (size_t)LOC_F * 2 * LOC_K))) return rc;
+            if ((rc = upload(wd, wl.take(), (size_t)A * LOC_F))) return rc;
         }
     } else {
-        if ((rc = upload(prior, w[i++], PRIOR_K))) return rc;
-        if ((rc = upload(wq, w[i++], (size_t)A * Q))) return rc;
-        if ((rc = upload(bq, w[i++], A))) return rc;
-        if ((rc = upload(wk, w[i++], (size_t)DCA_F * DCA_K * A))) return rc;
-        if ((rc = upload(ws, w[i++], (size_t)DCA_F * DCA_K))) return rc;
-        if ((rc = upload(wsl, w[i++], (size_t)A * DCA_F))) return rc;
-        if ((rc = upload(wdl, w[i++], (size_t)A * DCA_F))) return rc;
-        if ((rc = upload(bdl, w[i++], A))) return rc;
-        if ((rc = upload(v, w[i++], A))) return rc;
+        if ((rc = upload(prior, wl.take(), PRIOR_K))) return rc;
+        if ((rc = upload(wq, wl.take(), (size_t)A * Q))) return rc;
+        if ((rc = upload(bq, wl.take(), A))) return rc;
+        if ((rc = upload(wk, wl.take(), (size_t)DCA_F * DCA_K * A))) return rc;
+        if ((rc = upload(ws, wl.take(), (size_t)DCA_F * DCA_K))) return rc;
+        if ((rc = upload(wsl, wl.take(), (size_t)A * DCA_F))) return rc;
+        if ((rc = upload(wdl, wl.take(), (size_t)A * DCA_F))) return rc;
+        if ((rc = upload(bdl, wl.take(), A))) return rc;
+        if ((rc = upload(v, wl.take(), A))) return rc;
     }
-    *consumed = i;
     return 0;
 }
 

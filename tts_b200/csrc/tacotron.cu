@@ -174,16 +174,16 @@ void persist_layout(const Tacotron& e, Arena& ar, int B, int Tt, Persist& p) {
 }  // namespace
 
 // ------------------------------------------------------------------ CBHG
-int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int* consumed) {
+int Tacotron::Cbhg::init(int cin, int k_max, int p1, WeightList& wl) {
     Cin = cin; K = k_max; P1 = p1;
     B200_REQUIRE(Cin >= 1 && Cin <= HW_MAX_CIN && K >= 1, "tacotron: unsupported CBHG shape");
-    int rc, i = 0;
+    int rc;
     std::vector<float> wf, bf;
     {   // the bank: conv k (taps [-(k-1)/2, k/2]) placed in the union window [-(K-1)/2, K/2] of K taps
         const int padU = (K - 1) / 2;
         std::vector<float> wb((size_t)K * BANK * Cin * K, 0.f), bb((size_t)K * BANK);
-        for (int k = 1; k <= K; ++k, i += 5) {
-            fold_bn(w[i], nullptr, w + i + 1, 1e-3, BANK, (size_t)Cin * k, wf, bf);
+        for (int k = 1; k <= K; ++k) {
+            if ((rc = fold_bn(wl, false, 1e-3, BANK, (size_t)Cin * k, wf, bf))) return rc;
             const int off = padU - (k - 1) / 2;
             for (int o = 0; o < BANK; ++o) {
                 const int row = (k - 1) * BANK + o;
@@ -195,29 +195,31 @@ int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int*
         }
         if ((rc = pack_conv(bank, wb.data(), bb.data(), K * BANK, Cin, K, 1, padU))) return rc;
     }
-    fold_bn(w[i], nullptr, w + i + 1, 1e-3, P1, (size_t)K * BANK * 3, wf, bf);
+    if ((rc = fold_bn(wl, false, 1e-3, P1, (size_t)K * BANK * 3, wf, bf))) return rc;
     if ((rc = pack_conv(proj1, wf.data(), bf.data(), P1, K * BANK, 3, 1, 1))) return rc;
-    i += 5;
-    fold_bn(w[i], nullptr, w + i + 1, 1e-3, Cin, (size_t)P1 * 3, wf, bf);
+    if ((rc = fold_bn(wl, false, 1e-3, Cin, (size_t)P1 * 3, wf, bf))) return rc;
     if ((rc = pack_conv(proj2, wf.data(), bf.data(), Cin, P1, 3, 1, 1))) return rc;
-    i += 5;
     if (Cin != HW) {   // pre_highway [128][Cin] -> [Cin][128]
+        const float* pre = wl.take();
+        B200_REQUIRE(pre, "tacotron: null pre_highway weight");
         std::vector<float> pt((size_t)Cin * HW);
         for (int o = 0; o < HW; ++o)
-            for (int k = 0; k < Cin; ++k) pt[(size_t)k * HW + o] = w[i][(size_t)o * Cin + k];
+            for (int k = 0; k < Cin; ++k) pt[(size_t)k * HW + o] = pre[(size_t)o * Cin + k];
         if ((rc = upload(pre_w, pt.data(), pt.size()))) return rc;
-        ++i;
     }
     {   // highways: [H | T] rows transposed to [k][256]
         std::vector<float> hw((size_t)NHW * HW * 2 * HW), hb((size_t)NHW * 2 * HW);
-        for (int l = 0; l < NHW; ++l, i += 4)
+        for (int l = 0; l < NHW; ++l) {
+            const float *hw_H = wl.take(), *hb_H = wl.take(), *hw_T = wl.take(), *hb_T = wl.take();
+            B200_REQUIRE(hw_H && hb_H && hw_T && hb_T, "tacotron: null highway weight or bias");
             for (int o = 0; o < 2 * HW; ++o) {
-                const float* W = o < HW ? w[i] : w[i + 2];
-                const float* bsrc = o < HW ? w[i + 1] : w[i + 3];
+                const float* W = o < HW ? hw_H : hw_T;
+                const float* bsrc = o < HW ? hb_H : hb_T;
                 const int oo = o % HW;
                 hb[(size_t)l * 2 * HW + o] = bsrc[oo];
                 for (int k = 0; k < HW; ++k) hw[((size_t)l * HW + k) * 2 * HW + o] = W[(size_t)oo * HW + k];
             }
+        }
         if ((rc = upload(hw_w, hw.data(), hw.size()))) return rc;
         if ((rc = upload(hw_b, hb.data(), hb.size()))) return rc;
     }
@@ -225,18 +227,17 @@ int Tacotron::Cbhg::init(int cin, int k_max, int p1, const float* const* w, int*
         constexpr int H = GRU_H;
         std::vector<float> wi((size_t)6 * H * HW), bi((size_t)6 * H), img((size_t)2 * 3 * 32 * BIGRU_THREADS), bn(2 * H);
         for (int d = 0; d < 2; ++d) {
-            const float* const* p = w + i + 4 * d;
-            memcpy(wi.data() + (size_t)d * 3 * H * HW, p[0], sizeof(float) * 3 * H * HW);
-            for (int r = 0; r < 3 * H; ++r) bi[(size_t)d * 3 * H + r] = p[2][r] + (r < 2 * H ? p[3][r] : 0.f);
-            for (int j = 0; j < H; ++j) bn[d * H + j] = p[3][2 * H + j];
-            pack_bigru_whh(p[1], img.data() + (size_t)d * 3 * 32 * BIGRU_THREADS);
+            const float *w_ih = wl.take(), *w_hh = wl.take(), *b_ih = wl.take(), *b_hh = wl.take();
+            B200_REQUIRE(w_ih && b_ih && b_hh, "tacotron: null GRU weight or bias");
+            memcpy(wi.data() + (size_t)d * 3 * H * HW, w_ih, sizeof(float) * 3 * H * HW);
+            for (int r = 0; r < 3 * H; ++r) bi[(size_t)d * 3 * H + r] = b_ih[r] + (r < 2 * H ? b_hh[r] : 0.f);
+            for (int j = 0; j < H; ++j) bn[d * H + j] = b_hh[2 * H + j];
+            if ((rc = pack_bigru_whh(w_hh, img.data() + (size_t)d * 3 * 32 * BIGRU_THREADS))) return rc;
         }
         if ((rc = pack_conv(gru_in, wi.data(), bi.data(), 6 * H, HW, 1, 1, 0))) return rc;
         if ((rc = upload(whh, img.data(), img.size()))) return rc;
         if ((rc = upload(bhn, bn.data(), bn.size()))) return rc;
-        i += 8;
     }
-    *consumed = i;
     return 0;
 }
 
@@ -301,59 +302,51 @@ int Tacotron::init(const b200tts_tacotron_config& cfg, const float* const* w, in
     B200_REQUIRE(c.n_vocab > 0 && C > 0 && C <= HW_MAX_CIN && c.out_channels > 0 && c.r_init >= 1 &&
                  (c.attention_type == 0 || c.attention_type == 1), "tacotron: unsupported config");
     Cm = c.memory_size > 0 ? C * c.memory_size : C;
-    const int cbhg_n_enc = 16 * 5 + 10 + 16 + 8, cbhg_n_post = 8 * 5 + 10 + (C != HW ? 1 : 0) + 16 + 8;
-    const int expect = 1 + 4 + cbhg_n_enc + 2 * (c.prenet_bn ? 6 : 2) + 4 +
-                       TacoAttention::n_weights(c.attention_type, c.location_attn) + 2 + 8 + 2 + 2 + cbhg_n_post + 2;
-    B200_REQUIRE(nw == expect, "tacotron: expected %d weight tensors, got %d", expect, nw);
-    int rc, i = 0, used = 0;
-    if ((rc = upload(emb, w[i++], (size_t)c.n_vocab * EMB))) return rc;
-    if ((rc = pack_conv(eprenet[0], w[i], w[i + 1], PN0, EMB, 1, 1, 0))) return rc;
-    if ((rc = pack_conv(eprenet[1], w[i + 2], w[i + 3], PN1, PN0, 1, 1, 0))) return rc;
-    i += 4;
-    if ((rc = ecbhg.init(PN1, 16, 128, w + i, &used))) return rc;
-    i += used;
+    WeightList wl(w, nw);
+    int rc;
+    if ((rc = upload(emb, wl.take(), (size_t)c.n_vocab * EMB))) return rc;
+    const float *p0w = wl.take(), *p0b = wl.take(), *p1w = wl.take(), *p1b = wl.take();
+    if ((rc = pack_conv(eprenet[0], p0w, p0b, PN0, EMB, 1, 1, 0))) return rc;
+    if ((rc = pack_conv(eprenet[1], p1w, p1b, PN1, PN0, 1, 1, 0))) return rc;
+    if ((rc = ecbhg.init(PN1, 16, 128, wl))) return rc;
     std::vector<float> wf, bf;
     for (int l = 0; l < 2; ++l) {   // decoder prenet (with bias); "bn": eval BatchNorm (eps 1e-5) folded into the layer
         const int in = l ? PN0 : Cm, out = l ? PN1 : PN0;
         if (!c.prenet_bn) {
-            if ((rc = upload(prenet_w[l], w[i], (size_t)out * in))) return rc;
-            if ((rc = upload(prenet_b[l], w[i + 1], out))) return rc;
-            i += 2;
+            if ((rc = upload(prenet_w[l], wl.take(), (size_t)out * in))) return rc;
+            if ((rc = upload(prenet_b[l], wl.take(), out))) return rc;
             continue;
         }
-        fold_bn(w[i], w[i + 1], w + i + 2, 1e-5, out, in, wf, bf);
+        if ((rc = fold_bn(wl, true, 1e-5, out, in, wf, bf))) return rc;
         if ((rc = upload(prenet_w[l], wf.data(), wf.size()))) return rc;
         if ((rc = upload(prenet_b[l], bf.data(), bf.size()))) return rc;
-        i += 6;
     }
     // a GRUCell: W_ih, W_hh, bias [4][H] = (b_ir + b_hr, b_iz + b_hz, b_in, b_hn)
     auto gru = [&](DevBuf<float>& wih, DevBuf<float>& whh_, DevBuf<float>& bias, int in, int H) -> int {
         int r;
-        if ((r = upload(wih, w[i], (size_t)3 * H * in))) return r;
-        if ((r = upload(whh_, w[i + 1], (size_t)3 * H * H))) return r;
+        if ((r = upload(wih, wl.take(), (size_t)3 * H * in))) return r;
+        if ((r = upload(whh_, wl.take(), (size_t)3 * H * H))) return r;
+        const float *b_ih = wl.take(), *b_hh = wl.take();
+        B200_REQUIRE(b_ih && b_hh, "tacotron: null GRUCell bias");
         std::vector<float> b((size_t)4 * H);
-        for (int k = 0; k < 2 * H; ++k) b[k] = w[i + 2][k] + w[i + 3][k];
-        for (int k = 0; k < H; ++k) { b[2 * H + k] = w[i + 2][2 * H + k]; b[3 * H + k] = w[i + 3][2 * H + k]; }
-        i += 4;
+        for (int k = 0; k < 2 * H; ++k) b[k] = b_ih[k] + b_hh[k];
+        for (int k = 0; k < H; ++k) { b[2 * H + k] = b_ih[2 * H + k]; b[3 * H + k] = b_hh[2 * H + k]; }
         return upload(bias, b.data(), b.size());
     };
     if ((rc = gru(arnn_wih, arnn_whh, arnn_b, PN1 + E, Q))) return rc;
-    if ((rc = att.init(Q, E, c.attention_type, c.location_attn, c.attention_norm, w + i, &used))) return rc;
-    i += used;
-    if ((rc = upload(pdi_w, w[i], (size_t)D * (Q + E)))) return rc;
-    if ((rc = upload(pdi_b, w[i + 1], D))) return rc;
-    i += 2;
+    if ((rc = att.init(Q, E, c.attention_type, c.location_attn, c.attention_norm, wl))) return rc;
+    if ((rc = upload(pdi_w, wl.take(), (size_t)D * (Q + E)))) return rc;
+    if ((rc = upload(pdi_b, wl.take(), D))) return rc;
     for (int l = 0; l < 2; ++l)
         if ((rc = gru(drnn_wih[l], drnn_whh[l], drnn_b[l], D, D))) return rc;
-    if ((rc = upload(proj_w, w[i], (size_t)RC * D))) return rc;
-    if ((rc = upload(proj_b, w[i + 1], RC))) return rc;
-    if ((rc = upload(stop_w, w[i + 2], (size_t)D + RC))) return rc;
-    if ((rc = upload(stop_b, w[i + 3], 1))) return rc;
-    i += 4;
-    if ((rc = pcbhg.init(C, 8, 256, w + i, &used))) return rc;
-    i += used;
-    if ((rc = pack_conv(last, w[i], w[i + 1], c.out_channels, 2 * GRU_H, 1, 1, 0))) return rc;
-    return 0;
+    if ((rc = upload(proj_w, wl.take(), (size_t)RC * D))) return rc;
+    if ((rc = upload(proj_b, wl.take(), RC))) return rc;
+    if ((rc = upload(stop_w, wl.take(), (size_t)D + RC))) return rc;
+    if ((rc = upload(stop_b, wl.take(), 1))) return rc;
+    if ((rc = pcbhg.init(C, 8, 256, wl))) return rc;
+    const float *lw = wl.take(), *lb = wl.take();
+    if ((rc = pack_conv(last, lw, lb, c.out_channels, 2 * GRU_H, 1, 1, 0))) return rc;
+    return wl.finish("tacotron");
 }
 
 // encode: the loop state (kept until the loop ends), the embedding and its mask, the prenet outputs, the transposed

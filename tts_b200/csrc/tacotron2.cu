@@ -106,48 +106,43 @@ int Tacotron2::init(const b200tts_tacotron2_config& cfg, const float* const* w, 
     const int C = c.out_channels;
     B200_REQUIRE(c.n_vocab > 0 && C > 0 && c.r_init >= 1 && (c.attention_type == 0 || c.attention_type == 1),
                  "tacotron2: unsupported config");
-    const int expect = 1 + 6 * 3 + 8 + 2 * (c.prenet_bn ? 5 : 1) + 4 +
-                       TacoAttention::n_weights(c.attention_type, c.location_attn) + 4 + 2 + 2 + 6 * 5;
-    B200_REQUIRE(nw == expect, "tacotron2: expected %d weight tensors, got %d", expect, nw);
-    int rc, i = 0, used = 0;
-    if ((rc = enc.init(c.n_vocab, E, HE, 3, w, &used))) return rc;
-    i += used;
+    WeightList wl(w, nw);
+    int rc;
+    if ((rc = enc.init(c.n_vocab, E, HE, 3, wl))) return rc;
     std::vector<float> wf, bf;
     for (int l = 0; l < 2; ++l) {   // prenet (no bias); "bn": eval BatchNorm folded into the layer
         const int in = l ? PN : C;
         if (!c.prenet_bn) {
-            if ((rc = upload(prenet_w[l], w[i++], (size_t)PN * in))) return rc;
+            if ((rc = upload(prenet_w[l], wl.take(), (size_t)PN * in))) return rc;
             continue;
         }
-        fold_bn(w[i], nullptr, w + i + 1, 1e-5, PN, in, wf, bf);
+        if ((rc = fold_bn(wl, false, 1e-5, PN, in, wf, bf))) return rc;
         if ((rc = upload(prenet_w[l], wf.data(), wf.size()))) return rc;
         if ((rc = upload(prenet_b[l], bf.data(), bf.size()))) return rc;
-        i += 5;
     }
     auto lstm = [&](DevBuf<float>& wih, DevBuf<float>& whh, DevBuf<float>& bias, int in, int H) -> int {
         int r;
-        if ((r = upload(wih, w[i], (size_t)4 * H * in))) return r;
-        if ((r = upload(whh, w[i + 1], (size_t)4 * H * H))) return r;
+        if ((r = upload(wih, wl.take(), (size_t)4 * H * in))) return r;
+        if ((r = upload(whh, wl.take(), (size_t)4 * H * H))) return r;
+        const float *b_ih = wl.take(), *b_hh = wl.take();
+        B200_REQUIRE(b_ih && b_hh, "tacotron2: null LSTMCell bias");
         std::vector<float> b((size_t)4 * H);
-        for (int k = 0; k < 4 * H; ++k) b[k] = w[i + 2][k] + w[i + 3][k];
-        i += 4;
+        for (int k = 0; k < 4 * H; ++k) b[k] = b_ih[k] + b_hh[k];
         return upload(bias, b.data(), b.size());
     };
     if ((rc = lstm(arnn_wih, arnn_whh, arnn_b, PN + E, Q))) return rc;
-    if ((rc = att.init(Q, E, c.attention_type, c.location_attn, c.attention_norm, w + i, &used))) return rc;
-    i += used;
+    if ((rc = att.init(Q, E, c.attention_type, c.location_attn, c.attention_norm, wl))) return rc;
     if ((rc = lstm(drnn_wih, drnn_whh, drnn_b, Q + E, D))) return rc;
-    if ((rc = upload(proj_w, w[i], (size_t)C * c.r_init * (D + E)))) return rc;
-    if ((rc = upload(proj_b, w[i + 1], (size_t)C * c.r_init))) return rc;
-    if ((rc = upload(stop_w, w[i + 2], (size_t)D + C * c.r_init))) return rc;
-    if ((rc = upload(stop_b, w[i + 3], 1))) return rc;
-    i += 4;
-    for (int l = 0; l < 5; ++l, i += 6) {   // Postnet ConvBNBlocks, BatchNorm folded
+    if ((rc = upload(proj_w, wl.take(), (size_t)C * c.r_init * (D + E)))) return rc;
+    if ((rc = upload(proj_b, wl.take(), (size_t)C * c.r_init))) return rc;
+    if ((rc = upload(stop_w, wl.take(), (size_t)D + C * c.r_init))) return rc;
+    if ((rc = upload(stop_b, wl.take(), 1))) return rc;
+    for (int l = 0; l < 5; ++l) {   // Postnet ConvBNBlocks, BatchNorm folded
         const int ci = l ? 512 : C, co = l == 4 ? C : 512;
-        fold_bn(w[i], w[i + 1], w + i + 2, 1e-5, co, (size_t)ci * 5, wf, bf);
+        if ((rc = fold_bn(wl, true, 1e-5, co, (size_t)ci * 5, wf, bf))) return rc;
         if ((rc = pack_conv(post[l], wf.data(), bf.data(), co, ci, 5, 1, 2))) return rc;
     }
-    return 0;
+    return wl.finish("tacotron2");
 }
 
 int Tacotron2::encode(const long long* tokens, const long long* lengths, int B, int Tt, float* enc_out, void* ws,

@@ -266,38 +266,39 @@ int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, 
 }
 
 int RelPosTransformer::init(int channels, int ffn_channels, int kernel_size, int num_heads, int window_size,
-                            float ln_eps, int num_layers, const float* const* w, int* consumed) {
+                            float ln_eps, int num_layers, WeightList& wl) {
     C = channels; F = ffn_channels; heads = num_heads; window = window_size; eps = ln_eps;
     const int K = kernel_size, d = C / heads;
     const int nrel = 2 * window + 1;
-    const int per = window >= 0 ? 18 : 16;
     int rc;
     layers.resize(num_layers);
     for (int l = 0; l < num_layers; ++l) {
-        const float* const* p = w + (size_t)l * per;
         Layer& L = layers[l];
         if (window >= 0) {
-            if ((rc = upload(L.rel_k, p[0], (size_t)nrel * d))) return rc;
-            if ((rc = upload(L.rel_v, p[1], (size_t)nrel * d))) return rc;
-            p += 2;
+            if ((rc = upload(L.rel_k, wl.take(), (size_t)nrel * d))) return rc;
+            if ((rc = upload(L.rel_v, wl.take(), (size_t)nrel * d))) return rc;
         }
         // fused QKV: rows [q | k | v]
         std::vector<float> wq((size_t)3 * C * C), bq((size_t)3 * C);
         for (int s = 0; s < 3; ++s) {
-            memcpy(wq.data() + (size_t)s * C * C, p[2 * s], sizeof(float) * C * C);
-            memcpy(bq.data() + (size_t)s * C, p[2 * s + 1], sizeof(float) * C);
+            const float *sw = wl.take(), *sb = wl.take();
+            B200_REQUIRE(sw && sb, "rel_pos_transformer: null q / k / v weight or bias");
+            memcpy(wq.data() + (size_t)s * C * C, sw, sizeof(float) * C * C);
+            memcpy(bq.data() + (size_t)s * C, sb, sizeof(float) * C);
         }
         if ((rc = pack_conv(L.qkv, wq.data(), bq.data(), 3 * C, C, 1, 1, 0))) return rc;
-        if ((rc = pack_conv(L.o, p[6], p[7], C, C, 1, 1, 0))) return rc;
-        if ((rc = upload(L.ln1_g, p[8], C))) return rc;
-        if ((rc = upload(L.ln1_b, p[9], C))) return rc;
+        const float *ow = wl.take(), *ob = wl.take();
+        if ((rc = pack_conv(L.o, ow, ob, C, C, 1, 1, 0))) return rc;
+        if ((rc = upload(L.ln1_g, wl.take(), C))) return rc;
+        if ((rc = upload(L.ln1_b, wl.take(), C))) return rc;
         // FeedForwardNetwork._same_padding: pad_l = (k-1)//2 (transformer.py:307-313)
-        if ((rc = pack_conv(L.ffn1, p[10], p[11], F, C, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = pack_conv(L.ffn2, p[12], p[13], C, F, K, 1, (K - 1) / 2))) return rc;
-        if ((rc = upload(L.ln2_g, p[14], C))) return rc;
-        if ((rc = upload(L.ln2_b, p[15], C))) return rc;
+        const float *f1w = wl.take(), *f1b = wl.take();
+        if ((rc = pack_conv(L.ffn1, f1w, f1b, F, C, K, 1, (K - 1) / 2))) return rc;
+        const float *f2w = wl.take(), *f2b = wl.take();
+        if ((rc = pack_conv(L.ffn2, f2w, f2b, C, F, K, 1, (K - 1) / 2))) return rc;
+        if ((rc = upload(L.ln2_g, wl.take(), C))) return rc;
+        if ((rc = upload(L.ln2_b, wl.take(), C))) return rc;
     }
-    *consumed = per * num_layers;
     return 0;
 }
 
@@ -368,17 +369,15 @@ int TextEncoder::init(const b200tts_text_encoder_config& cfg, const float* const
     const int d = C / c.num_heads;
     B200_REQUIRE(d <= ATT_MAXD, "text_encoder: head dim %d > %d", d, ATT_MAXD);
     B200_REQUIRE(c.rel_attn_window_size >= 0 && 2 * c.rel_attn_window_size + 1 <= 32, "text_encoder: bad window");
-    const int per = 18;
-    B200_REQUIRE(nw == 1 + per * c.num_layers + 2, "text_encoder: expected %d weight tensors, got %d",
-                 1 + per * c.num_layers + 2, nw);
+    WeightList wl(w, nw);
     int rc;
-    if ((rc = upload(emb, w[0], (size_t)c.n_vocab * c.hidden_channels))) return rc;
-    int used = 0;
+    if ((rc = upload(emb, wl.take(), (size_t)c.n_vocab * c.hidden_channels))) return rc;
     if ((rc = tf.init(C, c.hidden_channels_ffn, c.kernel_size, c.num_heads, c.rel_attn_window_size, 1e-5f,
-                      c.num_layers, w + 1, &used)))
+                      c.num_layers, wl)))
         return rc;
-    const float* const* p = w + 1 + used;
-    return pack_conv(proj, p[0], p[1], 2 * c.out_channels, C, 1, 1, 0);
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(proj, pw, pb, 2 * c.out_channels, C, 1, 1, 0))) return rc;
+    return wl.finish("text_encoder");
 }
 
 // the whole workspace is the transformer's

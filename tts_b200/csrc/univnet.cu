@@ -314,14 +314,13 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
         hop_total *= c.upsample_factors[s];
     }
     B200_REQUIRE(hop_total <= 4096, "univnet: %d samples per frame (at most 4096)", hop_total);
-    const int expect = 2 + S * (2 + 2 + 12 + 4 + 2 * L) + 2;
-    B200_REQUIRE(nw == expect, "univnet: expected %d weight tensors, got %d", expect, nw);
     for (int i = 0; i < nw; ++i) B200_REQUIRE(w[i] != nullptr, "univnet: weight tensor %d is null", i);
     MP = L * (KSZ + CO);
-    int i = 0, rc;
+    WeightList wl(w, nw);
+    int rc;
     first.tc_prec = B200TTS_PRECISION_FP32;
-    if ((rc = pack_conv(first, w[0], w[1], C, c.in_channels, 7, 1, 3))) return rc;
-    i = 2;
+    const float *fw = wl.take(), *fb = wl.take();
+    if ((rc = pack_conv(first, fw, fb, C, c.in_channels, 7, 1, 3))) return rc;
     blocks.resize(S);
     int hop = 1;
     const int Kd = Kp * Ch, kpad = (Kp - 1) / 2;
@@ -331,20 +330,20 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
         hop *= u;
         bl.hop = hop;
         bl.up.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv_transpose(bl.up, w[i], w[i + 1], C, C, 2 * u, u, u / 2 + u % 2, u % 2))) return rc;
-        i += 2;
+        const float *uw = wl.take(), *ub = wl.take();
+        if ((rc = pack_conv_transpose(bl.up, uw, ub, C, C, 2 * u, u, u / 2 + u % 2, u % 2))) return rc;
         bl.kin.tc_prec = B200TTS_PRECISION_FP32;
-        if ((rc = pack_conv(bl.kin, w[i], w[i + 1], Ch, c.cond_channels, 5, 1, 2))) return rc;
-        i += 2;
+        const float *iw = wl.take(), *ib = wl.take();
+        if ((rc = pack_conv(bl.kin, iw, ib, Ch, c.cond_channels, 5, 1, 2))) return rc;
         bl.kres.resize(6);
         for (auto& l : bl.kres) {
             l.tc_prec = B200TTS_PRECISION_FP32;
-            if ((rc = pack_conv(l, w[i], w[i + 1], Ch, Ch, Kp, 1, kpad))) return rc;
-            i += 2;
+            const float *rw = wl.take(), *rb = wl.take();
+            if ((rc = pack_conv(l, rw, rb, Ch, Ch, Kp, 1, kpad))) return rc;
         }
         // kernel_conv | bias_conv as one GEMM, rows permuted into the frame-major layout (see the top of this file)
-        const float *kw = w[i], *kb = w[i + 1], *bw = w[i + 2], *bb = w[i + 3];
-        i += 4;
+        const float *kw = wl.take(), *kb = wl.take(), *bw = wl.take(), *bb = wl.take();
+        B200_REQUIRE(kw && kb && bw && bb, "univnet: null kernel_conv / bias_conv weight or bias");
         std::vector<float> W((size_t)MP * Kd), bias(MP);
         auto put = [&](int m, const float* src, float bsrc) {   // src: [Ch][Kp] of one reference output channel
             for (int tap = 0; tap < Kp; ++tap)
@@ -363,18 +362,22 @@ int Univnet::init(const b200tts_univnet_config& cfg, const float* const* w, int 
         if (upload(bl.pw, W.data(), W.size()) || upload(bl.pb, bias.data(), bias.size())) return 2;
         // conv_i: [layer][co][tap * 32 + ci]
         std::vector<float> cw((size_t)L * C * KK), cb((size_t)L * C);
-        for (int l = 0; l < L; ++l, i += 2) {
+        for (int l = 0; l < L; ++l) {
+            const float *lw = wl.take(), *lb = wl.take();
+            B200_REQUIRE(lw && lb, "univnet: null conv_i weight or bias");
             for (int co = 0; co < C; ++co) {
                 for (int ci = 0; ci < C; ++ci)
                     for (int tap = 0; tap < 3; ++tap)
-                        cw[((size_t)l * C + co) * KK + tap * C + ci] = w[i][((size_t)co * C + ci) * 3 + tap];
-                cb[(size_t)l * C + co] = w[i + 1][co];
+                        cw[((size_t)l * C + co) * KK + tap * C + ci] = lw[((size_t)co * C + ci) * 3 + tap];
+                cb[(size_t)l * C + co] = lb[co];
             }
         }
         if (upload(bl.cw, cw.data(), cw.size()) || upload(bl.cb, cb.data(), cb.size())) return 2;
     }
     last.tc_prec = B200TTS_PRECISION_FP32;
-    return pack_conv(last, w[i], w[i + 1], c.out_channels, C, 7, 1, 3);
+    const float *lw = wl.take(), *lb = wl.take();
+    if ((rc = pack_conv(last, lw, lb, c.out_channels, C, 7, 1, 3))) return rc;
+    return wl.finish("univnet");
 }
 
 // the KPnet hidden state (3 tensors); forward() also takes the predicted kernels of one block (P) and two x tensors at

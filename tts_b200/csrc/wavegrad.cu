@@ -96,16 +96,14 @@ int Wavegrad::init(const b200tts_wavegrad_config& cfg, const float* const* w, in
                          "wavegrad: dblock_out_channels[%d] = %d must equal ublock_out_channels[%d] = %d", i,
                          c.dblock_out_channels[i], n - 1 - i, c.ublock_out_channels[n - 1 - i]);
     }
-    const int expect = 2 + 8 * (n - 1) + 4 * n + 10 * n + 4;
-    B200_REQUIRE(nw == expect, "wavegrad: expected %d weight tensors, got %d", expect, nw);
     for (int i = 0; i < nw; ++i) B200_REQUIRE(w[i] != nullptr, "wavegrad: null weight %d", i);
-    int i = 0, rc;
+    WeightList wl(w, nw);
+    int rc;
     // split-fp16 operands where Cin % 16 == 0 (pack_rows falls back to 3xTF32 otherwise; y_conv's Cin 1 runs on FMA)
     auto conv = [&](ConvLayer& L, int Cout, int Cin, int K, int dil) -> int {
         L.tc_prec = B200TTS_PRECISION_F16X3;
-        const int r = pack_conv(L, w[i], w[i + 1], Cout, Cin, K, dil, (K - 1) / 2 * dil);
-        i += 2;
-        return r;
+        const float *cw = wl.take(), *cb = wl.take();
+        return pack_conv(L, cw, cb, Cout, Cin, K, dil, (K - 1) / 2 * dil);
     };
     if ((rc = conv(y_conv, c.y_conv_channels, 1, 5, 1))) return rc;
     db.resize(n - 1);
@@ -137,8 +135,8 @@ int Wavegrad::init(const b200tts_wavegrad_config& cfg, const float* const* w, in
         ic = hc;
     }
     if ((rc = conv(x_conv, c.x_conv_channels, c.in_channels, 3, 1))) return rc;
-    if (upload(out_w, w[i], (size_t)ic * 3) || upload(out_b, w[i + 1], 1)) return 2;
-    return 0;
+    if ((rc = upload(out_w, wl.take(), (size_t)ic * 3)) || (rc = upload(out_b, wl.take(), 1))) return rc;
+    return wl.finish("wavegrad");
 }
 
 // per-batch-row floats: [0] conditioning, [1 .. n] FiLM tensors, [n + 1] one stage buffer (five are used)
