@@ -163,6 +163,30 @@ int b200tts_debug_conv1d_create(const b200tts_conv1d_config* cfg, const float* w
                                 const int32_t* in_perm, const int32_t* out_perm, b200tts_conv1d** out);
 int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* io, void* stream);
 
+/* Debug / test aids: the transformer layers' attention and add + LayerNorm kernels, one launch at a time, as the engines
+ * call them (device pointers, [B, C, T] layouts, time contiguous).  Not a stable interface.
+ *   attention: the FP32-FMA multi-head attention of the VITS / Glow-TTS text encoders, ForwardTTS's text encoder and
+ *     the ForwardTTS decoder's fallback.  qkv [B, 3C, T] (rows q | k | v, head h owns channels [h d, (h + 1) d), d =
+ *     C / num_heads <= 384), mask [B, T] (1 valid, 0 padded), out [B, C, T]:
+ *       s_ij = (q_i . k_j + [|j - i| <= window] q_i . rel_k[j - i + window]) / sqrt(d);  s_ij = -1e4 where
+ *       mask_i mask_j == 0;  p = softmax_j(s);  out_i = sum_j p_ij v_j + sum_{|j - i| <= window} p_ij rel_v[j - i + window]
+ *     rel_k / rel_v [2 window + 1, d] (shared by the heads); window = -1: no relative terms and rel_k / rel_v unused
+ *     (NULL); window <= 15.  Every column below T is read, padded ones included: they must be finite.  A padded query
+ *     row is the uniform softmax over all T keys.  Status 1 (no launch) for d > 384, window > 15, or T past the
+ *     kernel's shared memory (8 (d + Tp) + 33 (d + 1) + 2 nrel d floats <= 200 KiB, Tp = T rounded up to 32, nrel =
+ *     2 window + 1, or 0 without a window).
+ *   add_layernorm: out[b, :, t] = LayerNorm over the C channels of v = x + y (y NULL: v = x), biased variance,
+ *     (v - mean) / sqrt(var + eps) * gamma + beta, then
+ *       kind 0 (VITS / Glow-TTS layers, Glow-TTS prenet, duration predictor): times mask[b, t] (mask NULL: 1); twice = 0;
+ *       kind 1 (ForwardTTS FFTransformer): v = (x + y) + y when twice != 0; y and mask required; an exact 0 where
+ *         mask[b, t] == 0, whatever x and y hold there (a select, so NaN does not leak); eps must be 1e-5.
+ *     out may be x (the layers run in place).  Status 1 (no launch) for anything else. */
+int b200tts_debug_attention(const float* qkv, const float* mask, const float* rel_k, const float* rel_v, float* out,
+                            int B, int C, int T, int num_heads, int window, void* stream);
+int b200tts_debug_add_layernorm(int kind, const float* x, const float* y, int twice, const float* gamma,
+                                const float* beta, const float* mask, float* out, int B, int C, int T, float eps,
+                                void* stream);
+
 /* ---- monotonic alignment search ------------------------------------------------------------
  * Replaces maximum_path_c / maximum_path_each, TTS/tts/utils/monotonic_align/core.pyx:11-47
  * (called through TTS/tts/utils/helpers.py:172-194 from Vits.forward_mas, vits.py:919).
@@ -661,6 +685,7 @@ int b200tts_forward_tts_decode(const b200tts_forward_tts* h, const float* o_en, 
  * Replaces nn.MultiheadAttention's attention core (softmax((q d^-1/2) k^T) v, torch/nn/functional.py
  * multi_head_attention_forward) over a fused [B, 3C, pitch] q|k|v tensor, per row over its first lens[b] (int32) frames.
  * out [B, C, pitch]; columns lens[b] .. pitch-1 are zeroed.  Heads need (C / num_heads) % 8 == 0 and <= 384.
+ * T <= pitch bounds the rows' lengths (lens[b] <= T); columns of q|k|v at or past lens[b] are never read.
  */
 int b200tts_attention_tc3(const float* qkv, const int* lens, int B, int C, int num_heads, int T, int pitch, float* out,
                           void* stream);

@@ -54,6 +54,26 @@ def test_library_exports_the_debug_conv_layer():
     assert ctypes.sizeof(_lib.DebugConvIOC) == 216    # static_assert in capi.cu
 
 
+def test_library_exports_the_debug_attention_and_layernorm():
+    """the per-kernel transformer aids (b200tts_debug_attention / _add_layernorm) are declared, exported and bound"""
+    from tts_b200 import _lib
+
+    syms = declared_symbols()
+    assert "b200tts_debug_attention" in syms and "b200tts_debug_add_layernorm" in syms
+    lib = _lib.lib()
+    vp, ci = ctypes.c_void_p, ctypes.c_int
+    assert lib.b200tts_debug_attention.restype is ci
+    assert lib.b200tts_debug_attention.argtypes == [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
+    assert lib.b200tts_debug_add_layernorm.restype is ci
+    assert lib.b200tts_debug_add_layernorm.argtypes == [ci, vp, vp, ci, vp, vp, vp, vp, ci, ci, ci, ctypes.c_float, vp]
+    # the bindings follow the header's parameter lists
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "tts_b200.h")).read(), flags=re.S)
+    for name, n in (("b200tts_debug_attention", 11), ("b200tts_debug_add_layernorm", 13)):
+        params = re.search(name + r"\(([^)]*)\);", src).group(1).split(",")
+        assert len(params) == n == len(getattr(lib, name).argtypes), name
+    assert "float eps" in re.search(r"b200tts_debug_add_layernorm\(([^)]*)\);", src).group(1).split(",")[11]
+
+
 def test_product_fails_loudly_without_cuda():
     import pytest
     import torch

@@ -4,6 +4,8 @@ Each handle the library offers is built through its Python module at a small siz
 b200tts_debug_device_buffers() counts the live device buffers of all handles, so it must rise with the build and come
 back to its earlier value with the drop: a buffer a handle leaks, or frees twice, shows up as a difference.
 """
+import gc
+
 import pytest
 import torch
 
@@ -162,6 +164,9 @@ HANDLES = [hifigan, flow_reverse, flow_forward, text_encoder, sdp, posterior, du
 def test_handle_frees_every_device_buffer_it_made(make):
     torch.manual_seed(0)
     build, drop = make()
+    # handles of earlier tests that only a garbage collection frees must not be freed during build(): the count would
+    # drop by theirs
+    gc.collect()
     before = live_buffers()
     for _ in range(2):
         build()

@@ -209,6 +209,10 @@ def _declare(lib):
                                                 ctypes.POINTER(vp)]
     lib.b200tts_debug_conv1d_launch.restype = ci
     lib.b200tts_debug_conv1d_launch.argtypes = [vp, ctypes.POINTER(DebugConvIOC), vp]
+    lib.b200tts_debug_attention.restype = ci
+    lib.b200tts_debug_attention.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
+    lib.b200tts_debug_add_layernorm.restype = ci
+    lib.b200tts_debug_add_layernorm.argtypes = [ci, vp, vp, ci, vp, vp, vp, vp, ci, ci, ci, ctypes.c_float, vp]
     lib.b200tts_melgan_create.restype = ci
     lib.b200tts_melgan_create.argtypes = [ctypes.POINTER(MelganConfigC), ctypes.POINTER(vp), ci, ctypes.POINTER(vp)]
     lib.b200tts_melgan_destroy.restype = None

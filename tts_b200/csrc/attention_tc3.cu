@@ -10,7 +10,8 @@
 //   S = (q * d^-1/2) . K     [FA_BQ x FA_BK]   warps: 2 query m-tiles x 4 groups of 2 key n-tiles
 //   O = O * alpha + P . V^T  [FA_BQ x d]       warps: 2 query m-tiles x 4 groups of channel n-tiles (<= 12 each)
 // q is scaled before the product, as torch does.  Key columns at or beyond lens[b] are never read (they may hold stale
-// scratch); they load as zero and score -inf.  Query columns in [lens[b], pitch) of the output are written as zero.
+// scratch, NaN included); they load as zero and score -inf.  Query columns in [lens[b], pitch) of the output are written
+// as zero: the grid covers every query tile below the pitch, not only those below T.
 // Heads need d % 8 == 0 and d <= FA_MAXD; the caller takes the FP32-FMA kernel otherwise.
 #include <math.h>
 
@@ -251,7 +252,7 @@ int launch_attention_tc3(const float* qkv, long long qkv_bs, int pitch, const in
     const int d = C / num_heads;
     B200_REQUIRE(attention_tc3_takes(d), "attention_tc3: head dim %d needs d %% 8 == 0 and d <= %d", d, FA_MAXD);
     B200_REQUIRE(T >= 0 && T <= pitch, "attention_tc3: T=%d exceeds the row pitch %d", T, pitch);
-    if (B == 0 || T == 0) return 0;
+    if (B == 0 || pitch == 0) return 0;
     const size_t smem = attention_tc3_smem(d);
     static DeviceOnce attr_once;
     if (int rc0 = device_once(attr_once, nullptr, [](int) -> int {
@@ -259,7 +260,8 @@ int launch_attention_tc3(const float* qkv, long long qkv_bs, int pitch, const in
                                               (int)attention_tc3_smem(FA_MAXD)));
             return 0;
         })) return rc0;
-    dim3 grid((T + FA_BQ - 1) / FA_BQ, num_heads, B);
+    // T only bounds the rows' lengths: the padded columns up to the pitch are zeroed too, so the grid spans the pitch
+    dim3 grid((pitch + FA_BQ - 1) / FA_BQ, num_heads, B);
     attention_tc3_kernel<<<grid, 32 * FA_WARPS, smem, st>>>(qkv, qkv_bs, pitch, lens, out, out_bs, C, d,
                                                            (float)sqrt(1.0 / (double)d));
     count_launch();

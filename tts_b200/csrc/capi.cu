@@ -212,6 +212,35 @@ int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_con
     return launch_conv(h->L, io, (cudaStream_t)stream);
 }
 
+int b200tts_debug_attention(const float* qkv, const float* mask, const float* rel_k, const float* rel_v, float* out,
+                            int B, int C, int T, int num_heads, int window, void* stream) {
+    if (!qkv || !mask || !out) { set_error("debug_attention: null argument"); return 1; }
+    if (B < 0 || T < 0) { set_error("debug_attention: B=%d, T=%d", B, T); return 1; }
+    if (int rc = launch_attention(qkv, mask, window < 0 ? nullptr : rel_k, window < 0 ? nullptr : rel_v, out, B, C, T,
+                                  num_heads, window, (cudaStream_t)stream))
+        return rc;
+    if (B > 0 && T > 0) dispatch_note(DISPATCH_ATTN_FMA);
+    return 0;
+}
+
+int b200tts_debug_add_layernorm(int kind, const float* x, const float* y, int twice, const float* gamma,
+                                const float* beta, const float* mask, float* out, int B, int C, int T, float eps,
+                                void* stream) {
+    if (!x || !gamma || !beta || !out) { set_error("debug_add_layernorm: null argument"); return 1; }
+    if (B < 0 || C < 1 || T < 0) { set_error("debug_add_layernorm: B=%d, C=%d, T=%d", B, C, T); return 1; }
+    if (kind == 0) {
+        if (twice) { set_error("debug_add_layernorm: kind 0 has no `twice` residual"); return 1; }
+        return launch_add_layernorm(x, y, gamma, beta, mask, out, B, C, T, eps, (cudaStream_t)stream);
+    }
+    if (kind == 1) {
+        if (!y || !mask) { set_error("debug_add_layernorm: kind 1 needs y and mask"); return 1; }
+        if (eps != 1e-5f) { set_error("debug_add_layernorm: kind 1 has eps 1e-5, not %g", (double)eps); return 1; }
+        return launch_add_norm(x, y, twice != 0, gamma, beta, mask, out, B, C, T, (cudaStream_t)stream);
+    }
+    set_error("debug_add_layernorm: unknown kind %d", kind);
+    return 1;
+}
+
 size_t b200tts_mas_workspace_bytes(int B, int Tx, int Ty) { return mas_workspace_bytes(B, Tx, Ty); }
 
 int b200tts_mas(const float* value, const float* mask, const int32_t* t_x, const int32_t* t_y, int B, int Tx,

@@ -92,6 +92,10 @@ struct DurPred {
 int launch_upsample_linear(const float* x, int rows, int Tin, float scale_factor, float* y, int Tout, cudaStream_t st);
 int launch_add_layernorm(const float* x, const float* y, const float* gamma, const float* beta, const float* mask,
                          float* out, int B, int C, int T, float eps, cudaStream_t st);
+// forward_tts.cu's FFTransformer norm: LayerNorm_c(twice ? (x + y) + y : x + y) (eps 1e-5) where mask[b, t] != 0, an
+// exact 0 elsewhere (a select: NaN in masked columns does not leak); y and mask are required
+int launch_add_norm(const float* x, const float* y, bool twice, const float* g, const float* bta, const float* mask,
+                    float* out, int B, int C, int T, cudaStream_t st);
 // text_encoder.cu's embedding (x = emb[tok] * sqrt(hidden) * mask, plus the x_mask; without the sqrt(hidden) scale when
 // scale_sqrt_hidden is false) and multi-head attention over a fused [B, 3C, T] q|k|v tensor; window < 0: no
 // relative-position terms (rel_k / rel_v unused).  Heads up to 384 channels.

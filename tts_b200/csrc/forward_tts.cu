@@ -114,15 +114,6 @@ __global__ void mel_out_kernel(const float* pm, const long long* y_lengths, floa
     mel[(size_t)b * Ty * Co + i] = (long long)t < y_lengths[b] ? pm[((size_t)b * Co + o) * Tp + t] : 0.f;
 }
 
-int launch_add_norm(const float* x, const float* y, bool twice, const float* g, const float* bta, const float* mask,
-                    float* out, int B, int C, int T, cudaStream_t st) {
-    dim3 grid((T + 31) / 32, B);
-    fft_add_norm_kernel<<<grid, 256, 0, st>>>(x, y, twice ? 1 : 0, g, bta, mask, out, C, T, 1e-5f);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
 int pack_layer(ForwardTTS::Layer& L, WeightList& wl, int C, int F, int prec) {
     int rc;
     L.qkv.tc_prec = L.o.tc_prec = L.ffn1.tc_prec = L.ffn2.tc_prec = prec;
@@ -139,6 +130,16 @@ int pack_layer(ForwardTTS::Layer& L, WeightList& wl, int C, int F, int prec) {
 }
 
 }  // namespace
+
+int launch_add_norm(const float* x, const float* y, bool twice, const float* g, const float* bta, const float* mask,
+                    float* out, int B, int C, int T, cudaStream_t st) {
+    if (B == 0 || T == 0) return 0;
+    dim3 grid((T + 31) / 32, B);
+    fft_add_norm_kernel<<<grid, 256, 0, st>>>(x, y, twice ? 1 : 0, g, bta, mask, out, C, T, 1e-5f);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
 
 int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* w, int nw) {
     c = cfg;

@@ -32,7 +32,11 @@ constexpr int ATT_KT = 32;      // keys per tile
 constexpr int ATT_MAXD = 256;   // max head dim of the VITS / Glow-TTS instantiation (8 values per lane)
 constexpr int ATT_MAXD_WIDE = 384;   // ForwardTTS's text encoder: one head of 384 channels (12 values per lane)
 
-// qkv [B, 3C, T] (q rows 0..C, k rows C..2C, v rows 2C..3C), head h owns channels [h*d, (h+1)*d); MAXD bounds d
+// qkv [B, 3C, T] (q rows 0..C, k rows C..2C, v rows 2C..3C), head h owns channels [h*d, (h+1)*d); MAXD bounds d.
+// Every column below T of q, k and v is read: a padded key is masked by its score (-1e4, as the reference's
+// masked_fill), not skipped, and its value still enters P.V with probability 0.  So the outputs of valid queries do not
+// depend on padded columns only as long as those are finite (0 * NaN = NaN); callers keep them finite (zero or computed
+// from zero inputs).  A padded query row is the reference's uniform softmax over all T keys, padded ones included.
 template <int MAXD>
 __global__ void __launch_bounds__(32 * ATT_Q) rel_attention_kernel(const float* __restrict__ qkv, const float* __restrict__ mask,
                                                                   const float* __restrict__ emb_rel_k, const float* __restrict__ emb_rel_v,
@@ -220,6 +224,7 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(const float* x, cons
 
 int launch_add_layernorm(const float* x, const float* y, const float* gamma, const float* beta, const float* mask,
                          float* out, int B, int C, int T, float eps, cudaStream_t st) {
+    if (B == 0 || T == 0) return 0;
     dim3 grid((T + 31) / 32, B);
     add_layernorm_kernel<<<grid, 256, 0, st>>>(x, y, gamma, beta, mask, out, C, T, eps);
     count_launch();
@@ -239,10 +244,12 @@ int launch_embed(const long long* tokens, const long long* lengths, const float*
 
 int launch_attention(const float* qkv, const float* x_mask, const float* rel_k, const float* rel_v, float* out, int B,
                      int C, int T, int num_heads, int window, cudaStream_t st) {
+    B200_REQUIRE(num_heads >= 1 && C >= num_heads, "attention: %d channels in %d heads", C, num_heads);
     const int d = C / num_heads;
     B200_REQUIRE(C % num_heads == 0 && d <= ATT_MAXD_WIDE, "attention: head dim %d (C=%d, %d heads) not supported", d, C,
                  num_heads);
     B200_REQUIRE(window < 0 || (rel_k && rel_v && 2 * window + 1 <= 32), "attention: bad relative window");
+    if (B == 0 || T == 0) return 0;
     const int Tp = (T + 31) & ~31;
     const int nrel = window < 0 ? 0 : 2 * window + 1;
     const size_t att_smem = sizeof(float) * ((size_t)ATT_Q * d + (size_t)ATT_Q * Tp + (size_t)(ATT_KT + 1) * (d + 1) +
