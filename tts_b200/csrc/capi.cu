@@ -122,9 +122,9 @@ int b200tts_conv1d_forward(const b200tts_conv1d* h, const float* x, int B, int T
     if (!h) { set_error("conv1d_forward: null handle"); return 1; }
     const int Tout = b200tts_conv1d_out_len(h, T);
     ConvIO io;
-    io.x = x; io.x_bs = (long long)h->c.in_channels * T; io.x_cs = T; io.Tin = T; io.in_slope = in_slope;
-    io.y = y; io.y_bs = (long long)h->c.out_channels * Tout; io.y_cs = Tout; io.Tout = Tout; io.B = B;
-    if (residual) { io.res = residual; io.res_bs = io.y_bs; io.res_cs = Tout; }
+    io.x = dense(x, h->c.in_channels, T); io.Tin = T; io.in_slope = in_slope;
+    io.y = dense(y, h->c.out_channels, Tout); io.Tout = Tout; io.B = B;
+    if (residual) io.res = dense(residual, h->c.out_channels, Tout);
     io.scale = scale; io.post_div = post_div;
     if (accumulate) io.flags |= EPI_ACCUM;
     io.reflect = h->reflect;
@@ -137,9 +137,9 @@ int b200tts_conv1d_forward_strided(const b200tts_conv1d* h, const float* x, long
     if (peak_bits && !tanh) { set_error("conv1d_forward_strided: peak_bits needs the tanh epilogue"); return 1; }
     const int Tout = b200tts_conv1d_out_len(h, T);
     ConvIO io;
-    io.x = x; io.x_bs = x_batch_stride; io.x_cs = x_channel_stride; io.Tin = T; io.in_slope = in_slope;
-    io.y = y; io.y_bs = (long long)h->c.out_channels * Tout; io.y_cs = Tout; io.Tout = Tout; io.B = B;
-    if (residual) { io.res = residual; io.res_bs = io.y_bs; io.res_cs = Tout; }
+    io.x = {x, x_batch_stride, x_channel_stride}; io.Tin = T; io.in_slope = in_slope;
+    io.y = dense(y, h->c.out_channels, Tout); io.Tout = Tout; io.B = B;
+    if (residual) io.res = dense(residual, h->c.out_channels, Tout);
     io.scale = scale; io.post_div = post_div;
     if (accumulate) io.flags |= EPI_ACCUM;
     if (tanh) { io.act = ACT_TANH; io.peak_bits = peak_bits; }
@@ -156,15 +156,15 @@ int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, lon
     if (h->c.transposed || h->reflect) { set_error("conv1d_forward_wavegrad: a zero-padded, non-transposed conv only"); return 1; }
     const int Tout = b200tts_conv1d_out_len(h, T);
     ConvIO io;
-    io.x = x; io.x_bs = x_batch_stride; io.x_cs = x_channel_stride; io.Tin = T; io.in_slope = in_slope;
-    io.y = y; io.y_bs = y_batch_stride; io.y_cs = y_channel_stride; io.Tout = Tout; io.B = B;
-    if (y2) { io.y2 = y2; io.y2_bs = y_batch_stride; io.y2_cs = y_channel_stride; }
-    if (residual) { io.res = residual; io.res_bs = res_batch_stride; io.res_cs = res_channel_stride; }
+    io.x = {x, x_batch_stride, x_channel_stride}; io.Tin = T; io.in_slope = in_slope;
+    io.y = {y, y_batch_stride, y_channel_stride}; io.Tout = Tout; io.B = B;
+    if (y2) io.y2 = {y2, y_batch_stride, y_channel_stride};
+    if (residual) io.res = {residual, res_batch_stride, res_channel_stride};
     io.flags = EPI_WAVEGRAD;
     io.near_src = near_src;
     if (lrelu) { io.act = ACT_LRELU; io.act_param = 0.2f; }
     io.act_add = act_add;
-    io.film = film; io.film_bs = film_batch_stride; io.film_cs = film_channel_stride; io.film_half = film_half;
+    io.film = {film, film_batch_stride, film_channel_stride}; io.film_half = film_half;
     return launch_conv(h->L, io, (cudaStream_t)stream);
 }
 
@@ -192,13 +192,13 @@ static_assert(sizeof(b200tts_debug_conv_io) == 216, "tts_b200/_lib.py DebugConvI
 int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, void* stream) {
     if (!h || !d) { set_error("debug_conv1d_launch: null argument"); return 1; }
     ConvIO io;
-    io.x = d->x; io.x_bs = d->x_batch_stride; io.x_cs = d->x_channel_stride; io.Tin = d->T;
-    io.xmask = d->xmask; io.xmask_bs = d->xmask_batch_stride; io.in_slope = d->in_slope;
-    io.cond = d->cond; io.cond_bs = d->cond_batch_stride;
-    io.y = d->y; io.y_bs = d->y_batch_stride; io.y_cs = d->y_channel_stride; io.Tout = b200tts_conv1d_out_len(h, d->T);
-    io.res = d->res; io.res_bs = d->res_batch_stride; io.res_cs = d->res_channel_stride;
-    io.ymask = d->ymask; io.ymask_bs = d->ymask_batch_stride;
-    io.y2 = d->y2; io.y2_bs = d->y2_batch_stride; io.y2_cs = d->y2_channel_stride;
+    io.x = {d->x, d->x_batch_stride, d->x_channel_stride}; io.Tin = d->T;
+    io.xmask = {d->xmask, d->xmask_batch_stride}; io.in_slope = d->in_slope;
+    io.cond = {d->cond, d->cond_batch_stride};
+    io.y = {d->y, d->y_batch_stride, d->y_channel_stride}; io.Tout = b200tts_conv1d_out_len(h, d->T);
+    io.res = {d->res, d->res_batch_stride, d->res_channel_stride};
+    io.ymask = {d->ymask, d->ymask_batch_stride};
+    io.y2 = {d->y2, d->y2_batch_stride, d->y2_channel_stride};
     io.split = d->split; io.scale = d->scale; io.post_div = d->post_div;
     io.act = d->act; io.act_param = d->act_param; io.flags = d->flags; io.B = d->B;
     io.lens = d->lens; io.rate_out = d->rate_out; io.need_out = d->need_out; io.rate_in = d->rate_in; io.need_in = d->need_in;

@@ -159,15 +159,38 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
     DevBuf<float> tc_rscale;  // device, [Rows] 2^-e_r of the split-fp16 images (tc_prec == PREC_F16X3), else empty
 };
 
+// One [B][C][T] operand of a conv launch: element (b, c, t) is at p[b * bs + c * cs + t].  The pointer and its strides
+// are set together (the only constructor that takes a pointer takes both strides), so no launch can give a tensor and
+// forget a stride.  An InView is read and an OutView written; an OutView converts to an InView, not the other way.
+template <class T> struct View {
+    T* p = nullptr; long long bs = 0; int cs = 0;
+    View() = default;
+    View(T* p_, long long bs_, int cs_) : p(p_), bs(bs_), cs(cs_) {}
+    View(const View<float>& v) : p(v.p), bs(v.bs), cs(v.cs) {}   // View<float>: the copy; View<const float>: from one
+    explicit operator bool() const { return p != nullptr; }
+};
+using InView = View<const float>;
+using OutView = View<float>;
+// the common case: a packed [B][C][pitch] tensor
+inline OutView dense(float* p, int C, int pitch) { return {p, (long long)C * pitch, pitch}; }
+inline InView dense(const float* p, int C, int pitch) { return {p, (long long)C * pitch, pitch}; }
+// a per-batch vector, read only: a mask [B, 1, T] or a conditioning bias [B, RowsPad]; element (b, i) is at p[b * bs + i]
+struct VecView {
+    const float* p = nullptr; long long bs = 0;
+    VecView() = default;
+    VecView(const float* p_, long long bs_) : p(p_), bs(bs_) {}
+    explicit operator bool() const { return p != nullptr; }
+};
+
 struct ConvIO {
-    const float* x = nullptr; long long x_bs = 0; int x_cs = 0; int Tin = 0;
-    const float* xmask = nullptr; long long xmask_bs = 0;
+    InView x; int Tin = 0;
+    VecView xmask;
     float in_slope = 1.0f;
-    const float* cond = nullptr; long long cond_bs = 0;   // [B, RowsPad-compatible] per-(b,row) bias
-    float* y = nullptr; long long y_bs = 0; int y_cs = 0; int Tout = 0;
-    const float* res = nullptr; long long res_bs = 0; int res_cs = 0;
-    const float* ymask = nullptr; long long ymask_bs = 0;
-    float* y2 = nullptr; long long y2_bs = 0; int y2_cs = 0;
+    VecView cond;   // [B, RowsPad-compatible] per-(b,row) bias
+    OutView y; int Tout = 0;
+    InView res;
+    VecView ymask;
+    OutView y2;
     int split = 0;
     float scale = 1.0f;
     float post_div = 1.0f;   // applied after accumulation (MRF mean: z_sum / num_kernels)
@@ -200,7 +223,7 @@ struct ConvIO {
     // FiLM (wavegrad.py shif_and_scale): v = shift + scale * v with shift = film[b, c, t] and scale = film[b, film_half + c,
     // t] (the two chunks of a FiLM output_conv tensor); y2 (nullable) receives v before it.  act_add (device [B], nullable):
     // added after the activation (the FiLM noise level).  With EPI_WAVEGRAD, act may be ACT_LRELU.
-    const float* film = nullptr; long long film_bs = 0; int film_cs = 0; int film_half = 0;
+    InView film; int film_half = 0;
     const float* act_add = nullptr;
 };
 
@@ -212,6 +235,16 @@ int pack_conv(ConvLayer& L, const float* w, const float* bias, int Cout, int Cin
 int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin, int Cout, int Kt, int stride,
                         int padding, int output_padding = 0);
 int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t stream);
+// a 1x1 conv of one vector per batch row, [B, L.Cin] -> [B, L.Rows] with output rows y_pitch apart (the speaker and
+// language conditioning projections); accum adds to y instead of overwriting it
+inline int launch_conv_vec(const ConvLayer& L, const float* x, float* y, int y_pitch, int B, bool accum,
+                           cudaStream_t stream) {
+    ConvIO io;
+    io.x = {x, L.Cin, 1}; io.Tin = 1;
+    io.y = {y, y_pitch, 1}; io.Tout = 1; io.B = B;
+    if (accum) io.flags = EPI_ACCUM;
+    return launch_conv(L, io, stream);
+}
 int conv_tc_error_flag();
 // one tensor-core weight image of logical weights Wl(r, ci, k) in the block layout of conv_tc3.cuh (see conv1d.cu);
 // prec PREC_F16X3 also uploads the row scales 2^-e_r into *rscale (when it is still empty)

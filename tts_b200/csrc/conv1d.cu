@@ -1003,15 +1003,15 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     B200_REQUIRE(L.w && io.x && io.y, "launch_conv: null tensor");
     ConvKArgs a;
     memset(&a, 0, sizeof(a));
-    a.x = io.x; a.x_bs = io.x_bs; a.x_cs = io.x_cs; a.Tin = io.Tin;
-    a.xmask = io.xmask; a.xmask_bs = io.xmask_bs; a.in_slope = io.in_slope;
-    a.w = L.w; a.bias = L.bias; a.cond = io.cond; a.cond_bs = io.cond_bs;
+    a.x = io.x.p; a.x_bs = io.x.bs; a.x_cs = io.x.cs; a.Tin = io.Tin;
+    a.xmask = io.xmask.p; a.xmask_bs = io.xmask.bs; a.in_slope = io.in_slope;
+    a.w = L.w; a.bias = L.bias; a.cond = io.cond.p; a.cond_bs = io.cond.bs;
     a.Cin = L.Cin; a.CinPad = L.CinPad; a.K = L.K; a.dil = L.dil; a.pad = L.pad; a.Rows = L.Rows; a.ups = L.ups;
-    a.y = io.y; a.y_bs = io.y_bs; a.y_cs = io.y_cs; a.Tout = io.Tout;
+    a.y = io.y.p; a.y_bs = io.y.bs; a.y_cs = io.y.cs; a.Tout = io.Tout;
     a.Tq = (L.ups > 1) ? (io.Tout + L.ups - 1) / L.ups : io.Tout;
-    a.res = io.res; a.res_bs = io.res_bs; a.res_cs = io.res_cs;
-    a.ymask = io.ymask; a.ymask_bs = io.ymask_bs;
-    a.y2 = io.y2; a.y2_bs = io.y2_bs; a.y2_cs = io.y2_cs; a.split = io.split;
+    a.res = io.res.p; a.res_bs = io.res.bs; a.res_cs = io.res.cs;
+    a.ymask = io.ymask.p; a.ymask_bs = io.ymask.bs;
+    a.y2 = io.y2.p; a.y2_bs = io.y2.bs; a.y2_cs = io.y2.cs; a.split = io.split;
     a.scale = io.scale; a.post_div = io.post_div; a.act = io.act; a.act_param = io.act_param; a.flags = io.flags;
     a.lens = io.lens; a.rate_out = io.rate_out; a.need_out = io.need_out; a.rate_in = io.rate_in; a.need_in = io.need_in;
     a.q_lo = std::max(0, io.q_lo); a.q_hi = io.q_hi; a.in_lo = std::max(0, io.in_lo); a.in_hi = io.in_hi;
@@ -1027,12 +1027,12 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
     if (a.flags & EPI_WAVEGRAD) {   // WaveGrad layers: their own kernel variants (tensor cores, else the FMA tile kernel)
         B200_REQUIRE(L.ups == 1 && !io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && !io.xmask && !io.ymask &&
                          !io.cond && !a.reflect && a.flags == EPI_WAVEGRAD && a.scale == 1.f && a.post_div == 1.f &&
-                         (a.act == ACT_NONE || a.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film_cs > 0)) &&
+                         (a.act == ACT_NONE || a.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film.cs > 0)) &&
                          io.near_src >= 0,
                      "launch_conv: the WaveGrad epilogue takes only lrelu / act_add / res / y2 / film, on a dense launch");
         a.near_src = io.near_src;
         a.near_scale = io.near_src > 0 ? (float)io.near_src / (float)io.Tin : 1.f;
-        a.film = io.film; a.film_bs = io.film_bs; a.film_cs = io.film_cs; a.film_half = io.film_half;
+        a.film = io.film.p; a.film_bs = io.film.bs; a.film_cs = io.film.cs; a.film_half = io.film_half;
         a.act_add = io.act_add;
         if (a.Tq <= 0 || io.B <= 0) return 0;
         if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;

@@ -39,34 +39,28 @@ int WaveNet::init(int hidden, int kernel_size, int dilation_rate, int num_layers
 int WaveNet::forward(float* h, float* out, const float* mask, const float* g, int B, int T, float* acts,
                      float* condv, cudaStream_t st, const int* lens) const {
     int rc;
-    const long long bs = (long long)H * T;
     const bool has_g = cond_ch > 0 && g != nullptr;
-    if (has_g) {
-        ConvIO io;
-        io.x = g; io.x_bs = cond_ch; io.x_cs = 1; io.Tin = 1;
-        io.y = condv; io.y_bs = cond.RowsPad; io.y_cs = 1; io.Tout = 1; io.B = B;
-        if ((rc = launch_conv(cond, io, st))) return rc;
-    }
+    if (has_g && (rc = launch_conv_vec(cond, g, condv, cond.RowsPad, B, false, st))) return rc;
     for (int l = 0; l < L; ++l) {
         {   // acts = tanh(a[:H]) * sigmoid(a[H:]),  a = in_layer(h) + g_l
             ConvIO io;
-            io.x = h; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = acts; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
+            io.x = dense(h, H, T); io.Tin = T;
+            io.y = dense(acts, H, T); io.Tout = T; io.B = B;
             io.flags = EPI_GATE;
             io.lens = lens;      // everything in the WaveNet is re-masked: rows end exactly at their length (need = 0)
-            if (has_g) { io.cond = condv + (size_t)l * 2 * H; io.cond_bs = cond.RowsPad; }
+            if (has_g) io.cond = {condv + (size_t)l * 2 * H, cond.RowsPad};
             if ((rc = launch_conv(in_layers[l], io, st))) return rc;
         }
         ConvIO io;
-        io.x = acts; io.x_bs = bs; io.x_cs = T; io.Tin = T; io.Tout = T; io.B = B;
-        io.ymask = mask; io.ymask_bs = T;
+        io.x = dense(acts, H, T); io.Tin = T; io.Tout = T; io.B = B;
+        io.ymask = {mask, T};
         io.lens = lens;
         if (l < L - 1) {  // h = (h + rs[:H]) * mask ; out (+)= rs[H:]
-            io.y = h; io.y_bs = bs; io.y_cs = T;
-            io.y2 = out; io.y2_bs = bs; io.y2_cs = T; io.split = H;
+            io.y = dense(h, H, T);
+            io.y2 = dense(out, H, T); io.split = H;
             io.flags = EPI_SPLIT | (l > 0 ? EPI_ACCUM2 : 0);
         } else {          // out = (out + rs) * mask
-            io.y = out; io.y_bs = bs; io.y_cs = T;
+            io.y = dense(out, H, T);
             io.flags = EPI_MASK_POST | (l > 0 ? EPI_ACCUM : 0);
         }
         if ((rc = launch_conv(res_skip[l], io, st))) return rc;
@@ -143,18 +137,18 @@ int Flow::reverse(float* z, const float* mask, const float* g, int B, int T, voi
         float* x1 = z + (b.odd ? 0 : (size_t)half * T);
         {   // h = pre(x0) * mask
             ConvIO io;
-            io.x = x0; io.x_bs = zbs; io.x_cs = T; io.Tin = T;
-            io.y = h; io.y_bs = (long long)H * T; io.y_cs = T; io.Tout = T; io.B = B;
-            io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+            io.x = {x0, zbs, T}; io.Tin = T;
+            io.y = dense(h, H, T); io.Tout = T; io.B = B;
+            io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
             io.lens = lens;
             if ((rc = launch_conv(b.pre, io, st))) return rc;
         }
         if ((rc = b.wn.forward(h, out, mask, g, B, T, acts, condv, st, lens))) return rc;
         {   // m = post(out) * mask ; x1 = (x1 - m) * mask     (mean_only: log_scale = 0)
             ConvIO io;
-            io.x = out; io.x_bs = (long long)H * T; io.x_cs = T; io.Tin = T;
-            io.y = x1; io.y_bs = zbs; io.y_cs = T; io.Tout = T; io.B = B;
-            io.ymask = mask; io.ymask_bs = T;
+            io.x = dense(out, H, T); io.Tin = T;
+            io.y = {x1, zbs, T}; io.Tout = T; io.B = B;
+            io.ymask = {mask, T};
             io.scale = fwd ? 1.f : -1.f;   // forward: x1 = m + x1*mask ; reverse: x1 = (x1 - m)*mask
             io.flags = EPI_MASK_PRE | EPI_ACCUM | EPI_MASK_POST;
             io.lens = lens;
@@ -210,17 +204,17 @@ int PosteriorEnc::forward(const float* x, const float* mask, const float* g, con
     int rc;
     {
         ConvIO io;
-        io.x = x; io.x_bs = (long long)c.in_channels * T; io.x_cs = T; io.Tin = T;
-        io.y = h; io.y_bs = (long long)H * T; io.y_cs = T; io.Tout = T; io.B = B;
-        io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+        io.x = dense(x, c.in_channels, T); io.Tin = T;
+        io.y = dense(h, H, T); io.Tout = T; io.B = B;
+        io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(pre, io, st))) return rc;
     }
     if ((rc = wn.forward(h, out, mask, g, B, T, acts, condv, st, nullptr))) return rc;
     {
         ConvIO io;
-        io.x = out; io.x_bs = (long long)H * T; io.x_cs = T; io.Tin = T;
-        io.y = stats; io.y_bs = (long long)2 * c.out_channels * T; io.y_cs = T; io.Tout = T; io.B = B;
-        io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+        io.x = dense(out, H, T); io.Tin = T;
+        io.y = dense(stats, 2 * c.out_channels, T); io.Tout = T; io.B = B;
+        io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(proj, io, st))) return rc;
     }
     dim3 grid((T + 127) / 128, c.out_channels, B);

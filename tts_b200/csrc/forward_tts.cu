@@ -249,50 +249,35 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
     Arena ar(ws, ws_bytes);
     const FttsEncWs w = ftts_encode_carve(*this, ar, B, Tt);
     float *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb, *gp = w.gp;
-    const long long bs = (long long)C * Tt;
     float* x = o_en;
     int rc;
     // x = emb(tokens), no scale (forward_tts.py:405), masked at the row's length
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, C, C, x, x_mask, st, false))) return rc;
+    ConvIO eio;   // what every encoder conv shares: Tt columns in and out
+    eio.Tin = eio.Tout = Tt; eio.B = B;
     for (const Layer& L : enc) {
-        {
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-            io.y = qkv; io.y_bs = 3 * bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L.qkv, io, st))) return rc;
-        }
+        ConvIO io = eio;
+        io.x = dense(x, C, Tt); io.y = dense(qkv, 3 * C, Tt);
+        if ((rc = launch_conv(L.qkv, io, st))) return rc;
         // key_padding_mask = ~x_mask (transformer.py:60-63): masked keys get no weight
         if ((rc = launch_attention(qkv, x_mask, nullptr, nullptr, att, B, C, Tt, c.enc_heads, -1, st))) return rc;
-        {
-            ConvIO io;
-            io.x = att; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-            io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L.o, io, st))) return rc;
-        }
+        io = eio;
+        io.x = dense(att, C, Tt); io.y = dense(yb, C, Tt);
+        if ((rc = launch_conv(L.o, io, st))) return rc;
         if ((rc = launch_add_norm(x, yb, true, L.ln1_g, L.ln1_b, x_mask, x, B, C, Tt, st))) return rc;
-        {
-            ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
-            io.y = hb; io.y_bs = (long long)F * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            io.act = ACT_RELU;
-            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
-        }
-        {
-            ConvIO io;
-            io.x = hb; io.x_bs = (long long)F * Tt; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
-            io.y = yb; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            if ((rc = launch_conv(L.ffn2, io, st))) return rc;
-        }
+        io = eio;
+        io.x = dense(x, C, Tt); io.xmask = {x_mask, Tt}; io.y = dense(hb, F, Tt); io.act = ACT_RELU;
+        if ((rc = launch_conv(L.ffn1, io, st))) return rc;
+        io = eio;
+        io.x = dense(hb, F, Tt); io.xmask = {x_mask, Tt}; io.y = dense(yb, C, Tt);
+        if ((rc = launch_conv(L.ffn2, io, st))) return rc;
         // norm2(x + ffn), masked: Encoder.forward's final o * x_mask (feed_forward/encoder.py:161-162)
         if ((rc = launch_add_norm(x, yb, false, L.ln2_g, L.ln2_b, x_mask, x, B, C, Tt, st))) return rc;
     }
     if (g) {   // o_en + g, g = emb_g(ids) / proj_g(d_vector) / d_vector (forward_tts.py:399-414)
         const float* gv = g;
         if (c.proj_g_in > 0) {
-            ConvIO io;
-            io.x = g; io.x_bs = c.proj_g_in; io.x_cs = 1; io.Tin = 1;
-            io.y = gp; io.y_bs = C; io.y_cs = 1; io.Tout = 1; io.B = B;
-            if ((rc = launch_conv(proj_g, io, st))) return rc;
+            if ((rc = launch_conv_vec(proj_g, g, gp, C, B, false, st))) return rc;
             gv = gp;
         }
         dim3 grid((Tt + 127) / 128, C, B);
@@ -309,10 +294,8 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
     for (int p = 0; p < 2; ++p) {
         if (!preds[p]) continue;
         if ((rc = preds[p]->forward(x, x_mask, nullptr, nullptr, B, Tt, outs[p], w.dp, w.dp_bytes, st))) return rc;
-        ConvIO io;
-        io.x = outs[p]; io.x_bs = Tt; io.x_cs = Tt; io.Tin = Tt;
-        io.y = x; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        io.flags = EPI_ACCUM;
+        ConvIO io = eio;
+        io.x = dense(outs[p], 1, Tt); io.y = dense(x, C, Tt); io.flags = EPI_ACCUM;
         if ((rc = launch_conv(*embs[p], io, st))) return rc;
     }
     return launch_durations_forward(logw, x_mask, length_scale, B, Tt, dur, cum, y_lengths, meta, st);
@@ -344,17 +327,16 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
     // (short batches) computes every column and reads the input through y_mask instead.
     const bool tc = Tp >= 128;
     const bool attn_tc = attention_tc3_takes(C / c.dec_heads);
-    auto io_for = [&](const float* in, int cin, float* out, int cout, bool ragged) {
-        ConvIO io;
-        io.x = in; io.x_bs = (long long)cin * Tp; io.x_cs = Tp; io.Tin = Tp;
-        io.y = out; io.y_bs = (long long)cout * Tp; io.y_cs = Tp; io.Tout = Tp; io.B = B;
-        if (!tc) { io.xmask = ymask; io.xmask_bs = Tp; }
-        else if (ragged) io.lens = lens;
-        return io;
-    };
+    ConvIO dio;   // what every decoder conv shares: Tp columns in and out, ragged rows as above
+    dio.Tin = dio.Tout = Tp; dio.B = B;
+    if (!tc) dio.xmask = {ymask, Tp};
+    else dio.lens = lens;
     for (const Layer& L : dec) {
+        ConvIO io = dio;
+        io.x = dense(x, C, Tp); io.y = dense(qkv, 3 * C, Tp);
         // the FMA attention fallback reads every column of q|k|v, so it gets them computed in full (from zero inputs)
-        if ((rc = launch_conv(L.qkv, io_for(x, C, qkv, 3 * C, attn_tc), st))) return rc;
+        if (!attn_tc) io.lens = nullptr;
+        if ((rc = launch_conv(L.qkv, io, st))) return rc;
         if (attn_tc) {
             if ((rc = launch_attention_tc3(qkv, (long long)3 * C * Tp, Tp, lens, att, (long long)C * Tp, B, C,
                                            c.dec_heads, Ty, st)))
@@ -363,17 +345,21 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
             if ((rc = launch_attention(qkv, ymask, nullptr, nullptr, att, B, C, Tp, c.dec_heads, -1, st))) return rc;
             dispatch_note(DISPATCH_ATTN_FMA);
         }
-        if ((rc = launch_conv(L.o, io_for(att, C, yb, C, true), st))) return rc;
+        io = dio;
+        io.x = dense(att, C, Tp); io.y = dense(yb, C, Tp);
+        if ((rc = launch_conv(L.o, io, st))) return rc;
         if ((rc = launch_add_norm(x, yb, true, L.ln1_g, L.ln1_b, ymask, x, B, C, Tp, st))) return rc;
-        {
-            ConvIO io = io_for(x, C, hb, F, true);
-            io.act = ACT_RELU;
-            if ((rc = launch_conv(L.ffn1, io, st))) return rc;
-        }
-        if ((rc = launch_conv(L.ffn2, io_for(hb, F, yb, C, true), st))) return rc;
+        io = dio;
+        io.x = dense(x, C, Tp); io.y = dense(hb, F, Tp); io.act = ACT_RELU;
+        if ((rc = launch_conv(L.ffn1, io, st))) return rc;
+        io = dio;
+        io.x = dense(hb, F, Tp); io.y = dense(yb, C, Tp);
+        if ((rc = launch_conv(L.ffn2, io, st))) return rc;
         if ((rc = launch_add_norm(x, yb, false, L.ln2_g, L.ln2_b, ymask, x, B, C, Tp, st))) return rc;
     }
-    if ((rc = launch_conv(postnet, io_for(x, C, pm, Co, true), st))) return rc;
+    ConvIO io = dio;
+    io.x = dense(x, C, Tp); io.y = dense(pm, Co, Tp);
+    if ((rc = launch_conv(postnet, io, st))) return rc;
     dim3 grid((unsigned)(((long long)Ty * Co + 255) / 256), B);
     mel_out_kernel<<<grid, 256, 0, st>>>(pm, y_lengths, mel, Co, Ty, Tp);
     count_launch();

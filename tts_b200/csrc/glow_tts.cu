@@ -153,23 +153,22 @@ int GlowDecoder::reverse(float* z, const float* msk, const float* g, int B, int 
     B200_REQUIRE(ar.ok(), "glow decoder: workspace of %zu bytes is too small", ws_bytes);
     float *zb = w.zb, *eo = w.eo, *h = w.h, *acts = w.acts, *out = w.out, *condv = w.condv;
     int rc;
-    const long long zbs = (long long)Cs * Tq, hbs = (long long)Hd * Tq;
     float* cur = z;
     float* nxt = zb;
     for (int n = (int)blocks.size() - 1; n >= 0; --n) {   // reversed(flows): coupling, InvConvNear, ActNorm per block
         const Block& bl = blocks[n];
-        {   // h = start(x0) * mask
+        {   // h = start(x0) * mask, x0 = the first half of cur's channels
             ConvIO io;
-            io.x = cur; io.x_bs = zbs; io.x_cs = Tq; io.Tin = Tq;
-            io.y = h; io.y_bs = hbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
-            io.ymask = msk; io.ymask_bs = Tq; io.flags = EPI_MASK_POST;
+            io.x = dense(cur, Cs, Tq); io.Tin = Tq;
+            io.y = dense(h, Hd, Tq); io.Tout = Tq; io.B = B;
+            io.ymask = {msk, Tq}; io.flags = EPI_MASK_POST;
             if ((rc = launch_conv(bl.start, io, st))) return rc;
         }
         if ((rc = bl.wn.forward(h, out, msk, g, B, Tq, acts, condv, st))) return rc;
         {   // [t | s] = end(WN(h))
             ConvIO io;
-            io.x = out; io.x_bs = hbs; io.x_cs = Tq; io.Tin = Tq;
-            io.y = eo; io.y_bs = zbs; io.y_cs = Tq; io.Tout = Tq; io.B = B;
+            io.x = dense(out, Hd, Tq); io.Tin = Tq;
+            io.y = dense(eo, Cs, Tq); io.Tout = Tq; io.B = B;
             if ((rc = launch_conv(bl.end, io, st))) return rc;
         }
         dim3 grid((Tq + 127) / 128, Cs / ns, B);
@@ -281,7 +280,6 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
     Arena ar(ws, ws_bytes);
     const GlowEncWs w = glow_encode_carve(*this, ar, B, Tt);
     float *x = w.x, *xdp = w.xdp;
-    const long long bs = (long long)H * Tt;
     int rc;
     // x = emb(tokens) * sqrt(H), masked: the prenet and the transformer both start with x * x_mask
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, H, H, x, x_mask, st))) return rc;
@@ -290,27 +288,27 @@ int GlowTTS::encode(const long long* tokens, const long long* lengths, const flo
         for (int l = 0; l < 3; ++l) {
             float* out = w.pre[l & 1];
             ConvIO io;
-            io.x = in; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt;
+            io.x = dense(in, H, Tt); io.Tin = Tt; io.xmask = {x_mask, Tt};
             if (l > 0) io.in_slope = 0.f;   // the previous layer's ReLU, applied to its masked output
-            io.y = out; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-            io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
+            io.y = dense(out, H, Tt); io.Tout = Tt; io.B = B;
+            io.ymask = {x_mask, Tt}; io.flags = EPI_MASK_POST;
             if ((rc = launch_conv(prenet[l].conv, io, st))) return rc;
             if ((rc = launch_add_layernorm(out, nullptr, prenet[l].g, prenet[l].b, nullptr, out, B, H, Tt, 1e-4f, st)))
                 return rc;
             in = out;
         }
         ConvIO io;
-        io.x = in; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt; io.xmask = x_mask; io.xmask_bs = Tt; io.in_slope = 0.f;
-        io.y = x; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_ACCUM | EPI_MASK_POST;
+        io.x = dense(in, H, Tt); io.Tin = Tt; io.xmask = {x_mask, Tt}; io.in_slope = 0.f;
+        io.y = dense(x, H, Tt); io.Tout = Tt; io.B = B;
+        io.ymask = {x_mask, Tt}; io.flags = EPI_ACCUM | EPI_MASK_POST;
         if ((rc = launch_conv(prenet_proj, io, st))) return rc;
     }
     if ((rc = tf.forward(x, x_mask, B, Tt, w.tf, w.tf_bytes, st))) return rc;
     {   // o_mean = proj_m(x) * mask, o_log_scale = proj_s(x) * mask (encoder.py:172-176)
         ConvIO io;
-        io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-        io.y = o_stats; io.y_bs = (long long)2 * c.out_channels * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        io.ymask = x_mask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
+        io.x = dense(x, H, Tt); io.Tin = Tt;
+        io.y = dense(o_stats, 2 * c.out_channels, Tt); io.Tout = Tt; io.B = B;
+        io.ymask = {x_mask, Tt}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(proj, io, st))) return rc;
     }
     const float* dp_in = x;

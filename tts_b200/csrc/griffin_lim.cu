@@ -327,8 +327,8 @@ int GriffinLim::forward(const float* x, long long x_bs, int x_cs, int x_ts, int 
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
         ConvIO io;
-        io.x = amp; io.x_bs = (long long)n_mels * T; io.x_cs = T; io.Tin = T;
-        io.y = lin; io.y_bs = (long long)F * T; io.y_cs = T; io.Tout = T; io.B = B;
+        io.x = dense(amp, n_mels, T); io.Tin = T;
+        io.y = dense(lin, F, T); io.Tout = T; io.B = B;
         if (int rc = launch_conv(pinv, io, st)) return rc;
         dispatch_note(DISPATCH_GL_PREPARE);
         gl_prepare_kernel<<<dim3((T + 31) / 32, (F + 31) / 32, B), tblk, 0, st>>>(

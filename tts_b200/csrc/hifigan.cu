@@ -212,17 +212,13 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
     }
     int rc;
     const bool has_cond = c.cond_channels > 0 && g != nullptr;
-    if (has_cond) {  // cond_layer(g): [B, cond, 1] -> [B, C0]
-        ConvIO io;
-        io.x = g; io.x_bs = c.cond_channels; io.x_cs = 1; io.Tin = 1;
-        io.y = condv; io.y_bs = cond.RowsPad; io.y_cs = 1; io.Tout = 1; io.B = B;
-        if ((rc = launch_conv(cond, io, st))) return rc;
-    }
+    // cond_layer(g): [B, cond, 1] -> [B, C0]
+    if (has_cond && (rc = launch_conv_vec(cond, g, condv, cond.RowsPad, B, false, st))) return rc;
     {  // conv_pre (+ cond broadcast over T)
         ConvIO io;
-        io.x = xin0; io.x_bs = (long long)c.in_channels * x_pitch; io.x_cs = x_pitch; io.Tin = T;
-        io.y = P; io.y_bs = (long long)C0 * Tp; io.y_cs = Tp; io.Tout = T; io.B = B;
-        if (has_cond) { io.cond = condv; io.cond_bs = cond.RowsPad; }
+        io.x = dense(xin0, c.in_channels, x_pitch); io.Tin = T;
+        io.y = dense(P, C0, Tp); io.Tout = T; io.B = B;
+        if (has_cond) io.cond = {condv, cond.RowsPad};
         io.lens = lens; io.rate_out = 1; io.need_out = need_P; io.rate_in = 1; io.need_in = T;   // z is defined everywhere
         window(io);
         if ((rc = launch_conv(conv_pre, io, st))) return rc;
@@ -232,11 +228,10 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
     const bool type1 = c.resblock_type == 1;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int Cs = C[s], Ls = L[s];
-        const long long bs = (long long)Cs * Ls;
         {  // o = ups(leaky_relu(o, 0.1))
             ConvIO io;
-            io.x = cur; io.x_bs = (long long)curC * curPitch; io.x_cs = curPitch; io.Tin = curL; io.in_slope = 0.1f;
-            io.y = U; io.y_bs = bs; io.y_cs = Ls; io.Tout = Ls; io.B = B;
+            io.x = dense(cur, curC, curPitch); io.Tin = curL; io.in_slope = 0.1f;
+            io.y = dense(U, Cs, Ls); io.Tout = Ls; io.B = B;
             io.lens = lens; io.rate_in = (s == 0) ? 1 : rate[s - 1]; io.need_in = (s == 0) ? need_P : need_OUT[s - 1];
             io.rate_out = io.rate_in; io.need_out = need_q_ups[s];      // tiles run over GEMM columns = input steps
             window(io);
@@ -254,8 +249,8 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
                 const ConvLayer* lastconv = &c1[n];
                 if (type1) {  // T1 = c1(lrelu(xin))
                     ConvIO io;
-                    io.x = xin; io.x_bs = bs; io.x_cs = Ls; io.Tin = Ls; io.in_slope = 0.1f;
-                    io.y = T1; io.y_bs = bs; io.y_cs = Ls; io.Tout = Ls; io.B = B;
+                    io.x = dense(xin, Cs, Ls); io.Tin = Ls; io.in_slope = 0.1f;
+                    io.y = dense(T1, Cs, Ls); io.Tout = Ls; io.B = B;
                     io.lens = lens; io.rate_in = io.rate_out = rate[s];
                     io.need_in = need_xin; io.need_out = need_T1[s * c.num_kernels + j][n];
                     window(io);
@@ -264,9 +259,9 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
                     lastconv = &c2[n];
                 }
                 ConvIO io;  // xnew = conv(lrelu(convin)) + xin ; MRF: OUT (+)= xnew, mean on the last resblock
-                io.x = convin; io.x_bs = bs; io.x_cs = Ls; io.Tin = Ls; io.in_slope = 0.1f;
-                io.res = xin; io.res_bs = bs; io.res_cs = Ls;
-                io.B = B; io.Tout = Ls; io.y_bs = bs; io.y_cs = Ls;
+                io.x = dense(convin, Cs, Ls); io.Tin = Ls; io.in_slope = 0.1f;
+                io.res = dense(xin, Cs, Ls);
+                io.B = B; io.Tout = Ls;
                 float* dst;
                 if (last) {
                     dst = OUT;
@@ -275,7 +270,7 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
                 } else {
                     dst = type1 ? R : pp[n & 1];
                 }
-                io.y = dst;
+                io.y = dense(dst, Cs, Ls);
                 io.lens = lens; io.rate_in = io.rate_out = rate[s];
                 io.need_in = type1 ? need_T1[s * c.num_kernels + j][n] : need_xin;
                 io.need_out = need_X[s * c.num_kernels + j][n];
@@ -294,8 +289,8 @@ int Hifigan::forward(const float* x, const float* g, int B, int T, float* wav, v
     }
     {  // tanh(conv_post(leaky_relu(o)))  -- default slope 0.01 (hifigan_generator.py:262)
         ConvIO io;
-        io.x = cur; io.x_bs = (long long)curC * curPitch; io.x_cs = curPitch; io.Tin = curL; io.in_slope = 0.01f;
-        io.y = wav; io.y_bs = (long long)c.out_channels * curL; io.y_cs = curL; io.Tout = curL; io.B = B;
+        io.x = dense(cur, curC, curPitch); io.Tin = curL; io.in_slope = 0.01f;
+        io.y = dense(wav, c.out_channels, curL); io.Tout = curL; io.B = B;
         io.act = ACT_TANH;
         io.peak_bits = peak_bits;
         io.lens = lens; io.rate_in = io.rate_out = rate.empty() ? 1 : rate.back(); io.need_in = need_OUT.empty() ? 0 : need_OUT.back();

@@ -216,8 +216,8 @@ int Melgan::forward(const float* x, int B, int T, int synthesize, float* out, un
     int rc;
     {   // conv_pre(reflect_pad(x))   (melgan_generator.py:32-35)
         ConvIO io;
-        io.x = xin; io.x_bs = (long long)c.in_channels * x_pitch; io.x_cs = x_pitch; io.Tin = T;
-        io.y = P; io.y_bs = (long long)C0 * Tp; io.y_cs = Tp; io.Tout = T; io.B = B;
+        io.x = dense(xin, c.in_channels, x_pitch); io.Tin = T;
+        io.y = dense(P, C0, Tp); io.Tout = T; io.B = B;
         io.reflect = 1;
         if ((rc = launch_conv(conv_pre, io, st))) return rc;
     }
@@ -225,24 +225,23 @@ int Melgan::forward(const float* x, int B, int T, int synthesize, float* out, un
     int curC = C0, curL = T, curP = Tp;
     for (int s = 0; s < c.num_upsamples; ++s) {
         const int Cs = C[s], Ls = L[s], Lp = round4(Ls);
-        const long long bs = (long long)Cs * Lp;
         float* xa = (cur == X) ? Y : X;    // never the buffer the upsampler reads
         float* ya = (xa == X) ? Y : X;
         {   // x = ups(lrelu(x, 0.2))   (:44-57)
             ConvIO io;
-            io.x = cur; io.x_bs = (long long)curC * curP; io.x_cs = curP; io.Tin = curL; io.in_slope = 0.2f;
-            io.y = xa; io.y_bs = bs; io.y_cs = Lp; io.Tout = Ls; io.B = B;
+            io.x = dense(cur, curC, curP); io.Tin = curL; io.in_slope = 0.2f;
+            io.y = dense(xa, Cs, Lp); io.Tout = Ls; io.B = B;
             if ((rc = launch_conv(ups[s], io, st))) return rc;
         }
         for (const Block& bl : blocks[s]) {   // x = shortcut(x) + block(x)   (melgan.py:33-36)
             ConvIO io;
-            io.x = xa; io.x_bs = bs; io.x_cs = Lp; io.Tin = Ls; io.in_slope = 0.2f;
-            io.y = H; io.y_bs = bs; io.y_cs = Lp; io.Tout = Ls; io.B = B;
+            io.x = dense(xa, Cs, Lp); io.Tin = Ls; io.in_slope = 0.2f;
+            io.y = dense(H, Cs, Lp); io.Tout = Ls; io.B = B;
             io.reflect = 1;
             if ((rc = launch_conv(bl.dil, io, st))) return rc;
-            io.in_slope = 1.f; io.reflect = 0; io.y = ya;
+            io.in_slope = 1.f; io.reflect = 0; io.y = dense(ya, Cs, Lp);
             if ((rc = launch_conv(bl.shortcut, io, st))) return rc;
-            io.x = H; io.in_slope = 0.2f; io.flags = EPI_ACCUM;
+            io.x = dense(H, Cs, Lp); io.in_slope = 0.2f; io.flags = EPI_ACCUM;
             if ((rc = launch_conv(bl.c1x1, io, st))) return rc;
             std::swap(xa, ya);
         }
@@ -250,8 +249,8 @@ int Melgan::forward(const float* x, int B, int T, int synthesize, float* out, un
     }
     {   // tanh(conv_post(reflect_pad(lrelu(x, 0.2))))   (:62-70); the band signals go to H when they are synthesised
         ConvIO io;
-        io.x = cur; io.x_bs = (long long)curC * curP; io.x_cs = curP; io.Tin = curL; io.in_slope = 0.2f;
-        io.y = synthesize ? H : out; io.y_bs = (long long)c.out_channels * curL; io.y_cs = curL; io.Tout = curL; io.B = B;
+        io.x = dense(cur, curC, curP); io.Tin = curL; io.in_slope = 0.2f;
+        io.y = dense(synthesize ? H : out, c.out_channels, curL); io.Tout = curL; io.B = B;
         io.act = ACT_TANH;
         io.reflect = 1;
         io.peak_bits = synthesize ? nullptr : peak_bits;

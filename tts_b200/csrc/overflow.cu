@@ -235,8 +235,8 @@ int Overflow::encode(const long long* tokens, const long long* lengths, int B, i
     if ((rc = launch_transpose(states, encT, B, N, E, st))) return rc;
     {   // hoisted: zc[b, r, n] = W_z[r] . state[b, n] + b_0[r] for every state n
         ConvIO io;
-        io.x = encT; io.x_bs = (long long)E * N; io.x_cs = N; io.Tin = N;
-        io.y = p.zc; io.y_bs = (long long)O1 * N; io.y_cs = N; io.Tout = N; io.B = B;
+        io.x = dense(encT, E, N); io.Tin = N;
+        io.y = dense(p.zc, O1, N); io.Tout = N; io.B = B;
         if ((rc = launch_conv(zproj, io, st))) return rc;
     }
     return 0;

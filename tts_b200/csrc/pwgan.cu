@@ -654,7 +654,6 @@ int Pwgan::forward(const float* mel, const float* noise, int B, int T, int pad, 
     int num_sms = 0;
     if (int rc = layer_device(&err, &num_sms)) return rc;
     const int L = c.num_res_blocks, Ts = Tf * P, pitch = round4(Ts);
-    const long long bs = (long long)RES * pitch;
     if (int rc = launch_aux(mel, B, T, pad, 0, L, A, st)) return rc;
     {
         const long long n = (long long)B * Ts;
@@ -671,10 +670,10 @@ int Pwgan::forward(const float* mel, const float* noise, int B, int T, int pad, 
     }
     float* H = X0;          // x is no longer needed
     ConvIO io;
-    io.x = S; io.x_bs = bs; io.x_cs = pitch; io.Tin = Ts; io.in_slope = 0.f;   // ReLU as the prologue
-    io.y = H; io.y_bs = bs; io.y_cs = pitch; io.Tout = Ts; io.B = B;
+    io.x = dense(S, RES, pitch); io.Tin = Ts; io.in_slope = 0.f;   // ReLU as the prologue
+    io.y = dense(H, RES, pitch); io.Tout = Ts; io.B = B;
     if (int rc = launch_conv(tail1, io, st)) return rc;
-    io.x = H; io.y = out; io.y_bs = Ts; io.y_cs = Ts;
+    io.x = dense(H, RES, pitch); io.y = dense(out, 1, Ts);
     return launch_conv(tail2, io, st);
 }
 

@@ -502,19 +502,18 @@ int SeqEncoder::encode(const long long* tokens, const long long* lengths, int B,
     int rc;
     // emb(x) without a scale, zero past each row's length (the reference runs each row at its own length)
     if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, E, E, x, xmask, st, false))) return rc;
-    const long long bs = (long long)E * Tt;
     for (int l = 0; l < n_convs; ++l) {   // conv -> BN (folded) -> ReLU -> Dropout (eval: identity), masked
         ConvIO io;
-        io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-        io.y = y; io.y_bs = bs; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        io.act = ACT_RELU; io.ymask = xmask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
+        io.x = dense(x, E, Tt); io.Tin = Tt;
+        io.y = dense(y, E, Tt); io.Tout = Tt; io.B = B;
+        io.act = ACT_RELU; io.ymask = {xmask, Tt}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(convs[l], io, st))) return rc;
         std::swap(x, y);
     }
     {   // pre[b, d*4H + row, t] = W_ih x + b_ih + b_hh, both directions
         ConvIO io;
-        io.x = x; io.x_bs = bs; io.x_cs = Tt; io.Tin = Tt;
-        io.y = pre; io.y_bs = (long long)8 * H * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
+        io.x = dense(x, E, Tt); io.Tin = Tt;
+        io.y = dense(pre, 8 * H, Tt); io.Tout = Tt; io.B = B;
         if ((rc = launch_conv(lstm_in, io, st))) return rc;
     }
     B200_CUDA_OK(cudaMemsetAsync(hb, 0, sizeof(float) * 2 * B * H, st));

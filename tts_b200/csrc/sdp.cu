@@ -292,41 +292,24 @@ int DurPred::forward(const float* x, const float* mask, const float* g, const fl
     const float* cur = x;
     const bool has_g = c.cond_channels > 0 && g, has_l = c.language_emb_dim > 0 && lang_emb;
     if (has_g || has_l) {       // x = x + cond(g) (+ cond_lang(lang_emb)) : per-utterance channel bias on the INPUT
-        bool first = true;
-        if (has_g) {
-            ConvIO io;
-            io.x = g; io.x_bs = c.cond_channels; io.x_cs = 1; io.Tin = 1;
-            io.y = cv; io.y_bs = cpad; io.y_cs = 1; io.Tout = 1; io.B = B;
-            if ((rc = launch_conv(cond, io, st))) return rc;
-            first = false;
-        }
-        if (has_l) {
-            ConvIO io;
-            io.x = lang_emb; io.x_bs = c.language_emb_dim; io.x_cs = 1; io.Tin = 1;
-            io.y = cv; io.y_bs = cpad; io.y_cs = 1; io.Tout = 1; io.B = B;
-            if (!first) io.flags = EPI_ACCUM;
-            if ((rc = launch_conv(cond_lang, io, st))) return rc;
-        }
+        if (has_g && (rc = launch_conv_vec(cond, g, cv, cpad, B, false, st))) return rc;
+        if (has_l && (rc = launch_conv_vec(cond_lang, lang_emb, cv, cpad, B, has_g, st))) return rc;
         dim3 grid((T + 127) / 128, Cin, B);
         add_chan_bias_kernel<<<grid, 128, 0, st>>>(x, cv, cpad, xin, Cin, T);
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
         cur = xin;
     }
-    auto conv_relu = [&](const ConvLayer& L, const float* in, int cin, float* out) {
-        ConvIO io;
-        io.x = in; io.x_bs = (long long)cin * T; io.x_cs = T; io.Tin = T; io.xmask = mask; io.xmask_bs = T;
-        io.y = out; io.y_bs = (long long)F * T; io.y_cs = T; io.Tout = T; io.B = B; io.act = ACT_RELU;
-        return launch_conv(L, io, st);
-    };
-    if ((rc = conv_relu(conv1, cur, Cin, h1))) return rc;
+    ConvIO io;   // conv1 and conv2 (ReLU, then LayerNorm), then proj: all read their input through the mask
+    io.Tin = io.Tout = T; io.B = B; io.xmask = {mask, T}; io.act = ACT_RELU;
+    io.x = dense(cur, Cin, T); io.y = dense(h1, F, T);
+    if ((rc = launch_conv(conv1, io, st))) return rc;
     if ((rc = launch_add_layernorm(h1, nullptr, g1, b1, nullptr, h1, B, F, T, 1e-4f, st))) return rc;
-    if ((rc = conv_relu(conv2, h1, F, h2))) return rc;
+    io.x = dense(h1, F, T); io.y = dense(h2, F, T);
+    if ((rc = launch_conv(conv2, io, st))) return rc;
     if ((rc = launch_add_layernorm(h2, nullptr, g2, b2, nullptr, h2, B, F, T, 1e-4f, st))) return rc;
-    ConvIO io;
-    io.x = h2; io.x_bs = (long long)F * T; io.x_cs = T; io.Tin = T; io.xmask = mask; io.xmask_bs = T;
-    io.y = logw; io.y_bs = T; io.y_cs = T; io.Tout = T; io.B = B;
-    io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+    io.x = dense(h2, F, T); io.y = dense(logw, 1, T); io.act = ACT_NONE;
+    io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
     return launch_conv(proj, io, st);
 }
 
@@ -359,8 +342,8 @@ int DDSConv::forward(float* x, const float* mask, int B, int T, float* y1, float
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
         ConvIO io;
-        io.x = y1; io.x_bs = (long long)C * T; io.x_cs = T; io.Tin = T;
-        io.y = y2; io.y_bs = (long long)C * T; io.y_cs = T; io.Tout = T; io.B = B;
+        io.x = dense(y1, C, T); io.Tin = T;
+        io.y = dense(y2, C, T); io.Tout = T; io.B = B;
         if ((rc = launch_conv(conv1x1[l], io, st))) return rc;
         dds_ln_gelu_res_kernel<<<grid, 256, 0, st>>>(x, y2, g2[l], b2[l], mask, C, T, l == L - 1 ? 1 : 0);
         count_launch();
@@ -436,41 +419,28 @@ int SDP::reverse(const float* x, const float* mask, const float* noise, const fl
     const SdpWs w = sdp_carve(*this, ar, B, T);
     float *xc = w.xc, *h = w.h, *y1 = w.y1, *y2 = w.y2, *z = w.z, *hp = w.hp, *condv = w.condv;
     float* cv = nullptr;
-    const long long bs = (long long)H * T;
     int rc;
     const bool has_g = c.cond_channels > 0 && g != nullptr;
     const bool has_l = c.language_emb_dim > 0 && lang_emb != nullptr;
+    const int cpad = has_g ? cond.RowsPad : cond_lang.RowsPad;
     if (has_g || has_l) {   // per-utterance bias: cond(g) (+ cond_lang(lang_emb)) -> [B, H]
         cv = condv;
-        bool first = true;
-        if (has_g) {
-            ConvIO io;
-            io.x = g; io.x_bs = c.cond_channels; io.x_cs = 1; io.Tin = 1;
-            io.y = cv; io.y_bs = cond.RowsPad; io.y_cs = 1; io.Tout = 1; io.B = B;
-            if ((rc = launch_conv(cond, io, st))) return rc;
-            first = false;
-        }
-        if (has_l) {
-            ConvIO io;
-            io.x = lang_emb; io.x_bs = c.language_emb_dim; io.x_cs = 1; io.Tin = 1;
-            io.y = cv; io.y_bs = (has_g ? cond.RowsPad : cond_lang.RowsPad); io.y_cs = 1; io.Tout = 1; io.B = B;
-            if (!first) io.flags = EPI_ACCUM;
-            if ((rc = launch_conv(cond_lang, io, st))) return rc;
-        }
+        if (has_g && (rc = launch_conv_vec(cond, g, cv, cpad, B, false, st))) return rc;
+        if (has_l && (rc = launch_conv_vec(cond_lang, lang_emb, cv, cpad, B, has_g, st))) return rc;
     }
     {   // xc = pre(x) + cond
         ConvIO io;
-        io.x = x; io.x_bs = (long long)pre.Cin * T; io.x_cs = T; io.Tin = T;
-        io.y = xc; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-        if (cv) { io.cond = cv; io.cond_bs = has_g ? cond.RowsPad : cond_lang.RowsPad; }
+        io.x = dense(x, pre.Cin, T); io.Tin = T;
+        io.y = dense(xc, H, T); io.Tout = T; io.B = B;
+        if (cv) io.cond = {cv, cpad};
         if ((rc = launch_conv(pre, io, st))) return rc;
     }
     if ((rc = convs.forward(xc, mask, B, T, y1, y2, st))) return rc;
     {   // xc = proj(xc) * mask     (into h, then swap roles)
         ConvIO io;
-        io.x = xc; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-        io.y = h; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-        io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+        io.x = dense(xc, H, T); io.Tin = T;
+        io.y = dense(h, H, T); io.Tout = T; io.B = B;
+        io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(proj, io, st))) return rc;
         float* tmp = xc; xc = h; h = tmp;
     }
@@ -505,9 +475,9 @@ int SDP::reverse(const float* x, const float* mask, const float* noise, const fl
         if ((rc = F.convs.forward(h, mask, B, T, y1, y2, st))) return rc;
         {
             ConvIO io;
-            io.x = h; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = hp; io.y_bs = (long long)nproj * T; io.y_cs = T; io.Tout = T; io.B = B;
-            io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+            io.x = dense(h, H, T); io.Tin = T;
+            io.y = dense(hp, nproj, T); io.Tout = T; io.B = B;
+            io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
             if ((rc = launch_conv(F.proj, io, st))) return rc;
         }
         {

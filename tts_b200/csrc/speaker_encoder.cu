@@ -533,8 +533,8 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
         const int H = g.H[1], C = g.C[1], L = g.L[1];
         if ((rc = zero_rows(A, H, (size_t)C * L, st)) || (rc = zero_rows(T1b, H, (size_t)C * L, st))) return rc;
         ConvIO io;
-        io.x = W.x0; io.x_bs = L; io.x_cs = L; io.Tin = L;
-        io.y = A + (size_t)C * L; io.y_bs = (long long)C * L; io.y_cs = L; io.Tout = L; io.B = H;
+        io.x = dense(W.x0, 1, L); io.Tin = L;
+        io.y = dense(A + (size_t)C * L, C, L); io.Tout = L; io.B = H;
         if ((rc = launch_conv(conv1, io, st))) return rc;
         relu_affine_kernel<<<grid_for((long long)H * C * L), NT, 0, st>>>(A, H, C, L, g.P[1], g.T[1], B, s0, t0);
         count_launch();
@@ -551,19 +551,19 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
             ConvIO io;
             if (b.down) {   // from the polyphase output of the previous stage: rows 2h .. 2h+2, K = 2
                 const size_t prow = (size_t)2 * b.Cin * L;
-                io.x = X; io.x_bs = (long long)(2 * prow); io.x_cs = L; io.Tin = L;
+                io.x = {X, (long long)(2 * prow), L}; io.Tin = L;
             } else {
-                io.x = A; io.x_bs = (long long)row; io.x_cs = L; io.Tin = L;
+                io.x = dense(A, C, L); io.Tin = L;
             }
-            io.y = T1b + row; io.y_bs = (long long)row; io.y_cs = L; io.Tout = L; io.B = H;
+            io.y = dense(T1b + row, C, L); io.Tout = L; io.B = H;
             if ((rc = launch_conv(b.c1, io, st))) return rc;
             relu_affine_kernel<<<grid_for((long long)H * row), NT, 0, st>>>(T1b, H, C, L, P, Ts, B, b.s1, b.t1);
             count_launch();
             B200_CUDA_OK(cudaGetLastError());
             // conv2 + bn2
             ConvIO io2;
-            io2.x = T1b; io2.x_bs = (long long)row; io2.x_cs = L; io2.Tin = L;
-            io2.y = T2b + row; io2.y_bs = (long long)row; io2.y_cs = L; io2.Tout = L; io2.B = H;
+            io2.x = dense(T1b, C, L); io2.Tin = L;
+            io2.y = dense(T2b + row, C, L); io2.Tout = L; io2.B = H;
             if ((rc = launch_conv(b.c2, io2, st))) return rc;
             // SE
             se_partial_kernel<<<H * C, NT, 0, st>>>(T2b, C, L, P, Ts, B, W.part);
@@ -575,8 +575,8 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
             if (b.down) {
                 const size_t prow = (size_t)2 * b.Cin * L;
                 ConvIO iod;
-                iod.x = X + prow; iod.x_bs = (long long)(2 * prow); iod.x_cs = L; iod.Tin = L;
-                iod.y = A + row; iod.y_bs = (long long)row; iod.y_cs = L; iod.Tout = L; iod.B = H;
+                iod.x = {X + prow, (long long)(2 * prow), L}; iod.Tin = L;
+                iod.y = dense(A + row, C, L); iod.Tout = L; iod.B = H;
                 if ((rc = launch_conv(b.ds, iod, st))) return rc;
             }
             // relu(se(y) + residual): in place into A, or polyphase into X at the end of stages 1..3
@@ -599,12 +599,12 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
     B200_REQUIRE(Hf == c.input_dim / 8, "speaker_encoder: input_dim=%d does not reduce to %d rows", c.input_dim, c.input_dim / 8);
     {
         ConvIO io;
-        io.x = A + (size_t)C4 * L4; io.x_bs = 0; io.x_cs = L4; io.Tin = L4;
-        io.y = W.atth; io.y_bs = 0; io.y_cs = L4; io.Tout = L4; io.B = 1; io.act = ACT_RELU;
+        io.x = {A + (size_t)C4 * L4, 0, L4}; io.Tin = L4;
+        io.y = {W.atth, 0, L4}; io.Tout = L4; io.B = 1; io.act = ACT_RELU;
         if ((rc = launch_conv(att1, io, st))) return rc;
         ConvIO io2;
-        io2.x = W.atth; io2.x_bs = 0; io2.x_cs = L4; io2.Tin = L4;
-        io2.y = W.logits; io2.y_bs = 0; io2.y_cs = L4; io2.Tout = L4; io2.B = 1;
+        io2.x = {W.atth, 0, L4}; io2.Tin = L4;
+        io2.y = {W.logits, 0, L4}; io2.Tout = L4; io2.B = 1;
         if ((rc = launch_conv(att2, io2, st))) return rc;
     }
     attn_pool_kernel<<<dim3(Ca, (B + NT / 32 - 1) / (NT / 32)), NT, 0, st>>>(W.logits, A + (size_t)C4 * L4, Hf, C4, L4, g.P[4],
@@ -613,8 +613,8 @@ int SpeakerEncoder::run(const float* x, const int* starts, int B, int T, int gro
     B200_CUDA_OK(cudaGetLastError());
     {
         ConvIO io;
-        io.x = W.pooled; io.x_bs = 0; io.x_cs = W.Bp; io.Tin = B;
-        io.y = W.fco; io.y_bs = 0; io.y_cs = W.Bp; io.Tout = B; io.B = 1;
+        io.x = {W.pooled, 0, W.Bp}; io.Tin = B;
+        io.y = {W.fco, 0, W.Bp}; io.Tout = B; io.B = 1;
         if ((rc = launch_conv(fc, io, st))) return rc;
     }
     const int nw = B / groups;

@@ -107,8 +107,8 @@ int Stft::mel_project(const float* spec, int B, int n_frames, float log_clamp, f
     B200_REQUIRE(mel.w, "mel_project: handle was created without a mel basis");
     const int F = n_fft / 2 + 1;
     ConvIO io;
-    io.x = spec; io.x_bs = (long long)F * n_frames; io.x_cs = n_frames; io.Tin = n_frames;
-    io.y = out; io.y_bs = (long long)n_mels * n_frames; io.y_cs = n_frames; io.Tout = n_frames; io.B = B;
+    io.x = dense(spec, F, n_frames); io.Tin = n_frames;
+    io.y = dense(out, n_mels, n_frames); io.Tout = n_frames; io.B = B;
     if (log_clamp > 0.f) { io.act = ACT_LOGCLAMP; io.act_param = log_clamp; }
     return launch_conv(mel, io, st);
 }

@@ -275,8 +275,8 @@ int TacoAttention::keys(const float* enc, float* encT, float* pin, int B, int Tt
     int rc;
     if ((rc = launch_transpose(enc, encT, B, Tt, E, st))) return rc;
     ConvIO io;
-    io.x = encT; io.x_bs = (long long)E * Tt; io.x_cs = Tt; io.Tin = Tt;
-    io.y = pin; io.y_bs = (long long)A * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
+    io.x = dense(encT, E, Tt); io.Tin = Tt;
+    io.y = dense(pin, A, Tt); io.Tout = Tt; io.B = B;
     return launch_conv(inproj, io, st);
 }
 

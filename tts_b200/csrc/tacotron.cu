@@ -257,10 +257,10 @@ int Tacotron::Cbhg::run(const float* x, const float* mask, const int* lens32, co
     int rc;
     auto conv = [&](const ConvLayer& L, const float* in, int ci, float* o, int co, int act, const float* res) {
         ConvIO io;
-        io.x = in; io.x_bs = (long long)ci * T; io.x_cs = T; io.Tin = T;
-        io.y = o; io.y_bs = (long long)co * T; io.y_cs = T; io.Tout = T; io.B = B;
-        io.act = act; io.ymask = mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
-        if (res) { io.res = res; io.res_bs = (long long)co * T; io.res_cs = T; }
+        io.x = dense(in, ci, T); io.Tin = T;
+        io.y = dense(o, co, T); io.Tout = T; io.B = B;
+        io.act = act; io.ymask = {mask, T}; io.flags = EPI_MASK_POST;
+        if (res) io.res = dense(res, co, T);
         return launch_conv(L, io, st);
     };
     if ((rc = conv(bank, x, Cin, bk, K * BANK, ACT_RELU, nullptr))) return rc;
@@ -285,8 +285,8 @@ int Tacotron::Cbhg::run(const float* x, const float* mask, const int* lens32, co
     }
     {
         ConvIO io;
-        io.x = hx; io.x_bs = (long long)HW * T; io.x_cs = T; io.Tin = T;
-        io.y = pre; io.y_bs = (long long)6 * GRU_H * T; io.y_cs = T; io.Tout = T; io.B = B;
+        io.x = dense(hx, HW, T); io.Tin = T;
+        io.y = dense(pre, 6 * GRU_H, T); io.Tout = T; io.B = B;
         if ((rc = launch_conv(gru_in, io, st))) return rc;
     }
     BiGruArgs g;
@@ -398,9 +398,9 @@ int Tacotron::encode(const long long* tokens, const long long* lengths, int B, i
         const int ci = l ? PN0 : EMB, co = l ? PN1 : PN0;
         float* o = l ? xin : x1;
         ConvIO io;
-        io.x = in; io.x_bs = (long long)ci * Tt; io.x_cs = Tt; io.Tin = Tt;
-        io.y = o; io.y_bs = (long long)co * Tt; io.y_cs = Tt; io.Tout = Tt; io.B = B;
-        io.act = ACT_RELU; io.ymask = mask; io.ymask_bs = Tt; io.flags = EPI_MASK_POST;
+        io.x = dense(in, ci, Tt); io.Tin = Tt;
+        io.y = dense(o, co, Tt); io.Tout = Tt; io.B = B;
+        io.act = ACT_RELU; io.ymask = {mask, Tt}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(eprenet[l], io, st))) return rc;
         in = o;
     }
@@ -519,9 +519,9 @@ int Tacotron::postnet(const float* dec_out, const int* frames, int B, int F, int
     if ((rc = pcbhg.run(x, mask, frames, nullptr, B, Tp, g, (long long)2 * GRU_H * Tp, 1, Tp, w.cbhg, st))) return rc;
     {
         ConvIO io;
-        io.x = g; io.x_bs = (long long)2 * GRU_H * Tp; io.x_cs = Tp; io.Tin = Tp;
-        io.y = y; io.y_bs = (long long)O * Tp; io.y_cs = Tp; io.Tout = Tp; io.B = B;
-        io.ymask = mask; io.ymask_bs = Tp; io.flags = EPI_MASK_POST;
+        io.x = dense(g, 2 * GRU_H, Tp); io.Tin = Tp;
+        io.y = dense(y, O, Tp); io.Tout = Tp; io.B = B;
+        io.ymask = {mask, Tp}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(last, io, st))) return rc;
     }
     return launch_frames_out(y, Tp, out, B, F, O, st);

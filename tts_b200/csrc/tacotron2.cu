@@ -261,13 +261,13 @@ int Tacotron2::postnet(const float* dec_out, const int* frames, int B, int F, in
         const int ci = l ? 512 : C, co = l == 4 ? C : 512;
         float* out = l == 4 ? y : (l & 1 ? h2 : h1);
         ConvIO io;
-        io.x = in; io.x_bs = (long long)ci * Tp; io.x_cs = Tp; io.Tin = Tp;
-        io.y = out; io.y_bs = (long long)co * Tp; io.y_cs = Tp; io.Tout = Tp; io.B = B;
-        if (l) { io.xmask = mask; io.xmask_bs = Tp; }
+        io.x = dense(in, ci, Tp); io.Tin = Tp;
+        io.y = dense(out, co, Tp); io.Tout = Tp; io.B = B;
+        if (l) io.xmask = {mask, Tp};
         io.act = l == 4 ? ACT_NONE : ACT_TANH;
         if (l == 4) {
-            io.res = x; io.res_bs = (long long)C * Tp; io.res_cs = Tp;
-            io.ymask = mask; io.ymask_bs = Tp; io.flags = EPI_MASK_POST;
+            io.res = dense(x, C, Tp);
+            io.ymask = {mask, Tp}; io.flags = EPI_MASK_POST;
         }
         if ((rc = launch_conv(post[l], io, st))) return rc;
         in = out;

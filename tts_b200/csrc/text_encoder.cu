@@ -329,35 +329,34 @@ int RelPosTransformer::forward(float* x, const float* x_mask, int B, int T, void
     const RelPosWs w = relpos_carve(*this, ar, B, T);
     B200_REQUIRE(ar.ok(), "rel_pos_transformer: workspace of %zu bytes is too small", ws_bytes);
     float *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb;
-    const long long bs = (long long)C * T;
     int rc;
     for (const Layer& L : layers) {
         {   // q,k,v = conv_{q,k,v}(x)       (x is already masked: the caller / previous norm2 epilogue)
             ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = qkv; io.y_bs = 3 * bs; io.y_cs = T; io.Tout = T; io.B = B;
+            io.x = dense(x, C, T); io.Tin = T;
+            io.y = dense(qkv, 3 * C, T); io.Tout = T; io.B = B;
             if ((rc = launch_conv(L.qkv, io, st))) return rc;
         }
         if ((rc = launch_attention(qkv, x_mask, L.rel_k, L.rel_v, att, B, C, T, heads, window, st))) return rc;
         {   // y = conv_o(att)
             ConvIO io;
-            io.x = att; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
+            io.x = dense(att, C, T); io.Tin = T;
+            io.y = dense(yb, C, T); io.Tout = T; io.B = B;
             if ((rc = launch_conv(L.o, io, st))) return rc;
         }
         if ((rc = launch_add_layernorm(x, yb, L.ln1_g, L.ln1_b, nullptr, x, B, C, T, eps, st))) return rc;
         {   // h = relu(conv_1(pad(x * mask)))
             ConvIO io;
-            io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
-            io.y = hb; io.y_bs = (long long)F * T; io.y_cs = T; io.Tout = T; io.B = B;
+            io.x = dense(x, C, T); io.Tin = T; io.xmask = {x_mask, T};
+            io.y = dense(hb, F, T); io.Tout = T; io.B = B;
             io.act = ACT_RELU;
             if ((rc = launch_conv(L.ffn1, io, st))) return rc;
         }
         {   // y = conv_2(pad(h * mask)) * mask
             ConvIO io;
-            io.x = hb; io.x_bs = (long long)F * T; io.x_cs = T; io.Tin = T; io.xmask = x_mask; io.xmask_bs = T;
-            io.y = yb; io.y_bs = bs; io.y_cs = T; io.Tout = T; io.B = B;
-            io.ymask = x_mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+            io.x = dense(hb, F, T); io.Tin = T; io.xmask = {x_mask, T};
+            io.y = dense(yb, C, T); io.Tout = T; io.B = B;
+            io.ymask = {x_mask, T}; io.flags = EPI_MASK_POST;
             if ((rc = launch_conv(L.ffn2, io, st))) return rc;
         }
         // x = norm2(x + y); the next layer and the stack's output (transformer.py:419, :431) use x * mask -> fold the
@@ -397,15 +396,14 @@ int TextEncoder::forward(const long long* tokens, const long long* lengths, cons
     const size_t need = workspace_bytes(B, T);
     B200_REQUIRE(ws_bytes >= need, "text_encoder_forward: workspace of %zu bytes, %zu needed", ws_bytes, need);
     if (B == 0 || T == 0) return 0;
-    const long long bs = (long long)C * T;
     int rc;
     if ((rc = launch_embed(tokens, lengths, emb, lang_emb, B, T, c.hidden_channels, C, x, x_mask, st))) return rc;
     if ((rc = tf.forward(x, x_mask, B, T, ws, ws_bytes, st))) return rc;
     {   // stats = proj(x) * mask  -> [m_p | logs_p]
         ConvIO io;
-        io.x = x; io.x_bs = bs; io.x_cs = T; io.Tin = T;
-        io.y = stats; io.y_bs = (long long)2 * c.out_channels * T; io.y_cs = T; io.Tout = T; io.B = B;
-        io.ymask = x_mask; io.ymask_bs = T; io.flags = EPI_MASK_POST;
+        io.x = dense(x, C, T); io.Tin = T;
+        io.y = dense(stats, 2 * c.out_channels, T); io.Tout = T; io.B = B;
+        io.ymask = {x_mask, T}; io.flags = EPI_MASK_POST;
         if ((rc = launch_conv(proj, io, st))) return rc;
     }
     return 0;

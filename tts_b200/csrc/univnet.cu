@@ -424,19 +424,18 @@ int Univnet::launch_predict(int blk, const float* mel, int B, int T, float* P, f
     const int Ch = c.kpnet_hidden_channels, Tp = round4(T);
     const long long hbs = (long long)Ch * Tp;
     ConvIO io;
-    io.x = mel; io.x_bs = (long long)c.cond_channels * T; io.x_cs = T; io.Tin = T;
-    io.y = H0; io.y_bs = hbs; io.y_cs = Tp; io.Tout = T; io.B = B;
+    io.x = dense(mel, c.cond_channels, T); io.Tin = T;
+    io.y = dense(H0, Ch, Tp); io.Tout = T; io.B = B;
     io.flags = EPI_WAVEGRAD; io.act = ACT_LRELU; io.act_param = 0.1f;   // input_conv + LeakyReLU(0.1)
     if (int rc = launch_conv(bl.kin, io, st)) return rc;
-    io.x_bs = hbs; io.x_cs = Tp;
     const float* in = H0;
     float* outs[2] = {H1, H2};
     for (int k = 0; k < 6; ++k) {   // residual_conv; the last conv's epilogue adds the block input: H = H0 + r
-        io.x = in;
-        io.y = outs[k & 1];
-        if (k == 5) { io.res = H0; io.res_bs = hbs; io.res_cs = Tp; }
+        io.x = dense(in, Ch, Tp);
+        io.y = dense(outs[k & 1], Ch, Tp);
+        if (k == 5) io.res = dense(H0, Ch, Tp);
         if (int rc = launch_conv(bl.kres[k], io, st)) return rc;
-        in = io.y;
+        in = outs[k & 1];
     }
     const long long N = (long long)B * T;
     const dim3 grid((unsigned)((N + uv::PT_N - 1) / uv::PT_N), (unsigned)((MP + uv::PT_M - 1) / uv::PT_M));
@@ -486,8 +485,8 @@ int Univnet::forward(const float* mel, const float* noise, int B, int T, float* 
     int rc;
     {   // first_conv(noise)
         ConvIO io;
-        io.x = noise; io.x_bs = (long long)c.in_channels * T; io.x_cs = T; io.Tin = T;
-        io.y = X0; io.y_bs = (long long)C * Tp; io.y_cs = Tp; io.Tout = T; io.B = B;
+        io.x = dense(noise, c.in_channels, T); io.Tin = T;
+        io.y = dense(X0, C, Tp); io.Tout = T; io.B = B;
         if ((rc = launch_conv(first, io, st))) return rc;
     }
     float *x = X0, *xo = X1;
@@ -498,8 +497,8 @@ int Univnet::forward(const float* mel, const float* noise, int B, int T, float* 
         const int Ls = T * bl.hop, Lp = round4(Ls);
         {   // x = upsample(lrelu(x, 0.2))
             ConvIO io;
-            io.x = x; io.x_bs = (long long)C * pitch; io.x_cs = pitch; io.Tin = len; io.in_slope = 0.2f;
-            io.y = xo; io.y_bs = (long long)C * Lp; io.y_cs = Lp; io.Tout = Ls; io.B = B;
+            io.x = dense(x, C, pitch); io.Tin = len; io.in_slope = 0.2f;
+            io.y = dense(xo, C, Lp); io.Tout = Ls; io.B = B;
             if ((rc = launch_conv(bl.up, io, st))) return rc;
         }
         std::swap(x, xo);
@@ -510,8 +509,8 @@ int Univnet::forward(const float* mel, const float* noise, int B, int T, float* 
         }
     }
     ConvIO io;   // tanh(last_conv(lrelu(x, 0.1)))
-    io.x = x; io.x_bs = (long long)C * pitch; io.x_cs = pitch; io.Tin = len; io.in_slope = 0.1f;
-    io.y = out; io.y_bs = (long long)c.out_channels * len; io.y_cs = len; io.Tout = len; io.B = B;
+    io.x = dense(x, C, pitch); io.Tin = len; io.in_slope = 0.1f;
+    io.y = dense(out, c.out_channels, len); io.Tout = len; io.B = B;
     io.act = ACT_TANH;
     return launch_conv(last, io, st);
 }

@@ -185,13 +185,6 @@ float* wg_pick(const WgBufs& o, const float* a, const float* b = nullptr, const 
         if (p != a && p != b && p != c && p != d) return p;
     return nullptr;
 }
-// ConvIO of a dense [B, C, pitch] -> [B, Co, pitch'] launch
-ConvIO wg_io(const float* x, int Cin, int xp, int Tin, float* y, int Cout, int yp, int Tout, int B) {
-    ConvIO io;
-    io.x = x; io.x_bs = (long long)Cin * xp; io.x_cs = xp; io.Tin = Tin;
-    io.y = y; io.y_bs = (long long)Cout * yp; io.y_cs = yp; io.Tout = Tout; io.B = B;
-    return io;
-}
 }  // namespace
 
 size_t Wavegrad::workspace_bytes(int B, int T) const {
@@ -205,7 +198,9 @@ int Wavegrad::condition(const float* x, int B, int T, void* ws, size_t ws_bytes,
     B200_REQUIRE(ws && ws_bytes >= need, "wavegrad: workspace of %zu bytes, %zu needed", ws_bytes, need);
     Arena ar(ws, ws_bytes);
     const WgBufs o = wg_carve(*this, ar, B, T);
-    ConvIO io = wg_io(x, c.in_channels, T, T, o.xc, c.x_conv_channels, round4(T), T, B);   // x_conv (wavegrad.py:115)
+    ConvIO io;   // x_conv (wavegrad.py:115)
+    io.x = dense(x, c.in_channels, T); io.Tin = T;
+    io.y = dense(o.xc, c.x_conv_channels, round4(T)); io.Tout = T; io.B = B;
     return launch_conv(x_conv, io, st);
 }
 
@@ -229,18 +224,22 @@ int Wavegrad::network(const float* y, const float* noise_level, const float* con
     float* cur = o.P[0];
     int curC = c.y_conv_channels;
     {   // y_conv(y): y is the caller's dense [B, 1, L0]
-        ConvIO io = wg_io(y, 1, L[0], L[0], cur, curC, round4(L[0]), L[0], B);
+        ConvIO io;
+        io.x = dense(y, 1, L[0]); io.Tin = L[0];
+        io.y = dense(cur, curC, round4(L[0])); io.Tout = L[0]; io.B = B;
         if ((rc = launch_conv(y_conv, io, st))) return rc;
     }
     for (int i = 0; i < n; ++i) {
         const int Li = L[i], Lp = round4(Li), oc = c.ublock_out_channels[n - 1 - i];
         {   // FiLM i (layers/wavegrad.py:50-54)
             float* h = wg_pick(o, cur);
-            ConvIO io = wg_io(cur, curC, Lp, Li, h, curC, Lp, Li, B);
+            ConvIO io;
+            io.x = dense(cur, curC, Lp); io.y = dense(h, curC, Lp); io.Tin = io.Tout = Li; io.B = B;
             io.flags = EPI_WAVEGRAD; io.act = ACT_LRELU; io.act_param = WG_SLOPE; io.act_add = noise_level;
-            io.res = pe[i]; io.res_bs = 0; io.res_cs = Lpe[i];                 // PositionalEncoding: + pe[:, :T] / 5000
+            io.res = {pe[i], 0, Lpe[i]};                          // PositionalEncoding: + pe[:, :T] / 5000
             if ((rc = launch_conv(film[i].in, io, st))) return rc;
-            io = wg_io(h, curC, Lp, Li, o.F[i], 2 * oc, Lp, Li, B);
+            io = ConvIO();
+            io.x = dense(h, curC, Lp); io.y = dense(o.F[i], 2 * oc, Lp); io.Tin = io.Tout = Li; io.B = B;
             if ((rc = launch_conv(film[i].out, io, st))) return rc;
         }
         if (i + 1 == n) break;
@@ -250,15 +249,17 @@ int Wavegrad::network(const float* y, const float* noise_level, const float* con
         float* A = wg_pick(o, cur, R);
         float* Bb = wg_pick(o, cur, R, A);
         float* D = wg_pick(o, cur, R, A, Bb);
-        ConvIO io = wg_io(cur, curC, Lp, Ld, R, dc, Ldp, Ld, B);
+        ConvIO io;
+        io.x = dense(cur, curC, Lp); io.y = dense(R, dc, Ldp); io.Tin = io.Tout = Ld; io.B = B;
         io.near_src = Li;                                                       // x[..., ::f]
         if ((rc = launch_conv(d.res, io, st))) return rc;
-        io.y = A; io.in_slope = WG_SLOPE;
+        io.y = dense(A, dc, Ldp); io.in_slope = WG_SLOPE;
         if ((rc = launch_conv(d.m0, io, st))) return rc;
-        io = wg_io(A, dc, Ldp, Ld, Bb, dc, Ldp, Ld, B);
+        io = ConvIO();
+        io.x = dense(A, dc, Ldp); io.y = dense(Bb, dc, Ldp); io.Tin = io.Tout = Ld; io.B = B;
         io.in_slope = WG_SLOPE;
         if ((rc = launch_conv(d.m1, io, st))) return rc;
-        io.x = Bb; io.y = D; io.res = R; io.res_bs = (long long)dc * Ldp; io.res_cs = Ldp;   // o + res
+        io.x = dense(Bb, dc, Ldp); io.y = dense(D, dc, Ldp); io.res = dense(R, dc, Ldp);   // o + res
         if ((rc = launch_conv(d.m2, io, st))) return rc;
         cur = D;
         curC = dc;
@@ -269,27 +270,30 @@ int Wavegrad::network(const float* y, const float* noise_level, const float* con
     for (int u = 0; u < n; ++u) {
         const UBlock& b = ub[u];   // layers/wavegrad.py:90-104
         const int k = n - 1 - u, Lu = L[k], Lup = round4(Lu), hc = c.ublock_out_channels[u];
-        const long long bs = (long long)hc * Lup;
         float* R = wg_pick(o, xu);
         float* O = wg_pick(o, xu, R);
         float* H = wg_pick(o, xu, R, O);
-        ConvIO io = wg_io(xu, xC, round4(xL), Lu, R, hc, Lup, Lu, B);
+        const InView film_k = dense(o.F[k], 2 * hc, Lup);                     // [shift | scale] of FiLM k
+        ConvIO io;
+        io.x = dense(xu, xC, round4(xL)); io.y = dense(R, hc, Lup); io.Tin = io.Tout = Lu; io.B = B;
         io.near_src = xL;                                                       // x_inter
         if ((rc = launch_conv(b.res, io, st))) return rc;
-        io.y = O; io.in_slope = WG_SLOPE;
-        io.flags = EPI_WAVEGRAD; io.film = o.F[k]; io.film_bs = 2 * bs; io.film_cs = Lup; io.film_half = hc;
+        io.y = dense(O, hc, Lup); io.in_slope = WG_SLOPE;
+        io.flags = EPI_WAVEGRAD; io.film = film_k; io.film_half = hc;
         if ((rc = launch_conv(b.m0, io, st))) return rc;
-        ConvIO f = wg_io(O, hc, Lup, Lu, H, hc, Lup, Lu, B);
+        ConvIO f;
+        f.x = dense(O, hc, Lup); f.y = dense(H, hc, Lup); f.Tin = f.Tout = Lu; f.B = B;
         f.in_slope = WG_SLOPE;
-        f.flags = EPI_WAVEGRAD; f.film = o.F[k]; f.film_bs = 2 * bs; f.film_cs = Lup; f.film_half = hc;
-        f.res = R; f.res_bs = bs; f.res_cs = Lup;                               // res2 = res + main1(...)
-        f.y2 = R; f.y2_bs = bs; f.y2_cs = Lup;
+        f.flags = EPI_WAVEGRAD; f.film = film_k; f.film_half = hc;
+        f.res = dense(R, hc, Lup);                                              // res2 = res + main1(...)
+        f.y2 = dense(R, hc, Lup);
         if ((rc = launch_conv(b.m1, f, st))) return rc;
-        f.x = H; f.y = O; f.res = nullptr; f.y2 = nullptr;
+        f.x = dense(H, hc, Lup); f.y = dense(O, hc, Lup); f.res = InView(); f.y2 = OutView();
         if ((rc = launch_conv(b.o0, f, st))) return rc;
-        ConvIO p = wg_io(O, hc, Lup, Lu, H, hc, Lup, Lu, B);
+        ConvIO p;
+        p.x = dense(O, hc, Lup); p.y = dense(H, hc, Lup); p.Tin = p.Tout = Lu; p.B = B;
         p.in_slope = WG_SLOPE;
-        p.res = R; p.res_bs = bs; p.res_cs = Lup;                               // out_block[1](...) + res2
+        p.res = dense(R, hc, Lup);                                              // out_block[1](...) + res2
         if ((rc = launch_conv(b.o1, p, st))) return rc;
         xu = H; xC = hc; xL = Lu;
     }
