@@ -8,6 +8,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace b200tts {
@@ -162,12 +163,20 @@ struct ConvLayer {            // immutable after pack(); owned by an engine hand
 // One [B][C][T] operand of a conv launch: element (b, c, t) is at p[b * bs + c * cs + t].  The pointer and its strides
 // are set together (the only constructor that takes a pointer takes both strides), so no launch can give a tensor and
 // forget a stride.  An InView is read and an OutView written; an OutView converts to an InView, not the other way.
+// Views are trivially copyable: the kernels take them as arguments, inside the launch's ConvIO.
 template <class T> struct View {
     T* p = nullptr; long long bs = 0; int cs = 0;
     View() = default;
     View(T* p_, long long bs_, int cs_) : p(p_), bs(bs_), cs(cs_) {}
-    View(const View<float>& v) : p(v.p), bs(v.bs), cs(v.cs) {}   // View<float>: the copy; View<const float>: from one
-    explicit operator bool() const { return p != nullptr; }
+    template <class U, std::enable_if_t<std::is_same_v<T, const U> && !std::is_const_v<U>, int> = 0>
+    View(const View<U>& v) : p(v.p), bs(v.bs), cs(v.cs) {}   // InView from an OutView
+    __host__ __device__ explicit operator bool() const { return p != nullptr; }
+    // row c of batch b (element t of it is row(b, c)[t])
+    __host__ __device__ T* row(int b, int c) const { return p + (long long)b * bs + (long long)c * cs; }
+    // every row starts on a 16-byte boundary (whole float4 accesses along T)
+    __host__ __device__ bool aligned16() const {
+        return (cs & 3) == 0 && (bs & 3) == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+    }
 };
 using InView = View<const float>;
 using OutView = View<float>;
@@ -179,8 +188,11 @@ struct VecView {
     const float* p = nullptr; long long bs = 0;
     VecView() = default;
     VecView(const float* p_, long long bs_) : p(p_), bs(bs_) {}
-    explicit operator bool() const { return p != nullptr; }
+    __host__ __device__ explicit operator bool() const { return p != nullptr; }
+    __host__ __device__ const float* row(int b) const { return p + (long long)b * bs; }
 };
+static_assert(std::is_trivially_copyable_v<InView> && std::is_trivially_copyable_v<OutView> &&
+              std::is_trivially_copyable_v<VecView>, "views are kernel arguments");
 
 struct ConvIO {
     InView x; int Tin = 0;

@@ -68,26 +68,6 @@ __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-struct ConvKArgs {
-    const float* x; long long x_bs; int x_cs; int Tin;
-    const float* xmask; long long xmask_bs; float in_slope;
-    const float* w; const float* bias; const float* cond; long long cond_bs;
-    int Cin, CinPad, K, dil, pad, Rows, ups, Tq;
-    float* y; long long y_bs; int y_cs; int Tout;
-    const float* res; long long res_bs; int res_cs;
-    const float* ymask; long long ymask_bs;
-    float* y2; long long y2_bs; int y2_cs; int split;
-    float scale; float post_div; int act; float act_param; int flags;
-    int XS;
-    const int* lens; int rate_out, need_out, rate_in, need_in;
-    int q_lo, q_hi, in_lo, in_hi;   // column window (ConvIO), q_lo / in_lo >= 0
-    int reflect;                    // reflection padding (ConvIO::reflect)
-    // WaveGrad (KEPI_WAVEGRAD only, see ConvIO): nearest-resampled input, FiLM, pre-FiLM store, per-batch add
-    int near_src; float near_scale;
-    const float* film; long long film_bs; int film_cs, film_half;
-    const float* act_add;
-};
-
 enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3, KEPI_WAVEGRAD = 4 };
 
 // CJ rows x TJ time steps per lane, WCO x WT warps, CIC input channels per stage, EPI epilogue family.
@@ -112,13 +92,13 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     };
     const int b = blockIdx.z, tile_co = blockIdx.y;
     const int q0 = blockIdx.x * T_T;
-    if (q0 >= a.q_hi || q0 + T_T <= a.q_lo) return;     // tile outside the column window: nothing to produce
+    if (q0 >= a.io.q_hi || q0 + T_T <= a.io.q_lo) return;     // tile outside the column window: nothing to produce
     const int tin0 = q0 - a.pad;
-    const float* xb = a.x + b * a.x_bs;
-    const float* mb = a.xmask ? a.xmask + b * a.xmask_bs : nullptr;
+    const float* xb = a.io.x.p + b * a.io.x.bs;
+    const float* mb = a.io.xmask ? a.io.xmask.row(b) : nullptr;
     const float* wg = a.w + (size_t)tile_co * a.CinPad * a.K * CO_T;
     const int nchunks = (a.Cin + CIC - 1) / CIC;   // CinPad is a multiple of CI_MAX >= CIC; skip all-zero chunks
-    const float slope = a.in_slope;
+    const float slope = a.io.in_slope;
 
     auto load_chunk = [&](int chunk, int buf) {
         const float* src = wg + (size_t)chunk * wchunk;
@@ -129,13 +109,13 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         const int c0 = chunk * CIC;
         for (int i = tid; i < XS; i += NT) {
             int t = tin0 + i;
-            if (a.reflect) t = t < 0 ? -t : (t >= a.Tin ? 2 * a.Tin - 2 - t : t);   // mirrored; columns past the reach stay out
-            const bool tok = (t >= a.in_lo) && (t < a.Tin);   // below in_lo: stale scratch of a windowed producer
+            if (a.io.reflect) t = t < 0 ? -t : (t >= a.io.Tin ? 2 * a.io.Tin - 2 - t : t);   // mirrored; columns past the reach stay out
+            const bool tok = (t >= a.io.in_lo) && (t < a.io.Tin);   // below in_lo: stale scratch of a windowed producer
             float m = 1.f;
             if (tok && mb) m = __ldg(mb + t);
             int ts = t;                                        // source column
             if constexpr (EPI == KEPI_WAVEGRAD) {
-                if (a.near_src && tok) ts = tc3::near_col(t, a.near_src, a.Tin, a.near_scale);
+                if (a.io.near_src && tok) ts = tc3::near_col(t, a.io.near_src, a.io.Tin, a.near_scale);
             }
 #pragma unroll
             for (int h = 0; h < CIC; h += 8) {
@@ -143,7 +123,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
 #pragma unroll
                 for (int ci = 0; ci < 8; ++ci) {
                     v[ci] = 0.f;
-                    if (tok && (c0 + h + ci) < a.Cin) v[ci] = __ldg(xb + (long long)(c0 + h + ci) * a.x_cs + ts);
+                    if (tok && (c0 + h + ci) < a.Cin) v[ci] = __ldg(xb + (long long)(c0 + h + ci) * a.io.x.cs + ts);
                 }
 #pragma unroll
                 for (int ci = 0; ci < 8; ++ci) {
@@ -227,7 +207,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     // ---------------------------------------------------------------- epilogue
     const int row_base = tile_co * CO_T + wco * CJ;
     const int qb = q0 + wt * 32 * TJ + lane;
-    auto inw = [&](int q) { return q < a.Tout && q >= a.q_lo && q < a.q_hi; };   // stored columns: the window only
+    auto inw = [&](int q) { return q < a.io.Tout && q >= a.io.q_lo && q < a.io.q_hi; };   // stored columns: the window only
     if (EPI == KEPI_GATE) {
         // rows (2p, 2p+1) = (tanh half, sigmoid half) of output row row_base/2 + p   (wavenet.py:6-13)
 #pragma unroll
@@ -235,8 +215,8 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
             const int r0 = row_base + 2 * p;
             if (r0 + 1 < a.Rows) {
                 float b0 = a.bias[r0], b1 = a.bias[r0 + 1];
-                if (a.cond) { b0 += __ldg(a.cond + b * a.cond_bs + r0); b1 += __ldg(a.cond + b * a.cond_bs + r0 + 1); }
-                float* yrow = a.y + b * a.y_bs + (long long)(r0 >> 1) * a.y_cs;
+                if (a.io.cond) { b0 += __ldg(a.io.cond.row(b) + r0); b1 += __ldg(a.io.cond.row(b) + r0 + 1); }
+                float* yrow = a.io.y.row(b, r0 >> 1);
 #pragma unroll
                 for (int j = 0; j < TJ; ++j) {
                     const int q = qb + 32 * j;
@@ -257,7 +237,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                 const int r = row_base + 2 * p + h;
                 if (r < a.Rows) {
                     const float bb = a.bias[r];
-                    float* yrow = a.y + b * a.y_bs + (long long)r * a.y_cs;
+                    float* yrow = a.io.y.row(b, r);
 #pragma unroll
                     for (int j = 0; j < TJ; ++j) {
                         const int q = qb + 32 * j;
@@ -273,8 +253,8 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     if (EPI == KEPI_WAVEGRAD) {
         // v = acc + bias; [lrelu]; [+ act_add[b]]; [+ res]; [y2 <- v]; [v = shift + scale * v]; y <- v, each operation
         // rounded on its own (the reference's order); res / y2 may alias element for element (load before store)
-        const bool lrelu = a.act == ACT_LRELU;
-        const float add = a.act_add ? __ldg(a.act_add + b) : 0.f;
+        const bool lrelu = a.io.act == ACT_LRELU;
+        const float add = a.io.act_add ? __ldg(a.io.act_add + b) : 0.f;
 #pragma unroll
         for (int p = 0; p < CJ / 2; ++p) {
 #pragma unroll
@@ -282,11 +262,10 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                 const int r = row_base + 2 * p + h;
                 if (r >= a.Rows) continue;
                 const float bb = a.bias[r];
-                const long long rr = r;
-                float* yrow = a.y + b * a.y_bs + rr * a.y_cs;
-                float* y2row = a.y2 ? a.y2 + b * a.y2_bs + rr * a.y2_cs : nullptr;
-                const float* rrow = a.res ? a.res + b * a.res_bs + rr * a.res_cs : nullptr;
-                const float* srow = a.film ? a.film + b * a.film_bs + rr * a.film_cs : nullptr;
+                float* yrow = a.io.y.row(b, r);
+                float* y2row = a.io.y2 ? a.io.y2.row(b, r) : nullptr;
+                const float* rrow = a.io.res ? a.io.res.row(b, r) : nullptr;
+                const float* srow = a.io.film ? a.io.film.row(b, r) : nullptr;
 #pragma unroll
                 for (int j = 0; j < TJ; ++j) {
                     const int q = qb + 32 * j;
@@ -294,11 +273,11 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                     float v0, v1;
                     unpack2(acc[p][j], v0, v1);
                     float u = __fadd_rn(h ? v1 : v0, bb);
-                    if (lrelu) u = u > 0.f ? u : __fmul_rn(u, a.act_param);
-                    if (a.act_add) u = __fadd_rn(u, add);
+                    if (lrelu) u = u > 0.f ? u : __fmul_rn(u, a.io.act_param);
+                    if (a.io.act_add) u = __fadd_rn(u, add);
                     if (rrow) u = __fadd_rn(u, rrow[q]);
                     if (y2row) y2row[q] = u;
-                    if (srow) u = __fadd_rn(srow[q], __fmul_rn(srow[(long long)a.film_half * a.film_cs + q], u));
+                    if (srow) u = __fadd_rn(srow[q], __fmul_rn(srow[(long long)a.io.film_half * a.io.film.cs + q], u));
                     yrow[q] = u;
                 }
             }
@@ -306,22 +285,22 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         return;
     }
     if (EPI == KEPI_PLAIN) {   // y = act(acc + bias + cond) [* mask]   -- no residual / accumulate / upsampling
-        const bool relu_p = a.act == ACT_RELU;
-        const bool logc_p = a.act == ACT_LOGCLAMP;
+        const bool relu_p = a.io.act == ACT_RELU;
+        const bool logc_p = a.io.act == ACT_LOGCLAMP;
         float mkp[TJ];
 #pragma unroll
         for (int j = 0; j < TJ; ++j) {
             const int q = qb + 32 * j;
-            mkp[j] = (a.ymask && q < a.Tout) ? __ldg(a.ymask + b * a.ymask_bs + q) : 1.f;
+            mkp[j] = (a.io.ymask && q < a.io.Tout) ? __ldg(a.io.ymask.row(b) + q) : 1.f;
         }
 #pragma unroll
         for (int p = 0; p < CJ / 2; ++p) {
             const int r0 = row_base + 2 * p;
             float b0 = 0.f, b1 = 0.f;
-            if (r0 < a.Rows) { b0 = a.bias[r0]; if (a.cond) b0 += __ldg(a.cond + b * a.cond_bs + r0); }
-            if (r0 + 1 < a.Rows) { b1 = a.bias[r0 + 1]; if (a.cond) b1 += __ldg(a.cond + b * a.cond_bs + r0 + 1); }
-            float* y0 = a.y + b * a.y_bs + (long long)r0 * a.y_cs;
-            float* y1 = y0 + a.y_cs;
+            if (r0 < a.Rows) { b0 = a.bias[r0]; if (a.io.cond) b0 += __ldg(a.io.cond.row(b) + r0); }
+            if (r0 + 1 < a.Rows) { b1 = a.bias[r0 + 1]; if (a.io.cond) b1 += __ldg(a.io.cond.row(b) + r0 + 1); }
+            float* y0 = a.io.y.row(b, r0);
+            float* y1 = y0 + a.io.y.cs;
 #pragma unroll
             for (int j = 0; j < TJ; ++j) {
                 const int q = qb + 32 * j;
@@ -329,7 +308,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
                 unpack2(acc[p][j], v0, v1);
                 v0 += b0; v1 += b1;
                 if (relu_p) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                if (logc_p) { v0 = logf(fmaxf(v0, a.act_param)); v1 = logf(fmaxf(v1, a.act_param)); }
+                if (logc_p) { v0 = logf(fmaxf(v0, a.io.act_param)); v1 = logf(fmaxf(v1, a.io.act_param)); }
                 v0 *= mkp[j]; v1 *= mkp[j];
                 if (inw(q)) {
                     if (r0 < a.Rows) y0[q] = v0;
@@ -342,41 +321,41 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
     // generic: v = act(acc + bias + cond) [*m] [+res] *scale [+y_old] [/div] [*m]; all loads are issued before
     // any store (res / y_old may alias y only element-for-element, never across threads)
     const int ups = a.ups;
-    const bool relu = a.act == ACT_RELU;
-    const bool split = (a.flags & EPI_SPLIT) != 0;
+    const bool relu = a.io.act == ACT_RELU;
+    const bool split = (a.io.flags & EPI_SPLIT) != 0;
     float mk[TJ];
     int tq[TJ];
 #pragma unroll
     for (int j = 0; j < TJ; ++j) {
         const int q = qb + 32 * j;
-        tq[j] = (q >= a.q_lo && q < a.q_hi) ? q * ups : 0x7fffffff;   // outside the window: fails every bound below
+        tq[j] = (q >= a.io.q_lo && q < a.io.q_hi) ? q * ups : 0x7fffffff;   // outside the window: fails every bound below
         mk[j] = 1.f;
-        if (a.ymask && ups == 1 && tq[j] < a.Tout) mk[j] = __ldg(a.ymask + b * a.ymask_bs + tq[j]);
+        if (a.io.ymask && ups == 1 && tq[j] < a.io.Tout) mk[j] = __ldg(a.io.ymask.row(b) + tq[j]);
     }
     // per-row destination: recomputed per phase instead of kept in registers (16 rows x 2 pointers would spill)
     auto rowinfo = [&](int i, float*& yp, const float*& rp, bool& accum, bool& mpost, int& tlim) -> bool {
         const int r = row_base + i;
         int chn = r, ph = 0;
         if (ups > 1) { chn = r / ups; ph = r - chn * ups; }
-        accum = (a.flags & EPI_ACCUM) != 0;
-        mpost = (a.flags & EPI_MASK_POST) != 0;
-        yp = a.y + b * a.y_bs + (long long)chn * a.y_cs + ph;
+        accum = (a.io.flags & EPI_ACCUM) != 0;
+        mpost = (a.io.flags & EPI_MASK_POST) != 0;
+        yp = a.io.y.row(b, chn) + ph;
         if (split) {
-            if (chn < a.split) { accum = true; mpost = true; }
-            else { yp = a.y2 + b * a.y2_bs + (long long)(chn - a.split) * a.y2_cs; accum = (a.flags & EPI_ACCUM2) != 0; mpost = false; }
+            if (chn < a.io.split) { accum = true; mpost = true; }
+            else { yp = a.io.y2.row(b, chn - a.io.split); accum = (a.io.flags & EPI_ACCUM2) != 0; mpost = false; }
         }
-        rp = a.res ? a.res + b * a.res_bs + (long long)chn * a.res_cs + ph : nullptr;
-        tlim = a.Tout - ph;   // element (q*ups + ph) exists iff q*ups < Tout - ph
+        rp = a.io.res ? a.io.res.row(b, chn) + ph : nullptr;
+        tlim = a.io.Tout - ph;   // element (q*ups + ph) exists iff q*ups < Tout - ph
         return r < a.Rows;
     };
-    const bool mpre = (a.flags & EPI_MASK_PRE) != 0;
+    const bool mpre = (a.io.flags & EPI_MASK_PRE) != 0;
     // phase 1: bias / cond / activation / pre-mask (registers only)
 #pragma unroll
     for (int p = 0; p < CJ / 2; ++p) {
         const int r0 = row_base + 2 * p;
         float b0 = 0.f, b1 = 0.f;
-        if (r0 < a.Rows) { b0 = a.bias[r0]; if (a.cond) b0 += __ldg(a.cond + b * a.cond_bs + r0); }
-        if (r0 + 1 < a.Rows) { b1 = a.bias[r0 + 1]; if (a.cond) b1 += __ldg(a.cond + b * a.cond_bs + r0 + 1); }
+        if (r0 < a.Rows) { b0 = a.bias[r0]; if (a.io.cond) b0 += __ldg(a.io.cond.row(b) + r0); }
+        if (r0 + 1 < a.Rows) { b1 = a.bias[r0 + 1]; if (a.io.cond) b1 += __ldg(a.io.cond.row(b) + r0 + 1); }
 #pragma unroll
         for (int j = 0; j < TJ; ++j) {
             float v0, v1;
@@ -388,7 +367,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         }
     }
     // phase 2: residual (all loads first)
-    if (a.res) {
+    if (a.io.res) {
 #pragma unroll
         for (int p = 0; p < CJ / 2; ++p) {
             float *yp0, *yp1; const float *rp0, *rp1; bool ac0, ac1, mp0, mp1; int tl0, tl1;
@@ -404,8 +383,8 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         }
     }
     // phase 3: scale, accumulate into the destination (all loads first)
-    const float scale = a.scale;
-    if (split || (a.flags & EPI_ACCUM)) {
+    const float scale = a.io.scale;
+    if (split || (a.io.flags & EPI_ACCUM)) {
 #pragma unroll
         for (int p = 0; p < CJ / 2; ++p) {
             float *yp0, *yp1; const float *rp0, *rp1; bool ac0, ac1, mp0, mp1; int tl0, tl1;
@@ -430,7 +409,7 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
             }
     }
     // phase 4: mean / post-mask / store
-    const float div = a.post_div;
+    const float div = a.io.post_div;
 #pragma unroll
     for (int p = 0; p < CJ / 2; ++p) {
         float *yp0, *yp1; const float *rp0, *rp1; bool ac0, ac1, mp0, mp1; int tl0, tl1;
@@ -647,38 +626,36 @@ int pack_conv_transpose(ConvLayer& L, const float* w, const float* bias, int Cin
 // (Cin * 4 B per output sample).  Reference: hifigan_generator.py:262-264.  Eight CTAs per SM (32 registers): a full
 // SM of warps to keep the loads in flight.
 // REFLECT: reflection padding (ConvIO::reflect, K = 7 only), a compile-time switch: the edge threads mirror their own
-// register window, no extra loads; 40 registers (six CTAs per SM), which the two edge fix-ups need to stay unspilled
+// register window, no extra loads; 40 registers (six CTAs per SM), which the two edge fix-ups need to stay unspilled.
+// w_stride: the distance of row 0's consecutive weights in the FMA image (the layer's co_tile); blk_lo: the grid's first
+// block (the column window's)
 template <int K, bool REFLECT>
-__global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const float* __restrict__ x, long long x_bs, int x_cs, int Cin,
-                                                          int T, const float* __restrict__ w, int w_stride,
-                                                          const float* __restrict__ bias, float slope, int act,
-                                                          float* __restrict__ y, long long y_bs,
-                                                          unsigned* __restrict__ peak_bits, const int* __restrict__ lens,
-                                                          int rate, int need_out, int need_in, int q_lo, int q_hi,
-                                                          int in_lo, int blk_lo) {
+__global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const ConvKArgs a, int w_stride, int blk_lo) {
     constexpr int PAD = (K - 1) / 2, NL = (4 + 4 + (K - 1 - PAD) + 3) / 4;   // float4 loads covering [t0 - 4, t0 + 4 + K-1-PAD)
     static_assert(!REFLECT || K == 7, "the in-window mirror below is laid out for K = 7");
+    const int Cin = a.Cin, T = a.io.Tout, q_lo = a.io.q_lo, q_hi = a.io.q_hi;
+    unsigned* const peak_bits = a.io.peak_bits;
     extern __shared__ float ws[];
-    for (int i = threadIdx.x; i < Cin * K; i += blockDim.x) ws[i] = w[(size_t)i * w_stride];
+    for (int i = threadIdx.x; i < Cin * K; i += blockDim.x) ws[i] = a.w[(size_t)i * w_stride];
     __syncthreads();
     const int b = blockIdx.y;
     // ragged batch: row b is computed below Tb only (a multiple of 4) and samples from Tb on are written as zeros, so the
     // padded tail of the waveform is clean; the input holds data below Ti (its producer's extent) and reads as zero beyond
     int Tb = T, Ti = T;
-    if (lens) {
-        const long long base = (long long)lens[b] * rate;
-        const long long e = (base + need_out + 3) / 4 * 4, ei = (base + need_in + 3) / 4 * 4;
+    if (a.io.lens) {
+        const long long base = (long long)a.io.lens[b] * a.io.rate_out;
+        const long long e = (base + a.io.need_out + 3) / 4 * 4, ei = (base + a.io.need_in + 3) / 4 * 4;
         Tb = (int)(e < (long long)T ? (e > 0 ? e : 0) : (long long)T);
         Ti = (int)(ei < (long long)T ? (ei > 0 ? ei : 0) : (long long)T);
     }
     // column window [q_lo, hi): the grid starts at block blk_lo, only samples inside the window are stored (and folded
     // into the peak), and the input holds data from in_lo on (whole float4s below it read as zero)
-    const int hi = min(q_hi, T), in_lo4 = in_lo & ~3;
+    const int hi = min(q_hi, T), in_lo4 = a.io.in_lo & ~3;
     const int blk0 = (int)((blockIdx.x + blk_lo) * blockDim.x) * 4;
     const int t0 = blk0 + (int)threadIdx.x * 4;
     const bool inside = t0 >= q_lo && t0 + 4 <= hi;              // all four samples in the window: one float4 store
     const bool any = t0 < hi && t0 + 4 > q_lo;
-    float* yp = y + b * y_bs + t0;
+    float* yp = a.io.y.row(b, 0) + t0;
     auto store = [&](const float4& v) {
         if (inside) {
             *reinterpret_cast<float4*>(yp) = v;
@@ -697,11 +674,11 @@ __global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const
     if (!valid && !peak_bits) return;
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
     if (valid) {
-        const float* xb = x + b * x_bs + t0;
+        const float* xb = a.io.x.p + b * a.io.x.bs + t0;
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 4
         for (int ci = 0; ci < Cin; ++ci) {
-            const float* xr = xb + (long long)ci * x_cs;
+            const float* xr = xb + (long long)ci * a.io.x.cs;
             float win[4 * NL];
 #pragma unroll
             for (int l = 0; l < NL; ++l) {
@@ -718,7 +695,7 @@ __global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const
                 if (t0 == 0) { win[0] = win[8]; win[1] = win[7]; win[2] = win[6]; win[3] = win[5]; }
             }
 #pragma unroll
-            for (int i = 0; i < 4 * NL; ++i) win[i] = win[i] > 0.f ? win[i] : win[i] * slope;
+            for (int i = 0; i < 4 * NL; ++i) win[i] = win[i] > 0.f ? win[i] : win[i] * a.io.in_slope;
 #pragma unroll
             for (int k = 0; k < K; ++k) {
                 const float wk = ws[ci * K + k];
@@ -726,12 +703,12 @@ __global__ void __launch_bounds__(256, REFLECT ? 6 : 8) conv1d_row1_kernel(const
                 for (int j = 0; j < 4; ++j) acc[j] = fmaf(wk, win[4 - PAD + j + k], acc[j]);
             }
         }
-        const float bv = bias[0];
+        const float bv = a.bias[0];
         float* po = &o.x;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             float u = acc[j] + bv;
-            if (act == ACT_TANH) u = tanhf(u);
+            if (a.io.act == ACT_TANH) u = tanhf(u);
             po[j] = u;
         }
         store(o);
@@ -767,7 +744,7 @@ static int launch_variant(const ConvKArgs& ka, int B, int RowsPad, cudaStream_t 
     B200_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "conv1d: grid too large");
     conv1d_kernel<CJ, TJ, WCO, WT, CIC, EPI, KG><<<grid, NT, smem, st>>>(a);
     count_launch();
-    dispatch_note(EPI == KEPI_WAVEGRAD ? DISPATCH_FMA_WG + (a.near_src > 0 ? 1 : 0) : DISPATCH_FMA);
+    dispatch_note(EPI == KEPI_WAVEGRAD ? DISPATCH_FMA_WG + (a.io.near_src > 0 ? 1 : 0) : DISPATCH_FMA);
     B200_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -836,22 +813,23 @@ static cudaError_t launch_tc3(tc3::Tc3Kernel k, int grid, size_t smem, cudaStrea
     return cudaLaunchKernelEx(&cfg, k, t);
 }
 // ragged batches: the prefix table lives behind everything else in dynamic shared memory (when it still fits)
-static void set_ragged(tc3::Tc3Args& t, const ConvKArgs& a, size_t& smem, size_t max_smem) {
-    t.lens = nullptr; t.rate_q = 1; t.need_q = 0; t.rate_in = 1; t.need_in = 0; t.pref_off = 0;
-    if (!a.lens) return;
-    const size_t off = (smem + 15) / 16 * 16, extra = tc3::ragged_table_bytes(t.B);
-    if (off + extra > max_smem) return;             // enormous batch: fall back to the dense schedule (still correct)
-    t.lens = a.lens; t.rate_q = a.rate_out; t.need_q = a.need_out; t.rate_in = a.rate_in; t.need_in = a.need_in;
+static void set_ragged(tc3::Tc3Args& t, size_t& smem, size_t max_smem) {
+    if (!t.io.lens) return;
+    const size_t off = (smem + 15) / 16 * 16, extra = tc3::ragged_table_bytes(t.io.B);
+    if (off + extra > max_smem) {                   // enormous batch: fall back to the dense schedule (still correct)
+        t.io.lens = nullptr;
+        return;
+    }
     t.pref_off = (int)off;
     smem = off + extra;
 }
 // column window: the window's tiles per row on the full call's tile grid (the whole tensor by default)
-static void set_window(tc3::Tc3Args& t, const ConvKArgs& a) {
+static void set_window(tc3::Tc3Args& t) {
     // the grouped mode's zero-padded taps (K not a multiple of GRP) read past the conv's reach: 0 * stale scratch must
     // not reach the window (NaN), so the input extent also stops where its producer's window ends
-    t.Tin = std::min(a.Tin, a.in_hi);
-    t.q_lo = a.q_lo; t.q_hi = a.q_hi; t.in_lo = a.in_lo; t.t_lo = a.q_lo / t.tstep;
-    const int hi = std::min(a.Tq, a.q_hi);
+    t.io.Tin = std::min(t.io.Tin, t.io.in_hi);
+    t.t_lo = t.io.q_lo / t.tstep;
+    const int hi = std::min(t.Tq, t.io.q_hi);
     t.n_ttiles = std::max(0, (hi + t.tstep - 1) / t.tstep - t.t_lo);
 }
 
@@ -905,26 +883,26 @@ int tc_device(int** err, int* num_sms, size_t* max_smem) {
     return 0;
 }
 
-static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& a, cudaStream_t st) {
+static int try_launch_tc(const ConvLayer& L, const ConvKArgs& a, cudaStream_t st) {
+    const ConvIO& io = a.io;
     if (L.tc_prec == TC_NONE || a.Tq < 128) return -1;
-    if (a.act == ACT_LOGCLAMP || a.act == ACT_TANH) return -1;
-    if (!(a.in_slope >= 0.f && a.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
-    const bool needs_v3 = (a.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
+    if (io.act == ACT_LOGCLAMP || io.act == ACT_TANH) return -1;
+    if (!(io.in_slope >= 0.f && io.in_slope <= 1.f)) return -1;   // the producers' leaky ReLU is max(x, slope * x)
+    const bool needs_v3 = (io.flags & (EPI_MASK_PRE | EPI_SPLIT | EPI_ACCUM2 | EPI_GATE)) != 0;
     int* g_tc_err = nullptr;
     int num_sms = 0;
     size_t max_smem = 0;
     if (int rc = tc_device(&g_tc_err, &num_sms, &max_smem)) return rc;
     // persistent kernels: 16-byte aligned activation rows for the cp.async staging, no input mask
-    const bool aligned = ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) && (a.x_cs % 4 == 0) && (a.x_bs % 4 == 0);
-    const bool persistent_ok = aligned && !a.xmask &&
-                               (L.ups == 1 || (!a.res && !(a.flags & EPI_ACCUM) && !a.ymask && !a.cond));
+    const bool persistent_ok = io.x.aligned16() && !io.xmask &&
+                               (L.ups == 1 || (!io.res && !(io.flags & EPI_ACCUM) && !io.ymask && !io.cond));
     auto fits = [&](int rp) { return rp <= 320 && tc3::smem_bytes3(rp, L.tc_prec) <= max_smem; };
     // grouped mode for the layers with a grouped image: M = tap groups x channels, N = 256 time steps, 240 per tile
     const int G = L.tc_grp, J = G ? (L.K + G - 1) / G : 0;
     const int rp_grouped = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
-    const bool wg = (a.flags & EPI_WAVEGRAD) != 0;   // WaveGrad epilogue / resampled input: conv1d_tc3w_kernel
+    const bool wg = (io.flags & EPI_WAVEGRAD) != 0;   // WaveGrad epilogue / resampled input: conv1d_tc3w_kernel
     if (wg && !tc3::wavegrad_kernel(L.tc_prec, false)) return -1;
-    const bool grouped = G && !wg && !needs_v3 && !a.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
+    const bool grouped = G && !wg && !needs_v3 && !io.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
     // plain mode otherwise: M = rows (128 per tile, zero padded), N = 256 time steps.  Everything neither mode takes
     // (unaligned or masked inputs, shared-memory budget) runs on the exact FP32-FMA kernel.
     // At PREC_F16X3 the grouped layers run on the time-major kernel (M = time, N = the 32 / 64 channels): 256-column tiles,
@@ -937,49 +915,33 @@ static int try_launch_tc(const ConvLayer& L, const ConvIO& io, const ConvKArgs& 
     const int rows_pad = tm ? (128 * tm_slices + reach + 7) / 8 * 8
                             : grouped ? rp_grouped : rp256;
     if (!persistent_ok || !fits(rows_pad)) return -1;
-    tc3::Tc3Args t;
-    memset(&t, 0, sizeof(t));
-    t.x = a.x; t.x_bs = a.x_bs; t.x_cs = a.x_cs; t.Tin = a.Tin; t.in_slope = a.in_slope;
-    t.w = grouped ? L.w_tcg : L.w_tc; t.rscale = L.tc_rscale; t.bias = L.bias; t.cond = a.cond; t.cond_bs = a.cond_bs;
-    t.Cin = L.Cin; t.K = L.K; t.dil = L.dil; t.pad = L.pad; t.Rows = L.Rows; t.N = tc3::MROWS;
+    tc3::Tc3Args t{a};
+    t.w_tc = grouped ? L.w_tcg : L.w_tc; t.rscale = L.tc_rscale;
     t.KJ = grouped && !tm ? J : L.K; t.dil_blk = grouped && !tm ? G * L.dil : L.dil;
     t.tstep = tm ? 128 * tm_slices : grouped ? tc3::TSTEP_GROUPED : tc3::TT2;
-    t.y = a.y; t.y_bs = a.y_bs; t.y_cs = a.y_cs; t.Tout = a.Tout; t.ups = L.ups; t.Tq = a.Tq;
-    t.res = a.res; t.res_bs = a.res_bs; t.res_cs = a.res_cs;
-    t.ymask = a.ymask; t.ymask_bs = a.ymask_bs;
-    t.scale = a.scale; t.post_div = a.post_div; t.relu = (a.act == ACT_RELU); t.accum = (a.flags & EPI_ACCUM) ? 1 : 0;
-    t.mask_post = (a.flags & EPI_MASK_POST) ? 1 : 0;
-    t.mask_pre = (a.flags & EPI_MASK_PRE) ? 1 : 0;
-    t.gate = (a.flags & EPI_GATE) ? 1 : 0;
-    t.split = (a.flags & EPI_SPLIT) ? a.split : 0;
-    t.y2 = a.y2; t.y2_bs = a.y2_bs; t.y2_cs = a.y2_cs; t.accum2 = (a.flags & EPI_ACCUM2) ? 1 : 0;
     t.rows_pad = rows_pad; t.raw_w = rows_pad + 4;
-    t.B = io.B; t.n_rtiles = (L.Rows + tc3::MROWS - 1) / tc3::MROWS;   // 1 in grouped mode (32 / 64 rows)
-    set_window(t, a);
+    t.n_rtiles = (L.Rows + tc3::MROWS - 1) / tc3::MROWS;   // 1 in grouped mode (32 / 64 rows)
+    set_window(t);
     t.err = g_tc_err;
     size_t smem = tm ? tc3::smem_bytes_tm(rows_pad, L.Rows, tm_slices) : tc3::smem_bytes3(rows_pad, L.tc_prec);
-    set_ragged(t, a, smem, max_smem);
+    set_ragged(t, smem, max_smem);
     // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
     // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
-    const bool plain_epi = L.ups == 1 && !t.gate && t.split == 0 && !t.relu && !t.ymask && t.scale == 1.f && t.post_div == 1.f;
-    const bool reflect = a.reflect != 0;   // reflection padding: the lean kernels' reflect variants only
+    const bool plain_epi = L.ups == 1 && !(io.flags & EPI_GATE) && io.split == 0 && io.act != ACT_RELU && !io.ymask &&
+                           io.scale == 1.f && io.post_div == 1.f;
+    const bool reflect = io.reflect != 0;   // reflection padding: the lean kernels' reflect variants only
     if (reflect && !grouped && !plain_epi) return -1;
-    if (wg) {
-        t.near_src = a.near_src; t.near_scale = a.near_scale;
-        t.film = a.film; t.film_bs = a.film_bs; t.film_cs = a.film_cs; t.film_half = a.film_half;
-        t.act_add = a.act_add; t.lrelu = a.act == ACT_LRELU; t.act_param = a.act_param;
-    }
-    const tc3::Tc3Kernel k = wg ? tc3::wavegrad_kernel(L.tc_prec, a.near_src > 0)
+    const tc3::Tc3Kernel k = wg ? tc3::wavegrad_kernel(L.tc_prec, io.near_src > 0)
                                 : tm      ? tc3::timemajor_kernel(L.Rows, tm_slices, reflect)
                                 : grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect)
                                           : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
-    const long long tiles = (long long)t.B * t.n_ttiles * t.n_rtiles;
+    const long long tiles = (long long)io.B * t.n_ttiles * t.n_rtiles;
     const int grid = (int)std::max(1LL, tiles < num_sms ? tiles : num_sms);
     B200_CUDA_OK(launch_tc3(k, grid, smem, st, t));
     count_launch();
     const bool b16 = L.tc_prec == tc::PREC_BF16 || L.tc_prec == tc::PREC_FP16;   // PREC_F16X3 logs as tc3
     if (wg)
-        dispatch_note((L.tc_prec == tc::PREC_F16X3 ? DISPATCH_TC3W_F16X3 : DISPATCH_TC3W_TF32) + (a.near_src > 0 ? 1 : 0));
+        dispatch_note((L.tc_prec == tc::PREC_F16X3 ? DISPATCH_TC3W_F16X3 : DISPATCH_TC3W_TF32) + (io.near_src > 0 ? 1 : 0));
     else
         dispatch_note(grouped ? (b16 ? DISPATCH_TC16_GROUPED : DISPATCH_TC3_GROUPED) : (b16 ? DISPATCH_TC16 : DISPATCH_TC3));
     B200_CUDA_OK(cudaGetLastError());
@@ -999,76 +961,63 @@ int conv_tc_error_flag() {
     return f;
 }
 
-int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
-    B200_REQUIRE(L.w && io.x && io.y, "launch_conv: null tensor");
-    ConvKArgs a;
-    memset(&a, 0, sizeof(a));
-    a.x = io.x.p; a.x_bs = io.x.bs; a.x_cs = io.x.cs; a.Tin = io.Tin;
-    a.xmask = io.xmask.p; a.xmask_bs = io.xmask.bs; a.in_slope = io.in_slope;
-    a.w = L.w; a.bias = L.bias; a.cond = io.cond.p; a.cond_bs = io.cond.bs;
+int launch_conv(const ConvLayer& L, const ConvIO& call, cudaStream_t st) {
+    B200_REQUIRE(L.w && call.x && call.y, "launch_conv: null tensor");
+    ConvKArgs a{call};
+    ConvIO& io = a.io;   // normalised here, so that every kernel family reads the same options
+    io.q_lo = std::max(0, io.q_lo);
+    io.in_lo = std::max(0, io.in_lo);
+    if (io.near_src > 0) io.flags |= EPI_WAVEGRAD;
+    if (!(io.flags & EPI_SPLIT)) io.split = 0;   // the tensor-core epilogues test split > 0, the FMA kernel the flag
+    a.w = L.w; a.bias = L.bias;
     a.Cin = L.Cin; a.CinPad = L.CinPad; a.K = L.K; a.dil = L.dil; a.pad = L.pad; a.Rows = L.Rows; a.ups = L.ups;
-    a.y = io.y.p; a.y_bs = io.y.bs; a.y_cs = io.y.cs; a.Tout = io.Tout;
     a.Tq = (L.ups > 1) ? (io.Tout + L.ups - 1) / L.ups : io.Tout;
-    a.res = io.res.p; a.res_bs = io.res.bs; a.res_cs = io.res.cs;
-    a.ymask = io.ymask.p; a.ymask_bs = io.ymask.bs;
-    a.y2 = io.y2.p; a.y2_bs = io.y2.bs; a.y2_cs = io.y2.cs; a.split = io.split;
-    a.scale = io.scale; a.post_div = io.post_div; a.act = io.act; a.act_param = io.act_param; a.flags = io.flags;
-    a.lens = io.lens; a.rate_out = io.rate_out; a.need_out = io.need_out; a.rate_in = io.rate_in; a.need_in = io.need_in;
-    a.q_lo = std::max(0, io.q_lo); a.q_hi = io.q_hi; a.in_lo = std::max(0, io.in_lo); a.in_hi = io.in_hi;
-    const bool windowed = a.q_lo > 0 || a.q_hi < a.Tq;
-    a.reflect = io.reflect ? 1 : 0;
-    if (a.reflect) {   // torch's ReflectionPad1d limit; nothing needs reflection together with the options below
+    a.near_scale = io.near_src > 0 ? (float)io.near_src / (float)io.Tin : 1.f;
+    const bool windowed = io.q_lo > 0 || io.q_hi < a.Tq;
+    if (io.reflect) {   // torch's ReflectionPad1d limit; nothing needs reflection together with the options below
         B200_REQUIRE(L.pad <= io.Tin - 1, "launch_conv: reflection padding %d needs at least %d input columns, got %d", L.pad,
                      L.pad + 1, io.Tin);
-        B200_REQUIRE(!io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && L.ups == 1 && !io.xmask,
+        B200_REQUIRE(!io.lens && !windowed && io.in_lo == 0 && io.in_hi == 0x7fffffff && L.ups == 1 && !io.xmask,
                      "launch_conv: reflection padding takes no lens, column window, input mask or upsampling");
     }
-    if (io.near_src > 0) a.flags |= EPI_WAVEGRAD;
-    if (a.flags & EPI_WAVEGRAD) {   // WaveGrad layers: their own kernel variants (tensor cores, else the FMA tile kernel)
-        B200_REQUIRE(L.ups == 1 && !io.lens && !windowed && a.in_lo == 0 && a.in_hi == 0x7fffffff && !io.xmask && !io.ymask &&
-                         !io.cond && !a.reflect && a.flags == EPI_WAVEGRAD && a.scale == 1.f && a.post_div == 1.f &&
-                         (a.act == ACT_NONE || a.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film.cs > 0)) &&
+    if (io.flags & EPI_WAVEGRAD) {   // WaveGrad layers: their own kernel variants (tensor cores, else the FMA tile kernel)
+        B200_REQUIRE(L.ups == 1 && !io.lens && !windowed && io.in_lo == 0 && io.in_hi == 0x7fffffff && !io.xmask && !io.ymask &&
+                         !io.cond && !io.reflect && io.flags == EPI_WAVEGRAD && io.scale == 1.f && io.post_div == 1.f &&
+                         (io.act == ACT_NONE || io.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film.cs > 0)) &&
                          io.near_src >= 0,
                      "launch_conv: the WaveGrad epilogue takes only lrelu / act_add / res / y2 / film, on a dense launch");
-        a.near_src = io.near_src;
-        a.near_scale = io.near_src > 0 ? (float)io.near_src / (float)io.Tin : 1.f;
-        a.film = io.film.p; a.film_bs = io.film.bs; a.film_cs = io.film.cs; a.film_half = io.film_half;
-        a.act_add = io.act_add;
         if (a.Tq <= 0 || io.B <= 0) return 0;
-        if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;
+        if (int rc = try_launch_tc(L, a, st); rc != -1) return rc;
         return launch_cic<KEPI_WAVEGRAD>(a, L.co_tile, io.B, L.RowsPad, st);
     }
-    B200_REQUIRE(a.act != ACT_LRELU, "launch_conv: the leaky-ReLU epilogue needs EPI_WAVEGRAD");
+    B200_REQUIRE(io.act != ACT_LRELU, "launch_conv: the leaky-ReLU epilogue needs EPI_WAVEGRAD");
     if (a.Tq <= 0 || io.B <= 0) return 0;
-    B200_REQUIRE(!(a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)) || io.ymask,
+    B200_REQUIRE(!(io.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)) || io.ymask,
                  "launch_conv: masked/split epilogue needs ymask");
-    B200_REQUIRE(!(a.flags & EPI_SPLIT) || io.y2, "launch_conv: split epilogue needs y2");
+    B200_REQUIRE(!(io.flags & EPI_SPLIT) || io.y2, "launch_conv: split epilogue needs y2");
     B200_REQUIRE(!(io.ymask && L.ups > 1), "launch_conv: output mask with an upsampling layer is not supported");
     // a mask without a flag saying where it applies: the FMA plain epilogue would apply it, the others would not
-    B200_REQUIRE(!io.ymask || (a.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)),
+    B200_REQUIRE(!io.ymask || (io.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)),
                  "launch_conv: ymask needs EPI_MASK_PRE, EPI_MASK_POST or EPI_SPLIT");
-    if (a.flags & EPI_GATE) {
-        B200_REQUIRE(L.ups == 1 && !io.res && !io.ymask && a.act == ACT_NONE && a.flags == EPI_GATE && a.scale == 1.f &&
-                         a.post_div == 1.f,
+    if (io.flags & EPI_GATE) {
+        B200_REQUIRE(L.ups == 1 && !io.res && !io.ymask && io.act == ACT_NONE && io.flags == EPI_GATE && io.scale == 1.f &&
+                         io.post_div == 1.f,
                      "launch_conv: gate epilogue takes no other options");
-        if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;
+        if (int rc = try_launch_tc(L, a, st); rc != -1) return rc;
         return launch_cic<KEPI_GATE>(a, L.co_tile, io.B, L.RowsPad, st);
     }
-    if (a.act == ACT_TANH) {
-        B200_REQUIRE(L.ups == 1 && !io.res && !io.cond && a.flags == 0 && a.scale == 1.f && a.post_div == 1.f,
+    if (io.act == ACT_TANH) {
+        B200_REQUIRE(L.ups == 1 && !io.res && !io.cond && io.flags == 0 && io.scale == 1.f && io.post_div == 1.f,
                      "launch_conv: tanh epilogue takes no other options");
         // conv_post (one output row, 7 taps): streaming kernel when rows are 16-byte aligned
-        if (L.Rows == 1 && L.K == 7 && L.dil == 1 && L.pad == 3 && !a.xmask && a.Tin == a.Tout && (a.Tout % 4) == 0 &&
-            (a.x_cs % 4) == 0 && (a.x_bs % 4) == 0 && (a.y_bs % 4) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0 &&
-            (reinterpret_cast<uintptr_t>(a.y) & 15) == 0 && (size_t)L.Cin * L.K * 4 <= 48 * 1024) {
-            const int blk_lo = a.q_lo / 1024, blk_hi = (std::min(a.q_hi, a.Tout) + 1023) / 1024;   // 1024 samples per CTA
+        if (L.Rows == 1 && L.K == 7 && L.dil == 1 && L.pad == 3 && !io.xmask && io.Tin == io.Tout && (io.Tout % 4) == 0 &&
+            io.x.aligned16() && (io.y.bs % 4) == 0 && (reinterpret_cast<uintptr_t>(io.y.p) & 15) == 0 &&
+            (size_t)L.Cin * L.K * 4 <= 48 * 1024) {
+            const int blk_lo = io.q_lo / 1024, blk_hi = (std::min(io.q_hi, io.Tout) + 1023) / 1024;   // 1024 samples per CTA
             dim3 grid(std::max(1, blk_hi - blk_lo), io.B);
             if (grid.y <= 65535) {
-                auto kern = a.reflect ? conv1d_row1_kernel<7, true> : conv1d_row1_kernel<7, false>;
-                kern<<<grid, 256, (size_t)L.Cin * L.K * 4, st>>>(a.x, a.x_bs, a.x_cs, L.Cin, a.Tout, L.w, L.co_tile, L.bias,
-                                                                 a.in_slope, a.act, a.y, a.y_bs, io.peak_bits, a.lens,
-                                                                 a.rate_out, a.need_out, a.need_in, a.q_lo, a.q_hi, a.in_lo,
-                                                                 blk_lo);
+                auto kern = io.reflect ? conv1d_row1_kernel<7, true> : conv1d_row1_kernel<7, false>;
+                kern<<<grid, 256, (size_t)L.Cin * L.K * 4, st>>>(a, L.co_tile, blk_lo);
                 count_launch();
                 dispatch_note(DISPATCH_ROW1);
                 B200_CUDA_OK(cudaGetLastError());
@@ -1077,18 +1026,18 @@ int launch_conv(const ConvLayer& L, const ConvIO& io, cudaStream_t st) {
         }
         if (int rc = launch_cic<KEPI_TANH>(a, L.co_tile, io.B, L.RowsPad, st)) return rc;
         if (io.peak_bits) {   // the streaming kernel was not eligible: fold the peak in a pass of its own
-            B200_REQUIRE(a.y_cs == a.Tout && a.y_bs == (long long)L.Rows * a.Tout, "launch_conv: peak needs a dense output");
+            B200_REQUIRE(io.y.cs == io.Tout && io.y.bs == (long long)L.Rows * io.Tout, "launch_conv: peak needs a dense output");
             if (windowed)   // only the samples this launch stored
-                return launch_absmax_window(a.y, io.B * L.Rows, a.Tout, a.q_lo, std::min(a.q_hi, a.Tout), io.peak_bits, st);
-            return launch_absmax(a.y, (long long)io.B * L.Rows * a.Tout, io.peak_bits, st);
+                return launch_absmax_window(io.y.p, io.B * L.Rows, io.Tout, io.q_lo, std::min(io.q_hi, io.Tout), io.peak_bits, st);
+            return launch_absmax(io.y.p, (long long)io.B * L.Rows * io.Tout, io.peak_bits, st);
         }
         return 0;
     }
-    if (int rc = try_launch_tc(L, io, a, st); rc != -1) return rc;
-    const bool plain = L.ups == 1 && !io.res && a.scale == 1.f && a.post_div == 1.f &&
-                       (a.flags & ~(EPI_MASK_POST | EPI_MASK_PRE)) == 0;
+    if (int rc = try_launch_tc(L, a, st); rc != -1) return rc;
+    const bool plain = L.ups == 1 && !io.res && io.scale == 1.f && io.post_div == 1.f &&
+                       (io.flags & ~(EPI_MASK_POST | EPI_MASK_PRE)) == 0;
     if (plain) return launch_cic<KEPI_PLAIN>(a, L.co_tile, io.B, L.RowsPad, st);
-    B200_REQUIRE(a.act != ACT_LOGCLAMP, "launch_conv: log-clamp activation only with the plain epilogue");
+    B200_REQUIRE(io.act != ACT_LOGCLAMP, "launch_conv: log-clamp activation only with the plain epilogue");
     return launch_cic<KEPI_GENERIC>(a, L.co_tile, io.B, L.RowsPad, st);
 }
 

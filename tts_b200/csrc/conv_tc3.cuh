@@ -42,9 +42,24 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
 #include "conv_tc.cuh"   // descriptor / barrier / wgmma helpers
 
 namespace b200tts {
+
+// One conv launch as every conv kernel reads it (the FMA tile and single-row kernels of conv1d.cu, and Tc3Args below):
+// the call's operands and options, the layer, and what launch_conv derives from them.  launch_conv normalises `io`:
+// q_lo / in_lo >= 0, near_src > 0 sets EPI_WAVEGRAD, and split is 0 unless EPI_SPLIT is set.
+struct ConvKArgs {
+    ConvIO io;
+    const float* w; const float* bias;   // the FMA kernels' weight image [row_tiles][CinPad][K][co_tile], bias [RowsPad]
+    int Cin, CinPad, K, dil, pad, Rows, ups;
+    int Tq;                              // GEMM columns in time (= Tout for ups == 1)
+    int XS;                              // FMA tile kernel: staged window row length (launch_variant)
+    float near_scale;                    // (float)near_src / Tin (WaveGrad nearest resampling)
+};
+static_assert(std::is_trivially_copyable_v<ConvKArgs>, "ConvKArgs is a kernel argument");
+
 namespace tc3 {
 
 using namespace tc;       // smem_u32, mbar_*, make_desc, wgmma_*
@@ -66,52 +81,30 @@ constexpr int NCONS = 256;        // consumer threads (two warpgroups)
 constexpr int W_PROD = 8, W_LOAD = 8 + NPW;
 constexpr int NTHREADS2 = 32 * (W_LOAD + 1);
 
-struct Tc3Args {
-    const float* x; long long x_bs; int x_cs; int Tin;
-    float in_slope;
-    const void* w;             // packed [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32 (16-bit: [2][128][8];
-                               // PREC_F16X3: {hi, lo}[2][128][8] fp16)
+// The launch (ConvKArgs) plus the tensor-core schedule.  Ragged batches (io.lens; null: every row spans the full tensor):
+// row b only has tiles for GEMM columns below min(Tq, lens[b] * rate_out + need_out) and its input is read as zero from
+// min(Tin, lens[b] * rate_in + need_in) on, so padded frames cost nothing and `need` keeps every sample below lens[b]
+// bit-identical to the full computation (it is the receptive field of the layers that still follow, worked out per
+// launch by the engine).  Column window (io.q_lo / q_hi / in_lo): a row's tiles run from floor(q_lo / tstep) to
+// ceil(min(extent, q_hi) / tstep); tile origins stay multiples of tstep counted from column 0, so every column is computed
+// (and takes the same epilogue) as in the unwindowed launch.  Input columns below in_lo are stale scratch and read as
+// zero (whole 16-byte vectors: the ones below in_lo rounded down to a multiple of 4); the host stops io.Tin where the
+// producer's window ends, so the grouped mode's zero-padded taps never multiply stale data.
+struct Tc3Args : ConvKArgs {
+    const void* w_tc;          // the plain or grouped image: [row_tile][chunk][tap]{hi[2][128][4], lo[2][128][4]} fp32
+                               // (16-bit: [2][128][8]; PREC_F16X3: {hi, lo}[2][128][8] fp16), see pack_tc / pack_tc_tm
     const float* rscale;       // PREC_F16X3: [Rows] 2^-e_r, the inverse of the pack-time row scaling (see pack_tc)
-    const float* bias;
-    const float* cond; long long cond_bs;
-    int Cin, K, dil, pad, Rows, N;
-    float* y; long long y_bs; int y_cs; int Tout;
-    int ups;                   // 1, or the polyphase factor of a transposed conv (row r -> channel r/ups, phase r%ups)
-    int Tq;                    // GEMM columns in time (= Tout for ups == 1)
-    const float* res; long long res_bs; int res_cs;
-    const float* ymask; long long ymask_bs;
-    float scale; float post_div; int relu; int accum; int mask_post;
-    int mask_pre;              // multiply by ymask before the residual / accumulate (coupling `post`)
-    int gate;                  // rows are (tanh, sigmoid) pairs: out[r/2] = tanh(v[2p]) * sigmoid(v[2p+1])  (WaveNet)
-    int split;                 // > 0: rows < split -> y (accumulate, mask); rows >= split -> y2 (accumulate iff accum2)
-    float* y2; long long y2_bs; int y2_cs; int accum2;
     int KJ;                    // tap blocks per chunk (= K, or ceil(K / GRP) in grouped mode)
     int dil_blk;               // B-row shift between tap blocks (= dil, or GRP * dil)
     int tstep;                 // time steps a tile advances (= TT2, or 240 in grouped mode)
     int rows_pad;              // slab rows  (TT2 + halo, multiple of 8)
     int raw_w;                 // raw row width in floats (rows_pad + 4, multiple of 4)
-    int B, n_ttiles, n_rtiles;
+    int n_ttiles, n_rtiles;    // the window's tiles per row (dense schedule), row tiles
+    int t_lo;                  // floor(q_lo / tstep): the window's first tile
+    int pref_off;              // byte offset in dynamic shared memory of the (B + 1)-entry tile prefix table (ragged)
     int* err;
-    // ---- ragged batches (null lens: every row spans the full tensor).  Row b only has tiles for GEMM columns below
-    // min(Tq, lens[b] * rate_q + need_q) and its input is read as zero from min(Tin, lens[b] * rate_in + need_in) on:
-    // padded frames cost nothing, and `need` keeps every sample below lens[b] bit-identical to the full computation
-    // (it is the receptive field of the layers that still follow, worked out per launch by the engine).
-    const int* lens; int rate_q, need_q, rate_in, need_in;
-    int pref_off;               // byte offset in dynamic shared memory of the (B + 1)-entry tile prefix table
-    // ---- column window (default [0, INT_MAX), in_lo 0: the whole tensor).  A row's tiles run from floor(q_lo / tstep) to
-    // ceil(min(extent, q_hi) / tstep); tile origins stay multiples of tstep counted from column 0, so every column is
-    // computed (and takes the same epilogue) as in the unwindowed launch.  Input columns below in_lo are stale scratch
-    // and read as zero (whole 16-byte vectors: the ones below in_lo rounded down to a multiple of 4); the host stops Tin
-    // where the producer's window ends, so the grouped mode's zero-padded taps never multiply stale data.  n_ttiles counts
-    // the window's tiles per row (dense schedule), t_lo = floor(q_lo / tstep) is the first one.
-    int q_lo, q_hi, in_lo, t_lo;
-    // ---- WaveGrad kernels only (conv1d_tc3w_kernel, see ConvIO): nearest-resampled input (near_src source columns, 0: off;
-    // near_scale = (float)near_src / Tin), FiLM (shift / scale rows of `film`), y2 store of the pre-FiLM value, leaky ReLU
-    // (lrelu, slope act_param) and the per-batch act_add after it
-    int near_src; float near_scale;
-    const float* film; long long film_bs; int film_cs, film_half;
-    const float* act_add; int lrelu; float act_param;
 };
+static_assert(std::is_trivially_copyable_v<Tc3Args>, "Tc3Args is a kernel argument");
 
 // torch's nearest source index (upsample_nearest1d's nearest_idx): identity, the exact-2x shortcut, else
 // min(floor(dst * scale), src - 1) with the float scale src / dst
@@ -250,16 +243,17 @@ __device__ __forceinline__ void bulk_combine(const float* d, float* st_row, cons
 //   v = acc + bias; [lrelu]; [+ act_add[b]]; [+ res]; [y2 <- v]; [v = shift + scale * v]; y <- v
 // with every product and sum rounded on its own (no FMA contraction), in the reference's order.
 template <bool SC, bool WG = false>
-__device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float* arow, int b, int rt, int q0, int lq, int half,
-                                                  int lane) {
+__device__ __forceinline__ void general_tile_body(const ConvKArgs& a, const float* rscale, const float* arow, int b, int rt,
+                                                  int q0, int lq, int half, int lane) {
+    const ConvIO& io = a.io;
     const int ups = a.ups;
     const int r = rt * MROWS + lq * 32 + lane;             // GEMM row of this lane
     const bool rok = r < a.Rows;
     const int rc = rok ? r : a.Rows - 1;
     const int qb = q0 + half * 128;
     float bias = a.bias[rc];
-    if (a.cond) bias += __ldg(a.cond + (long long)b * a.cond_bs + rc);
-    const float rs = SC ? a.rscale[rc] : 1.f;
+    if (io.cond) bias += __ldg(io.cond.row(b) + rc);
+    const float rs = SC ? rscale[rc] : 1.f;
     auto acc_ld = [&](const float* p, float* v) {
         acc_ld16(p, v);
         if constexpr (SC) {
@@ -269,15 +263,14 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
     };
     if constexpr (WG) {
         if (!rok) return;
-        const long long rcs = (long long)rc;
-        float* yrow = a.y + (long long)b * a.y_bs + rcs * a.y_cs;
-        float* y2row = a.y2 ? a.y2 + (long long)b * a.y2_bs + rcs * a.y2_cs : nullptr;
-        const float* rrow = a.res ? a.res + (long long)b * a.res_bs + rcs * a.res_cs : nullptr;
-        const float* srow = a.film ? a.film + (long long)b * a.film_bs + rcs * a.film_cs : nullptr;
-        const float* crow = srow ? srow + (long long)a.film_half * a.film_cs : nullptr;
-        const float add = a.act_add ? __ldg(a.act_add + b) : 0.f;
-        const bool has_add = a.act_add != nullptr, lrelu = a.lrelu != 0;
-        const float slope = a.act_param;
+        float* yrow = io.y.row(b, rc);
+        float* y2row = io.y2 ? io.y2.row(b, rc) : nullptr;
+        const float* rrow = io.res ? io.res.row(b, rc) : nullptr;
+        const float* srow = io.film ? io.film.row(b, rc) : nullptr;
+        const float* crow = srow ? srow + (long long)io.film_half * io.film.cs : nullptr;
+        const float add = io.act_add ? __ldg(io.act_add + b) : 0.f;
+        const bool has_add = io.act_add != nullptr, lrelu = io.act == ACT_LRELU;
+        const float slope = io.act_param;
         // float4 accesses when every row pointer is 16-byte aligned (all pitches multiples of 4 floats)
         const bool vec_ok = ((reinterpret_cast<uintptr_t>(yrow) | reinterpret_cast<uintptr_t>(y2row) |
                               reinterpret_cast<uintptr_t>(rrow) | reinterpret_cast<uintptr_t>(srow) |
@@ -288,8 +281,8 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int qq = qb + cg + 4 * j;
-                if (qq >= a.Tout) break;
-                const bool vec = vec_ok && qq + 3 < a.Tout;
+                if (qq >= io.Tout) break;
+                const bool vec = vec_ok && qq + 3 < io.Tout;
                 float r4[4] = {0.f, 0.f, 0.f, 0.f}, s4[4] = {0.f, 0.f, 0.f, 0.f}, c4[4] = {1.f, 1.f, 1.f, 1.f};
                 if (vec) {
                     if (rrow) { const float4 t = *reinterpret_cast<const float4*>(rrow + qq); r4[0] = t.x; r4[1] = t.y; r4[2] = t.z; r4[3] = t.w; }
@@ -300,7 +293,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
                 } else {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
-                        const int qe = min(qq + e, a.Tout - 1);
+                        const int qe = min(qq + e, io.Tout - 1);
                         if (rrow) r4[e] = rrow[qe];
                         if (srow) { s4[e] = srow[qe]; c4[e] = crow[qe]; }
                     }
@@ -321,7 +314,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
                 } else {
 #pragma unroll
                     for (int e = 0; e < 4; ++e)
-                        if (qq + e < a.Tout) {
+                        if (qq + e < io.Tout) {
                             if (y2row) y2row[qq + e] = p[e];
                             yrow[qq + e] = o[e];
                         }
@@ -330,10 +323,10 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
         }
         return;
     }
-    if (a.gate) {
+    if (io.flags & EPI_GATE) {
         // WaveNet gate (wavenet.py:6-13): even lane = tanh argument, odd lane = sigmoid argument of row r/2
-        float* yrow = a.y + (long long)b * a.y_bs + (long long)(rc >> 1) * a.y_cs;
-        const bool vec_ok = ((a.y_cs & 3) == 0) && ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0);
+        float* yrow = io.y.row(b, rc >> 1);
+        const bool vec_ok = ((io.y.cs & 3) == 0) && ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0);
         const bool even = (lane & 1) == 0;
         for (int cg = 0; cg < 128; cg += 16) {
             float v[16];
@@ -350,25 +343,25 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int qq = q + 4 * j;
-                    if (vec_ok && qq + 3 < a.Tout) *reinterpret_cast<float4*>(yrow + qq) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                    if (vec_ok && qq + 3 < io.Tout) *reinterpret_cast<float4*>(yrow + qq) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
                     else {
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) if (qq + e < a.Tout) yrow[qq + e] = v[4 * j + e];
+                        for (int e = 0; e < 4; ++e) if (qq + e < io.Tout) yrow[qq + e] = v[4 * j + e];
                     }
                 }
             }
         }
     } else if (ups == 1) {
-        float* yrow = a.y + (long long)b * a.y_bs + (long long)rc * a.y_cs;
-        bool acc_r = a.accum != 0, mpost_r = a.mask_post != 0;
-        if (a.split > 0) {          // WaveNet res/skip rows (wavenet.py:108-113)
-            if (rc < a.split) { acc_r = true; mpost_r = true; }
-            else { yrow = a.y2 + (long long)b * a.y2_bs + (long long)(rc - a.split) * a.y2_cs; acc_r = a.accum2 != 0; mpost_r = false; }
+        float* yrow = io.y.row(b, rc);
+        bool acc_r = (io.flags & EPI_ACCUM) != 0, mpost_r = (io.flags & EPI_MASK_POST) != 0;
+        if (io.split > 0) {         // WaveNet res/skip rows (wavenet.py:108-113)
+            if (rc < io.split) { acc_r = true; mpost_r = true; }
+            else { yrow = io.y2.row(b, rc - io.split); acc_r = (io.flags & EPI_ACCUM2) != 0; mpost_r = false; }
         }
-        const float* rrow = a.res ? a.res + (long long)b * a.res_bs + (long long)rc * a.res_cs : nullptr;
-        const float* mrow = a.ymask ? a.ymask + (long long)b * a.ymask_bs : nullptr;
-        const int ycs_eff = (a.split > 0 && rc >= a.split) ? a.y2_cs : a.y_cs;
-        const bool vec_ok = ((ycs_eff & 3) == 0) && (!a.res || (a.res_cs & 3) == 0) &&
+        const float* rrow = io.res ? io.res.row(b, rc) : nullptr;
+        const float* mrow = io.ymask ? io.ymask.row(b) : nullptr;
+        const int ycs_eff = (io.split > 0 && rc >= io.split) ? io.y2.cs : io.y.cs;
+        const bool vec_ok = ((ycs_eff & 3) == 0) && (!io.res || (io.res.cs & 3) == 0) &&
                             ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0) &&
                             (!rrow || (reinterpret_cast<uintptr_t>(rrow) & 15) == 0);
         // software pipeline: the (volatile) loads of group j+1 are issued before group j is finished, into the OTHER of
@@ -379,13 +372,13 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int qq = q + 4 * j;
-                if (vec_ok && qq + 3 < a.Tout) {
+                if (vec_ok && qq + 3 < io.Tout) {
                     if (rrow) asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r_[4 * j]), "=f"(r_[4 * j + 1]), "=f"(r_[4 * j + 2]), "=f"(r_[4 * j + 3]) : "l"(rrow + qq));
                     if (acc_r) asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(o_[4 * j]), "=f"(o_[4 * j + 1]), "=f"(o_[4 * j + 2]), "=f"(o_[4 * j + 3]) : "l"(yrow + qq));
                 } else {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
-                        const int qe = min(qq + e, a.Tout - 1);
+                        const int qe = min(qq + e, io.Tout - 1);
                         if (rrow) asm volatile("ld.global.f32 %0, [%1];" : "=f"(r_[4 * j + e]) : "l"(rrow + qe));
                         if (acc_r) asm volatile("ld.global.f32 %0, [%1];" : "=f"(o_[4 * j + e]) : "l"(yrow + qe));
                     }
@@ -400,13 +393,13 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
                 float u = v[i] + bias;
-                if (a.relu) u = fmaxf(u, 0.f);
-                const float mk = mrow ? __ldg(mrow + min(q + i, a.Tout - 1)) : 1.f;
-                if (a.mask_pre) u *= mk;
-                if (a.res) u += rv[i];
-                u *= a.scale;
+                if (io.act == ACT_RELU) u = fmaxf(u, 0.f);
+                const float mk = mrow ? __ldg(mrow + min(q + i, io.Tout - 1)) : 1.f;
+                if (io.flags & EPI_MASK_PRE) u *= mk;
+                if (io.res) u += rv[i];
+                u *= io.scale;
                 if (acc_r) u += ov[i];
-                if (a.post_div != 1.f) u = u / a.post_div;
+                if (io.post_div != 1.f) u = u / io.post_div;
                 if (mpost_r) u *= mk;
                 v[i] = u;
             }
@@ -414,11 +407,11 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int qq = q + 4 * j;
-                    if (vec_ok && qq + 3 < a.Tout) {
+                    if (vec_ok && qq + 3 < io.Tout) {
                         *reinterpret_cast<float4*>(yrow + qq) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
                     } else {
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) if (qq + e < a.Tout) yrow[qq + e] = v[4 * j + e];
+                        for (int e = 0; e < 4; ++e) if (qq + e < io.Tout) yrow[qq + e] = v[4 * j + e];
                     }
                 }
             }
@@ -434,7 +427,7 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
         // groups of `ups` phases, i.e. contiguous runs of `ups` output samples per channel
         if (!rok) return;
         const int co = rc / ups, ph = rc - co * ups;
-        float* yrow = a.y + (long long)b * a.y_bs + (long long)co * a.y_cs + ph;
+        float* yrow = io.y.row(b, co) + ph;
         for (int cg = 0; cg < 128; cg += 16) {
             float v[16];
             acc_ld(arow + cg, v);
@@ -442,22 +435,22 @@ __device__ __forceinline__ void general_tile_body(const Tc3Args& a, const float*
             for (int i = 0; i < 16; ++i) {
                 const int q = qb + cg + i;
                 float u = v[i] + bias;
-                if (a.relu) u = fmaxf(u, 0.f);
+                if (io.act == ACT_RELU) u = fmaxf(u, 0.f);
                 const long long t = (long long)q * ups;
-                if (q < a.Tq && t + ph < a.Tout) yrow[t] = u;
+                if (q < a.Tq && t + ph < io.Tout) yrow[t] = u;
             }
         }
     }
 }
 
 // Out-of-line call of the general epilogue for the kernel whose hot path is the lean one (edge tiles only): inlined into
-// its tile loop the general code's loop invariants were hoisted across the lean path.  One copy of the arguments per
-// call: through the reference every field use would be a generic load.
+// its tile loop the general code's loop invariants were hoisted across the lean path.  One copy of the launch per call:
+// through the reference every field use would be a generic load.
 template <bool SC>
 __device__ __noinline__ void general_tile_call(const Tc3Args& a_ref, const float* arow, int b, int rt, int q0, int lq, int half,
                                                int lane) {
-    const Tc3Args a = a_ref;
-    general_tile_body<SC>(a, arow, b, rt, q0, lq, half, lane);
+    const ConvKArgs a = a_ref;
+    general_tile_body<SC>(a, a_ref.rscale, arow, b, rt, q0, lq, half, lane);
 }
 
 // Grouped epilogue, one tile half: out[c, t] = sum_g D_g[c, t + g*dil] with MMA row m = g * CH + c (CH = 128 / GRP
@@ -474,25 +467,25 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
     const int coff = 4 * ((tq & (4 / NQ - 1)) * NQ);
     const int cbeg = half ? 128 : 0;
     const int cend = half ? a.tstep : min(128, a.tstep);
-    const bool has_res = a.res != nullptr, acc_r = a.accum != 0;
-    const bool vec_ok = ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
-                        (!a.res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
-    const bool fast = vec_ok && (q0 + a.tstep <= a.Tout);   // interior tile: no bounds checks
-    const float* rrow = has_res ? a.res + (long long)b * a.res_bs + (long long)co * a.res_cs : nullptr;
-    float* yrow = a.y + (long long)b * a.y_bs + (long long)co * a.y_cs;
+    const ConvIO& io = a.io;
+    const bool has_res = io.res.p != nullptr, acc_r = (io.flags & EPI_ACCUM) != 0;
+    const bool vec_ok = io.y.aligned16() && (!has_res || io.res.aligned16());
+    const bool fast = vec_ok && (q0 + a.tstep <= io.Tout);   // interior tile: no bounds checks
+    const float* rrow = has_res ? io.res.row(b, co) : nullptr;
+    float* yrow = io.y.row(b, co);
     float bias = a.bias[co];
-    if (a.cond) bias += __ldg(a.cond + (long long)b * a.cond_bs + co);
+    if (io.cond) bias += __ldg(io.cond.row(b) + co);
     const float rs = SC ? a.rscale[co] : 1.f;
     auto load = [&](const float* rr, int q, float* dst) {     // one thread's values of a column group of a row
 #pragma unroll
         for (int j = 0; j < NQ; ++j) {
             const int qq = q + 4 * j;
-            if (fast || (vec_ok && qq + 3 < a.Tout)) {
+            if (fast || (vec_ok && qq + 3 < io.Tout)) {
                 const float4 t = *reinterpret_cast<const float4*>(rr + qq);
                 dst[4 * j] = t.x; dst[4 * j + 1] = t.y; dst[4 * j + 2] = t.z; dst[4 * j + 3] = t.w;
             } else {
 #pragma unroll
-                for (int e = 0; e < 4; ++e) dst[4 * j + e] = rr[min(qq + e, a.Tout - 1)];
+                for (int e = 0; e < 4; ++e) dst[4 * j + e] = rr[min(qq + e, io.Tout - 1)];
             }
         }
     };
@@ -513,22 +506,22 @@ __device__ __forceinline__ void grouped_tile(const Tc3Args& a, const float* accs
 #pragma unroll
         for (int i = 0; i < NV; ++i) {
             float u = R[i] + bias;
-            if (a.relu) u = fmaxf(u, 0.f);
+            if (io.act == ACT_RELU) u = fmaxf(u, 0.f);
             if (has_res) u += rv[i];
-            u *= a.scale;
+            u *= io.scale;
             if (acc_r) u += ov[i];
-            if (a.post_div != 1.f) u = u / a.post_div;
+            if (io.post_div != 1.f) u = u / io.post_div;
             R[i] = u;
         }
         const int q = q0 + cg + coff;
 #pragma unroll
         for (int j = 0; j < NQ; ++j) {
             const int qq = q + 4 * j;
-            if (fast || (vec_ok && qq + 3 < a.Tout)) {
+            if (fast || (vec_ok && qq + 3 < io.Tout)) {
                 *reinterpret_cast<float4*>(yrow + qq) = make_float4(R[4 * j], R[4 * j + 1], R[4 * j + 2], R[4 * j + 3]);
             } else {
 #pragma unroll
-                for (int e = 0; e < 4; ++e) if (qq + e < a.Tout) yrow[qq + e] = R[4 * j + e];
+                for (int e = 0; e < 4; ++e) if (qq + e < io.Tout) yrow[qq + e] = R[4 * j + e];
             }
         }
     }
@@ -562,9 +555,9 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
     float* const rbuf = epi + (size_t)wg * 2 * C * P;           // residual in, output out
     float* const obuf = rbuf + C * P;                           // accumulate operand
     const uint64_t wdesc0 = make_desc(smem_u32(smB), C * 16);
-    const bool has_res = a.res != nullptr, acc_r = a.accum != 0, relu = a.relu != 0;
-    const bool bulk_layer = ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
-                            (!has_res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
+    const ConvIO& io = a.io;
+    const bool has_res = io.res.p != nullptr, acc_r = (io.flags & EPI_ACCUM) != 0, relu = io.act == ACT_RELU;
+    const bool bulk_layer = io.y.aligned16() && (!has_res || io.res.aligned16());
     const int c0 = 2 * (lane & 3), t0 = 16 * lq + (lane >> 2);  // fragment: channels 8j + c0 + {0,1}, time steps t0 (+8) + 64 s
     bool ok = true;
     int sa = 0; uint32_t pa = 0;                                // activation stage / its parity
@@ -575,7 +568,7 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
         int b, rt, q0;
         decode(it, b, rt, q0);
         const int qw = q0 + wg * HW;                            // this warpgroup's first column
-        const bool bulk = bulk_layer && q0 + 2 * HW <= a.Tout;
+        const bool bulk = bulk_layer && q0 + 2 * HW <= io.Tout;
         const bool pre = bulk && (has_res || acc_r);
         if (bulk && lane == 0) {
             bulk_wait_read();                                   // this warp's previous bulk stores are done reading its rows
@@ -584,9 +577,9 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
                 mbar_expect_tx(rf, (uint32_t)((has_res ? 1 : 0) + (acc_r ? 1 : 0)) * CW * HW * 4);
                 for (int c = lq * CW; c < (lq + 1) * CW; ++c) {
                     if (has_res)
-                        bulk_g2s(smem_u32(rbuf + c * P), a.res + (long long)b * a.res_bs + (long long)c * a.res_cs + qw, HW * 4, rf);
+                        bulk_g2s(smem_u32(rbuf + c * P), io.res.row(b, c) + qw, HW * 4, rf);
                     if (acc_r)
-                        bulk_g2s(smem_u32(obuf + c * P), a.y + (long long)b * a.y_bs + (long long)c * a.y_cs + qw, HW * 4, rf);
+                        bulk_g2s(smem_u32(obuf + c * P), io.y.row(b, c) + qw, HW * 4, rf);
                 }
             }
         }
@@ -651,16 +644,16 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
             for (int e = 0; e < 2; ++e) {
                 const int ch = 8 * j + c0 + e;
                 bv[j][e] = a.bias[ch];
-                if (a.cond) bv[j][e] += __ldg(a.cond + (long long)b * a.cond_bs + ch);
+                if (io.cond) bv[j][e] += __ldg(io.cond.row(b) + ch);
                 sv[j][e] = a.rscale[ch];
             }
         auto finish = [&](float v, int j, int e, float r, float o) {
             float u = v * sv[j][e] + bv[j][e];
             if (relu) u = fmaxf(u, 0.f);
             if (has_res) u += r;
-            u *= a.scale;
+            u *= io.scale;
             if (acc_r) u += o;
-            if (a.post_div != 1.f) u = u / a.post_div;
+            if (io.post_div != 1.f) u = u / io.post_div;
             return u;
         };
         if (bulk) {
@@ -693,7 +686,7 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
             named_bar_sync(5 + wg, 128);
             if (ok && lane == 0) {
                 for (int c = lq * CW; c < (lq + 1) * CW; ++c)
-                    bulk_s2g(a.y + (long long)b * a.y_bs + (long long)c * a.y_cs + qw, smem_u32(rbuf + c * P), HW * 4);
+                    bulk_s2g(io.y.row(b, c) + qw, smem_u32(rbuf + c * P), HW * 4);
                 bulk_commit();
             }
         } else if (ok) {
@@ -706,9 +699,9 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int ch = 8 * j + c0 + e, q = qw + 64 * s + t0 + 8 * h;
-                            if (q >= a.Tout) continue;
-                            float* yp = a.y + (long long)b * a.y_bs + (long long)ch * a.y_cs + q;
-                            const float r = has_res ? a.res[(long long)b * a.res_bs + (long long)ch * a.res_cs + q] : 0.f;
+                            if (q >= io.Tout) continue;
+                            float* yp = io.y.row(b, ch) + q;
+                            const float r = has_res ? io.res.p[(long long)b * io.res.bs + (long long)ch * io.res.cs + q] : 0.f;
                             const float o = acc_r ? *yp : 0.f;
                             *yp = finish(d[s][4 * j + 2 * h + e], j, e, r, o);
                         }
@@ -759,20 +752,20 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
 
     const int nchunks = (a.Cin + KCH - 1) / KCH;
-    const bool ragged = a.lens != nullptr;
+    const bool ragged = a.io.lens != nullptr;
     int* pref = reinterpret_cast<int*>(smem + a.pref_off);    // pref[b] = first tile of row b (ragged only)
     if (ragged) {
         // tiles per row from its own length; exclusive prefix by warp 0 (rows in lane-contiguous chunks).  `lens` was
         // written several launches ago (durations kernel), so reading it before griddepcontrol.wait is safe.
-        for (int b = tid; b < a.B; b += NTHREADS2) {
-            const long long e = (long long)a.lens[b] * a.rate_q + a.need_q;
+        for (int b = tid; b < a.io.B; b += NTHREADS2) {
+            const long long e = (long long)a.io.lens[b] * a.io.rate_out + a.io.need_out;
             const int ext = (int)(e < (long long)a.Tq ? (e > 0 ? e : 0) : (long long)a.Tq);
-            const int t_hi = (min(ext, a.q_hi) + a.tstep - 1) / a.tstep;
+            const int t_hi = (min(ext, a.io.q_hi) + a.tstep - 1) / a.tstep;
             pref[b + 1] = max(0, t_hi - a.t_lo) * a.n_rtiles;
         }
         __syncthreads();
         if (warp == 0) {
-            const int per = (a.B + 31) / 32, lo = lane * per, hi = min(a.B, lo + per);
+            const int per = (a.io.B + 31) / 32, lo = lane * per, hi = min(a.io.B, lo + per);
             int sum = 0;
             for (int b = lo; b < hi; ++b) sum += pref[b + 1];
             int incl = sum;
@@ -784,7 +777,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         }
         __syncthreads();
     }
-    const int tiles_total = ragged ? pref[a.B] : a.B * a.n_rtiles * a.n_ttiles;
+    const int tiles_total = ragged ? pref[a.io.B] : a.io.B * a.n_rtiles * a.n_ttiles;
     const int my_tiles = (tiles_total > (int)blockIdx.x) ? (tiles_total - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
     if (tid == 0) {
@@ -803,7 +796,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     auto decode = [&](int it, int& b, int& rt, int& q0) {
         const int tile = (int)blockIdx.x + it * (int)gridDim.x;
         if (ragged) {
-            int lo = 0, hi = a.B;                   // largest b with pref[b] <= tile (rows without tiles are skipped)
+            int lo = 0, hi = a.io.B;                   // largest b with pref[b] <= tile (rows without tiles are skipped)
             while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (pref[mid] <= tile) lo = mid; else hi = mid; }
             b = lo;
             const int local = tile - pref[b], nt = (pref[b + 1] - pref[b]) / a.n_rtiles;
@@ -817,9 +810,9 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         q0 = (a.t_lo + tt) * a.tstep;
     };
     auto input_extent = [&](int b) -> int {       // columns of x[b] that hold data; beyond it the operand is zero
-        if (!ragged) return a.Tin;
-        const long long e = (long long)a.lens[b] * a.rate_in + a.need_in;
-        return (int)(e < (long long)a.Tin ? (e > 0 ? e : 0) : (long long)a.Tin);
+        if (!ragged) return a.io.Tin;
+        const long long e = (long long)a.io.lens[b] * a.io.rate_in + a.io.need_in;
+        return (int)(e < (long long)a.io.Tin ? (e > 0 ? e : 0) : (long long)a.io.Tin);
     };
 
     if (warp >= W_PROD && warp < W_PROD + NPW) {
@@ -828,10 +821,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         const int total = my_tiles * nchunks * SPC;                      // raw stages to fill and transform
         const int vec_per_row = RAWW / 4;
         const int nvec = KC2 * vec_per_row;
-        const float slope = a.in_slope;
-        const float* const xg = a.x;
-        const long long x_bs = a.x_bs;
-        const int x_cs = a.x_cs, Cin = a.Cin, pad = a.pad;
+        const float slope = a.io.in_slope;
+        const float* const xg = a.io.x.p;
+        const long long x_bs = a.io.x.bs;
+        const int x_cs = a.io.x.cs, Cin = a.Cin, pad = a.pad;
         bool ok = true;
         // Per-thread work items are decoded ONCE (no divisions in the loop), the raw row stride is a compile-time constant
         // (shared loads take immediate offsets), interior windows take a copy path without any bounds logic, and leaky
@@ -875,7 +868,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                     iss_Tin = input_extent(b_);
                     iss_tal = (q0_ - pad) & ~3;                            // 16-byte aligned window start (may be < 0)
                     iss_row = xg + (long long)b_ * x_bs;
-                    iss_int = !NEAR && iss_tal >= (a.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
+                    iss_int = !NEAR && iss_tal >= (a.io.in_lo & ~3) && iss_tal + RAWW <= iss_Tin && (Cin & (KCH - 1)) == 0;
                     iss_new = false;
                 }
                 // a raw stage is RCH / 8 slots of 8 channels (two for BF16 / FP16): the per-thread work items cover one slot
@@ -902,7 +895,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                                 for (int q = 0; q < 4; ++q) {
                                     const int tt = t + q;
                                     const bool in = cg < Cin && tt >= 0 && tt < iss_Tin;
-                                    const int src = in ? near_col(tt, a.near_src, iss_Tin, a.near_scale) : 0;
+                                    const int src = in ? near_col(tt, a.io.near_src, iss_Tin, a.near_scale) : 0;
                                     cp_async4_zfill(dst0 + v_dst[e] + 4u * q, rowp + src, in ? 4u : 0u);
                                 }
                                 continue;
@@ -924,7 +917,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                             // t is a multiple of 4, so a vector is either wholly before the data start (zero fill),
                             // wholly inside, or cut by its end (partial source size, rest zero-filled by the hardware)
                             int nb = 0;
-                            if (cg < Cin && t >= (a.in_lo & ~3)) nb = 4 * max(0, min(4, iss_Tin - t));
+                            if (cg < Cin && t >= (a.io.in_lo & ~3)) nb = 4 * max(0, min(4, iss_Tin - t));
                             const int tsafe = (t >= 0 && t < iss_Tin) ? t : 0;
                             const float* src = iss_row + (long long)(cg < Cin ? cg : 0) * x_cs + tsafe;
                             cp_async16_zfill(dst0 + v_dst[e], src, (uint32_t)nb);
@@ -1034,7 +1027,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 if (it != cur_it) {
                     int b_, rt, q0_;
                     decode(it, b_, rt, q0_);
-                    wsrc = reinterpret_cast<const unsigned char*>(a.w) + (size_t)rt * total * stageB;
+                    wsrc = reinterpret_cast<const unsigned char*>(a.w_tc) + (size_t)rt * total * stageB;
                     cur_it = it;
                 }
                 if (!first) { ok = mbar_wait(empty, par, a.err); if (!ok) break; }
@@ -1074,10 +1067,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
         // is fenced off by a barrier when a bulk tile follows it and by the warp's bulk_wait_read when it follows one.
         // The residual may alias y: a tile reads and writes only its own columns, and only the next tile is prefetched.
         const int row_w = wg * 64 + lq * 16;            // this warp's first tile row
-        const bool bulk_layer = BULK && a.ups == 1 && !a.gate && a.split == 0 && !a.relu && !a.ymask &&
-                                a.scale == 1.f && a.post_div == 1.f && a.accum == 0 &&
-                                ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
-                                (!a.res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
+        const ConvIO& io = a.io;
+        const bool bulk_layer = BULK && a.ups == 1 && !(io.flags & (EPI_GATE | EPI_ACCUM)) && io.split == 0 &&
+                                io.act != ACT_RELU && !io.ymask && io.scale == 1.f && io.post_div == 1.f &&
+                                io.y.aligned16() && (!io.res || io.res.aligned16());
         uint32_t pr = 0;                                // parity of RES_FULL[warp]
         bool shared_epi = false;                        // the previous tile's epilogue read other warps' rows of `accs`
 #pragma unroll 1
@@ -1087,8 +1080,8 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 int b, rt, q0;
                 decode(it, b, rt, q0);
                 const int nrows = min(16, a.Rows - (rt * MROWS + row_w));
-                bulk = bulk_layer && q0 + TT2 <= a.Tout;
-                pre = bulk && a.res != nullptr && nrows > 0;
+                bulk = bulk_layer && q0 + TT2 <= io.Tout;
+                pre = bulk && io.res && nrows > 0;
                 if (bulk) {
                     if (shared_epi) { fence_async_smem(); named_bar_sync(4, NCONS); }
                     if (lane == 0) bulk_wait_read();    // this warp's previous bulk stores are done reading its rows
@@ -1096,10 +1089,10 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 }
                 if (pre && lane == 0) {
                     const uint32_t rf = BAR(RES_FULL + warp);
-                    const float* src = a.res + (long long)b * a.res_bs + (long long)(rt * MROWS + row_w) * a.res_cs + q0;
+                    const float* src = io.res.row(b, rt * MROWS + row_w) + q0;
                     mbar_expect_tx(rf, (uint32_t)nrows * TT2 * 4);
                     for (int r = 0; r < nrows; ++r)
-                        bulk_g2s(smem_u32(accs + (row_w + r) * ACC_LD), src + (long long)r * a.res_cs, TT2 * 4, rf);
+                        bulk_g2s(smem_u32(accs + (row_w + r) * ACC_LD), src + (long long)r * io.res.cs, TT2 * 4, rf);
                 }
             }
             float d[128];                              // per tile: not live across the epilogue
@@ -1180,7 +1173,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 for (int h = 0; h < 2; ++h) {
                     const int rc = min(rl + 8 * h, a.Rows - 1);
                     bv[h] = a.bias[rc];
-                    if (a.cond) bv[h] += __ldg(a.cond + (long long)b * a.cond_bs + rc);
+                    if (io.cond) bv[h] += __ldg(io.cond.row(b) + rc);
                     sv[h] = SC ? a.rscale[rc] : 1.f;
                 }
                 if (pre) bulk_combine<true, SC>(d, st_row, bv, sv);
@@ -1189,9 +1182,9 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 __syncwarp();
                 if (lane == 0) {
                     const int nrows = min(16, a.Rows - r0);
-                    float* dst = a.y + (long long)b * a.y_bs + (long long)r0 * a.y_cs + q0;
+                    float* dst = io.y.row(b, r0) + q0;
                     for (int r = 0; r < nrows; ++r)
-                        bulk_s2g(dst + (long long)r * a.y_cs, smem_u32(accs + (row_w + r) * ACC_LD), TT2 * 4);
+                        bulk_s2g(dst + (long long)r * io.y.cs, smem_u32(accs + (row_w + r) * ACC_LD), TT2 * 4);
                     bulk_commit();
                 }
                 continue;
@@ -1214,25 +1207,24 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
             } else {
                 const int qb = q0 + half * 128;
                 const float* at = accs + lq * 32 * ACC_LD + half * 128;            // this warp's 32 rows x 128 columns
-                const bool lean = LEAN && a.ups == 1 && !a.gate && a.split == 0 && !a.relu && !a.ymask && a.scale == 1.f &&
-                                  a.post_div == 1.f && qb + 128 <= a.Tout &&
-                                  ((a.y_cs & 3) == 0) && ((a.y_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.y) & 15) == 0) &&
-                                  (!a.res || (((a.res_cs & 3) == 0) && ((a.res_bs & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.res) & 15) == 0)));
+                const bool lean = LEAN && a.ups == 1 && !(io.flags & EPI_GATE) && io.split == 0 && io.act != ACT_RELU &&
+                                  !io.ymask && io.scale == 1.f && io.post_div == 1.f && qb + 128 <= io.Tout &&
+                                  io.y.aligned16() && (!io.res || io.res.aligned16());
                 if (lean) {
                     // every interior tile half of the plain layers: coalesced global accesses, no per-option branches
                     const int row0 = rt * MROWS + lq * 32;
-                    const float* cond = a.cond ? a.cond + (long long)b * a.cond_bs : nullptr;
-                    float* yq = a.y + (long long)b * a.y_bs + qb;
-                    const bool hres = a.res != nullptr, hacc = a.accum != 0;
-                    const float* rq = hres ? a.res + (long long)b * a.res_bs + qb : yq;
-                    if (hres) { if (hacc) lean_tile<true, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true);
-                                else lean_tile<true, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, a.res_cs, a.y_cs, row0, a.Rows, true); }
-                    else { if (hacc) lean_tile<false, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true);
-                           else lean_tile<false, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, a.y_cs, row0, a.Rows, true); }
+                    const float* cond = io.cond ? io.cond.row(b) : nullptr;
+                    float* yq = io.y.row(b, 0) + qb;
+                    const bool hres = io.res.p != nullptr, hacc = (io.flags & EPI_ACCUM) != 0;
+                    const float* rq = hres ? io.res.row(b, 0) + qb : yq;
+                    if (hres) { if (hacc) lean_tile<true, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, io.res.cs, io.y.cs, row0, a.Rows, true);
+                                else lean_tile<true, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, io.res.cs, io.y.cs, row0, a.Rows, true); }
+                    else { if (hacc) lean_tile<false, true, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, io.y.cs, row0, a.Rows, true);
+                           else lean_tile<false, false, SC>(at, a.bias, a.rscale, cond, lane, rq, yq, 0, io.y.cs, row0, a.Rows, true); }
                 } else if constexpr (LEAN) {
                     general_tile_call<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 } else {
-                    general_tile_body<SC, WG>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
+                    general_tile_body<SC, WG>(a, a.rscale, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 }
             }
         }
