@@ -133,13 +133,19 @@ int b200tts_conv1d_forward_wavegrad(const b200tts_conv1d* h, const float* x, lon
  *     mask_post (EPI_MASK_POST 4): v *= ymask[b, t]
  *     split     (EPI_SPLIT 16, WaveNet res/skip): rows r < split go to y[b, r] with accumulate and mask_post forced on,
  *               rows r >= split to y2[b, r - split], accumulating only with EPI_ACCUM2 (32), never masked
+ *   Conv1dBN (SpeedySpeech's layers, b200tts_debug_conv1d_launch_bn; no gate, split, conditioning or column window):
+ *     window    (EPI_WINDOW 128): v = 0 instead of conv + bias outside columns [bn->edge_lo, len_b - bn->edge_hi) of
+ *               row b, len_b = min(lens[b], out_len) with lens, else out_len
+ *     affine    (bn->aff_s, aff_h: device [out_channels], both or neither): v = v * aff_s[r] + aff_h[r] right after act
+ *               (relu or none)
  *   ymask needs EPI_MASK_PRE, EPI_MASK_POST or EPI_SPLIT (status 1 otherwise).  lens (device int32 [B], nullable): row b
  *   is computed below lens[b] * rate_out + need_out and reads its input as zero from lens[b] * rate_in + need_in on (the
  *   FP32-FMA kernel computes every column).  [q_lo, q_hi): the output columns to produce (the tensor-core kernels may
  *   write other columns of their tiles too); [in_lo, in_hi): the input columns that hold data.  Returns the engine's
  *   status. */
 enum { B200TTS_DEBUG_EPI_GATE = 1, B200TTS_DEBUG_EPI_MASK_PRE = 2, B200TTS_DEBUG_EPI_MASK_POST = 4,
-       B200TTS_DEBUG_EPI_ACCUM = 8, B200TTS_DEBUG_EPI_SPLIT = 16, B200TTS_DEBUG_EPI_ACCUM2 = 32 };
+       B200TTS_DEBUG_EPI_ACCUM = 8, B200TTS_DEBUG_EPI_SPLIT = 16, B200TTS_DEBUG_EPI_ACCUM2 = 32,
+       B200TTS_DEBUG_EPI_WINDOW = 128 };
 enum { B200TTS_DEBUG_ACT_NONE = 0, B200TTS_DEBUG_ACT_RELU = 1, B200TTS_DEBUG_ACT_TANH = 2, B200TTS_DEBUG_ACT_LOGCLAMP = 3 };
 typedef struct {
     const float* x; long long x_batch_stride; int x_channel_stride; int T;
@@ -162,6 +168,12 @@ int b200tts_debug_conv1d_create(const b200tts_conv1d_config* cfg, const float* w
                                 int allow_tensor_cores, int precision, int padding_mode, int gate_half,
                                 const int32_t* in_perm, const int32_t* out_perm, b200tts_conv1d** out);
 int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* io, void* stream);
+typedef struct {
+    int edge_lo, edge_hi;
+    const float* aff_s; const float* aff_h;
+} b200tts_debug_conv_bn;
+int b200tts_debug_conv1d_launch_bn(const b200tts_conv1d* h, const b200tts_debug_conv_io* io, const b200tts_debug_conv_bn* bn,
+                                   void* stream);
 
 /* Debug / test aids: the transformer layers' attention and add + LayerNorm kernels, one launch at a time, as the engines
  * call them (device pointers, [B, C, T] layouts, time contiguous).  Not a stable interface.
@@ -650,7 +662,8 @@ int b200tts_glow_tts_decode(const b200tts_glow_tts* h, const float* o_stats, con
  * encode: tokens int64 [B,Tt], lengths int64 [B], g [B, C] (emb_g row or d-vector) or [B, proj_g_in] (d-vector to
  *   project) or NULL -> o_en [B, C, Tt] (encoder output + g, + pitch / energy embeddings), logw [B,Tt] (durations_log),
  *   pitch / energy [B,Tt] (NULL without the predictor), x_mask [B,Tt], dur [B,Tt] (frames per token), cum [B,Tt],
- *   y_lengths int64 [B], meta int64 [2] = {max_b y_lengths, 0}: read it to size the decode call (Ty = meta[0]).
+ *   y_lengths int64 [B], meta int64 [2] = {max_b y_lengths, min_b y_lengths}: read it to size the decode call
+ *   (Ty = meta[0]).
  * decode: attn [B, Ty, Tt] (the returned alignments; or NULL), mel [B, Ty, out_channels] (model_outputs, zero past each
  *   row's y_length).  Ty > pe_len is an error, as in PositionalEncoding.forward.
  * No float atomics: repeat calls are bit-identical.
@@ -680,6 +693,41 @@ int b200tts_forward_tts_encode(const b200tts_forward_tts* h, const int64_t* toke
 int b200tts_forward_tts_decode(const b200tts_forward_tts* h, const float* o_en, const float* x_mask, const float* cum,
                                const int64_t* y_lengths, int B, int Tt, int Ty, float* attn, float* mel, void* workspace,
                                size_t workspace_bytes, void* stream);
+
+/* ---- SpeedySpeech inference (ForwardTTS with encoder_type and decoder_type "residual_conv_bn") ------------------------
+ * The same inference as above, with ResidualConv1dBNEncoder (TTS/tts/layers/feed_forward/encoder.py:41-73) and
+ * ResidualConv1dBNDecoder (decoder.py:125-160) in place of the FFTransformer stacks.  Their layer is Conv1dBN
+ * (generic/res_conv_bn.py:18-46): an unpadded conv with kernel k and dilation d whose output is zero padded by
+ * floor(d (k - 1) / 2) columns in front and the rest behind, then ReLU, then BatchNorm (eps 1e-5).  A row needs more than
+ * d (k - 1) columns in every such layer, as in the reference; meta[1] of encode is the shortest row's frame count.
+ * The handle is a b200tts_forward_tts: destroy, the workspace calls, encode and decode apply.  The encoder runs on the
+ * exact FP32 conv, the decoder on 3xTF32 tensor-core convs from 128 frames on.
+ * weights (host, PyTorch layouts; "bn" = BatchNorm1d weight, bias, running_mean, running_var [C], num_batches_tracked
+ * left out), in this order:
+ *   emb.weight [n_vocab, C]
+ *   encoder.encoder: prenet.0.w [C, C, 1], .b; per res block, per conv: conv_bn_blocks.j.conv1d.w [C, C, enc_kernel], .b,
+ *     conv_bn_blocks.j.norm (bn); postnet.0.w [C, C, 1], .b, postnet.2 (bn), postnet.3.w [C, C, 1], .b
+ *   proj_g, the predictors and embeddings and pos_encoder.pe as for b200tts_forward_tts_create
+ *   decoder.decoder: per res block, per conv: as in the encoder (dec_kernel); post_conv.w [C, C, 1], .b;
+ *     postnet.0.conv_bn_blocks.{0,1}: conv1d.w [C, C, dec_kernel], .b, norm (bn); postnet.1.w [out_channels, C, 1], .b
+ */
+#define B200TTS_CONV_BN_MAX_BLOCKS 32
+typedef struct {
+    int n_vocab;
+    int hidden_channels;       /* C */
+    int out_channels;
+    int enc_kernel, enc_blocks, enc_convs;              /* kernel size, residual blocks, convs per block */
+    int enc_dilations[B200TTS_CONV_BN_MAX_BLOCKS];      /* one per residual block */
+    int dec_kernel, dec_blocks, dec_convs;
+    int dec_dilations[B200TTS_CONV_BN_MAX_BLOCKS];
+    int proj_g_in;
+    int dp_hidden, dp_kernel;
+    int use_pitch, pitch_hidden, pitch_kernel, pitch_emb_kernel;
+    int use_energy, energy_hidden, energy_kernel, energy_emb_kernel;
+    int pe_len;
+} b200tts_speedy_speech_config;
+int b200tts_speedy_speech_create(const b200tts_speedy_speech_config* cfg, const float* const* weights, int num_weights,
+                                 b200tts_forward_tts** out);
 
 /* ---- self-attention on the tensor cores (ForwardTTS decoder) --------------------------------------------------------
  * Replaces nn.MultiheadAttention's attention core (softmax((q d^-1/2) k^T) v, torch/nn/functional.py

@@ -85,6 +85,20 @@ class ForwardTTSConfigC(ctypes.Structure):
                                             "energy_emb_kernel", "pe_len")]
 
 
+CONV_BN_MAX_BLOCKS = 32   # B200TTS_CONV_BN_MAX_BLOCKS
+
+
+class SpeedySpeechConfigC(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int) for n in ("n_vocab", "hidden_channels", "out_channels", "enc_kernel", "enc_blocks",
+                                            "enc_convs")] + \
+               [("enc_dilations", ctypes.c_int * CONV_BN_MAX_BLOCKS)] + \
+               [(n, ctypes.c_int) for n in ("dec_kernel", "dec_blocks", "dec_convs")] + \
+               [("dec_dilations", ctypes.c_int * CONV_BN_MAX_BLOCKS)] + \
+               [(n, ctypes.c_int) for n in ("proj_g_in", "dp_hidden", "dp_kernel", "use_pitch", "pitch_hidden",
+                                            "pitch_kernel", "pitch_emb_kernel", "use_energy", "energy_hidden",
+                                            "energy_kernel", "energy_emb_kernel", "pe_len")]
+
+
 class MelganConfigC(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int) for n in ("in_channels", "out_channels", "base_channels", "proj_kernel", "res_kernel",
                                             "num_res_blocks", "num_upsamples")] + \
@@ -136,7 +150,7 @@ PADDING_MODES = {"zeros": 0, "reflect": 1}
 
 
 # b200tts_debug_conv1d_launch's arguments and its flag / activation values (B200TTS_DEBUG_* in include/tts_b200.h)
-EPI_GATE, EPI_MASK_PRE, EPI_MASK_POST, EPI_ACCUM, EPI_SPLIT, EPI_ACCUM2 = 1, 2, 4, 8, 16, 32
+EPI_GATE, EPI_MASK_PRE, EPI_MASK_POST, EPI_ACCUM, EPI_SPLIT, EPI_ACCUM2, EPI_WINDOW = 1, 2, 4, 8, 16, 32, 128
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_LOGCLAMP = 0, 1, 2, 3
 
 
@@ -158,6 +172,11 @@ class DebugConvIOC(ctypes.Structure):
                 ("lens", ctypes.c_void_p), ("rate_out", ctypes.c_int), ("need_out", ctypes.c_int), ("rate_in", ctypes.c_int),
                 ("need_in", ctypes.c_int),
                 ("q_lo", ctypes.c_int), ("q_hi", ctypes.c_int), ("in_lo", ctypes.c_int), ("in_hi", ctypes.c_int)]
+
+
+class DebugConvBNC(ctypes.Structure):
+    """b200tts_debug_conv1d_launch_bn's Conv1dBN options (b200tts_debug_conv_bn)."""
+    _fields_ = [("edge_lo", ctypes.c_int), ("edge_hi", ctypes.c_int), ("aff_s", ctypes.c_void_p), ("aff_h", ctypes.c_void_p)]
 
 
 class AudioNormC(ctypes.Structure):
@@ -209,6 +228,8 @@ def _declare(lib):
                                                 ctypes.POINTER(vp)]
     lib.b200tts_debug_conv1d_launch.restype = ci
     lib.b200tts_debug_conv1d_launch.argtypes = [vp, ctypes.POINTER(DebugConvIOC), vp]
+    lib.b200tts_debug_conv1d_launch_bn.restype = ci
+    lib.b200tts_debug_conv1d_launch_bn.argtypes = [vp, ctypes.POINTER(DebugConvIOC), ctypes.POINTER(DebugConvBNC), vp]
     lib.b200tts_debug_attention.restype = ci
     lib.b200tts_debug_attention.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
     lib.b200tts_debug_add_layernorm.restype = ci
@@ -353,6 +374,9 @@ def _declare(lib):
     lib.b200tts_forward_tts_create.restype = ci
     lib.b200tts_forward_tts_create.argtypes = [ctypes.POINTER(ForwardTTSConfigC), ctypes.POINTER(vp), ci,
                                                ctypes.POINTER(vp)]
+    lib.b200tts_speedy_speech_create.restype = ci
+    lib.b200tts_speedy_speech_create.argtypes = [ctypes.POINTER(SpeedySpeechConfigC), ctypes.POINTER(vp), ci,
+                                                 ctypes.POINTER(vp)]
     lib.b200tts_forward_tts_destroy.restype = None
     lib.b200tts_forward_tts_destroy.argtypes = [vp]
     lib.b200tts_forward_tts_encode_workspace_bytes.restype = sz

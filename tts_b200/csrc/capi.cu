@@ -189,7 +189,8 @@ int b200tts_debug_conv1d_create(const b200tts_conv1d_config* cfg, const float* w
                               out_perm);
 }
 static_assert(sizeof(b200tts_debug_conv_io) == 216, "tts_b200/_lib.py DebugConvIOC mirrors this layout");
-int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, void* stream) {
+static int debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, const b200tts_debug_conv_bn* bn,
+                               void* stream) {
     if (!h || !d) { set_error("debug_conv1d_launch: null argument"); return 1; }
     ConvIO io;
     io.x = {d->x, d->x_batch_stride, d->x_channel_stride}; io.Tin = d->T;
@@ -203,13 +204,22 @@ int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_con
     io.act = d->act; io.act_param = d->act_param; io.flags = d->flags; io.B = d->B;
     io.lens = d->lens; io.rate_out = d->rate_out; io.need_out = d->need_out; io.rate_in = d->rate_in; io.need_in = d->need_in;
     io.q_lo = d->q_lo; io.q_hi = d->q_hi; io.in_lo = d->in_lo; io.in_hi = d->in_hi;
+    if (bn) { io.edge_lo = bn->edge_lo; io.edge_hi = bn->edge_hi; io.aff_s = bn->aff_s; io.aff_h = bn->aff_h; }
     io.reflect = h->reflect;
-    if (io.flags & ~(EPI_GATE | EPI_MASK_PRE | EPI_MASK_POST | EPI_ACCUM | EPI_SPLIT | EPI_ACCUM2) ||
+    if (io.flags & ~(EPI_GATE | EPI_MASK_PRE | EPI_MASK_POST | EPI_ACCUM | EPI_SPLIT | EPI_ACCUM2 | (bn ? EPI_WINDOW : 0)) ||
         !(io.act >= ACT_NONE && io.act <= ACT_LOGCLAMP)) {
         set_error("debug_conv1d_launch: unknown flags 0x%x or act %d", io.flags, io.act);
         return 1;
     }
     return launch_conv(h->L, io, (cudaStream_t)stream);
+}
+int b200tts_debug_conv1d_launch(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, void* stream) {
+    return debug_conv1d_launch(h, d, nullptr, stream);
+}
+int b200tts_debug_conv1d_launch_bn(const b200tts_conv1d* h, const b200tts_debug_conv_io* d, const b200tts_debug_conv_bn* bn,
+                                   void* stream) {
+    if (!bn) { set_error("debug_conv1d_launch_bn: null argument"); return 1; }
+    return debug_conv1d_launch(h, d, bn, stream);
 }
 
 int b200tts_debug_attention(const float* qkv, const float* mask, const float* rel_k, const float* rel_v, float* out,
@@ -559,6 +569,17 @@ int b200tts_forward_tts_create(const b200tts_forward_tts_config* cfg, const floa
     b200tts_forward_tts* h = new (std::nothrow) b200tts_forward_tts();
     if (!h) { set_error("forward_tts_create: out of host memory"); return 1; }
     int rc = h->impl.init(*cfg, weights, num_weights);
+    if (rc) { delete h; return rc; }
+    *out = h;
+    return 0;
+}
+int b200tts_speedy_speech_create(const b200tts_speedy_speech_config* cfg, const float* const* weights, int num_weights,
+                                 b200tts_forward_tts** out) {
+    if (!cfg || !weights || !out) { set_error("speedy_speech_create: null argument"); return 1; }
+    *out = nullptr;
+    b200tts_forward_tts* h = new (std::nothrow) b200tts_forward_tts();
+    if (!h) { set_error("speedy_speech_create: out of host memory"); return 1; }
+    int rc = h->impl.init_conv_bn(*cfg, weights, num_weights);
     if (rc) { delete h; return rc; }
     *out = h;
     return 0;

@@ -86,10 +86,12 @@ inline void count_launch(int n = 1) { g_launch_count += (unsigned long long)n; }
 //            SPLIT, and GATE with ymask, another flag, a residual, an act, scale or post_div (no engine sends these)
 //            WAVEGRAD (EPI_WAVEGRAD / ConvIO::near_src): v = acc + bias; [lrelu(v, act_param)]; [+ act_add[b]]; [+ res];
 //                       [y2 <- v]; [v = shift + scale * v]; y <- v   (own kernel variants, see ConvIO)
+//            Conv1dBN (EPI_WINDOW / ConvIO::aff_s): the valid window replaces acc + bias, the affine v = v * s[r] + h[r]
+//                       follows act; mask_pre, res, accum and mask_post as above (own kernel variants, see ConvIO)
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2, ACT_LOGCLAMP = 3,   // LOGCLAMP: log(max(v, act_param))
              ACT_LRELU = 4 };                                             // LRELU: leaky ReLU, slope act_param (WaveGrad)
 enum : int { EPI_GATE = 1, EPI_MASK_PRE = 2, EPI_MASK_POST = 4, EPI_ACCUM = 8, EPI_SPLIT = 16, EPI_ACCUM2 = 32,
-             EPI_WAVEGRAD = 64 };
+             EPI_WAVEGRAD = 64, EPI_WINDOW = 128 };
 
 // ------------------------------------------------------------------ device memory
 // Device buffers held by the engines, all made by upload() below.
@@ -237,6 +239,14 @@ struct ConvIO {
     // added after the activation (the FiLM noise level).  With EPI_WAVEGRAD, act may be ACT_LRELU.
     InView film; int film_half = 0;
     const float* act_add = nullptr;
+    // ---- Conv1dBN (SpeedySpeech's residual conv-BN layers: an unpadded conv whose OUTPUT is zero padded, then ReLU, then
+    // BatchNorm; res_conv_bn.py:18-46).  Like the WaveGrad variants they run on kernel instantiations of their own.
+    // valid window (flag EPI_WINDOW): output column t of row b takes pre-activation 0 -- no bias -- outside
+    // [edge_lo, len_b - edge_hi), len_b = min(lens[b], Tout) on a ragged launch, else Tout.  It replaces acc + bias.
+    int edge_lo = 0, edge_hi = 0;
+    // per-row affine after the activation (device [Rows], both or neither): v = v * aff_s[r] + aff_h[r] (eval BatchNorm
+    // as s = gamma / sqrt(var + eps), h = beta - mean * s), before mask_pre / res / accum / mask_post
+    const float* aff_s = nullptr; const float* aff_h = nullptr;
 };
 
 // Host weights in PyTorch layout.  conv: w[Cout][Cin][K];  transposed: w[Cin][Cout][Kt].

@@ -68,7 +68,9 @@ __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3, KEPI_WAVEGRAD = 4 };
+// KEPI_BN: the generic epilogue plus the Conv1dBN options (ConvIO::edge_lo / aff_s), compiled only into its own
+// instantiations so that the generic ones keep their code
+enum : int { KEPI_GENERIC = 0, KEPI_GATE = 1, KEPI_TANH = 2, KEPI_PLAIN = 3, KEPI_WAVEGRAD = 4, KEPI_BN = 5 };
 
 // CJ rows x TJ time steps per lane, WCO x WT warps, CIC input channels per stage, EPI epilogue family.
 // KG > 1: intra-CTA split-K for launch-starved shapes (text encoder / duration predictor: 64 frames x 32 utterances
@@ -349,6 +351,19 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         return r < a.Rows;
     };
     const bool mpre = (a.io.flags & EPI_MASK_PRE) != 0;
+    // Conv1dBN: the valid window [edge_lo, len_b - edge_hi) of this row, per column of this lane (a select: columns
+    // outside it read data past the row), and the per-row affine
+    bool vw[TJ];
+    const bool aff = EPI == KEPI_BN && a.io.aff_s != nullptr;
+    if constexpr (EPI == KEPI_BN) {
+        const bool win = (a.io.flags & EPI_WINDOW) != 0;
+        const int hi = (a.io.lens ? min(a.io.lens[b], a.io.Tout) : a.io.Tout) - a.io.edge_hi;
+#pragma unroll
+        for (int j = 0; j < TJ; ++j) {
+            const int q = qb + 32 * j;
+            vw[j] = !win || (q >= a.io.edge_lo && q < hi);
+        }
+    }
     // phase 1: bias / cond / activation / pre-mask (registers only)
 #pragma unroll
     for (int p = 0; p < CJ / 2; ++p) {
@@ -356,12 +371,21 @@ __global__ void __launch_bounds__(32 * WCO * WT * KG, (KG > 1) ? 1 : ((WCO * WT 
         float b0 = 0.f, b1 = 0.f;
         if (r0 < a.Rows) { b0 = a.bias[r0]; if (a.io.cond) b0 += __ldg(a.io.cond.row(b) + r0); }
         if (r0 + 1 < a.Rows) { b1 = a.bias[r0 + 1]; if (a.io.cond) b1 += __ldg(a.io.cond.row(b) + r0 + 1); }
+        float s0 = 1.f, s1 = 1.f, h0 = 0.f, h1 = 0.f;
+        if (aff) {
+            if (r0 < a.Rows) { s0 = a.io.aff_s[r0]; h0 = a.io.aff_h[r0]; }
+            if (r0 + 1 < a.Rows) { s1 = a.io.aff_s[r0 + 1]; h1 = a.io.aff_h[r0 + 1]; }
+        }
 #pragma unroll
         for (int j = 0; j < TJ; ++j) {
             float v0, v1;
             unpack2(acc[p][j], v0, v1);
             v0 += b0; v1 += b1;
+            if constexpr (EPI == KEPI_BN) {
+                if (!vw[j]) { v0 = 0.f; v1 = 0.f; }
+            }
             if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (aff) { v0 = fmaf(v0, s0, h0); v1 = fmaf(v1, s1, h1); }
             if (mpre) { v0 *= mk[j]; v1 *= mk[j]; }
             acc[p][j] = pack2(v0, v1);
         }
@@ -855,6 +879,7 @@ static int tc_device_init(int d) {
                 B200_CUDA_OK(cudaFuncSetAttribute(tc3::wavegrad_kernel(p, near), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                   smem_optin));
     }
+    B200_CUDA_OK(cudaFuncSetAttribute(tc3::bn_kernel(), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
     int* flag = nullptr;   // [0] pipeline timeout, [tc::ERR_RANGE] fp16 range (PREC_F16X3)
     B200_CUDA_OK(cudaHostAlloc((void**)&flag, 2 * sizeof(int), cudaHostAllocMapped | cudaHostAllocPortable));
     flag[0] = flag[tc::ERR_RANGE] = 0;
@@ -902,7 +927,9 @@ static int try_launch_tc(const ConvLayer& L, const ConvKArgs& a, cudaStream_t st
     const int rp_grouped = (tc3::TT2 + (J - 1) * G * L.dil + 7) / 8 * 8;
     const bool wg = (io.flags & EPI_WAVEGRAD) != 0;   // WaveGrad epilogue / resampled input: conv1d_tc3w_kernel
     if (wg && !tc3::wavegrad_kernel(L.tc_prec, false)) return -1;
-    const bool grouped = G && !wg && !needs_v3 && !io.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
+    const bool bn = (io.flags & EPI_WINDOW) || io.aff_s;   // Conv1dBN: conv1d_tc3bn_kernel, plain mode, 3xTF32 only
+    if (bn && L.tc_prec != tc::PREC_FP32) return -1;
+    const bool grouped = G && !wg && !bn && !needs_v3 && !io.ymask && (G - 1) * L.dil <= 15 && a.Tq >= 256 && fits(rp_grouped);
     // plain mode otherwise: M = rows (128 per tile, zero padded), N = 256 time steps.  Everything neither mode takes
     // (unaligned or masked inputs, shared-memory budget) runs on the exact FP32-FMA kernel.
     // At PREC_F16X3 the grouped layers run on the time-major kernel (M = time, N = the 32 / 64 channels): 256-column tiles,
@@ -928,10 +955,11 @@ static int try_launch_tc(const ConvLayer& L, const ConvKArgs& a, cudaStream_t st
     // plain layers (bias, residual, accumulate): the kernel with the lean epilogue; everything else (WaveNet gate / split,
     // masks, ReLU, scale, final divide, transposed convs) the one with the general epilogue inline
     const bool plain_epi = L.ups == 1 && !(io.flags & EPI_GATE) && io.split == 0 && io.act != ACT_RELU && !io.ymask &&
-                           io.scale == 1.f && io.post_div == 1.f;
+                           io.scale == 1.f && io.post_div == 1.f && !bn;
     const bool reflect = io.reflect != 0;   // reflection padding: the lean kernels' reflect variants only
     if (reflect && !grouped && !plain_epi) return -1;
     const tc3::Tc3Kernel k = wg ? tc3::wavegrad_kernel(L.tc_prec, io.near_src > 0)
+                                : bn      ? tc3::bn_kernel()
                                 : tm      ? tc3::timemajor_kernel(L.Rows, tm_slices, reflect)
                                 : grouped ? tc3::grouped_kernel(G, L.tc_prec, reflect)
                                           : tc3::plain_kernel(L.tc_prec, plain_epi, reflect);
@@ -984,7 +1012,7 @@ int launch_conv(const ConvLayer& L, const ConvIO& call, cudaStream_t st) {
         B200_REQUIRE(L.ups == 1 && !io.lens && !windowed && io.in_lo == 0 && io.in_hi == 0x7fffffff && !io.xmask && !io.ymask &&
                          !io.cond && !io.reflect && io.flags == EPI_WAVEGRAD && io.scale == 1.f && io.post_div == 1.f &&
                          (io.act == ACT_NONE || io.act == ACT_LRELU) && (!io.film || (io.film_half > 0 && io.film.cs > 0)) &&
-                         io.near_src >= 0,
+                         io.near_src >= 0 && !io.aff_s && !io.aff_h,
                      "launch_conv: the WaveGrad epilogue takes only lrelu / act_add / res / y2 / film, on a dense launch");
         if (a.Tq <= 0 || io.B <= 0) return 0;
         if (int rc = try_launch_tc(L, a, st); rc != -1) return rc;
@@ -999,6 +1027,15 @@ int launch_conv(const ConvLayer& L, const ConvIO& call, cudaStream_t st) {
     // a mask without a flag saying where it applies: the FMA plain epilogue would apply it, the others would not
     B200_REQUIRE(!io.ymask || (io.flags & (EPI_MASK_PRE | EPI_MASK_POST | EPI_SPLIT)),
                  "launch_conv: ymask needs EPI_MASK_PRE, EPI_MASK_POST or EPI_SPLIT");
+    if ((io.flags & EPI_WINDOW) || io.aff_s || io.aff_h) {   // Conv1dBN layers: their own kernel variants
+        B200_REQUIRE(L.ups == 1 && !io.reflect && !windowed && !io.cond && !(io.flags & (EPI_GATE | EPI_SPLIT | EPI_ACCUM2)) &&
+                         (io.act == ACT_NONE || io.act == ACT_RELU) && io.scale == 1.f && io.post_div == 1.f &&
+                         !io.aff_s == !io.aff_h && io.edge_lo >= 0 && io.edge_hi >= 0,
+                     "launch_conv: the Conv1dBN epilogue takes a window, relu, an affine, masks, res and accumulate, on an "
+                     "unwindowed launch without conditioning");
+        if (int rc = try_launch_tc(L, a, st); rc != -1) return rc;
+        return launch_cic<KEPI_BN>(a, L.co_tile, io.B, L.RowsPad, st);
+    }
     if (io.flags & EPI_GATE) {
         B200_REQUIRE(L.ups == 1 && !io.res && !io.ymask && io.act == ACT_NONE && io.flags == EPI_GATE && io.scale == 1.f &&
                          io.post_div == 1.f,

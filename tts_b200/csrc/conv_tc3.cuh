@@ -40,6 +40,7 @@
 // channels -- so every tap is summed in the accumulator and no MMA multiplies a padded tap.
 #pragma once
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "common.cuh"
@@ -242,7 +243,8 @@ __device__ __forceinline__ void bulk_combine(const float* d, float* st_row, cons
 // WG: the WaveGrad epilogue instead (conv1d_tc3w_kernel):
 //   v = acc + bias; [lrelu]; [+ act_add[b]]; [+ res]; [y2 <- v]; [v = shift + scale * v]; y <- v
 // with every product and sum rounded on its own (no FMA contraction), in the reference's order.
-template <bool SC, bool WG = false>
+// BN: the Conv1dBN options too (conv1d_tc3bn_kernel): the valid window replaces acc + bias, the affine follows act.
+template <bool SC, bool WG = false, bool BN = false>
 __device__ __forceinline__ void general_tile_body(const ConvKArgs& a, const float* rscale, const float* arow, int b, int rt,
                                                   int q0, int lq, int half, int lane) {
     const ConvIO& io = a.io;
@@ -361,6 +363,15 @@ __device__ __forceinline__ void general_tile_body(const ConvKArgs& a, const floa
         const float* rrow = io.res ? io.res.row(b, rc) : nullptr;
         const float* mrow = io.ymask ? io.ymask.row(b) : nullptr;
         const int ycs_eff = (io.split > 0 && rc >= io.split) ? io.y2.cs : io.y.cs;
+        // Conv1dBN: this row's valid window and affine
+        int w_lo = 0, w_hi = 0;
+        float a_s = 1.f, a_h = 0.f;
+        if constexpr (BN) {
+            const bool win = (io.flags & EPI_WINDOW) != 0;
+            w_lo = win ? io.edge_lo : INT_MIN;
+            w_hi = win ? (io.lens ? min(io.lens[b], io.Tout) : io.Tout) - io.edge_hi : INT_MAX;
+            if (io.aff_s) { a_s = io.aff_s[rc]; a_h = io.aff_h[rc]; }
+        }
         const bool vec_ok = ((ycs_eff & 3) == 0) && (!io.res || (io.res.cs & 3) == 0) &&
                             ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0) &&
                             (!rrow || (reinterpret_cast<uintptr_t>(rrow) & 15) == 0);
@@ -393,7 +404,13 @@ __device__ __forceinline__ void general_tile_body(const ConvKArgs& a, const floa
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
                 float u = v[i] + bias;
+                if constexpr (BN) {
+                    if (q + i < w_lo || q + i >= w_hi) u = 0.f;
+                }
                 if (io.act == ACT_RELU) u = fmaxf(u, 0.f);
+                if constexpr (BN) {
+                    if (io.aff_s) u = fmaf(u, a_s, a_h);
+                }
                 const float mk = mrow ? __ldg(mrow + min(q + i, io.Tout - 1)) : 1.f;
                 if (io.flags & EPI_MASK_PRE) u *= mk;
                 if (io.res) u += rv[i];
@@ -712,7 +729,7 @@ __device__ __forceinline__ void tm_consumers(const Tc3Args& a, const unsigned ch
 }
 
 template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false, bool NEAR = false, bool WG = false,
-          int TMC = 0, int TMS = 2>
+          int TMC = 0, int TMS = 2, bool BN = false>
                                        // TMC: the time-major kernel's output channels (32 / 64; 0: off), TMS: its m64
                                        // slices per warpgroup (tile width 128 * TMS), see tm_consumers;
                                        // GRP: tap groups stacked in the 128 MMA rows (1 = plain); LEAN:
@@ -723,6 +740,7 @@ template <int GRP, bool LEAN = true, int PREC = PREC_FP32, bool REFL = false, bo
                                        // that the zero-padding kernels keep their register allocation.
                                        // NEAR: nearest-resampled input (ConvIO::near_src): column t in [0, Tin) reads
                                        // x[near_col(t)], staged by 4-byte copies; WG: the WaveGrad epilogue (general_tile_body).
+                                       // BN: the Conv1dBN options in the general epilogue (with LEAN false).
 __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr bool X3 = PREC == PREC_F16X3;      // 3-product fp16 split
@@ -1224,7 +1242,7 @@ __device__ __forceinline__ void tc3_body(const Tc3Args& a) {
                 } else if constexpr (LEAN) {
                     general_tile_call<SC>(a, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 } else {
-                    general_tile_body<SC, WG>(a, a.rscale, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
+                    general_tile_body<SC, WG, BN>(a, a.rscale, at + lane * ACC_LD, b, rt, q0, lq, half, lane);
                 }
             }
         }
@@ -1249,7 +1267,14 @@ __global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3w_kernel(const __grid_
     tc3_body<1, false, PREC, false, NEAR, true>(a);
 }
 
+// Conv1dBN layers (EPI_WINDOW / ConvIO::aff_s): the general epilogue with the window and affine, 3xTF32 operands
+template <int PREC>
+__global__ void __launch_bounds__(NTHREADS2, 1) conv1d_tc3bn_kernel(const __grid_constant__ Tc3Args a) {
+    tc3_body<1, false, PREC, false, false, false, 0, 2, true>(a);
+}
+
 typedef void (*Tc3Kernel)(const Tc3Args);
+static inline Tc3Kernel bn_kernel() { return conv1d_tc3bn_kernel<PREC_FP32>; }
 // the WaveGrad kernels exist for 3xTF32 and the split-fp16 operands (the precisions WaveGrad packs)
 static inline Tc3Kernel wavegrad_kernel(int prec, bool near) {
     if (prec == PREC_F16X3) return near ? conv1d_tc3w_kernel<PREC_F16X3, true> : conv1d_tc3w_kernel<PREC_F16X3, false>;

@@ -508,15 +508,29 @@ struct Tacotron {
 // predictors and embeddings, durations); after the caller's one host read of max(y_lengths), decode expands the encoder
 // output with the positional encoding and runs the decoder on the 3xTF32 tensor-core convs and attention_tc3.cu.
 // Decoder tensors are [B, C, Tp] with Tp = frames rounded up to 4 (16-byte rows); every row stops at its y_length.
+// SpeedySpeech (init_conv_bn) swaps the FFTransformer stacks for residual conv-BatchNorm ones (feed_forward/encoder.py:41-73,
+// decoder.py:125-160): its encoder runs on the FP32 FMA conv like the rest of the text side, its decoder on 3xTF32 from
+// Tp >= 128 frames, as the FFTransformer decoder's convs do.
 struct ForwardTTS {
     using Layer = RelPosTransformer::Layer;   // FFTransformer (TTS/tts/layers/generic/transformer.py:6-35)
+    // Conv1dBN (res_conv_bn.py:18-46): unpadded conv, zero-padded output (edges lo / hi), ReLU, then eval BatchNorm as the
+    // per-channel affine s, h
+    struct ConvBN { ConvLayer conv; DevBuf<float> s, h; int lo = 0, hi = 0; };
+    using ResStack = std::vector<std::vector<ConvBN>>;   // ResidualConv1dBNBlock: [block][conv]
     b200tts_forward_tts_config c;
+    bool conv_bn = false;              // SpeedySpeech: the members below replace enc / dec
     DevBuf<float> emb;
     DevBuf<float> pe;                  // pos_encoder.pe [C][pe_len] (empty without positional encoding)
     std::vector<Layer> enc, dec;
-    ConvLayer proj_g, pitch_emb, energy_emb, postnet;
+    ConvLayer proj_g, pitch_emb, energy_emb, postnet;   // SpeedySpeech: postnet = decoder.postnet.1
+    ResStack enc_res, dec_res;
+    ConvLayer enc_prenet, enc_out, dec_post_conv;       // encoder prenet.0 / postnet.3, decoder post_conv
+    ConvBN enc_post;                                    // encoder postnet.0-2: 1x1 conv, ReLU, BatchNorm
+    std::vector<ConvBN> dec_post;                       // decoder postnet.0: Conv1dBNBlock (dilation 1)
     DurPred dp, pitch_dp, energy_dp;
     int init(const b200tts_forward_tts_config& cfg, const float* const* w, int nw);
+    int init_conv_bn(const b200tts_speedy_speech_config& cfg, const float* const* w, int nw);
+    int init_shared(WeightList& wl);   // proj_g, the predictors and embeddings, pe: between the encoder and the decoder
     static int tp(int Ty) { return (Ty + 3) / 4 * 4; }
     size_t encode_bytes(int B, int Tt) const;
     size_t decode_bytes(int B, int Ty) const;

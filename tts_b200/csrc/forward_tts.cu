@@ -10,6 +10,10 @@
 //   x = norm2(x + conv2(relu(conv1(x))))                       (k3 convs, zero padding, LayerNorm eps 1e-5)
 // Batched rows: encoder keys and conv inputs stop at the row's token count, decoder keys and conv inputs at its frame
 // count; a padded token gets no frame.  Row b thereby computes the single-utterance inference of x[b, :len[b]].
+// SpeedySpeech (init_conv_bn): residual conv-BN stacks instead (res_conv_bn.py:18-137, feed_forward/encoder.py:41-73,
+// decoder.py:125-160).  Each Conv1dBN is one launch with the valid window at the row's own length, so row b again
+// computes its single-utterance result: a valid output column reads only columns of its row, the window replaces every
+// other column's sum, and the masks zero what lies past the row.
 #include <math.h>
 
 #include "engines.cuh"
@@ -114,6 +118,86 @@ __global__ void mel_out_kernel(const float* pm, const long long* y_lengths, floa
     mel[(size_t)b * Ty * Co + i] = (long long)t < y_lengths[b] ? pm[((size_t)b * Co + o) * Tp + t] : 0.f;
 }
 
+// lens32[b] = lengths[b] (the token counts as the conv windows read them)
+__global__ void lens32_kernel(const long long* lengths, int* lens32, int B) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < B) lens32[b] = (int)lengths[b];
+}
+
+// one Conv1dBN of C channels: conv1d.weight, .bias, norm.weight, .bias, .running_mean, .running_var
+int pack_conv_bn(ForwardTTS::ConvBN& L, WeightList& wl, int C, int K, int dil, int prec) {
+    const float *w = wl.take(), *b = wl.take(), *g = wl.take(), *beta = wl.take(), *mean = wl.take(), *var = wl.take();
+    if (!w || !b || !g || !beta || !mean || !var) return wl.finish("speedy_speech");   // the list ran out
+    const int R = dil * (K - 1);
+    L.lo = R / 2;
+    L.hi = R - L.lo;
+    L.conv.tc_prec = prec;
+    if (int rc = pack_conv(L.conv, w, b, C, C, K, dil, L.lo)) return rc;
+    std::vector<float> s(C), h(C);   // eval BatchNorm: y = x * s + h
+    for (int i = 0; i < C; ++i) {
+        s[i] = (float)((double)g[i] / sqrt((double)var[i] + 1e-5));
+        h[i] = (float)((double)beta[i] - (double)mean[i] * (double)s[i]);
+    }
+    if (int rc = upload(L.s, s.data(), C)) return rc;
+    return upload(L.h, h.data(), C);
+}
+
+int pack_res_stack(ForwardTTS::ResStack& st, WeightList& wl, int C, int K, int blocks, int convs, const int* dil, int prec) {
+    st.clear();
+    st.resize(blocks);
+    for (int i = 0; i < blocks; ++i) {
+        st[i].resize(convs);
+        for (ForwardTTS::ConvBN& L : st[i])
+            if (int rc = pack_conv_bn(L, wl, C, K, dil[i], prec)) return rc;
+    }
+    return 0;
+}
+
+// one Conv1dBN launch in -> out: window at the row lengths of `base`, ReLU, affine; `res` (nullable) and `flags` for the
+// last conv of a residual block
+int launch_conv_bn(const ForwardTTS::ConvBN& L, const ConvIO& base, const float* in, float* out, const float* res,
+                   const float* mask, int flags, int C, int T, cudaStream_t st) {
+    ConvIO io = base;
+    io.x = dense(in, C, T); io.y = dense(out, C, T);
+    io.flags = EPI_WINDOW | flags; io.edge_lo = L.lo; io.edge_hi = L.hi;
+    io.act = ACT_RELU; io.aff_s = L.s; io.aff_h = L.h;
+    if (res) io.res = dense(res, C, T);
+    if (mask) io.ymask = {mask, T};
+    return launch_conv(L.conv, io, st);
+}
+
+// ResidualConv1dBNBlock.forward (res_conv_bn.py:129-137) on an input `cur` that is already masked: per block
+// o = (convs(o) + o) * mask.  Scratch: three [B][C][T] buffers (`cur` may be one of them); the result is in *out.  With
+// `last`, the last block writes (... + o) + last into `last` instead, before the mask (an addend that is zero where the
+// mask is)
+int run_res_stack(const ForwardTTS::ResStack& stack, const ConvIO& base, const float* mask, int C, int T, float* cur,
+                  float* const pool[3], float* last, float** out, cudaStream_t st) {
+    for (size_t i = 0; i < stack.size(); ++i) {
+        float* in = cur;
+        for (size_t j = 0; j < stack[i].size(); ++j) {
+            const bool end = j + 1 == stack[i].size(), into_last = end && last && i + 1 == stack.size();
+            float* o = into_last ? last : nullptr;
+            for (int p = 0; p < 3 && !o; ++p)
+                if (pool[p] != cur && pool[p] != in) o = pool[p];
+            if (int rc = launch_conv_bn(stack[i][j], base, in, o, end ? cur : nullptr, end ? mask : nullptr,
+                                        end ? (EPI_MASK_POST | (into_last ? EPI_ACCUM : 0)) : 0, C, T, st))
+                return rc;
+            in = o;
+        }
+        cur = in;
+    }
+    *out = cur;
+    return 0;
+}
+
+int launch_mel_out(const float* pm, const long long* y_lengths, float* mel, int B, int Co, int Ty, int Tp, cudaStream_t st) {
+    dim3 grid((unsigned)(((long long)Ty * Co + 255) / 256), B);
+    mel_out_kernel<<<grid, 256, 0, st>>>(pm, y_lengths, mel, Co, Ty, Tp);
+    count_launch();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 int pack_layer(ForwardTTS::Layer& L, WeightList& wl, int C, int F, int prec) {
     int rc;
     L.qkv.tc_prec = L.o.tc_prec = L.ffn1.tc_prec = L.ffn2.tc_prec = prec;
@@ -161,6 +245,19 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
     enc.resize(c.enc_layers);
     for (int l = 0; l < c.enc_layers; ++l)
         if ((rc = pack_layer(enc[l], wl, C, c.enc_ffn, TC_NONE))) return rc;
+    if ((rc = init_shared(wl))) return rc;
+    dec.resize(c.dec_layers);
+    for (int l = 0; l < c.dec_layers; ++l)
+        if ((rc = pack_layer(dec[l], wl, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
+    postnet.tc_prec = B200TTS_PRECISION_FP32;
+    const float *pw = wl.take(), *pb = wl.take();
+    if ((rc = pack_conv(postnet, pw, pb, c.out_channels, C, 1, 1, 0))) return rc;
+    return wl.finish("forward_tts");
+}
+
+int ForwardTTS::init_shared(WeightList& wl) {
+    const int C = c.hidden_channels;
+    int rc;
     if (c.proj_g_in > 0) {   // nn.Linear(d_vector_dim, C) as a 1x1 conv over a one-column input
         const float *gw = wl.take(), *gb = wl.take();
         if ((rc = pack_conv(proj_g, gw, gb, C, c.proj_g_in, 1, 1, 0))) return rc;
@@ -184,25 +281,74 @@ int ForwardTTS::init(const b200tts_forward_tts_config& cfg, const float* const* 
         if ((rc = pack_conv(energy_emb, ew, eb, C, 1, k, 1, (k - 1) / 2))) return rc;
     }
     if (c.pe_len > 0 && (rc = upload(pe, wl.take(), (size_t)C * c.pe_len))) return rc;
-    dec.resize(c.dec_layers);
-    for (int l = 0; l < c.dec_layers; ++l)
-        if ((rc = pack_layer(dec[l], wl, C, c.dec_ffn, B200TTS_PRECISION_FP32))) return rc;
-    postnet.tc_prec = B200TTS_PRECISION_FP32;
+    return 0;
+}
+
+int ForwardTTS::init_conv_bn(const b200tts_speedy_speech_config& s, const float* const* w, int nw) {
+    c = b200tts_forward_tts_config{};
+    c.n_vocab = s.n_vocab; c.hidden_channels = s.hidden_channels; c.out_channels = s.out_channels;
+    c.proj_g_in = s.proj_g_in; c.dp_hidden = s.dp_hidden; c.dp_kernel = s.dp_kernel;
+    c.use_pitch = s.use_pitch; c.pitch_hidden = s.pitch_hidden; c.pitch_kernel = s.pitch_kernel;
+    c.pitch_emb_kernel = s.pitch_emb_kernel;
+    c.use_energy = s.use_energy; c.energy_hidden = s.energy_hidden; c.energy_kernel = s.energy_kernel;
+    c.energy_emb_kernel = s.energy_emb_kernel;
+    c.pe_len = s.pe_len;
+    conv_bn = true;
+    const int C = c.hidden_channels;
+    B200_REQUIRE(c.n_vocab > 0 && C > 0 && c.out_channels > 0 && c.dp_hidden > 0 && c.dp_kernel >= 1 &&
+                     c.proj_g_in >= 0 && c.pe_len >= 0 && s.enc_kernel >= 1 && s.dec_kernel >= 1 && s.enc_convs >= 1 &&
+                     s.dec_convs >= 1 && s.enc_blocks >= 1 && s.enc_blocks <= B200TTS_CONV_BN_MAX_BLOCKS &&
+                     s.dec_blocks >= 1 && s.dec_blocks <= B200TTS_CONV_BN_MAX_BLOCKS,
+                 "speedy_speech: unsupported config");
+    for (int i = 0; i < s.enc_blocks; ++i) B200_REQUIRE(s.enc_dilations[i] >= 1, "speedy_speech: encoder dilation < 1");
+    for (int i = 0; i < s.dec_blocks; ++i) B200_REQUIRE(s.dec_dilations[i] >= 1, "speedy_speech: decoder dilation < 1");
+    B200_REQUIRE(!c.use_pitch || (c.pitch_hidden > 0 && c.pitch_kernel >= 1 && c.pitch_emb_kernel % 2 == 1),
+                 "speedy_speech: bad pitch predictor config");
+    B200_REQUIRE(!c.use_energy || (c.energy_hidden > 0 && c.energy_kernel >= 1 && c.energy_emb_kernel % 2 == 1),
+                 "speedy_speech: bad energy predictor config");
+    WeightList wl(w, nw);
+    int rc;
+    if ((rc = upload(emb, wl.take(), (size_t)c.n_vocab * C))) return rc;
+    const float *w0 = wl.take(), *b0 = wl.take();
+    if ((rc = pack_conv(enc_prenet, w0, b0, C, C, 1, 1, 0))) return rc;
+    if ((rc = pack_res_stack(enc_res, wl, C, s.enc_kernel, s.enc_blocks, s.enc_convs, s.enc_dilations, TC_NONE))) return rc;
+    if ((rc = pack_conv_bn(enc_post, wl, C, 1, 1, TC_NONE))) return rc;
+    const float *w3 = wl.take(), *b3 = wl.take();
+    if ((rc = pack_conv(enc_out, w3, b3, C, C, 1, 1, 0))) return rc;
+    if ((rc = init_shared(wl))) return rc;
+    const int P = B200TTS_PRECISION_FP32;
+    if ((rc = pack_res_stack(dec_res, wl, C, s.dec_kernel, s.dec_blocks, s.dec_convs, s.dec_dilations, P))) return rc;
+    dec_post_conv.tc_prec = P;
+    const float *pcw = wl.take(), *pcb = wl.take();
+    if ((rc = pack_conv(dec_post_conv, pcw, pcb, C, C, 1, 1, 0))) return rc;
+    const int one[1] = {1};
+    ResStack post;
+    if ((rc = pack_res_stack(post, wl, C, s.dec_kernel, 1, 2, one, P))) return rc;
+    dec_post = std::move(post[0]);
+    postnet.tc_prec = P;
     const float *pw = wl.take(), *pb = wl.take();
     if ((rc = pack_conv(postnet, pw, pb, c.out_channels, C, 1, 1, 0))) return rc;
-    return wl.finish("forward_tts");
+    return wl.finish("speedy_speech");
 }
 
 // the encoder layers' scratch, the projected speaker vector and one block the duration, pitch and energy predictors
 // take in turn
-struct FttsEncWs { float *qkv, *att, *yb, *hb, *gp; void* dp; size_t dp_bytes; };
+// (SpeedySpeech: the embedding, two residual-stack buffers and the int32 token counts instead of the layer scratch)
+struct FttsEncWs { float *qkv, *att, *yb, *hb, *gp; float *e, *r1, *r2; int* lens; void* dp; size_t dp_bytes; };
 static FttsEncWs ftts_encode_carve(const ForwardTTS& m, Arena& ar, int B, int Tt) {
     const int C = m.c.hidden_channels;
-    FttsEncWs w;
-    w.qkv = ar.f32((size_t)B * 3 * C * Tt);
-    w.att = ar.f32((size_t)B * C * Tt);
-    w.yb = ar.f32((size_t)B * C * Tt);
-    w.hb = ar.f32((size_t)B * m.c.enc_ffn * Tt);
+    FttsEncWs w{};
+    if (m.conv_bn) {
+        w.e = ar.f32((size_t)B * C * Tt);
+        w.r1 = ar.f32((size_t)B * C * Tt);
+        w.r2 = ar.f32((size_t)B * C * Tt);
+        w.lens = reinterpret_cast<int*>(ar.f32((size_t)B));
+    } else {
+        w.qkv = ar.f32((size_t)B * 3 * C * Tt);
+        w.att = ar.f32((size_t)B * C * Tt);
+        w.yb = ar.f32((size_t)B * C * Tt);
+        w.hb = ar.f32((size_t)B * m.c.enc_ffn * Tt);
+    }
     w.gp = ar.f32((size_t)B * C);
     w.dp_bytes = m.dp.workspace_bytes(B, Tt);
     if (m.c.use_pitch) w.dp_bytes = std::max(w.dp_bytes, m.pitch_dp.workspace_bytes(B, Tt));
@@ -215,15 +361,20 @@ size_t ForwardTTS::encode_bytes(int B, int Tt) const {
     return arena_size([&](Arena& ar) { ftts_encode_carve(*this, ar, B, Tt); });
 }
 
-struct FttsDecWs { float *x, *qkv, *att, *yb, *hb, *pm, *ymask; int* lens; };
+// (SpeedySpeech: three residual-stack buffers r instead of the layer scratch)
+struct FttsDecWs { float *x, *qkv, *att, *yb, *hb, *pm, *ymask; float* r[3]; int* lens; };
 static FttsDecWs ftts_decode_carve(const ForwardTTS& m, Arena& ar, int B, int Ty) {
     const size_t C = m.c.hidden_channels, Tp = ForwardTTS::tp(Ty);
-    FttsDecWs w;
+    FttsDecWs w{};
     w.x = ar.f32(B * C * Tp);
-    w.qkv = ar.f32(B * 3 * C * Tp);
-    w.att = ar.f32(B * C * Tp);
-    w.yb = ar.f32(B * C * Tp);
-    w.hb = ar.f32(B * m.c.dec_ffn * Tp);
+    if (m.conv_bn) {
+        for (float*& r : w.r) r = ar.f32(B * C * Tp);
+    } else {
+        w.qkv = ar.f32(B * 3 * C * Tp);
+        w.att = ar.f32(B * C * Tp);
+        w.yb = ar.f32(B * C * Tp);
+        w.hb = ar.f32(B * m.c.dec_ffn * Tp);
+    }
     w.pm = ar.f32(B * m.c.out_channels * Tp);
     w.ymask = ar.f32(B * Tp);
     w.lens = reinterpret_cast<int*>(ar.f32((size_t)B));
@@ -251,11 +402,31 @@ int ForwardTTS::encode(const long long* tokens, const long long* lengths, const 
     float *qkv = w.qkv, *att = w.att, *yb = w.yb, *hb = w.hb, *gp = w.gp;
     float* x = o_en;
     int rc;
-    // x = emb(tokens), no scale (forward_tts.py:405), masked at the row's length
-    if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, C, C, x, x_mask, st, false))) return rc;
     ConvIO eio;   // what every encoder conv shares: Tt columns in and out
     eio.Tin = eio.Tout = Tt; eio.B = B;
-    for (const Layer& L : enc) {
+    if (conv_bn) {
+        // ResidualConv1dBNEncoder (feed_forward/encoder.py:62-73): e = emb(tokens); o = relu(prenet(e)) * mask;
+        // o = res(o); o_en = postnet(o + e) * mask, the sum made by the last residual conv (into e)
+        if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, C, C, w.e, x_mask, st, false))) return rc;
+        lens32_kernel<<<(B + 127) / 128, 128, 0, st>>>(lengths, w.lens, B);
+        count_launch();
+        B200_CUDA_OK(cudaGetLastError());
+        eio.lens = w.lens;
+        ConvIO io = eio;
+        io.x = dense(w.e, C, Tt); io.y = dense(x, C, Tt); io.act = ACT_RELU; io.ymask = {x_mask, Tt};
+        io.flags = EPI_MASK_POST;
+        if ((rc = launch_conv(enc_prenet, io, st))) return rc;
+        float* const pool[3] = {x, w.r1, w.r2};
+        float* o = nullptr;
+        if ((rc = run_res_stack(enc_res, eio, x_mask, C, Tt, x, pool, w.e, &o, st))) return rc;
+        if ((rc = launch_conv_bn(enc_post, eio, w.e, w.r1, nullptr, nullptr, 0, C, Tt, st))) return rc;
+        io = eio;
+        io.x = dense(w.r1, C, Tt); io.y = dense(x, C, Tt); io.ymask = {x_mask, Tt}; io.flags = EPI_MASK_POST;
+        if ((rc = launch_conv(enc_out, io, st))) return rc;
+    } else if ((rc = launch_embed(tokens, lengths, emb, nullptr, B, Tt, C, C, x, x_mask, st, false))) {
+        return rc;   // x = emb(tokens), no scale (forward_tts.py:405), masked at the row's length
+    }
+    for (const Layer& L : enc) {   // FFTransformer layers (none for SpeedySpeech)
         ConvIO io = eio;
         io.x = dense(x, C, Tt); io.y = dense(qkv, 3 * C, Tt);
         if ((rc = launch_conv(L.qkv, io, st))) return rc;
@@ -323,6 +494,28 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
         count_launch();
         B200_CUDA_OK(cudaGetLastError());
     }
+    if (conv_bn) {
+        // ResidualConv1dBNDecoder (feed_forward/decoder.py:154-160): o = post_conv(res(x)) + x; postnet = Conv1dBNBlock
+        // (dilation 1, no mask between its convs), then a 1x1 conv; * mask in mel_out.  x is zero past each row, so
+        // res's leading x * mask is x.  Ragged rows: the windows stop at lens[b], and the tensor-core convs (Tp >= 128)
+        // only compute tiles below it and read the input as zero from there (the FMA conv computes every column).
+        ConvIO dio;
+        dio.Tin = dio.Tout = Tp; dio.B = B; dio.lens = lens;
+        float* o = nullptr;
+        if ((rc = run_res_stack(dec_res, dio, ymask, C, Tp, x, w.r, nullptr, &o, st))) return rc;
+        float* t[2];
+        for (int p = 0, n = 0; p < 3; ++p)
+            if (w.r[p] != o && n < 2) t[n++] = w.r[p];
+        ConvIO io = dio;
+        io.x = dense(o, C, Tp); io.y = dense(t[0], C, Tp); io.res = dense(x, C, Tp);
+        if ((rc = launch_conv(dec_post_conv, io, st))) return rc;
+        if ((rc = launch_conv_bn(dec_post[0], dio, t[0], t[1], nullptr, nullptr, 0, C, Tp, st))) return rc;
+        if ((rc = launch_conv_bn(dec_post[1], dio, t[1], t[0], nullptr, nullptr, 0, C, Tp, st))) return rc;
+        io = dio;
+        io.x = dense(t[0], C, Tp); io.y = dense(pm, Co, Tp);
+        if ((rc = launch_conv(postnet, io, st))) return rc;
+        return launch_mel_out(pm, y_lengths, mel, B, Co, Ty, Tp, st);
+    }
     // Ragged rows: the tensor-core convs (Tp >= 128) stop at lens[b] and read the input as zero from there; the FMA conv
     // (short batches) computes every column and reads the input through y_mask instead.
     const bool tc = Tp >= 128;
@@ -360,11 +553,7 @@ int ForwardTTS::decode(const float* o_en, const float* x_mask, const float* cum,
     ConvIO io = dio;
     io.x = dense(x, C, Tp); io.y = dense(pm, Co, Tp);
     if ((rc = launch_conv(postnet, io, st))) return rc;
-    dim3 grid((unsigned)(((long long)Ty * Co + 255) / 256), B);
-    mel_out_kernel<<<grid, 256, 0, st>>>(pm, y_lengths, mel, Co, Ty, Tp);
-    count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_mel_out(pm, y_lengths, mel, B, Co, Ty, Tp, st);
 }
 
 }  // namespace b200tts

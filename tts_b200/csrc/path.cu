@@ -4,6 +4,7 @@
 //   m_p, logs_p = matmul(attn^T, .)                   (a gather, exact because attn is one-hot)
 //   z_p = m_p + noise * exp(logs_p) * inference_noise_scale
 // Stage 1 runs before the one unavoidable host sync (max y_length fixes T_dec); stage 2 after it.
+#include <limits.h>
 #include "engines.cuh"
 
 namespace b200tts {
@@ -12,7 +13,8 @@ namespace {
 
 // one warp per utterance (one CTA, warps stride over the batch): inclusive scan of integral-valued fp32 durations
 // (exact below 2^24).  The same CTA reduces max(y_lengths) and forwards the duration predictor's error flag into
-// `meta` = {max y_length, flag}, so the caller's one host read fetches both (no second synchronisation).
+// `meta` = {max y_length, flag}, so the caller's one host read fetches both (no second synchronisation); the FORWARD rule
+// has no flag and reports the shortest row's y_length instead (SpeedySpeech's convs need a minimum length).
 // GLOW: the Glow-TTS rule (glow_tts.py:350-352), w = (exp(logw) - 1) * x_mask * length_scale and w_ceil =
 // clamp_min(ceil(w), 1) -- the clamp gives every padded token one frame too -- plus dur_log = log(1 + sum(attn, -1)) *
 // x_mask of compute_outputs (:147): a valid token's path row holds w_ceil ones, a padded token's none.
@@ -24,9 +26,9 @@ template <int RULE>
 __global__ void durations_kernel(const float* logw, const float* x_mask, float length_scale, float* w_ceil,
                                  float* cum, long long* y_lengths, int B, int T, const int* err_flag, long long* meta,
                                  float* dur_log) {
-    __shared__ long long wmax[32];
+    __shared__ long long wmax[32], wmin[32];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-    long long mymax = 0;
+    long long mymax = 0, mymin = LLONG_MAX;
     for (int b = warp; b < B; b += nwarps) {
         float carry = 0.f;
         for (int t0 = 0; t0 < T; t0 += 32) {
@@ -61,15 +63,19 @@ __global__ void durations_kernel(const float* logw, const float* x_mask, float l
         const long long yl = RULE == RULE_FORWARD ? (long long)carry : (long long)fmaxf(carry, 1.f);
         if (lane == 0) y_lengths[b] = yl;
         mymax = yl > mymax ? yl : mymax;
+        mymin = yl < mymin ? yl : mymin;
     }
     if (meta) {
-        if (lane == 0) wmax[warp] = mymax;
+        if (lane == 0) { wmax[warp] = mymax; wmin[warp] = mymin; }
         __syncthreads();
         if (threadIdx.x == 0) {
-            long long m = 0;
-            for (int i = 0; i < nwarps; ++i) m = wmax[i] > m ? wmax[i] : m;
+            long long m = 0, n = LLONG_MAX;
+            for (int i = 0; i < nwarps; ++i) {
+                m = wmax[i] > m ? wmax[i] : m;
+                n = wmin[i] < n ? wmin[i] : n;
+            }
             meta[0] = m;
-            meta[1] = err_flag ? (long long)err_flag[0] : 0;
+            meta[1] = RULE == RULE_FORWARD ? n : err_flag ? (long long)err_flag[0] : 0;
         }
     }
 }

@@ -16,7 +16,8 @@ Kept surface: ``ForwardTTS(config, ap, tokenizer, speaker_manager)``, ``ForwardT
 ``load_checkpoint(config, path, eval)``, ``length_scale``, ``init_multispeaker`` and the reference ``state_dict`` keys
 (``pos_encoder.pe`` and the training-only ``aligner.*`` included; the aligner is loaded and never run).  Built for
 ``encoder_type`` / ``decoder_type`` "fftransformer"; other types, training and ``forward`` raise
-``NotImplementedError``.
+``NotImplementedError``.  ``SpeedySpeech`` is the same model with the "residual_conv_bn" encoder and decoder
+(``SpeedySpeechConfig``, ``tts_models/en/ljspeech/speedy-speech``).
 """
 import copy
 import ctypes
@@ -145,7 +146,7 @@ Fastspeech2Config = FastSpeech2Config   # the reference's spelling (TTS/tts/conf
 @dataclass
 class SpeedySpeechConfig(_ForwardTTSConfig):
     """TTS/tts/configs/speedy_speech_config.py (model-side fields).  Its ``residual_conv_bn`` encoder and decoder are
-    not built: ``ForwardTTS`` raises ``NotImplementedError`` for it."""
+    built by ``SpeedySpeech``; ``ForwardTTS`` raises ``NotImplementedError`` for it."""
     model: str = "speedy_speech"
     model_args: ForwardTTSArgs = field(default_factory=lambda: ForwardTTSArgs(
         use_pitch=False, encoder_type="residual_conv_bn",
@@ -186,7 +187,8 @@ class _FFTransformerBlock(nn.Module):
 
 def _check_type(kind, name):
     if name.lower() != "fftransformer":
-        raise NotImplementedError(f"tts_b200.ForwardTTS: {kind}_type {name!r} is not built (fftransformer only)")
+        hint = "; tts_b200.SpeedySpeech builds residual_conv_bn" if name.lower() == "residual_conv_bn" else ""
+        raise NotImplementedError(f"tts_b200.ForwardTTS: {kind}_type {name!r} is not built (fftransformer only{hint})")
 
 
 class _Encoder(nn.Module):
@@ -268,11 +270,10 @@ class ForwardTTS(EngineModule):
         self.binary_loss_weight = 0.0
         self.length_scale = float(a.length_scale) if isinstance(a.length_scale, int) else a.length_scale
         self.emb = nn.Embedding(a.num_chars, a.hidden_channels)
-        self.encoder = _Encoder(a.hidden_channels, a.hidden_channels, a.encoder_type, a.encoder_params,
-                                self.embedded_speaker_dim)
+        self.encoder = self._encoder(a)
         if a.positional_encoding:
             self.pos_encoder = _PositionalEncoding(a.hidden_channels)
-        self.decoder = _Decoder(a.out_channels, a.hidden_channels, a.decoder_type, a.decoder_params)
+        self.decoder = self._decoder(a)
         self.duration_predictor = DurationPredictor(a.hidden_channels, a.duration_predictor_hidden_channels,
                                                     a.duration_predictor_kernel_size, a.duration_predictor_dropout_p)
         if a.use_pitch:
@@ -304,10 +305,16 @@ class ForwardTTS(EngineModule):
             self.emb_g = nn.Embedding(self.num_speakers, self.args.hidden_channels)
             nn.init.uniform_(self.emb_g.weight, -0.1, 0.1)
 
-    @staticmethod
-    def init_from_config(config, samples=None):  # pylint: disable=unused-argument
+    def _encoder(self, a):
+        return _Encoder(a.hidden_channels, a.hidden_channels, a.encoder_type, a.encoder_params, self.embedded_speaker_dim)
+
+    def _decoder(self, a):
+        return _Decoder(a.out_channels, a.hidden_channels, a.decoder_type, a.decoder_params)
+
+    @classmethod
+    def init_from_config(cls, config, samples=None):  # pylint: disable=unused-argument
         """forward_tts.py:848-862 without the host-side managers (tokenizer / AudioProcessor are built by the caller)."""
-        return ForwardTTS(copy.deepcopy(config))
+        return cls(copy.deepcopy(config))
 
     # ------------------------------------------------------------------ packing
     def _create(self, device):
@@ -384,10 +391,12 @@ class ForwardTTS(EngineModule):
         lens = x_lengths.to(device=dev, dtype=torch.int64).contiguous()
         if lens.shape != (b,):
             raise ValueError(f"tts_b200.ForwardTTS: x_lengths must be [{b}], got {tuple(lens.shape)}")
-        if tt == 1 or bool((lens == 1).any()):
+        shortest, one_token = torch.stack([lens.min(), (lens == 1).any().long()]).tolist() if b else (tt, 0)
+        if tt == 1 or one_token:
             # the reference's o_en.squeeze() (:691) also drops the time axis of a one-token utterance
             raise RuntimeError("tts_b200.ForwardTTS: a one-token input fails in the reference's duration predictor "
                                "(o_en.squeeze() drops its time axis)")
+        self._check_length(shortest, "token", "encoder")
         g = self._speaker_vector(aux_input, b, dev)
         a = self.args
         f32 = dict(dtype=torch.float32, device=dev)
@@ -411,7 +420,9 @@ class ForwardTTS(EngineModule):
                                               _lib.ptr(dur), _lib.ptr(cum), _lib.ptr(y_lengths), _lib.ptr(meta),
                                               _lib.ptr(ws), ctypes.c_size_t(ws.numel()), st)
             _lib.check(rc, "forward_tts_encode")
-            t_dec = int(meta[0].item())     # the one host read: y_max_length of sequence_mask(y_lengths, None)
+            # the one host read: y_max_length of sequence_mask(y_lengths, None), and the shortest row's frames
+            t_dec, shortest = meta.tolist()
+            self._check_length(shortest, "frame", "decoder")
             if hasattr(self, "pos_encoder") and t_dec > self.pos_encoder.pe.size(2):
                 raise RuntimeError(f"Sequence is {t_dec} but PositionalEncoding is limited to "
                                    f"{self.pos_encoder.pe.size(2)}. See max_len argument.")
@@ -425,6 +436,9 @@ class ForwardTTS(EngineModule):
         return {"model_outputs": mel, "alignments": attn, "pitch": pitch, "energy": energy, "durations_log": logw,
                 "durations": dur, "y_lengths": y_lengths}
 
+    def _check_length(self, n, unit, stack):
+        """Raises RuntimeError when the shortest row (n tokens / frames) is too short for the encoder / decoder."""
+
     # ------------------------------------------------------------------ out of scope
     def forward(self, *args, **kwargs):
         raise NotImplementedError("tts_b200.ForwardTTS implements inference only; training (forward) is out of scope")
@@ -437,6 +451,150 @@ class ForwardTTS(EngineModule):
         if eval:
             self.eval()
             assert not self.training
+
+
+# ----------------------------------------------------------------------------- SpeedySpeech
+class _Conv1dBN(nn.Module):
+    """Parameters of TTS/tts/layers/generic/res_conv_bn.py:18-46: conv (unpadded), output zero padding, ReLU, BatchNorm."""
+
+    def __init__(self, channels, kernel_size, dilation):
+        super().__init__()
+        self.conv1d = nn.Conv1d(channels, channels, kernel_size, dilation=dilation)
+        self.norm = nn.BatchNorm1d(channels)
+
+    def weights(self):
+        n = self.norm
+        return _wb(self.conv1d) + [_host(n.weight), _host(n.bias), _host(n.running_mean), _host(n.running_var)]
+
+
+class _Conv1dBNBlock(nn.Module):
+    """Parameters of res_conv_bn.py:49-83 (in = out = hidden channels)."""
+
+    def __init__(self, channels, kernel_size, dilation, num_conv_blocks):
+        super().__init__()
+        self.conv_bn_blocks = nn.Sequential(*[_Conv1dBN(channels, kernel_size, dilation)
+                                              for _ in range(num_conv_blocks)])
+
+    def weights(self):
+        return [t for layer in self.conv_bn_blocks for t in layer.weights()]
+
+
+class _ResidualConv1dBNBlock(nn.Module):
+    """Parameters of res_conv_bn.py:86-137."""
+
+    def __init__(self, channels, kernel_size, dilations, num_res_blocks, num_conv_blocks):
+        super().__init__()
+        assert len(dilations) == num_res_blocks
+        self.res_blocks = nn.ModuleList([_Conv1dBNBlock(channels, kernel_size, d, num_conv_blocks) for d in dilations])
+
+    def weights(self):
+        return [t for block in self.res_blocks for t in block.weights()]
+
+
+class _ResidualConv1dBNEncoder(nn.Module):
+    """Parameters of TTS/tts/layers/feed_forward/encoder.py:41-73."""
+
+    def __init__(self, channels, params):
+        super().__init__()
+        self.prenet = nn.Sequential(nn.Conv1d(channels, channels, 1), nn.ReLU())
+        self.res_conv_block = _ResidualConv1dBNBlock(channels, **params)
+        self.postnet = nn.Sequential(nn.Conv1d(channels, channels, 1), nn.ReLU(), nn.BatchNorm1d(channels),
+                                     nn.Conv1d(channels, channels, 1))
+
+    def weights(self):
+        n = self.postnet[2]
+        return _wb(self.prenet[0]) + self.res_conv_block.weights() + _wb(self.postnet[0]) + \
+            [_host(n.weight), _host(n.bias), _host(n.running_mean), _host(n.running_var)] + _wb(self.postnet[3])
+
+
+class _ResidualConv1dBNDecoder(nn.Module):
+    """Parameters of TTS/tts/layers/feed_forward/decoder.py:125-160."""
+
+    def __init__(self, channels, out_channels, params):
+        super().__init__()
+        self.res_conv_block = _ResidualConv1dBNBlock(channels, **params)
+        self.post_conv = nn.Conv1d(channels, channels, 1)
+        self.postnet = nn.Sequential(_Conv1dBNBlock(channels, params["kernel_size"], 1, 2),
+                                     nn.Conv1d(channels, out_channels, 1))
+
+    def weights(self):
+        return self.res_conv_block.weights() + _wb(self.post_conv) + self.postnet[0].weights() + _wb(self.postnet[1])
+
+
+def _conv_bn_params(params):
+    p = dict(params)
+    for k in ("kernel_size", "dilations", "num_res_blocks", "num_conv_blocks"):
+        if k not in p:
+            raise ValueError(f"tts_b200.SpeedySpeech: residual_conv_bn params need {k!r}")
+    return {k: p[k] for k in ("kernel_size", "dilations", "num_res_blocks", "num_conv_blocks")}
+
+
+class SpeedySpeech(ForwardTTS):
+    """SpeedySpeech (``SpeedySpeechConfig``: ForwardTTS with the "residual_conv_bn" encoder and decoder) on sm_90a
+    kernels.  Everything but the two stacks is ``ForwardTTS``'s: ``inference`` with its batched ``x_lengths``, speaker
+    conditioning, ``load_checkpoint``, ``init_from_config``.  Each residual conv-BN layer is one launch of the conv engine
+    with the layer's output window and BatchNorm in the epilogue; the encoder runs on the exact FP32 conv, the decoder on
+    3xTF32 tensor-core convs from 128 frames on.
+
+    Like the reference, a row needs more tokens than the widest encoder layer's reach d (k - 1) and more frames than the
+    widest decoder layer's (13 tokens and 25 frames at the defaults); ``inference`` raises RuntimeError otherwise."""
+
+    def _encoder(self, a):
+        _check_conv_bn("encoder", a.encoder_type)
+        enc = nn.Module()
+        enc.encoder = _ResidualConv1dBNEncoder(a.hidden_channels, _conv_bn_params(a.encoder_params))
+        return enc
+
+    def _decoder(self, a):
+        _check_conv_bn("decoder", a.decoder_type)
+        dec = nn.Module()
+        dec.decoder = _ResidualConv1dBNDecoder(a.hidden_channels, a.out_channels, _conv_bn_params(a.decoder_params))
+        return dec
+
+    @staticmethod
+    def _reach(params):
+        return max(d * (params["kernel_size"] - 1) for d in list(params["dilations"]) + [1])
+
+    def _check_length(self, n, unit, stack):
+        need = self._reach(self.args.encoder_params if stack == "encoder" else self.args.decoder_params) + 1
+        if n < need:
+            raise RuntimeError(f"tts_b200.SpeedySpeech: a row of {n} {unit}s is shorter than the {stack}'s widest "
+                               f"layer (kernel size and dilation need {need}); the reference fails on it too")
+
+    def _create(self, device):
+        a = self.args
+        ep, dp = _conv_bn_params(a.encoder_params), _conv_bn_params(a.decoder_params)
+        for p in (ep, dp):
+            if p["num_res_blocks"] > _lib.CONV_BN_MAX_BLOCKS:
+                raise ValueError(f"tts_b200.SpeedySpeech: at most {_lib.CONV_BN_MAX_BLOCKS} residual blocks")
+        proj_in = self.proj_g.in_features if hasattr(self, "proj_g") else 0
+        pe_len = self.pos_encoder.pe.shape[2] if hasattr(self, "pos_encoder") else 0
+        dil = lambda p: (ctypes.c_int * _lib.CONV_BN_MAX_BLOCKS)(*p["dilations"])  # noqa: E731
+        cfg = _lib.SpeedySpeechConfigC(
+            a.num_chars, a.hidden_channels, a.out_channels, ep["kernel_size"], ep["num_res_blocks"],
+            ep["num_conv_blocks"], dil(ep), dp["kernel_size"], dp["num_res_blocks"], dp["num_conv_blocks"], dil(dp),
+            proj_in, a.duration_predictor_hidden_channels, a.duration_predictor_kernel_size, int(a.use_pitch),
+            a.pitch_predictor_hidden_channels, a.pitch_predictor_kernel_size, a.pitch_embedding_kernel_size,
+            int(a.use_energy), a.energy_predictor_hidden_channels, a.energy_predictor_kernel_size,
+            a.energy_embedding_kernel_size, pe_len)
+        t = [_host(self.emb.weight)] + self.encoder.encoder.weights()
+        if proj_in:
+            t += _wb(self.proj_g)
+        t += self.duration_predictor.ordered_weights()
+        if a.use_pitch:
+            t += self.pitch_predictor.ordered_weights() + _wb(self.pitch_emb)
+        if a.use_energy:
+            t += self.energy_predictor.ordered_weights() + _wb(self.energy_emb)
+        if pe_len:
+            t += [_host(self.pos_encoder.pe[0])]
+        t += self.decoder.decoder.weights()
+        return self._make("b200tts_speedy_speech_create", cfg, t)
+
+
+def _check_conv_bn(kind, name):
+    if name.lower() != "residual_conv_bn":
+        raise NotImplementedError(f"tts_b200.SpeedySpeech: {kind}_type {name!r} is not built (residual_conv_bn only; "
+                                  "tts_b200.ForwardTTS builds fftransformer)")
 
 
 def attention(qkv, lengths, num_heads, out=None):
